@@ -3,7 +3,6 @@
 // here the context plays both roles for device memory: every buffer is carved once from cudaMalloc at
 // nb_create and reused every step, nothing is allocated or synchronised inside the step.
 #include "nb_shard.cuh"
-#define NB_DEFAULT_COOP_LAUNCH 1
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -29,23 +28,21 @@ struct nb_context {
 	u32 stride;    // scratch stride
 	u32 cstride;   // row plane stride
 	u32 slots_per_bucket;
-	int coop_blocks_solve; int coop_launch;
+	int coop_blocks_solve;
 	u64* keybits;  // OR, AND of the Morton codes of the current collide
 	bool defer_warm_start;  // nb_step: the warm start runs inside the first solver launch
 	// nb_step as a CUDA graph: captured once per (stream, parameters, scene shape), replayed afterwards
 	struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode; unsigned long long urow_version; } graph_key;
 	cudaGraphExec_t graph_exec; unsigned long long graph_launches; int graph_enabled; bool capturing;
 	int graph_is_coop;  // the recorded graph holds cooperative kernel nodes
-	int graph_coop;  // 1: grid-synchronising kernels keep the cooperative-launch attribute inside the captured graph (co-residency guaranteed by the driver)
+	int graph_coop;  // 1: grid-synchronising kernels keep the cooperative-launch attribute inside the captured graph (co-residency guaranteed by the driver); 0 once the driver refused it
 	u32* chain_start; u32* chain_len;  // per body: first entry / number of entries in the (body, batch) chain sort
 	bool contacts_internal;  // the current contact set came from nb_collide (not nb_upload_contacts)
-	u32 solve_backoff_ns;
 	// throughput mode (nb_set_solver_mode): mass-splitting Jacobi, nb_jacobi.cuh
-	int solver_mode; u32* jcnt; float4* jd; int jacobi_blocks1, jacobi_blocks2, jacobi_stages;
+	int solver_mode; u32* jcnt; float4* jd; int jacobi_blocks1, jacobi_blocks2;
 	// CUDA-event timing of the dominant solver kernel (nb_debug_timing): bench.py's roofline numerator is measured live
 	int timing; cudaEvent_t tev[2][64]; int tev_n; bool tev_made;
-	// nb_step overlaps independent branches of the step on a second stream (fork/join with events; also inside the captured graph)
-	bool rows_on_side, join_before_solve, zero_chain_len; int overlap; cudaStream_t side; cudaEvent_t ev_fork, ev_fork2, ev_join, ev_join2; u32* flags2; u32* offs2; u32* block_sums2;
+	bool zero_chain_len;  // nb_shard_step's dataflow solve: bodies without contacts on this rank must read chain length 0
 	// user constraint rows (nb_upload_constraint_rows, nb_rows_api.cuh)
 	float4* instances;   // nb_instance_matrices with a host destination (allocated on first use)
 	// nb_upload_bodies sends what the collision stage does not read (momentum, properties) on a second stream, so that copy runs under
@@ -61,8 +58,8 @@ struct nb_context {
 	u32* counts;
 	// collide
 	nb_transform* world_xf; float4* aabb_min; float4* aabb_max; u32* col_tag; u32* col_body; u32* order; u32* rank;
-	float4* tree_min; float4* tree_max;
-	u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask; int use_tree;
+	float4* leaf_min; float4* leaf_max;  // AABBs in Morton order
+	u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask;
 	SortBuffers sb; u32 sort_cap;
 	u64* pair_keys;  // alias into sb.keys[] after the pair sort
 	u64* pair_keys_debug;  // copy kept for parity tests when debug is enabled (the sort buffers are reused later in the step)
@@ -199,30 +196,24 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->counts, CNT__COUNT); ALLOC(ctx->keybits, 2);
 	ALLOC(ctx->world_xf, K); ALLOC(ctx->aabb_min, K); ALLOC(ctx->aabb_max, K); ALLOC(ctx->col_tag, K); ALLOC(ctx->col_body, K);
 	ALLOC(ctx->order, K); ALLOC(ctx->rank, K);
-	size_t tree_nodes = 0; { u32 n = K ? K : 1; tree_nodes = n; while (n > 8) { n = (n + 7) / 8; tree_nodes += n; } }
-	ALLOC(ctx->tree_min, tree_nodes + 8); ALLOC(ctx->tree_max, tree_nodes + 8);
+	ALLOC(ctx->leaf_min, K); ALLOC(ctx->leaf_max, K);
 	{
 		u32 tsz = 1024; while (tsz < 2 * (K ? K : 1)) tsz *= 2;
 		ctx->table_mask = tsz - 1;
 		ALLOC(ctx->mkeys, K); ALLOC(ctx->smallf, K); ALLOC(ctx->large_list, K); ALLOC(ctx->table_keys, tsz); ALLOC(ctx->table_vals, tsz);
-		const char* e = getenv("NB_BROADPHASE");
-		ctx->use_tree = e && !strcmp(e, "tree");
 	}
 	ctx->sort_cap = std::max(std::max(K, P), 2 * C);
 	for (int i = 0; i < 2; ++i) { ALLOC(ctx->sb.keys[i], ctx->sort_cap); ALLOC(ctx->sb.vals[i], ctx->sort_cap); }
-	ALLOC(ctx->sb.hist, 256 * NB_SORT_GRID);
+	ALLOC(ctx->sb.hist, 256 * (size_t)ctx->sms);
 	ctx->sb.bar = ctx->counts + CNT_BAR0;
-	{ const char* e = getenv("NB_SORT"); ctx->sb.coop_blocks = (e && !strcmp(e, "legacy")) ? 0 : ctx->sms; }
-	// Grid-synchronising kernels (one block per SM for the sort, the occupancy-derived grid for the solver) are launched as
-	// ordinary kernels unless NB_COOP_LAUNCH=1: the grid fits the idle device by construction, and a cooperative launch costs
-	// several microseconds more per launch.
+	// Grid-synchronising kernels (one block per SM for the sort, the occupancy-derived grid for the solver) are launched
+	// cooperatively, so the driver guarantees that their blocks are co-resident even with other work on the device.
+	ctx->sb.coop_launch = 1;
+	ctx->graph_coop = 1;
 	{ const char* e = getenv("NB_GRAPH"); ctx->graph_enabled = e ? atoi(e) != 0 : 1; }
-	{ const char* e = getenv("NB_GRAPH_COOP"); ctx->graph_coop = e ? atoi(e) != 0 : 1; }
-	{ const char* e = getenv("NB_COOP_LAUNCH"); ctx->coop_launch = e ? atoi(e) != 0 : NB_DEFAULT_COOP_LAUNCH; ctx->sb.coop_launch = ctx->coop_launch; }
 	CK(cudaFuncSetAttribute(k_sort_coop<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSortSmem)));
-	CK(cudaFuncSetAttribute(k_sort_coop<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSortSmem))); ALLOC(ctx->sb.block_sums, 8 * NB_SCAN_GRID);
+	CK(cudaFuncSetAttribute(k_sort_coop<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSortSmem)));
 	ALLOC(ctx->flags, 5 * (size_t)ctx->stride); ALLOC(ctx->offs, 5 * (size_t)ctx->stride); ALLOC(ctx->block_sums, 16 * NB_SCAN_GRID);
-	{ const char* e = getenv("NB_SCAN"); g_nb_scan_three_kernels = !(e && !strcmp(e, "single")); }  // the single-launch variant was the slower one where it was measured
 	ALLOC(ctx->live, P); ALLOC(ctx->np_pen, P); ALLOC(ctx->np_info, P); ALLOC(ctx->np_list, P); ALLOC(ctx->np_start, P);
 	ALLOC(ctx->staged.data, 2 * (size_t)C); ALLOC(ctx->staged.bodies, C); ALLOC(ctx->staged.tags, C); ALLOC(ctx->staged.features, C);
 	ALLOC(ctx->fin.data, 2 * (size_t)C); ALLOC(ctx->fin.bodies, C); ALLOC(ctx->fin.tags, C); ALLOC(ctx->fin.features, C);
@@ -241,13 +232,6 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->rows.a, ctx->cstride); ALLOC(ctx->rows.b, ctx->cstride); ALLOC(ctx->rows.contact, ctx->cstride); ALLOC(ctx->rows.wait, 2 * (size_t)ctx->cstride); ALLOC(ctx->chain_start, B); ALLOC(ctx->chain_len, B);
 	ctx->rows.stride = ctx->cstride;
 	ALLOC(ctx->jcnt, B); ALLOC(ctx->jd, 2 * (size_t)B);
-	ALLOC(ctx->flags2, ctx->stride); ALLOC(ctx->offs2, ctx->stride); ALLOC(ctx->block_sums2, 16 * NB_SCAN_GRID);
-	// The two branches on the second stream are short next to the sort / scheduler they run beside, and the extra graph edges cost
-	// what they save (no gain where it was measured; not measured on the H100).  Kept opt-in (NB_OVERLAP=1).
-	{ const char* e = getenv("NB_OVERLAP"); ctx->overlap = e ? atoi(e) != 0 : 0; }
-	CK(cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking));
-	CK(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ctx->ev_fork2, cudaEventDisableTiming));
-	CK(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ctx->ev_join2, cudaEventDisableTiming));
 	// upload of the rows `collide` does not read, on a copy stream of its own (NB_COPY_OVERLAP=0: everything on the caller's stream)
 	{ const char* e = getenv("NB_COPY_OVERLAP"); ctx->copy_overlap = e ? atoi(e) != 0 : 1; }
 	CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
@@ -264,8 +248,6 @@ int nb_create(const nb_config* config, nb_context** out) {
 		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per2, k_jacobi_sweep<false, 2>, NJ_TILE, sizeof(JacobiSmem<2>)));
 		if (per1 < 1 || per2 < 1) { ctx->error = "k_jacobi_sweep does not fit on an SM"; return NB_ERR_CUDA; }
 		ctx->jacobi_blocks1 = ctx->sms * per1; ctx->jacobi_blocks2 = ctx->sms * per2;   // persistent: every CTA walks tiles blockIdx.x, + gridDim.x, ...
-		ctx->jacobi_stages = 0;   // 0 = by body count at launch
-		if (const char* e = getenv("NB_JACOBI_STAGES")) ctx->jacobi_stages = atoi(e);
 		if (const char* e = getenv("NB_SOLVER")) ctx->solver_mode = !strcmp(e, "throughput") ? NB_SOLVER_THROUGHPUT : NB_SOLVER_PARITY;
 	}
 	ctx->pair_keys = ctx->sb.keys[0];
@@ -283,9 +265,6 @@ int nb_create(const nb_config* config, nb_context** out) {
 	int per_sm = 0;
 	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve, NB_BLOCK, 0));
 	if (per_sm < 1) { ctx->error = "k_solve does not fit on an SM"; return NB_ERR_CUDA; }
-	if (const char* e = getenv("NB_SOLVE_BLOCKS_PER_SM")) { int v = atoi(e); if (v >= 1 && v < per_sm) per_sm = v; }
-	ctx->solve_backoff_ns = 150;  // sleep per missing application while a contact is >= 2 applications away (nanosleep may take up to 2x)
-	if (const char* e = getenv("NB_SOLVE_HOP_NS")) ctx->solve_backoff_ns = (u32)atoi(e);
 	ctx->coop_blocks_solve = ctx->sms * per_sm;  // all co-resident: the dataflow solver relies on it
 	CK(cudaDeviceSynchronize());
 	return NB_OK;
@@ -297,7 +276,6 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->graph_exec) cudaGraphExecDestroy(ctx->graph_exec);
 	if (ctx->tev_made) for (int i = 0; i < 64; ++i) { cudaEventDestroy(ctx->tev[0][i]); cudaEventDestroy(ctx->tev[1][i]); }
 	if (ctx->copy_stream) { cudaStreamDestroy(ctx->copy_stream); cudaEventDestroy(ctx->ev_up_begin); cudaEventDestroy(ctx->ev_up_done); }
-	if (ctx->side) { cudaStreamDestroy(ctx->side); cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_fork2); cudaEventDestroy(ctx->ev_join); cudaEventDestroy(ctx->ev_join2); }
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
 	delete ctx;
 }
@@ -454,30 +432,14 @@ int nb_collide(nb_context* ctx, void* stream) {
 	ctx->launches += 2;
 	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
 	int cur = nb_radix_sort(L, ctx->sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, ctx->keybits);
-	Tree T;
-	{
-		size_t off = 0; u32 n = K; int l = 0;
-		while (true) { T.mn[l] = ctx->tree_min + off; T.mx[l] = ctx->tree_max + off; T.n[l] = n; off += n; ++l; if (n <= 8) break; n = (n + 7) / 8; }
-		T.levels = l;
-	}
-	k_leaves<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->aabb_min, ctx->aabb_max, ctx->order, ctx->rank, (float4*)T.mn[0], (float4*)T.mx[0], ctx->mkeys);
+	k_leaves<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->aabb_min, ctx->aabb_max, ctx->order, ctx->rank, ctx->leaf_min, ctx->leaf_max, ctx->mkeys);
 	++ctx->launches;
-	if (ctx->use_tree) {  // NB_BROADPHASE=tree: the implicit 8-ary AABB tree (kept for comparison)
-		for (int l = 1; l < T.levels; ++l) {
-			k_build_level<<<GRID(T.n[l]), NB_BLOCK, 0, st>>>(T.mn[l - 1], T.mx[l - 1], T.n[l - 1], (float4*)T.mn[l], (float4*)T.mx[l], T.n[l]);
-			++ctx->launches;
-		}
-		k_find_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(T, K, ctx->order, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-		++ctx->launches;
-	}
-	else {
-		CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
-		k_grid_setup<<<1, 1, 0, st>>>(K, counts);
-		k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, (float4*)T.mn[0], T.mx[0], ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
-		k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, T.mn[0], T.mx[0], ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-		k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, T.mn[0], T.mx[0], ctx->smallf, ctx->large_list, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-		ctx->launches += 4;
-	}
+	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
+	k_grid_setup<<<1, 1, 0, st>>>(K, counts);
+	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
+	k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	ctx->launches += 4;
 	k_clamp_count<<<1, 1, 0, st>>>(counts, CNT_PAIRS, ctx->cfg.max_pairs);
 	++ctx->launches;
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0);  // nudge.cpp:3498
@@ -544,16 +506,17 @@ int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, fl
 }
 
 // ---------------- contact cache ----------------
-// The two halves of read_cached_impulses are independent of each other: (a) the tag ORDER of the contacts (one sort), (b) the cache
-// LOOKUP of every contact's impulse plus the entries of sleeping pairs that survive the frame.  nb_step runs (b) on a second stream.
-static int read_lookup(nb_context* ctx, cudaStream_t st, u32* flags, u32* offs, u32* block_sums) {
-	Launch L = { st, &ctx->launches, ctx->sms };
-	u32* counts = ctx->counts;
+// The two halves of read_cached_impulses: (a) the tag ORDER of the contacts (one sort), (b) the cache LOOKUP of every contact's
+// impulse plus the entries of sleeping pairs that survive the frame.
+static int read_lookup(nb_context* ctx, void* stream) {
+	Launch L = mk_launch(ctx, stream);
+	cudaStream_t st = L.stream;
+	u32* counts = ctx->counts, *flags = ctx->flags, *offs = ctx->offs;
 	const u32 C = ctx->cfg.max_contacts, S = ctx->stride;
 	k_cache_lookup<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->fin.tags, ctx->fin.features, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->impulses, counts);
 	k_culled_flags<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->cache_tags, ctx->sleeping, flags, counts);
 	ctx->launches += 2;
-	nb_scan<1>(L, flags, offs, S, counts + CNT_CACHE, 0, block_sums, counts + CNT_CULLED);
+	nb_scan<1>(L, flags, offs, S, counts + CNT_CACHE, 0, ctx->block_sums, counts + CNT_CULLED);
 	k_culled_scatter<<<GRID(C), NB_BLOCK, 0, st>>>(flags, offs, ctx->cache_tags, ctx->cache_features, ctx->cache_data,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, counts);
 	++ctx->launches;
@@ -588,7 +551,7 @@ static int read_sort(nb_context* ctx, void* stream) {
 int nb_read_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_read_cached_impulses");
 	int r = read_sort(ctx, stream); if (r) return r;
-	return read_lookup(ctx, (cudaStream_t)stream, ctx->flags, ctx->offs, ctx->block_sums);
+	return read_lookup(ctx, stream);
 }
 
 int nb_write_cached_impulses(nb_context* ctx, void* stream) {
@@ -619,7 +582,7 @@ static int launch_solve_jacobi(nb_context* ctx, int mode, u32 sweeps, cudaStream
 	k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
 	++ctx->launches;
 	// two tiles per CTA in flight once the body arrays (64 B per body: velocities + accumulators) take a large share of L2, else more CTAs
-	const int stages = ctx->jacobi_stages == 1 || ctx->jacobi_stages == 2 ? ctx->jacobi_stages : (B > 600000u ? 2 : 1);
+	const int stages = B > 600000u ? 2 : 1;
 	if (mode == 0 || mode == 2) {
 		if (stages == 1) k_jacobi_sweep<true, 1><<<ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
 		else k_jacobi_sweep<true, 2><<<ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
@@ -646,10 +609,10 @@ static int launch_solve_core(nb_context* ctx, int mode, u32 sweeps, cudaStream_t
 	const float4* impulses = ctx->impulses;
 	float4* mw = ctx->mw;
 	u32* counts = ctx->counts;
-	u32 backoff = ctx->solve_backoff_ns;
+	u32 backoff = NB_SOLVE_BACKOFF_NS;
 	void* args[] = { &R, &impulses, &mw, &mode, &sweeps, &backoff, &counts };
 	if (mode) timing_begin(ctx, st);
-	if (ctx->coop_launch && (!ctx->capturing || ctx->graph_coop)) CK(cudaLaunchCooperativeKernel((void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
+	if (!ctx->capturing || ctx->graph_coop) CK(cudaLaunchCooperativeKernel((void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
 	else k_solve<<<ctx->coop_blocks_solve, NB_BLOCK, 0, st>>>(R, impulses, mw, mode, sweeps, backoff, counts);
 	if (mode) timing_end(ctx, st);
 	++ctx->launches;
@@ -682,7 +645,6 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, ctx->rows, counts, ctx->jcnt);
 		ctx->launches += 3;
 		if (!ctx->defer_warm_start) {
-			if (ctx->join_before_solve) { ctx->join_before_solve = false; CK(cudaStreamWaitEvent(st, ctx->ev_join, 0)); }   // the warm start reads the looked-up impulses
 			int r = launch_solve(ctx, 0, 1, st); if (r) return r; if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
 		}
 		CK(cudaGetLastError());
@@ -702,20 +664,13 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	k_batch_index<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
 		ctx->offs, ctx->left_count, ctx->batch_of, ctx->slot_idx, ctx->rows.contact, ctx->cstride, ctx->sb.keys[0], ctx->sb.vals[0], ctx->batchbits, B, dummy_span, counts);
 	++ctx->launches;
-	if (ctx->rows_on_side) CK(cudaEventRecord(ctx->ev_fork2, st));   // slots are final here
 	int cur = nb_radix_sort(L, ctx->sb, counts + CNT_ENTRIES, 0, (int)(chain_bodybits + ctx->batchbits), true, 0);
 	if (ctx->zero_chain_len) CK(cudaMemsetAsync(ctx->chain_len, 0, sizeof(u32) * B, st));
 	k_chain_heads<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sb.keys[cur], ctx->batchbits, B, ctx->chain_start, ctx->chain_len, counts); ++ctx->launches;
 	k_waits<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sb.keys[cur], ctx->sb.vals[cur], ctx->batchbits, B, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->rows.wait, ctx->cstride, counts);
-	// the rows only need the slot of every contact (k_batch_index), not the chains: inside nb_step they are built on the second stream
-	// while the chain sort runs (rows_stream != st; joined before the solver)
-	cudaStream_t rows_stream = ctx->rows_on_side ? ctx->side : st;
-	if (ctx->rows_on_side) CK(cudaStreamWaitEvent(ctx->side, ctx->ev_fork2, 0));
-	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, rows_stream>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, ctx->rows, counts, nullptr);
-	if (ctx->rows_on_side) { CK(cudaEventRecord(ctx->ev_join2, ctx->side)); CK(cudaStreamWaitEvent(st, ctx->ev_join2, 0)); }
+	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, ctx->rows, counts, nullptr);
 	ctx->launches += 2;
 	if (!ctx->defer_warm_start) {  // warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
-		if (ctx->join_before_solve) { ctx->join_before_solve = false; CK(cudaStreamWaitEvent(st, ctx->ev_join, 0)); }
 		int r = launch_solve(ctx, 0, 1, st); if (r) return r;
 		if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
 	}
@@ -761,25 +716,11 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 	int r;
 	if ((r = nb_collide(ctx, stream))) return r;
 	if ((r = nb_apply_gravity_damping(ctx, time_step, gravity, damping, stream))) return r;
-	const bool fork = ctx->overlap && stream != nullptr && !ctx->debug;
-	cudaStream_t st = (cudaStream_t)stream;
-	if (fork) {
-		// branch A on the second stream: cache lookup + culled entries (needs the contacts and the sorted sleeping pairs, not the tag order);
-		// it joins before the solver's warm start reads the impulses.  Own scan scratch: the scheduler uses the main one meanwhile.
-		CK(cudaEventRecord(ctx->ev_fork, st)); CK(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0));
-		if ((r = read_lookup(ctx, ctx->side, ctx->flags2, ctx->offs2, ctx->block_sums2))) return r;
-		CK(cudaEventRecord(ctx->ev_join, ctx->side));
-		if ((r = read_sort(ctx, stream))) return r;
-	}
-	else if ((r = nb_read_cached_impulses(ctx, stream))) return r;
+	if ((r = nb_read_cached_impulses(ctx, stream))) return r;
 	ctx->defer_warm_start = iterations > 0 && !ctx->urow_n;  // warm start + sweeps in one solver launch (same arithmetic, same order); not with user rows between the sweeps
-	ctx->rows_on_side = fork && ctx->solver_mode == NB_SOLVER_PARITY;   // branch B: constraint rows while the chain sort runs
-	ctx->join_before_solve = fork;
 	r = nb_setup_contact_constraints(ctx, stream);
-	ctx->rows_on_side = false;
-	if (!r && ctx->join_before_solve) { ctx->join_before_solve = false; CK(cudaStreamWaitEvent(st, ctx->ev_join, 0)); }   // (setup joins itself when it runs the warm start)
 	if (!r) r = nb_apply_impulses(ctx, iterations, stream);
-	ctx->defer_warm_start = false; ctx->join_before_solve = false;
+	ctx->defer_warm_start = false;
 	if (r) return r;
 	if ((r = nb_update_cached_impulses(ctx, stream))) return r;
 	if ((r = nb_write_cached_impulses(ctx, stream))) return r;

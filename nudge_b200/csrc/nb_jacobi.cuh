@@ -38,8 +38,7 @@
 // STAGES shared-memory stages per CTA.  A thread moves its 46 values into registers as soon as a tile has landed, so the registers are
 // one more stage of the ring and a shared stage can be refilled at once.  STAGES = 1: 47 KB per CTA, three CTAs (24 warps) per SM —
 // meant for body arrays that are small next to L2;  STAGES = 2: 94 KB, two CTAs per SM but two tiles per CTA in flight — meant for
-// scenes of a million bodies, whose gathers miss L2 (the choice is not yet re-measured on the H100).  nb_api.cu picks by body count
-// (NB_JACOBI_STAGES overrides).
+// scenes of a million bodies, whose gathers miss L2 (the choice is not yet re-measured on the H100).  nb_api.cu picks by body count.
 template<int STAGES>
 struct JacobiSmem {
 	float tile[STAGES][NJ_PLANES][NJ_TILE];

@@ -127,207 +127,12 @@ __global__ void __launch_bounds__(NB_BLOCK) k_scan_down(const u32* in, u32* out,
 	}
 }
 
-// The same scan in ONE launch (decoupled look-back): every block sums its range and publishes (flag | sum) per counter, the
-// first warp looks back over its predecessors' words 32 at a time until it meets an inclusive prefix, publishes its own, and the
-// block writes its outputs.  status: u64[N][grid] + one u32 completion counter behind it, all zero between launches (the last
-// block to finish its look-back clears them, so a launch needs no host-side epoch and replays from a CUDA graph).
-#define NB_SCAN_AGG  ((u64)1 << 32)
-#define NB_SCAN_INCL ((u64)2 << 32)
 template<int N>
-__global__ void __launch_bounds__(NB_BLOCK) k_scan_single(const u32* in, u32* out, u32 stride, const u32* n_ptr, u32 n_host, u64* status, u32* totals) {
-	__shared__ u32 sm[NB_WARPS + 1];
-	__shared__ u32 s_excl[N];
-	const u32 G = gridDim.x, b = blockIdx.x, lane = threadIdx.x & 31;
-	u32* done = reinterpret_cast<u32*>(status + (size_t)N * G);
-	u32 n = n_ptr ? *n_ptr : n_host;
-	u32 begin, end; scan_tile_range(n, begin, end);
-	u32 acc[N];
-	#pragma unroll
-	for (int c = 0; c < N; ++c) acc[c] = 0;
-	for (u32 i = begin + threadIdx.x; i < end; i += NB_BLOCK)
-		#pragma unroll
-		for (int c = 0; c < N; ++c) acc[c] += in[c*stride + i];
-	u32 sum[N];
-	#pragma unroll
-	for (int c = 0; c < N; ++c) { block_excl_scan(acc[c], &sum[c], sm); }
-	if (threadIdx.x < 32) {
-		volatile u64* st = status;
-		if (lane == 0) {
-			#pragma unroll
-			for (int c = 0; c < N; ++c) st[(size_t)c * G + b] = (b ? NB_SCAN_AGG : NB_SCAN_INCL) | sum[c];
-		}
-		u32 excl[N];
-		#pragma unroll
-		for (int c = 0; c < N; ++c) excl[c] = 0;
-		u32 open_mask = (1u << N) - 1u;  // counters whose look-back has not met an inclusive prefix yet
-		for (int j = (int)b - 1; j >= 0 && open_mask; j -= 32) {  // window j, j-1, ..., j-31; all counters in one round trip
-			int idx = j - (int)lane;
-			u64 w[N];
-			#pragma unroll
-			for (int c = 0; c < N; ++c) {
-				w[c] = NB_SCAN_INCL;  // lanes before block 0 read as "inclusive prefix 0"
-				if (idx >= 0 && ((open_mask >> c) & 1)) w[c] = st[(size_t)c * G + idx];
-			}
-			#pragma unroll
-			for (int c = 0; c < N; ++c) {
-				if (!((open_mask >> c) & 1)) continue;
-				if (idx >= 0) while ((w[c] >> 32) == 0) w[c] = st[(size_t)c * G + idx];
-				u32 incl_mask = __ballot_sync(0xffffffffu, (w[c] >> 32) == 2);
-				u32 upto = incl_mask ? (u32)__ffs(incl_mask) - 1 : 31;  // nearest inclusive prefix in the window, if any
-				u32 v = lane <= upto ? (u32)w[c] : 0;
-				#pragma unroll
-				for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-				excl[c] += v;
-				if (incl_mask) open_mask &= ~(1u << c);
-			}
-		}
-		if (lane == 0) {
-			#pragma unroll
-			for (int c = 0; c < N; ++c) {
-				if (b) st[(size_t)c * G + b] = NB_SCAN_INCL | (u32)(excl[c] + sum[c]);
-				s_excl[c] = excl[c];
-				if (b == G - 1 && totals) totals[c] = excl[c] + sum[c];
-			}
-		}
-		__syncwarp();
-		u32 last = 0;
-		if (lane == 0) { __threadfence(); last = atomicAdd(done, 1u) == G - 1; }
-		if (__shfl_sync(0xffffffffu, last, 0)) {  // every look-back is over: clear the words for the next launch
-			for (u32 i = lane; i < (u32)N * G; i += 32) status[i] = 0;
-			if (lane == 0) *done = 0;
-		}
-	}
-	__syncthreads();
-	u32 run[N];
-	#pragma unroll
-	for (int c = 0; c < N; ++c) run[c] = s_excl[c];
-	for (u32 base = begin; base < end; base += NB_BLOCK * NB_SCAN_ITEMS) {
-		u32 i0 = base + threadIdx.x * NB_SCAN_ITEMS;
-		#pragma unroll
-		for (int c = 0; c < N; ++c) {
-			u32 v[NB_SCAN_ITEMS]; u32 s = 0;
-			#pragma unroll
-			for (int k = 0; k < NB_SCAN_ITEMS; ++k) { v[k] = (i0 + k < end) ? in[c*stride + i0 + k] : 0; s += v[k]; }
-			u32 total; u32 ex = block_excl_scan(s, &total, sm) + run[c];
-			#pragma unroll
-			for (int k = 0; k < NB_SCAN_ITEMS; ++k) { if (i0 + k < end) out[c*stride + i0 + k] = ex; ex += v[k]; }
-			run[c] += total;
-		}
-	}
-}
-
-static bool g_nb_scan_three_kernels = true;  // NB_SCAN=single selects k_scan_single (the slower one where it was measured; not measured on the H100)
-template<int N>
-static void nb_scan(const Launch& L, const u32* in, u32* out, u32 stride, const u32* n_ptr, u32 n_host, u32* block_sums /*16*NB_SCAN_GRID, zero*/, u32* totals) {
-	if (!g_nb_scan_three_kernels) {
-		k_scan_single<N><<<L.sms, NB_BLOCK, 0, L.stream>>>(in, out, stride, n_ptr, n_host, reinterpret_cast<u64*>(block_sums), totals);
-		*L.counter += 1;
-		return;
-	}
+static void nb_scan(const Launch& L, const u32* in, u32* out, u32 stride, const u32* n_ptr, u32 n_host, u32* block_sums /*N*NB_SCAN_GRID*/, u32* totals) {
 	k_scan_reduce<N><<<NB_SCAN_GRID, NB_BLOCK, 0, L.stream>>>(in, stride, n_ptr, n_host, block_sums);
 	k_scan_spine<N><<<1, 1024, 0, L.stream>>>(block_sums, totals);
 	k_scan_down<N><<<NB_SCAN_GRID, NB_BLOCK, 0, L.stream>>>(in, out, stride, n_ptr, n_host, block_sums);
 	*L.counter += 3;
-}
-
-// ---------------- stable LSD radix sort, 8 bits per pass, u64 keys + u32 payload ----------------
-#define NB_SORT_GRID 592
-
-NB_DEV void sort_tile_range(u32 n, u32& begin, u32& end) {
-	u32 chunks = (n + NB_BLOCK - 1) / NB_BLOCK;
-	u32 per = (chunks + gridDim.x - 1) / gridDim.x;
-	begin = min(n, blockIdx.x * per * NB_BLOCK);
-	end = min(n, begin + per * NB_BLOCK);
-}
-
-__global__ void __launch_bounds__(NB_BLOCK) k_sort_hist(const u64* keys, const u32* n_ptr, u32 shift, u32* hist /*[256][NB_SORT_GRID]*/) {
-	__shared__ u32 h[256];
-	h[threadIdx.x] = 0;
-	__syncthreads();
-	u32 n = *n_ptr;
-	u32 begin, end; sort_tile_range(n, begin, end);
-	for (u32 i = begin + threadIdx.x; i < end; i += NB_BLOCK)
-		atomicAdd(&h[(u32)(keys[i] >> shift) & 0xff], 1u);
-	__syncthreads();
-	hist[threadIdx.x * NB_SORT_GRID + blockIdx.x] = h[threadIdx.x];
-}
-
-template<bool HAS_VALS>
-__global__ void __launch_bounds__(NB_BLOCK) k_sort_scatter(const u64* keys_in, u64* keys_out, const u32* vals_in, u32* vals_out,
-															const u32* n_ptr, u32 shift, const u32* hist_scanned, const u32* digit_base) {
-	__shared__ u32 running[256];
-	__shared__ u32 chunk_base[256];
-	__shared__ u32 wc[NB_WARPS][256];
-	u32 n = *n_ptr;
-	u32 begin, end; sort_tile_range(n, begin, end);
-	running[threadIdx.x] = digit_base[threadIdx.x] + hist_scanned[threadIdx.x * NB_SORT_GRID + blockIdx.x];
-	u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	for (u32 base = begin; base < end; base += NB_BLOCK) {
-		u32 i = base + threadIdx.x;
-		bool valid = i < end;
-		u64 key = valid ? keys_in[i] : 0;
-		u32 val = (HAS_VALS && valid) ? vals_in[i] : 0;
-		u32 d = valid ? ((u32)(key >> shift) & 0xff) : 0xffffffffu;
-		u32 peers = __match_any_sync(0xffffffffu, d);
-		u32 rank = __popc(peers & ((1u << lane) - 1u));
-		#pragma unroll
-		for (int w = 0; w < NB_WARPS; ++w) wc[w][threadIdx.x] = 0;
-		__syncthreads();
-		if (valid && rank == 0) wc[wid][d] = __popc(peers);
-		__syncthreads();
-		{
-			u32 sum = 0;
-			#pragma unroll
-			for (int w = 0; w < NB_WARPS; ++w) { u32 c = wc[w][threadIdx.x]; wc[w][threadIdx.x] = sum; sum += c; }
-			u32 b = running[threadIdx.x];
-			chunk_base[threadIdx.x] = b;
-			running[threadIdx.x] = b + sum;
-		}
-		__syncthreads();
-		if (valid) {
-			u32 pos = chunk_base[d] + wc[wid][d] + rank;
-			keys_out[pos] = key;
-			if (HAS_VALS) vals_out[pos] = val;
-		}
-		__syncthreads();
-	}
-}
-
-// Turns the block histogram hist[digit][block] into scatter offsets in ONE launch: block d scans row d in place (exclusive over
-// the sort blocks) and publishes the digit total; the last block to finish (completion counter) prefixes the 256 totals into
-// digit_base[].  A key's final position is digit_base[d] + hist[d][block] + its rank inside the block.
-__global__ void __launch_bounds__(1024) k_sort_offsets(u32* hist /*[256][NB_SORT_GRID]*/, u32* digit_base /*[256] + [256] totals + [1] counter*/) {
-	__shared__ u32 sm[33];
-	__shared__ bool last;
-	const u32 d = blockIdx.x;
-	u32* totals = digit_base + 256;
-	u32* counter = digit_base + 512;
-	u32 v = threadIdx.x < NB_SORT_GRID ? hist[d * NB_SORT_GRID + threadIdx.x] : 0;
-	u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-	u32 incl = warp_incl_scan(v);
-	if (lane == 31) sm[wid] = incl;
-	__syncthreads();
-	if (wid == 0) { u32 w = sm[lane]; u32 wi = warp_incl_scan(w); sm[lane] = wi - w; if (lane == 31) sm[32] = wi; }
-	__syncthreads();
-	if (threadIdx.x < NB_SORT_GRID) hist[d * NB_SORT_GRID + threadIdx.x] = incl - v + sm[wid];
-	if (threadIdx.x == 0) {
-		totals[d] = sm[32];
-		__threadfence();
-		last = atomicAdd(counter, 1u) == gridDim.x - 1;
-	}
-	__syncthreads();
-	if (last) {
-		__threadfence();
-		u32 t = threadIdx.x < 256 ? ((volatile u32*)totals)[threadIdx.x] : 0;
-		u32 inc2 = warp_incl_scan(t);
-		__syncthreads();
-		if (lane == 31) sm[wid] = inc2;
-		__syncthreads();
-		if (wid == 0) { u32 w = sm[lane]; u32 wi = warp_incl_scan(w); sm[lane] = wi - w; }
-		__syncthreads();
-		if (threadIdx.x < 256) digit_base[threadIdx.x] = inc2 - t + sm[wid];
-		if (threadIdx.x == 0) *counter = 0;  // ready for the next pass
-	}
 }
 
 // ---------------- grid-wide barrier for cooperative (co-resident) launches ----------------
@@ -365,7 +170,7 @@ NB_DEV void grid_barrier(u32* bar /* [0]=arrivals, [1]=generation */, u32 nblock
 //                       memory when it has <= NB_CS_CAP keys, tile by tile through global memory when it is larger (a hot
 //                       key).  Two grid barriers per SORT instead of two per digit.
 //   a bucket > 8 caps   (very skewed keys, or large n): plain LSD over all digits, two grid barriers per digit.
-// The result always lands in k1/v1.  Stable, same order as nb_radix_sort.  n == 0 costs one empty launch.
+// The result always lands in k1/v1.  Stable.  n == 0 costs one empty launch.
 #define NB_CS_THREADS 1024
 #define NB_CS_WARPS 32
 #define NB_CS_ITEMS 4                       // keys per thread while scattering through global memory
@@ -701,40 +506,28 @@ __global__ void __launch_bounds__(NB_CS_THREADS) k_sort_coop(u64* k0, u64* k1, u
 		for (u32 i = blockIdx.x * NB_CS_THREADS + tid; i < n; i += G * NB_CS_THREADS) { k1[i] = __ldcg(k0 + i); if (HAS_VALS) v1[i] = __ldcg(v0 + i); }
 }
 
-struct SortBuffers { u64* keys[2]; u32* vals[2]; u32* hist; u32* block_sums; u32* bar; int coop_blocks; /* 0 = three launches per pass */ int coop_launch; };
+struct SortBuffers { u64* keys[2]; u32* vals[2]; u32* hist /*[L.sms][256]*/; u32* bar; int coop_launch; /* 0: ordinary launch, in a graph capture's non-cooperative attempt */ };
 
-// Sorts bits [begin_bit, end_bit) of keys[cur] (+vals[cur]); returns which buffer (0/1) holds the result.
+// Sorts bits [begin_bit, end_bit) of keys[cur] (+vals[cur]), then stably on [begin_bit2, end_bit2); returns which buffer (0/1)
+// holds the result.  One k_sort_coop launch, one block per SM.
 static int nb_radix_sort(const Launch& L, const SortBuffers& B, const u32* n_ptr, int begin_bit, int end_bit, bool has_vals, int cur, int begin_bit2 = 0, int end_bit2 = 0, const u64* keybits = nullptr) {
-	if (B.coop_blocks) {
-		// 8-bit digits, top-aligned per bit range; the lowest digit of a range may overlap the next one (harmless for LSD order)
-		SortPasses P; P.n = 0;
-		auto add_range = [&](int lo, int hi) {
-			int first = P.n;
-			for (int shift = hi - 8; shift > lo; shift -= 8) P.shift[P.n++] = shift;
-			if (hi > lo) P.shift[P.n++] = lo;
-			for (int i = first, j = P.n - 1; i < j; ++i, --j) { int t = P.shift[i]; P.shift[i] = P.shift[j]; P.shift[j] = t; }  // ascending
-		};
-		add_range(begin_bit, end_bit);
-		add_range(begin_bit2, end_bit2);
-		u64* k0 = B.keys[cur]; u64* k1 = B.keys[cur ^ 1]; u32* v0 = B.vals[cur]; u32* v1 = B.vals[cur ^ 1]; u32* hist = B.hist; u32* bar = B.bar;
-		void* args[] = { &k0, &k1, &v0, &v1, &n_ptr, &hist, &bar, &P, &keybits };
-		if (B.coop_launch) cudaLaunchCooperativeKernel(has_vals ? (void*)k_sort_coop<true> : (void*)k_sort_coop<false>, dim3(B.coop_blocks), dim3(NB_CS_THREADS), args, sizeof(CoopSortSmem), L.stream);
-		else if (has_vals) k_sort_coop<true><<<B.coop_blocks, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits);
-		else k_sort_coop<false><<<B.coop_blocks, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits);
-		*L.counter += 1;
-		return cur ^ 1;
-	}
-	if (end_bit2 > begin_bit2) { cur = nb_radix_sort(L, B, n_ptr, begin_bit, end_bit, has_vals, cur); begin_bit = begin_bit2; end_bit = end_bit2; }
-	for (int shift = begin_bit; shift < end_bit; shift += 8) {
-		k_sort_hist<<<NB_SORT_GRID, NB_BLOCK, 0, L.stream>>>(B.keys[cur], n_ptr, (u32)shift, B.hist);
-		*L.counter += 1;
-		k_sort_offsets<<<256, 1024, 0, L.stream>>>(B.hist, B.block_sums);
-		if (has_vals) k_sort_scatter<true><<<NB_SORT_GRID, NB_BLOCK, 0, L.stream>>>(B.keys[cur], B.keys[cur ^ 1], B.vals[cur], B.vals[cur ^ 1], n_ptr, (u32)shift, B.hist, B.block_sums);
-		else k_sort_scatter<false><<<NB_SORT_GRID, NB_BLOCK, 0, L.stream>>>(B.keys[cur], B.keys[cur ^ 1], nullptr, nullptr, n_ptr, (u32)shift, B.hist, B.block_sums);
-		*L.counter += 2;
-		cur ^= 1;
-	}
-	return cur;
+	// 8-bit digits, top-aligned per bit range; the lowest digit of a range may overlap the next one (harmless for LSD order)
+	SortPasses P; P.n = 0;
+	auto add_range = [&](int lo, int hi) {
+		int first = P.n;
+		for (int shift = hi - 8; shift > lo; shift -= 8) P.shift[P.n++] = shift;
+		if (hi > lo) P.shift[P.n++] = lo;
+		for (int i = first, j = P.n - 1; i < j; ++i, --j) { int t = P.shift[i]; P.shift[i] = P.shift[j]; P.shift[j] = t; }  // ascending
+	};
+	add_range(begin_bit, end_bit);
+	add_range(begin_bit2, end_bit2);
+	u64* k0 = B.keys[cur]; u64* k1 = B.keys[cur ^ 1]; u32* v0 = B.vals[cur]; u32* v1 = B.vals[cur ^ 1]; u32* hist = B.hist; u32* bar = B.bar;
+	void* args[] = { &k0, &k1, &v0, &v1, &n_ptr, &hist, &bar, &P, &keybits };
+	if (B.coop_launch) cudaLaunchCooperativeKernel(has_vals ? (void*)k_sort_coop<true> : (void*)k_sort_coop<false>, dim3(L.sms), dim3(NB_CS_THREADS), args, sizeof(CoopSortSmem), L.stream);
+	else if (has_vals) k_sort_coop<true><<<L.sms, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits);
+	else k_sort_coop<false><<<L.sms, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits);
+	*L.counter += 1;
+	return cur ^ 1;
 }
 
 // ---------------- warp-aggregated append ----------------

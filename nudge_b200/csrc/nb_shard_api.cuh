@@ -215,11 +215,11 @@ static int shard_solve_flow(nb_shard* sh, uint32_t iterations, cudaStream_t st) 
 	X.export_row = sh->d_export_row; X.ghost_slot = sh->d_ghost_slot; X.ghost_cap = sh->ghost_cap; X.passes_cap = sh->passes_cap;
 	const u32 passes = iterations + 1;
 	k_mw_in_flow<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, ctx->chain_len, X, P, sh->epoch, passes); ++ctx->launches;
-	Rows R = ctx->rows; const float4* impulses = ctx->impulses; float4* mw = ctx->mw; u32* counts = ctx->counts; u32 hop = ctx->solve_backoff_ns; u32 sweeps = iterations;
+	Rows R = ctx->rows; const float4* impulses = ctx->impulses; float4* mw = ctx->mw; u32* counts = ctx->counts; u32 hop = NB_SOLVE_BACKOFF_NS; u32 sweeps = iterations;
 	const u32* epoch = sh->epoch; long long timeout = sh->pull_timeout_cycles;
 	void* args[] = { &R, &impulses, &mw, &sweeps, &hop, &counts, &X, (void*)&P, &epoch, &timeout };
 	timing_begin(ctx, st);
-	if (ctx->coop_launch && (!ctx->capturing || ctx->graph_coop)) SCK(cudaLaunchCooperativeKernel((void*)k_solve_flow, dim3(sh->flow_blocks), dim3(NB_BLOCK), args, 0, st));
+	if (!ctx->capturing || ctx->graph_coop) SCK(cudaLaunchCooperativeKernel((void*)k_solve_flow, dim3(sh->flow_blocks), dim3(NB_BLOCK), args, 0, st));
 	else k_solve_flow<<<sh->flow_blocks, NB_BLOCK, 0, st>>>(R, impulses, mw, sweeps, hop, counts, X, P, epoch, timeout);
 	timing_end(ctx, st);
 	++ctx->launches;

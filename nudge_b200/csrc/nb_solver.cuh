@@ -752,6 +752,7 @@ NB_DEV void solve_contact(const Rows& R, u32 j, const float (&rv)[ROW_PLANES_TOT
 // Waiting: the body's token says how many applications are still ahead of this contact (k_chain_heads).  While that number is
 // >= 2 on either body only the linear halves are polled, and the warp sleeps hop_ns per missing application when all of its
 // lanes are that far away; from 1 on, all four halves are fetched in one round trip so the hand-off costs a single L2 access.
+#define NB_SOLVE_BACKOFF_NS 150u  // hop_ns of k_solve and k_solve_flow (__nanosleep may sleep up to twice as long)
 __global__ void __launch_bounds__(NB_BLOCK, 2) k_solve(Rows R, const float4* impulses, float4* mw, int mode, u32 sweeps, u32 hop_ns, u32* counts) {
 	__shared__ u32 s_rcp[2048];
 	__shared__ u32 s_rsqrt[2048];
