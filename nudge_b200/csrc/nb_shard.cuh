@@ -218,7 +218,7 @@ NB_DEV void flow_publish(const ShardFlow& X, const ShardPlanDev& P, u32 row, u32
 }
 
 // working copy like k_mw_in; an exported body WITHOUT contacts on this rank never gets a "last contact": its (unchanging) row is
-// published for every pass up front.  chain_len must be zero for bodies without chain entries (memset before k_chain_heads).
+// published for every pass up front.  chain_len is zero for bodies without chain entries (memset before k_batch_index counts them).
 __global__ void __launch_bounds__(NB_BLOCK) k_mw_in_flow(u32 B, const nb_body_momentum* momentum, float4* mw, const u32* chain_len, ShardFlow X, ShardPlanDev P, const u32* epoch, u32 passes) {
 	const u32 ep = *epoch + 1;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {

@@ -239,9 +239,8 @@ static int shard_step_body(nb_shard* sh, float time_step, uint32_t iterations, f
 	if (sh->world > 1 && transport == NB_SHARD_PEER && sh->fuse && sh->peers_ready && ctx->solver_mode == NB_SOLVER_PARITY && !ctx->urow_n) {
 		const bool flow = sh->fuse == 2 && sh->flow_blocks > 0 && iterations > 0 && iterations + 1 <= sh->passes_cap;
 		ctx->defer_warm_start = true;                          // setup without its warm-start launch: it runs inside the fused solve
-		ctx->zero_chain_len = flow;                            // "no contacts on this rank" must read as chain length 0
-		r = nb_setup_contact_constraints(ctx, stream);
-		ctx->defer_warm_start = false; ctx->zero_chain_len = false;
+		r = nb_setup_contact_constraints(ctx, stream);         // (chain_len reads 0 for bodies without contacts on this rank)
+		ctx->defer_warm_start = false;
 		if (r) return r;
 		if ((r = flow ? shard_solve_flow(sh, iterations, (cudaStream_t)stream) : shard_solve_fused(sh, iterations, (cudaStream_t)stream))) return r;
 		if ((r = nb_update_cached_impulses(ctx, stream))) return r;

@@ -82,11 +82,12 @@ __global__ void __launch_bounds__(NB_BLOCK) k_culled_flags(const u64* cache_tags
 		flags[e] = (lo < s && sleeping[lo] == t) ? 1u : 0u;
 	}
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_culled_scatter(const u32* flags, const u32* offs, const u64* cache_tags, const u32* cache_features, const float4* cache_data,
+// NB_SCAN_GRID blocks, after nb_scan_reduce<1> over the flags
+__global__ void __launch_bounds__(NB_BLOCK) k_culled_scatter(const u32* flags, const u32* block_sums, const u64* cache_tags, const u32* cache_features, const float4* cache_data,
 															 u64* culled_tags, u32* culled_features, float4* culled_data, const u32* counts) {
-	u32 m = counts[CNT_CACHE];
-	for (u32 e = blockIdx.x * blockDim.x + threadIdx.x; e < m; e += gridDim.x * blockDim.x)
-		if (flags[e]) { u32 d = offs[e]; culled_tags[d] = cache_tags[e]; culled_features[d] = cache_features[e]; culled_data[d] = cache_data[e]; }
+	scan_consume<1>(flags, 0, counts[CNT_CACHE], block_sums, [&](u32 e, const u32 (&v)[1], const u32 (&d)[1]) {
+		if (v[0]) { culled_tags[d[0]] = cache_tags[e]; culled_features[d[0]] = cache_features[e]; culled_data[d[0]] = cache_data[e]; }
+	});
 }
 
 // ---------------- contact cache write: 2-way merge by rank (nudge.cpp:4110-4158) ----------------
@@ -393,10 +394,10 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 	for (u32 k = lane; k < spill_high * 16; k += 32) G_ent[k] = NB_NONE;   // leave the spill area empty for the next launch
 }
 
-// batch index and slot (batch*8 + lane) of every contact + the (body, batch) chain entries
+// batch index and slot (batch*8 + lane) of every contact + the length of every body's chain (chain_len: zero on entry)
 __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, const uint2* bodies, const u32* slot_of, const u32* slot_done, const u32* slot_left,
 		u32 slots_per_bucket, const u32* complete_off, const u32* left_count, u32* batch_of, u32* slot_idx, u32* slot_contact, u32 max_slots,
-		u64* chain_keys, u32* chain_vals, u32 batchbits, u32 nbodies, u32 dummy_span, u32* counts) {
+		u32* chain_len, u32* counts) {
 	u32 n = counts[CNT_CONTACTS];
 	u32 nfull = counts[CNT_FULL_BATCHES];
 	u32 left_base[17]; left_base[0] = 0;
@@ -411,6 +412,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, con
 		u32 nb = nfull + left_base[16];
 		if (sched_ovf) { atomicOr(&counts[CNT_OVERFLOW], OVF_SCHED); nb = 0; }
 		counts[CNT_BATCHES] = nb; counts[CNT_ENTRIES] = sched_ovf ? 0 : 2 * n;
+		counts[CNT_CHAIN_CURSOR] = 0;
 	}
 	if (sched_ovf) return;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -422,44 +424,61 @@ __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, con
 		slot_idx[i] = slot;
 		if (slot < max_slots) slot_contact[slot] = sorted[i];
 		uint2 ab = bodies[sorted[i]];
-		// A side on the static world (body 0) has no chain.  Its entry still goes through the sort, as a DUMMY whose body field lies beyond
-		// the real bodies, spread evenly over [nbodies, nbodies + dummy_span): one shared key (round 1) put every ground contact of
-		// the pile - 10 % of all entries - into a single sort bucket, the slowest block of the step.
-		const u64 dummy = ((u64)(nbodies + i % dummy_span) << batchbits) | batch;
-		chain_keys[2*i] = ab.x ? (((u64)ab.x << batchbits) | batch) : dummy;
-		chain_keys[2*i + 1] = ab.y ? (((u64)ab.y << batchbits) | batch) : dummy;
-		chain_vals[2*i] = 2*i; chain_vals[2*i + 1] = 2*i + 1;
+		if (ab.x) atomicAdd(&chain_len[ab.x], 1u);   // a side on the static world (body 0) has no chain
+		if (ab.y) atomicAdd(&chain_len[ab.y], 1u);
 	}
 }
 
-// For each contact side: the slot whose token it must see on that body before it may run.  In (body, batch) order the
-// predecessor is the previous entry of the same body; the first entry of a body waits for the body's LAST entry of the
-// previous sweep (flag bit 31).  Body 0 (static world) is never waited for.
-// Per body the solver keeps a sequence token = number of contact applications the body has received in this launch.  The
-// contact at position `seq` of a body's chain of length `len` therefore runs in sweep w when the token reads w*len + seq, and
-// leaves w*len + seq + 1.  (expected - seen) is the number of applications still ahead of a waiting contact, which is what the
-// solver's back-off sleeps on.  Body 0 (static world) is never waited for: its entries carry the key ~0.
-__global__ void __launch_bounds__(NB_BLOCK) k_chain_heads(const u64* chain_keys, u32 batchbits, u32 nbodies, u32* chain_start, u32* chain_len, const u32* counts) {
-	u32 n2 = counts[CNT_ENTRIES];
-	for (u32 e = blockIdx.x * blockDim.x + threadIdx.x; e < n2; e += gridDim.x * blockDim.x) {
-		u64 k = chain_keys[e];
-		u64 body = k >> batchbits;
-		if (body >= nbodies) continue;   // dummy entry of a static-world side
-		if (e > 0 && (chain_keys[e - 1] >> batchbits) == body) continue;
-		u32 lo = e, hi = n2;  // first index with a larger body
-		while (lo < hi) { u32 mid = (lo + hi) >> 1; u64 km = chain_keys[mid]; if ((km >> batchbits) <= body) lo = mid + 1; else hi = mid; }
-		chain_start[body] = e; chain_len[body] = lo - e;
+// Per-body chains.  Entry e = 2*i + side is side `side` of the contact at tag position i; a body's chain is its entries in
+// (batch, e) order, which is the order a stable sort of (body | batch) keys over e = 0, 1, ... would give.  The chains are built
+// without that sort: k_batch_index counts the entries per body, k_chain_alloc hands every body a segment of that length (segments
+// in any order), k_chain_scatter drops each entry into its body's segment (in any order), and k_chain_rank takes an entry's
+// position in its chain as the number of entries of its segment with a smaller (batch, e).  Chains average about five entries;
+// a hub body's segment is long, but it is read by all its entries at once and stays in L1.
+//
+// For each contact side: the slot whose token it must see on that body before it may run.  Per body the solver keeps a sequence
+// token = number of contact applications the body has received in this launch.  The contact at position `seq` of a body's chain
+// of length `len` therefore runs in sweep w when the token reads w*len + seq, and leaves w*len + seq + 1.  (expected - seen) is
+// the number of applications still ahead of a waiting contact, which is what the solver's back-off sleeps on.  Body 0 (static
+// world) is never waited for: its sides get (0, 0).
+__global__ void __launch_bounds__(NB_BLOCK) k_chain_alloc(u32 nbodies, const u32* chain_len, u32* chain_next /* out: first free position of the segment */, u32* counts) {
+	const u32 lane = threadIdx.x & 31;
+	for (u32 base = blockIdx.x * blockDim.x; base < nbodies; base += gridDim.x * blockDim.x) {  // warp-uniform trip count
+		const u32 b = base + threadIdx.x;
+		const u32 len = b < nbodies ? chain_len[b] : 0;
+		const u32 incl = warp_incl_scan(len);
+		u32 at = 0;
+		if (lane == 31 && incl) at = atomicAdd(&counts[CNT_CHAIN_CURSOR], incl);
+		at = __shfl_sync(0xffffffffu, at, 31);
+		if (len) chain_next[b] = at + incl - len;
 	}
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_waits(const u64* chain_keys, const u32* chain_vals, u32 batchbits, u32 nbodies, const u32* slot_idx, const u32* chain_start, const u32* chain_len,
-		uint2* wait /*[2][stride]: seq, len*/, u32 stride, const u32* counts) {
-	u32 n2 = counts[CNT_ENTRIES];
+NB_DEV u64 chain_key(u32 batch, u32 e) { return ((u64)batch << 32) | e; }
+__global__ void __launch_bounds__(NB_BLOCK) k_chain_scatter(const u32* sorted, const uint2* bodies, const u32* batch_of, u32* chain_next, u64* chain_keys, const u32* counts) {
+	const u32 n = counts[CNT_ENTRIES] >> 1;
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const uint2 ab = bodies[sorted[i]];
+		const u32 batch = batch_of[i];
+		if (ab.x) chain_keys[atomicAdd(&chain_next[ab.x], 1u)] = chain_key(batch, 2*i);
+		if (ab.y) chain_keys[atomicAdd(&chain_next[ab.y], 1u)] = chain_key(batch, 2*i + 1);
+	}
+}
+__global__ void __launch_bounds__(NB_BLOCK) k_chain_rank(const u32* sorted, const uint2* bodies, const u32* batch_of, const u32* slot_idx, const u32* chain_end, const u32* chain_len,
+		const u64* chain_keys, uint2* wait /*[2][stride]: seq, len*/, u32 stride, const u32* counts) {
+	const u32 n2 = counts[CNT_ENTRIES];
 	for (u32 e = blockIdx.x * blockDim.x + threadIdx.x; e < n2; e += gridDim.x * blockDim.x) {
-		u64 k = chain_keys[e];
-		u32 v = chain_vals[e];
-		u32 slot = slot_idx[v >> 1], side = v & 1;
+		const u32 i = e >> 1, side = e & 1;
+		const uint2 ab = bodies[sorted[i]];
+		const u32 body = side ? ab.y : ab.x;
 		uint2 w = make_uint2(0, 0);
-		if ((k >> batchbits) < nbodies) { u32 body = (u32)(k >> batchbits); w = make_uint2(e - chain_start[body], chain_len[body]); }
+		if (body) {
+			const u32 len = chain_len[body], end = chain_end[body];
+			const u64 mine = chain_key(batch_of[i], e);
+			u32 seq = 0;
+			for (u32 j = end - len; j < end; ++j) seq += chain_keys[j] < mine ? 1u : 0u;
+			w = make_uint2(seq, len);
+		}
+		const u32 slot = slot_idx[i];
 		if (slot < stride) wait[side * stride + slot] = w;
 	}
 }
@@ -749,7 +768,7 @@ NB_DEV void solve_contact(const Rows& R, u32 j, const float (&rv)[ROW_PLANES_TOT
 // unfinished item is always runnable.  Inside a warp the lanes poll instead of blocking, so a lane may depend on another
 // lane of its own warp.  mw must come from k_mw_in (all tokens 0).
 //
-// Waiting: the body's token says how many applications are still ahead of this contact (k_chain_heads).  While that number is
+// Waiting: the body's token says how many applications are still ahead of this contact (k_chain_rank).  While that number is
 // >= 2 on either body only the linear halves are polled, and the warp sleeps hop_ns per missing application when all of its
 // lanes are that far away; from 1 on, all four halves are fetched in one round trip so the hand-off costs a single L2 access.
 #define NB_SOLVE_BACKOFF_NS 150u  // hop_ns of k_solve and k_solve_flow (__nanosleep may sleep up to twice as long)
