@@ -6,12 +6,14 @@
 Settles the scene the way bench.py does, times `--steps` graph replays of nb_step with CUDA events (L2 flushed between steps,
 profiler off), then replays the same number of steps under torch.profiler with CUDA activities in a run of its own.  Writes
 DIR/kernels.csv (kernel, launches per step, µs per step), DIR/summary.json (card, power limit, step time, summed kernel time and
-the difference: the idle time between graph nodes) and prints the table."""
+the difference: the idle time between graph nodes, contacts, and the box-box pairs that survived the face SAT and went to k_np_clip)
+and prints the table."""
 import argparse, csv, json, os, subprocess, sys
 from collections import defaultdict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+CNT_SURV = 40   # position of CNT_SURV in the device counters (the enum at the top of nudge_b200/csrc/nb_collide.cuh)
 
 
 def card():
@@ -31,6 +33,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--presim", type=int, default=-1)
     args = ap.parse_args()
+    import numpy as np
     import torch
     import nudge_b200
     from bench import CONFIGS, settle_gpu
@@ -91,6 +94,7 @@ def main():
         for n, c, us in rows:
             w.writerow([n, "%.2f" % c, "%.2f" % us])
     summary = {"card": card(), "config": args.config, "solver": args.solver, "steps": K, "contacts": int(sim.counts().contacts),
+               "clip_survivors": int(sim.debug("counts", np.uint32)[CNT_SURV]),
                "library_launches_per_step": launches, "traced_ops_per_step": sum(r[1] for r in rows),
                "step_us_graph_replay": step_us, "kernel_us_per_step": kernel_us, "idle_between_nodes_us": step_us - kernel_us,
                "note": "step_us from CUDA events without the profiler; kernel_us from the profiler's trace of the same number of replays"}
