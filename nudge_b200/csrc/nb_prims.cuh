@@ -563,11 +563,12 @@ __global__ void __launch_bounds__(NB_CS_THREADS) k_sort_coop(u64* k0, u64* k1, u
 		for (u32 i = blockIdx.x * NB_CS_THREADS + tid; i < n; i += G * NB_CS_THREADS) { k1[i] = __ldcg(k0 + i); if (HAS_VALS) v1[i] = __ldcg(v0 + i); }
 }
 
-struct SortBuffers { u64* keys[2]; u32* vals[2]; u32* hist /*[L.sms][256]*/; u32* bar; int coop_launch; /* 0: ordinary launch, in a graph capture's non-cooperative attempt */ };
+struct SortBuffers { u64* keys[2]; u32* vals[2]; u32* hist /*[L.sms][256]*/; u32* bar; };
 
 // Sorts bits [begin_bit, end_bit) of keys[cur] (+vals[cur]), then stably on [begin_bit2, end_bit2); returns which buffer (0/1)
-// holds the result.  One k_sort_coop launch, one block per SM.  The first min(*n_ptr, n_max) keys are sorted, and *n_ptr is
-// lowered to n_max if it was larger.
+// holds the result.  One k_sort_coop launch, one block per SM, cooperative: the driver guarantees that the blocks meeting at its
+// grid barriers are co-resident, also next to other work on the device.  The first min(*n_ptr, n_max) keys are sorted, and *n_ptr
+// is lowered to n_max if it was larger.
 static int nb_radix_sort(const Launch& L, const SortBuffers& B, u32* n_ptr, int begin_bit, int end_bit, bool has_vals, int cur, int begin_bit2 = 0, int end_bit2 = 0, const u64* keybits = nullptr, u32 n_max = 0xffffffffu) {
 	// 8-bit digits, top-aligned per bit range; the lowest digit of a range may overlap the next one (harmless for LSD order)
 	SortPasses P; P.n = 0;
@@ -581,9 +582,7 @@ static int nb_radix_sort(const Launch& L, const SortBuffers& B, u32* n_ptr, int 
 	add_range(begin_bit2, end_bit2);
 	u64* k0 = B.keys[cur]; u64* k1 = B.keys[cur ^ 1]; u32* v0 = B.vals[cur]; u32* v1 = B.vals[cur ^ 1]; u32* hist = B.hist; u32* bar = B.bar;
 	void* args[] = { &k0, &k1, &v0, &v1, &n_ptr, &hist, &bar, &P, &keybits, &n_max };
-	if (B.coop_launch) cudaLaunchCooperativeKernel(has_vals ? (void*)k_sort_coop<true> : (void*)k_sort_coop<false>, dim3(L.sms), dim3(NB_CS_THREADS), args, sizeof(CoopSortSmem), L.stream);
-	else if (has_vals) k_sort_coop<true><<<L.sms, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits, n_max);
-	else k_sort_coop<false><<<L.sms, NB_CS_THREADS, sizeof(CoopSortSmem), L.stream>>>(k0, k1, v0, v1, n_ptr, hist, bar, P, keybits, n_max);
+	cudaLaunchCooperativeKernel(has_vals ? (void*)k_sort_coop<true> : (void*)k_sort_coop<false>, dim3(L.sms), dim3(NB_CS_THREADS), args, sizeof(CoopSortSmem), L.stream);
 	*L.counter += 1;
 	return cur ^ 1;
 }

@@ -39,20 +39,18 @@ NB_DEV void st_release_sys(u32* p, u32 v) { asm volatile("st.release.sys.global.
 NB_DEV u32 ld_acquire_sys(const u32* p) { u32 v; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 NB_DEV float4 ld_volatile_f4(const float4* p) { float4 v; asm volatile("ld.volatile.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p) : "memory"); return v; }
 
-// rows -> subscribers' inboxes; the last block to finish raises this rank's flag on every peer.  peers[r] = base of rank r's inbox
-// allocation (flags first, then [2][ghost_cap][2] float4).  *epoch is advanced by the last block, so the pull that follows reads it.
-__global__ void __launch_bounds__(NB_BLOCK) k_shard_push(const float4* mom, ShardPlanDev P, unsigned char* const* peers, u32 ghost_cap, u32 rank, u32 world,
-														 u32* epoch, u32* done) {
-	const u32 ep = *epoch + 1;
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n_export; i += gridDim.x * blockDim.x) {
-		const u32 body = P.export_local[i];
-		const float4 l = mom[2 * body], w = mom[2 * body + 1];
-		for (u32 t = P.sub_off[i]; t < P.sub_off[i + 1]; ++t) {
-			const uint2 tg = P.sub_tgt[t];
-			float4* dst = reinterpret_cast<float4*>(peers[tg.x] + NB_SHARD_FLAG_WORDS * 4) + 2 * ((size_t)(ep & 1u) * ghost_cap + tg.y);
-			dst[0] = l; dst[1] = w;
-		}
+// The inbox push protocol of k_shard_push and k_mw_out_push.  peers[r] = base of rank r's inbox allocation (flags first, then
+// [2][ghost_cap][2] float4); the push of epoch ep fills parity ep & 1.  push_row stores export row i into the inbox slot of every
+// subscriber.  push_arrive, after a block's last push_row, lets the last block to finish raise this rank's flag on every peer and
+// advance *epoch, so the pull that follows reads it.
+NB_DEV void push_row(const ShardPlanDev& P, unsigned char* const* peers, u32 ghost_cap, u32 ep, u32 i, float4 l, float4 w) {
+	for (u32 t = P.sub_off[i]; t < P.sub_off[i + 1]; ++t) {
+		const uint2 tg = P.sub_tgt[t];
+		float4* dst = reinterpret_cast<float4*>(peers[tg.x] + NB_SHARD_FLAG_WORDS * 4) + 2 * ((size_t)(ep & 1u) * ghost_cap + tg.y);
+		dst[0] = l; dst[1] = w;
 	}
+}
+NB_DEV void push_arrive(unsigned char* const* peers, u32 rank, u32 world, u32 ep, u32* epoch, u32* done) {
 	__threadfence_system();
 	__syncthreads();
 	if (threadIdx.x == 0) {
@@ -65,6 +63,17 @@ __global__ void __launch_bounds__(NB_BLOCK) k_shard_push(const float4* mom, Shar
 			*epoch = ep;
 		}
 	}
+}
+
+// rows -> subscribers' inboxes
+__global__ void __launch_bounds__(NB_BLOCK) k_shard_push(const float4* mom, ShardPlanDev P, unsigned char* const* peers, u32 ghost_cap, u32 rank, u32 world,
+														 u32* epoch, u32* done) {
+	const u32 ep = *epoch + 1;
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n_export; i += gridDim.x * blockDim.x) {
+		const u32 body = P.export_local[i];
+		push_row(P, peers, ghost_cap, ep, i, mom[2 * body], mom[2 * body + 1]);
+	}
+	push_arrive(peers, rank, world, ep, epoch, done);
 }
 
 // waits until every peer has pushed this epoch, then scatters the inbox into the ghost rows
@@ -91,14 +100,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_shard_pull(float4* mom, ShardPlanD
 		mom[2 * P.ghost_local[i >> 1] + (i & 1)] = ld_volatile_f4(rows + i);
 }
 
-// ---- the same exchange fused into the solver's working-copy kernels (peer transport, exact-order solver) ----
-// Unfused, a sweep of the sharded step is  k_mw_in, k_solve, k_mw_out, k_shard_push, k_shard_pull;  fused it is
-// k_pull_mw_in, k_solve, k_mw_out_push: the push reads the rows it sends from the working copy the solver just left, the pull
-// writes the ghosts' rows into both the momentum array and the next working copy.  Same values, two launches less per sweep.
-
-// k_mw_out (nb_solver.cuh) + k_shard_push.  A pushed row is the BodyMomentum row k_mw_out writes: (velocity, unused0 kept,
-// angular velocity, unused1 = 0 if a contact touched the body in a sweep); computed from mw and the OLD row, so it does not matter
-// whether the block that copies the body back has run yet.
+// k_mw_out (nb_solver.cuh) + k_shard_push: the end of the dataflow hand-over below.  A pushed row is the BodyMomentum row k_mw_out
+// writes: (velocity, unused0 kept, angular velocity, unused1 = 0 if a contact touched the body in a sweep); computed from mw and the
+// OLD row, so it does not matter whether the block that copies the body back has run yet.
 __global__ void __launch_bounds__(NB_BLOCK) k_mw_out_push(u32 B, nb_body_momentum* momentum, const float4* mw, int mode, ShardPlanDev P, unsigned char* const* peers,
 														  u32 ghost_cap, u32 rank, u32 world, u32* epoch, u32* done) {
 	const u32 ep = *epoch + 1;
@@ -117,64 +121,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_mw_out_push(u32 B, nb_body_momentu
 		const bool touched = asu(l.w) != 0;
 		const float u0 = p[0].w, u1 = p[1].w;      // unused0 never changes here; unused1 only ever changes to what the rule below gives
 		l.w = u0; w.w = (mode && touched) ? 0.0f : u1;
-		for (u32 t = P.sub_off[i]; t < P.sub_off[i + 1]; ++t) {
-			const uint2 tg = P.sub_tgt[t];
-			float4* dst = reinterpret_cast<float4*>(peers[tg.x] + NB_SHARD_FLAG_WORDS * 4) + 2 * ((size_t)(ep & 1u) * ghost_cap + tg.y);
-			dst[0] = l; dst[1] = w;
-		}
+		push_row(P, peers, ghost_cap, ep, i, l, w);
 	}
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0) {
-		const u32 old = atomicAdd(done, 1u);
-		if (old == gridDim.x - 1) {
-			__threadfence_system();
-			for (u32 r = 0; r < world; ++r)
-				if (r != rank) st_release_sys(reinterpret_cast<u32*>(peers[r]) + rank, ep);
-			*done = 0;
-			*epoch = ep;
-		}
-	}
-}
-
-// k_shard_pull + k_mw_in: ghosts take their owner's row (into the momentum array AND the new working copy), everybody else's working
-// copy comes from the momentum array.  is_ghost[body] != 0 marks the ghost rows (they are skipped by the plain copy, so no two
-// blocks write the same working-copy row).
-__global__ void __launch_bounds__(NB_BLOCK) k_pull_mw_in(u32 B, nb_body_momentum* momentum, float4* mw, ShardPlanDev P, const unsigned char* is_ghost, unsigned char* inbox,
-														 u32 ghost_cap, u32 rank, u32 world, const u32* epoch, u32* counts, long long timeout_cycles) {
-	const u32 ep = *epoch;
-	__shared__ int ok;
-	if (threadIdx.x == 0) {
-		const u32* flags = reinterpret_cast<const u32*>(inbox);
-		const long long t0 = clock64();
-		int good = 1;
-		for (u32 r = 0; r < world && good; ++r) {
-			if (r == rank) continue;
-			while ((int)(ld_acquire_sys(flags + r) - ep) < 0) {
-				if (clock64() - t0 > timeout_cycles) { good = 0; atomicOr(&counts[CNT_OVERFLOW], OVF_EXCHANGE); break; }
-				__nanosleep(200);
-			}
-		}
-		ok = good;
-	}
-	__syncthreads();
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
-		if (is_ghost[i] && ok) continue;
-		const float4* p = reinterpret_cast<const float4*>(momentum + i);
-		float4 l = p[0], w = p[1];
-		l.w = 0.0f; w.w = 0.0f;
-		mw[2*i] = l; mw[2*i + 1] = w;
-	}
-	if (!ok) return;
-	const float4* rows = reinterpret_cast<const float4*>(inbox + NB_SHARD_FLAG_WORDS * 4) + 2 * (size_t)(ep & 1u) * ghost_cap;
-	for (u32 j = blockIdx.x * blockDim.x + threadIdx.x; j < P.n_ghost; j += gridDim.x * blockDim.x) {
-		const u32 body = P.ghost_local[j];
-		float4 l = ld_volatile_f4(rows + 2 * j), w = ld_volatile_f4(rows + 2 * j + 1);
-		float4* p = reinterpret_cast<float4*>(momentum + body);
-		p[0] = l; p[1] = w;
-		l.w = 0.0f; w.w = 0.0f;
-		mw[2*body] = l; mw[2*body + 1] = w;
-	}
+	push_arrive(peers, rank, world, ep, epoch, done);
 }
 
 // ---- the ghost hand-over carried by the solver's own dataflow: ALL passes of a sharded step in one launch per GPU ----
