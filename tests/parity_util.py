@@ -8,13 +8,33 @@ def bits(a):
     return np.ascontiguousarray(a).view(np.uint8)
 
 
+def nan_canonical(a):
+    """A copy of `a` with every NaN in its float32 fields (whole array or structured fields) replaced by one bit pattern.  x86 and the GPU
+    give a NaN made by arithmetic different sign bits, and x86 propagates the first operand's NaN, so an operand order that differs
+    from the reference's changes only the sign of a NaN.  Comparisons that must tolerate that compare these copies."""
+    a = np.array(a, copy=True)
+
+    def fix(v):
+        if v.dtype.names:
+            for f in v.dtype.names:
+                fix(v[f])
+        elif v.dtype == np.float32:
+            v[np.isnan(v)] = np.float32(np.nan)
+    fix(a)
+    return a
+
+
 class Report:
-    def __init__(self, label=""):
+    def __init__(self, label="", nan_blind=False):
+        """nan_blind: a NaN equals any NaN in float32 fields (nan_canonical); every other bit must still match."""
         self.label = label
         self.failures = []
+        self.nan_blind = nan_blind
 
     def eq(self, name, x, y):
         x = np.asarray(x); y = np.asarray(y)
+        if self.nan_blind:
+            x, y = nan_canonical(x), nan_canonical(y)
         ok = x.shape == y.shape and x.dtype.itemsize == y.dtype.itemsize and np.array_equal(bits(x), bits(y))
         if not ok:
             msg = "%s %s: shapes %s vs %s" % (self.label, name, x.shape, y.shape)
@@ -112,14 +132,15 @@ def digest(a):
     return np.frombuffer(h.digest()[:8], np.uint8)
 
 
-def stage_digests(s, wide, steps, before_step=None):
-    """Labels and digests of every stage of `steps` steps of `s` (ref_layout_stages); before_step(i, s) runs ahead of step i."""
+def stage_digests(s, wide, steps, before_step=None, nan_blind=False):
+    """Labels and digests of every stage of `steps` steps of `s` (ref_layout_stages); before_step(i, s) runs ahead of step i.
+    nan_blind: digest nan_canonical(stage) instead, so that only the sign and payload of NaNs may differ."""
     labels, out = [], []
     for i in range(steps):
         if before_step:
             before_step(i, s)
         for name, a in ref_layout_stages(s, wide):
-            labels.append("step %d %s" % (i, name)); out.append(digest(a))
+            labels.append("step %d %s" % (i, name)); out.append(digest(nan_canonical(a) if nan_blind else a))
     return labels, np.array(out, np.uint8).reshape(-1, 8)
 
 
