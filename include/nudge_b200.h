@@ -15,6 +15,7 @@
  *   nb_upload_contacts              <- "custom contacts can be added here" example/main.cpp:288
  *   nb_upload_constraint_rows       <- "custom constraint impulses"        example/main.cpp:316
  *   nb_instance_matrices            <- the draw loops of render()          example/main.cpp:224-268 (helpers :53-110)
+ *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -174,6 +175,37 @@ typedef struct {
 } nb_constraint_row;            /* 80 bytes */
 int nb_upload_constraint_rows(nb_context*, const nb_constraint_row* host_rows, uint32_t n, void* stream);   /* replaces the set; n = 0 removes it; synchronises */
 int nb_download_constraint_rows(nb_context*, nb_constraint_row* host_rows, uint32_t n, void* stream);       /* caller's order; synchronises */
+
+/* Contact events (collision callbacks; DESIGN.md section 8.5): which collider pairs started or stopped touching, computed on the device inside
+ * nb_write_cached_impulses (so the stage calls, nb_step and its graph replay give the same stream).  A pair (key tags = A | (uint64)B << 32,
+ * the pair word of nb_contact_data.tags) is touching after a step if the contact cache that step wrote holds an entry with that key (the
+ * step's contacts plus the kept entries of sleeping pairs); after nb_upload_cache / nb_load_state the uploaded cache defines it.  With `old` =
+ * the cache before the call, `cur` = the step's contacts and `culled` = the kept entries of sleeping pairs:
+ *   NB_CONTACT_END:   key in old, not in cur, not in culled (a sleeping pair never ends; a pair ends when its island wakes and it is gone);
+ *   NB_CONTACT_BEGIN: key in cur, not in old (a pair whose island wakes still touching does not begin again).
+ * One call appends all its END events in ascending key order, then all its BEGIN events in ascending key order.  A BEGIN event carries the
+ * pair's contact count, its deepest contact (the first of the pair's contacts in (tag, feature) order, replaced only by a later one with a
+ * strictly greater penetration: position, normal, penetration, bodies) and the sum of the pair's final cached impulses in (tag, feature)
+ * order (fp32, sequential; in NB_SOLVER_THROUGHPUT the impulses vary from run to run, everything else is deterministic).  An END event
+ * carries tags, kind and step only, every other field is 0.  `step` counts the nb_write_cached_impulses calls since enabling (0 first).
+ * Cost when enabled: 3 kernel launches per step; none when disabled (the default).  Not supported by nb_shard_step (NB_ERR_ARGUMENT): ghost
+ * pairs would be reported by several ranks. */
+typedef struct {
+	uint64_t tags;                 /* A | (uint64)B << 32: the pair's collider tags (the cache key) */
+	uint32_t kind, step;           /* NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2; device sub-step counter */
+	uint32_t body_a, body_b, contacts;
+	float penetration, position[3], normal[3], impulse[3];
+	uint32_t reserved[3];
+} nb_contact_event;                /* 80 bytes */
+enum nb_contact_event_kind { NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2 };
+/* capacity = events the device buffer holds between two drains; 0 disables.  Every call resets count, dropped and step; the buffer is reused
+ * unless the capacity grows.  Synchronises the device. */
+int nb_enable_contact_events(nb_context*, uint32_t capacity);
+/* Synchronises `stream`, copies the stored events to `host` and empties the device buffer.  *count / *dropped = events stored / events lost
+ * because the buffer was full (the stored ones are always the first of the sequence).  NB_ERR_CAPACITY if `capacity` < *count (nothing is
+ * drained; *count says how much room is needed); NB_ERR_OVERFLOW if events were dropped (the outputs are filled and the buffer is emptied);
+ * NB_ERR_ARGUMENT if events are not enabled. */
+int nb_download_contact_events(nb_context*, nb_contact_event* host, uint32_t capacity, uint32_t* count, uint32_t* dropped, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

@@ -21,7 +21,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_shard_step", "nb_shard_graph_active", "nb_shard_partition", "nb_shard_debug_no_exchange",
            "nb_set_solver_mode", "nb_get_solver_mode", "nb_debug_timing_enable", "nb_debug_timing",
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
-           "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene"]
+           "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
+           "nb_enable_contact_events", "nb_download_contact_events"]
 
 
 class Config(C.Structure):
@@ -94,6 +95,8 @@ def load_library():
         lib.nb_instance_matrices.argtypes = [V, V, C.c_uint32, C.c_int, V, V]
         lib.nb_shard_build_plan.argtypes = [V, C.c_uint32, V, V, C.c_uint32, C.c_uint32, V, V, V, V, V, V, V, V]
         lib.nb_shard_local_scene.argtypes = [V, C.c_uint32, V, C.c_uint32, C.c_uint32, V, C.c_uint32, V, C.c_uint32, V, V, V, V, V]
+        lib.nb_enable_contact_events.argtypes = [V, C.c_uint32]
+        lib.nb_download_contact_events.argtypes = [V, V, C.c_uint32, V, V, V]
         _lib = lib
     return _lib
 
@@ -190,6 +193,7 @@ class Sim(abi.HostState):
         super().__init__(scene, contact_capacity or max(1024, 24 * mb))
         self.lib = load_library()
         self.stream = C.c_void_p(stream)
+        self.event_capacity = 0
         cfg = Config(mb, mx, ms, max(1, len(scene.connections)),
                      pair_capacity or max(4096, 16 * (mx + ms)), self.cap, device)
         self.ctx = C.c_void_p()
@@ -360,6 +364,23 @@ class Sim(abi.HostState):
             out = np.zeros((k, 16), np.float32)
         self._ck(self.lib.nb_instance_matrices(self.ctx, abi.ptr(out), len(out), 0, C.byref(n), self.stream), "nb_instance_matrices")
         return out[:n.value]
+
+    # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
+    def enable_contact_events(self, capacity):
+        """capacity = events held between two drains (0 disables); resets the stored events, the dropped count and the step counter."""
+        self._ck(self.lib.nb_enable_contact_events(self.ctx, int(capacity)), "nb_enable_contact_events")
+        self.event_capacity = int(capacity)
+
+    def contact_events(self, capacity=None):
+        """Drains the device buffer: (events as a scenes.CONTACT_EVENT array, number of events dropped since the last drain because the
+        buffer was full).  The events are always the first of the sequence; a drain with dropped > 0 still empties the buffer."""
+        cap = self.event_capacity if capacity is None else int(capacity)
+        out = np.zeros(max(cap, 1), scenes.CONTACT_EVENT)
+        n = C.c_uint32(0); dropped = C.c_uint32(0)
+        r = self.lib.nb_download_contact_events(self.ctx, abi.ptr(out), cap, C.byref(n), C.byref(dropped), self.stream)
+        if r != -4:   # NB_ERR_OVERFLOW fills the outputs: the caller reads `dropped`
+            self._ck(r, "nb_download_contact_events")
+        return out[:n.value].copy(), int(dropped.value)
 
     # ---- state files (nb_save_state / nb_load_state; tools/nb_replay steps them headless) ----
     def save_state(self, path):

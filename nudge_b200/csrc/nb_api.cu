@@ -3,6 +3,7 @@
 // here the context plays both roles for device memory: every buffer is carved once from cudaMalloc at
 // nb_create and reused every step, nothing is allocated or synchronised inside the step.
 #include "nb_shard.cuh"
+#include "nb_events.cuh"
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -17,7 +18,7 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 
 // A sub-step as a CUDA graph (nb_step, nb_shard_step; run_graphed): captured once per key and replayed while the key holds.  Every
 // count the kernels need lives in device memory, so the graph only depends on the parameters and the scene shape held in the key.
-struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version; };
+struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
 struct nb_context {
@@ -48,6 +49,8 @@ struct nb_context {
 	// `collide`; the first consumer waits for ev_up_done (inside a captured step: an external event-wait node, re-armed by every upload)
 	cudaStream_t copy_stream; cudaEvent_t ev_up_begin, ev_up_done; bool upload_pending, capture_joined; int copy_overlap;
 	nb_constraint_row* urows; u32 urow_cap, urow_n, urow_levels; unsigned long long urow_version; std::vector<u32> urow_level_off, urow_order;
+	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer holds ev_alloc events and is kept while it is large enough
+	nb_contact_event* events; u32 ev_cap, ev_alloc; unsigned long long events_version;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -155,7 +158,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	memset(&key, 0, sizeof(key));  // padding bytes included: the key is compared with memcmp
 	key.stream = st; key.ts = time_step; key.gravity = gravity; key.damping = damping; key.iterations = iterations;
 	key.B = ctx->B; key.nboxes = ctx->nboxes; key.nspheres = ctx->nspheres; key.nconn = ctx->nconn; key.tagbits = ctx->tagbits; key.kbits = ctx->kbits;
-	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version;
+	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version; key.events_version = ctx->events_version;
 	if (!g.exec || memcmp(&key, &g.key, sizeof(key)) != 0) {
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -315,6 +318,7 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->tev_made) for (int i = 0; i < 64; ++i) { cudaEventDestroy(ctx->tev[0][i]); cudaEventDestroy(ctx->tev[1][i]); }
 	if (ctx->copy_stream) { cudaStreamDestroy(ctx->copy_stream); cudaEventDestroy(ctx->ev_up_begin); cudaEventDestroy(ctx->ev_up_done); }
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
+	if (ctx->events) cudaFree(ctx->events);
 	delete ctx;
 }
 
@@ -593,10 +597,46 @@ int nb_read_cached_impulses(nb_context* ctx, void* stream) {
 int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_write_cached_impulses");
 	const u32 C = ctx->cfg.max_contacts;
+	if (ctx->ev_cap)   // the old cache is still intact here
+		launch_contact_events(mk_launch(ctx, stream), GRID(2 * (size_t)C), ctx->flags, ctx->stride, ctx->block_sums, ctx->cache_tags, ctx->sorted, ctx->fin,
+							  ctx->culled_tags, ctx->impulses, ctx->events, ctx->ev_cap, ctx->counts);
 	k_cache_merge<<<GRID(C), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sorted, ctx->fin.tags, ctx->fin.features, ctx->impulses,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->counts);
 	++ctx->launches;
 	CK(cudaGetLastError());
+	return NB_OK;
+}
+
+// ---------------- contact events (nb_events.cuh) ----------------
+int nb_enable_contact_events(nb_context* ctx, uint32_t capacity) {
+	CK(cudaDeviceSynchronize());   // nothing in flight may still write the counters or the buffer
+	ctx->ev_cap = 0;           // off until the buffer below exists (a failed allocation leaves events disabled)
+	++ctx->events_version;     // nb_step's graph re-records with or without the event launches
+	if (capacity > ctx->ev_alloc) {
+		if (ctx->events) { cudaFree(ctx->events); ctx->events = nullptr; ctx->ev_alloc = 0; }
+		void* p = nullptr;
+		CK(cudaMalloc(&p, sizeof(nb_contact_event) * (size_t)capacity));
+		ctx->events = (nb_contact_event*)p; ctx->ev_alloc = capacity;
+	}
+	CK(cudaMemset(ctx->counts + CNT_EV_COUNT, 0, 3 * sizeof(u32)));   // count, dropped, step
+	CK(cudaDeviceSynchronize());
+	ctx->ev_cap = capacity;
+	return NB_OK;
+}
+int nb_download_contact_events(nb_context* ctx, nb_contact_event* host, uint32_t capacity, uint32_t* count, uint32_t* dropped, void* stream) {
+	NB_RANGE("nb_download_contact_events");
+	if (!ctx->ev_cap) { ctx->error = "contact events are not enabled (nb_enable_contact_events)"; return NB_ERR_ARGUMENT; }
+	u32 c[CNT__COUNT];
+	int r = get_counts(ctx, c, stream); if (r) return r;
+	const u32 n = c[CNT_EV_COUNT], d = c[CNT_EV_DROPPED];
+	if (count) *count = n;
+	if (dropped) *dropped = d;
+	if (n > capacity) { ctx->error = "host event buffer too small: " + std::to_string(n) + " events are stored"; return NB_ERR_CAPACITY; }
+	if (n && !host) { ctx->error = "null host event buffer"; return NB_ERR_ARGUMENT; }
+	D2H(host, ctx->events, n, nb_contact_event);
+	CK(cudaMemsetAsync(ctx->counts + CNT_EV_COUNT, 0, 2 * sizeof(u32), (cudaStream_t)stream));   // count, dropped; in stream order
+	CK(cudaStreamSynchronize((cudaStream_t)stream));
+	if (d) { ctx->error = std::to_string(d) + " contact events were dropped: the event buffer was full (raise the nb_enable_contact_events capacity or drain more often)"; return NB_ERR_OVERFLOW; }
 	return NB_OK;
 }
 
@@ -751,7 +791,7 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 	return nb_advance(ctx, time_step, stream);
 }
 
-// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (58 launches in parity mode).
+// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (58 launches in parity mode, 3 more with contact events).
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy

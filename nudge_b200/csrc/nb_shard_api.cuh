@@ -237,6 +237,7 @@ static int shard_step_body(nb_shard* sh, float time_step, uint32_t iterations, f
 int nb_shard_step(nb_shard* sh, float time_step, uint32_t iterations, float gravity, float damping, int transport, void* stream) {
 	NB_RANGE("nb_shard_step");
 	nb_context* ctx = sh->ctx;
+	if (ctx->ev_cap) { ctx->error = "contact events are not supported by nb_shard_step: ghost pairs would be reported by several ranks"; return NB_ERR_ARGUMENT; }
 	if (sh->no_exchange) return nb_step(ctx, time_step, iterations, gravity, damping, stream);   // diagnostic: this rank's local problem alone
 	{ int jr = join_uploads(ctx, (cudaStream_t)stream); if (jr) return jr; }   // a pending side copy of nb_upload_bodies: ordered here, on the host side (the sharded graph has no event-wait node)
 	ctx->capture_joined = true;

@@ -20,8 +20,12 @@ CONTACT = np.dtype([("position", "<f4", 3), ("penetration", "<f4"), ("normal", "
 IMPULSE = np.dtype([("impulse", "<f4", 3), ("unused", "<f4")])
 PAIR16 = np.dtype([("a", "<u2"), ("b", "<u2")])
 PAIR32 = np.dtype([("a", "<u4"), ("b", "<u4")])
+# nb_contact_event (include/nudge_b200.h): kind CONTACT_BEGIN or CONTACT_END; an END event has only tags, kind and step set
+CONTACT_EVENT = np.dtype([("tags", "<u8"), ("kind", "<u4"), ("step", "<u4"), ("body_a", "<u4"), ("body_b", "<u4"), ("contacts", "<u4"),
+                          ("penetration", "<f4"), ("position", "<f4", 3), ("normal", "<f4", 3), ("impulse", "<f4", 3), ("reserved", "<u4", 3)])
+CONTACT_BEGIN, CONTACT_END = 1, 2
 
-assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32
+assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80
 
 
 class Scene:

@@ -7,10 +7,12 @@ import numpy as np, nudge_b200
 from nudge_b200 import scenes
 s = scenes.demo_scene(96, 96, iterations=4, spread=2.0, height=8.0)
 g = nudge_b200.Sim(s)
+g.enable_contact_events(4096)   # the event kernels run inside nb_write_cached_impulses
 for _ in range(6): g.step_staged()
 g.set_solver_mode("throughput")
 for _ in range(4): g.step_staged()
-c = g.counts(); print("contacts", c.contacts, "overflow", c.overflow)
+ev, dropped = g.contact_events()
+c = g.counts(); print("contacts", c.contacts, "overflow", c.overflow, "events", len(ev), "dropped", dropped)
 PY
 for tool in memcheck racecheck; do
   timeout 900 compute-sanitizer --tool $tool --error-exitcode 9 env PYTHONPATH=$PWD python /tmp/nb_sanitize_case.py > gpurun_out/sanitize_$tool.log 2>&1
