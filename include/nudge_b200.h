@@ -162,6 +162,7 @@ int nb_step(nb_context*, float time_step, uint32_t iterations, float gravity, fl
  * should be applied here", after every apply_impulses sweep).  One row = one scalar velocity constraint between bodies a and b
  * (0 = the static world):  J v + bias -> 0  with the accumulated impulse kept inside [lo, hi]; rows are applied by sequential impulses in
  * upload order after every contact sweep, their accumulated impulses warm-start the next step (nudge_b200/csrc/nb_rows_api.cuh).
+ * a and b must differ unless both are 0: a row on one body puts its whole Jacobian on a with b = 0 (a == b != 0 is NB_ERR_ARGUMENT).
  * Connect the bodies of a joint with nb_upload_connections too, so that islands treat them as one (example/main.cpp:285). */
 typedef struct {
 	uint32_t a, b;

@@ -651,14 +651,17 @@ static void timing_end(nb_context* ctx, cudaStream_t st) {
 	cudaEventRecord(ctx->tev[1][ctx->tev_n++], st);
 }
 
+// Shared-memory stages of k_jacobi_sweep for the current body count: two tiles per CTA in flight once the body arrays (64 B per body:
+// velocities + accumulators) take a large share of L2, else one stage and more CTAs.
+static int jacobi_stages(const nb_context* ctx) { return ctx->B > 600000u ? 2 : 1; }
+
 // throughput mode: warm start and sweeps as Jacobi passes (k_jacobi_sweep + k_jacobi_apply per pass), nb_jacobi.cuh
 static int launch_solve_jacobi(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) {
 	Rows R = ctx->rows;
 	const u32 B = ctx->B;
 	k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
 	++ctx->launches;
-	// two tiles per CTA in flight once the body arrays (64 B per body: velocities + accumulators) take a large share of L2, else more CTAs
-	const int stages = B > 600000u ? 2 : 1;
+	const int stages = jacobi_stages(ctx);
 	if (mode == 0 || mode == 2) {
 		if (stages == 1) k_jacobi_sweep<true, 1><<<ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
 		else k_jacobi_sweep<true, 2><<<ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
@@ -864,6 +867,9 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
+	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
+	if (!strcmp(name, "jacobi_stages")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)jacobi_stages(ctx); if (bytes) *bytes = 4; return NB_OK; }
+	if (!strcmp(name, "jacobi_blocks")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)(jacobi_stages(ctx) == 2 ? ctx->jacobi_blocks2 : ctx->jacobi_blocks1); if (bytes) *bytes = 4; return NB_OK; }
 	for (size_t i = 0; i < sizeof(table) / sizeof(table[0]); ++i)
 		if (!strcmp(name, table[i].name)) {
 			if (bytes) *bytes = table[i].bytes;

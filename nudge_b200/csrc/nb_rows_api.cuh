@@ -80,6 +80,8 @@ int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, ui
 	for (u32 i = 0; i < n; ++i) {
 		const u32 a = rows[i].a, b = rows[i].b;
 		if (a >= ctx->cfg.max_bodies || b >= ctx->cfg.max_bodies) { ctx->error = "constraint row references a body beyond max_bodies"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
+		// k_user_rows gives each side its own read-modify-write of the momentum row, and the effective mass has no cross terms
+		if (a && a == b) { ctx->error = "constraint row names the same body as a and b: put the whole Jacobian on a and set b = 0"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
 		u32 l = 0;
 		if (a) { auto it = last.find(a); if (it != last.end()) l = std::max(l, it->second + 1); }
 		if (b) { auto it = last.find(b); if (it != last.end()) l = std::max(l, it->second + 1); }

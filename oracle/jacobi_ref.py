@@ -53,11 +53,14 @@ def _first_on_nan_min(x, y):
         return np.where(y < x, y, x)
 
 
-def jacobi_pass(P, states, a, b, lin, ang, warm=False, impulses=None):
+def jacobi_pass(P, states, a, b, lin, ang, warm=False, impulses=None, abs_sums=False):
     """One Jacobi pass over all contacts.  P[41, n] rows (split planes already in place), states[3, n] accumulated impulses,
     a/b body indices, lin/ang [B, 3] velocities at the START of the pass.  Returns (lin', ang', states').
     Per-contact arithmetic: nudge.cpp:4646-4853 (sweep) / 4563-4632 (warm start); coupling: every contact sees the start-of-pass
-    velocities and the per-body changes are summed (Jacobi)."""
+    velocities and the per-body changes are summed (Jacobi).
+
+    abs_sums: also return (|dlin|, |dang|) [B, 3], the per-body sums of the absolute per-contact velocity changes.  They bound the
+    rounding of a float32 sum whose order is free (the kernel's atomics): |error| <= (terms) * 2^-24 * sum of |terms|."""
     f = np.float64
     g = lambda n: P[IX[n]].astype(f)
     va, wa, vb, wb = lin[a].astype(f), ang[a].astype(f), lin[b].astype(f), ang[b].astype(f)
@@ -96,9 +99,17 @@ def jacobi_pass(P, states, a, b, lin, ang, warm=False, impulses=None):
             dfx, dfy = fx - old_fx, fy - old_fy
             new_states = np.stack([ni, fx, fy])
     J = n * dn[:, None] + u * dfx[:, None] + v * dfy[:, None]
+    la, lb = -J * ma[:, None], J * mb[:, None]
+    wa_, wb_ = NA * dn[:, None] + UA * dfx[:, None] + VA * dfy[:, None], NB * dn[:, None] + UB * dfx[:, None] + VB * dfy[:, None]
     dlin = np.zeros(lin.shape, f); dang = np.zeros(ang.shape, f)
-    np.add.at(dlin, a, -J * ma[:, None]); np.add.at(dlin, b, J * mb[:, None])
-    np.add.at(dang, a, NA * dn[:, None] + UA * dfx[:, None] + VA * dfy[:, None])
-    np.add.at(dang, b, NB * dn[:, None] + UB * dfx[:, None] + VB * dfy[:, None])
+    np.add.at(dlin, a, la); np.add.at(dlin, b, lb)
+    np.add.at(dang, a, wa_); np.add.at(dang, b, wb_)
     dlin[0] = 0; dang[0] = 0   # body 0 is the static world
-    return lin.astype(f) + dlin, ang.astype(f) + dang, new_states
+    out = (lin.astype(f) + dlin, ang.astype(f) + dang, new_states)
+    if not abs_sums:
+        return out
+    alin = np.zeros(lin.shape, f); aang = np.zeros(ang.shape, f)
+    np.add.at(alin, a, np.abs(la)); np.add.at(alin, b, np.abs(lb))
+    np.add.at(aang, a, np.abs(wa_)); np.add.at(aang, b, np.abs(wb_))
+    alin[0] = 0; aang[0] = 0
+    return out + (alin, aang)

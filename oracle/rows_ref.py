@@ -19,7 +19,10 @@ def world_inverse_inertia(rotation, inertia_inverse):
 
 
 def apply_rows(rows, lin, ang, mass_inverse, inv_inertia, warm=False):
-    """One pass over the rows in order (in place on lin, ang [B, 3] float64 and rows['impulse'])."""
+    """One pass over the rows in order (in place on lin, ang [B, 3] float64 and rows['impulse']).
+
+    Rows with a == b != 0 are outside the model: their effective mass would need the cross terms 2 m lin_a.lin_b + 2 ang_a.I^-1 ang_b,
+    which neither this loop nor the kernel computes; nb_upload_constraint_rows refuses them (put the whole Jacobian on a, b = 0)."""
     for r in rows:
         a, b = int(r["a"]), int(r["b"])
         la, aa, lb, ab = (r[k].astype(np.float64) for k in ("lin_a", "ang_a", "lin_b", "ang_b"))

@@ -40,6 +40,36 @@ def test_split_with_unit_counts_reproduces_the_reference_planes():
         assert np.abs(t[k] - want).max() <= 2e-5 * scale, k
 
 
+def test_jacobi_pass_absolute_sums_add_every_contact_change_once():
+    """abs_sums (the per-body rounding scale of the kernel's free-order float32 sums): equal to the per-contact velocity changes, read
+    off a pass in which every contact side gets a private copy of its body, taken absolute and added per real body."""
+    o = pyoracle.OracleSim(scenes.demo_scene(120, 120, iterations=4, spread=3.0, height=12.0))
+    for _ in range(60):
+        o.step()
+    _setup(o)
+    P, st, a, b = _rows41(o)
+    n, B = P.shape[1], o.scene.n_bodies
+    lin, ang = o.momentum["velocity"].astype(np.float64), o.momentum["angular_velocity"].astype(np.float64)
+    for warm in (True, False):
+        imp = o.impulses_view()["data"]["impulse"] if warm else None
+        l1, w1, s1, alin, aang = J.jacobi_pass(P, st, a, b, lin, ang, warm=warm, impulses=imp, abs_sums=True)
+        l0, w0, s0 = J.jacobi_pass(P, st, a, b, lin, ang, warm=warm, impulses=imp)
+        assert np.array_equal(l0, l1) and np.array_equal(w0, w1) and np.array_equal(s0, s1)
+        # private copies: side a of contact k is body 1 + 2k, side b is 2 + 2k (the world stays body 0)
+        pa, pb = np.where(a != 0, 1 + 2 * np.arange(n), 0), np.where(b != 0, 2 + 2 * np.arange(n), 0)
+        plin, pang = np.zeros((1 + 2 * n, 3)), np.zeros((1 + 2 * n, 3))
+        plin[pa], pang[pa], plin[pb], pang[pb] = lin[a], ang[a], lin[b], ang[b]
+        ql, qw, _ = J.jacobi_pass(P, st, pa, pb, plin, pang, warm=warm, impulses=imp)
+        want_l, want_w = np.zeros((B, 3)), np.zeros((B, 3))
+        np.add.at(want_l, np.concatenate([a, b]), np.abs(ql - plin)[np.concatenate([pa, pb])])
+        np.add.at(want_w, np.concatenate([a, b]), np.abs(qw - pang)[np.concatenate([pa, pb])])
+        want_l[0] = 0; want_w[0] = 0
+        eps = 1e-12 * max(1.0, np.abs(lin).max(), np.abs(ang).max())    # (v + d) - v is d up to float64 rounding of v
+        assert np.abs(alin - want_l).max() <= eps and np.abs(aang - want_w).max() <= eps
+        assert (np.abs(l1 - lin) <= alin + eps).all() and (np.abs(w1 - ang) <= aang + eps).all()
+        assert alin.max() > 1e-3 and (np.bincount(np.concatenate([a, b]), minlength=B)[1:] > 1).any()
+
+
 def test_jacobi_pass_equals_a_gauss_seidel_sweep_when_no_body_has_two_contacts():
     n = 36
     s = scenes.demo_scene(0, n, iterations=1)
