@@ -79,6 +79,9 @@ struct nb_context {
 	float4* inertia;
 	u32* sched_spill_ent; u32* sched_spill_uid; u32 sched_spill_cap;   // k_schedule's open-slot list beyond its on-chip positions
 	u32* slot_of; u32* slot_done; u32* slot_left; u32* left_count; u32* batch_of; u32* slot_idx; float4* mw; uint2* cab; uint8_t* back;
+	// the segmented scheduler replay (nb_solver.cuh above k_schedule): per speculative run its slots, "list empty after contact i"
+	// and end state; per segment the run picked by the join
+	u32* sched_slot_v; uint8_t* sched_empty; u32* sched_state; u32* sched_join_slot; uint2* sched_pick; uint2* sched_pick_res;
 	Rows rows;
 };
 
@@ -269,6 +272,9 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->sched_spill_ent, 16 * (size_t)ctx->sched_spill_cap * 16); ALLOC(ctx->sched_spill_uid, 16 * (size_t)ctx->sched_spill_cap);
 	CK(cudaMemset(ctx->sched_spill_ent, 0xff, sizeof(u32) * 16 * (size_t)ctx->sched_spill_cap * 16));
 	ALLOC(ctx->left_count, 16); ALLOC(ctx->batch_of, C); ALLOC(ctx->slot_idx, C); ALLOC(ctx->mw, 2 * (size_t)B); ALLOC(ctx->cab, C); ALLOC(ctx->back, C);
+	ALLOC(ctx->sched_slot_v, 8 * (size_t)C); ALLOC(ctx->sched_empty, ((size_t)C + 3) & ~(size_t)3);   // 33 B per contact of capacity
+	ALLOC(ctx->sched_state, 16 * NB_SCHED_SEGS * 8 * (size_t)NB_SCHED_STATE); ALLOC(ctx->sched_join_slot, 16 * NB_SCHED_SEGS * 8 * NB_SCHED_JOIN);
+	ALLOC(ctx->sched_pick, 16 * NB_SCHED_SEGS * 8); ALLOC(ctx->sched_pick_res, 16 * NB_SCHED_SEGS);
 	ALLOC(ctx->rows.plane, (size_t)ROW_PLANES_TOTAL * ctx->cstride); ALLOC(ctx->rows.state, 3 * (size_t)ctx->cstride);
 	ALLOC(ctx->rows.a, ctx->cstride); ALLOC(ctx->rows.b, ctx->cstride); ALLOC(ctx->rows.contact, ctx->cstride); ALLOC(ctx->rows.wait, 2 * (size_t)ctx->cstride); ALLOC(ctx->chain_start, B); ALLOC(ctx->chain_len, B);
 	ctx->rows.stride = ctx->cstride;
@@ -721,10 +727,17 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 		CK(cudaGetLastError());
 		return NB_OK;
 	}
-	k_sched_prep<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->cab, ctx->back, counts);
+	k_sched_prep<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->cab, ctx->back, ctx->sched_empty, counts);
+	// the scheduler replay in segments (nb_solver.cuh above k_schedule, DESIGN §2.7): speculative runs, the joins of every segment
+	// from every run of the previous one, then per bucket the chain of picked runs (or the sequential replay if it broke), and the
+	// merge of the picked joins and runs
+	k_sched_spec<<<dim3(16, NB_SCHED_SEGS, 8), 32, 0, st>>>(ctx->cab, ctx->back, ctx->sched_slot_v, ctx->sched_empty, C, ctx->sched_state, counts);
+	k_sched_join<<<dim3(16, NB_SCHED_SEGS - 1, 8), 32, 0, st>>>(ctx->cab, ctx->back, ctx->sched_join_slot, ctx->sched_empty, ctx->sched_state, ctx->sched_pick, counts);
 	k_schedule<<<16, 32, 0, st>>>(ctx->cab, ctx->back, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
-		ctx->flags, ctx->left_count, ctx->sched_spill_ent, ctx->sched_spill_uid, ctx->sched_spill_cap, counts);
-	ctx->launches += 3;
+		ctx->flags, ctx->left_count, ctx->sched_spill_ent, ctx->sched_spill_uid, ctx->sched_spill_cap, ctx->sched_state, ctx->sched_pick, ctx->sched_pick_res, counts);
+	k_sched_merge<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->slot_of, ctx->sched_slot_v, C, ctx->sched_join_slot, ctx->slot_done, ctx->slots_per_bucket, ctx->flags,
+		ctx->sched_pick_res, counts);
+	ctx->launches += 5;
 	nb_scan<1>(L, ctx->flags, ctx->offs, S, counts + CNT_CONTACTS, 0, ctx->block_sums, counts + CNT_FULL_BATCHES);
 	// per-body chains (nb_solver.cuh, above k_chain_alloc): count, segment, scatter, rank.  chain_len is zero for bodies without
 	// entries, which nb_shard_step's dataflow solve relies on.  The entries go through sb.keys[0], free until the next collide.
@@ -794,7 +807,7 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 	return nb_advance(ctx, time_step, stream);
 }
 
-// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (58 launches in parity mode, 3 more with contact events).
+// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (60 launches in parity mode, 3 more with contact events).
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
@@ -852,6 +865,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "culled_tags", ctx->culled_tags, sizeof(u64) * c[CNT_CULLED] },
 		{ "culled_features", ctx->culled_features, sizeof(u32) * c[CNT_CULLED] },
 		{ "culled_data", ctx->culled_data, sizeof(float4) * c[CNT_CULLED] },
+		{ "cab", ctx->cab, sizeof(uint2) * c[CNT_CONTACTS] },
 		{ "batch_of", ctx->batch_of, sizeof(u32) * c[CNT_CONTACTS] },
 		{ "slot_idx", ctx->slot_idx, sizeof(u32) * c[CNT_CONTACTS] },
 		{ "row_contact", ctx->rows.contact, sizeof(u32) * 8 * c[CNT_BATCHES] },
@@ -866,6 +880,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }
+	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
 	if (!strcmp(name, "jacobi_stages")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)jacobi_stages(ctx); if (bytes) *bytes = 4; return NB_OK; }

@@ -19,6 +19,7 @@ enum {  // device counters (u32 each)
 	CNT_CACHE, CNT_CULLED, CNT_FULL_BATCHES, CNT_BATCHES, CNT_LEVELS, CNT_ENTRIES, CNT_OVERFLOW, CNT_LVCH0, CNT_LVCH1, CNT_LVCH2,
 	CNT_BMIN0, CNT_BMIN1, CNT_BMIN2, CNT_BMIN3, CNT_BMAX0, CNT_BMAX1, CNT_BMAX2, CNT_BMAX3,
 	CNT_BAR0, CNT_BAR1, CNT_SCRATCH0, CNT_SCRATCH1, CNT_EXT_SUM, CNT_GRID_LEVEL, CNT_LARGE, CNT_SURV, CNT_TMP, CNT_CHAIN_CURSOR,
+	CNT_SCHED_FALLBACK /* buckets the sequential scheduler replayed */, CNT_SCHED_FB0 /* 16 per-bucket fall-back flags */,
 	CNT_EXT_HIST = 64 /* 18 bins */,
 	// contact events (nb_events.cuh): kept across steps, k_reset_collide leaves them alone
 	CNT_EV_COUNT = 82, CNT_EV_DROPPED, CNT_EV_STEP, CNT_EV_N, CNT_EV_FLAGGED, CNT_EV_BASE, CNT_EV_STAMP,

@@ -151,8 +151,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_inertia(u32 B, const nb_transform*
 // nudge.cpp:4238-4240 applied, and `back` = distance (in contacts of the same bucket, 1..7) to the nearest earlier contact of
 // the bucket that shares a body, 0 if there is none within 7.  A run of 8 consecutive bucket contacts starting at a fresh
 // slot is conflict free iff none of them has 0 < back <= its offset in the run.
-__global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, const uint2* bodies, uint2* cab, uint8_t* back, const u32* counts) {
+__global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, const uint2* bodies, uint2* cab, uint8_t* back, uint8_t* sempty, u32* counts) {
 	u32 n = counts[CNT_CONTACTS];
+	if (blockIdx.x == 0 && threadIdx.x <= 16) counts[CNT_SCHED_FALLBACK + threadIdx.x] = 0;   // the fall-back counter and flags
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		uint2 ab = bodies[sorted[i]];
 		u32 ca = ab.x ? ab.x : ab.y, cb = ab.y ? ab.y : ab.x;
@@ -167,10 +168,13 @@ __global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, cons
 			}
 		}
 		back[i] = (uint8_t)b;
+		sempty[i] = 0;   // k_sched_spec's eight runs OR their bits in
 	}
 }
 
-// slot_of[i] = uid << 3 | lane, where lane is the SIMD lane the contact lands in (= number of contacts already in its slot)
+// slot_of[i] = uid << 3 | lane, where lane is the SIMD lane the contact lands in (= number of contacts already in its slot) and
+// uid, the slot's id, is the bucket-local index (i >> 4) of the contact that opened the slot: unique within a bucket in any
+// replay, whatever part of the bucket the replay covers, and below slots_per_bucket.
 //
 // ~99.9 % of all contacts go to list position 0 (measured), so the replay speculates: the next 8 - fill(position 0)
 // contacts are tested against position 0 and against each other with ONE __match_any_sync; all contacts before the first
@@ -180,28 +184,64 @@ __global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, cons
 // A list longer than the on-chip positions (a body with thousands of contacts: all of them conflict with each other, each opens its
 // own slot) SPILLS to global memory: positions >= NB_SCHED_REGPOS + NB_SCHED_SHARED live in spill_ent / spill_uid (per bucket,
 // `spill_cap` positions, all entries NB_NONE between launches: the kernel clears what it used).  The reference has no limit here.
-__global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t* back, u32* slot_of, u32* slot_done, u32* slot_left, u32 slots_per_bucket,
-												 u32* complete_flag, u32* left_count /*[16]*/, u32* spill_ent, u32* spill_uid, u32 spill_cap, u32* counts) {
-	__shared__ u32 S_ent[NB_SCHED_SHARED][16];
-	__shared__ u32 S_uid[NB_SCHED_REGPOS + NB_SCHED_SHARED];
-	const u32 bucket = blockIdx.x, lane = threadIdx.x, half = lane >> 4, ent = lane & 15, cidx = lane & 7;
-	const u32 n = counts[CNT_CONTACTS];
-	for (u32 k = lane; k < NB_SCHED_SHARED * 16; k += 32) (&S_ent[0][0])[k] = NB_NONE;
+//
+// One replay runs over the bucket-local contacts [lo, hi) of one bucket (DESIGN §2.7):
+//   SCHED_SEQ   the whole bucket from the empty list, spilling as above (k_schedule);
+//   SCHED_SPEC  one segment from the empty list (k_sched_spec); also sets bit `run` of sempty[i] where "the list is empty after
+//               contact i" and leaves its end state (the open slots in list order) in `state`;
+//   SCHED_JOIN  one segment from the end state in `state` (k_sched_join), until the first contact t after which its own list
+//               AND the list of the speculative run of the same phase (sempty) are empty: from there on the two runs decide
+//               identically.  Writes the slots of the contacts it replays to slot_of[m - lo].
+// SPEC and JOIN hold at most SHARED + NB_SCHED_REGPOS - 1 open slots and report a longer list instead of spilling.
+enum { SCHED_SEQ, SCHED_SPEC, SCHED_JOIN };
+enum { SCHED_RAN, SCHED_COUPLED, SCHED_FULL };
+#define NB_SCHED_SEG_SHARED 56                                    // list positions in shared memory per segment run
+#define NB_SCHED_SEG_POS (NB_SCHED_REGPOS + NB_SCHED_SEG_SHARED)
+#define NB_SCHED_STATE (1 + 17 * NB_SCHED_SEG_POS)                // end state of a segment: vcount, then per position 16 entries + uid
+#define NB_SCHED_SEGS 32                                          // segments per bucket at most
+#define NB_SCHED_MIN_SEG 256                                      // contacts per segment at least
+#define NB_SCHED_JOIN 64                                          // contacts a join may replay before its bucket falls back
+
+// Segments per bucket and their length (bucket-local contacts) for n contacts: the same for all buckets, bucket b's segment k
+// covers [min(k * len, nb), min((k + 1) * len, nb)) of its nb = ceil((n - b) / 16) contacts.
+__device__ __forceinline__ void sched_segments(u32 n, u32& segs, u32& len) {
+	const u32 nbmax = (n + 15) / 16;
+	segs = max(1u, min((u32)NB_SCHED_SEGS, nbmax / NB_SCHED_MIN_SEG));
+	len = (nbmax + segs - 1) / segs;
+}
+__device__ __forceinline__ u32 sched_bucket_len(u32 n, u32 bucket) { return n > bucket ? (n - bucket + 15) / 16 : 0; }
+
+template <int MODE, int SHARED>
+__device__ __forceinline__ u32 sched_replay(u32 (*S_ent)[16], u32* S_uid, u32 bucket, u32 lo, u32 hi, const uint2* cab, const uint8_t* back,
+		u32* slot_of, u32* done, u32* left, u32* complete_flag, u32* left_count, uint8_t* sempty, u32 run, u32* state,
+		u32* G_ent, u32* G_uid, u32 spill_cap, u32* counts, u32& t_out) {
+	const u32 lane = threadIdx.x, half = lane >> 4, ent = lane & 15, cidx = lane & 7;
+	for (u32 k = lane; k < SHARED * 16; k += 32) (&S_ent[0][0])[k] = NB_NONE;
 	__syncwarp();
-	u32* const G_ent = spill_ent + (size_t)bucket * spill_cap * 16;
-	u32* const G_uid = spill_uid + (size_t)bucket * spill_cap;
 	u32 spill_high = 0;   // positions of the spill area this launch has touched (warp uniform)
-	const u32 ONCHIP = NB_SCHED_REGPOS + NB_SCHED_SHARED;
+	const u32 ONCHIP = NB_SCHED_REGPOS + SHARED;
 	// entries / uid of a list position that is not in registers (pos >= NB_SCHED_REGPOS)
 	auto ent_of = [&](u32 pos) -> u32* { return pos < ONCHIP ? &S_ent[pos - NB_SCHED_REGPOS][0] : G_ent + (size_t)(pos - ONCHIP) * 16; };
 	auto uid_of = [&](u32 pos) -> u32* { return pos < ONCHIP ? &S_uid[pos] : G_uid + (pos - ONCHIP); };
-	u32 vcount = 0, next_uid = 0;
+	// the slot of contact i: a join writes the contacts it replays, lo.., to its own buffer (slot_of), everything else to slot_of[i]
+	auto put = [&](u32 i, u32 v) { if (MODE == SCHED_JOIN) slot_of[(i >> 4) - lo] = v; else slot_of[i] = v; };
+	// SPEC: bit `run` of sempty[i] (the eight runs of a segment share the byte; k_sched_prep cleared it)
+	auto set_empty = [&](u32 i) { atomicOr(reinterpret_cast<u32*>(sempty + (i & ~3u)), (1u << run) << (8 * (i & 3))); };
+	u32 vcount = 0;
 	u32 f0 = 0, uid0 = 0;  // fill count and uid of list position 0 (warp uniform)
 	u32 reg[NB_SCHED_REGSETS];
 	#pragma unroll
 	for (int k = 0; k < NB_SCHED_REGSETS; ++k) reg[k] = NB_NONE;
-	u32* done = slot_done + (size_t)bucket * slots_per_bucket;
-	u32* left = slot_left + (size_t)bucket * slots_per_bucket;
+	if (MODE == SCHED_JOIN) {  // start from the end state of the previous segment's speculative run
+		vcount = state[0];
+		#pragma unroll
+		for (u32 k = 0; k < NB_SCHED_REGSETS; ++k) if (2 * k + half < vcount) reg[k] = state[1 + (2 * k + half) * 17 + ent];
+		for (u32 pos = NB_SCHED_REGPOS; pos < vcount; ++pos) if (lane < 16) S_ent[pos - NB_SCHED_REGPOS][lane] = state[1 + pos * 17 + lane];
+		for (u32 pos = lane; pos < vcount; pos += 32) S_uid[pos] = state[1 + pos * 17 + 16];
+		uid0 = state[1 + 16];
+		f0 = __popc(__ballot_sync(0xffffffffu, reg[0] != NB_NONE) & 0xffu);
+		__syncwarp();
+	}
 
 	// Removes the completed slot at list position j: the last slot of the list takes its place (nudge.cpp:4294-4306).
 	auto remove_pos = [&](u32 j) {
@@ -256,8 +296,8 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 		if (j == NB_NONE) {  // all eight register positions conflict: continue in shared memory, two positions per round
 			for (u32 pb = 0; ; pb += 2) {   // shared positions, then the spill area; the position right after the list is all empty: the search ends there at the latest
 				u32 pos = pb + half;
-				if (pb >= NB_SCHED_SHARED + spill_cap) return false;
-				u32 v = pos < NB_SCHED_SHARED ? S_ent[pos][ent] : (pos < NB_SCHED_SHARED + spill_cap ? G_ent[(size_t)(pos - NB_SCHED_SHARED) * 16 + ent] : ca);
+				if (pb >= SHARED + spill_cap) return false;
+				u32 v = pos < SHARED ? S_ent[pos][ent] : (pos < SHARED + spill_cap ? G_ent[(size_t)(pos - SHARED) * 16 + ent] : ca);
 				u32 hit = __ballot_sync(0xffffffffu, v == ca || v == cb);
 				u32 occ = __ballot_sync(0xffffffffu, v != NB_NONE);
 				if (!(hit & 0xffffu)) { j = NB_SCHED_REGPOS + pb; f = __popc(occ & 0xffu); break; }
@@ -282,52 +322,73 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 		}
 		u32 uid;
 		if (j == vcount) {  // the sentinel was taken: a new slot (f is 0)
-			uid = next_uid++;
-			if (lane == 0) { *uid_of(j) = uid; done[uid] = NB_NONE; }
+			uid = i >> 4;
+			if (lane == 0) { *uid_of(j) = uid; if (MODE == SCHED_SEQ) done[uid] = NB_NONE; }
 			if (j == 0) uid0 = uid;
 			++vcount;
 			__syncwarp();
 		}
 		else uid = j ? *uid_of(j) : uid0;
-		if (lane == 0) slot_of[i] = (uid << 3) | f;
+		if (lane == 0) put(i, (uid << 3) | f);
 		if (f == 7) {
-			if (lane == 0) { done[uid] = i; complete_flag[i] = 1; }
+			if (lane == 0 && MODE == SCHED_SEQ) { done[uid] = i; complete_flag[i] = 1; }
 			remove_pos(j);
 		}
 		return true;
 	};
 
-	// software pipeline: the (ca, cb) of the next 32 contacts of this bucket are fetched while the current 32 are placed
-	u32 nx_ca = 0, nx_cb = 0, nx_back = 0;
-	{
-		u32 i0 = bucket + 16 * lane;
-		if (i0 < n) { uint2 ab = cab[i0]; nx_ca = ab.x; nx_cb = ab.y; nx_back = back[i0]; complete_flag[i0] = 0; }
-	}
-	for (u32 base = bucket; base < n; base += 16 * 32) {
-		const u32 my_ca = nx_ca, my_cb = nx_cb, my_back = nx_back;
-		{
-			u32 i1 = base + 16 * 32 + 16 * lane;
-			if (i1 < n) { uint2 ab = cab[i1]; nx_ca = ab.x; nx_cb = ab.y; nx_back = back[i1]; complete_flag[i1] = 0; }
+	// software pipeline: the (ca, cb) of the next 32 contacts of this bucket are fetched while the current 32 are placed.  The
+	// contact at chunk position c is fetched (and its complete_flag cleared) by lane c.
+	u32 nx_ca = 0, nx_cb = 0, nx_back = 0, nx_se = 0;
+	auto fetch = [&](u32 m) {
+		if (m < hi) {
+			const u32 i = bucket + 16 * m;
+			uint2 ab = cab[i]; nx_ca = ab.x; nx_cb = ab.y; nx_back = back[i];
+			if (MODE == SCHED_JOIN) nx_se = sempty[i];   // bit r: the speculative run r of this segment has an empty list after contact i
+			if (MODE == SCHED_SEQ) complete_flag[i] = 0;
 		}
-		const u32 steps = min(32u, (n - base + 15) / 16);
+	};
+	fetch(lo + lane);
+	// JOIN: the replay may stop after contact m (its list being empty there) if speculative run r = (m + 1 - lo) mod 8 starts right
+	// after m or has an empty list after m too; `mask` is m's sempty bits
+	auto couples = [&](u32 mask, u32 m) -> bool { return m + 1 - lo < 8 || ((mask >> ((m + 1 - lo) & 7)) & 1); };
+	u32 se_prev = 0;   // JOIN: sempty bits of the contact before chunk position 0 (warp uniform)
+	u32 t_couple = NB_NONE;
+	for (u32 m0 = lo; m0 < hi; m0 += 32) {
+		const u32 base = bucket + 16 * m0;
+		const u32 my_ca = nx_ca, my_cb = nx_cb, my_back = nx_back, my_se = nx_se;
+		fetch(m0 + 32 + lane);
+		__syncwarp();   // orders the clears above before the writes of other lanes to the same contacts
+		const u32 steps = min(32u, hi - m0);
 		u32 s = 0;
 		while (s < steps) {
+			if (MODE != SCHED_SEQ && vcount == 0 && m0 + s > lo) {   // the list is empty after the previous contact
+				if (MODE == SCHED_SPEC && lane == 0) set_empty(base + 16 * s - 16);
+				if (MODE == SCHED_JOIN && couples(s ? __shfl_sync(0xffffffffu, my_se, s - 1) : se_prev, m0 + s - 1)) { t_couple = m0 + s - 1; break; }
+			}
 			// ---- fresh list: whole 8-contact runs with no internal conflict are complete slots; accept as many as are clean with one ballot ----
 			if (vcount == 0 && steps - s >= 8) {
 				const u32 off = (lane - s) & 7;                       // offset of this lane's contact in its run (runs start at s)
 				const bool bad = lane >= s && lane < steps && my_back != 0 && my_back <= off;
 				const u32 bal = __ballot_sync(0xffffffffu, bad);
 				const u32 first_bad = bal ? (u32)(__ffs(bal) - 1) : steps;
-				const u32 runs = (first_bad - s) >> 3;
+				u32 runs = (first_bad - s) >> 3;
+				const u32 rel = lane - s;
+				if (MODE == SCHED_JOIN && runs) {   // stop after the first run whose end the speculative run has an empty list after
+					const u32 cb = __ballot_sync(0xffffffffu, lane >= s && rel < 8 * runs && (rel & 7) == 7 && couples(my_se, m0 + lane));
+					if (cb) runs = ((u32)(__ffs(cb) - 1) - s) / 8 + 1;
+				}
 				if (runs) {
-					const u32 rel = lane - s;
 					if (lane >= s && rel < 8 * runs) {
-						const u32 uid = next_uid + (rel >> 3);
+						const u32 uid = m0 + lane - (rel & 7);
 						const u32 i = base + 16 * lane;
-						slot_of[i] = (uid << 3) | (rel & 7);
-						if ((rel & 7) == 7) { done[uid] = i; complete_flag[i] = 1; }
+						put(i, (uid << 3) | (rel & 7));
+						if ((rel & 7) == 7) {
+							if (MODE == SCHED_SEQ) { done[uid] = i; complete_flag[i] = 1; }
+							if (MODE == SCHED_SPEC) set_empty(i);
+						}
 					}
-					next_uid += runs; s += 8 * runs;
+					s += 8 * runs;
 					continue;
 				}
 			}
@@ -348,10 +409,14 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 			if (fresh && cm == 0 && (vbal & 0xffu) == 0xffu) {
 				// the first eight contacts are conflict free: a whole slot, emitted at once; same for the second eight if clean
 				bool two = ((cbal >> 16) == 0) && (((vbal >> 16) & 0xffu) == 0xffu);
-				u32 uid = next_uid + half;
-				if ((!half || two) && ent < 8) slot_of[base + 16 * src] = (uid << 3) | cidx;
-				if ((!half || two) && ent == 7) { u32 il = base + 16 * src; done[uid] = il; complete_flag[il] = 1; }
-				next_uid += two ? 2 : 1;
+				if (MODE == SCHED_JOIN && two && couples(__shfl_sync(0xffffffffu, my_se, s + 7), m0 + s + 7)) two = false;   // couples after the first eight
+				u32 uid = m0 + s + 8 * half;
+				if ((!half || two) && ent < 8) put(base + 16 * src, (uid << 3) | cidx);
+				if ((!half || two) && ent == 7) {
+					u32 il = base + 16 * src;
+					if (MODE == SCHED_SEQ) { done[uid] = il; complete_flag[il] = 1; }
+					if (MODE == SCHED_SPEC) set_empty(il);
+				}
 				s += two ? 16 : 8;
 				continue;
 			}
@@ -359,16 +424,16 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 			u32 k = cm ? (u32)(__ffs(cm) - 1) : f0 + avail;   // first conflicting lane of position 0, or one past the last candidate
 			if (k > f0) {
 				if (vcount == 0) {  // position 0 was the sentinel: a new slot
-					uid0 = next_uid++; vcount = 1;
-					if (lane == 0) { S_uid[0] = uid0; done[uid0] = NB_NONE; }
+					uid0 = m0 + s; vcount = 1;
+					if (lane == 0) { S_uid[0] = uid0; if (MODE == SCHED_SEQ) done[uid0] = NB_NONE; }
 				}
 				bool take = !half && isnew && cidx < k;
 				if (take) reg[0] = cand;
-				if (take && ent < 8) slot_of[base + 16 * src] = (uid0 << 3) | cidx;
+				if (take && ent < 8) put(base + 16 * src, (uid0 << 3) | cidx);
 				s += k - f0; f0 = k;
 				if (k == 8) {  // position 0 is complete
 					u32 i_last = base + 16 * (s - 1);
-					if (lane == 0) { done[uid0] = i_last; complete_flag[i_last] = 1; }
+					if (lane == 0 && MODE == SCHED_SEQ) { done[uid0] = i_last; complete_flag[i_last] = 1; }
 					__syncwarp();
 					remove_pos(0);
 					continue;  // re-evaluate against the slot that moved into position 0
@@ -376,22 +441,151 @@ __global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t
 			}
 			if (cm && s < steps) {  // the contact at s conflicts with position 0: general first-fit
 				u32 ca = __shfl_sync(0xffffffffu, my_ca, s), cb = __shfl_sync(0xffffffffu, my_cb, s);
-				if (!place_general(base + 16 * s, ca, cb)) {   // the list outgrew even the spill area: report, leave the spill area clean
-					if (lane == 0) atomicOr(&counts[CNT_OVERFLOW], OVF_SCHED);
-					__syncwarp();
-					for (u32 k = lane; k < spill_high * 16; k += 32) G_ent[k] = NB_NONE;
-					return;
+				if (!place_general(base + 16 * s, ca, cb)) {
+					if (MODE == SCHED_SEQ) {   // the list outgrew even the spill area: report, leave the spill area clean
+						if (lane == 0) atomicOr(&counts[CNT_OVERFLOW], OVF_SCHED);
+						__syncwarp();
+						for (u32 k = lane; k < spill_high * 16; k += 32) G_ent[k] = NB_NONE;
+					}
+					return SCHED_FULL;
 				}
 				++s;
 			}
 		}
+		if (MODE == SCHED_JOIN) {
+			if (t_couple != NB_NONE) break;
+			se_prev = __shfl_sync(0xffffffffu, my_se, steps - 1);
+		}
 	}
-	// leftovers are flushed bucket-major in list order (nudge.cpp:4316-4338)
+	if (MODE == SCHED_JOIN) {
+		if (t_couple == NB_NONE && vcount == 0 && hi > lo && couples(se_prev, hi - 1)) t_couple = hi - 1;   // both lists empty after the last contact
+		t_out = t_couple;
+		__syncwarp();
+		return t_couple == NB_NONE ? SCHED_RAN : SCHED_COUPLED;
+	}
 	__syncwarp();
-	for (u32 jj = lane; jj < vcount; jj += 32) left[*uid_of(jj)] = jj;
-	if (lane == 0) left_count[bucket] = vcount;
-	__syncwarp();
-	for (u32 k = lane; k < spill_high * 16; k += 32) G_ent[k] = NB_NONE;   // leave the spill area empty for the next launch
+	if (MODE == SCHED_SPEC) {
+		if (vcount == 0 && hi > lo && lane == 0) set_empty(bucket + 16 * (hi - 1));
+		// the end state, for the join of the next segment
+		if (lane == 0) state[0] = vcount;
+		#pragma unroll
+		for (u32 k = 0; k < NB_SCHED_REGSETS; ++k) if (2 * k + half < vcount) state[1 + (2 * k + half) * 17 + ent] = reg[k];
+		for (u32 pos = NB_SCHED_REGPOS; pos < vcount; ++pos) if (lane < 16) state[1 + pos * 17 + lane] = S_ent[pos - NB_SCHED_REGPOS][lane];
+		for (u32 pos = lane; pos < vcount; pos += 32) state[1 + pos * 17 + 16] = S_uid[pos];
+	}
+	if constexpr (MODE == SCHED_SEQ) {
+		// leftovers are flushed bucket-major in list order (nudge.cpp:4316-4338)
+		for (u32 jj = lane; jj < vcount; jj += 32) left[*uid_of(jj)] = jj;
+		if (lane == 0) left_count[bucket] = vcount;
+		__syncwarp();
+		for (u32 k = lane; k < spill_high * 16; k += 32) G_ent[k] = NB_NONE;   // leave the spill area empty for the next launch
+	}
+	return SCHED_RAN;
+}
+
+// Per bucket: resolves the runs the segments pick and writes the leftovers, or, when the segmented replay fell back (a speculative
+// run outgrew its list, or the join on the picked chain did not couple), replays the bucket sequentially and rewrites all its outputs.
+// pick[(bucket, k, r)] = (contacts the join of segment k from run r of segment k-1 replayed, or NB_NONE; the run it picked);
+// pick_res[(bucket, k)] = (contacts from the join, picked run | incoming run << 8), the chain from run 0 of segment 0.
+__global__ void __launch_bounds__(32) k_schedule(const uint2* cab, const uint8_t* back, u32* slot_of, u32* slot_done, u32* slot_left, u32 slots_per_bucket,
+												 u32* complete_flag, u32* left_count /*[16]*/, u32* spill_ent, u32* spill_uid, u32 spill_cap,
+												 const u32* state, const uint2* pick, uint2* pick_res, u32* counts) {
+	__shared__ u32 S_ent[NB_SCHED_SHARED][16];
+	__shared__ u32 S_uid[NB_SCHED_REGPOS + NB_SCHED_SHARED];
+	__shared__ uint2 P[NB_SCHED_SEGS * 8];
+	const u32 bucket = blockIdx.x, lane = threadIdx.x, n = counts[CNT_CONTACTS];
+	u32* done = slot_done + (size_t)bucket * slots_per_bucket;
+	u32* left = slot_left + (size_t)bucket * slots_per_bucket;
+	if (!counts[CNT_SCHED_FB0 + bucket]) {
+		u32 segs, len; sched_segments(n, segs, len);
+		for (u32 k = lane; k < segs * 8; k += 32) P[k] = pick[bucket * NB_SCHED_SEGS * 8 + k];
+		__syncwarp();
+		u32 r = 0, ok = 1;
+		if (lane == 0) {
+			pick_res[bucket * NB_SCHED_SEGS] = make_uint2(0, 0);
+			for (u32 seg = 1; seg < segs; ++seg) {
+				const uint2 p = P[seg * 8 + r];
+				if (p.x == NB_NONE) { ok = 0; break; }
+				pick_res[bucket * NB_SCHED_SEGS + seg] = make_uint2(p.x, p.y | r << 8);
+				r = p.y;
+			}
+		}
+		ok = __shfl_sync(0xffffffffu, ok, 0); r = __shfl_sync(0xffffffffu, r, 0);
+		if (ok) {   // leftovers of the picked run of the last segment, bucket-major in list order (nudge.cpp:4316-4338)
+			const u32* st = state + ((size_t)(bucket * NB_SCHED_SEGS + segs - 1) * 8 + r) * NB_SCHED_STATE;
+			const u32 vcount = st[0];
+			for (u32 jj = lane; jj < vcount; jj += 32) { const u32 uid = st[1 + jj * 17 + 16]; left[uid] = jj; done[uid] = NB_NONE; }
+			if (lane == 0) left_count[bucket] = vcount;
+			return;
+		}
+		if (lane == 0) counts[CNT_SCHED_FB0 + bucket] = 1;   // k_sched_merge leaves this bucket alone
+	}
+	if (lane == 0) atomicAdd(&counts[CNT_SCHED_FALLBACK], 1u);
+	u32 t;
+	sched_replay<SCHED_SEQ, NB_SCHED_SHARED>(S_ent, S_uid, bucket, 0, sched_bucket_len(n, bucket), cab, back, slot_of, done, left,
+		complete_flag, left_count, nullptr, 0, nullptr, spill_ent + (size_t)bucket * spill_cap * 16, spill_uid + (size_t)bucket * spill_cap, spill_cap, counts, t);
+}
+
+// Speculative run r = blockIdx.z of segment blockIdx.y of bucket blockIdx.x: from the empty list, starting r contacts into the
+// segment (the first segment has run 0 only).  Writes plane r of slot_of_v (`plane` entries apart), bit r of sempty and its end state.
+__global__ void __launch_bounds__(32) k_sched_spec(const uint2* cab, const uint8_t* back, u32* slot_of_v, uint8_t* sempty, u32 plane, u32* state, u32* counts) {
+	__shared__ u32 S_ent[NB_SCHED_SEG_SHARED][16];
+	__shared__ u32 S_uid[NB_SCHED_SEG_POS];
+	const u32 bucket = blockIdx.x, seg = blockIdx.y, r = blockIdx.z, n = counts[CNT_CONTACTS];
+	u32 segs, len; sched_segments(n, segs, len);
+	const u32 nb = sched_bucket_len(n, bucket), lo = min(seg * len, nb) + r, hi = min((seg + 1) * len, nb);
+	if (seg >= segs || (seg == 0 && r) || lo > hi) return;
+	u32 t;
+	u32 res = sched_replay<SCHED_SPEC, NB_SCHED_SEG_SHARED>(S_ent, S_uid, bucket, lo, hi, cab, back, slot_of_v + (size_t)r * plane,
+		nullptr, nullptr, nullptr, nullptr, sempty, r, state + ((size_t)(bucket * NB_SCHED_SEGS + seg) * 8 + r) * NB_SCHED_STATE,
+		nullptr, nullptr, 0, counts, t);
+	if (res == SCHED_FULL && threadIdx.x == 0) counts[CNT_SCHED_FB0 + bucket] = 1;
+}
+
+// Join of segment k = blockIdx.y + 1 from the end state of speculative run r_in = blockIdx.z of segment k-1: replays segment k until
+// the first contact t after which its list is empty and so is that of the speculative run r = (t + 1 - start of k) mod 8 of segment
+// k, which started from the empty list r contacts (mod 8) after the segment start.  From t + 1 on the two runs are the same, so run r
+// is picked.  The eight joins of a segment run at once, one per run the previous segment may have picked; k_schedule follows the
+// chain of picks.  The replayed contacts' slots go to this join's buffer of NB_SCHED_JOIN entries; a join that does not couple
+// within them records NB_NONE.
+__global__ void __launch_bounds__(32) k_sched_join(const uint2* cab, const uint8_t* back, u32* join_slot, const uint8_t* sempty,
+												   const u32* state, uint2* pick, u32* counts) {
+	__shared__ u32 S_ent[NB_SCHED_SEG_SHARED][16];
+	__shared__ u32 S_uid[NB_SCHED_SEG_POS];
+	const u32 bucket = blockIdx.x, seg = blockIdx.y + 1, rin = blockIdx.z, n = counts[CNT_CONTACTS];
+	u32 segs, len; sched_segments(n, segs, len);
+	if (seg >= segs || (seg == 1 && rin) || counts[CNT_SCHED_FB0 + bucket]) return;
+	const u32 nb = sched_bucket_len(n, bucket), lo = min(seg * len, nb), hi = min((seg + 1) * len, nb);
+	if (min((seg - 1) * len, nb) + rin > lo) return;   // no such run in the previous segment
+	const size_t id = (size_t)(bucket * NB_SCHED_SEGS + seg) * 8 + rin;
+	const u32* st = state + ((size_t)(bucket * NB_SCHED_SEGS + seg - 1) * 8 + rin) * NB_SCHED_STATE;
+	u32 t = lo - 1;   // the previous segment ends with an empty list: run 0 is the true one
+	if (st[0] && sched_replay<SCHED_JOIN, NB_SCHED_SEG_SHARED>(S_ent, S_uid, bucket, lo, min(hi, lo + NB_SCHED_JOIN), cab, back,
+			join_slot + id * NB_SCHED_JOIN, nullptr, nullptr, nullptr, nullptr, const_cast<uint8_t*>(sempty), 0, const_cast<u32*>(st),
+			nullptr, nullptr, 0, counts, t) != SCHED_COUPLED) {
+		if (threadIdx.x == 0) pick[id] = make_uint2(NB_NONE, 0);
+		return;
+	}
+	if (threadIdx.x == 0) pick[id] = make_uint2(t + 1 - lo, (t + 1 - lo) & 7);
+}
+
+// The segmented schedule of every contact: its slot from the join where the picked join replayed it, else from the picked
+// speculative run; complete_flag and slot_done of the slot it completes, if it takes lane 7.  Buckets that fell back are left alone.
+__global__ void __launch_bounds__(NB_BLOCK) k_sched_merge(u32* slot_of, const u32* slot_of_v, u32 plane, const u32* join_slot, u32* slot_done,
+														  u32 slots_per_bucket, u32* complete_flag, const uint2* pick_res, const u32* counts) {
+	const u32 n = counts[CNT_CONTACTS];
+	u32 segs, len; sched_segments(n, segs, len);
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const u32 bucket = i & 15, m = i >> 4;
+		if (counts[CNT_SCHED_FB0 + bucket]) continue;
+		const u32 seg = m / len, off = m - seg * len;
+		const uint2 p = pick_res[bucket * NB_SCHED_SEGS + seg];
+		const u32 v = off < p.x ? join_slot[((size_t)(bucket * NB_SCHED_SEGS + seg) * 8 + (p.y >> 8)) * NB_SCHED_JOIN + off]
+		                        : slot_of_v[(size_t)(p.y & 0xffu) * plane + i];
+		slot_of[i] = v;
+		complete_flag[i] = (v & 7) == 7;
+		if ((v & 7) == 7) slot_done[(size_t)bucket * slots_per_bucket + (v >> 3)] = i;
+	}
 }
 
 // batch index and slot (batch*8 + lane) of every contact + the length of every body's chain (chain_len: zero on entry)
