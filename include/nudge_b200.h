@@ -16,6 +16,7 @@
  *   nb_upload_constraint_rows       <- "custom constraint impulses"        example/main.cpp:316
  *   nb_instance_matrices            <- the draw loops of render()          example/main.cpp:224-268 (helpers :53-110)
  *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
+ *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -163,7 +164,8 @@ int nb_step(nb_context*, float time_step, uint32_t iterations, float gravity, fl
  * (0 = the static world):  J v + bias -> 0  with the accumulated impulse kept inside [lo, hi]; rows are applied by sequential impulses in
  * upload order after every contact sweep, their accumulated impulses warm-start the next step (nudge_b200/csrc/nb_rows_api.cuh).
  * a and b must differ unless both are 0: a row on one body puts its whole Jacobian on a with b = 0 (a == b != 0 is NB_ERR_ARGUMENT).
- * Connect the bodies of a joint with nb_upload_connections too, so that islands treat them as one (example/main.cpp:285). */
+ * Connect the bodies of a joint with nb_upload_connections too, so that islands treat them as one (example/main.cpp:285), and set
+ * NB_FILTER_SKIP_CONNECTED (nb_upload_collision_filters) so that the joined bodies do not also collide where they overlap. */
 typedef struct {
 	uint32_t a, b;
 	float lin_a[3], ang_a[3];   /* Jacobian of body a: linear and angular part */
@@ -207,6 +209,22 @@ int nb_enable_contact_events(nb_context*, uint32_t capacity);
  * drained; *count says how much room is needed); NB_ERR_OVERFLOW if events were dropped (the outputs are filled and the buffer is emptied);
  * NB_ERR_ARGUMENT if events are not enabled. */
 int nb_download_contact_events(nb_context*, nb_contact_event* host, uint32_t capacity, uint32_t* count, uint32_t* dropped, void* stream);
+
+/* Collision filters (DESIGN.md section 8.6): which collider pairs nb_collide reports.  One nb_collision_filter per collider, boxes first then
+ * spheres (the collider index order of nb_upload_colliders).  Colliders i and j collide iff
+ *   (category_i & mask_j) != 0 && (category_j & mask_i) != 0            (Box2D's rule; without a table every pair passes)
+ * and, with NB_FILTER_SKIP_CONNECTED, their bodies are not joined by an entry of nb_upload_connections (either order, body 0 included;
+ * connections still merge islands).  A rejected pair is not a broadphase pair: it is not counted in nb_counts.pairs, does not link or
+ * wake islands, and never appears in the sleeping pairs, contacts, contact cache or events, except that a pair that was touching gets
+ * the ordinary NB_CONTACT_END when it becomes rejected.  Contacts uploaded with nb_upload_contacts are taken as given.
+ * n = boxes + spheres uploads a table, n = 0 removes it, any other n is NB_ERR_ARGUMENT; flags apply with or without a table.
+ * nb_upload_colliders keeps the table while the total collider count is unchanged and removes it when the count changes (the flags
+ * stay).  nb_save_state writes the table and flags (state version 2; version 1 without them), nb_load_state restores them.
+ * In nb_shard_step every rank filters with the global filter of its colliders, ghosts included; shards carry no connections, so
+ * NB_FILTER_SKIP_CONNECTED has no effect there.  Synchronises `stream`. */
+typedef struct { uint16_t category, mask; } nb_collision_filter;   /* 4 bytes */
+enum nb_filter_flags { NB_FILTER_SKIP_CONNECTED = 1 };
+int nb_upload_collision_filters(nb_context*, const nb_collision_filter* host, uint32_t n, uint32_t flags, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

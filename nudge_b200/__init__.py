@@ -22,7 +22,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_set_solver_mode", "nb_get_solver_mode", "nb_debug_timing_enable", "nb_debug_timing",
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
-           "nb_enable_contact_events", "nb_download_contact_events"]
+           "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters"]
 
 
 class Config(C.Structure):
@@ -97,6 +97,7 @@ def load_library():
         lib.nb_shard_local_scene.argtypes = [V, C.c_uint32, V, C.c_uint32, C.c_uint32, V, C.c_uint32, V, C.c_uint32, V, V, V, V, V]
         lib.nb_enable_contact_events.argtypes = [V, C.c_uint32]
         lib.nb_download_contact_events.argtypes = [V, V, C.c_uint32, V, V, V]
+        lib.nb_upload_collision_filters.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
         _lib = lib
     return _lib
 
@@ -230,6 +231,7 @@ class Sim(abi.HostState):
         self._ck(self.lib.nb_upload_bodies(self.ctx, C.byref(self.bodies), self.stream), "nb_upload_bodies")
         self._ck(self.lib.nb_upload_colliders(self.ctx, C.byref(self.colliders), self.stream), "nb_upload_colliders")
         self._ck(self.lib.nb_upload_connections(self.ctx, C.byref(self.conn), self.stream), "nb_upload_connections")
+        self._upload_scene_filters()
 
     def pack_momentum(self, dev_indices_ptr, n, dev_out_ptr):
         self._ck(self.lib.nb_pack_momentum(self.ctx, C.c_void_p(dev_indices_ptr), int(n), C.c_void_p(dev_out_ptr), self.stream), "nb_pack_momentum")
@@ -277,6 +279,12 @@ class Sim(abi.HostState):
         self._ck(self.lib.nb_upload_colliders(self.ctx, C.byref(self.colliders), self.stream), "nb_upload_colliders")
         self._ck(self.lib.nb_upload_connections(self.ctx, C.byref(self.conn), self.stream), "nb_upload_connections")
         self._ck(self.lib.nb_upload_cache(self.ctx, C.byref(self.cache), self.stream), "nb_upload_cache")
+        self._upload_scene_filters()
+
+    def _upload_scene_filters(self):
+        s = self.scene
+        if getattr(s, "collision_filters", None) is not None or getattr(s, "filter_flags", 0):
+            self.upload_collision_filters(s.collision_filters, s.filter_flags)
 
     def upload_bodies(self):
         self._ck(self.lib.nb_upload_bodies(self.ctx, C.byref(self.bodies), self.stream), "nb_upload_bodies")
@@ -364,6 +372,14 @@ class Sim(abi.HostState):
             out = np.zeros((k, 16), np.float32)
         self._ck(self.lib.nb_instance_matrices(self.ctx, abi.ptr(out), len(out), 0, C.byref(n), self.stream), "nb_instance_matrices")
         return out[:n.value]
+
+    # ---- collision filters (nb_collision_filter, include/nudge_b200.h) ----
+    def upload_collision_filters(self, filters, flags=0):
+        """filters: one scenes.FILTER row (category, mask) per collider, boxes first then spheres, or None / empty to remove the table.
+        flags: FILTER_SKIP_CONNECTED also rejects pairs whose bodies are joined by a connection.  Colliders i and j collide iff
+        category_i & mask_j and category_j & mask_i are both nonzero."""
+        f = np.zeros(0, scenes.FILTER) if filters is None else np.ascontiguousarray(filters, scenes.FILTER)
+        self._ck(self.lib.nb_upload_collision_filters(self.ctx, abi.ptr(f) if len(f) else None, len(f), int(flags), self.stream), "nb_upload_collision_filters")
 
     # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
     def enable_contact_events(self, capacity):

@@ -18,7 +18,7 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 
 // A sub-step as a CUDA graph (nb_step, nb_shard_step; run_graphed): captured once per key and replayed while the key holds.  Every
 // count the kernels need lives in device memory, so the graph only depends on the parameters and the scene shape held in the key.
-struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version; };
+struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
 struct nb_context {
@@ -51,6 +51,9 @@ struct nb_context {
 	nb_constraint_row* urows; u32 urow_cap, urow_n, urow_levels; unsigned long long urow_version; std::vector<u32> urow_level_off, urow_order;
 	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer holds ev_alloc events and is kept while it is large enough
 	nb_contact_event* events; u32 ev_cap, ev_alloc; unsigned long long events_version;
+	// collision filters (nb_upload_collision_filters): one category | mask << 16 word per collider while has_filter; with
+	// NB_FILTER_SKIP_CONNECTED and connections, conn_keys holds the sorted connection keys and conn_probe = their count (else 0)
+	u32* filter; bool has_filter; u32 filter_flags; u64* conn_keys; u64* conn_scratch; u32* conn_sort_n; u32 conn_probe; unsigned long long filter_version;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -162,6 +165,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	key.stream = st; key.ts = time_step; key.gravity = gravity; key.damping = damping; key.iterations = iterations;
 	key.B = ctx->B; key.nboxes = ctx->nboxes; key.nspheres = ctx->nspheres; key.nconn = ctx->nconn; key.tagbits = ctx->tagbits; key.kbits = ctx->kbits;
 	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version; key.events_version = ctx->events_version;
+	key.filter_version = ctx->filter_version;
 	if (!g.exec || memcmp(&key, &g.key, sizeof(key)) != 0) {
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -188,6 +192,20 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	ctx->upload_pending = false;   // a pending side copy is ordered before the replay: by the graph's event-wait node or by the caller's host-side join
 	ctx->launches += g.launches;
 	ctx->contacts_internal = true;
+	return NB_OK;
+}
+
+// The connected opt-out's lookup: the connection keys min(a,b) | max(a,b) << 32, radix sorted on the device, for the binary search of
+// the broadphase (nb_collide.cuh, connected()).  Rebuilt when connections are uploaded or loaded and when the flag is set; never per step.
+static int build_conn_lookup(nb_context* ctx, cudaStream_t st) {
+	const u32 n = (ctx->filter_flags & NB_FILTER_SKIP_CONNECTED) ? ctx->nconn : 0;
+	ctx->conn_probe = n;
+	if (!n) return NB_OK;
+	k_conn_keys<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->conn, n, ctx->conn_scratch); ++ctx->launches;
+	CK(cudaMemcpyAsync(ctx->conn_sort_n, &n, 4, cudaMemcpyHostToDevice, st));
+	SortBuffers cs = { { ctx->conn_scratch, ctx->conn_keys }, { nullptr, nullptr }, ctx->sb.hist, ctx->sb.bar };
+	nb_radix_sort(mk_launch(ctx, st), cs, ctx->conn_sort_n, 0, 64, false, 0);   // the result lands in keys[1] = conn_keys
+	CK(cudaGetLastError());
 	return NB_OK;
 }
 
@@ -241,6 +259,7 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->box_tags, c.max_boxes); ALLOC(ctx->box_data, c.max_boxes); ALLOC(ctx->box_xf, c.max_boxes);
 	ALLOC(ctx->sph_tags, c.max_spheres); ALLOC(ctx->sph_data, c.max_spheres); ALLOC(ctx->sph_xf, c.max_spheres);
 	ALLOC(ctx->conn, c.max_connections);
+	ALLOC(ctx->filter, K); ALLOC(ctx->conn_keys, c.max_connections); ALLOC(ctx->conn_scratch, c.max_connections); ALLOC(ctx->conn_sort_n, 1);
 	ALLOC(ctx->counts, CNT__COUNT); ALLOC(ctx->keybits, 2);
 	ALLOC(ctx->world_xf, K); ALLOC(ctx->aabb_min, K); ALLOC(ctx->aabb_max, K); ALLOC(ctx->col_tag, K); ALLOC(ctx->col_body, K);
 	ALLOC(ctx->order, K); ALLOC(ctx->rank, K);
@@ -362,6 +381,7 @@ int nb_download_transforms(nb_context* ctx, nb_transform* h, uint32_t count, voi
 
 int nb_upload_colliders(nb_context* ctx, const nb_collider_data* h, void* stream) {
 	if (h->boxes.count > ctx->cfg.max_boxes || h->spheres.count > ctx->cfg.max_spheres) { ctx->error = "too many colliders"; return NB_ERR_CAPACITY; }
+	if (ctx->has_filter && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_filter = false; ++ctx->filter_version; }  // the table belongs to a collider count
 	ctx->nboxes = h->boxes.count; ctx->nspheres = h->spheres.count;
 	u32 maxtag = 1;
 	for (u32 i = 0; i < h->boxes.count; ++i) maxtag = std::max(maxtag, h->boxes.tags[i]);
@@ -378,6 +398,20 @@ int nb_upload_connections(nb_context* ctx, const nb_body_connections* h, void* s
 	if (h->count > ctx->cfg.max_connections) { ctx->error = "too many connections"; return NB_ERR_CAPACITY; }
 	ctx->nconn = h->count;
 	H2D(ctx->conn, h->data, h->count, nb_body_pair);
+	return build_conn_lookup(ctx, (cudaStream_t)stream);
+}
+
+int nb_upload_collision_filters(nb_context* ctx, const nb_collision_filter* h, uint32_t n, uint32_t flags, void* stream) {
+	const u32 K = ctx->nboxes + ctx->nspheres;
+	if (n != 0 && n != K) { ctx->error = "collision filter count must be 0 or boxes + spheres (" + std::to_string(K) + ")"; return NB_ERR_ARGUMENT; }
+	if (n && !h) { ctx->error = "null collision filter table"; return NB_ERR_ARGUMENT; }
+	if (flags & ~(u32)NB_FILTER_SKIP_CONNECTED) { ctx->error = "unknown collision filter flags"; return NB_ERR_ARGUMENT; }
+	cudaStream_t st = (cudaStream_t)stream;
+	if (n) CK(cudaMemcpyAsync(ctx->filter, h, sizeof(nb_collision_filter) * (size_t)n, cudaMemcpyHostToDevice, st));   // category | mask << 16 as a u32
+	ctx->has_filter = n != 0; ctx->filter_flags = flags;
+	++ctx->filter_version;   // nb_step's graph re-records with the new kernel arguments
+	int r = build_conn_lookup(ctx, st); if (r) return r;
+	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
 int nb_upload_cache(nb_context* ctx, const nb_contact_cache* h, void* stream) {
@@ -475,7 +509,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 	k_reset_collide<<<1, 32, 0, st>>>(counts, K, ctx->keybits); ++ctx->launches;
 	if (K == 0 || B == 0) return NB_OK;
 	k_collider_world<<<GRID(K), NB_BLOCK, 0, st>>>(ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
-		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
+		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
 	k_morton<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->aabb_min, ctx->aabb_max, counts, ctx->sb.keys[0], ctx->sb.vals[0], ctx->keybits);
 	ctx->launches += 2;
 	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
@@ -484,8 +518,10 @@ int nb_collide(nb_context* ctx, void* stream) {
 	++ctx->launches;
 	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
 	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
-	k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	ctx->launches += 3;
 	// nudge.cpp:3498; the sort also clamps CNT_PAIRS to the capacity (the overflow bit is already set by emit_pair)
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);

@@ -27,10 +27,30 @@ enum {  // device counters (u32 each)
 };
 enum { OVF_PAIRS = 1, OVF_CONTACTS = 2, OVF_SCHED = 4, OVF_LEVELS = 8 };
 
+// ---------------- collision filters (nb_upload_collision_filters, DESIGN.md section 8.6) ----------------
+// A collider's filter word is category | mask << 16; it rides in the otherwise unused w lane of its AABB max corner, so the broadphase
+// reads it with the box it already loads.  0xffffffff (every category, every mask) is the word without a table: every pair passes.
+#define NB_FILTER_ALL 0xffffffffu
+NB_DEV bool filter_pass(u32 wa, u32 wb) { return (wa & (wb >> 16)) != 0 && (wb & (wa >> 16)) != 0; }  // Box2D's rule
+// Connected opt-out: `conn_keys` holds min(a,b) | max(a,b) << 32 of every uploaded connection, ascending; conn_n = 0 disables the probe.
+NB_DEV bool connected(const u64* conn_keys, u32 conn_n, u32 a, u32 b) {
+	const u64 k = a < b ? (u64)a | ((u64)b << 32) : (u64)b | ((u64)a << 32);
+	u32 lo = 0, hi = conn_n;
+	while (lo < hi) { const u32 mid = (lo + hi) >> 1; if (__ldg(conn_keys + mid) < k) lo = mid + 1; else hi = mid; }
+	return lo < conn_n && __ldg(conn_keys + lo) == k;
+}
+__global__ void __launch_bounds__(NB_BLOCK) k_conn_keys(const nb_body_pair* conn, u32 n, u64* keys) {
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const u32 a = conn[i].a, b = conn[i].b;
+		keys[i] = a < b ? (u64)a | ((u64)b << 32) : (u64)b | ((u64)a << 32);
+	}
+}
+
 // ---------------- K1: collider world transform + AABB (nudge.cpp:3021-3079) ----------------
+// filter: one word per collider (category | mask << 16) or null; it goes to aabb_max[i].w, which no geometry reads.
 __global__ void __launch_bounds__(NB_BLOCK) k_collider_world(u32 nboxes, u32 nspheres, const nb_transform* body_xf,
 		const nb_transform* box_xf, const nb_box_collider* box_data, const u32* box_tags,
-		const nb_transform* sph_xf, const nb_sphere_collider* sph_data, const u32* sph_tags,
+		const nb_transform* sph_xf, const nb_sphere_collider* sph_data, const u32* sph_tags, const u32* filter,
 		nb_transform* world_xf, float4* aabb_min, float4* aabb_max, u32* col_tag, u32* col_body, u32* counts) {
 	u32 K = nboxes + nspheres;
 	float mn[3] = { INFINITY, INFINITY, INFINITY }, mx[3] = { -INFINITY, -INFINITY, -INFINITY };
@@ -57,7 +77,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_collider_world(u32 nboxes, u32 nsp
 			ext = mk3(r, r, r);
 		}
 		float4 lo = make_float4(p.x - ext.x, p.y - ext.y, p.z - ext.z, 0.0f);
-		float4 hi = make_float4(p.x + ext.x, p.y + ext.y, p.z + ext.z, 0.0f);
+		float4 hi = make_float4(p.x + ext.x, p.y + ext.y, p.z + ext.z, asf(filter ? filter[i] : NB_FILTER_ALL));
 		st_xform(world_xf, i, w);
 		aabb_min[i] = lo; aabb_max[i] = hi;
 		col_tag[i] = is_box ? box_tags[i] : sph_tags[i - nboxes];
@@ -243,7 +263,8 @@ NB_DEV void emit_pair(u32 p, u32 q, const u32* order, u32 kbits, u64* pair_keys,
 // atomic per ~64 pairs: one global atomic per pair would serialise on the counter.
 #define NB_GP_BUF 128
 __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order, const float4* leaf_min, const float4* leaf_max, const uint8_t* smallf, const u64* mkeys,
-		const u64* table_keys, const u64* table_vals, u32 table_mask, u32 kbits, u64* pair_keys, u32 max_pairs, u32* counts) {
+		const u64* table_keys, const u64* table_vals, u32 table_mask, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n,
+		u64* pair_keys, u32 max_pairs, u32* counts) {
 	__shared__ u64 buf[NB_WARPS][NB_GP_BUF];
 	__shared__ u32 fill[NB_WARPS];
 	const MortonFrame f = morton_frame(counts);
@@ -292,7 +313,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 			}
 		}
 		const u32 incl = warp_incl_scan(len), off = incl - len, total = __shfl_sync(0xffffffffu, incl, 31);
-		const u64 hi_key = (u64)order[p] << kbits;  // hi = earlier, lo = later (nudge.cpp:3495)
+		const u32 op = order[p];
+		const u64 hi_key = (u64)op << kbits;  // hi = earlier, lo = later (nudge.cpp:3495)
+		const u32 fp = asu(hi.w);               // this collider's filter word
 		for (u32 t0 = 0; t0 < total; t0 += 32) {
 			const u32 t = t0 + lane;
 			// cell of candidate t: the last lane whose offset is <= t (offsets are non-decreasing)
@@ -305,15 +328,21 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 			const u32 q = __shfl_sync(0xffffffffu, qb, c) + (t - __shfl_sync(0xffffffffu, off, c));
 			bool hit = false;
 			if (t < total) {
-				const float4 a = __ldg(leaf_min + q), bq = __ldg(leaf_max + q);  // two 128-bit loads; a.w carries the class
-				hit = (bq.x > lo.x) & (hi.x > a.x) & (bq.y > lo.y) & (hi.y > a.y) & (bq.z > lo.z) & (hi.z > a.z) & (0.0f > a.w);  // strict, nudge.cpp:3306-3310
+				const float4 a = __ldg(leaf_min + q), bq = __ldg(leaf_max + q);  // two 128-bit loads; a.w carries the class, bq.w the filter word
+				hit = (bq.x > lo.x) & (hi.x > a.x) & (bq.y > lo.y) & (hi.y > a.y) & (bq.z > lo.z) & (hi.z > a.z) & (0.0f > a.w)  // strict, nudge.cpp:3306-3310
+					& filter_pass(fp, asu(bq.w));
+			}
+			u32 oq = 0;
+			if (hit) {
+				oq = order[q];
+				if (conn_n) hit = !connected(conn_keys, conn_n, __ldg(col_body + op), __ldg(col_body + oq));
 			}
 			if (hit) {
 				u32 slot = atomicAdd(&fill[wid], 1u);
-				if (slot < NB_GP_BUF) buf[wid][slot] = hi_key | (u64)order[q];
+				if (slot < NB_GP_BUF) buf[wid][slot] = hi_key | (u64)oq;
 				else {  // more than a buffer of hits from one step: straight to the list
 					u32 g = atomicAdd(&counts[CNT_PAIRS], 1u);
-					if (g < max_pairs) pair_keys[g] = hi_key | (u64)order[q];
+					if (g < max_pairs) pair_keys[g] = hi_key | (u64)oq;
 					else atomicOr(&counts[CNT_OVERFLOW], OVF_PAIRS);
 				}
 			}
@@ -325,14 +354,17 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 }
 
 __global__ void __launch_bounds__(NB_BLOCK) k_large_pairs(u32 K, const u32* order, const float4* leaf_min, const float4* leaf_max, const uint8_t* smallf,
-		const u32* large_list, u32 kbits, u64* pair_keys, u32 max_pairs, u32* counts) {
+		const u32* large_list, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n, u64* pair_keys, u32 max_pairs, u32* counts) {
 	const u32 nlarge = counts[CNT_LARGE];
 	for (u32 l = 0; l < nlarge; ++l) {
 		const u32 pl = large_list[l];
 		const float4 lo = leaf_min[pl], hi = leaf_max[pl];
 		for (u32 q = blockIdx.x * blockDim.x + threadIdx.x; q < K; q += gridDim.x * blockDim.x) {
 			if (q == pl || (!smallf[q] && q < pl)) continue;  // a pair of two large colliders is reported from the earlier one
-			if (boxes_overlap(lo, hi, leaf_min[q], leaf_max[q])) emit_pair(min(pl, q), max(pl, q), order, kbits, pair_keys, max_pairs, counts);
+			const float4 bq = leaf_max[q];
+			if (boxes_overlap(lo, hi, leaf_min[q], bq) && filter_pass(asu(hi.w), asu(bq.w))
+				&& !(conn_n && connected(conn_keys, conn_n, col_body[order[pl]], col_body[order[q]])))
+				emit_pair(min(pl, q), max(pl, q), order, kbits, pair_keys, max_pairs, counts);
 		}
 	}
 }

@@ -9,6 +9,9 @@
 //   box_tags[boxes] (4) | box_data[boxes] (16) | box_transforms[boxes] (32)
 //   sphere_tags[spheres] (4) | sphere_data[spheres] (4) | sphere_transforms[spheres] (32)
 //   connections[connections] (8) | cache_tags[cache] (8) | cache_features[cache] (4) | cache_data[cache] (16)
+// Version 2 (a context with collision filters, nb_upload_collision_filters): the same header with reserved[0] = filter flags and
+// reserved[1] = 1 if the table follows, and then filter[boxes + spheres] (4, category | mask << 16) after cache_data.  A context
+// without a table or flags writes version 1; both versions load, and a version-1 load removes any table and flags.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
@@ -38,7 +41,10 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	FILE* f = fopen(path, "wb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
 	NbStateHeader h; memset(&h, 0, sizeof(h));
-	memcpy(h.magic, "NBSTATE1", 8); h.version = 1;
+	memcpy(h.magic, "NBSTATE1", 8);
+	const bool filtered = ctx->has_filter || ctx->filter_flags;
+	h.version = filtered ? 2 : 1;
+	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = c[CNT_CACHE]; h.solver_mode = (u32)ctx->solver_mode;
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
@@ -48,6 +54,7 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 		&& state_put(f, ctx->sph_tags, 4 * (size_t)h.spheres, tmp, st) && state_put(f, ctx->sph_data, sizeof(nb_sphere_collider) * (size_t)h.spheres, tmp, st) && state_put(f, ctx->sph_xf, sizeof(nb_transform) * (size_t)h.spheres, tmp, st)
 		&& state_put(f, ctx->conn, sizeof(nb_body_pair) * (size_t)h.connections, tmp, st)
 		&& state_put(f, ctx->cache_tags, 8 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_features, 4 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_data, 16 * (size_t)h.cache, tmp, st);
+	if (h.reserved[1]) ok = ok && state_put(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -58,7 +65,7 @@ int nb_state_info(const char* path, uint32_t counts[5]) {
 	FILE* f = fopen(path, "rb");
 	if (!f) return NB_ERR_ARGUMENT;
 	NbStateHeader h;
-	bool ok = fread(&h, sizeof(h), 1, f) == 1 && !memcmp(h.magic, "NBSTATE1", 8) && h.version == 1;
+	bool ok = fread(&h, sizeof(h), 1, f) == 1 && !memcmp(h.magic, "NBSTATE1", 8) && (h.version == 1 || h.version == 2);
 	fclose(f);
 	if (!ok) return NB_ERR_ARGUMENT;
 	counts[0] = h.bodies; counts[1] = h.boxes; counts[2] = h.spheres; counts[3] = h.connections; counts[4] = h.cache;
@@ -71,7 +78,7 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	FILE* f = fopen(path, "rb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
 	NbStateHeader h;
-	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8) || h.version != 1) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
+	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8) || (h.version != 1 && h.version != 2)) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
 	const nb_config& c = ctx->cfg;
 	if (h.bodies > c.max_bodies || h.boxes > c.max_boxes || h.spheres > c.max_spheres || h.connections > c.max_connections || h.cache > c.max_contacts) {
 		fclose(f); ctx->error = "state file exceeds the context's capacities"; return NB_ERR_CAPACITY;
@@ -89,6 +96,8 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	ok = ok && state_get(f, ctx->sph_data, sizeof(nb_sphere_collider) * (size_t)h.spheres, tmp, st) && state_get(f, ctx->sph_xf, sizeof(nb_transform) * (size_t)h.spheres, tmp, st)
 		&& state_get(f, ctx->conn, sizeof(nb_body_pair) * (size_t)h.connections, tmp, st)
 		&& state_get(f, ctx->cache_tags, 8 * (size_t)h.cache, tmp, st) && state_get(f, ctx->cache_features, 4 * (size_t)h.cache, tmp, st) && state_get(f, ctx->cache_data, 16 * (size_t)h.cache, tmp, st);
+	const bool table = h.version == 2 && h.reserved[1];
+	if (table) ok = ok && state_get(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->B = h.bodies; ctx->nboxes = h.boxes; ctx->nspheres = h.spheres; ctx->nconn = h.connections;
@@ -97,6 +106,10 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	CK(cudaMemcpyAsync(ctx->counts + CNT_CACHE, &h.cache, 4, cudaMemcpyHostToDevice, st));
 	CK(cudaStreamSynchronize(st));
 	if (h.solver_mode == NB_SOLVER_PARITY || h.solver_mode == NB_SOLVER_THROUGHPUT) ctx->solver_mode = (int)h.solver_mode;
+	ctx->has_filter = table; ctx->filter_flags = h.version == 2 ? (h.reserved[0] & NB_FILTER_SKIP_CONNECTED) : 0;
+	++ctx->filter_version;
+	{ int r = build_conn_lookup(ctx, st); if (r) return r; }
+	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
 

@@ -24,8 +24,11 @@ PAIR32 = np.dtype([("a", "<u4"), ("b", "<u4")])
 CONTACT_EVENT = np.dtype([("tags", "<u8"), ("kind", "<u4"), ("step", "<u4"), ("body_a", "<u4"), ("body_b", "<u4"), ("contacts", "<u4"),
                           ("penetration", "<f4"), ("position", "<f4", 3), ("normal", "<f4", 3), ("impulse", "<f4", 3), ("reserved", "<u4", 3)])
 CONTACT_BEGIN, CONTACT_END = 1, 2
+# nb_collision_filter (include/nudge_b200.h): colliders i and j collide iff category_i & mask_j and category_j & mask_i are both nonzero
+FILTER = np.dtype([("category", "<u2"), ("mask", "<u2")])
+FILTER_SKIP_CONNECTED = 1
 
-assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80
+assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4
 
 
 class Scene:
@@ -46,6 +49,9 @@ class Scene:
         self.sphere_transforms = np.zeros(n_spheres, TRANSFORM)
         self.sphere_transforms["rotation"][:, 3] = 1.0
         self.connections = np.zeros(0, PAIR32)
+        # optional collision filters: one FILTER row per collider (boxes first, then spheres) or None, and FILTER_* flags
+        self.collision_filters = None
+        self.filter_flags = 0
         # step parameters the reference leaves to the caller (example/main.cpp:275-305)
         self.time_step = np.float32(1.0 / 120.0)
         self.iterations = 8

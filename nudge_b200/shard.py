@@ -77,8 +77,10 @@ def local_scene(g, owned, ghosts):
     s.box_transforms["body"] = lb
     s.sphere_data[:] = g.sphere_data[ks]; s.sphere_transforms[:] = g.sphere_transforms[ks]; s.sphere_tags[:] = g.sphere_tags[ks]
     s.sphere_transforms["body"] = ls
-    for k in ("time_step", "iterations", "gravity", "damping"):
+    for k in ("time_step", "iterations", "gravity", "damping", "filter_flags"):
         setattr(s, k, getattr(g, k))
+    if g.collision_filters is not None:   # ghosts keep their global filter: every rank decides a cross-shard pair the same way
+        s.collision_filters = np.concatenate([g.collision_filters[:g.n_boxes][kb], g.collision_filters[g.n_boxes:][ks]])
     return s, gids
 
 
