@@ -17,6 +17,7 @@
  *   nb_instance_matrices            <- the draw loops of render()          example/main.cpp:224-268 (helpers :53-110)
  *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
  *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
+ *   nb_upload_sensors               <- no reference counterpart (the reference has no trigger volumes)
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -195,12 +196,12 @@ int nb_download_constraint_rows(nb_context*, nb_constraint_row* host_rows, uint3
  * pairs would be reported by several ranks. */
 typedef struct {
 	uint64_t tags;                 /* A | (uint64)B << 32: the pair's collider tags (the cache key) */
-	uint32_t kind, step;           /* NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2; device sub-step counter */
+	uint32_t kind, step;           /* NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2 (NB_SENSOR_BEGIN = 3, NB_SENSOR_END = 4: nb_upload_sensors); device sub-step counter */
 	uint32_t body_a, body_b, contacts;
 	float penetration, position[3], normal[3], impulse[3];
 	uint32_t reserved[3];
 } nb_contact_event;                /* 80 bytes */
-enum nb_contact_event_kind { NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2 };
+enum nb_contact_event_kind { NB_CONTACT_BEGIN = 1, NB_CONTACT_END = 2, NB_SENSOR_BEGIN = 3, NB_SENSOR_END = 4 };
 /* capacity = events the device buffer holds between two drains; 0 disables.  Every call resets count, dropped and step; the buffer is reused
  * unless the capacity grows.  Synchronises the device. */
 int nb_enable_contact_events(nb_context*, uint32_t capacity);
@@ -225,6 +226,31 @@ int nb_download_contact_events(nb_context*, nb_contact_event* host, uint32_t cap
 typedef struct { uint16_t category, mask; } nb_collision_filter;   /* 4 bytes */
 enum nb_filter_flags { NB_FILTER_SKIP_CONNECTED = 1 };
 int nb_upload_collision_filters(nb_context*, const nb_collision_filter* host, uint32_t n, uint32_t flags, void* stream);
+
+/* Sensor colliders (trigger volumes; DESIGN.md section 8.7): colliders that detect overlap and exert no force.  One byte per collider, boxes
+ * first then spheres (the order of nb_upload_colliders): nonzero = sensor.  A pair of colliders is a SENSOR PAIR when exactly one of them is a
+ * sensor (two sensors never interact), they are on different bodies, their AABBs overlap strictly and the pair passes the collision filter
+ * and NB_FILTER_SKIP_CONNECTED as an ordinary pair would.  A sensor pair is not a broadphase pair: it is not counted in nb_counts.pairs,
+ * does not link or wake islands, and never reaches the sleeping pairs, contacts, contact cache, solver or contact events.  It OVERLAPS when
+ * the narrowphase would give it at least one contact (the same code and pair orientation as the contact pipeline), evaluated in every
+ * nb_collide whether its bodies sleep or not.
+ * Overlap list of the last nb_collide: one entry per overlapping pair, key tags = min(tag_i, tag_j) | (uint64)max(tag_i, tag_j) << 32 (the
+ * collider tags, like the contact-event key), body_a = the body of the lower-tag collider, body_b = the other's; ascending by tags.
+ * Events (with nb_enable_contact_events): nb_write_cached_impulses compares the overlap list of the step's nb_collide (cur) with the one as of
+ * its previous call (old) and appends, after the contact ENDs and BEGINs, NB_SENSOR_END for every key in old and not in cur, then NB_SENSOR_BEGIN
+ * for every key in cur and not in old, each in ascending key order.  A sensor event carries tags, kind, step, body_a and body_b; every other
+ * field is 0.  After nb_upload_sensors and nb_load_state old is empty, so the next step begins every overlap.
+ * n = boxes + spheres uploads a table, n = 0 removes it, any other n is NB_ERR_ARGUMENT.  max_sensor_pairs = capacity for candidate sensor
+ * pairs (AABB hits) per nb_collide; 0 = 256 per sensor collider, at least 1024, at most the context's scratch capacity (the largest of
+ * max_pairs, max_contacts, bodies and colliders, which is also the upper limit: NB_ERR_CAPACITY above it).  More candidates set bit 32 of
+ * nb_counts.overflow (nb_download_counts returns NB_ERR_OVERFLOW), and that step's overlaps and sensor events are undefined.
+ * nb_upload_colliders keeps the table while the collider count is unchanged and removes it when the count changes.  nb_save_state writes it
+ * (state version 3), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT): a ghost's overlaps would be reported by
+ * several ranks.  Cost: 5 kernel launches per nb_collide and 1 per nb_write_cached_impulses with a table, none without.  Synchronises `stream`. */
+typedef struct { uint64_t tags; uint32_t body_a, body_b; } nb_sensor_overlap;   /* 16 bytes */
+int nb_upload_sensors(nb_context*, const uint8_t* host_flags, uint32_t n, uint32_t max_sensor_pairs, void* stream);
+/* The overlaps of the last nb_collide, ascending by tags.  *count = their number; NB_ERR_CAPACITY if capacity < *count.  Synchronises `stream`. */
+int nb_download_sensor_overlaps(nb_context*, nb_sensor_overlap* host, uint32_t capacity, uint32_t* count, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

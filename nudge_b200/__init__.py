@@ -22,7 +22,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_set_solver_mode", "nb_get_solver_mode", "nb_debug_timing_enable", "nb_debug_timing",
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
-           "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters"]
+           "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
+           "nb_upload_sensors", "nb_download_sensor_overlaps"]
 
 
 class Config(C.Structure):
@@ -98,6 +99,8 @@ def load_library():
         lib.nb_enable_contact_events.argtypes = [V, C.c_uint32]
         lib.nb_download_contact_events.argtypes = [V, V, C.c_uint32, V, V, V]
         lib.nb_upload_collision_filters.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
+        lib.nb_upload_sensors.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
+        lib.nb_download_sensor_overlaps.argtypes = [V, V, C.c_uint32, V, V]
         _lib = lib
     return _lib
 
@@ -285,6 +288,8 @@ class Sim(abi.HostState):
         s = self.scene
         if getattr(s, "collision_filters", None) is not None or getattr(s, "filter_flags", 0):
             self.upload_collision_filters(s.collision_filters, s.filter_flags)
+        if getattr(s, "sensors", None) is not None:
+            self.upload_sensors(s.sensors)
 
     def upload_bodies(self):
         self._ck(self.lib.nb_upload_bodies(self.ctx, C.byref(self.bodies), self.stream), "nb_upload_bodies")
@@ -380,6 +385,25 @@ class Sim(abi.HostState):
         category_i & mask_j and category_j & mask_i are both nonzero."""
         f = np.zeros(0, scenes.FILTER) if filters is None else np.ascontiguousarray(filters, scenes.FILTER)
         self._ck(self.lib.nb_upload_collision_filters(self.ctx, abi.ptr(f) if len(f) else None, len(f), int(flags), self.stream), "nb_upload_collision_filters")
+
+    # ---- sensor colliders (nb_upload_sensors, include/nudge_b200.h): overlap without force ----
+    def upload_sensors(self, flags, max_pairs=0):
+        """flags: one uint8 per collider, boxes first then spheres (nonzero = sensor), or None / empty to remove the table.  max_pairs =
+        candidate sensor pairs per collide (0: 256 per sensor collider, at least 1024).  The overlaps are sensor_overlaps(); with contact
+        events enabled, SENSOR_BEGIN / SENSOR_END events follow the contact events of every step."""
+        f = np.zeros(0, np.uint8) if flags is None else np.ascontiguousarray(flags, np.uint8)
+        self._ck(self.lib.nb_upload_sensors(self.ctx, abi.ptr(f) if len(f) else None, len(f), int(max_pairs), self.stream), "nb_upload_sensors")
+
+    def sensor_overlaps(self):
+        """The overlaps of the last collide as a scenes.SENSOR_OVERLAP array, ascending by tags."""
+        n = C.c_uint32(0)
+        out = np.zeros(1, scenes.SENSOR_OVERLAP)
+        r = self.lib.nb_download_sensor_overlaps(self.ctx, abi.ptr(out), 1, C.byref(n), self.stream)
+        if r == -2:   # NB_ERR_CAPACITY: *count says how many are stored
+            out = np.zeros(n.value, scenes.SENSOR_OVERLAP)
+            r = self.lib.nb_download_sensor_overlaps(self.ctx, abi.ptr(out), len(out), C.byref(n), self.stream)
+        self._ck(r, "nb_download_sensor_overlaps")
+        return out[:n.value].copy()
 
     # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
     def enable_contact_events(self, capacity):

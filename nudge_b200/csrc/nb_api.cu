@@ -18,7 +18,7 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 
 // A sub-step as a CUDA graph (nb_step, nb_shard_step; run_graphed): captured once per key and replayed while the key holds.  Every
 // count the kernels need lives in device memory, so the graph only depends on the parameters and the scene shape held in the key.
-struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version; };
+struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version, sensor_version; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
 struct nb_context {
@@ -54,6 +54,11 @@ struct nb_context {
 	// collision filters (nb_upload_collision_filters): one category | mask << 16 word per collider while has_filter; with
 	// NB_FILTER_SKIP_CONNECTED and connections, conn_keys holds the sorted connection keys and conn_probe = their count (else 0)
 	u32* filter; bool has_filter; u32 filter_flags; u64* conn_keys; u64* conn_scratch; u32* conn_sort_n; u32 conn_probe; unsigned long long filter_version;
+	// sensor colliders (nb_upload_sensors, DESIGN.md section 8.7): one 0/1 byte per collider while has_sensor; sensor_cap = candidate sensor
+	// pairs per collide.  The candidate keys, the sort buffers and the current / old overlap lists hold sensor_alloc entries and are kept while
+	// large enough.
+	uint8_t* sensor; bool has_sensor; u32 sensor_cap, sensor_alloc; u64* sensor_keys; SortBuffers sensor_sb; uint4* sensor_cur; uint4* sensor_old;
+	unsigned long long sensor_version;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -116,6 +121,7 @@ __global__ void k_reset_collide(u32* counts, u32 K, u64* keybits) {
 		keybits[0] = 0; keybits[1] = ~(u64)0;
 		counts[CNT_SCRATCH1] = K;  // key count of the Morton sort
 		counts[CNT_PAIRS] = 0; counts[CNT_OVERFLOW] = 0; counts[CNT_EXT_SUM] = 0;
+		counts[CNT_SENSOR_PAIRS] = 0; counts[CNT_SENSOR_HITS] = 0; counts[CNT_SENSOR_TMP] = 0;
 		for (int k = 0; k < 18; ++k) counts[CNT_EXT_HIST + k] = 0;
 		for (int k = 0; k < 4; ++k) { counts[CNT_BMIN0 + k] = 0xffffffffu; counts[CNT_BMAX0 + k] = 0; }
 	}
@@ -165,7 +171,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	key.stream = st; key.ts = time_step; key.gravity = gravity; key.damping = damping; key.iterations = iterations;
 	key.B = ctx->B; key.nboxes = ctx->nboxes; key.nspheres = ctx->nspheres; key.nconn = ctx->nconn; key.tagbits = ctx->tagbits; key.kbits = ctx->kbits;
 	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version; key.events_version = ctx->events_version;
-	key.filter_version = ctx->filter_version;
+	key.filter_version = ctx->filter_version; key.sensor_version = ctx->sensor_version;
 	if (!g.exec || memcmp(&key, &g.key, sizeof(key)) != 0) {
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -207,6 +213,64 @@ static int build_conn_lookup(nb_context* ctx, cudaStream_t st) {
 	nb_radix_sort(mk_launch(ctx, st), cs, ctx->conn_sort_n, 0, 64, false, 0);   // the result lands in keys[1] = conn_keys
 	CK(cudaGetLastError());
 	return NB_OK;
+}
+
+// Installs a sensor table of n flags (n = 0 removes it) with room for max_pairs candidate pairs (0: NB_SENSOR_PAIRS_PER_SENSOR per sensor
+// collider, at least NB_SENSOR_PAIRS_MIN, at most the context's scratch stride), and empties the old overlap list, so that the next
+// nb_write_cached_impulses begins every overlap.  Synchronises `st`.
+#define NB_SENSOR_PAIRS_PER_SENSOR 256u
+#define NB_SENSOR_PAIRS_MIN 1024u
+static void free_sensor_lists(nb_context* ctx) {
+	void* p[] = { ctx->sensor_keys, ctx->sensor_sb.keys[0], ctx->sensor_sb.keys[1], ctx->sensor_sb.vals[0], ctx->sensor_sb.vals[1], ctx->sensor_cur, ctx->sensor_old };
+	for (void* q : p) if (q) cudaFree(q);
+	ctx->sensor_keys = nullptr; ctx->sensor_sb.keys[0] = ctx->sensor_sb.keys[1] = nullptr; ctx->sensor_sb.vals[0] = ctx->sensor_sb.vals[1] = nullptr;
+	ctx->sensor_cur = ctx->sensor_old = nullptr; ctx->sensor_alloc = 0;
+}
+static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pairs, cudaStream_t st) {
+	CK(cudaStreamSynchronize(st));
+	u32 cap = 0;
+	if (n) {
+		std::vector<uint8_t> f(n);
+		u32 ns = 0;
+		for (u32 i = 0; i < n; ++i) { f[i] = host[i] ? 1 : 0; ns += f[i]; }
+		cap = max_pairs ? max_pairs : std::min<u64>(std::max<u64>(NB_SENSOR_PAIRS_MIN, (u64)NB_SENSOR_PAIRS_PER_SENSOR * ns), ctx->stride);
+		if (cap > ctx->stride) {   // k_sensor_np's flags and the event flags live in the scratch planes
+			ctx->error = "max_sensor_pairs exceeds the context's scratch capacity (" + std::to_string(ctx->stride) + ": the largest of max_pairs, max_contacts, bodies, colliders)";
+			return NB_ERR_CAPACITY;
+		}
+		if (cap > ctx->sensor_alloc) {
+			free_sensor_lists(ctx);
+			CK(cudaMalloc(&ctx->sensor_keys, sizeof(u64) * (size_t)cap));
+			for (int i = 0; i < 2; ++i) { CK(cudaMalloc(&ctx->sensor_sb.keys[i], sizeof(u64) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_sb.vals[i], sizeof(u32) * (size_t)cap)); }
+			CK(cudaMalloc(&ctx->sensor_cur, sizeof(uint4) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_old, sizeof(uint4) * (size_t)cap));
+			ctx->sensor_alloc = cap;
+		}
+		ctx->sensor_sb.hist = ctx->sb.hist; ctx->sensor_sb.bar = ctx->sb.bar;
+		CK(cudaMemcpyAsync(ctx->sensor, f.data(), n, cudaMemcpyHostToDevice, st));
+	}
+	CK(cudaMemsetAsync(ctx->counts + CNT_SENSOR_PAIRS, 0, 3 * sizeof(u32), st));   // candidates, current and old overlaps
+	CK(cudaStreamSynchronize(st));
+	ctx->has_sensor = n != 0; ctx->sensor_cap = cap;
+	++ctx->sensor_version;   // nb_step's graph re-records with or without the sensor launches
+	return NB_OK;
+}
+
+// The sensor pairs' overlaps of one collide (nb_collide.cuh, below k_np_emit): test, compact, sort by key, gather.  5 launches.
+static void launch_sensor_overlaps(nb_context* ctx, const Launch& L) {
+	cudaStream_t st = L.stream;
+	u32* counts = ctx->counts;
+	const u32 cap = ctx->sensor_cap;
+	k_sensor_np<<<GRID((size_t)cap * 4), NB_BLOCK, 0, st>>>(ctx->sensor_keys, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
+		ctx->col_tag, ctx->col_body, ctx->flags, counts);
+	++ctx->launches;
+	nb_scan_reduce<1>(L, ctx->flags, ctx->stride, counts + CNT_SENSOR_PAIRS, 0, ctx->block_sums, counts + CNT_SENSOR_HITS);
+	k_sensor_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->sensor_keys, ctx->kbits, ctx->col_tag,
+		ctx->sensor_sb.keys[0], ctx->sensor_sb.vals[0], counts);
+	++ctx->launches;
+	const int cur = nb_radix_sort(L, ctx->sensor_sb, counts + CNT_SENSOR_HITS, 0, (int)ctx->tagbits, true, 0, 32, (int)(32 + ctx->tagbits));
+	k_sensor_gather<<<GRID(cap), NB_BLOCK, 0, st>>>(ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys, ctx->kbits, ctx->col_tag, ctx->col_body,
+		ctx->sensor_cur, counts);
+	++ctx->launches;
 }
 
 extern "C" {
@@ -259,7 +323,7 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->box_tags, c.max_boxes); ALLOC(ctx->box_data, c.max_boxes); ALLOC(ctx->box_xf, c.max_boxes);
 	ALLOC(ctx->sph_tags, c.max_spheres); ALLOC(ctx->sph_data, c.max_spheres); ALLOC(ctx->sph_xf, c.max_spheres);
 	ALLOC(ctx->conn, c.max_connections);
-	ALLOC(ctx->filter, K); ALLOC(ctx->conn_keys, c.max_connections); ALLOC(ctx->conn_scratch, c.max_connections); ALLOC(ctx->conn_sort_n, 1);
+	ALLOC(ctx->filter, K); ALLOC(ctx->sensor, K); ALLOC(ctx->conn_keys, c.max_connections); ALLOC(ctx->conn_scratch, c.max_connections); ALLOC(ctx->conn_sort_n, 1);
 	ALLOC(ctx->counts, CNT__COUNT); ALLOC(ctx->keybits, 2);
 	ALLOC(ctx->world_xf, K); ALLOC(ctx->aabb_min, K); ALLOC(ctx->aabb_max, K); ALLOC(ctx->col_tag, K); ALLOC(ctx->col_body, K);
 	ALLOC(ctx->order, K); ALLOC(ctx->rank, K);
@@ -344,6 +408,7 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->copy_stream) { cudaStreamDestroy(ctx->copy_stream); cudaEventDestroy(ctx->ev_up_begin); cudaEventDestroy(ctx->ev_up_done); }
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
 	if (ctx->events) cudaFree(ctx->events);
+	free_sensor_lists(ctx);
 	delete ctx;
 }
 
@@ -382,6 +447,7 @@ int nb_download_transforms(nb_context* ctx, nb_transform* h, uint32_t count, voi
 int nb_upload_colliders(nb_context* ctx, const nb_collider_data* h, void* stream) {
 	if (h->boxes.count > ctx->cfg.max_boxes || h->spheres.count > ctx->cfg.max_spheres) { ctx->error = "too many colliders"; return NB_ERR_CAPACITY; }
 	if (ctx->has_filter && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_filter = false; ++ctx->filter_version; }  // the table belongs to a collider count
+	if (ctx->has_sensor && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_sensor = false; ++ctx->sensor_version; }  // so does the sensor table
 	ctx->nboxes = h->boxes.count; ctx->nspheres = h->spheres.count;
 	u32 maxtag = 1;
 	for (u32 i = 0; i < h->boxes.count; ++i) maxtag = std::max(maxtag, h->boxes.tags[i]);
@@ -414,6 +480,12 @@ int nb_upload_collision_filters(nb_context* ctx, const nb_collision_filter* h, u
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
+int nb_upload_sensors(nb_context* ctx, const uint8_t* h, uint32_t n, uint32_t max_sensor_pairs, void* stream) {
+	const u32 K = ctx->nboxes + ctx->nspheres;
+	if (n != 0 && n != K) { ctx->error = "sensor table count must be 0 or boxes + spheres (" + std::to_string(K) + ")"; return NB_ERR_ARGUMENT; }
+	if (n && !h) { ctx->error = "null sensor table"; return NB_ERR_ARGUMENT; }
+	return set_sensors(ctx, h, n, max_sensor_pairs, (cudaStream_t)stream);
+}
 int nb_upload_cache(nb_context* ctx, const nb_contact_cache* h, void* stream) {
 	if (h->count > ctx->cfg.max_contacts) { ctx->error = "cache too large"; return NB_ERR_CAPACITY; }
 	H2D(ctx->cache_tags, h->tags, h->count, u64); H2D(ctx->cache_features, h->features, h->count, u32); H2D(ctx->cache_data, h->data, h->count, nb_cached_impulse);
@@ -441,7 +513,23 @@ int nb_download_counts(nb_context* ctx, nb_counts* out, void* stream) {
 	out->pairs = h[CNT_PAIRS]; out->live_pairs = h[CNT_LIVE_TOTAL]; out->contacts = h[CNT_CONTACTS]; out->sleeping = h[CNT_SLEEPING];
 	out->active = h[CNT_ACTIVE]; out->cache = h[CNT_CACHE]; out->culled = h[CNT_CULLED]; out->batches = h[CNT_BATCHES]; out->levels = h[CNT_LEVELS];
 	out->overflow = h[CNT_OVERFLOW];
-	if (h[CNT_OVERFLOW]) { ctx->error = "capacity overflow during the last step (nb_counts.overflow: 1 pairs, 2 contacts, 4 batch scheduler)"; return NB_ERR_OVERFLOW; }
+	if (h[CNT_OVERFLOW]) {
+		ctx->error = "capacity overflow during the last step (nb_counts.overflow: 1 pairs, 2 contacts, 4 batch scheduler, 32 sensor pairs)";
+		if (h[CNT_OVERFLOW] & OVF_SENSORS) ctx->error += "; bit 32: more candidate sensor pairs than max_sensor_pairs (nb_upload_sensors), the step's overlaps and sensor events are undefined";
+		return NB_ERR_OVERFLOW;
+	}
+	return NB_OK;
+}
+int nb_download_sensor_overlaps(nb_context* ctx, nb_sensor_overlap* host, uint32_t capacity, uint32_t* count, void* stream) {
+	NB_RANGE("nb_download_sensor_overlaps");
+	u32 c[CNT__COUNT];
+	int r = get_counts(ctx, c, stream); if (r) return r;
+	const u32 n = ctx->has_sensor ? c[CNT_SENSOR_HITS] : 0;
+	if (count) *count = n;
+	if (n > capacity) { ctx->error = "host overlap buffer too small: " + std::to_string(n) + " overlaps"; return NB_ERR_CAPACITY; }
+	if (n && !host) { ctx->error = "null host overlap buffer"; return NB_ERR_ARGUMENT; }
+	D2H(host, ctx->sensor_cur, n, nb_sensor_overlap);
+	CK(cudaStreamSynchronize((cudaStream_t)stream));
 	return NB_OK;
 }
 int nb_download_contacts(nb_context* ctx, nb_contact_data* h, nb_active_bodies* ha, void* stream) {
@@ -518,10 +606,11 @@ int nb_collide(nb_context* ctx, void* stream) {
 	++ctx->launches;
 	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
 	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
+	const uint8_t* sensor = ctx->has_sensor ? ctx->sensor : nullptr;   // null: the kernels never touch the sensor list
 	k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	ctx->launches += 3;
 	// nudge.cpp:3498; the sort also clamps CNT_PAIRS to the capacity (the overflow bit is already set by emit_pair)
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);
@@ -573,6 +662,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 	k_copy_u64<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sleeping, ctx->sb.keys[0], counts + CNT_SLEEPING); ++ctx->launches;
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_SLEEPING, 0, (int)ctx->tagbits, false, 0, 32, (int)(32 + ctx->tagbits));
 	k_copy_u64<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sb.keys[cur], ctx->sleeping, counts + CNT_SLEEPING); ++ctx->launches;
+	if (ctx->has_sensor) launch_sensor_overlaps(ctx, L);   // the scratch planes are free again here
 	ctx->contacts_internal = true;
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -639,9 +729,12 @@ int nb_read_cached_impulses(nb_context* ctx, void* stream) {
 int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_write_cached_impulses");
 	const u32 C = ctx->cfg.max_contacts;
+	const uint4* s_old = ctx->has_sensor ? ctx->sensor_old : nullptr;
+	const uint4* s_cur = ctx->has_sensor ? ctx->sensor_cur : nullptr;
 	if (ctx->ev_cap)   // the old cache is still intact here
 		launch_contact_events(mk_launch(ctx, stream), GRID(2 * (size_t)C), ctx->flags, ctx->stride, ctx->block_sums, ctx->cache_tags, ctx->sorted, ctx->fin,
-							  ctx->culled_tags, ctx->impulses, ctx->events, ctx->ev_cap, ctx->counts);
+							  ctx->culled_tags, ctx->impulses, s_old, s_cur, ctx->events, ctx->ev_cap, ctx->counts);
+	if (ctx->has_sensor) { k_sensor_keep<<<GRID(ctx->sensor_cap), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sensor_cur, ctx->sensor_old, ctx->counts); ++ctx->launches; }
 	k_cache_merge<<<GRID(C), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sorted, ctx->fin.tags, ctx->fin.features, ctx->impulses,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->counts);
 	++ctx->launches;
@@ -843,7 +936,8 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 	return nb_advance(ctx, time_step, stream);
 }
 
-// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (60 launches in parity mode, 3 more with contact events).
+// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (60 launches in parity mode, 3 more with contact events,
+// 6 more with sensor colliders).
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
@@ -913,6 +1007,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "inertia", ctx->inertia, sizeof(float4) * 2 * ctx->B },
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
+		{ "sensor_pairs", ctx->sensor_keys, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }

@@ -23,9 +23,12 @@ enum {  // device counters (u32 each)
 	CNT_EXT_HIST = 64 /* 18 bins */,
 	// contact events (nb_events.cuh): kept across steps, k_reset_collide leaves them alone
 	CNT_EV_COUNT = 82, CNT_EV_DROPPED, CNT_EV_STEP, CNT_EV_N, CNT_EV_FLAGGED, CNT_EV_BASE, CNT_EV_STAMP,
+	// sensor colliders (DESIGN.md section 8.7): candidate sensor pairs of the broadphase, the overlaps of the last collide, the overlaps as of
+	// the last nb_write_cached_impulses (kept across steps, k_reset_collide leaves it alone), bb_clip's slot counter (nothing is written)
+	CNT_SENSOR_PAIRS = 89, CNT_SENSOR_HITS, CNT_SENSOR_OLD, CNT_SENSOR_TMP,
 	CNT__COUNT = 96
 };
-enum { OVF_PAIRS = 1, OVF_CONTACTS = 2, OVF_SCHED = 4, OVF_LEVELS = 8 };
+enum { OVF_PAIRS = 1, OVF_CONTACTS = 2, OVF_SCHED = 4, OVF_LEVELS = 8, OVF_SENSORS = 32 /* 16 is OVF_EXCHANGE, nb_shard.cuh */ };
 
 // ---------------- collision filters (nb_upload_collision_filters, DESIGN.md section 8.6) ----------------
 // A collider's filter word is category | mask << 16; it rides in the otherwise unused w lane of its AABB max corner, so the broadphase
@@ -255,6 +258,13 @@ NB_DEV void emit_pair(u32 p, u32 q, const u32* order, u32 kbits, u64* pair_keys,
 	if (slot < max_pairs) pair_keys[slot] = ((u64)order[p] << kbits) | (u64)order[q];  // hi = earlier, lo = later (nudge.cpp:3495)
 	else atomicOr(&counts[CNT_OVERFLOW], OVF_PAIRS);
 }
+// Sensor colliders (nb_upload_sensors, DESIGN.md section 8.7): `sensor` holds one 0/1 byte per collider, or is null without a table.  A hit
+// with exactly one sensor goes to the sensor list (same key as a broadphase pair) instead of the pair list; a hit of two sensors is dropped.
+NB_DEV void emit_sensor(u64 key, u64* sensor_keys, u32 max_sensor_pairs, u32* counts) {
+	u32 slot = warp_append_slot(&counts[CNT_SENSOR_PAIRS]);
+	if (slot < max_sensor_pairs) sensor_keys[slot] = key;
+	else atomicOr(&counts[CNT_OVERFLOW], OVF_SENSORS);
+}
 
 // One warp per small collider.  Lanes 0..26 each look up one neighbouring cell (cells whose Morton prefix is below the
 // collider's own hold only earlier positions and are skipped); the candidate ranges are then flattened with a warp scan and
@@ -264,7 +274,7 @@ NB_DEV void emit_pair(u32 p, u32 q, const u32* order, u32 kbits, u64* pair_keys,
 #define NB_GP_BUF 128
 __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order, const float4* leaf_min, const float4* leaf_max, const uint8_t* smallf, const u64* mkeys,
 		const u64* table_keys, const u64* table_vals, u32 table_mask, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n,
-		u64* pair_keys, u32 max_pairs, u32* counts) {
+		const uint8_t* sensor, u64* sensor_keys, u32 max_sensor_pairs, u64* pair_keys, u32 max_pairs, u32* counts) {
 	__shared__ u64 buf[NB_WARPS][NB_GP_BUF];
 	__shared__ u32 fill[NB_WARPS];
 	const MortonFrame f = morton_frame(counts);
@@ -336,6 +346,17 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 			if (hit) {
 				oq = order[q];
 				if (conn_n) hit = !connected(conn_keys, conn_n, __ldg(col_body + op), __ldg(col_body + oq));
+				if (hit && sensor) {   // only for hits, only with a table: the candidate's flag, and this collider's (the same byte for the whole warp)
+					const u32 s = (u32)__ldg(sensor + op) | (u32)__ldg(sensor + oq) << 1;
+					if (s) {
+						if (s != 3) {
+							const u32 g = atomicAdd(&counts[CNT_SENSOR_PAIRS], 1u);
+							if (g < max_sensor_pairs) sensor_keys[g] = hi_key | (u64)oq;
+							else atomicOr(&counts[CNT_OVERFLOW], OVF_SENSORS);
+						}
+						hit = false;
+					}
+				}
 			}
 			if (hit) {
 				u32 slot = atomicAdd(&fill[wid], 1u);
@@ -354,7 +375,8 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 }
 
 __global__ void __launch_bounds__(NB_BLOCK) k_large_pairs(u32 K, const u32* order, const float4* leaf_min, const float4* leaf_max, const uint8_t* smallf,
-		const u32* large_list, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n, u64* pair_keys, u32 max_pairs, u32* counts) {
+		const u32* large_list, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n, const uint8_t* sensor, u64* sensor_keys, u32 max_sensor_pairs,
+		u64* pair_keys, u32 max_pairs, u32* counts) {
 	const u32 nlarge = counts[CNT_LARGE];
 	for (u32 l = 0; l < nlarge; ++l) {
 		const u32 pl = large_list[l];
@@ -363,8 +385,12 @@ __global__ void __launch_bounds__(NB_BLOCK) k_large_pairs(u32 K, const u32* orde
 			if (q == pl || (!smallf[q] && q < pl)) continue;  // a pair of two large colliders is reported from the earlier one
 			const float4 bq = leaf_max[q];
 			if (boxes_overlap(lo, hi, leaf_min[q], bq) && filter_pass(asu(hi.w), asu(bq.w))
-				&& !(conn_n && connected(conn_keys, conn_n, col_body[order[pl]], col_body[order[q]])))
-				emit_pair(min(pl, q), max(pl, q), order, kbits, pair_keys, max_pairs, counts);
+				&& !(conn_n && connected(conn_keys, conn_n, col_body[order[pl]], col_body[order[q]]))) {
+				const u32 p0 = min(pl, q), p1 = max(pl, q);
+				const u32 s = sensor ? (u32)sensor[order[p0]] | (u32)sensor[order[p1]] << 1 : 0u;
+				if (!s) emit_pair(p0, p1, order, kbits, pair_keys, max_pairs, counts);
+				else if (s != 3) emit_sensor(((u64)order[p0] << kbits) | (u64)order[p1], sensor_keys, max_sensor_pairs, counts);
+			}
 		}
 	}
 }
@@ -1020,4 +1046,73 @@ __global__ void __launch_bounds__(NB_BLOCK) k_contact_compact(ContactOut st, Con
 		}
 		if (v[1]) sleeping_pairs[sleep_base + off[1]] = st.tags[i];
 	});
+}
+
+// ---------------- sensor overlaps (nb_upload_sensors, DESIGN.md section 8.7) ----------------
+// A sensor pair overlaps iff the narrowphase would give it at least one contact, decided by the narrowphase's own code in the orientation
+// k_partition and k_np_faces give the pair's class: box-box -> bb_faces on (low, high), then bb_clip with a's face owner first and a zero
+// limit (it counts the contacts and writes none); box-sphere -> box_sphere with the box as a; sphere-sphere -> sphere_sphere with a = high
+// half (bucket 2 has its halves swapped, so its box is the low half).  Four lanes per pair as in k_np_clip, so that the whole warp meets
+// bb_clip's shuffles; sphere pairs and pairs on one body run bb_clip as invalid groups.  flags[k] = pair k overlaps.
+__global__ void __launch_bounds__(NB_BLOCK, 3) k_sensor_np(const u64* sensor_keys, u32 max_sensor_pairs, u32 kbits, u32 nboxes, const nb_transform* world_xf,
+		const nb_box_collider* box_data, const nb_sphere_collider* sph_data, const u32* col_tag, const u32* col_body, u32* flags, u32* counts) {
+	__shared__ u32 s_rsqrt[2048];
+	for (u32 i = threadIdx.x; i < 2048; i += blockDim.x) s_rsqrt[i] = g_rsqrt_lut[i];
+	__syncthreads();
+	const u32 n = min(counts[CNT_SENSOR_PAIRS], max_sensor_pairs);
+	if (blockIdx.x == 0 && threadIdx.x == 0) counts[CNT_SENSOR_PAIRS] = n;   // the scan's length; every block reads min(count, capacity)
+	const u64 mask = ((u64)1 << kbits) - 1;
+	const u32 warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, warps = (gridDim.x * blockDim.x) >> 5, g = (threadIdx.x & 31) >> 2;
+	const ContactOut none = { nullptr, nullptr, nullptr, nullptr };
+	for (u32 k0 = warp * 8; k0 < n; k0 += warps * 8) {
+		const u32 k = k0 + g;
+		u32 lo = 0, hi = 0;
+		if (k < n) { const u64 key = sensor_keys[k]; lo = (u32)(key & mask); hi = (u32)(key >> kbits); }
+		const bool apart = k < n && col_body[lo] != col_body[hi];   // k_pair_flags: a pair on one body is no pair
+		const u32 cls = (lo >= nboxes ? 1u : 0u) | (hi >= nboxes ? 2u : 0u);
+		BoxIn A = {}, B = {};
+		float pen = 0.0f; u32 face = 0;
+		bool clip = false, hit = false;
+		if (apart && cls == 0) {
+			const BoxIn L = load_box(world_xf, box_data, col_tag, lo), H = load_box(world_xf, box_data, col_tag, hi);   // k_np_faces: a = low, b = high
+			bool swapped;
+			clip = bb_faces(L, H, pen, face, swapped);
+			A = swapped ? H : L; B = swapped ? L : H;   // load_pair: a owns the most separating face
+		}
+		else if (apart) {
+			const u32 a = cls == 2 ? lo : hi, b = cls == 2 ? hi : lo;
+			const xform ta = ld_xform(world_xf, a), tb = ld_xform(world_xf, b);
+			float o[7];
+			if (cls != 3) { const float4 sz = reinterpret_cast<const float4*>(box_data)[a]; hit = box_sphere(make_float3(sz.x, sz.y, sz.z), sph_data[b - nboxes].radius, ta, tb, o); }
+			else hit = sphere_sphere(sph_data[a - nboxes].radius, sph_data[b - nboxes].radius, ta, tb, o);
+		}
+		u32 at, nface, nedge;
+		bb_clip(A, B, pen, face, clip, s_rsqrt, &counts[CNT_SENSOR_TMP], none, 0, at, nface, nedge);
+		if (k < n && (threadIdx.x & 3) == 0) flags[k] = (hit || nface + nedge != 0) ? 1u : 0u;
+	}
+}
+
+NB_DEV u64 sensor_overlap_key(u64 pair_key, u32 kbits, const u32* col_tag) {   // min(tag) | max(tag) << 32, the contact-event key
+	const u32 ta = col_tag[(u32)(pair_key & (((u64)1 << kbits) - 1))], tb = col_tag[(u32)(pair_key >> kbits)];
+	return ta < tb ? (u64)ta | ((u64)tb << 32) : (u64)tb | ((u64)ta << 32);
+}
+// NB_SCAN_GRID blocks, after nb_scan_reduce<1> over k_sensor_np's flags (total in CNT_SENSOR_HITS): the overlapping pairs' keys and their
+// index in the candidate list, for the radix sort by key
+__global__ void __launch_bounds__(NB_BLOCK) k_sensor_compact(const u32* flags, const u32* block_sums, const u64* sensor_keys, u32 kbits, const u32* col_tag,
+		u64* keys, u32* vals, const u32* counts) {
+	scan_consume<1>(flags, 0, counts[CNT_SENSOR_PAIRS], block_sums, [&](u32 i, const u32 (&v)[1], const u32 (&off)[1]) {
+		if (v[0]) { keys[off[0]] = sensor_overlap_key(sensor_keys[i], kbits, col_tag); vals[off[0]] = i; }
+	});
+}
+// The sorted overlap list: nb_sensor_overlap { tags, body of the lower-tag collider, body of the other } as one uint4 per entry
+__global__ void __launch_bounds__(NB_BLOCK) k_sensor_gather(const u64* keys, const u32* vals, const u64* sensor_keys, u32 kbits, const u32* col_tag,
+		const u32* col_body, uint4* out, const u32* counts) {
+	const u32 n = counts[CNT_SENSOR_HITS];
+	const u64 mask = ((u64)1 << kbits) - 1;
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const u64 pk = sensor_keys[vals[i]], t = keys[i];
+		const u32 lo = (u32)(pk & mask), hi = (u32)(pk >> kbits);
+		const bool lo_first = col_tag[lo] == (u32)t;
+		out[i] = make_uint4((u32)t, (u32)(t >> 32), col_body[lo_first ? lo : hi], col_body[lo_first ? hi : lo]);
+	}
 }

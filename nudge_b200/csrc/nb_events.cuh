@@ -10,10 +10,14 @@
 //                    the deepest contact and the impulse sum.
 // The event counters live in counts[] (CNT_EV_*) and survive k_reset_collide.  k_event_flags snapshots count and step into CNT_EV_BASE /
 // CNT_EV_STAMP, so the scatter's blocks read stable values while its block 0 advances count, dropped and step.
+// With sensor colliders (DESIGN.md section 8.7) the concatenation goes on with [old overlaps | current overlaps], both sorted by key (one
+// entry per pair): an old key that is not current is a SENSOR_END, a current key that was not old a SENSOR_BEGIN.  So the same scan ranks
+// contact ENDs, contact BEGINs, sensor ENDs, sensor BEGINs, each in ascending key order.  Without sensors both lists are null and empty.
 #pragma once
 #include "nb_solver.cuh"
 
 static_assert(sizeof(nb_contact_event) == 80, "nb_contact_event is 5 x 16 bytes");
+static_assert(sizeof(nb_sensor_overlap) == 16, "nb_sensor_overlap is one uint4 { tags lo, tags hi, body_a, body_b }");
 
 NB_DEV bool sorted_has(const u64* keys, u32 n, u64 t) {
 	u32 lo = 0, hi = n;
@@ -26,19 +30,39 @@ NB_DEV bool contacts_have(const u32* sorted, const u64* tags, u32 n, u64 t) {
 	return lo < n && tags[sorted[lo]] == t;
 }
 
-__global__ void __launch_bounds__(NB_BLOCK) k_event_flags(const u64* cache_tags, const u32* sorted, const u64* tags, const u64* culled_tags, u32* flags, u32* counts) {
+NB_DEV u64 overlap_key(const uint4* list, u32 i) { const uint4 e = list[i]; return (u64)e.x | ((u64)e.y << 32); }
+NB_DEV bool overlaps_have(const uint4* list, u32 n, u64 t) {
+	u32 lo = 0, hi = n;
+	while (lo < hi) { u32 mid = (lo + hi) >> 1; if (overlap_key(list, mid) < t) lo = mid + 1; else hi = mid; }
+	return lo < n && overlap_key(list, lo) == t;
+}
+
+// s_old / s_cur: the overlaps as of the last call (CNT_SENSOR_OLD entries) and of the last collide (CNT_SENSOR_HITS), or null without sensors
+__global__ void __launch_bounds__(NB_BLOCK) k_event_flags(const u64* cache_tags, const u32* sorted, const u64* tags, const u64* culled_tags,
+		const uint4* s_old, const uint4* s_cur, u32* flags, u32* counts) {
 	const u32 m = counts[CNT_CACHE], n = counts[CNT_CONTACTS], mc = counts[CNT_CULLED];
-	if (blockIdx.x == 0 && threadIdx.x == 0) { counts[CNT_EV_N] = m + n; counts[CNT_EV_BASE] = counts[CNT_EV_COUNT]; counts[CNT_EV_STAMP] = counts[CNT_EV_STEP]; }
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < m + n; i += gridDim.x * blockDim.x) {
+	const u32 so = s_old ? counts[CNT_SENSOR_OLD] : 0u, sc = s_cur ? counts[CNT_SENSOR_HITS] : 0u, mn = m + n;
+	if (blockIdx.x == 0 && threadIdx.x == 0) { counts[CNT_EV_N] = mn + so + sc; counts[CNT_EV_BASE] = counts[CNT_EV_COUNT]; counts[CNT_EV_STAMP] = counts[CNT_EV_STEP]; }
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < mn + so + sc; i += gridDim.x * blockDim.x) {
 		u32 f = 0;
 		if (i < m) {
 			const u64 t = cache_tags[i];
 			if ((i == 0 || cache_tags[i - 1] != t) && !contacts_have(sorted, tags, n, t) && !sorted_has(culled_tags, mc, t)) f = 1;
 		}
-		else {
+		else if (i < mn) {
 			const u32 j = i - m;
 			const u64 t = tags[sorted[j]];
 			if ((j == 0 || tags[sorted[j - 1]] != t) && !sorted_has(cache_tags, m, t)) f = 1;
+		}
+		else if (i < mn + so) {
+			const u32 j = i - mn;
+			const u64 t = overlap_key(s_old, j);
+			if ((j == 0 || overlap_key(s_old, j - 1) != t) && !overlaps_have(s_cur, sc, t)) f = 1;
+		}
+		else {
+			const u32 j = i - mn - so;
+			const u64 t = overlap_key(s_cur, j);
+			if ((j == 0 || overlap_key(s_cur, j - 1) != t) && !overlaps_have(s_old, so, t)) f = 1;
 		}
 		flags[i] = f;
 	}
@@ -46,8 +70,10 @@ __global__ void __launch_bounds__(NB_BLOCK) k_event_flags(const u64* cache_tags,
 
 // NB_SCAN_GRID blocks, after nb_scan_reduce<1> over the flags (total in CNT_EV_FLAGGED)
 __global__ void __launch_bounds__(NB_BLOCK) k_event_scatter(const u32* flags, const u32* block_sums, const u64* cache_tags, const u32* sorted, const u64* tags,
-		const float4* data, const uint2* bodies, const float4* impulses, uint4* events /* 5 words per event */, u32 capacity, u32* counts) {
+		const float4* data, const uint2* bodies, const float4* impulses, const uint4* s_old, const uint4* s_cur, uint4* events /* 5 words per event */,
+		u32 capacity, u32* counts) {
 	const u32 m = counts[CNT_CACHE], n = counts[CNT_CONTACTS], base = counts[CNT_EV_BASE], step = counts[CNT_EV_STAMP];
+	const u32 so = s_old ? counts[CNT_SENSOR_OLD] : 0u;
 	if (blockIdx.x == 0 && threadIdx.x == 0) {
 		const u64 end = (u64)base + counts[CNT_EV_FLAGGED];
 		const u64 kept = end < capacity ? end : capacity;
@@ -62,6 +88,14 @@ __global__ void __launch_bounds__(NB_BLOCK) k_event_scatter(const u32* flags, co
 			const u64 t = cache_tags[i];
 			e[0] = make_uint4((u32)t, (u32)(t >> 32), NB_CONTACT_END, step);
 			e[1] = e[2] = e[3] = e[4] = make_uint4(0, 0, 0, 0);
+			return;
+		}
+		if (i >= m + n) {   // a sensor event: tags, kind, step and the two bodies
+			const bool end = i < m + n + so;
+			const uint4 o = end ? s_old[i - m - n] : s_cur[i - m - n - so];
+			e[0] = make_uint4(o.x, o.y, end ? NB_SENSOR_END : NB_SENSOR_BEGIN, step);
+			e[1] = make_uint4(o.z, o.w, 0, 0);
+			e[2] = e[3] = e[4] = make_uint4(0, 0, 0, 0);
 			return;
 		}
 		const u32 j = i - m;
@@ -88,12 +122,19 @@ __global__ void __launch_bounds__(NB_BLOCK) k_event_scatter(const u32* flags, co
 	});
 }
 
-// The three launches of an enabled nb_write_cached_impulses.
+// The three launches of an enabled nb_write_cached_impulses.  `flags` holds the old cache, the contacts and both overlap lists.
 static void launch_contact_events(const Launch& L, u32 grid, u32* flags, u32 stride, u32* block_sums, const u64* cache_tags, const u32* sorted, const ContactOut& fin,
-								  const u64* culled_tags, const float4* impulses, nb_contact_event* events, u32 capacity, u32* counts) {
-	k_event_flags<<<grid, NB_BLOCK, 0, L.stream>>>(cache_tags, sorted, fin.tags, culled_tags, flags, counts);
+								  const u64* culled_tags, const float4* impulses, const uint4* s_old, const uint4* s_cur, nb_contact_event* events, u32 capacity, u32* counts) {
+	k_event_flags<<<grid, NB_BLOCK, 0, L.stream>>>(cache_tags, sorted, fin.tags, culled_tags, s_old, s_cur, flags, counts);
 	nb_scan_reduce<1>(L, flags, stride, counts + CNT_EV_N, 0, block_sums, counts + CNT_EV_FLAGGED);
-	k_event_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, L.stream>>>(flags, block_sums, cache_tags, sorted, fin.tags, fin.data, fin.bodies, impulses,
+	k_event_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, L.stream>>>(flags, block_sums, cache_tags, sorted, fin.tags, fin.data, fin.bodies, impulses, s_old, s_cur,
 		reinterpret_cast<uint4*>(events), capacity, counts);
 	*L.counter += 2;
+}
+
+// With sensors, at the end of every nb_write_cached_impulses (events on or off): the current overlaps become the old ones
+__global__ void __launch_bounds__(NB_BLOCK) k_sensor_keep(const uint4* cur, uint4* old, u32* counts) {
+	const u32 n = counts[CNT_SENSOR_HITS];
+	if (blockIdx.x == 0 && threadIdx.x == 0) counts[CNT_SENSOR_OLD] = n;
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) old[i] = cur[i];
 }

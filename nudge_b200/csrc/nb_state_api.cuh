@@ -12,6 +12,10 @@
 // Version 2 (a context with collision filters, nb_upload_collision_filters): the same header with reserved[0] = filter flags and
 // reserved[1] = 1 if the table follows, and then filter[boxes + spheres] (4, category | mask << 16) after cache_data.  A context
 // without a table or flags writes version 1; both versions load, and a version-1 load removes any table and flags.
+// Version 3 (a context with sensor colliders, nb_upload_sensors): reserved[0..1] as in version 2, reserved[2] = 1 (the sensor table follows;
+// a version-3 header without it is not a state file), reserved[3] = the context's max_sensor_pairs, and then sensor[boxes + spheres] (1 byte
+// each, 0 or 1) after the filter table, if any.  A context without sensors writes version 1 or 2 as before; every version loads, and a
+// version-1 or 2 load removes any sensor table.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
@@ -23,6 +27,7 @@ static bool state_put(FILE* f, const void* dev, size_t bytes, std::vector<unsign
 	if (cudaStreamSynchronize(st) != cudaSuccess) return false;
 	return padded == 0 || fwrite(tmp.data(), 1, padded, f) == padded;
 }
+static bool state_version_ok(const NbStateHeader& h) { return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1); }
 static bool state_get(FILE* f, void* dev, size_t bytes, std::vector<unsigned char>& tmp, cudaStream_t st) {
 	const size_t padded = (bytes + 15) & ~(size_t)15;
 	tmp.resize(padded);
@@ -43,8 +48,9 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = filtered ? 2 : 1;
+	h.version = ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
+	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = c[CNT_CACHE]; h.solver_mode = (u32)ctx->solver_mode;
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
@@ -55,6 +61,7 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 		&& state_put(f, ctx->conn, sizeof(nb_body_pair) * (size_t)h.connections, tmp, st)
 		&& state_put(f, ctx->cache_tags, 8 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_features, 4 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_data, 16 * (size_t)h.cache, tmp, st);
 	if (h.reserved[1]) ok = ok && state_put(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
+	if (h.reserved[2]) ok = ok && state_put(f, ctx->sensor, (size_t)h.boxes + h.spheres, tmp, st);
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -65,7 +72,7 @@ int nb_state_info(const char* path, uint32_t counts[5]) {
 	FILE* f = fopen(path, "rb");
 	if (!f) return NB_ERR_ARGUMENT;
 	NbStateHeader h;
-	bool ok = fread(&h, sizeof(h), 1, f) == 1 && !memcmp(h.magic, "NBSTATE1", 8) && (h.version == 1 || h.version == 2);
+	bool ok = fread(&h, sizeof(h), 1, f) == 1 && !memcmp(h.magic, "NBSTATE1", 8) && state_version_ok(h);
 	fclose(f);
 	if (!ok) return NB_ERR_ARGUMENT;
 	counts[0] = h.bodies; counts[1] = h.boxes; counts[2] = h.spheres; counts[3] = h.connections; counts[4] = h.cache;
@@ -78,7 +85,7 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	FILE* f = fopen(path, "rb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
 	NbStateHeader h;
-	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8) || (h.version != 1 && h.version != 2)) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
+	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8) || !state_version_ok(h)) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
 	const nb_config& c = ctx->cfg;
 	if (h.bodies > c.max_bodies || h.boxes > c.max_boxes || h.spheres > c.max_spheres || h.connections > c.max_connections || h.cache > c.max_contacts) {
 		fclose(f); ctx->error = "state file exceeds the context's capacities"; return NB_ERR_CAPACITY;
@@ -96,8 +103,14 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	ok = ok && state_get(f, ctx->sph_data, sizeof(nb_sphere_collider) * (size_t)h.spheres, tmp, st) && state_get(f, ctx->sph_xf, sizeof(nb_transform) * (size_t)h.spheres, tmp, st)
 		&& state_get(f, ctx->conn, sizeof(nb_body_pair) * (size_t)h.connections, tmp, st)
 		&& state_get(f, ctx->cache_tags, 8 * (size_t)h.cache, tmp, st) && state_get(f, ctx->cache_features, 4 * (size_t)h.cache, tmp, st) && state_get(f, ctx->cache_data, 16 * (size_t)h.cache, tmp, st);
-	const bool table = h.version == 2 && h.reserved[1];
+	const bool table = h.version >= 2 && h.reserved[1];
 	if (table) ok = ok && state_get(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
+	std::vector<uint8_t> sensors;
+	if (ok && h.version == 3) {
+		const size_t k = (size_t)h.boxes + h.spheres, padded = (k + 15) & ~(size_t)15;
+		sensors.resize(padded);
+		ok = padded == 0 || fread(sensors.data(), 1, padded, f) == padded;
+	}
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->B = h.bodies; ctx->nboxes = h.boxes; ctx->nspheres = h.spheres; ctx->nconn = h.connections;
@@ -106,9 +119,10 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	CK(cudaMemcpyAsync(ctx->counts + CNT_CACHE, &h.cache, 4, cudaMemcpyHostToDevice, st));
 	CK(cudaStreamSynchronize(st));
 	if (h.solver_mode == NB_SOLVER_PARITY || h.solver_mode == NB_SOLVER_THROUGHPUT) ctx->solver_mode = (int)h.solver_mode;
-	ctx->has_filter = table; ctx->filter_flags = h.version == 2 ? (h.reserved[0] & NB_FILTER_SKIP_CONNECTED) : 0;
+	ctx->has_filter = table; ctx->filter_flags = h.version >= 2 ? (h.reserved[0] & NB_FILTER_SKIP_CONNECTED) : 0;
 	++ctx->filter_version;
 	{ int r = build_conn_lookup(ctx, st); if (r) return r; }
+	{ int r = set_sensors(ctx, sensors.data(), h.version == 3 ? h.boxes + h.spheres : 0, h.version == 3 ? h.reserved[3] : 0, st); if (r) return r; }
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }

@@ -27,8 +27,12 @@ CONTACT_BEGIN, CONTACT_END = 1, 2
 # nb_collision_filter (include/nudge_b200.h): colliders i and j collide iff category_i & mask_j and category_j & mask_i are both nonzero
 FILTER = np.dtype([("category", "<u2"), ("mask", "<u2")])
 FILTER_SKIP_CONNECTED = 1
+# nb_sensor_overlap (include/nudge_b200.h): tags = min(tag_i, tag_j) | max(tag_i, tag_j) << 32, body_a = the body of the lower-tag collider;
+# sensor events are CONTACT_EVENT rows of kind SENSOR_BEGIN / SENSOR_END with tags, kind, step, body_a and body_b set
+SENSOR_OVERLAP = np.dtype([("tags", "<u8"), ("body_a", "<u4"), ("body_b", "<u4")])
+SENSOR_BEGIN, SENSOR_END = 3, 4
 
-assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4
+assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4 and SENSOR_OVERLAP.itemsize == 16
 
 
 class Scene:
@@ -52,6 +56,8 @@ class Scene:
         # optional collision filters: one FILTER row per collider (boxes first, then spheres) or None, and FILTER_* flags
         self.collision_filters = None
         self.filter_flags = 0
+        # optional sensor colliders: one uint8 per collider (boxes first, then spheres; nonzero = sensor) or None
+        self.sensors = None
         # step parameters the reference leaves to the caller (example/main.cpp:275-305)
         self.time_step = np.float32(1.0 / 120.0)
         self.iterations = 8

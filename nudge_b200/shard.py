@@ -81,6 +81,8 @@ def local_scene(g, owned, ghosts):
         setattr(s, k, getattr(g, k))
     if g.collision_filters is not None:   # ghosts keep their global filter: every rank decides a cross-shard pair the same way
         s.collision_filters = np.concatenate([g.collision_filters[:g.n_boxes][kb], g.collision_filters[g.n_boxes:][ks]])
+    if getattr(g, "sensors", None) is not None:   # selected like the filter rows (nb_shard_step itself refuses a context with sensors)
+        s.sensors = np.concatenate([g.sensors[:g.n_boxes][kb], g.sensors[g.n_boxes:][ks]]).astype(np.uint8)
     return s, gids
 
 
