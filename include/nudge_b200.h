@@ -18,6 +18,7 @@
  *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
  *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
  *   nb_upload_sensors               <- no reference counterpart (the reference has no trigger volumes)
+ *   nb_upload_kinematic_bodies      <- no reference counterpart (the reference's only non-dynamic body is the static world, body 0)
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -251,6 +252,27 @@ typedef struct { uint64_t tags; uint32_t body_a, body_b; } nb_sensor_overlap;   
 int nb_upload_sensors(nb_context*, const uint8_t* host_flags, uint32_t n, uint32_t max_sensor_pairs, void* stream);
 /* The overlaps of the last nb_collide, ascending by tags.  *count = their number; NB_ERR_CAPACITY if capacity < *count.  Synchronises `stream`. */
 int nb_download_sensor_overlaps(nb_context*, nb_sensor_overlap* host, uint32_t capacity, uint32_t* count, void* stream);
+
+/* Kinematic bodies (moving platforms, elevators, doors, turntables; DESIGN.md section 8.8): bodies that move at the velocity the application
+ * gives them, push dynamic bodies and are never pushed back.  The call replaces the set of kinematic bodies with the n listed bodies and writes
+ * each one's velocity and angular_velocity into its momentum row (the unused lanes are left alone); n = 0 removes the set, and every body is
+ * dynamic again with its momentum row as it stands.  NB_ERR_ARGUMENT, changing nothing: body 0, a body at or beyond the uploaded body count,
+ * or a body listed twice.  Asynchronous on `stream`, ordered like nb_upload_momentum; the host array may be reused when the call returns.
+ * Calling it every step with the same set and new velocities is the intended way to drive platforms: one small copy and one scatter launch,
+ * and nb_step's graph is kept.  A changed set re-records the graph.
+ * A kinematic body has infinite mass and inertia wherever the step reads them (setup writes 0 into its momentum unused0), whatever its
+ * properties row says.  Only the caller changes its velocity (this call, nb_upload_momentum, nb_upload_bodies): gravity, damping, the warm
+ * start, the contact sweeps of both solver modes and the user constraint rows read it and never write it.  It is MOVING when any of its six
+ * velocity components is nonzero (-0.0 counts as zero), as the momentum row stands at nb_collide.  A moving kinematic body is active (in the
+ * active list, in body-index order) and nb_advance integrates it; one at rest is neither.  Islands: a kinematic body never joins a set; an
+ * edge between a dynamic body and a moving kinematic body makes the dynamic body's set active; an edge to a kinematic body at rest is
+ * ignored like an edge to body 0.  A pair of colliders on two non-dynamic bodies (kinematic or body 0), at least one of them kinematic, is not
+ * a broadphase pair (not counted, no islands, contacts, cache or events), two colliders of one kinematic body included; sensor pairs keep
+ * their rules.  The solver substitutes a kinematic side like body 0: no chain, never waited for, excluded from the throughput mass split.
+ * nb_upload_bodies keeps the set while the body count is unchanged and removes it when the count changes.  nb_save_state writes it (state
+ * version 4), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).  No extra launch per step. */
+typedef struct { uint32_t body; float velocity[3]; float angular_velocity[3]; uint32_t reserved; } nb_kinematic_body;   /* 32 bytes */
+int nb_upload_kinematic_bodies(nb_context*, const nb_kinematic_body* host, uint32_t n, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

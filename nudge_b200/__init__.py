@@ -23,7 +23,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
            "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
-           "nb_upload_sensors", "nb_download_sensor_overlaps"]
+           "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies"]
 
 
 class Config(C.Structure):
@@ -101,6 +101,7 @@ def load_library():
         lib.nb_upload_collision_filters.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
         lib.nb_upload_sensors.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
         lib.nb_download_sensor_overlaps.argtypes = [V, V, C.c_uint32, V, V]
+        lib.nb_upload_kinematic_bodies.argtypes = [V, V, C.c_uint32, V]
         _lib = lib
     return _lib
 
@@ -290,6 +291,8 @@ class Sim(abi.HostState):
             self.upload_collision_filters(s.collision_filters, s.filter_flags)
         if getattr(s, "sensors", None) is not None:
             self.upload_sensors(s.sensors)
+        if getattr(s, "kinematic", None) is not None:
+            self.upload_kinematic_bodies(s.kinematic)
 
     def upload_bodies(self):
         self._ck(self.lib.nb_upload_bodies(self.ctx, C.byref(self.bodies), self.stream), "nb_upload_bodies")
@@ -404,6 +407,14 @@ class Sim(abi.HostState):
             r = self.lib.nb_download_sensor_overlaps(self.ctx, abi.ptr(out), len(out), C.byref(n), self.stream)
         self._ck(r, "nb_download_sensor_overlaps")
         return out[:n.value].copy()
+
+    # ---- kinematic bodies (nb_upload_kinematic_bodies, include/nudge_b200.h): driven at a set velocity, never pushed back ----
+    def upload_kinematic_bodies(self, rows):
+        """rows: scenes.KINEMATIC rows (or anything np.asarray turns into them, e.g. tuples (body, velocity, angular_velocity, 0)), or
+        None / empty to remove the set.  Replaces the set and writes each body's velocity and angular velocity into its momentum row on the
+        device; call it every step with the same bodies and new velocities to drive them."""
+        k = np.ascontiguousarray(np.asarray(rows if rows is not None else [], scenes.KINEMATIC).reshape(-1))
+        self._ck(self.lib.nb_upload_kinematic_bodies(self.ctx, abi.ptr(k) if len(k) else None, len(k), self.stream), "nb_upload_kinematic_bodies")
 
     # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
     def enable_contact_events(self, capacity):

@@ -18,7 +18,7 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 
 // A sub-step as a CUDA graph (nb_step, nb_shard_step; run_graphed): captured once per key and replayed while the key holds.  Every
 // count the kernels need lives in device memory, so the graph only depends on the parameters and the scene shape held in the key.
-struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version, sensor_version; };
+struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version, sensor_version, kinematic_version; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
 struct nb_context {
@@ -59,6 +59,9 @@ struct nb_context {
 	// large enough.
 	uint8_t* sensor; bool has_sensor; u32 sensor_cap, sensor_alloc; u64* sensor_keys; SortBuffers sensor_sb; uint4* sensor_cur; uint4* sensor_old;
 	unsigned long long sensor_version;
+	// kinematic bodies (nb_upload_kinematic_bodies, DESIGN.md section 8.8): kind[body] as in nb_collide.cuh (bit 0 kinematic, bit 1 moving),
+	// allocated for max_bodies on the first upload of a set; kin_list = the set (host copy, ascending); kin_rows = the scatter's staging rows
+	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; nb_kinematic_body* kin_rows; u32 kin_rows_cap; unsigned long long kinematic_version;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -157,6 +160,22 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 }
 #define JOIN_UPLOADS() do { int r_ = join_uploads(ctx, (cudaStream_t)stream); if (r_) return r_; } while (0)
 
+// The kinematic table as the kernels take it: null without a set, so that they load nothing extra.
+static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
+static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->kinematic_version; } }
+
+// The velocity scatter of nb_upload_kinematic_bodies: each listed body's velocity and angular velocity into its momentum row (the unused lanes
+// are left alone), and its kind byte (the caller clears the table first when the set changes).
+__global__ void __launch_bounds__(NB_BLOCK) k_kinematic_scatter(const nb_kinematic_body* rows, u32 n, nb_body_momentum* momentum, uint8_t* kind) {
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const nb_kinematic_body r = rows[i];
+		nb_body_momentum& m = momentum[r.body];
+		m.velocity[0] = r.velocity[0]; m.velocity[1] = r.velocity[1]; m.velocity[2] = r.velocity[2];
+		m.angular_velocity[0] = r.angular_velocity[0]; m.angular_velocity[1] = r.angular_velocity[1]; m.angular_velocity[2] = r.angular_velocity[2];
+		if (!kind[r.body]) kind[r.body] = 1;   // a new member; an old one keeps its moving bit until the next k_uf_init
+	}
+}
+
 // Runs one sub-step `body()` through the graph slot `g`: on a capturable stream its launches are recorded once per key into a CUDA
 // graph and replayed afterwards.  The grid-synchronising kernels (k_sort_coop's software grid barriers, k_solve's and
 // k_solve_flow's spin waits) are captured as cooperative nodes, so the driver guarantees their co-residency at replay, also next to
@@ -171,7 +190,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	key.stream = st; key.ts = time_step; key.gravity = gravity; key.damping = damping; key.iterations = iterations;
 	key.B = ctx->B; key.nboxes = ctx->nboxes; key.nspheres = ctx->nspheres; key.nconn = ctx->nconn; key.tagbits = ctx->tagbits; key.kbits = ctx->kbits;
 	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version; key.events_version = ctx->events_version;
-	key.filter_version = ctx->filter_version; key.sensor_version = ctx->sensor_version;
+	key.filter_version = ctx->filter_version; key.sensor_version = ctx->sensor_version; key.kinematic_version = ctx->kinematic_version;
 	if (!g.exec || memcmp(&key, &g.key, sizeof(key)) != 0) {
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -394,6 +413,7 @@ int nb_create(const nb_config* config, nb_context** out) {
 
 	int per_sm = 0;
 	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve, NB_BLOCK, 0));
+	{ int per_kin = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_kin, k_solve_kin, NB_BLOCK, 0)); per_sm = std::min(per_sm, per_kin); }
 	if (per_sm < 1) { ctx->error = "k_solve does not fit on an SM"; return NB_ERR_CUDA; }
 	ctx->coop_blocks_solve = ctx->sms * per_sm;  // all co-resident: the dataflow solver relies on it
 	CK(cudaDeviceSynchronize());
@@ -409,6 +429,7 @@ void nb_destroy(nb_context* ctx) {
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
 	if (ctx->events) cudaFree(ctx->events);
 	free_sensor_lists(ctx);
+	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
 	delete ctx;
 }
 
@@ -422,6 +443,7 @@ int nb_lut_model_exact(const nb_context* ctx) { return ctx->lut_exact; }
 int nb_upload_bodies(nb_context* ctx, const nb_body_data* h, void* stream) {
 	NB_RANGE("nb_upload_bodies");
 	if (h->count > ctx->cfg.max_bodies) { ctx->error = "too many bodies"; return NB_ERR_CAPACITY; }
+	if (h->count != ctx->B) drop_kinematic(ctx);   // the kinematic set belongs to a body count
 	ctx->B = h->count;
 	cudaStream_t st = (cudaStream_t)stream;
 	H2D(ctx->xf, h->transforms, h->count, nb_transform); H2D(ctx->idle, h->idle_counters, h->count, uint8_t);   // all the collision stage reads
@@ -485,6 +507,38 @@ int nb_upload_sensors(nb_context* ctx, const uint8_t* h, uint32_t n, uint32_t ma
 	if (n != 0 && n != K) { ctx->error = "sensor table count must be 0 or boxes + spheres (" + std::to_string(K) + ")"; return NB_ERR_ARGUMENT; }
 	if (n && !h) { ctx->error = "null sensor table"; return NB_ERR_ARGUMENT; }
 	return set_sensors(ctx, h, n, max_sensor_pairs, (cudaStream_t)stream);
+}
+int nb_upload_kinematic_bodies(nb_context* ctx, const nb_kinematic_body* h, uint32_t n, void* stream) {
+	NB_RANGE("nb_upload_kinematic_bodies");
+	if (n && !h) { ctx->error = "null kinematic body table"; return NB_ERR_ARGUMENT; }
+	std::vector<u32> list(n);
+	for (u32 i = 0; i < n; ++i) {
+		const u32 b = h[i].body;
+		if (b == 0) { ctx->error = "body 0 is the static world and cannot be kinematic"; return NB_ERR_ARGUMENT; }
+		if (b >= ctx->B) { ctx->error = "kinematic body " + std::to_string(b) + " is at or beyond the body count (" + std::to_string(ctx->B) + ")"; return NB_ERR_ARGUMENT; }
+		list[i] = b;
+	}
+	std::sort(list.begin(), list.end());
+	if (std::adjacent_find(list.begin(), list.end()) != list.end()) { ctx->error = "a kinematic body is listed twice"; return NB_ERR_ARGUMENT; }
+	cudaStream_t st = (cudaStream_t)stream;
+	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
+	if (!n) { drop_kinematic(ctx); return NB_OK; }
+	if (!ctx->kind) ALLOC(ctx->kind, ctx->cfg.max_bodies);
+	if (n > ctx->kin_rows_cap) {
+		CK(cudaStreamSynchronize(st));   // the old staging rows may still be read by an earlier scatter
+		if (ctx->kin_rows) cudaFree(ctx->kin_rows);
+		ctx->kin_rows = nullptr; ctx->kin_rows_cap = 0;
+		CK(cudaMalloc(&ctx->kin_rows, sizeof(nb_kinematic_body) * (size_t)n));
+		ctx->kin_rows_cap = n;
+	}
+	const bool same = ctx->has_kin && list == ctx->kin_list;
+	if (!same) CK(cudaMemsetAsync(ctx->kind, 0, ctx->cfg.max_bodies, st));
+	CK(cudaMemcpyAsync(ctx->kin_rows, h, sizeof(nb_kinematic_body) * (size_t)n, cudaMemcpyHostToDevice, st));
+	k_kinematic_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->kin_rows, n, ctx->mom, ctx->kind);
+	++ctx->launches;
+	CK(cudaGetLastError());
+	if (!same) { ctx->has_kin = true; ctx->kin_list.swap(list); ++ctx->kinematic_version; }   // nb_step's graph re-records with the table
+	return NB_OK;
 }
 int nb_upload_cache(nb_context* ctx, const nb_contact_cache* h, void* stream) {
 	if (h->count > ctx->cfg.max_contacts) { ctx->error = "cache too large"; return NB_ERR_CAPACITY; }
@@ -594,10 +648,12 @@ int nb_collide(nb_context* ctx, void* stream) {
 	cudaStream_t st = L.stream;
 	const u32 K = ctx->nboxes + ctx->nspheres, B = ctx->B, nboxes = ctx->nboxes;
 	u32* counts = ctx->counts;
+	uint8_t* kind = ctx->has_kin ? ctx->kind : nullptr;
+	if (kind) JOIN_UPLOADS();   // k_uf_init reads the kinematic bodies' momentum rows
 	k_reset_collide<<<1, 32, 0, st>>>(counts, K, ctx->keybits); ++ctx->launches;
 	if (K == 0 || B == 0) return NB_OK;
 	k_collider_world<<<GRID(K), NB_BLOCK, 0, st>>>(ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
-		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
+		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, kind, ctx->has_sensor ? ctx->sensor : nullptr, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
 	k_morton<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->aabb_min, ctx->aabb_max, counts, ctx->sb.keys[0], ctx->sb.vals[0], ctx->keybits);
 	ctx->launches += 2;
 	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
@@ -607,7 +663,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
 	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
 	const uint8_t* sensor = ctx->has_sensor ? ctx->sensor : nullptr;   // null: the kernels never touch the sensor list
-	k_grid_pairs<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
+	(kind ? k_grid_pairs<true> : k_grid_pairs<false>)<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
 		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
 		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
@@ -619,11 +675,11 @@ int nb_collide(nb_context* ctx, void* stream) {
 
 	// coarse islands (nudge.cpp:3500-3703)
 	const u32 P = ctx->cfg.max_pairs, S = ctx->stride;
-	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, B); ++ctx->launches;
-	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, ctx->conn, ctx->nconn); ++ctx->launches; }
-	k_uf_union_pairs<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, ctx->pair_keys, ctx->kbits, ctx->col_body, counts);
-	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, B);
-	k_pair_flags<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->kbits, nboxes, ctx->col_body, ctx->parent, ctx->active, ctx->flags, S, counts);
+	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B); ++ctx->launches;
+	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn); ++ctx->launches; }
+	k_uf_union_pairs<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->pair_keys, ctx->kbits, ctx->col_body, counts);
+	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
+	k_pair_flags<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->kbits, nboxes, ctx->col_body, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
 	ctx->launches += 3;
 	nb_scan_reduce<5>(L, ctx->flags, S, counts + CNT_PAIRS, 0, ctx->block_sums, counts + CNT_LIVE0);  // -> LIVE0..3, SLEEP_COARSE
 	k_partition<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->kbits, ctx->flags, ctx->block_sums, S, ctx->col_tag, ctx->live, ctx->sleeping, counts);
@@ -644,15 +700,15 @@ int nb_collide(nb_context* ctx, void* stream) {
 
 	// fine islands, active bodies, contact compaction (nudge.cpp:3788-4006)
 	const u32 C = ctx->cfg.max_contacts;
-	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, B); ++ctx->launches;
-	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, ctx->conn, ctx->nconn); ++ctx->launches; }
-	k_uf_union_contacts<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, ctx->staged.bodies, counts);
-	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, B);
+	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B); ++ctx->launches;
+	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn); ++ctx->launches; }
+	k_uf_union_contacts<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->staged.bodies, counts);
+	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
 	k_body_flags<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->flags, B);
 	ctx->launches += 3;
 	nb_scan_reduce<1>(L, ctx->flags, S, nullptr, B, ctx->block_sums, counts + CNT_ACTIVE);
 	k_active_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->active_idx, B);
-	k_contact_flags<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->staged.bodies, ctx->staged.tags, ctx->parent, ctx->active, ctx->flags, S, counts);
+	k_contact_flags<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->staged.bodies, ctx->staged.tags, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
 	ctx->launches += 2;
 	nb_scan_reduce<2>(L, ctx->flags, S, counts + CNT_STAGED, 0, ctx->block_sums, counts + CNT_CONTACTS);  // -> CONTACTS, SLEEP_FINE
 	k_contact_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->staged, ctx->fin, ctx->flags, ctx->block_sums, S, ctx->sleeping, counts);
@@ -671,7 +727,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_apply_gravity_damping");
 	JOIN_UPLOADS();   // first reader of the momentum rows in a step
-	k_gravity_damping<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, ctx->mom, time_step, gravity, damping, ctx->counts);
+	k_gravity_damping<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->mom, time_step, gravity, damping, ctx->counts);
 	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -828,7 +884,7 @@ static int launch_solve(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) 
 	u32 backoff = NB_SOLVE_BACKOFF_NS;
 	void* args[] = { &R, &impulses, &mw, &mode, &sweeps, &backoff, &counts };
 	if (mode) timing_begin(ctx, st);
-	CK(cudaLaunchCooperativeKernel((void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
+	CK(cudaLaunchCooperativeKernel(ctx->has_kin ? (void*)k_solve_kin : (void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
 	if (mode) timing_end(ctx, st);
 	k_mw_out<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, mode ? 1 : 0);
 	ctx->launches += 3;
@@ -842,13 +898,14 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	cudaStream_t st = L.stream;
 	u32* counts = ctx->counts;
 	const u32 C = ctx->cfg.max_contacts, S = ctx->stride, B = ctx->B;
-	k_inertia<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->xf, ctx->props, ctx->inertia, ctx->mom);
+	const uint8_t* kind = kin_table(ctx);
+	k_inertia<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->xf, ctx->props, kind, ctx->inertia, ctx->mom);
 	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) {
 		// no batch schedule, no per-body chains: slots in tag order, per-body contact counts for the mass split, split rows
 		CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
 		CK(cudaMemsetAsync(ctx->jcnt, 0, sizeof(u32) * B, st));
-		k_jacobi_prepare<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->jcnt, ctx->rows, ctx->cstride, counts);
-		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, ctx->rows, counts, ctx->jcnt);
+		k_jacobi_prepare<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->jcnt, ctx->rows, ctx->cstride, counts);
+		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, ctx->jcnt);
 		ctx->launches += 3;
 		if (!ctx->defer_warm_start) {
 			int r = launch_solve(ctx, 0, 1, st); if (r) return r; if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
@@ -856,7 +913,7 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 		CK(cudaGetLastError());
 		return NB_OK;
 	}
-	k_sched_prep<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->cab, ctx->back, ctx->sched_empty, counts);
+	k_sched_prep<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->cab, ctx->back, ctx->sched_empty, counts);
 	// the scheduler replay in segments (nb_solver.cuh above k_schedule, DESIGN §2.7): speculative runs, the joins of every segment
 	// from every run of the previous one, then per bucket the chain of picked runs (or the sequential replay if it broke), and the
 	// merge of the picked joins and runs
@@ -873,11 +930,11 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
 	CK(cudaMemsetAsync(ctx->chain_len, 0, sizeof(u32) * B, st));
 	k_batch_index<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
-		ctx->offs, ctx->left_count, ctx->batch_of, ctx->slot_idx, ctx->rows.contact, ctx->cstride, ctx->chain_len, counts);
+		ctx->offs, ctx->left_count, kind, ctx->batch_of, ctx->slot_idx, ctx->rows.contact, ctx->cstride, ctx->chain_len, counts);
 	k_chain_alloc<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->chain_len, ctx->chain_start, counts);
-	k_chain_scatter<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->batch_of, ctx->chain_start, ctx->sb.keys[0], counts);
-	k_chain_rank<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->batch_of, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->sb.keys[0], ctx->rows.wait, ctx->cstride, counts);
-	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, ctx->rows, counts, nullptr);
+	k_chain_scatter<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->chain_start, ctx->sb.keys[0], counts);
+	k_chain_rank<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->sb.keys[0], ctx->rows.wait, ctx->cstride, counts);
+	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, nullptr);
 	ctx->launches += 5;
 	if (!ctx->defer_warm_start) {  // warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
 		int r = launch_solve(ctx, 0, 1, st); if (r) return r;
@@ -1007,6 +1064,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "inertia", ctx->inertia, sizeof(float4) * 2 * ctx->B },
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
+		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
 		{ "sensor_pairs", ctx->sensor_keys, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }

@@ -49,11 +49,28 @@ __global__ void __launch_bounds__(NB_BLOCK) k_conn_keys(const nb_body_pair* conn
 	}
 }
 
+// ---------------- kinematic bodies (nb_upload_kinematic_bodies, DESIGN.md section 8.8) ----------------
+// kind[body]: 0 = dynamic; bit 0 = kinematic (set by the upload); bit 1 = moving (any nonzero velocity component, rewritten by every
+// k_uf_init from the momentum row as it stands at nb_collide).  Kernels take the table as a pointer that is null without a set.
+NB_DEV bool kin_is(const uint8_t* kind, u32 body) { return kind && kind[body]; }
+NB_DEV u32 solver_body(const uint8_t* kind, u32 body) { return kin_is(kind, body) ? 0u : body; }   // the solver treats a kinematic side as body 0
+// Broadphase class of a collider's body, carried as the magnitude of leaf_min.w (whose sign is the size class, k_grid_build): dynamic =
+// infinity (also body 0 without a kinematic set, and every sensor collider, whose pairs keep their own rules), body 0 = 8, kinematic = 1.
+// A pair is rejected iff the magnitudes sum to less than 10: kinematic + body 0 (9) or kinematic + kinematic (2), never body 0 + body 0
+// (16) or anything with a dynamic body or a sensor (infinity).  One add and one compare of values the broadphase already holds, so a scene
+// without a set loads nothing more.
+#define NB_KIN_WORLD 8.0f
+#define NB_KIN_KINEMATIC 1.0f
+NB_DEV float kin_class(u32 body, const uint8_t* kind) { return body == 0 ? NB_KIN_WORLD : (kind[body] ? NB_KIN_KINEMATIC : 0.0f); }
+NB_DEV bool kin_reject(float wa, float wb) { return fabsf(wa) + fabsf(wb) < 10.0f; }
+
 // ---------------- K1: collider world transform + AABB (nudge.cpp:3021-3079) ----------------
 // filter: one word per collider (category | mask << 16) or null; it goes to aabb_max[i].w, which no geometry reads.
+// kind: the kinematic table (nb_upload_kinematic_bodies) or null; with a table aabb_min[i].w gets the body's broadphase class
+// (kin_class above; 0 = dynamic, also for a sensor collider), without one it stays 0.
 __global__ void __launch_bounds__(NB_BLOCK) k_collider_world(u32 nboxes, u32 nspheres, const nb_transform* body_xf,
 		const nb_transform* box_xf, const nb_box_collider* box_data, const u32* box_tags,
-		const nb_transform* sph_xf, const nb_sphere_collider* sph_data, const u32* sph_tags, const u32* filter,
+		const nb_transform* sph_xf, const nb_sphere_collider* sph_data, const u32* sph_tags, const u32* filter, const uint8_t* kind, const uint8_t* sensor,
 		nb_transform* world_xf, float4* aabb_min, float4* aabb_max, u32* col_tag, u32* col_body, u32* counts) {
 	u32 K = nboxes + nspheres;
 	float mn[3] = { INFINITY, INFINITY, INFINITY }, mx[3] = { -INFINITY, -INFINITY, -INFINITY };
@@ -79,7 +96,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_collider_world(u32 nboxes, u32 nsp
 			float r = sph_data[i - nboxes].radius;
 			ext = mk3(r, r, r);
 		}
-		float4 lo = make_float4(p.x - ext.x, p.y - ext.y, p.z - ext.z, 0.0f);
+		float4 lo = make_float4(p.x - ext.x, p.y - ext.y, p.z - ext.z, kind && !(sensor && sensor[i]) ? kin_class(body, kind) : 0.0f);
 		float4 hi = make_float4(p.x + ext.x, p.y + ext.y, p.z + ext.z, asf(filter ? filter[i] : NB_FILTER_ALL));
 		st_xform(world_xf, i, w);
 		aabb_min[i] = lo; aabb_max[i] = hi;
@@ -233,7 +250,8 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_build(u32 K, const u32* order
 		u32 qx, qy, qz; morton_quantise(f, lo, order[p], qx, qy, qz);
 		bool small = grid_level_needed(lo, hi, f.L[0]) <= j && qx < 65536u && qy < 65536u && qz < 65536u;  // NaN extents are "large" too
 		smallf[p] = small ? 1 : 0;
-		lo.w = small ? -INFINITY : INFINITY; leaf_min[p] = lo;  // k_grid_pairs reads the class with the box: 0 > lo.w <=> small
+		const float cls = lo.w != 0.0f ? lo.w : INFINITY;   // kinematic class (k_collider_world), infinity without a kinematic set
+		lo.w = small ? -cls : cls; leaf_min[p] = lo;  // k_grid_pairs reads the class with the box: 0 > lo.w <=> small
 		if (!small) large_list[atomicAdd(&counts[CNT_LARGE], 1u)] = p;
 		const u64 prefix = mkeys[p] >> (3 * j);
 		if (p == 0 || (mkeys[p - 1] >> (3 * j)) != prefix) {  // first collider of its cell: publish the cell's range
@@ -272,6 +290,8 @@ NB_DEV void emit_sensor(u64 key, u64* sensor_keys, u32 max_sensor_pairs, u32* co
 // Hits go to a per-warp shared buffer (shared-memory atomic for the slot) that is flushed to the pair list with one global
 // atomic per ~64 pairs: one global atomic per pair would serialise on the counter.
 #define NB_GP_BUF 128
+// KIN: a kinematic set exists and the pair test includes kin_reject; without one the classes are all infinite and the test is left out.
+template<bool KIN>
 __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order, const float4* leaf_min, const float4* leaf_max, const uint8_t* smallf, const u64* mkeys,
 		const u64* table_keys, const u64* table_vals, u32 table_mask, u32 kbits, const u32* col_body, const u64* conn_keys, u32 conn_n,
 		const uint8_t* sensor, u64* sensor_keys, u32 max_sensor_pairs, u64* pair_keys, u32 max_pairs, u32* counts) {
@@ -339,7 +359,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_grid_pairs(u32 K, const u32* order
 			bool hit = false;
 			if (t < total) {
 				const float4 a = __ldg(leaf_min + q), bq = __ldg(leaf_max + q);  // two 128-bit loads; a.w carries the class, bq.w the filter word
-				hit = (bq.x > lo.x) & (hi.x > a.x) & (bq.y > lo.y) & (hi.y > a.y) & (bq.z > lo.z) & (hi.z > a.z) & (0.0f > a.w)  // strict, nudge.cpp:3306-3310
+				// strict, nudge.cpp:3306-3310; the candidate is small (0 > a.w) and the pair is not rejected as two non-dynamic bodies, one of
+				// them kinematic (kin_reject for two negative classes: without a kinematic set both are -infinity)
+				hit = (bq.x > lo.x) & (hi.x > a.x) & (bq.y > lo.y) & (hi.y > a.y) & (bq.z > lo.z) & (hi.z > a.z) & (0.0f > a.w) & (!KIN || lo.w + a.w <= -10.0f)
 					& filter_pass(fp, asu(bq.w));
 			}
 			u32 oq = 0;
@@ -383,8 +405,8 @@ __global__ void __launch_bounds__(NB_BLOCK) k_large_pairs(u32 K, const u32* orde
 		const float4 lo = leaf_min[pl], hi = leaf_max[pl];
 		for (u32 q = blockIdx.x * blockDim.x + threadIdx.x; q < K; q += gridDim.x * blockDim.x) {
 			if (q == pl || (!smallf[q] && q < pl)) continue;  // a pair of two large colliders is reported from the earlier one
-			const float4 bq = leaf_max[q];
-			if (boxes_overlap(lo, hi, leaf_min[q], bq) && filter_pass(asu(hi.w), asu(bq.w))
+			const float4 aq = leaf_min[q], bq = leaf_max[q];
+			if (boxes_overlap(lo, hi, aq, bq) && !kin_reject(lo.w, aq.w) && filter_pass(asu(hi.w), asu(bq.w))
 				&& !(conn_n && connected(conn_keys, conn_n, col_body[order[pl]], col_body[order[q]]))) {
 				const u32 p0 = min(pl, q), p1 = max(pl, q);
 				const u32 s = sensor ? (u32)sensor[order[p0]] | (u32)sensor[order[p1]] << 1 : 0u;
@@ -428,42 +450,63 @@ NB_DEV void uf_unite(u32* parent, u32 a, u32 b) {
 // asleep and an awake body "taints" the asleep one (its whole asleep component is then active), and edges between awake bodies
 // carry no information.  The resulting active/inactive decision per body is exactly the reference's, at almost no cost while the
 // scene is moving.  active[] is indexed by the root of a body's asleep-component (an awake body is its own root).
-NB_DEV void island_edge(u32* parent, u32* taint, const uint8_t* idle, u32 a, u32 b) {
+// Kinematic bodies (kind non-null): a kinematic body never joins a set; an edge to a moving one makes the dynamic side's set active (the
+// taint), an edge to one at rest is ignored like an edge to body 0.
+NB_DEV void island_edge(u32* parent, u32* taint, const uint8_t* idle, const uint8_t* kind, u32 a, u32 b) {
 	if (!a || !b || a == b) return;  // body 0 is the static world and is ignored (nudge.cpp:3517-3519, 3583-3585)
+	if (kind) {
+		const u32 ka = kind[a], kb = kind[b];
+		if (ka | kb) {
+			const u32 d = ka ? b : a;
+			if (!(ka && kb) && ((ka | kb) & 2u) && idle[d] == 0xff) taint[d] = 1;
+			return;
+		}
+	}
 	const bool sa = idle[a] == 0xff, sb = idle[b] == 0xff;
 	if (sa && sb) uf_unite(parent, a, b);
 	else if (sa) taint[a] = 1;
 	else if (sb) taint[b] = 1;
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_uf_init(u32* parent, u32* active, u32* taint, u32 B) {
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) { parent[i] = i; active[i] = 0; taint[i] = 0; }
+// With a kinematic set it also derives the step's kind of every kinematic body: moving iff a velocity component is nonzero (-0.0 is zero).
+__global__ void __launch_bounds__(NB_BLOCK) k_uf_init(u32* parent, u32* active, u32* taint, uint8_t* kind, const nb_body_momentum* momentum, u32 B) {
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
+		parent[i] = i; active[i] = 0; taint[i] = 0;
+		if (kind && kind[i]) {
+			const float4* m = reinterpret_cast<const float4*>(momentum + i);
+			const float4 l = m[0], w = m[1];
+			const bool moving = l.x != 0.0f || l.y != 0.0f || l.z != 0.0f || w.x != 0.0f || w.y != 0.0f || w.z != 0.0f;
+			kind[i] = moving ? 3 : 1;
+		}
+	}
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_conn(u32* parent, u32* taint, const uint8_t* idle, const nb_body_pair* conn, u32 n) {
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) island_edge(parent, taint, idle, conn[i].a, conn[i].b);
+__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_conn(u32* parent, u32* taint, const uint8_t* idle, const uint8_t* kind, const nb_body_pair* conn, u32 n) {
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) island_edge(parent, taint, idle, kind, conn[i].a, conn[i].b);
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_pairs(u32* parent, u32* taint, const uint8_t* idle, const u64* pair_keys, u32 kbits, const u32* col_body, const u32* counts) {
+__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_pairs(u32* parent, u32* taint, const uint8_t* idle, const uint8_t* kind, const u64* pair_keys, u32 kbits, const u32* col_body, const u32* counts) {
 	u32 n = counts[CNT_PAIRS];
 	u64 mask = ((u64)1 << kbits) - 1;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		u64 k = pair_keys[i];
-		island_edge(parent, taint, idle, col_body[(u32)(k & mask)], col_body[(u32)(k >> kbits)]);
+		island_edge(parent, taint, idle, kind, col_body[(u32)(k & mask)], col_body[(u32)(k >> kbits)]);
 	}
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_contacts(u32* parent, u32* taint, const uint8_t* idle, const uint2* bodies, const u32* counts) {
+__global__ void __launch_bounds__(NB_BLOCK) k_uf_union_contacts(u32* parent, u32* taint, const uint8_t* idle, const uint8_t* kind, const uint2* bodies, const u32* counts) {
 	u32 n = counts[CNT_STAGED];
-	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) { uint2 ab = bodies[i]; island_edge(parent, taint, idle, ab.x, ab.y); }
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) { uint2 ab = bodies[i]; island_edge(parent, taint, idle, kind, ab.x, ab.y); }
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_uf_flatten_active(u32* parent, u32* active, const u32* taint, const uint8_t* idle, u32 B) {
+// A kinematic body is its own set, active iff it is moving; its idle counter is never consulted.
+__global__ void __launch_bounds__(NB_BLOCK) k_uf_flatten_active(u32* parent, u32* active, const u32* taint, const uint8_t* idle, const uint8_t* kind, u32 B) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
 		u32 r = uf_find_fresh(parent, i);
 		parent[i] = r;  // roots never change here, so concurrent flattening is benign
-		if (i >= 1 && (idle[i] != 0xff || taint[i])) active[r] = 1;  // nudge.cpp:3669-3672
+		const u32 k = kind ? kind[i] : 0u;
+		if (i >= 1 && (k ? (k & 2u) != 0 : (idle[i] != 0xff || taint[i]))) active[r] = 1;  // nudge.cpp:3669-3672
 	}
 }
 
 // ---------------- coarse island filter + partition by shape type (nudge.cpp:3674-3751) ----------------
 __global__ void __launch_bounds__(NB_BLOCK) k_pair_flags(const u64* pair_keys, u32 kbits, u32 nboxes, const u32* col_body, const u32* parent, const u32* active,
-														 u32* flags /*[5][stride]*/, u32 stride, const u32* counts) {
+														 const uint8_t* kind, u32* flags /*[5][stride]*/, u32 stride, const u32* counts) {
 	u32 n = counts[CNT_PAIRS];
 	u64 mask = ((u64)1 << kbits) - 1;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -472,7 +515,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_pair_flags(const u64* pair_keys, u
 		u32 a = col_body[lo], b = col_body[hi];
 		int cls = -1;
 		if (a != b) {
-			u32 set = a ? parent[a] : parent[b];  // sets[0] = 0 and both bodies share a set (nudge.cpp:3663, 3688)
+			u32 set = solver_body(kind, a) ? parent[a] : parent[b];  // sets[0] = 0 and both bodies share a set (nudge.cpp:3663, 3688); the dynamic side of a kinematic pair
 			cls = active[set] ? (int)((lo >= nboxes ? 1u : 0u) | (hi >= nboxes ? 2u : 0u)) : 4;
 		}
 		#pragma unroll
@@ -1022,13 +1065,13 @@ __global__ void __launch_bounds__(NB_BLOCK) k_body_flags(const u32* parent, cons
 __global__ void __launch_bounds__(NB_BLOCK) k_active_scatter(const u32* flags, const u32* block_sums, u32* active_idx, u32 B) {  // NB_SCAN_GRID blocks
 	scan_consume<1>(flags, 0, B, block_sums, [&](u32 i, const u32 (&v)[1], const u32 (&off)[1]) { if (v[0]) active_idx[off[0]] = i; });
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_contact_flags(const uint2* bodies, const u64* tags, const u32* parent, const u32* active, u32* flags, u32 stride, const u32* counts) {
+__global__ void __launch_bounds__(NB_BLOCK) k_contact_flags(const uint2* bodies, const u64* tags, const u32* parent, const u32* active, const uint8_t* kind, u32* flags, u32 stride, const u32* counts) {
 	u32 n = counts[CNT_STAGED];
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		uint2 ab = bodies[i];
 		// The reference decides per span of equal pair tags from the span's first contact (nudge.cpp:3976-3999);
 		// every contact of a span has the same bodies, so the per-contact decision is the same.
-		u32 set = ab.x ? parent[ab.x] : parent[ab.y];
+		u32 set = solver_body(kind, ab.x) ? parent[ab.x] : parent[ab.y];
 		bool keep = active[set] != 0;
 		flags[i] = keep ? 1u : 0u;
 		flags[stride + i] = (!keep && (i == 0 || tags[i - 1] != tags[i])) ? 1u : 0u;

@@ -62,14 +62,14 @@ NB_DEV void red_add_v4(float4* p, float x, float y, float z) {
 	asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" :: "l"(p), "f"(x), "f"(y), "f"(z), "f"(0.0f) : "memory");
 }
 
-// tag order: slot i = contact sorted[i]; per-body contact counts for the mass split (body 0 is static and never split)
-__global__ void __launch_bounds__(NB_BLOCK) k_jacobi_prepare(const u32* sorted, const uint2* bodies, u32* cnt, Rows R, u32 max_slots, u32* counts) {
+// tag order: slot i = contact sorted[i]; per-body contact counts for the mass split (body 0 and kinematic bodies are never split)
+__global__ void __launch_bounds__(NB_BLOCK) k_jacobi_prepare(const u32* sorted, const uint2* bodies, const uint8_t* kind, u32* cnt, Rows R, u32 max_slots, u32* counts) {
 	u32 n = counts[CNT_CONTACTS];
 	if (n > max_slots) n = max_slots;
 	if (blockIdx.x == 0 && threadIdx.x == 0) { counts[CNT_BATCHES] = (n + 7) / 8; counts[CNT_FULL_BATCHES] = n / 8; counts[CNT_ENTRIES] = 0; }
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		u32 c = sorted[i];
-		uint2 ab = bodies[c];
+		uint2 ab = solver_pair(kind, bodies[c]);
 		R.contact[i] = c;
 		if (ab.x) atomicAdd(&cnt[ab.x], 1u);
 		if (ab.y) atomicAdd(&cnt[ab.y], 1u);
@@ -141,7 +141,8 @@ __global__ void __launch_bounds__(NJ_TILE, 4 - STAGES) k_jacobi_sweep(Rows R, co
 		const u32 slot = tile * NJ_TILE + threadIdx.x;
 		const bool valid = slot < n;
 		const float* T = &sm.tile[stage][0][threadIdx.x];
-		const u32 a = valid ? asu(T[NJ_PLANE_A * NJ_TILE]) : 0u, b = valid ? asu(T[NJ_PLANE_B * NJ_TILE]) : 0u;
+		const u32 ra = valid ? asu(T[NJ_PLANE_A * NJ_TILE]) : 0u, rb = valid ? asu(T[NJ_PLANE_B * NJ_TILE]) : 0u;   // NB_READ_ONLY on a kinematic side
+		const u32 a = NB_BODY_INDEX(ra), b = NB_BODY_INDEX(rb);
 		float4 al = V[2*a], aw = V[2*a + 1], bl = V[2*b], bw = V[2*b + 1];      // body 0 for invalid lanes: zeros, harmless
 		float4 ci = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		if (WARM && valid) ci = impulses[R.contact[slot]];
@@ -166,8 +167,8 @@ __global__ void __launch_bounds__(NJ_TILE, 4 - STAGES) k_jacobi_sweep(Rows R, co
 		const bool head_a = lane == 0 || pa != a, head_b = lane == 0 || pb != b;
 		seg_reduce6(__ballot_sync(0xffffffffu, head_a), da);
 		seg_reduce6(__ballot_sync(0xffffffffu, head_b), db);
-		if (a && head_a) { red_add_v4(D + 2*a, da[0], da[1], da[2]); red_add_v4(D + 2*a + 1, da[3], da[4], da[5]); }
-		if (b && head_b) { red_add_v4(D + 2*b, db[0], db[1], db[2]); red_add_v4(D + 2*b + 1, db[3], db[4], db[5]); }
+		if ((int)ra > 0 && head_a) { red_add_v4(D + 2*a, da[0], da[1], da[2]); red_add_v4(D + 2*a + 1, da[3], da[4], da[5]); }   // neither body 0 nor kinematic
+		if ((int)rb > 0 && head_b) { red_add_v4(D + 2*b, db[0], db[1], db[2]); red_add_v4(D + 2*b + 1, db[3], db[4], db[5]); }
 	}
 }
 

@@ -20,14 +20,17 @@
 
 struct RowsDev { nb_constraint_row* rows; u32* level_off; u32 n, levels; };
 
-__global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows, u32 begin, u32 end, nb_body_momentum* momentum, const nb_body_properties* props, const float4* inertia, int warm) {
+// A kinematic side (kind non-null) is like body 0: infinite mass, its velocity read and never written.
+__global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows, u32 begin, u32 end, nb_body_momentum* momentum, const nb_body_properties* props, const float4* inertia,
+		const uint8_t* kind, int warm) {
 	for (u32 i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
 		nb_constraint_row r = rows[i];
 		const u32 a = r.a, b = r.b;
-		const float ma = a ? props[a].mass_inverse : 0.0f, mb = b ? props[b].mass_inverse : 0.0f;
+		const bool da = solver_body(kind, a) != 0, db = solver_body(kind, b) != 0;   // dynamic sides
+		const float ma = da ? props[a].mass_inverse : 0.0f, mb = db ? props[b].mass_inverse : 0.0f;
 		float4 Ad = inertia[2*a], Ao = inertia[2*a + 1], Bd = inertia[2*b], Bo = inertia[2*b + 1];   // (xx,yy,zz,-) (xy,xz,yz,-)
-		if (!a) { Ad = make_float4(0, 0, 0, 0); Ao = Ad; }
-		if (!b) { Bd = make_float4(0, 0, 0, 0); Bo = Bd; }
+		if (!da) { Ad = make_float4(0, 0, 0, 0); Ao = Ad; }
+		if (!db) { Bd = make_float4(0, 0, 0, 0); Bo = Bd; }
 		// I^-1 J_ang
 		const float iax = Ad.x*r.ang_a[0] + Ao.x*r.ang_a[1] + Ao.y*r.ang_a[2], iay = Ao.x*r.ang_a[0] + Ad.y*r.ang_a[1] + Ao.z*r.ang_a[2], iaz = Ao.y*r.ang_a[0] + Ao.z*r.ang_a[1] + Ad.z*r.ang_a[2];
 		const float ibx = Bd.x*r.ang_b[0] + Bo.x*r.ang_b[1] + Bo.y*r.ang_b[2], iby = Bo.x*r.ang_b[0] + Bd.y*r.ang_b[1] + Bo.z*r.ang_b[2], ibz = Bo.y*r.ang_b[0] + Bo.z*r.ang_b[1] + Bd.z*r.ang_b[2];
@@ -46,15 +49,15 @@ __global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows,
 			delta = next - r.impulse;
 			rows[i].impulse = next;
 		}
-		if (a) { al.x += ma * r.lin_a[0] * delta; al.y += ma * r.lin_a[1] * delta; al.z += ma * r.lin_a[2] * delta; aw.x += iax * delta; aw.y += iay * delta; aw.z += iaz * delta; pa[0] = al; pa[1] = aw; }
-		if (b) { bl.x += mb * r.lin_b[0] * delta; bl.y += mb * r.lin_b[1] * delta; bl.z += mb * r.lin_b[2] * delta; bw.x += ibx * delta; bw.y += iby * delta; bw.z += ibz * delta; pb[0] = bl; pb[1] = bw; }
+		if (da) { al.x += ma * r.lin_a[0] * delta; al.y += ma * r.lin_a[1] * delta; al.z += ma * r.lin_a[2] * delta; aw.x += iax * delta; aw.y += iay * delta; aw.z += iaz * delta; pa[0] = al; pa[1] = aw; }
+		if (db) { bl.x += mb * r.lin_b[0] * delta; bl.y += mb * r.lin_b[1] * delta; bl.z += mb * r.lin_b[2] * delta; bw.x += ibx * delta; bw.y += iby * delta; bw.z += ibz * delta; pb[0] = bl; pb[1] = bw; }
 	}
 }
 
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st) {
 	for (u32 l = 0; l < ctx->urow_levels; ++l) {
 		const u32 b = ctx->urow_level_off[l], e = ctx->urow_level_off[l + 1];
-		if (e > b) { k_user_rows<<<GRID(e - b), NB_BLOCK, 0, st>>>(ctx->urows, b, e, ctx->mom, ctx->props, ctx->inertia, warm); ++ctx->launches; }
+		if (e > b) { k_user_rows<<<GRID(e - b), NB_BLOCK, 0, st>>>(ctx->urows, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm); ++ctx->launches; }
 	}
 	CK(cudaGetLastError());
 	return NB_OK;

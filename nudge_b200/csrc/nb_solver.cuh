@@ -114,10 +114,12 @@ __global__ void __launch_bounds__(NB_BLOCK) k_cache_merge(const u32* sorted, con
 }
 
 // ---------------- per-body world inverse inertia (nudge.cpp:4182-4199) ----------------
-__global__ void __launch_bounds__(NB_BLOCK) k_inertia(u32 B, const nb_transform* xf, const nb_body_properties* props, float4* inertia, nb_body_momentum* momentum) {
+// A kinematic body (kind non-null and set) gets zero inverse mass and inertia whatever its properties row says.
+__global__ void __launch_bounds__(NB_BLOCK) k_inertia(u32 B, const nb_transform* xf, const nb_body_properties* props, const uint8_t* kind, float4* inertia, nb_body_momentum* momentum) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
 		float4 q = reinterpret_cast<const float4*>(xf + i)[1];
 		float4 pr = reinterpret_cast<const float4*>(props)[i];
+		if (kin_is(kind, i)) pr = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 		mat3 m = qmatrix(mkq(q));
 		float ix = pr.x, iy = pr.y, iz = pr.z;
 		float xx = ix*m.c0.x*m.c0.x + iy*m.c1.x*m.c1.x + iz*m.c2.x*m.c2.x;
@@ -148,21 +150,23 @@ __global__ void __launch_bounds__(NB_BLOCK) k_inertia(u32 B, const nb_transform*
 #define NB_SCHED_MAXV (NB_SCHED_REGPOS + NB_SCHED_SHARED - 1)   // positions held on chip; beyond that the list spills to global memory
 
 // Parallel pre-pass for the replay: the body pair of every contact in tag order with the body-0 substitution of
-// nudge.cpp:4238-4240 applied, and `back` = distance (in contacts of the same bucket, 1..7) to the nearest earlier contact of
+// nudge.cpp:4238-4240 applied (a kinematic side is body 0 here), and `back` = distance (in contacts of the same bucket, 1..7) to the nearest earlier contact of
 // the bucket that shares a body, 0 if there is none within 7.  A run of 8 consecutive bucket contacts starting at a fresh
 // slot is conflict free iff none of them has 0 < back <= its offset in the run.
-__global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, const uint2* bodies, uint2* cab, uint8_t* back, uint8_t* sempty, u32* counts) {
+// A kinematic side (kind non-null) is substituted exactly like body 0.
+NB_DEV uint2 solver_pair(const uint8_t* kind, uint2 ab) { return kind ? make_uint2(solver_body(kind, ab.x), solver_body(kind, ab.y)) : ab; }
+__global__ void __launch_bounds__(NB_BLOCK) k_sched_prep(const u32* sorted, const uint2* bodies, const uint8_t* kind, uint2* cab, uint8_t* back, uint8_t* sempty, u32* counts) {
 	u32 n = counts[CNT_CONTACTS];
 	if (blockIdx.x == 0 && threadIdx.x <= 16) counts[CNT_SCHED_FALLBACK + threadIdx.x] = 0;   // the fall-back counter and flags
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-		uint2 ab = bodies[sorted[i]];
+		uint2 ab = solver_pair(kind, bodies[sorted[i]]);
 		u32 ca = ab.x ? ab.x : ab.y, cb = ab.y ? ab.y : ab.x;
 		cab[i] = make_uint2(ca, cb);
 		u32 b = 0;
 		#pragma unroll
 		for (u32 k = 1; k <= 7; ++k) {
 			if (!b && i >= 16 * k) {
-				uint2 o = bodies[sorted[i - 16 * k]];
+				uint2 o = solver_pair(kind, bodies[sorted[i - 16 * k]]);
 				u32 oa = o.x ? o.x : o.y, ob = o.y ? o.y : o.x;
 				if (oa == ca || ob == ca || oa == cb || ob == cb) b = k;
 			}
@@ -590,7 +594,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_sched_merge(u32* slot_of, const u3
 
 // batch index and slot (batch*8 + lane) of every contact + the length of every body's chain (chain_len: zero on entry)
 __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, const uint2* bodies, const u32* slot_of, const u32* slot_done, const u32* slot_left,
-		u32 slots_per_bucket, const u32* complete_off, const u32* left_count, u32* batch_of, u32* slot_idx, u32* slot_contact, u32 max_slots,
+		u32 slots_per_bucket, const u32* complete_off, const u32* left_count, const uint8_t* kind, u32* batch_of, u32* slot_idx, u32* slot_contact, u32 max_slots,
 		u32* chain_len, u32* counts) {
 	u32 n = counts[CNT_CONTACTS];
 	u32 nfull = counts[CNT_FULL_BATCHES];
@@ -617,8 +621,8 @@ __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, con
 		u32 slot = batch * 8 + lane;
 		slot_idx[i] = slot;
 		if (slot < max_slots) slot_contact[slot] = sorted[i];
-		uint2 ab = bodies[sorted[i]];
-		if (ab.x) atomicAdd(&chain_len[ab.x], 1u);   // a side on the static world (body 0) has no chain
+		uint2 ab = solver_pair(kind, bodies[sorted[i]]);
+		if (ab.x) atomicAdd(&chain_len[ab.x], 1u);   // a side on the static world (body 0) or on a kinematic body has no chain
 		if (ab.y) atomicAdd(&chain_len[ab.y], 1u);
 	}
 }
@@ -634,7 +638,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_batch_index(const u32* sorted, con
 // token = number of contact applications the body has received in this launch.  The contact at position `seq` of a body's chain
 // of length `len` therefore runs in sweep w when the token reads w*len + seq, and leaves w*len + seq + 1.  (expected - seen) is
 // the number of applications still ahead of a waiting contact, which is what the solver's back-off sleeps on.  Body 0 (static
-// world) is never waited for: its sides get (0, 0).
+// world) and a kinematic body are never waited for: their sides get (0, 0).
 __global__ void __launch_bounds__(NB_BLOCK) k_chain_alloc(u32 nbodies, const u32* chain_len, u32* chain_next /* out: first free position of the segment */, u32* counts) {
 	const u32 lane = threadIdx.x & 31;
 	for (u32 base = blockIdx.x * blockDim.x; base < nbodies; base += gridDim.x * blockDim.x) {  // warp-uniform trip count
@@ -648,21 +652,21 @@ __global__ void __launch_bounds__(NB_BLOCK) k_chain_alloc(u32 nbodies, const u32
 	}
 }
 NB_DEV u64 chain_key(u32 batch, u32 e) { return ((u64)batch << 32) | e; }
-__global__ void __launch_bounds__(NB_BLOCK) k_chain_scatter(const u32* sorted, const uint2* bodies, const u32* batch_of, u32* chain_next, u64* chain_keys, const u32* counts) {
+__global__ void __launch_bounds__(NB_BLOCK) k_chain_scatter(const u32* sorted, const uint2* bodies, const uint8_t* kind, const u32* batch_of, u32* chain_next, u64* chain_keys, const u32* counts) {
 	const u32 n = counts[CNT_ENTRIES] >> 1;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-		const uint2 ab = bodies[sorted[i]];
+		const uint2 ab = solver_pair(kind, bodies[sorted[i]]);
 		const u32 batch = batch_of[i];
 		if (ab.x) chain_keys[atomicAdd(&chain_next[ab.x], 1u)] = chain_key(batch, 2*i);
 		if (ab.y) chain_keys[atomicAdd(&chain_next[ab.y], 1u)] = chain_key(batch, 2*i + 1);
 	}
 }
-__global__ void __launch_bounds__(NB_BLOCK) k_chain_rank(const u32* sorted, const uint2* bodies, const u32* batch_of, const u32* slot_idx, const u32* chain_end, const u32* chain_len,
+__global__ void __launch_bounds__(NB_BLOCK) k_chain_rank(const u32* sorted, const uint2* bodies, const uint8_t* kind, const u32* batch_of, const u32* slot_idx, const u32* chain_end, const u32* chain_len,
 		const u64* chain_keys, uint2* wait /*[2][stride]: seq, len*/, u32 stride, const u32* counts) {
 	const u32 n2 = counts[CNT_ENTRIES];
 	for (u32 e = blockIdx.x * blockDim.x + threadIdx.x; e < n2; e += gridDim.x * blockDim.x) {
 		const u32 i = e >> 1, side = e & 1;
-		const uint2 ab = bodies[sorted[i]];
+		const uint2 ab = solver_pair(kind, bodies[sorted[i]]);
 		const u32 body = side ? ab.y : ab.x;
 		uint2 w = make_uint2(0, 0);
 		if (body) {
@@ -679,13 +683,17 @@ __global__ void __launch_bounds__(NB_BLOCK) k_chain_rank(const u32* sorted, cons
 
 // ---------------- constraint rows (nudge.cpp:4350-4561), one thread per contact, SoA planes ----------------
 struct Rows { float* plane; u32 stride; u32* a; u32* b; u32* contact; float* state; uint2* wait; };  // plane[k*stride + slot], wait[side*stride + slot] = (seq, len)
+// a[slot] / b[slot] carry NB_READ_ONLY on a kinematic side: the solvers read that body's velocity and never write it.  A side is written
+// iff (int)a > 0, which also excludes body 0.
+#define NB_READ_ONLY 0x80000000u
+#define NB_BODY_INDEX(x) ((x) & ~NB_READ_ONLY)
 
 // SPLIT (throughput mode, nb_jacobi.cuh): body i is split into cnt[i] sub-bodies of mass m_i / cnt[i], one per contact (Tonge et al.,
 // "Mass splitting for jitter-free parallel rigid body simulation", 2012), so every effective-mass term of body i is scaled by
 // cnt[i]; the planes that APPLY an impulse to a body (NA.., UA.., MASS_A/B) stay unscaled because the sub-bodies are averaged back.
 template<bool SPLIT>
 __global__ void __launch_bounds__(NB_BLOCK) k_build_rows(const float4* contacts, const uint2* bodies,
-		const nb_transform* xf, const float4* inertia, const nb_body_momentum* momentum, Rows R, const u32* counts, const u32* cnt) {
+		const nb_transform* xf, const float4* inertia, const nb_body_momentum* momentum, const uint8_t* kind, Rows R, const u32* counts, const u32* cnt) {
 	__shared__ u32 s_rsqrt[2048];
 	for (u32 i = threadIdx.x; i < 2048; i += blockDim.x) s_rsqrt[i] = g_rsqrt_lut[i];
 	__syncthreads();
@@ -773,7 +781,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_build_rows(const float4* contacts,
 		P[UB_X*S] = ub_xt; P[UB_Y*S] = ub_yt; P[UB_Z*S] = ub_zt; P[VB_X*S] = vb_xt; P[VB_Y*S] = vb_yt; P[VB_Z*S] = vb_zt;
 		P[NB_X*S] = nb_x; P[NB_Y*S] = nb_y; P[NB_Z*S] = nb_z;
 		P[MASS_A*S] = a_mass_inverse; P[MASS_B*S] = b_mass_inverse;
-		R.a[j] = a; R.b[j] = b;
+		R.a[j] = kin_is(kind, a) ? a | NB_READ_ONLY : a; R.b[j] = kin_is(kind, b) ? b | NB_READ_ONLY : b;
 	}
 }
 
@@ -966,59 +974,19 @@ NB_DEV void solve_contact(const Rows& R, u32 j, const float (&rv)[ROW_PLANES_TOT
 // >= 2 on either body only the linear halves are polled, and the warp sleeps hop_ns per missing application when all of its
 // lanes are that far away; from 1 on, all four halves are fetched in one round trip so the hand-off costs a single L2 access.
 #define NB_SOLVE_BACKOFF_NS 150u  // hop_ns of k_solve and k_solve_flow (__nanosleep may sleep up to twice as long)
-__global__ void __launch_bounds__(NB_BLOCK, 2) k_solve(Rows R, const float4* impulses, float4* mw, int mode, u32 sweeps, u32 hop_ns, u32* counts) {
-	__shared__ u32 s_rcp[2048];
-	__shared__ u32 s_rsqrt[2048];
-	for (u32 i = threadIdx.x; i < 2048; i += blockDim.x) { s_rcp[i] = g_rcp_lut[i]; s_rsqrt[i] = g_rsqrt_lut[i]; }
-	__syncthreads();
-	const u32 NS = 8 * counts[CNT_BATCHES];
-	const u32 tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
-	const u32 passes = mode == 0 ? 1 : (mode == 1 ? sweeps : sweeps + 1);
-	const u32 S = R.stride;
-	for (u32 w = 0; w < passes; ++w) {
-		const bool sweep = mode == 1 || (mode == 2 && w > 0);  // this pass is a PGS sweep (else: the warm start)
-		for (u32 s0 = 0; s0 < NS; s0 += nth) {  // uniform trip count for the whole grid
-			u32 slot = s0 + tid;
-			bool pending = false, near = false;
-			u32 a = 0, b = 0, exp_a = 0, exp_b = 0;
-			float rv[ROW_PLANES_TOTAL], st[3];
-			if (slot < NS && R.contact[slot] != NB_NONE) {
-				pending = true;
-				a = R.a[slot]; b = R.b[slot];
-				uint2 wa = R.wait[slot], wb = R.wait[S + slot];
-				exp_a = w * wa.y + wa.x; exp_b = w * wb.y + wb.x;
-				if (sweep) {
-					const float* c = R.plane + slot;
-					#pragma unroll
-					for (int k = 0; k < ROW_PLANES_TOTAL; ++k) rv[k] = c[(size_t)k * S];
-					st[0] = R.state[0*S + slot]; st[1] = R.state[1*S + slot]; st[2] = R.state[2*S + slot];
-				}
-			}
-			while (__any_sync(0xffffffffu, pending)) {
-				u32 want = 0xffffffffu;
-				if (pending) {
-					float4 al = ld128(mw + 2*a), bl = ld128(mw + 2*b), aw, bw;
-					if (near) { aw = ld128(mw + 2*a + 1); bw = ld128(mw + 2*b + 1); }
-					u32 ra = a ? exp_a - asu(al.w) : 0, rb = b ? exp_b - asu(bl.w) : 0;
-					u32 r = max(ra, rb);
-					if (r == 0 && near && (!a || asu(aw.w) == exp_a) && (!b || asu(bw.w) == exp_b)) {
-						if (sweep) solve_contact(R, slot, rv, st, al, aw, bl, bw, LutMath{ s_rcp, s_rsqrt });
-						else warm_start_contact(R, slot, impulses, al, aw, bl, bw, LutMath{ s_rcp, s_rsqrt });
-						if (a) { float tk = asf(exp_a + 1); al.w = tk; aw.w = tk; st128(mw + 2*a, al); st128(mw + 2*a + 1, aw); }  // body 0 is static: never written (DESIGN.md §1)
-						if (b) { float tk = asf(exp_b + 1); bl.w = tk; bw.w = tk; st128(mw + 2*b, bl); st128(mw + 2*b + 1, bw); }
-						pending = false;
-					}
-					else {
-						near = r <= 1;
-						want = r >= 2 ? (r - 1) * hop_ns : 0;
-					}
-				}
-				want = __reduce_min_sync(0xffffffffu, want);
-				if (want != 0xffffffffu && want) __nanosleep(min(want, 20000u));
-			}
-		}
-	}
-}
+// k_solve: without a kinematic set, a side is written iff its index is nonzero (body 0 is read only).  k_solve_kin, launched only with a set:
+// iff (int)index > 0, which also keeps a kinematic side (NB_READ_ONLY) from being written.  One source, nb_solve_kernel.inc, so that
+// k_solve stays the kernel it was before kinematic bodies, instruction for instruction.
+#define NB_SOLVE_NAME k_solve
+#define NB_SOLVE_WRITES(x) ((x) != 0)
+#include "nb_solve_kernel.inc"
+#undef NB_SOLVE_NAME
+#undef NB_SOLVE_WRITES
+#define NB_SOLVE_NAME k_solve_kin
+#define NB_SOLVE_WRITES(x) ((int)(x) > 0)
+#include "nb_solve_kernel.inc"
+#undef NB_SOLVE_NAME
+#undef NB_SOLVE_WRITES
 
 // ---------------- update_cached_impulses (nudge.cpp:4857-4884) ----------------
 __global__ void __launch_bounds__(NB_BLOCK) k_update_impulses(Rows R, float4* impulses, const u32* counts) {
@@ -1037,12 +1005,14 @@ __global__ void __launch_bounds__(NB_BLOCK) k_update_impulses(Rows R, float4* im
 }
 
 // ---------------- user gravity/damping loop (example/main.cpp:291-305) and advance (nudge.cpp:4886-4926) ----------------
-__global__ void __launch_bounds__(NB_BLOCK) k_gravity_damping(const u32* active_idx, nb_body_momentum* momentum, float time_step, float gravity, float damping_base, const u32* counts) {
+// A moving kinematic body is active but keeps its velocity.
+__global__ void __launch_bounds__(NB_BLOCK) k_gravity_damping(const u32* active_idx, const uint8_t* kind, nb_body_momentum* momentum, float time_step, float gravity, float damping_base, const u32* counts) {
 	u32 n = counts[CNT_ACTIVE];
 	float damping = 1.0f - time_step*damping_base;
 	float dv = gravity * time_step;
 	for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
 		u32 i = active_idx[k];
+		if (kin_is(kind, i)) continue;
 		float4* p = reinterpret_cast<float4*>(momentum + i);
 		float4 l = p[0], w = p[1];
 		l.y -= dv;

@@ -16,6 +16,9 @@
 // a version-3 header without it is not a state file), reserved[3] = the context's max_sensor_pairs, and then sensor[boxes + spheres] (1 byte
 // each, 0 or 1) after the filter table, if any.  A context without sensors writes version 1 or 2 as before; every version loads, and a
 // version-1 or 2 load removes any sensor table.
+// Version 4 (a context with kinematic bodies, nb_upload_kinematic_bodies): reserved[0..3] as in version 3 (reserved[2] = 0 without sensors),
+// reserved[4] = the number of kinematic bodies (at least 1), and then their indices (u32, ascending) after the sensor table, if any.  The
+// velocities are the momentum rows.  Versions 1-3 load and remove any kinematic set.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
@@ -27,13 +30,27 @@ static bool state_put(FILE* f, const void* dev, size_t bytes, std::vector<unsign
 	if (cudaStreamSynchronize(st) != cudaSuccess) return false;
 	return padded == 0 || fwrite(tmp.data(), 1, padded, f) == padded;
 }
-static bool state_version_ok(const NbStateHeader& h) { return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1); }
+static bool state_version_ok(const NbStateHeader& h) {
+	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1);
+}
 static bool state_get(FILE* f, void* dev, size_t bytes, std::vector<unsigned char>& tmp, cudaStream_t st) {
 	const size_t padded = (bytes + 15) & ~(size_t)15;
 	tmp.resize(padded);
 	if (padded && fread(tmp.data(), 1, padded, f) != padded) return false;
 	if (bytes && cudaMemcpyAsync(dev, tmp.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
 	return cudaStreamSynchronize(st) == cudaSuccess;
+}
+
+// Fills the velocities of `kin` (bodies set) from the device momentum rows.  Synchronises.
+static int download_rows_into(nb_context* ctx, std::vector<nb_kinematic_body>& kin, cudaStream_t st) {
+	std::vector<nb_body_momentum> m(ctx->B);
+	CK(cudaMemcpyAsync(m.data(), ctx->mom, sizeof(nb_body_momentum) * (size_t)ctx->B, cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	for (nb_kinematic_body& k : kin) {
+		const nb_body_momentum& r = m[k.body];
+		for (int c = 0; c < 3; ++c) { k.velocity[c] = r.velocity[c]; k.angular_velocity[c] = r.angular_velocity[c]; }
+	}
+	return NB_OK;
 }
 
 extern "C" {
@@ -48,9 +65,10 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
+	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = c[CNT_CACHE]; h.solver_mode = (u32)ctx->solver_mode;
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
@@ -62,6 +80,12 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 		&& state_put(f, ctx->cache_tags, 8 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_features, 4 * (size_t)h.cache, tmp, st) && state_put(f, ctx->cache_data, 16 * (size_t)h.cache, tmp, st);
 	if (h.reserved[1]) ok = ok && state_put(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
 	if (h.reserved[2]) ok = ok && state_put(f, ctx->sensor, (size_t)h.boxes + h.spheres, tmp, st);
+	if (h.reserved[4]) {
+		const size_t bytes = 4 * ctx->kin_list.size(), padded = (bytes + 15) & ~(size_t)15;
+		tmp.assign(padded, 0);
+		memcpy(tmp.data(), ctx->kin_list.data(), bytes);
+		ok = ok && fwrite(tmp.data(), 1, padded, f) == padded;
+	}
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -106,10 +130,22 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	const bool table = h.version >= 2 && h.reserved[1];
 	if (table) ok = ok && state_get(f, ctx->filter, 4 * ((size_t)h.boxes + h.spheres), tmp, st);
 	std::vector<uint8_t> sensors;
-	if (ok && h.version == 3) {
+	const bool has_sensors = h.version == 3 || (h.version == 4 && h.reserved[2]);
+	if (ok && has_sensors) {
 		const size_t k = (size_t)h.boxes + h.spheres, padded = (k + 15) & ~(size_t)15;
 		sensors.resize(padded);
 		ok = padded == 0 || fread(sensors.data(), 1, padded, f) == padded;
+	}
+	std::vector<nb_kinematic_body> kin;
+	if (ok && h.version == 4) {
+		const size_t n = h.reserved[4], padded = (4 * n + 15) & ~(size_t)15;
+		std::vector<u32> idx(padded / 4);
+		ok = fread(idx.data(), 1, padded, f) == padded;
+		kin.resize(n);
+		for (size_t i = 0; ok && i < n; ++i) {
+			if (idx[i] == 0 || idx[i] >= h.bodies || (i && idx[i] <= idx[i - 1])) ok = false;   // nonzero, in range, ascending
+			memset(&kin[i], 0, sizeof(kin[i])); kin[i].body = idx[i];
+		}
 	}
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
@@ -122,7 +158,13 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	ctx->has_filter = table; ctx->filter_flags = h.version >= 2 ? (h.reserved[0] & NB_FILTER_SKIP_CONNECTED) : 0;
 	++ctx->filter_version;
 	{ int r = build_conn_lookup(ctx, st); if (r) return r; }
-	{ int r = set_sensors(ctx, sensors.data(), h.version == 3 ? h.boxes + h.spheres : 0, h.version == 3 ? h.reserved[3] : 0, st); if (r) return r; }
+	{ int r = set_sensors(ctx, sensors.data(), has_sensors ? h.boxes + h.spheres : 0, has_sensors ? h.reserved[3] : 0, st); if (r) return r; }
+	// the kinematic set: the velocities are already in the loaded momentum rows, so the scatter rewrites them with their own values
+	drop_kinematic(ctx);
+	if (!kin.empty()) {
+		{ int r = download_rows_into(ctx, kin, st); if (r) return r; }
+		{ int r = nb_upload_kinematic_bodies(ctx, kin.data(), (u32)kin.size(), st); if (r) return r; }
+	}
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }

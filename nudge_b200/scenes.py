@@ -31,8 +31,11 @@ FILTER_SKIP_CONNECTED = 1
 # sensor events are CONTACT_EVENT rows of kind SENSOR_BEGIN / SENSOR_END with tags, kind, step, body_a and body_b set
 SENSOR_OVERLAP = np.dtype([("tags", "<u8"), ("body_a", "<u4"), ("body_b", "<u4")])
 SENSOR_BEGIN, SENSOR_END = 3, 4
+# nb_kinematic_body (include/nudge_b200.h): a kinematic body and the velocity it is driven at
+KINEMATIC = np.dtype([("body", "<u4"), ("velocity", "<f4", 3), ("angular_velocity", "<f4", 3), ("reserved", "<u4")])
 
 assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4 and SENSOR_OVERLAP.itemsize == 16
+assert KINEMATIC.itemsize == 32
 
 
 class Scene:
@@ -58,6 +61,8 @@ class Scene:
         self.filter_flags = 0
         # optional sensor colliders: one uint8 per collider (boxes first, then spheres; nonzero = sensor) or None
         self.sensors = None
+        # optional kinematic bodies: KINEMATIC rows (body, velocity, angular velocity) or None
+        self.kinematic = None
         # step parameters the reference leaves to the caller (example/main.cpp:275-305)
         self.time_step = np.float32(1.0 / 120.0)
         self.iterations = 8

@@ -6,6 +6,8 @@ import nudge_b200, bench
 from nudge_b200 import scenes
 
 def depth(a, b, sweeps):
+    """a, b: row_a / row_b in slot order.  A side with NB_READ_ONLY (bit 31, a kinematic body) is never waited for, like body 0."""
+    a = [0 if x >> 31 else x for x in a]; b = [0 if x >> 31 else x for x in b]
     last = {}
     per_sweep = []
     for w in range(sweeps):
