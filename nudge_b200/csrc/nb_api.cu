@@ -18,7 +18,7 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 
 // A sub-step as a CUDA graph (nb_step, nb_shard_step; run_graphed): captured once per key and replayed while the key holds.  Every
 // count the kernels need lives in device memory, so the graph only depends on the parameters and the scene shape held in the key.
-struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long urow_version, plan_version, events_version, filter_version, sensor_version, kinematic_version; };
+struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long plan_version, graph_epoch; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
 struct nb_context {
@@ -37,6 +37,7 @@ struct nb_context {
 	u64* keybits;  // OR, AND of the Morton codes of the current collide
 	bool defer_warm_start;  // nb_step: the warm start runs inside the first solver launch
 	StepGraph graph; bool capturing;  // nb_step's graph; capturing: run_graphed is recording a step of this context
+	unsigned long long graph_epoch;   // in the graphs' key: bumped by every change of which kernels a step launches or of their arguments
 	u32* chain_start; u32* chain_len;  // per body: segment cursor (the segment's end once k_chain_scatter ran) / number of chain entries
 	bool contacts_internal;  // the current contact set came from nb_collide (not nb_upload_contacts)
 	// throughput mode (nb_set_solver_mode): mass-splitting Jacobi, nb_jacobi.cuh
@@ -48,20 +49,19 @@ struct nb_context {
 	// nb_upload_bodies sends what the collision stage does not read (momentum, properties) on a second stream, so that copy runs under
 	// `collide`; the first consumer waits for ev_up_done (inside a captured step: an external event-wait node, re-armed by every upload)
 	cudaStream_t copy_stream; cudaEvent_t ev_up_begin, ev_up_done; bool upload_pending, capture_joined; int copy_overlap;
-	nb_constraint_row* urows; u32 urow_cap, urow_n, urow_levels; unsigned long long urow_version; std::vector<u32> urow_level_off, urow_order;
+	nb_constraint_row* urows; u32 urow_cap, urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order;
 	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer holds ev_alloc events and is kept while it is large enough
-	nb_contact_event* events; u32 ev_cap, ev_alloc; unsigned long long events_version;
+	nb_contact_event* events; u32 ev_cap, ev_alloc;
 	// collision filters (nb_upload_collision_filters): one category | mask << 16 word per collider while has_filter; with
 	// NB_FILTER_SKIP_CONNECTED and connections, conn_keys holds the sorted connection keys and conn_probe = their count (else 0)
-	u32* filter; bool has_filter; u32 filter_flags; u64* conn_keys; u64* conn_scratch; u32* conn_sort_n; u32 conn_probe; unsigned long long filter_version;
+	u32* filter; bool has_filter; u32 filter_flags; u64* conn_keys; u64* conn_scratch; u32* conn_sort_n; u32 conn_probe;
 	// sensor colliders (nb_upload_sensors, DESIGN.md section 8.7): one 0/1 byte per collider while has_sensor; sensor_cap = candidate sensor
 	// pairs per collide.  The candidate keys, the sort buffers and the current / old overlap lists hold sensor_alloc entries and are kept while
 	// large enough.
 	uint8_t* sensor; bool has_sensor; u32 sensor_cap, sensor_alloc; u64* sensor_keys; SortBuffers sensor_sb; uint4* sensor_cur; uint4* sensor_old;
-	unsigned long long sensor_version;
 	// kinematic bodies (nb_upload_kinematic_bodies, DESIGN.md section 8.8): kind[body] as in nb_collide.cuh (bit 0 kinematic, bit 1 moving),
 	// allocated for max_bodies on the first upload of a set; kin_list = the set (host copy, ascending); kin_rows = the scatter's staging rows
-	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; nb_kinematic_body* kin_rows; u32 kin_rows_cap; unsigned long long kinematic_version;
+	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; nb_kinematic_body* kin_rows; u32 kin_rows_cap;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -162,7 +162,7 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 
 // The kinematic table as the kernels take it: null without a set, so that they load nothing extra.
 static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
-static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->kinematic_version; } }
+static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->graph_epoch; } }
 
 // The velocity scatter of nb_upload_kinematic_bodies: each listed body's velocity and angular velocity into its momentum row (the unused lanes
 // are left alone), and its kind byte (the caller clears the table first when the set changes).
@@ -189,8 +189,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	memset(&key, 0, sizeof(key));  // padding bytes included: the key is compared with memcmp
 	key.stream = st; key.ts = time_step; key.gravity = gravity; key.damping = damping; key.iterations = iterations;
 	key.B = ctx->B; key.nboxes = ctx->nboxes; key.nspheres = ctx->nspheres; key.nconn = ctx->nconn; key.tagbits = ctx->tagbits; key.kbits = ctx->kbits;
-	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.urow_version = ctx->urow_version; key.plan_version = plan_version; key.events_version = ctx->events_version;
-	key.filter_version = ctx->filter_version; key.sensor_version = ctx->sensor_version; key.kinematic_version = ctx->kinematic_version;
+	key.debug = ctx->debug; key.solver_mode = ctx->solver_mode; key.transport = transport; key.plan_version = plan_version; key.graph_epoch = ctx->graph_epoch;
 	if (!g.exec || memcmp(&key, &g.key, sizeof(key)) != 0) {
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -270,7 +269,7 @@ static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pair
 	CK(cudaMemsetAsync(ctx->counts + CNT_SENSOR_PAIRS, 0, 3 * sizeof(u32), st));   // candidates, current and old overlaps
 	CK(cudaStreamSynchronize(st));
 	ctx->has_sensor = n != 0; ctx->sensor_cap = cap;
-	++ctx->sensor_version;   // nb_step's graph re-records with or without the sensor launches
+	++ctx->graph_epoch;   // nb_step's graph re-records with or without the sensor launches
 	return NB_OK;
 }
 
@@ -468,8 +467,8 @@ int nb_download_transforms(nb_context* ctx, nb_transform* h, uint32_t count, voi
 
 int nb_upload_colliders(nb_context* ctx, const nb_collider_data* h, void* stream) {
 	if (h->boxes.count > ctx->cfg.max_boxes || h->spheres.count > ctx->cfg.max_spheres) { ctx->error = "too many colliders"; return NB_ERR_CAPACITY; }
-	if (ctx->has_filter && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_filter = false; ++ctx->filter_version; }  // the table belongs to a collider count
-	if (ctx->has_sensor && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_sensor = false; ++ctx->sensor_version; }  // so does the sensor table
+	if (ctx->has_filter && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_filter = false; ++ctx->graph_epoch; }  // the table belongs to a collider count
+	if (ctx->has_sensor && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_sensor = false; ++ctx->graph_epoch; }  // so does the sensor table
 	ctx->nboxes = h->boxes.count; ctx->nspheres = h->spheres.count;
 	u32 maxtag = 1;
 	for (u32 i = 0; i < h->boxes.count; ++i) maxtag = std::max(maxtag, h->boxes.tags[i]);
@@ -497,7 +496,7 @@ int nb_upload_collision_filters(nb_context* ctx, const nb_collision_filter* h, u
 	cudaStream_t st = (cudaStream_t)stream;
 	if (n) CK(cudaMemcpyAsync(ctx->filter, h, sizeof(nb_collision_filter) * (size_t)n, cudaMemcpyHostToDevice, st));   // category | mask << 16 as a u32
 	ctx->has_filter = n != 0; ctx->filter_flags = flags;
-	++ctx->filter_version;   // nb_step's graph re-records with the new kernel arguments
+	++ctx->graph_epoch;   // nb_step's graph re-records with the new kernel arguments
 	int r = build_conn_lookup(ctx, st); if (r) return r;
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
@@ -537,7 +536,7 @@ int nb_upload_kinematic_bodies(nb_context* ctx, const nb_kinematic_body* h, uint
 	k_kinematic_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->kin_rows, n, ctx->mom, ctx->kind);
 	++ctx->launches;
 	CK(cudaGetLastError());
-	if (!same) { ctx->has_kin = true; ctx->kin_list.swap(list); ++ctx->kinematic_version; }   // nb_step's graph re-records with the table
+	if (!same) { ctx->has_kin = true; ctx->kin_list.swap(list); ++ctx->graph_epoch; }   // nb_step's graph re-records with the table
 	return NB_OK;
 }
 int nb_upload_cache(nb_context* ctx, const nb_contact_cache* h, void* stream) {
@@ -802,7 +801,7 @@ int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 int nb_enable_contact_events(nb_context* ctx, uint32_t capacity) {
 	CK(cudaDeviceSynchronize());   // nothing in flight may still write the counters or the buffer
 	ctx->ev_cap = 0;           // off until the buffer below exists (a failed allocation leaves events disabled)
-	++ctx->events_version;     // nb_step's graph re-records with or without the event launches
+	++ctx->graph_epoch;        // nb_step's graph re-records with or without the event launches
 	if (capacity > ctx->ev_alloc) {
 		if (ctx->events) { cudaFree(ctx->events); ctx->events = nullptr; ctx->ev_alloc = 0; }
 		void* p = nullptr;

@@ -75,7 +75,7 @@ int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, ui
 		ALLOC(p, (size_t)n + n / 2 + 64);
 		ctx->urows = p; ctx->urow_cap = n + n / 2 + 64;
 	}
-	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->urow_version;
+	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->graph_epoch;
 	if (!n) return NB_OK;
 	std::vector<u32> level(n);
 	std::map<u32, u32> last;   // body -> level of the last row that touched it

@@ -9,6 +9,7 @@ The filter only takes pairs out of the broadphase list, and everything else in n
     keep their order, fine islands over connections and those contacts give the active bodies and the contacts of sleeping fine islands
     (appended to the sleeping pairs, one tag per pair), and the sleeping pairs are sorted (nudge.cpp:4008).
 A pair's contacts depend only on its two colliders, so dropping pairs leaves the others' contacts and their relative order unchanged.
+restate_collide does this for any pair rule, and with the kinematic island rules for tests/kinematic_ref.py.
 With no table and no flag the result is the oracle's own, bit for bit (tests/test_collision_filter_oracle.py checks this over a run
 with sleeping islands).  Contacts are matched to pairs by their collider tags, so scenes must give every collider a distinct tag."""
 import numpy as np
@@ -16,10 +17,12 @@ from oracle import pyoracle
 
 
 class Sets:
-    """The oracle's union-find (oracle/nudge_oracle.cpp Sets): body 0, the static world, never joins."""
+    """The oracle's union-find (oracle/nudge_oracle.cpp Sets): body 0, the static world, never joins, and neither do the bodies in
+    `fixed` (kinematic bodies, tests/kinematic_ref.py)."""
 
-    def __init__(self, n):
+    def __init__(self, n, fixed=()):
         self.parent = list(range(n))
+        self.fixed = fixed
 
     def find(self, x):
         p = self.parent
@@ -28,7 +31,7 @@ class Sets:
         return x
 
     def join(self, a, b):
-        if not a or not b:
+        if not a or not b or a in self.fixed or b in self.fixed:
             return
         a, b = self.find(a), self.find(b)
         if a != b:
@@ -46,6 +49,94 @@ def pair_passes(filters, flags, connected, body, lo, hi):
     return keep
 
 
+def restate_collide(sim, run_oracle, pair_keep, kin=(), moving=()):
+    """The collide stage of `sim` restated from the all-awake oracle run `run_oracle()` (module docstring).  `pair_keep(body, lo, hi)` is the
+    mask of the broadphase pairs kept (collider indices lo, hi; body = each collider's body).  `kin` are the kinematic bodies, which never
+    join a set, and `moving` those of them that move: each is active itself and makes the dynamic side of each of its edges active.  With
+    `kin` empty these are the oracle's island rules.  Records the all-awake run's pair list and contact tags as sim.awake_pairs and
+    sim.awake_tags, and the kept pairs for pairs_view as sim._pairs."""
+    idle = sim.idle.copy()
+    sim.idle[:] = 0
+    try:
+        run_oracle()
+    finally:
+        sim.idle[:] = idle
+    v = pyoracle.OracleSim.pairs_view(sim)
+    sim.awake_pairs = v
+    sim.awake_tags = sim.contact_tags[:sim.contacts.count].copy()
+    body = np.concatenate([sim.box_transforms["body"], sim.sphere_transforms["body"]]).astype(np.int64)
+    tag = np.concatenate([sim.box_tags, sim.sphere_tags]).astype(np.uint64)
+    lo, hi = v["lo"].astype(np.int64), v["hi"].astype(np.int64)
+    keep = pair_keep(body, lo, hi)
+    lo, hi = lo[keep], hi[keep]
+    sim._pairs = dict(lo=v["lo"][keep].copy(), hi=v["hi"][keep].copy(), order=v["order"])
+    B = sim.scene.n_bodies
+    nondyn = set(kin) | {0}
+    conn = [(int(c["a"]), int(c["b"])) for c in sim.connections]
+
+    def islands(edges):
+        sets = Sets(B, kin)
+        for a, b in edges:
+            sets.join(a, b)
+        act = np.zeros(B, bool)
+        for i in range(1, B):
+            if i in kin:
+                act[i] = i in moving
+            elif idle[i] != 0xff:
+                act[sets.find(i)] = True
+        for a, b in edges:   # the taint of a moving kinematic body
+            if a in moving and b not in nondyn:
+                act[sets.find(b)] = True
+            elif b in moving and a not in nondyn:
+                act[sets.find(a)] = True
+        return sets, act
+
+    def set_of(sets, a, b):
+        return sets.find(a) if a not in nondyn else sets.find(b)
+
+    # coarse islands (nudge.cpp:3500-3703)
+    ba, bb = body[lo], body[hi]
+    sets, act = islands(conn + list(zip(ba.tolist(), bb.tolist())))
+    sleeping, live = [], set()
+    for a, b, x, y in zip(ba.tolist(), bb.tolist(), lo.tolist(), hi.tolist()):
+        if a == b:
+            continue
+        if act[set_of(sets, a, b)]:
+            live.add((min(int(tag[x]), int(tag[y])), max(int(tag[x]), int(tag[y]))))
+        else:
+            ta, tb = int(tag[x]), int(tag[y])
+            sleeping.append(ta | (tb << 32) if ta > tb else tb | (ta << 32))
+    # the live pairs' contacts, in the oracle's order
+    n = sim.contacts.count
+    tags = sim.contact_tags[:n]
+    t0, t1 = (tags & np.uint64(0xffffffff)).astype(np.int64), (tags >> np.uint64(32)).astype(np.int64)
+    sel = np.array([(min(a, b), max(a, b)) in live for a, b in zip(t0.tolist(), t1.tolist())], bool) if n else np.zeros(0, bool)
+    data, bodies, tags, feats = sim.contact_data[:n][sel], sim.contact_bodies[:n][sel], tags[sel], sim.contact_features[:n][sel]
+    # fine islands, active bodies, contact compaction (nudge.cpp:3788-4006)
+    sets, act = islands(conn + list(zip(bodies["a"].tolist(), bodies["b"].tolist())))
+    active = [i for i in range(1, B) if (act[i] if i in kin else act[sets.find(i)])]
+    out = np.zeros(len(tags), bool)
+    i = 0
+    while i < len(tags):
+        j = i
+        while j < len(tags) and tags[j] == tags[i]:
+            j += 1
+        a, b = int(bodies["a"][i]), int(bodies["b"][i])
+        if act[set_of(sets, a, b)]:
+            out[i:j] = True
+        else:
+            sleeping.append(int(tags[i]))
+        i = j
+    m = int(out.sum())
+    sim.contact_data[:m] = data[out]; sim.contact_bodies[:m] = bodies[out]; sim.contact_tags[:m] = tags[out]; sim.contact_features[:m] = feats[out]
+    sim.contacts.count = m
+    sl = np.sort(np.array(sleeping, np.uint64))
+    sim.sleeping_pairs[:len(sl)] = sl
+    sim.contacts.sleeping_count = len(sl)
+    sim.active_indices[:len(active)] = active
+    sim.active.count = len(active)
+
+
 class FilteredOracleSim(pyoracle.OracleSim):
     """OracleSim whose collide stage applies the scene's (or the uploaded) collision filters; every later stage is the oracle's own."""
 
@@ -59,80 +150,8 @@ class FilteredOracleSim(pyoracle.OracleSim):
         self.filter_flags = int(flags)
 
     def collide(self):
-        s = self.scene
-        idle = self.idle.copy()
-        self.idle[:] = 0
-        try:
-            super().collide()
-        finally:
-            self.idle[:] = idle
-        v = super().pairs_view()
-        body = np.concatenate([self.box_transforms["body"], self.sphere_transforms["body"]]).astype(np.int64)
-        tag = np.concatenate([self.box_tags, self.sphere_tags]).astype(np.uint64)
-        lo, hi = v["lo"].astype(np.int64), v["hi"].astype(np.int64)
-        conn = [(int(c["a"]), int(c["b"])) for c in self.connections]
-        connected = set((min(a, b), max(a, b)) for a, b in conn)
-        keep = pair_passes(self.filters, self.filter_flags, connected, body, lo, hi)
-        lo, hi = lo[keep], hi[keep]
-        self._pairs = dict(lo=v["lo"][keep].copy(), hi=v["hi"][keep].copy(), order=v["order"])
-        B = s.n_bodies
-        # coarse islands (nudge.cpp:3500-3703)
-        sets = Sets(B)
-        for a, b in conn:
-            sets.join(a, b)
-        ba, bb = body[lo], body[hi]
-        for a, b in zip(ba.tolist(), bb.tolist()):
-            sets.join(a, b)
-        act = np.zeros(B, bool)
-        for i in range(1, B):
-            if idle[i] != 0xff:
-                act[sets.find(i)] = True
-        sleeping, live = [], set()
-        for a, b, x, y in zip(ba.tolist(), bb.tolist(), lo.tolist(), hi.tolist()):
-            if a == b:
-                continue
-            if act[sets.find(a) if a else sets.find(b)]:
-                live.add((min(int(tag[x]), int(tag[y])), max(int(tag[x]), int(tag[y]))))
-            else:
-                ta, tb = int(tag[x]), int(tag[y])
-                sleeping.append(ta | (tb << 32) if ta > tb else tb | (ta << 32))
-        # the live pairs' contacts, in the oracle's order
-        n = self.contacts.count
-        tags = self.contact_tags[:n]
-        t0, t1 = (tags & np.uint64(0xffffffff)).astype(np.int64), (tags >> np.uint64(32)).astype(np.int64)
-        sel = np.array([(min(a, b), max(a, b)) in live for a, b in zip(t0.tolist(), t1.tolist())], bool) if n else np.zeros(0, bool)
-        data, bodies, tags, feats = self.contact_data[:n][sel], self.contact_bodies[:n][sel], tags[sel], self.contact_features[:n][sel]
-        # fine islands, active bodies, contact compaction (nudge.cpp:3788-4006)
-        sets = Sets(B)
-        for a, b in conn:
-            sets.join(a, b)
-        for a, b in zip(bodies["a"].tolist(), bodies["b"].tolist()):
-            sets.join(a, b)
-        act = np.zeros(B, bool)
-        for i in range(1, B):
-            if idle[i] != 0xff:
-                act[sets.find(i)] = True
-        active = [i for i in range(1, B) if act[sets.find(i)]]
-        out = np.zeros(len(tags), bool)
-        i = 0
-        while i < len(tags):
-            j = i
-            while j < len(tags) and tags[j] == tags[i]:
-                j += 1
-            a, b = int(bodies["a"][i]), int(bodies["b"][i])
-            if act[sets.find(a) if a else sets.find(b)]:
-                out[i:j] = True
-            else:
-                sleeping.append(int(tags[i]))
-            i = j
-        m = int(out.sum())
-        self.contact_data[:m] = data[out]; self.contact_bodies[:m] = bodies[out]; self.contact_tags[:m] = tags[out]; self.contact_features[:m] = feats[out]
-        self.contacts.count = m
-        sl = np.sort(np.array(sleeping, np.uint64))
-        self.sleeping_pairs[:len(sl)] = sl
-        self.contacts.sleeping_count = len(sl)
-        self.active_indices[:len(active)] = active
-        self.active.count = len(active)
+        connected = set((min(int(c["a"]), int(c["b"])), max(int(c["a"]), int(c["b"]))) for c in self.connections)
+        restate_collide(self, super().collide, lambda body, lo, hi: pair_passes(self.filters, self.filter_flags, connected, body, lo, hi))
 
     def pairs_view(self):
         return dict(self._pairs)

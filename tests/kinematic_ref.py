@@ -5,7 +5,7 @@ mass and inertia of its properties row, substitutes it in the scheduler and neve
 static world (body 0) carries no collider, every oracle stage runs with K and body 0 swapped (K's properties row zeroed: infinite mass), and
 the results are mapped back.  Any other set (several kinematic bodies, or colliders left on body 0) is restated through the collide stage,
 gravity and advance, which need no swap; setup and the sweeps refuse it (tests step the device and copy its state in, sync_oracle_from_gpu).  What the oracle cannot know is restated here:
-  - the collide stage, in the way tests/filter_ref.py restates the filter: the oracle runs with every body awake (all pairs, every pair's
+  - the collide stage, by tests/filter_ref.py restate_collide as for the filter: the oracle runs with every body awake (all pairs, every pair's
     contacts in pipeline order), pairs of two non-dynamic bodies with a kinematic one are dropped, and both island passes are redone with the
     kinematic rules: a kinematic body never joins a set, an edge to a MOVING one (any nonzero velocity component) makes the dynamic side's set
     active, an edge to one at rest is ignored; a moving kinematic body is active itself;
@@ -19,20 +19,7 @@ that sleeps and wakes).  Contacts are matched to pairs by their collider tags, s
 import numpy as np
 from nudge_b200 import scenes as S
 from oracle import pyoracle
-from tests.filter_ref import Sets
-
-
-class KinematicSets(Sets):
-    """Union-find in which body 0 and the kinematic bodies never join."""
-
-    def __init__(self, n, kin):
-        super().__init__(n)
-        self.kin = kin
-
-    def join(self, a, b):
-        if a in self.kin or b in self.kin:
-            return
-        super().join(a, b)
+from tests.filter_ref import restate_collide
 
 
 def moving(momentum, body):
@@ -98,85 +85,13 @@ class KinematicOracleSim(pyoracle.OracleSim):
 
     # ---- stages ----
     def collide(self):
-        s = self.scene
-        idle = self.idle.copy()
-        self.idle[:] = 0
-        try:
-            self._oracle(super().collide)
-        finally:
-            self.idle[:] = idle
-        v = super().pairs_view()
-        body = np.concatenate([self.box_transforms["body"], self.sphere_transforms["body"]]).astype(np.int64)
-        tag = np.concatenate([self.box_tags, self.sphere_tags]).astype(np.uint64)
-        lo, hi = v["lo"].astype(np.int64), v["hi"].astype(np.int64)
         kin = set(self.kin)
         nondyn = kin | {0}
-        mov = set(k for k in self.kin if moving(self.momentum, k))
-        # pairs of two non-dynamic bodies, one of them kinematic, are not broadphase pairs
-        keep = np.array([not (a in nondyn and b in nondyn and (a in kin or b in kin)) for a, b in zip(body[lo].tolist(), body[hi].tolist())], bool)
-        lo, hi = lo[keep], hi[keep]
-        self._pairs = dict(lo=v["lo"][keep].copy(), hi=v["hi"][keep].copy(), order=v["order"])
-        B = s.n_bodies
-        conn = [(int(c["a"]), int(c["b"])) for c in self.connections]
 
-        def islands(edges):
-            sets = KinematicSets(B, nondyn)
-            for a, b in edges:
-                sets.join(a, b)
-            act = np.zeros(B, bool)
-            for i in range(1, B):
-                if i in kin:
-                    act[i] = i in mov
-                elif idle[i] != 0xff:
-                    act[sets.find(i)] = True
-            for a, b in edges:   # the taint of a moving kinematic body
-                if a in mov and b not in nondyn:
-                    act[sets.find(b)] = True
-                elif b in mov and a not in nondyn:
-                    act[sets.find(a)] = True
-            return sets, act
-
-        def set_of(sets, a, b):
-            return sets.find(a) if a not in nondyn else sets.find(b)
-
-        ba, bb = body[lo], body[hi]
-        sets, act = islands(conn + list(zip(ba.tolist(), bb.tolist())))
-        sleeping, live = [], set()
-        for a, b, x, y in zip(ba.tolist(), bb.tolist(), lo.tolist(), hi.tolist()):
-            if a == b:
-                continue
-            if act[set_of(sets, a, b)]:
-                live.add((min(int(tag[x]), int(tag[y])), max(int(tag[x]), int(tag[y]))))
-            else:
-                ta, tb = int(tag[x]), int(tag[y])
-                sleeping.append(ta | (tb << 32) if ta > tb else tb | (ta << 32))
-        n = self.contacts.count
-        tags = self.contact_tags[:n]
-        t0, t1 = (tags & np.uint64(0xffffffff)).astype(np.int64), (tags >> np.uint64(32)).astype(np.int64)
-        sel = np.array([(min(a, b), max(a, b)) in live for a, b in zip(t0.tolist(), t1.tolist())], bool) if n else np.zeros(0, bool)
-        data, bodies, tags, feats = self.contact_data[:n][sel], self.contact_bodies[:n][sel], tags[sel], self.contact_features[:n][sel]
-        sets, act = islands(conn + list(zip(bodies["a"].tolist(), bodies["b"].tolist())))
-        active = [i for i in range(1, B) if (act[i] if i in kin else act[sets.find(i)])]
-        out = np.zeros(len(tags), bool)
-        i = 0
-        while i < len(tags):
-            j = i
-            while j < len(tags) and tags[j] == tags[i]:
-                j += 1
-            a, b = int(bodies["a"][i]), int(bodies["b"][i])
-            if act[set_of(sets, a, b)]:
-                out[i:j] = True
-            else:
-                sleeping.append(int(tags[i]))
-            i = j
-        m = int(out.sum())
-        self.contact_data[:m] = data[out]; self.contact_bodies[:m] = bodies[out]; self.contact_tags[:m] = tags[out]; self.contact_features[:m] = feats[out]
-        self.contacts.count = m
-        sl = np.sort(np.array(sleeping, np.uint64))
-        self.sleeping_pairs[:len(sl)] = sl
-        self.contacts.sleeping_count = len(sl)
-        self.active_indices[:len(active)] = active
-        self.active.count = len(active)
+        def keep(body, lo, hi):   # pairs of two non-dynamic bodies, one of them kinematic, are not broadphase pairs
+            return np.array([not (a in nondyn and b in nondyn and (a in kin or b in kin)) for a, b in zip(body[lo].tolist(), body[hi].tolist())], bool)
+        oracle_collide = super().collide
+        restate_collide(self, lambda: self._oracle(oracle_collide), keep, kin, set(k for k in self.kin if moving(self.momentum, k)))
 
     def pairs_view(self):
         return dict(self._pairs)

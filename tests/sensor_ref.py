@@ -5,24 +5,14 @@ restatement of the CPU oracle (tests/filter_ref.py).
     sensor with a collider of its own body go nowhere), so the physics is FilteredOracleSim with every pair that involves a sensor collider
     rejected, which is what category 0 and mask 0 on the sensor colliders do.
   - Overlaps: FilteredOracleSim.collide first runs the unmodified oracle with every body awake, which gives every pair and its contacts in
-    the pipeline's own orientation.  A sensor pair (exactly one sensor, different bodies, passing the user's filter and connected opt-out)
+    the pipeline's own orientation (kept as awake_pairs and awake_tags).  A sensor pair (exactly one sensor, different bodies, passing the user's filter and connected opt-out)
     overlaps iff it has at least one of those contacts.  Entry: tags = min | max << 32 of the collider tags, body_a = the body of the
     lower-tag collider; the list is sorted by tags.
   - Events: write_cached_impulses diffs the step's overlaps against those of its previous call, like the device.
 Contacts are matched to pairs by their collider tags, so scenes must give every collider a distinct tag."""
 import numpy as np
 from nudge_b200 import scenes
-from oracle import pyoracle
 from tests.filter_ref import FilteredOracleSim, pair_passes
-
-
-class _AwakeTap(pyoracle.OracleSim):
-    """Sits right below FilteredOracleSim in the MRO: keeps the all-awake oracle run's pair list and contact tags."""
-
-    def collide(self):
-        super().collide()
-        self._awake_pairs = pyoracle.OracleSim.pairs_view(self)
-        self._awake_tags = self.contact_tags[:self.contacts.count].copy()
 
 
 def overlap_events(old, cur, step):
@@ -37,7 +27,7 @@ def overlap_events(old, cur, step):
     return out
 
 
-class SensorOracleSim(FilteredOracleSim, _AwakeTap):
+class SensorOracleSim(FilteredOracleSim):
     """FilteredOracleSim with the scene's (or the uploaded) sensor table: physics without the sensor pairs, plus the overlap list of every
     collide (self.overlaps) and the sensor events of every write_cached_impulses (self.sensor_events(step))."""
 
@@ -78,7 +68,7 @@ class SensorOracleSim(FilteredOracleSim, _AwakeTap):
         out = np.zeros(0, scenes.SENSOR_OVERLAP)
         if self.sensors is None:
             return out
-        v = self._awake_pairs
+        v = self.awake_pairs
         lo, hi = v["lo"].astype(np.int64), v["hi"].astype(np.int64)
         body = np.concatenate([self.box_transforms["body"], self.sphere_transforms["body"]]).astype(np.int64)
         tag = np.concatenate([self.box_tags, self.sphere_tags]).astype(np.uint64)
@@ -86,7 +76,7 @@ class SensorOracleSim(FilteredOracleSim, _AwakeTap):
         s = self.sensors
         cand = (s[lo] ^ s[hi]) & (body[lo] != body[hi]) & pair_passes(self.user_filters, self.filter_flags, connected, body, lo, hi)
         lo, hi = lo[cand], hi[cand]
-        t = self._awake_tags
+        t = self.awake_tags
         touching = set(zip(np.minimum(t & np.uint64(0xffffffff), t >> np.uint64(32)).tolist(), np.maximum(t & np.uint64(0xffffffff), t >> np.uint64(32)).tolist()))
         tl, th = tag[lo], tag[hi]
         a = np.minimum(tl, th); b = np.maximum(tl, th)

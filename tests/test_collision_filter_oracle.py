@@ -2,13 +2,14 @@
 table, and with an all-pass table, is the unmodified oracle bit for bit over a run with sleeping and waking islands; its pair list is the
 oracle's minus the pairs the category / mask rule or the connected opt-out rejects, and its contacts only join passing colliders; a
 sharded local scene carries the filter rows of its colliders, Scene.copy keeps them, and nb_state_info reads version-1 and 2 headers."""
-import ctypes, os, struct
+import ctypes, os
 import numpy as np
 import nudge_b200
 from nudge_b200 import scenes, shard
 from oracle import pyoracle
 from tests.parity_util import stage_digests
 from tests.filter_ref import FilteredOracleSim
+from tests.gpu_util import state_header
 
 
 def _scene():
@@ -133,18 +134,14 @@ def test_shard_local_scene_carries_the_filter_rows_of_its_colliders():
     assert seen > 0                                                 # ghosts exist, and they kept their global rows
 
 
-def _header(version, reserved=(0,) * 8):
-    return b"NBSTATE1" + struct.pack("<15I", version, 1000, 600, 400, 7, 12345, 0, *reserved)
-
-
 def test_state_info_reads_version_1_and_version_2_headers(tmp_path):
     lib = nudge_b200.load_library()
     counts = (ctypes.c_uint32 * 5)()
     for version, reserved in ((1, (0,) * 8), (2, (1, 1) + (0,) * 6), (2, (0, 1) + (0,) * 6)):
         p = tmp_path / ("v%d_%d.bin" % (version, reserved[0]))
-        p.write_bytes(_header(version, reserved))
+        p.write_bytes(state_header(version, reserved))
         assert lib.nb_state_info(os.fsencode(str(p)), counts) == 0
         assert list(counts) == [1000, 600, 400, 7, 12345]
     p = tmp_path / "v3.bin"
-    p.write_bytes(_header(3))
+    p.write_bytes(state_header(3))
     assert lib.nb_state_info(os.fsencode(str(p)), counts) != 0

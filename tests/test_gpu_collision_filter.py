@@ -9,6 +9,7 @@ import nudge_b200
 from nudge_b200 import scenes
 from tests.parity_util import Report, compare_oracle_gpu_step, sync_oracle_from_gpu
 from tests.test_gpu_rows import ball_joint_rows, _quat_rotate
+from tests.gpu_util import fnv1a, side_stream, state_size
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -18,11 +19,6 @@ NB_ERR_ARGUMENT = -3
 def _oracle(scene):
     from tests.filter_ref import FilteredOracleSim
     return FilteredOracleSim(scene)
-
-
-def _stream():
-    import torch
-    return torch.cuda.Stream().cuda_stream
 
 
 def _filters(n, nboxes, seed=4):
@@ -104,7 +100,7 @@ def test_bit_parity_with_the_filtered_oracle_stage_by_stage():
 
 def test_all_pass_and_removed_tables_equal_a_plain_context():
     s = scenes.demo_scene(150, 150, iterations=4, spread=3.0, height=15.0, seed=3)
-    plain, passing, removed = (nudge_b200.Sim(s, stream=_stream()) for _ in range(3))
+    plain, passing, removed = (nudge_b200.Sim(s, stream=side_stream()) for _ in range(3))
     allpass = np.zeros(s.n_colliders, scenes.FILTER); allpass["category"] = 0xffff; allpass["mask"] = 0xffff
     passing.upload_collision_filters(allpass)
     removed.upload_collision_filters(_filters(s.n_colliders, s.n_boxes)); removed.upload_collision_filters(None)
@@ -205,7 +201,7 @@ def test_graph_replay_equals_staged_calls_while_the_table_changes():
     s = _mixed(seed=12)
     table = s.collision_filters
     s.collision_filters = None
-    a = nudge_b200.Sim(s, stream=_stream()); b = nudge_b200.Sim(s, stream=_stream())
+    a = nudge_b200.Sim(s, stream=side_stream()); b = nudge_b200.Sim(s, stream=side_stream())
     other = _filters(s.n_colliders, s.n_boxes, seed=8)
     for i in range(40):
         if i in (10, 20, 30):
@@ -224,7 +220,7 @@ def test_a_touching_pair_that_becomes_rejected_ends_once():
     from oracle import events_ref
     s = scenes.demo_scene(150, 150, iterations=4, spread=5.0, height=12.0, seed=4)
     o = _oracle(s); rec = events_ref.OracleEvents(o)
-    g = nudge_b200.Sim(s, contact_capacity=o.cap, stream=_stream())
+    g = nudge_b200.Sim(s, contact_capacity=o.cap, stream=side_stream())
     g.enable_contact_events(1 << 16)
 
     def same(what):
@@ -275,22 +271,8 @@ def test_throughput_mode_collides_like_parity_mode_and_never_joins_rejected_coll
     assert t.counts().contacts > 0
 
 
-def _state_size(B, nb, ns, nc, cache, filters):
-    pad = lambda x: (x + 15) // 16 * 16
-    n = 68 + pad(32 * B) + pad(16 * B) + pad(32 * B) + pad(B) + pad(4 * nb) + pad(16 * nb) + pad(32 * nb) + pad(4 * ns) + pad(4 * ns) + pad(32 * ns)
-    n += pad(8 * nc) + pad(8 * cache) + pad(4 * cache) + pad(16 * cache)
-    return n + (pad(4 * (nb + ns)) if filters else 0)
-
-
-def _fnv1a(b):
-    h = 1469598103934665603
-    for x in b:
-        h = ((h ^ x) * 1099511628211) & 0xffffffffffffffff
-    return h
-
-
 def test_filtered_state_saves_as_version_2_loads_and_replays():
-    side = _stream()
+    side = side_stream()
     s = _mixed(seed=14)
     s.connections = np.zeros(3, scenes.PAIR32); s.connections["a"] = (1, 5, 9); s.connections["b"] = (2, 6, 10)
     s.filter_flags = scenes.FILTER_SKIP_CONNECTED
@@ -304,7 +286,7 @@ def test_filtered_state_saves_as_version_2_loads_and_replays():
     version, = struct.unpack_from("<I", raw, 8); reserved = struct.unpack_from("<8I", raw, 36)
     assert version == 2 and reserved[0] == scenes.FILTER_SKIP_CONNECTED and reserved[1] == 1
     cache = struct.unpack_from("<I", raw, 28)[0]
-    assert len(raw) == _state_size(s.n_bodies, s.n_boxes, s.n_spheres, 3, cache, True)
+    assert len(raw) == state_size(s.n_bodies, s.n_boxes, s.n_spheres, 3, cache, True)
     tail = raw[len(raw) - (4 * s.n_colliders + 15) // 16 * 16:][:4 * s.n_colliders]
     assert tail == s.collision_filters.tobytes()
     other = scenes.demo_scene(120, 120, iterations=4, seed=99); other.connections = np.zeros(3, scenes.PAIR32)
@@ -317,14 +299,14 @@ def test_filtered_state_saves_as_version_2_loads_and_replays():
     out = subprocess.run([exe, p1, "--steps", "10", "--iterations", str(int(s.iterations)), "--dump", p2], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stdout + out.stderr
     last = out.stdout.strip().splitlines()[-1].split()
-    assert int(last[last.index("xf") + 1], 16) == _fnv1a(g.transforms.tobytes())
+    assert int(last[last.index("xf") + 1], 16) == fnv1a(g.transforms.tobytes())
     assert open(p2, "rb").read()[8:12] == struct.pack("<I", 2)
     # a version-1 load removes the table and the flags: the context steps like a plain one
     plain_scene = scenes.demo_scene(120, 120, iterations=4, spread=3.0, height=12.0, seed=14)
     plain = nudge_b200.Sim(plain_scene, stream=side)
     plain.save_state(p3)
     raw = open(p3, "rb").read()
-    assert struct.unpack_from("<I", raw, 8)[0] == 1 and len(raw) == _state_size(plain_scene.n_bodies, plain_scene.n_boxes, plain_scene.n_spheres, 0, 0, False)
+    assert struct.unpack_from("<I", raw, 8)[0] == 1 and len(raw) == state_size(plain_scene.n_bodies, plain_scene.n_boxes, plain_scene.n_spheres, 0, 0, False)
     h.load_state(p3)
     for _ in range(5):
         h.step(); plain.step()

@@ -7,6 +7,7 @@ import pytest
 import nudge_b200
 from nudge_b200 import scenes
 from tests.parity_util import sync_oracle_from_gpu
+from tests.gpu_util import side_stream
 
 pytestmark = pytest.mark.gpu
 NB_ERR_CAPACITY, NB_ERR_ARGUMENT, NB_ERR_OVERFLOW = -2, -3, -4
@@ -20,11 +21,6 @@ def _oracle(scene):
 def _recorder(o):
     from oracle import events_ref
     return events_ref.OracleEvents(o)
-
-
-def _stream():
-    import torch
-    return torch.cuda.Stream().cuda_stream
 
 
 def _sim(scene, o, stream=0, capacity=1 << 16):
@@ -55,7 +51,7 @@ def _falling():
 def test_graph_replay_equals_restatement_and_late_drains_get_the_concatenation():
     s = _falling()
     o = _oracle(s); rec = _recorder(o)
-    g = _sim(s, o, _stream()); late = _sim(s, o, _stream())
+    g = _sim(s, o, side_stream()); late = _sim(s, o, side_stream())
     kinds, want_late = set(), []
     for i in range(40):
         want = rec.step()
@@ -113,11 +109,11 @@ def test_stage_calls_equal_graph_replay_and_throughput_mode_follows_the_contract
     from oracle import events_ref
     s = _falling()
     o = _oracle(s)
-    a = _sim(s, o, _stream()); b = _sim(s, o)
+    a = _sim(s, o, side_stream()); b = _sim(s, o)
     for i in range(25):
         a.step(); b.step_staged()
         _same(a.contact_events()[0], b.contact_events()[0], "step %d" % i)
-    t = _sim(s, o, _stream())
+    t = _sim(s, o, side_stream())
     t.set_solver_mode("throughput")
     t.enable_contact_events(1 << 16)
     fields = [f for f in scenes.CONTACT_EVENT.names if f != "impulse"]
@@ -167,7 +163,7 @@ def test_a_small_buffer_keeps_the_first_events_and_counts_the_rest():
 
 def test_launches_per_step_and_graph_rerecording():
     s = _falling()
-    g = nudge_b200.Sim(s, stream=_stream())
+    g = nudge_b200.Sim(s, stream=side_stream())
 
     def per_step():
         g.step(); g.download_bodies()
@@ -246,7 +242,7 @@ def test_more_than_50k_contacts_from_an_emptied_cache():
 
 def test_sharded_step_refuses_a_context_with_events():
     s = _falling()
-    b = nudge_b200.Sim(s, stream=_stream())
+    b = nudge_b200.Sim(s, stream=side_stream())
     b.shard_create(0, 1, None, 1, 1)
     b.enable_contact_events(64)
     with pytest.raises(nudge_b200.NudgeError, match=r"\(-3\)"):

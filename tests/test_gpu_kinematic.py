@@ -10,15 +10,11 @@ import nudge_b200
 from nudge_b200 import scenes
 from tests.kinematic_ref import KinematicOracleSim, with_kinematic_ground, two_kinematic_platforms
 from tests.parity_util import Report, compare_oracle_gpu_step
+from tests.gpu_util import fnv1a, side_stream
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NB_ERR_ARGUMENT = -3
-
-
-def _stream():
-    import torch
-    return torch.cuda.Stream().cuda_stream
 
 
 def _rows(k, v=(0.0, 0.0, 0.0), w=(0.0, 0.0, 0.0)):
@@ -48,7 +44,7 @@ def _mapped_state(x, k):
 
 def test_no_set_and_empty_set_are_a_plain_context_with_the_same_launches():
     s = scenes.demo_scene(300, 300, iterations=4, spread=8.0, height=14.0, seed=31)
-    plain, empty, removed = (nudge_b200.Sim(s, stream=_stream(), pair_capacity=1 << 16, contact_capacity=1 << 17) for _ in range(3))
+    plain, empty, removed = (nudge_b200.Sim(s, stream=side_stream(), pair_capacity=1 << 16, contact_capacity=1 << 17) for _ in range(3))
     empty.upload_kinematic_bodies(np.zeros(0, scenes.KINEMATIC))
     removed.upload_kinematic_bodies(_rows(5, (0.0, 1.0, 0.0)))
     removed.upload_kinematic_bodies(None)
@@ -72,7 +68,7 @@ def test_no_set_and_empty_set_are_a_plain_context_with_the_same_launches():
 def test_kinematic_ground_at_rest_is_the_plain_context_mapped(n):
     base = scenes.box_drop(n, iterations=8)
     ks, k = with_kinematic_ground(base)
-    plain, kin = nudge_b200.Sim(base, stream=_stream()), nudge_b200.Sim(ks, stream=_stream())
+    plain, kin = nudge_b200.Sim(base, stream=side_stream()), nudge_b200.Sim(ks, stream=side_stream())
     for i in range(40 if n == 8191 else 20):
         a, b = plain.launch_count(), kin.launch_count()
         plain.step(); kin.step()
@@ -119,7 +115,7 @@ def test_moving_platforms_equal_the_restatement_bit_for_bit(motion):
 
 def test_pile_sleeps_on_a_stopped_platform_wakes_when_it_moves_and_sleeps_again():
     ks, k = with_kinematic_ground(scenes.box_drop(400, iterations=4, density_L=12.0, spacing=(2.2, 2.2, 2.2), rotate=False))
-    g = nudge_b200.Sim(ks, stream=_stream())
+    g = nudge_b200.Sim(ks, stream=side_stream())
 
     def until_asleep(limit):
         for i in range(limit):
@@ -196,9 +192,9 @@ def test_sensor_contacts_and_pairs_of_a_kinematic_body():
 
 def test_graph_replay_with_new_velocities_every_step():
     ks, k = _platform_scene((0.0, 0.0, 0.0), (0.0, 0.0, 0.0))
-    a, b = nudge_b200.Sim(ks, stream=_stream()), nudge_b200.Sim(ks, stream=_stream())
+    a, b = nudge_b200.Sim(ks, stream=side_stream()), nudge_b200.Sim(ks, stream=side_stream())
     plain = ks.copy(); plain.kinematic = None
-    c = nudge_b200.Sim(plain, stream=_stream())
+    c = nudge_b200.Sim(plain, stream=side_stream())
     a.step(); b.step_staged(); c.step()
     before = c.launch_count(); c.step()
     per_step = c.launch_count() - before   # a context without a set
@@ -219,15 +215,8 @@ def test_graph_replay_with_new_velocities_every_step():
     assert a.debug_scalar("graph_active") == 1
 
 
-def _fnv1a(b):
-    h = 1469598103934665603
-    for x in b:
-        h = ((h ^ x) * 1099511628211) & 0xffffffffffffffff
-    return h
-
-
 def test_state_files_carry_the_set_and_replay():
-    side = _stream()
+    side = side_stream()
     ks, k = _platform_scene((0.0, 0.2, 0.0), (0.0, 0.1, 0.0))
     g = nudge_b200.Sim(ks, stream=side)
     for _ in range(20):
@@ -253,7 +242,7 @@ def test_state_files_carry_the_set_and_replay():
     for _ in range(10):
         h.step()
     h.download_bodies()
-    assert int(last[last.index("xf") + 1], 16) == _fnv1a(h.transforms.tobytes())
+    assert int(last[last.index("xf") + 1], 16) == fnv1a(h.transforms.tobytes())
     assert open(p2, "rb").read()[8:12] == struct.pack("<I", 4)
     # a version-1 file drops the set: the platform is dynamic again and falls
     plain = nudge_b200.Sim(with_kinematic_ground(scenes.box_drop(600, iterations=8, density_L=14.0, spacing=(2.2, 2.4, 2.2)))[0], stream=side)
@@ -377,7 +366,7 @@ def test_ball_joint_chain_hung_from_a_moving_kinematic_body_follows_it():
 def test_state_versions_3_and_4_with_sensors():
     """Sensors and a set: version 4 with reserved[2] = 1 carries both; loading a version-3 file (sensors, no set) removes a set."""
     from tests.sensor_ref import add_sensors
-    side = _stream()
+    side = side_stream()
     ks, k = _platform_scene((0.0, 0.2, 0.0), (0.0, 0.0, 0.0))
     kin = ks.kinematic
     ks = add_sensors(ks, zones=[((0.0, 1.0, 0.0), (3.0, 1.0, 3.0))])

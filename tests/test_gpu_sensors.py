@@ -9,17 +9,13 @@ import nudge_b200
 from nudge_b200 import scenes
 from tests import np_edge_cases as E
 from tests.sensor_ref import SensorOracleSim, add_sensors, masked_out
+from tests.gpu_util import fnv1a, side_stream
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "np_edge_cases.npz")
 NB_ERR_ARGUMENT, NB_ERR_OVERFLOW = -3, -4
 SENSOR_KINDS = (scenes.SENSOR_BEGIN, scenes.SENSOR_END)
-
-
-def _stream():
-    import torch
-    return torch.cuda.Stream().cuda_stream
 
 
 def _pile():
@@ -61,7 +57,7 @@ def _state(x):
 def test_sensors_change_no_physics_bit_for_bit_at_every_step(which):
     s = _pile() if which == "pile_8191" else _mixed()
     steps, sleep_at = (160, 120) if which == "pile_8191" else (80, 50)
-    a = nudge_b200.Sim(s, stream=_stream()); b = nudge_b200.Sim(masked_out(s), stream=_stream())
+    a = nudge_b200.Sim(s, stream=side_stream()); b = nudge_b200.Sim(masked_out(s), stream=side_stream())
     for x in (a, b):
         x.enable_contact_events(1 << 18)
     overlapped = sensor_events = 0
@@ -87,7 +83,7 @@ def test_overlaps_and_sensor_events_equal_the_restatement_through_sleep_and_wake
     from oracle import events_ref
     s = _mixed(seed=22)
     o = SensorOracleSim(s, contact_capacity=1 << 17); rec = events_ref.OracleEvents(o)   # the all-awake oracle run holds every pair's contacts
-    g = nudge_b200.Sim(s, contact_capacity=o.cap, stream=_stream())
+    g = nudge_b200.Sim(s, contact_capacity=o.cap, stream=side_stream())
     g.enable_contact_events(1 << 16)
     asleep = []
     for i in range(70):
@@ -143,7 +139,7 @@ def test_graph_replay_equals_the_stage_calls_while_the_table_changes():
     s.sensors = None
     other = table.copy(); other[::5] = 1 - other[::5]
     # without the table the zones and sensor spheres are solid colliders inside the starting pile: room for the pairs and contacts that makes
-    a, b = (nudge_b200.Sim(s, stream=_stream(), pair_capacity=1 << 16, contact_capacity=1 << 17) for _ in range(2))
+    a, b = (nudge_b200.Sim(s, stream=side_stream(), pair_capacity=1 << 16, contact_capacity=1 << 17) for _ in range(2))
     for x in (a, b):
         x.enable_contact_events(1 << 16)
     for i in range(40):
@@ -162,12 +158,12 @@ def test_graph_replay_equals_the_stage_calls_while_the_table_changes():
 
 def test_launch_counts_and_throughput_mode():
     s = _mixed(seed=24)
-    plain = nudge_b200.Sim(masked_out(s), stream=_stream())
+    plain = nudge_b200.Sim(masked_out(s), stream=side_stream())
     plain.upload_collision_filters(None)
-    nosens = nudge_b200.Sim(scenes.demo_scene(300, 300, iterations=4, spread=4.0, height=14.0, seed=24), stream=_stream())
-    sens = nudge_b200.Sim(s, stream=_stream())
-    zero = nudge_b200.Sim(s, stream=_stream()); zero.upload_sensors(np.zeros(s.n_colliders, np.uint8))
-    removed = nudge_b200.Sim(s, stream=_stream()); removed.upload_sensors(None)
+    nosens = nudge_b200.Sim(scenes.demo_scene(300, 300, iterations=4, spread=4.0, height=14.0, seed=24), stream=side_stream())
+    sens = nudge_b200.Sim(s, stream=side_stream())
+    zero = nudge_b200.Sim(s, stream=side_stream()); zero.upload_sensors(np.zeros(s.n_colliders, np.uint8))
+    removed = nudge_b200.Sim(s, stream=side_stream()); removed.upload_sensors(None)
     used = {}
     for name, x in (("none", nosens), ("plain", plain), ("sensors", sens), ("zero", zero), ("removed", removed)):
         for i in range(3):
@@ -217,15 +213,8 @@ def test_wrong_count_collider_change_and_overflow():
     assert h.counts().overflow == 0 and len(h.sensor_overlaps()) > 0
 
 
-def _fnv1a(b):
-    h = 1469598103934665603
-    for x in b:
-        h = ((h ^ x) * 1099511628211) & 0xffffffffffffffff
-    return h
-
-
 def test_state_files_carry_the_table_and_replay():
-    side = _stream()
+    side = side_stream()
     s = _mixed(seed=26)
     g = nudge_b200.Sim(s, stream=side)
     for _ in range(25):
@@ -258,7 +247,7 @@ def test_state_files_carry_the_table_and_replay():
     for _ in range(10):
         h.step()
     h.download_bodies()
-    assert int(last[last.index("xf") + 1], 16) == _fnv1a(h.transforms.tobytes())
+    assert int(last[last.index("xf") + 1], 16) == fnv1a(h.transforms.tobytes())
     assert open(p2, "rb").read()[8:12] == struct.pack("<I", 3)
     plain = nudge_b200.Sim(scenes.demo_scene(120, 120, iterations=4, seed=3), stream=side)
     plain.save_state(p3)

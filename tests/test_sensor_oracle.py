@@ -2,7 +2,7 @@
 all-zero one, is the unmodified oracle bit for bit over a run that sleeps and wakes; with sensors its physics is the filtered restatement with
 the sensor colliders given category 0 and mask 0; its overlap lists follow their own BEGIN / END events while a pile sleeps inside a zone and
 wakes again; Scene.copy and shard.local_scene carry the table, and nb_state_info reads the sensor state header."""
-import ctypes, os, struct
+import ctypes, os
 import numpy as np
 import nudge_b200
 from nudge_b200 import scenes, shard
@@ -10,6 +10,7 @@ from oracle import pyoracle
 from tests.parity_util import stage_digests
 from tests.filter_ref import FilteredOracleSim
 from tests.sensor_ref import SensorOracleSim, add_sensors, masked_out, overlap_events
+from tests.gpu_util import state_header
 
 ZONES = [((0.0, -9.0, 0.0), (1.5, 1.5, 1.5)), ((2.5, -8.0, 1.0), (1.0, 2.5, 1.0)), ((-2.0, -7.0, -2.0), (2.0, 1.0, 2.0))]
 
@@ -118,17 +119,17 @@ def test_scene_copy_and_shard_rows_carry_the_sensor_table():
     assert loc.sensors is None
 
 
-def _header(version, reserved=(0,) * 8):
-    return b"NBSTATE1" + struct.pack("<15I", version, 1000, 600, 400, 7, 12345, 0, *reserved)
-
-
 def test_state_info_reads_the_sensor_header(tmp_path):
     lib = nudge_b200.load_library()
     counts = (ctypes.c_uint32 * 5)()
     for name, version, reserved, ok in (("v3", 3, (0, 0, 1, 4096) + (0,) * 4, True), ("v3f", 3, (1, 1, 1, 0) + (0,) * 4, True),
-                                        ("v3bad", 3, (0, 0, 0, 4096) + (0,) * 4, False), ("v4", 4, (0, 0, 1, 0) + (0,) * 4, False)):
+                                        ("v3bad", 3, (0, 0, 0, 4096) + (0,) * 4, False), ("v4", 4, (0, 0, 1, 0) + (0,) * 4, False),
+                                        ("v4s", 4, (0, 0, 1, 4096, 1, 0, 0, 0), True), ("v4k", 4, (1, 1, 0, 0, 3, 0, 0, 0), True),
+                                        ("v4s2", 4, (0, 0, 2, 0, 1, 0, 0, 0), False), ("v4k0", 4, (0, 0, 0, 0, 0, 0, 0, 0), False),
+                                        ("v5", 5, (0, 0, 1, 0, 1, 0, 0, 0), False), ("v1r", 1, (7, 9, 2, 5, 0, 3, 3, 3), True),
+                                        ("v2r", 2, (1, 1, 2, 0, 0, 0, 0, 0), True)):
         p = tmp_path / (name + ".bin")
-        p.write_bytes(_header(version, reserved))
+        p.write_bytes(state_header(version, reserved))
         r = lib.nb_state_info(os.fsencode(str(p)), counts)
         assert (r == 0) == ok, name
         if ok:
