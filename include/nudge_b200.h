@@ -19,6 +19,8 @@
  *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
  *   nb_upload_sensors               <- no reference counterpart (the reference has no trigger volumes)
  *   nb_upload_kinematic_bodies      <- no reference counterpart (the reference's only non-dynamic body is the static world, body 0)
+ *   nb_apply_body_impulses          <- no reference counterpart: the application's edit of BodyData between calls
+ *   nb_apply_radial_impulse         <- no reference counterpart: the application's edit of BodyData between calls
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -273,6 +275,39 @@ int nb_download_sensor_overlaps(nb_context*, nb_sensor_overlap* host, uint32_t c
  * version 4), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).  No extra launch per step. */
 typedef struct { uint32_t body; float velocity[3]; float angular_velocity[3]; uint32_t reserved; } nb_kinematic_body;   /* 32 bytes */
 int nb_upload_kinematic_bodies(nb_context*, const nb_kinematic_body* host, uint32_t n, void* stream);
+
+/* Body impulses (hits, kicks, thrusters, explosions, waking; DESIGN.md section 8.9): edits of chosen bodies' momentum rows and idle counters on
+ * the device between any two calls, the edit a reference application makes to its host BodyData.  The result is bit-identical to that host
+ * loop written with the float32 operations below, left to right, without fused multiply-adds.
+ * nb_apply_body_impulses applies the n entries one after the other, in list order wherever two entries name the same body.  For an entry with
+ * body b, offset o, impulse J and angular impulse L, with m = b's mass_inverse and W = b's world inverse inertia (computed from b's current
+ * rotation and properties row exactly as nb_setup_contact_constraints computes it, nudge.cpp:4182-4199):
+ *   v.x += m * J.x                                    (likewise y, z)
+ *   t.x  = (o.y*J.z - o.z*J.y) + L.x                  (cyclically for y, z: t = cross(o, J) + L)
+ *   w.x += (W.xx*t.x + W.xy*t.y) + W.xz*t.z           (w.y += (W.xy*t.x + W.yy*t.y) + W.yz*t.z; w.z += (W.xz*t.x + W.yz*t.y) + W.zz*t.z)
+ * Only the velocity and angular_velocity lanes are written (unused0 / unused1 are left alone), and every listed body gets idle counter 0, also
+ * with a zero impulse: a zero impulse is the way to wake a body.  Its island (connected bodies included) is active from the next nb_collide.
+ * NB_ERR_ARGUMENT, changing nothing (every entry is checked on the host before any device work): body 0, a body at or beyond the uploaded body
+ * count, a kinematic body (drive those with nb_upload_kinematic_bodies), or n > 0 with a null pointer.  n = 0 is a no-op.
+ * nb_apply_radial_impulse considers every body i in 1..count-1 that is not kinematic.  With d = p_i - center (p_i = the body's POSITION, its
+ * centre of mass, not its colliders' surfaces) and dist = sqrtf((d.x*d.x + d.y*d.y) + d.z*d.z), the body is hit iff dist < radius.  A hit body
+ * gets idle counter 0 and, if dist > 0, k = (impulse * (1.0f - dist / radius)) / dist, J = (d.x*k, d.y*k, d.z*k), v += m * J as above (no
+ * angular part).  A negative impulse pulls inwards; impulse 0 only wakes.  NB_ERR_ARGUMENT: a null `e`, or a radius that is not finite or not
+ * above 0.
+ * Both calls are asynchronous on `stream` and ordered like nb_upload_momentum (after a pending nb_upload_bodies side copy); the host array may
+ * be reused when the call returns.  They are legal between any two stage calls and keep nb_step's graph.  Launches per call: 3 for a list
+ * (n > 0: keys, one radix sort by (body, list position), one thread per body run), 1 for the radial impulse; none per step.  Not tested on a
+ * rank's context of nb_shard_step. */
+typedef struct {
+	uint32_t body;
+	float offset[3];            /* world-frame vector from the body's position (its centre of mass) to where the impulse acts; 0 = the centre */
+	float impulse[3];           /* linear impulse: velocity += mass_inverse * impulse */
+	float angular_impulse[3];   /* extra angular impulse, world frame */
+	uint32_t reserved[2];
+} nb_body_impulse;              /* 48 bytes */
+int nb_apply_body_impulses(nb_context*, const nb_body_impulse* host, uint32_t n, void* stream);
+typedef struct { float center[3]; float radius; float impulse; uint32_t reserved[3]; } nb_radial_impulse;   /* 32 bytes */
+int nb_apply_radial_impulse(nb_context*, const nb_radial_impulse* e, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

@@ -23,7 +23,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
            "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
-           "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies"]
+           "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse"]
 
 
 class Config(C.Structure):
@@ -102,6 +102,8 @@ def load_library():
         lib.nb_upload_sensors.argtypes = [V, V, C.c_uint32, C.c_uint32, V]
         lib.nb_download_sensor_overlaps.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_upload_kinematic_bodies.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_apply_body_impulses.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_apply_radial_impulse.argtypes = [V, V, V]
         _lib = lib
     return _lib
 
@@ -415,6 +417,21 @@ class Sim(abi.HostState):
         device; call it every step with the same bodies and new velocities to drive them."""
         k = np.ascontiguousarray(np.asarray(rows if rows is not None else [], scenes.KINEMATIC).reshape(-1))
         self._ck(self.lib.nb_upload_kinematic_bodies(self.ctx, abi.ptr(k) if len(k) else None, len(k), self.stream), "nb_upload_kinematic_bodies")
+
+    # ---- body impulses (nb_apply_body_impulses, nb_apply_radial_impulse, include/nudge_b200.h): hits, kicks, explosions, waking ----
+    def apply_body_impulses(self, rows):
+        """rows: scenes.BODY_IMPULSE rows (or anything np.asarray turns into them, e.g. tuples (body, offset, impulse, angular_impulse, (0, 0))),
+        applied on the device in list order: velocity += mass_inverse * impulse, angular velocity += world inverse inertia * (offset x impulse +
+        angular_impulse), and the body woken (idle counter 0).  An empty list does nothing."""
+        r = np.ascontiguousarray(np.asarray(rows if rows is not None else [], scenes.BODY_IMPULSE).reshape(-1))
+        self._ck(self.lib.nb_apply_body_impulses(self.ctx, abi.ptr(r) if len(r) else None, len(r), self.stream), "nb_apply_body_impulses")
+
+    def apply_radial_impulse(self, center, radius, impulse):
+        """An explosion (impulse > 0) or implosion (impulse < 0) on the device: every dynamic body whose position lies within `radius` of
+        `center` is woken and pushed along the line from the center with an impulse falling linearly from `impulse` to 0 at the radius."""
+        e = np.zeros(1, scenes.RADIAL_IMPULSE)
+        e["center"] = center; e["radius"] = radius; e["impulse"] = impulse
+        self._ck(self.lib.nb_apply_radial_impulse(self.ctx, abi.ptr(e), self.stream), "nb_apply_radial_impulse")
 
     # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
     def enable_contact_events(self, capacity):

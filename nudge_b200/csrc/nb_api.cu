@@ -62,6 +62,9 @@ struct nb_context {
 	// kinematic bodies (nb_upload_kinematic_bodies, DESIGN.md section 8.8): kind[body] as in nb_collide.cuh (bit 0 kinematic, bit 1 moving),
 	// allocated for max_bodies on the first upload of a set; kin_list = the set (host copy, ascending); kin_rows = the scatter's staging rows
 	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; nb_kinematic_body* kin_rows; u32 kin_rows_cap;
+	// body impulses (nb_apply_body_impulses, DESIGN.md section 8.9): the call's own staging rows and sort buffers (imp_cap entries, kept while
+	// large enough), host staging, and its sort histogram, grid barrier and key count; none of it is shared with the step
+	nb_body_impulse* imp_rows; u32 imp_cap; SortBuffers imp_sb; u32* imp_n; std::vector<nb_body_impulse> imp_host;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -118,6 +121,7 @@ static Launch mk_launch(nb_context* ctx, void* stream) { Launch L = { (cudaStrea
 struct NbRange { NbRange(const char* name) { nvtxRangePushA(name); } ~NbRange() { nvtxRangePop(); } };
 #define NB_RANGE(name) NbRange nb_range_(name)
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb_rows_api.cuh
+static void free_impulse_rows(nb_context* ctx);                            // nb_impulse_api.cuh
 
 __global__ void k_reset_collide(u32* counts, u32 K, u64* keybits) {
 	if (threadIdx.x == 0) {
@@ -429,6 +433,7 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->events) cudaFree(ctx->events);
 	free_sensor_lists(ctx);
 	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
+	free_impulse_rows(ctx);
 	delete ctx;
 }
 
@@ -1131,3 +1136,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_state_api.cuh"
 #include "nb_rows_api.cuh"
 #include "nb_render_api.cuh"
+#include "nb_impulse_api.cuh"

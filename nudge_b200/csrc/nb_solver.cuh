@@ -114,22 +114,28 @@ __global__ void __launch_bounds__(NB_BLOCK) k_cache_merge(const u32* sorted, con
 }
 
 // ---------------- per-body world inverse inertia (nudge.cpp:4182-4199) ----------------
+// R diag(inertia_inverse) R^T of rotation q and properties row pr: d = (xx, yy, zz), o = (xy, xz, yz).  Also used by nb_apply_body_impulses,
+// whose results must carry these bits.
+NB_DEV void world_inverse_inertia(float4 q, float4 pr, float3& d, float3& o) {
+	mat3 m = qmatrix(mkq(q));
+	float ix = pr.x, iy = pr.y, iz = pr.z;
+	d.x = ix*m.c0.x*m.c0.x + iy*m.c1.x*m.c1.x + iz*m.c2.x*m.c2.x;
+	d.y = ix*m.c0.y*m.c0.y + iy*m.c1.y*m.c1.y + iz*m.c2.y*m.c2.y;
+	d.z = ix*m.c0.z*m.c0.z + iy*m.c1.z*m.c1.z + iz*m.c2.z*m.c2.z;
+	o.x = ix*m.c0.x*m.c0.y + iy*m.c1.x*m.c1.y + iz*m.c2.x*m.c2.y;
+	o.y = ix*m.c0.x*m.c0.z + iy*m.c1.x*m.c1.z + iz*m.c2.x*m.c2.z;
+	o.z = ix*m.c0.y*m.c0.z + iy*m.c1.y*m.c1.z + iz*m.c2.y*m.c2.z;
+}
 // A kinematic body (kind non-null and set) gets zero inverse mass and inertia whatever its properties row says.
 __global__ void __launch_bounds__(NB_BLOCK) k_inertia(u32 B, const nb_transform* xf, const nb_body_properties* props, const uint8_t* kind, float4* inertia, nb_body_momentum* momentum) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
 		float4 q = reinterpret_cast<const float4*>(xf + i)[1];
 		float4 pr = reinterpret_cast<const float4*>(props)[i];
 		if (kin_is(kind, i)) pr = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-		mat3 m = qmatrix(mkq(q));
-		float ix = pr.x, iy = pr.y, iz = pr.z;
-		float xx = ix*m.c0.x*m.c0.x + iy*m.c1.x*m.c1.x + iz*m.c2.x*m.c2.x;
-		float yy = ix*m.c0.y*m.c0.y + iy*m.c1.y*m.c1.y + iz*m.c2.y*m.c2.y;
-		float zz = ix*m.c0.z*m.c0.z + iy*m.c1.z*m.c1.z + iz*m.c2.z*m.c2.z;
-		float xy = ix*m.c0.x*m.c0.y + iy*m.c1.x*m.c1.y + iz*m.c2.x*m.c2.y;
-		float xz = ix*m.c0.x*m.c0.z + iy*m.c1.x*m.c1.z + iz*m.c2.x*m.c2.z;
-		float yz = ix*m.c0.y*m.c0.z + iy*m.c1.y*m.c1.z + iz*m.c2.y*m.c2.z;
-		inertia[2*i] = make_float4(xx, yy, zz, 0.0f);
-		inertia[2*i + 1] = make_float4(xy, xz, yz, 0.0f);
+		float3 d, o;
+		world_inverse_inertia(q, pr, d, o);
+		inertia[2*i] = make_float4(d.x, d.y, d.z, 0.0f);
+		inertia[2*i + 1] = make_float4(o.x, o.y, o.z, 0.0f);
 		momentum[i].unused0 = pr.w;  // nudge.cpp:4198
 	}
 }

@@ -33,9 +33,14 @@ SENSOR_OVERLAP = np.dtype([("tags", "<u8"), ("body_a", "<u4"), ("body_b", "<u4")
 SENSOR_BEGIN, SENSOR_END = 3, 4
 # nb_kinematic_body (include/nudge_b200.h): a kinematic body and the velocity it is driven at
 KINEMATIC = np.dtype([("body", "<u4"), ("velocity", "<f4", 3), ("angular_velocity", "<f4", 3), ("reserved", "<u4")])
+# nb_body_impulse / nb_radial_impulse (include/nudge_b200.h): an impulse on one body (offset = world-frame lever arm from its position) and an
+# explosion over every body whose position lies inside the sphere
+BODY_IMPULSE = np.dtype([("body", "<u4"), ("offset", "<f4", 3), ("impulse", "<f4", 3), ("angular_impulse", "<f4", 3), ("reserved", "<u4", 2)])
+RADIAL_IMPULSE = np.dtype([("center", "<f4", 3), ("radius", "<f4"), ("impulse", "<f4"), ("reserved", "<u4", 3)])
 
 assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4 and SENSOR_OVERLAP.itemsize == 16
 assert KINEMATIC.itemsize == 32
+assert BODY_IMPULSE.itemsize == 48 and RADIAL_IMPULSE.itemsize == 32
 
 
 class Scene:
