@@ -21,6 +21,7 @@
  *   nb_upload_kinematic_bodies      <- no reference counterpart (the reference's only non-dynamic body is the static world, body 0)
  *   nb_apply_body_impulses          <- no reference counterpart: the application's edit of BodyData between calls
  *   nb_apply_radial_impulse         <- no reference counterpart: the application's edit of BodyData between calls
+ *   nb_add_bodies / nb_remove_bodies <- no reference counterpart: the application's edit of its caller-owned arrays between steps
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
@@ -308,6 +309,65 @@ typedef struct {
 int nb_apply_body_impulses(nb_context*, const nb_body_impulse* host, uint32_t n, void* stream);
 typedef struct { float center[3]; float radius; float impulse; uint32_t reserved[3]; } nb_radial_impulse;   /* 32 bytes */
 int nb_apply_radial_impulse(nb_context*, const nb_radial_impulse* e, void* stream);
+
+/* Spawning and despawning (projectiles, debris, pickups, destroyed crates; DESIGN.md section 8.10): bodies and colliders appended to or removed
+ * from the device-resident scene between steps, with every table that holds body or collider indices kept.  Each call's result is bit-identical
+ * to the host edit below applied to the arrays the context holds, followed by a re-upload of all of them (nb_upload_bodies, nb_upload_colliders,
+ * nb_upload_connections, nb_upload_collision_filters with the same flags, nb_upload_sensors with the same max_sensor_pairs,
+ * nb_upload_kinematic_bodies with the kinematic bodies' current velocities, nb_upload_constraint_rows with the rows' current impulses), except
+ * that the sensor overlap lists are kept (remapped) where nb_upload_sensors would empty them.
+ *
+ * nb_remove_bodies(list of n bodies), host edit:
+ *   wake:        before anything moves, every kept body gets idle counter 0 when (a) a contact-cache entry's key pairs the tag of one of its
+ *                colliders with the tag of a removed collider (tags are compared, so with duplicate tags every collider carrying one counts;
+ *                the cache holds the kept entries of sleeping pairs, so a sleeping stack is found), or (b) a connection joins it to a removed
+ *                body.  Body 0 and kinematic bodies are never woken.
+ *   bodies:      the kept bodies keep their order: old index i becomes i - (number of removed indices below i).  Transform, properties, momentum
+ *                row (unused lanes included) and idle counter move with their body.
+ *   colliders:   every box and sphere whose transform.body is removed is removed; the kept ones keep their order and get the new index of their
+ *                body in transform.body.  Tags are not changed.  The filter and sensor tables (boxes first, then spheres) drop the same entries.
+ *   connections: an entry naming a removed body is dropped, the others keep their order with both sides remapped (body 0 stays 0).
+ *   kinematic:   removed members leave the set, the others are remapped; an empty set is no set.
+ *   rows:        a user constraint row naming a removed body is deleted; the others keep their upload order, their accumulated impulse and the
+ *                rest of the row, with a and b remapped (nb_download_constraint_rows then takes the new row count).
+ *   overlaps:    the sensor overlap lists (the current one and the one nb_write_cached_impulses compares against) keep their keys; body_a and
+ *                body_b are remapped, a removed side becomes NB_REMOVED_BODY.
+ *   The contact cache is NOT edited: its keys are collider tags, so the kept entries stay valid.  A removed collider's entries drop out at the
+ *   next nb_write_cached_impulses like any pair that stopped touching (with events: the ordinary NB_CONTACT_END, and NB_SENSOR_END with
+ *   NB_REMOVED_BODY from the remapped overlap list).  A collider added with a removed collider's tag before that write continues its cache
+ *   entries, as a re-upload with nb_upload_colliders would.
+ *   NB_ERR_ARGUMENT, changing nothing (every check runs on the host before any device work): body 0, a body at or beyond the body count, a body
+ *   listed twice, a null list with n > 0, a context that nb_shard_create was called on, a user constraint row or a connection that names a
+ *   body at or beyond the body count (their uploads accept such indices; every collider's body must be below it too).  NB_ERR_CAPACITY: more connections than the context's
+ *   scratch stride (the largest of max_pairs, max_contacts, max_bodies and the collider capacity).  n = 0 is a no-op without a launch.
+ *   Synchronises `stream` once (the new collider counts and largest tag decide tagbits and kbits exactly as nb_upload_colliders does).
+ *   Launches: 8 (mark, flags, one radix sort of (tag, body) keys, cache wake, body scan + gather, collider scan + gather), + 2 with connections
+ *   (scan + gather), + 2 for the NB_FILTER_SKIP_CONNECTED lookup when connections remain, + 1 with user rows left, + 1 with a sensor table.
+ *
+ * nb_add_bodies, host edit: the bodies->count rows go to indices B .. B+n-1 and are dynamic; the boxes are appended after the existing boxes and
+ *   the spheres after the existing spheres (a collider's transform.body may name any body below B + n, so n = 0 adds colliders to existing
+ *   bodies).  While a filter or sensor table exists, `tables` gives the new colliders' entries (boxes first, then spheres), inserted at the
+ *   same places: [old boxes][new boxes][old spheres][new spheres].  Connections, rows, the kinematic set and the overlap lists are unchanged.
+ *   NB_ERR_ARGUMENT, changing nothing: a null array with a nonzero count, a collider body at or beyond B + n, a table pointer that is null
+ *   while that table exists and colliders are added, a table pointer given while that table does not exist, a shard context.
+ *   NB_ERR_CAPACITY, changing nothing: max_bodies, max_boxes or max_spheres exceeded.  Asynchronous on `stream`, ordered like
+ *   nb_upload_momentum; the host arrays may be reused when the call returns, and only the new rows cross PCIe.  Launches: none (copies only).
+ *
+ * Both calls are for the time between steps (after nb_advance or nb_step, before nb_collide).  After either, the stage calls that use the last
+ * nb_collide's outputs (nb_read_cached_impulses, nb_setup_contact_constraints, nb_apply_impulses, nb_update_cached_impulses,
+ * nb_write_cached_impulses, nb_advance) return NB_ERR_ARGUMENT until the next nb_collide, nb_step, nb_upload_contacts or nb_load_state.  nb_step re-records its
+ * graph when the body, collider or connection counts, tagbits, kbits, the kinematic set or the user rows changed (removing n bodies and adding
+ * n back in one gap keeps it); a step of the edited context launches what a freshly uploaded context of the same shape and tables launches.
+ * Nothing runs per step.
+ * nb_download_colliders fills the host struct (its counts are capacities on input, the stored counts on output; NB_ERR_CAPACITY when one is
+ * too small); nb_download_connections fills `capacity` pairs at most (host->count = the stored count; NB_ERR_CAPACITY when it is larger).
+ * Both synchronise. */
+typedef struct { const nb_collision_filter* filters; const uint8_t* sensor_flags; } nb_spawn_tables;   /* entries of the ADDED colliders, boxes then spheres */
+#define NB_REMOVED_BODY 0xffffffffu
+int nb_add_bodies(nb_context*, const nb_body_data* bodies, const nb_collider_data* colliders, const nb_spawn_tables* tables /* may be null */, void* stream);
+int nb_remove_bodies(nb_context*, const uint32_t* bodies, uint32_t n, void* stream);
+int nb_download_colliders(nb_context*, nb_collider_data* host, void* stream);
+int nb_download_connections(nb_context*, nb_body_connections* host, uint32_t capacity, void* stream);
 
 /* CUDA streams for hosts that do not link the CUDA runtime (cgo / JNI / ctypes callers): a created stream is capturable, so nb_step
  * replays its CUDA graph there; a null stream means the legacy default stream and plain launches. */

@@ -23,7 +23,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_stream_create", "nb_stream_destroy", "nb_stream_synchronize", "nb_save_state", "nb_load_state", "nb_state_info",
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
            "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
-           "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse"]
+           "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
+           "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections"]
 
 
 class Config(C.Structure):
@@ -104,8 +105,16 @@ def load_library():
         lib.nb_upload_kinematic_bodies.argtypes = [V, V, C.c_uint32, V]
         lib.nb_apply_body_impulses.argtypes = [V, V, C.c_uint32, V]
         lib.nb_apply_radial_impulse.argtypes = [V, V, V]
+        lib.nb_add_bodies.argtypes = [V, V, V, V, V]
+        lib.nb_remove_bodies.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_download_colliders.argtypes = [V, V, V]
+        lib.nb_download_connections.argtypes = [V, V, C.c_uint32, V]
         _lib = lib
     return _lib
+
+
+class SpawnTables(C.Structure):
+    _fields_ = [("filters", C.c_void_p), ("sensor_flags", C.c_void_p)]
 
 
 class NudgeError(RuntimeError):
@@ -432,6 +441,102 @@ class Sim(abi.HostState):
         e = np.zeros(1, scenes.RADIAL_IMPULSE)
         e["center"] = center; e["radius"] = radius; e["impulse"] = impulse
         self._ck(self.lib.nb_apply_radial_impulse(self.ctx, abi.ptr(e), self.stream), "nb_apply_radial_impulse")
+
+    # ---- spawning and despawning (nb_add_bodies, nb_remove_bodies, include/nudge_b200.h): the scene changes shape on the device ----
+    def add_bodies(self, fragment, filters=None, sensors=None):
+        """Appends the bodies and colliders of `fragment` (a scenes.Scene, e.g. from scenes.fragment) on the device: its bodies become
+        bodies B .., its boxes and spheres follow the existing ones.  The fragment's collider `body` fields count from its own first body.
+        filters / sensors: the fragment colliders' entries (boxes, then spheres) for the context's filter / sensor table, required while that
+        table exists.  sim.scene and the host mirrors follow the edit (transforms, momentum and idle counters are the host mirrors' values)."""
+        s, fr = self.scene, fragment
+        B = s.n_bodies
+        new = s.copy()
+        for k in ("transforms", "properties", "momentum", "idle"):
+            setattr(new, k, np.concatenate([getattr(self, k), getattr(fr, k)]))
+        bx, sx = fr.box_transforms.copy(), fr.sphere_transforms.copy()
+        bx["body"] += np.uint32(B); sx["body"] += np.uint32(B)
+        for k, v in (("box_tags", fr.box_tags), ("box_data", fr.box_data), ("box_transforms", bx), ("sphere_tags", fr.sphere_tags),
+                     ("sphere_data", fr.sphere_data), ("sphere_transforms", sx)):
+            setattr(new, k, np.concatenate([getattr(s, k), v]))
+        f = sn = None
+        if filters is not None:
+            f = np.ascontiguousarray(filters, scenes.FILTER)
+            if s.collision_filters is not None:
+                new.collision_filters = np.concatenate([s.collision_filters[:s.n_boxes], f[:fr.n_boxes], s.collision_filters[s.n_boxes:], f[fr.n_boxes:]])
+        if sensors is not None:
+            sn = np.ascontiguousarray(sensors, np.uint8)
+            if s.sensors is not None:
+                new.sensors = np.concatenate([s.sensors[:s.n_boxes], sn[:fr.n_boxes], s.sensors[s.n_boxes:], sn[fr.n_boxes:]])
+        parts = [np.ascontiguousarray(a) for a in (fr.transforms, fr.properties, fr.momentum, fr.idle, fr.box_tags, fr.box_data, bx, fr.sphere_tags, fr.sphere_data, sx)]
+        P = lambda a: abi.ptr(a) if len(a) else None
+        bodies = abi.BodyData(P(parts[0]), P(parts[1]), P(parts[2]), P(parts[3]), fr.n_bodies)
+        cols = abi.ColliderData(abi.Shapes(P(parts[4]), P(parts[5]), P(parts[6]), fr.n_boxes), abi.Shapes(P(parts[7]), P(parts[8]), P(parts[9]), fr.n_spheres))
+        t = SpawnTables(P(f) if f is not None else None, P(sn) if sn is not None else None)
+        self._ck(self.lib.nb_add_bodies(self.ctx, C.byref(bodies), C.byref(cols), C.byref(t), self.stream), "nb_add_bodies")
+        self._mirror(new)
+
+    def remove_bodies(self, indices):
+        """Removes the listed bodies (never body 0), their colliders, the connections, user rows and kinematic entries naming them, and
+        compacts every index on the device (include/nudge_b200.h, nb_remove_bodies).  Bodies touching a removed one through the contact cache
+        or a connection are woken.  sim.scene and the host mirrors follow the edit (transforms, momentum and idle counters are the host
+        mirrors' values; download_bodies() fetches the device's)."""
+        idx = np.ascontiguousarray(np.asarray(indices, np.uint32).reshape(-1))
+        self._ck(self.lib.nb_remove_bodies(self.ctx, abi.ptr(idx) if len(idx) else None, len(idx), self.stream), "nb_remove_bodies")
+        if not len(idx):
+            return
+        s = self.scene
+        keep = np.ones(s.n_bodies, bool); keep[idx] = False
+        new = s.copy()
+        for k in ("transforms", "properties", "momentum", "idle"):
+            setattr(new, k, getattr(self, k)[keep].copy())
+        kc = keep[np.concatenate([s.box_transforms["body"], s.sphere_transforms["body"]]).astype(np.int64)]
+        for k, v in self.download_colliders().items():
+            setattr(new, k, v)
+        new.connections = self.download_connections()
+        if s.collision_filters is not None:
+            new.collision_filters = s.collision_filters[kc].copy()
+        if s.sensors is not None:
+            new.sensors = s.sensors[kc].copy()
+        if s.kinematic is not None:
+            rank = (np.cumsum(keep) - 1).astype(np.uint32)
+            k = s.kinematic[keep[s.kinematic["body"].astype(np.int64)]].copy()
+            k["body"] = rank[k["body"].astype(np.int64)]
+            new.kinematic = k if len(k) else None
+        self._mirror(new)
+
+    def _mirror(self, scene):
+        """Host mirrors for the edited scene; the contact capacity is kept."""
+        abi.HostState.__init__(self, scene, self.cap)
+
+    def download_colliders(self):
+        """The device's colliders as a dict of Scene fields: box_tags, box_data, box_transforms, sphere_tags, sphere_data, sphere_transforms."""
+        A = abi.aligned_array
+        nb, ns = max(self.scene.n_boxes, 1), max(self.scene.n_spheres, 1)
+        while True:
+            out = dict(box_tags=A(nb, np.uint32), box_data=A(nb, scenes.BOX), box_transforms=A(nb, scenes.TRANSFORM),
+                       sphere_tags=A(ns, np.uint32), sphere_data=A(ns, scenes.SPHERE), sphere_transforms=A(ns, scenes.TRANSFORM))
+            h = abi.ColliderData(abi.Shapes(abi.ptr(out["box_tags"]), abi.ptr(out["box_data"]), abi.ptr(out["box_transforms"]), nb),
+                                 abi.Shapes(abi.ptr(out["sphere_tags"]), abi.ptr(out["sphere_data"]), abi.ptr(out["sphere_transforms"]), ns))
+            r = self.lib.nb_download_colliders(self.ctx, C.byref(h), self.stream)
+            if r != -2:   # NB_ERR_CAPACITY: the counts say how much room is needed
+                break
+            nb, ns = max(h.boxes.count, 1), max(h.spheres.count, 1)
+        self._ck(r, "nb_download_colliders")
+        kb, ks = h.boxes.count, h.spheres.count
+        return {k: v[:kb if k.startswith("box") else ks].copy() for k, v in out.items()}
+
+    def download_connections(self):
+        """The device's connections as a scenes.PAIR32 array."""
+        n = max(len(self.scene.connections), 1)
+        while True:
+            out = abi.aligned_array(n, scenes.PAIR32)
+            h = abi.Connections(abi.ptr(out), 0)
+            r = self.lib.nb_download_connections(self.ctx, C.byref(h), n, self.stream)
+            if r != -2:
+                break
+            n = max(h.count, 1)
+        self._ck(r, "nb_download_connections")
+        return out[:h.count].copy()
 
     # ---- contact events (nb_contact_event, include/nudge_b200.h): which collider pairs began or ended touching, computed on the device ----
     def enable_contact_events(self, capacity):

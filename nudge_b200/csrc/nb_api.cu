@@ -65,6 +65,11 @@ struct nb_context {
 	// body impulses (nb_apply_body_impulses, DESIGN.md section 8.9): the call's own staging rows and sort buffers (imp_cap entries, kept while
 	// large enough), host staging, and its sort histogram, grid barrier and key count; none of it is shared with the step
 	nb_body_impulse* imp_rows; u32 imp_cap; SortBuffers imp_sb; u32* imp_n; std::vector<nb_body_impulse> imp_host;
+	// spawning (nb_add_bodies, nb_remove_bodies, DESIGN.md section 8.10): scene_edited refuses the stage calls that read the last collide's
+	// outputs until the next collide; sharded = nb_shard_create was called on this context (edits are refused); urow_ab = each user row's
+	// (a, b) in upload order, for re-levelling after a removal; spawn_idx / urows_spare = the removal's index staging and row gather buffers
+	// conn_host = the connections as uploaded or loaded, for the removal's index checks
+	bool scene_edited, sharded; std::vector<nb_body_pair> urow_ab, conn_host; u32* spawn_idx; u32 spawn_idx_cap; nb_constraint_row* urows_spare; u32 urows_spare_cap;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -122,6 +127,8 @@ struct NbRange { NbRange(const char* name) { nvtxRangePushA(name); } ~NbRange() 
 #define NB_RANGE(name) NbRange nb_range_(name)
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb_rows_api.cuh
 static void free_impulse_rows(nb_context* ctx);                            // nb_impulse_api.cuh
+// The stage calls that read the last nb_collide's outputs: refused after nb_add_bodies / nb_remove_bodies until the next collide
+#define NOT_AFTER_EDIT() do { if (ctx->scene_edited) { ctx->error = "the scene was edited (nb_add_bodies / nb_remove_bodies) since the last nb_collide"; return NB_ERR_ARGUMENT; } } while (0)
 
 __global__ void k_reset_collide(u32* counts, u32 K, u64* keybits) {
 	if (threadIdx.x == 0) {
@@ -434,6 +441,8 @@ void nb_destroy(nb_context* ctx) {
 	free_sensor_lists(ctx);
 	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
 	free_impulse_rows(ctx);
+	if (ctx->spawn_idx) cudaFree(ctx->spawn_idx);
+	if (ctx->urows_spare) cudaFree(ctx->urows_spare);
 	delete ctx;
 }
 
@@ -489,6 +498,7 @@ int nb_upload_colliders(nb_context* ctx, const nb_collider_data* h, void* stream
 int nb_upload_connections(nb_context* ctx, const nb_body_connections* h, void* stream) {
 	if (h->count > ctx->cfg.max_connections) { ctx->error = "too many connections"; return NB_ERR_CAPACITY; }
 	ctx->nconn = h->count;
+	ctx->conn_host.assign(h->data, h->data + h->count);
 	H2D(ctx->conn, h->data, h->count, nb_body_pair);
 	return build_conn_lookup(ctx, (cudaStream_t)stream);
 }
@@ -614,6 +624,7 @@ int nb_download_contacts(nb_context* ctx, nb_contact_data* h, nb_active_bodies* 
 }
 // Host -> HBM for the outputs of collide (the reference lets user code add or edit contacts between the calls, example/main.cpp:288).
 int nb_upload_contacts(nb_context* ctx, const nb_contact_data* h, const nb_active_bodies* ha, void* stream) {
+	ctx->scene_edited = false;
 	if (h) {
 		if (h->count > ctx->cfg.max_contacts || h->sleeping_count > ctx->cfg.max_contacts) { ctx->error = "too many contacts"; return NB_ERR_CAPACITY; }
 		ctx->contacts_internal = false;
@@ -648,6 +659,7 @@ int nb_download_cache(nb_context* ctx, nb_contact_cache* h, void* stream) {
 // ---------------- collide ----------------
 int nb_collide(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_collide");
+	ctx->scene_edited = false;
 	Launch L = mk_launch(ctx, stream);
 	cudaStream_t st = L.stream;
 	const u32 K = ctx->nboxes + ctx->nspheres, B = ctx->B, nboxes = ctx->nboxes;
@@ -782,12 +794,14 @@ static int read_sort(nb_context* ctx, void* stream) {
 
 int nb_read_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_read_cached_impulses");
+	NOT_AFTER_EDIT();
 	int r = read_sort(ctx, stream); if (r) return r;
 	return read_lookup(ctx, stream);
 }
 
 int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_write_cached_impulses");
+	NOT_AFTER_EDIT();
 	const u32 C = ctx->cfg.max_contacts;
 	const uint4* s_old = ctx->has_sensor ? ctx->sensor_old : nullptr;
 	const uint4* s_cur = ctx->has_sensor ? ctx->sensor_cur : nullptr;
@@ -897,6 +911,7 @@ static int launch_solve(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) 
 
 int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_setup_contact_constraints");
+	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	Launch L = mk_launch(ctx, stream);
 	cudaStream_t st = L.stream;
@@ -950,6 +965,7 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 
 int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 	NB_RANGE("nb_apply_impulses");
+	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	if (!sweeps) return NB_OK;
 	if (ctx->urow_n && !ctx->defer_warm_start) {   // user rows run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
@@ -967,6 +983,7 @@ int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 
 int nb_update_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_update_cached_impulses");
+	NOT_AFTER_EDIT();
 	k_update_impulses<<<GRID(ctx->cstride), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->rows, ctx->impulses, ctx->counts);
 	++ctx->launches;
 	CK(cudaGetLastError());
@@ -975,6 +992,7 @@ int nb_update_cached_impulses(nb_context* ctx, void* stream) {
 
 int nb_advance(nb_context* ctx, float time_step, void* stream) {
 	NB_RANGE("nb_advance");
+	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	k_advance<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts);
 	++ctx->launches;
@@ -1002,6 +1020,7 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
+	ctx->scene_edited = false;     // the step begins with nb_collide (also when its graph is replayed)
 	return run_graphed(ctx, ctx->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, 0, 0,
 					   [&] { return step_body(ctx, time_step, iterations, gravity, damping, stream); });
 }
@@ -1137,3 +1156,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_rows_api.cuh"
 #include "nb_render_api.cuh"
 #include "nb_impulse_api.cuh"
+#include "nb_spawn_api.cuh"

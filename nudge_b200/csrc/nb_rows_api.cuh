@@ -63,6 +63,31 @@ static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st) {
 	return NB_OK;
 }
 
+// The levels of rows (a, b) in upload order: a row's level is 1 + the highest level of an earlier row on either of its bodies (body 0 is
+// shared freely).  Fills level_off (levels + 1 offsets) and order (upload index -> device position: rows by level, upload order within one);
+// returns the number of levels.
+static u32 level_rows(const std::vector<nb_body_pair>& ab, std::vector<u32>& level_off, std::vector<u32>& order) {
+	const u32 n = (u32)ab.size();
+	std::vector<u32> level(n);
+	std::map<u32, u32> last;   // body -> level of the last row that touched it
+	u32 levels = 0;
+	for (u32 i = 0; i < n; ++i) {
+		const u32 a = ab[i].a, b = ab[i].b;
+		u32 l = 0;
+		if (a) { auto it = last.find(a); if (it != last.end()) l = std::max(l, it->second + 1); }
+		if (b) { auto it = last.find(b); if (it != last.end()) l = std::max(l, it->second + 1); }
+		level[i] = l; if (a) last[a] = l; if (b) last[b] = l;
+		levels = std::max(levels, l + 1);
+	}
+	level_off.assign(levels + 1, 0);
+	for (u32 i = 0; i < n; ++i) ++level_off[level[i] + 1];
+	for (u32 l = 0; l < levels; ++l) level_off[l + 1] += level_off[l];
+	std::vector<u32> cursor(level_off.begin(), level_off.end() - 1);
+	order.resize(n);
+	for (u32 i = 0; i < n; ++i) order[i] = cursor[level[i]]++;
+	return levels;
+}
+
 extern "C" {
 
 // Replaces the set of user rows (host pointer; n = 0 removes them).  Rows stay in effect, with their accumulated impulses carried
@@ -75,30 +100,23 @@ int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, ui
 		ALLOC(p, (size_t)n + n / 2 + 64);
 		ctx->urows = p; ctx->urow_cap = n + n / 2 + 64;
 	}
-	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->graph_epoch;
+	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_ab.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->graph_epoch;
 	if (!n) return NB_OK;
-	std::vector<u32> level(n);
-	std::map<u32, u32> last;   // body -> level of the last row that touched it
-	u32 levels = 0;
+	std::vector<nb_body_pair> ab(n);
 	for (u32 i = 0; i < n; ++i) {
 		const u32 a = rows[i].a, b = rows[i].b;
 		if (a >= ctx->cfg.max_bodies || b >= ctx->cfg.max_bodies) { ctx->error = "constraint row references a body beyond max_bodies"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
 		// k_user_rows gives each side its own read-modify-write of the momentum row, and the effective mass has no cross terms
 		if (a && a == b) { ctx->error = "constraint row names the same body as a and b: put the whole Jacobian on a and set b = 0"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
-		u32 l = 0;
-		if (a) { auto it = last.find(a); if (it != last.end()) l = std::max(l, it->second + 1); }
-		if (b) { auto it = last.find(b); if (it != last.end()) l = std::max(l, it->second + 1); }
-		level[i] = l; if (a) last[a] = l; if (b) last[b] = l;
-		levels = std::max(levels, l + 1);
+		ab[i].a = a; ab[i].b = b;
 	}
+	std::vector<u32> level_off, order;
+	const u32 levels = level_rows(ab, level_off, order);
 	if (levels > 4096) { ctx->error = "constraint rows form a dependency chain longer than 4096 levels: reorder them (e.g. red-black along a chain)"; ctx->urow_n = 0; return NB_ERR_CAPACITY; }
-	ctx->urow_level_off.assign(levels + 1, 0);
-	for (u32 i = 0; i < n; ++i) ++ctx->urow_level_off[level[i] + 1];
-	for (u32 l = 0; l < levels; ++l) ctx->urow_level_off[l + 1] += ctx->urow_level_off[l];
-	std::vector<u32> cursor(ctx->urow_level_off.begin(), ctx->urow_level_off.end() - 1);
 	std::vector<nb_constraint_row> sorted(n);
-	for (u32 i = 0; i < n; ++i) { const u32 d = cursor[level[i]]++; sorted[d] = rows[i]; ctx->urow_order[i] = d; }
+	for (u32 i = 0; i < n; ++i) sorted[order[i]] = rows[i];
 	CK(cudaMemcpy(ctx->urows, sorted.data(), sizeof(nb_constraint_row) * n, cudaMemcpyHostToDevice));
+	ctx->urow_level_off.swap(level_off); ctx->urow_order.swap(order); ctx->urow_ab.swap(ab);
 	ctx->urow_levels = levels;
 	return NB_OK;
 }

@@ -43,6 +43,7 @@ int nb_shard_create(nb_context* ctx, uint32_t rank, uint32_t world, const void* 
 	nb_shard* sh = new nb_shard();
 	*out = sh;
 	sh->ctx = ctx; sh->rank = rank; sh->world = world; sh->ghost_cap = ghost_capacity;
+	ctx->sharded = true;   // nb_add_bodies / nb_remove_bodies refuse a rank's context
 	sh->cap_export = export_capacity; sh->cap_ghost = ghost_capacity; sh->cap_sub = 4 * export_capacity + 64;
 	CK(cudaSetDevice(ctx->cfg.device));
 	sh->passes_cap = 24;

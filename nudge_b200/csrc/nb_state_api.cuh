@@ -35,10 +35,11 @@ static bool state_header_read(FILE* f, NbStateHeader& h) {
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
 // `host` when it is given and then copies to `dev` when that is given.
 struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; };
-struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, sensor, kin; };
+struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin; };
 
 // The sections of the file with header `h`, in file order.  A load keeps in `hc` the momentum rows (the kinematic velocities), the tags
-// (tagbits), the sensor flags (set_sensors) and the kinematic indices; a save writes the kinematic indices from hc.kin.
+// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors) and the kinematic indices; a save writes the
+// kinematic indices from hc.kin.
 static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, StateHostCopies& hc, bool load) {
 	const size_t K = (size_t)h.boxes + h.spheres;
 	return {
@@ -48,7 +49,7 @@ static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHe
 		{ ctx->box_xf, nullptr, sizeof(nb_transform), h.boxes, true },
 		{ ctx->sph_tags, &hc.sph_tags, 4, h.spheres, true }, { ctx->sph_data, nullptr, sizeof(nb_sphere_collider), h.spheres, true },
 		{ ctx->sph_xf, nullptr, sizeof(nb_transform), h.spheres, true },
-		{ ctx->conn, nullptr, sizeof(nb_body_pair), h.connections, true },
+		{ ctx->conn, &hc.conn, sizeof(nb_body_pair), h.connections, true },
 		{ ctx->cache_tags, nullptr, 8, h.cache, true }, { ctx->cache_features, nullptr, 4, h.cache, true }, { ctx->cache_data, nullptr, 16, h.cache, true },
 		{ ctx->filter, nullptr, 4, K, h.reserved[1] != 0 },
 		{ load ? nullptr : ctx->sensor, &hc.sensor, 1, K, h.reserved[2] != 0 },
@@ -149,6 +150,8 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->B = h.bodies; ctx->nboxes = h.boxes; ctx->nspheres = h.spheres; ctx->nconn = h.connections;
+	{ const nb_body_pair* p = reinterpret_cast<const nb_body_pair*>(hc.conn.data()); ctx->conn_host.assign(p, p + h.connections); }
+	ctx->scene_edited = false;   // the loaded scene replaces an edited one
 	ctx->tagbits = bits_for((u64)maxtag + 1);
 	ctx->kbits = bits_for(std::max(1u, h.boxes + h.spheres));
 	CK(cudaMemcpyAsync(ctx->counts + CNT_CACHE, &h.cache, 4, cudaMemcpyHostToDevice, st));

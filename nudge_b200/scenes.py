@@ -246,6 +246,28 @@ def two_boxes(pos_b=(0.0, 1.9, 0.0), rot_b=(0.0, 0.0, 0.0, 1.0), size_a=(1.0, 1.
     return s
 
 
+def fragment(positions, shape="box", sizes=None, first_tag=0):
+    """Bodies to spawn (Sim.add_bodies): one box (half extents `sizes`, (n, 3); default 0.5) or sphere (radii `sizes`, (n,); default 0.5)
+    per position, upright and at rest, with mass and inertia from the size laws of example/main.cpp:119-129 / 154-160 and tags first_tag,
+    first_tag + 1, ...  The collider `body` fields count from the fragment's first body."""
+    pos = np.asarray(positions, np.float32).reshape(-1, 3)
+    n = len(pos)
+    box = shape == "box"
+    s = Scene(n, n if box else 0, 0 if box else n)
+    s.name = "fragment"
+    s.transforms["position"] = pos
+    tags = np.uint32(first_tag) + np.arange(n, dtype=np.uint32)
+    if box:
+        size = np.broadcast_to(np.asarray(0.5 if sizes is None else sizes, np.float32), (n, 3))
+        s.box_tags[:] = tags; s.box_data["size"] = size; s.box_transforms["body"] = np.arange(n, dtype=np.uint32)
+        s.properties[:] = _box_props(np.ascontiguousarray(size))
+    else:
+        radius = np.broadcast_to(np.asarray(0.5 if sizes is None else sizes, np.float32), (n,))
+        s.sphere_tags[:] = tags; s.sphere_data["radius"] = radius; s.sphere_transforms["body"] = np.arange(n, dtype=np.uint32)
+        s.properties[:] = _sphere_props(np.ascontiguousarray(radius))
+    return s
+
+
 def hub_platform(n_side=55, iterations=4):
     """One DYNAMIC platform box carrying n_side^2 small boxes: every box-platform contact shares the platform's body, so the
     reference's batch scheduler (nudge.cpp:4206-4340) can never put two of them into one 8-lane batch.  Exercises the scheduler's
