@@ -273,7 +273,8 @@ int nb_download_sensor_overlaps(nb_context*, nb_sensor_overlap* host, uint32_t c
  * a broadphase pair (not counted, no islands, contacts, cache or events), two colliders of one kinematic body included; sensor pairs keep
  * their rules.  The solver substitutes a kinematic side like body 0: no chain, never waited for, excluded from the throughput mass split.
  * nb_upload_bodies keeps the set while the body count is unchanged and removes it when the count changes.  nb_save_state writes it (state
- * version 4), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).  No extra launch per step. */
+ * version 4), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).  No extra launch per step.
+ * A body made kinematic keeps its nb_set_body_forces entry, which the force stage ignores while the body is kinematic. */
 typedef struct { uint32_t body; float velocity[3]; float angular_velocity[3]; uint32_t reserved; } nb_kinematic_body;   /* 32 bytes */
 int nb_upload_kinematic_bodies(nb_context*, const nb_kinematic_body* host, uint32_t n, void* stream);
 
@@ -310,12 +311,61 @@ int nb_apply_body_impulses(nb_context*, const nb_body_impulse* host, uint32_t n,
 typedef struct { float center[3]; float radius; float impulse; uint32_t reserved[3]; } nb_radial_impulse;   /* 32 bytes */
 int nb_apply_radial_impulse(nb_context*, const nb_radial_impulse* e, void* stream);
 
+/* Per-body forces (balloons, zero-g debris, water drag, thrusters, wind, rockets; DESIGN.md section 8.11): a gravity scale, extra damping and a
+ * constant force and torque per body, applied on the device inside the step's force stage (nb_apply_gravity_damping, also inside nb_step).
+ * nb_set_body_forces writes the n listed bodies' entries into a per-body table; every other body keeps its entry.  The first call (n = 0
+ * included) creates the table for max_bodies, every body with the default entry (flags 0, gravity_scale 1, everything else 0).  Every listed
+ * body gets idle counter 0, so a body asleep on the ground wakes when its gravity scale changes.  NB_ERR_ARGUMENT, changing nothing (every
+ * entry is checked on the host before any device work): body 0, a body at or beyond the body count, a kinematic body, a body listed twice, a
+ * null list with n > 0, a field that is not finite, a negative damping, unknown flag bits.  Asynchronous on `stream`, ordered like
+ * nb_upload_momentum; the host array may be reused when the call returns.  One copy and one scatter launch (plus one fill launch when it
+ * creates the table); legal between any two calls; editing entries keeps nb_step's graph, creating or removing the table re-records it.
+ * nb_clear_body_forces removes the table: the step then launches exactly what it launched before the table existed.
+ * nb_download_body_forces fills B rows (B = the body count) with body = the row index; without a table these are default rows.
+ * NB_ERR_CAPACITY when capacity < B (*count = B).  Synchronises `stream`.  The stored reserved word is 0.
+ * The force stage with a table, float32, left to right, without fused multiply-adds.  For every body i of the active list that is not
+ * kinematic, with e = i's entry, m = its mass_inverse, q = its rotation, W = its world inverse inertia (computed from q and its properties
+ * row exactly as nb_setup_contact_constraints computes it), dt, g and d = the call's time step, gravity and damping:
+ *   dv  = g * dt
+ *   v.y = v.y - dv * e.gravity_scale
+ *   if e.force has a nonzero component (-0.0 counts as zero):
+ *       f = LOCAL ? qrot(q, e.force) : e.force        (qrot(q, r): t = 2 * cross(q.xyz, r); r + q.w * t + cross(q.xyz, t), nudge.cpp:1117-1120)
+ *       k = m * dt;  v.x = v.x + f.x * k               (likewise y, z)
+ *   if e.torque has a nonzero component:
+ *       t = LOCAL ? qrot(q, e.torque) : e.torque
+ *       w.x = w.x + ((W.xx*t.x + W.xy*t.y) + W.xz*t.z) * dt   (w.y: (W.xy*t.x + W.yy*t.y) + W.yz*t.z; w.z: (W.xz*t.x + W.yz*t.y) + W.zz*t.z)
+ *   lin = 1 - dt * (d + e.linear_damping);  ang = 1 - dt * (d + e.angular_damping)
+ *   v *= lin (x, y, z);  w *= ang (x, y, z)
+ *   if force or torque has a nonzero component: idle[i] = 0
+ * A default entry gives exactly the bits of the stage without a table (dv * 1 == dv, d + 0 damps like d, a zero force or torque is skipped).
+ * Sleeping: only active bodies get the stage, as without a table.  A body carrying a nonzero force or torque gets idle counter 0 in every
+ * step, so its island never sleeps while it is pushed; gravity scale and damping alone do not keep a body awake.
+ * A kinematic body's entry is kept but ignored while it is kinematic.  nb_upload_bodies keeps the table while the body count is unchanged and
+ * removes it when the count changes.  nb_add_bodies gives the new bodies the default entry; nb_remove_bodies moves the entries with their
+ * bodies.  nb_save_state writes the table (state version 5), nb_load_state restores it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).
+ * Cost per step: the stage's one launch reads the 48-byte entry of every active body; no extra launch. */
+typedef struct {
+	uint32_t body;
+	uint32_t flags;             /* NB_BODY_FORCE_LOCAL: force and torque are in the body frame */
+	float gravity_scale;        /* multiplies the step's gravity; default 1 */
+	float linear_damping;       /* added to the step's damping rate for the velocity; default 0 */
+	float angular_damping;      /* added to the step's damping rate for the angular velocity; default 0 */
+	float force[3];             /* constant force through the centre of mass; default 0 */
+	float torque[3];            /* constant torque; default 0 */
+	uint32_t reserved;
+} nb_body_force;                /* 48 bytes */
+enum nb_body_force_flags { NB_BODY_FORCE_LOCAL = 1 };
+int nb_set_body_forces(nb_context*, const nb_body_force* host, uint32_t n, void* stream);
+int nb_clear_body_forces(nb_context*, void* stream);
+int nb_download_body_forces(nb_context*, nb_body_force* host, uint32_t capacity, uint32_t* count, void* stream);
+
 /* Spawning and despawning (projectiles, debris, pickups, destroyed crates; DESIGN.md section 8.10): bodies and colliders appended to or removed
  * from the device-resident scene between steps, with every table that holds body or collider indices kept.  Each call's result is bit-identical
  * to the host edit below applied to the arrays the context holds, followed by a re-upload of all of them (nb_upload_bodies, nb_upload_colliders,
  * nb_upload_connections, nb_upload_collision_filters with the same flags, nb_upload_sensors with the same max_sensor_pairs,
- * nb_upload_kinematic_bodies with the kinematic bodies' current velocities, nb_upload_constraint_rows with the rows' current impulses), except
- * that the sensor overlap lists are kept (remapped) where nb_upload_sensors would empty them.
+ * nb_upload_kinematic_bodies with the kinematic bodies' current velocities, nb_upload_constraint_rows with the rows' current impulses,
+ * nb_set_body_forces with every non-default entry of the body force table), except that the sensor overlap lists are kept (remapped) where
+ * nb_upload_sensors would empty them.
  *
  * nb_remove_bodies(list of n bodies), host edit:
  *   wake:        before anything moves, every kept body gets idle counter 0 when (a) a contact-cache entry's key pairs the tag of one of its
@@ -328,6 +378,7 @@ int nb_apply_radial_impulse(nb_context*, const nb_radial_impulse* e, void* strea
  *                body in transform.body.  Tags are not changed.  The filter and sensor tables (boxes first, then spheres) drop the same entries.
  *   connections: an entry naming a removed body is dropped, the others keep their order with both sides remapped (body 0 stays 0).
  *   kinematic:   removed members leave the set, the others are remapped; an empty set is no set.
+ *   forces:      the body force table's entries move with their bodies (a removed body's entry is dropped); the table stays.
  *   rows:        a user constraint row naming a removed body is deleted; the others keep their upload order, their accumulated impulse and the
  *                rest of the row, with a and b remapped (nb_download_constraint_rows then takes the new row count).
  *   overlaps:    the sensor overlap lists (the current one and the one nb_write_cached_impulses compares against) keep their keys; body_a and
@@ -342,12 +393,14 @@ int nb_apply_radial_impulse(nb_context*, const nb_radial_impulse* e, void* strea
  *   scratch stride (the largest of max_pairs, max_contacts, max_bodies and the collider capacity).  n = 0 is a no-op without a launch.
  *   Synchronises `stream` once (the new collider counts and largest tag decide tagbits and kbits exactly as nb_upload_colliders does).
  *   Launches: 8 (mark, flags, one radix sort of (tag, body) keys, cache wake, body scan + gather, collider scan + gather), + 2 with connections
- *   (scan + gather), + 2 for the NB_FILTER_SKIP_CONNECTED lookup when connections remain, + 1 with user rows left, + 1 with a sensor table.
+ *   (scan + gather), + 2 for the NB_FILTER_SKIP_CONNECTED lookup when connections remain, + 1 with user rows left, + 1 with a sensor table;
+ *   the body force table adds none (the body gather moves its entries).
  *
  * nb_add_bodies, host edit: the bodies->count rows go to indices B .. B+n-1 and are dynamic; the boxes are appended after the existing boxes and
  *   the spheres after the existing spheres (a collider's transform.body may name any body below B + n, so n = 0 adds colliders to existing
  *   bodies).  While a filter or sensor table exists, `tables` gives the new colliders' entries (boxes first, then spheres), inserted at the
  *   same places: [old boxes][new boxes][old spheres][new spheres].  Connections, rows, the kinematic set and the overlap lists are unchanged.
+ *   While a body force table exists the new bodies get the default entry (set theirs with nb_set_body_forces afterwards).
  *   NB_ERR_ARGUMENT, changing nothing: a null array with a nonzero count, a collider body at or beyond B + n, a table pointer that is null
  *   while that table exists and colliders are added, a table pointer given while that table does not exist, a shard context.
  *   NB_ERR_CAPACITY, changing nothing: max_bodies, max_boxes or max_spheres exceeded.  Asynchronous on `stream`, ordered like
@@ -377,7 +430,8 @@ int nb_stream_synchronize(nb_context*, void* stream);
 
 /* State serialisation (SURVEY.md section 8 f3): the caller-owned PODs of nudge.h:73-129 (BodyData, ColliderData, BodyConnections,
  * ContactCache, widened layout) as one flat file, from / into the device-resident context.  Checkpoint, and what tools/nb_replay
- * steps headless; layout in nudge_b200/csrc/nb_state_api.cuh.  All three synchronise. */
+ * steps headless; layout in nudge_b200/csrc/nb_state_api.cuh.  All three synchronise.  A context with a body force table writes version 5
+ * (the table's B rows after the kinematic section); loading a file of versions 1-4 removes the context's table. */
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);

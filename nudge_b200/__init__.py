@@ -24,7 +24,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_upload_constraint_rows", "nb_download_constraint_rows", "nb_instance_matrices", "nb_shard_build_plan", "nb_shard_local_scene",
            "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
-           "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections"]
+           "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
+           "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces"]
 
 
 class Config(C.Structure):
@@ -109,6 +110,9 @@ def load_library():
         lib.nb_remove_bodies.argtypes = [V, V, C.c_uint32, V]
         lib.nb_download_colliders.argtypes = [V, V, V]
         lib.nb_download_connections.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_set_body_forces.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_clear_body_forces.argtypes = [V, V]
+        lib.nb_download_body_forces.argtypes = [V, V, C.c_uint32, V, V]
         _lib = lib
     return _lib
 
@@ -304,6 +308,10 @@ class Sim(abi.HostState):
             self.upload_sensors(s.sensors)
         if getattr(s, "kinematic", None) is not None:
             self.upload_kinematic_bodies(s.kinematic)
+        if getattr(s, "body_forces", None) is not None:
+            rows = s.body_forces
+            self.clear_body_forces()   # every body not listed gets the default entry
+            self.set_body_forces(rows)
 
     def upload_bodies(self):
         self._ck(self.lib.nb_upload_bodies(self.ctx, C.byref(self.bodies), self.stream), "nb_upload_bodies")
@@ -442,6 +450,40 @@ class Sim(abi.HostState):
         e["center"] = center; e["radius"] = radius; e["impulse"] = impulse
         self._ck(self.lib.nb_apply_radial_impulse(self.ctx, abi.ptr(e), self.stream), "nb_apply_radial_impulse")
 
+    # ---- per-body forces (nb_set_body_forces, include/nudge_b200.h): gravity scale, damping, constant force and torque inside the step ----
+    def set_body_forces(self, rows):
+        """rows: scenes.BODY_FORCE rows (or anything np.asarray turns into them), one per listed body; every other body keeps its entry.  The
+        first call creates the table with the default entry for every body.  Each listed body is woken.  sim.scene.body_forces follows."""
+        r = np.ascontiguousarray(np.asarray(rows if rows is not None else [], scenes.BODY_FORCE).reshape(-1))
+        self._ck(self.lib.nb_set_body_forces(self.ctx, abi.ptr(r) if len(r) else None, len(r), self.stream), "nb_set_body_forces")
+        old = self.scene.body_forces if self.scene.body_forces is not None else np.zeros(0, scenes.BODY_FORCE)
+        merged = np.concatenate([old[~np.isin(old["body"], r["body"])], r])
+        merged["reserved"] = 0
+        self._own_scene().body_forces = merged[np.argsort(merged["body"], kind="stable")]
+
+    def clear_body_forces(self):
+        """Removes the table: the step is again the one without per-body forces."""
+        self._ck(self.lib.nb_clear_body_forces(self.ctx, self.stream), "nb_clear_body_forces")
+        if self.scene.body_forces is not None:
+            self._own_scene().body_forces = None
+
+    def _own_scene(self):
+        """sim.scene, copied once so that edits of its tables do not reach the caller's Scene."""
+        if self.scene is not getattr(self, "_owned_scene", None):
+            self.scene = self._owned_scene = self.scene.copy()
+        return self.scene
+
+    def download_body_forces(self):
+        """The device's entries as scenes.BODY_FORCE rows, one per body (body = the row index); default rows without a table."""
+        n = C.c_uint32(0)
+        out = np.zeros(max(self.scene.n_bodies, 1), scenes.BODY_FORCE)
+        r = self.lib.nb_download_body_forces(self.ctx, abi.ptr(out), len(out), C.byref(n), self.stream)
+        if r == -2:   # NB_ERR_CAPACITY: *count says how many bodies there are
+            out = np.zeros(n.value, scenes.BODY_FORCE)
+            r = self.lib.nb_download_body_forces(self.ctx, abi.ptr(out), len(out), C.byref(n), self.stream)
+        self._ck(r, "nb_download_body_forces")
+        return out[:n.value].copy()
+
     # ---- spawning and despawning (nb_add_bodies, nb_remove_bodies, include/nudge_b200.h): the scene changes shape on the device ----
     def add_bodies(self, fragment, filters=None, sensors=None):
         """Appends the bodies and colliders of `fragment` (a scenes.Scene, e.g. from scenes.fragment) on the device: its bodies become
@@ -502,6 +544,11 @@ class Sim(abi.HostState):
             k = s.kinematic[keep[s.kinematic["body"].astype(np.int64)]].copy()
             k["body"] = rank[k["body"].astype(np.int64)]
             new.kinematic = k if len(k) else None
+        if s.body_forces is not None:
+            rank = (np.cumsum(keep) - 1).astype(np.uint32)
+            f = s.body_forces[keep[s.body_forces["body"].astype(np.int64)]].copy()
+            f["body"] = rank[f["body"].astype(np.int64)]
+            new.body_forces = f
         self._mirror(new)
 
     def _mirror(self, scene):

@@ -70,6 +70,11 @@ struct nb_context {
 	// (a, b) in upload order, for re-levelling after a removal; spawn_idx / urows_spare = the removal's index staging and row gather buffers
 	// conn_host = the connections as uploaded or loaded, for the removal's index checks
 	bool scene_edited, sharded; std::vector<nb_body_pair> urow_ab, conn_host; u32* spawn_idx; u32 spawn_idx_cap; nb_constraint_row* urows_spare; u32 urows_spare_cap;
+	// per-body forces (nb_set_body_forces, DESIGN.md section 8.11): frc = one entry per body while has_frc, allocated for max_bodies on the
+	// first call, together with frc_spare (nb_remove_bodies gathers into it); frc_rows = the scatter's staging rows (frc_rows_cap entries);
+	// frc_seen = the duplicate check's byte per body, all zeros between calls
+	nb_body_force* frc; nb_body_force* frc_spare; bool has_frc; nb_body_force* frc_rows; u32 frc_rows_cap; std::vector<nb_body_force> frc_host;
+	std::vector<uint8_t> frc_seen;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -174,6 +179,7 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 // The kinematic table as the kernels take it: null without a set, so that they load nothing extra.
 static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
 static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->graph_epoch; } }
+static void drop_body_forces(nb_context* ctx) { if (ctx->has_frc) { ctx->has_frc = false; ++ctx->graph_epoch; } }   // the step launches k_gravity_damping again
 
 // The velocity scatter of nb_upload_kinematic_bodies: each listed body's velocity and angular velocity into its momentum row (the unused lanes
 // are left alone), and its kind byte (the caller clears the table first when the set changes).
@@ -440,6 +446,7 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->events) cudaFree(ctx->events);
 	free_sensor_lists(ctx);
 	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
+	if (ctx->frc_rows) cudaFree(ctx->frc_rows);
 	free_impulse_rows(ctx);
 	if (ctx->spawn_idx) cudaFree(ctx->spawn_idx);
 	if (ctx->urows_spare) cudaFree(ctx->urows_spare);
@@ -456,7 +463,7 @@ int nb_lut_model_exact(const nb_context* ctx) { return ctx->lut_exact; }
 int nb_upload_bodies(nb_context* ctx, const nb_body_data* h, void* stream) {
 	NB_RANGE("nb_upload_bodies");
 	if (h->count > ctx->cfg.max_bodies) { ctx->error = "too many bodies"; return NB_ERR_CAPACITY; }
-	if (h->count != ctx->B) drop_kinematic(ctx);   // the kinematic set belongs to a body count
+	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); }   // the kinematic set and the force table belong to a body count
 	ctx->B = h->count;
 	cudaStream_t st = (cudaStream_t)stream;
 	H2D(ctx->xf, h->transforms, h->count, nb_transform); H2D(ctx->idle, h->idle_counters, h->count, uint8_t);   // all the collision stage reads
@@ -743,7 +750,11 @@ int nb_collide(nb_context* ctx, void* stream) {
 int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_apply_gravity_damping");
 	JOIN_UPLOADS();   // first reader of the momentum rows in a step
-	k_gravity_damping<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->mom, time_step, gravity, damping, ctx->counts);
+	if (ctx->has_frc)   // the per-body force table (nb_force_api.cuh): the same stage, one launch
+		k_body_forces<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->frc, ctx->xf, ctx->props, ctx->mom, ctx->idle,
+			time_step, gravity, damping, ctx->counts);
+	else
+		k_gravity_damping<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->mom, time_step, gravity, damping, ctx->counts);
 	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -1151,6 +1162,7 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 
 }
 
+#include "nb_force_api.cuh"   // before nb_state_api.cuh, whose version-5 section uses its entry checks
 #include "nb_shard_api.cuh"
 #include "nb_state_api.cuh"
 #include "nb_rows_api.cuh"

@@ -1028,6 +1028,51 @@ __global__ void __launch_bounds__(NB_BLOCK) k_gravity_damping(const u32* active_
 	}
 }
 
+// The same stage with a per-body force table (nb_set_body_forces, DESIGN.md section 8.11), launched instead of k_gravity_damping while the
+// table exists; include/nudge_b200.h states the arithmetic.  A default entry gives k_gravity_damping's bits: dv * 1 == dv, d + 0 damps like
+// d, and a zero force or torque is skipped.  The rotation and properties are read only for a body with a force or torque.
+NB_DEV bool nonzero3(float x, float y, float z) { return x != 0.0f || y != 0.0f || z != 0.0f; }   // -0.0 counts as zero
+__global__ void __launch_bounds__(NB_BLOCK) k_body_forces(const u32* active_idx, const uint8_t* kind, const nb_body_force* table, const nb_transform* xf,
+		const nb_body_properties* props, nb_body_momentum* momentum, uint8_t* idle, float time_step, float gravity, float damping_base, const u32* counts) {
+	u32 n = counts[CNT_ACTIVE];
+	float dv = gravity * time_step;
+	for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
+		u32 i = active_idx[k];
+		if (kin_is(kind, i)) continue;
+		const float4* e = reinterpret_cast<const float4*>(table + i);
+		const float4 a = e[0], b = e[1], c = e[2];   // (body, flags, gravity_scale, linear_damping), (angular_damping, force), (torque, reserved)
+		float4* p = reinterpret_cast<float4*>(momentum + i);
+		float4 l = p[0], w = p[1];
+		l.y = l.y - dv * a.z;
+		const bool has_f = nonzero3(b.y, b.z, b.w), has_t = nonzero3(c.x, c.y, c.z);
+		if (has_f || has_t) {
+			const bool local = (asu(a.y) & NB_BODY_FORCE_LOCAL) != 0;
+			const float4 q = reinterpret_cast<const float4*>(xf + i)[1];
+			const float4 pr = reinterpret_cast<const float4*>(props)[i];
+			if (has_f) {
+				f3 f = mk3(b.y, b.z, b.w);
+				if (local) f = qrot(mkq(q), f);
+				const float m = pr.w * time_step;
+				l.x = l.x + f.x * m; l.y = l.y + f.y * m; l.z = l.z + f.z * m;
+			}
+			if (has_t) {
+				f3 t = mk3(c.x, c.y, c.z);
+				if (local) t = qrot(mkq(q), t);
+				float3 Wd, Wo;
+				world_inverse_inertia(q, pr, Wd, Wo);
+				w.x = w.x + ((Wd.x*t.x + Wo.x*t.y) + Wo.y*t.z) * time_step;
+				w.y = w.y + ((Wo.x*t.x + Wd.y*t.y) + Wo.z*t.z) * time_step;
+				w.z = w.z + ((Wo.y*t.x + Wo.z*t.y) + Wd.z*t.z) * time_step;
+			}
+			idle[i] = 0;
+		}
+		const float lin = 1.0f - time_step * (damping_base + a.w), ang = 1.0f - time_step * (damping_base + b.x);
+		l.x *= lin; l.y *= lin; l.z *= lin;
+		w.x *= ang; w.y *= ang; w.z *= ang;
+		p[0] = l; p[1] = w;
+	}
+}
+
 __global__ void __launch_bounds__(NB_BLOCK) k_advance(const u32* active_idx, nb_transform* xf, const nb_body_momentum* momentum, uint8_t* idle, float time_step, const u32* counts) {
 	u32 n = counts[CNT_ACTIVE];
 	float half_time_step = 0.5f * time_step;

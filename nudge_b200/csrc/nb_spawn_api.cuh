@@ -3,7 +3,7 @@
 //
 // A reference application spawns or despawns a body by editing its caller-owned arrays between two steps.  Here those arrays live in HBM,
 // together with tables that hold body and collider indices (connections, filters, sensors, the kinematic set, user rows, the sensor overlap
-// lists), so the edit runs on the device and gives the bits that host edit followed by a re-upload gives (include/nudge_b200.h states it).
+// lists, the body force table), so the edit runs on the device and gives the bits that host edit followed by a re-upload gives (include/nudge_b200.h states it).
 //
 // Add is copies only: the new rows go to the ends of their arrays, and the filter / sensor entries of the existing spheres move up by the
 // number of added boxes through a staging copy.
@@ -13,7 +13,8 @@
 //                    the colliders' (tag, body, removed) keys; the connection half of the wake set
 //   nb_radix_sort    of those keys; k_spawn_wake then binary-searches both tags of every cache entry: the other side of a removed tag wakes
 //   nb_scan_reduce + k_spawn_bodies / k_spawn_colliders / k_spawn_conns: the fused scan ranks each array once, and its consumer gathers the
-//                    kept rows out of place into collide-stage scratch (the body gather also writes the old -> new map)
+//                    kept rows out of place into collide-stage scratch (the body gather also writes the old -> new map, and moves the
+//                    body force rows into frc_spare)
 //   k_spawn_rows     the kept user rows, by a host-computed permutation that re-levels them (nb_rows_api.cuh, level_rows)
 //   k_spawn_overlaps the sensor overlap lists' bodies through the map
 // then one synchronise for the new counts and largest tag, and device-to-device copies back.  No float atomics; the one atomic is a u32 max.
@@ -83,9 +84,10 @@ __global__ void __launch_bounds__(NB_BLOCK) k_spawn_wake(const u64* cache_tags, 
 }
 
 // Launched with NB_SCAN_GRID blocks after nb_scan_reduce<1> over the body flags.  map[i] = the new index of body i, or NB_REMOVED_BODY.
+// With a body force table (frc non-null) its rows move too, their body field rewritten to the new index.
 __global__ void __launch_bounds__(NB_BLOCK) k_spawn_bodies(u32 B, const u32* flags, const u32* block_sums, const nb_transform* xf, const nb_body_properties* props,
-		const nb_body_momentum* mom, const uint8_t* idle, const uint8_t* kind, nb_transform* xf_out, float4* props_out, float4* mom_out, uint8_t* idle_out,
-		uint8_t* kind_out, u32* map) {
+		const nb_body_momentum* mom, const uint8_t* idle, const uint8_t* kind, const nb_body_force* frc, nb_transform* xf_out, float4* props_out, float4* mom_out,
+		uint8_t* idle_out, uint8_t* kind_out, nb_body_force* frc_out, u32* map) {
 	scan_consume<1>(flags, 0, B, block_sums, [&](u32 i, const u32 (&v)[1], const u32 (&off)[1]) {
 		if (!v[0]) { map[i] = NB_REMOVED_BODY; return; }
 		const u32 d = off[0];
@@ -95,6 +97,13 @@ __global__ void __launch_bounds__(NB_BLOCK) k_spawn_bodies(u32 B, const u32* fla
 		mom_out[2 * d] = m[0]; mom_out[2 * d + 1] = m[1];
 		idle_out[d] = idle[i];
 		if (kind) kind_out[d] = kind[i];
+		if (frc) {
+			const float4* e = reinterpret_cast<const float4*>(frc + i);
+			float4* o = reinterpret_cast<float4*>(frc_out + d);
+			float4 a = e[0];
+			a.x = asf(d);
+			o[0] = a; o[1] = e[1]; o[2] = e[2];
+		}
 		map[i] = d;
 	});
 }
@@ -234,8 +243,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	// bodies: xf -> mw, properties -> inertia, idle -> taint, kind -> active (each rewritten by the step before it is read: k_mw_in, k_inertia,
 	// k_uf_init); momentum -> jd, the throughput solver's accumulator, which must be all zeros between passes and is cleared after the copy back
 	nb_scan_reduce<1>(L, flags, S, nullptr, B, ctx->block_sums, counts + CNT_SPAWN_B);
-	k_spawn_bodies<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(B, flags, ctx->block_sums, ctx->xf, ctx->props, ctx->mom, ctx->idle, ctx->kind,
-		reinterpret_cast<nb_transform*>(ctx->mw), ctx->inertia, ctx->jd, reinterpret_cast<uint8_t*>(ctx->taint), reinterpret_cast<uint8_t*>(ctx->active), map);
+	k_spawn_bodies<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(B, flags, ctx->block_sums, ctx->xf, ctx->props, ctx->mom, ctx->idle, ctx->kind, ctx->has_frc ? ctx->frc : nullptr,
+		reinterpret_cast<nb_transform*>(ctx->mw), ctx->inertia, ctx->jd, reinterpret_cast<uint8_t*>(ctx->taint), reinterpret_cast<uint8_t*>(ctx->active), ctx->frc_spare, map);
 	++ctx->launches;
 	// colliders, by table index: tags -> col_tag, transforms -> world_xf, filter -> order, sensor -> rank; box data -> aabb_min, radii -> col_body
 	if (K) {
@@ -264,6 +273,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	CK(d2d(ctx->mom, ctx->jd, sizeof(nb_body_momentum) * (size_t)B2)); CK(d2d(ctx->idle, ctx->taint, B2));
 	CK(cudaMemsetAsync(ctx->jd, 0, sizeof(nb_body_momentum) * (size_t)B2, st));
 	if (ctx->kind) { CK(d2d(ctx->kind, ctx->active, B2)); CK(cudaMemsetAsync(ctx->kind + B2, 0, B - B2, st)); }   // bodies added later are dynamic
+	if (ctx->has_frc) CK(d2d(ctx->frc, ctx->frc_spare, sizeof(nb_body_force) * (size_t)B2));
 	CK(d2d(ctx->box_tags, ctx->col_tag, 4 * (size_t)nb2)); CK(d2d(ctx->sph_tags, ctx->col_tag + nb2, 4 * (size_t)ns2));
 	CK(d2d(ctx->box_xf, ctx->world_xf, sizeof(nb_transform) * (size_t)nb2)); CK(d2d(ctx->sph_xf, ctx->world_xf + nb2, sizeof(nb_transform) * (size_t)ns2));
 	CK(d2d(ctx->box_data, ctx->aabb_min, sizeof(nb_box_collider) * (size_t)nb2)); CK(d2d(ctx->sph_data, ctx->col_body, sizeof(nb_sphere_collider) * (size_t)ns2));
@@ -326,6 +336,11 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 	CK(put(ctx->mom + B0, bodies ? bodies->momentum : nullptr, sizeof(nb_body_momentum) * (size_t)n));
 	CK(put(ctx->idle + B0, bodies ? bodies->idle_counters : nullptr, (size_t)n));
 	if (ctx->kind && n) CK(cudaMemsetAsync(ctx->kind + B0, 0, n, st));   // new bodies are dynamic
+	std::vector<nb_body_force> frc;   // with the default force entry
+	if (ctx->has_frc && n) {
+		for (u32 i = 0; i < n; ++i) frc.push_back(default_body_force(B0 + i));
+		CK(put(ctx->frc + B0, frc.data(), sizeof(nb_body_force) * (size_t)n));
+	}
 	const u32 ob = ctx->nboxes, os = ctx->nspheres;
 	if (nb) {
 		CK(put(ctx->box_tags + ob, colliders->boxes.tags, 4 * (size_t)nb)); CK(put(ctx->box_data + ob, colliders->boxes.data, sizeof(nb_box_collider) * (size_t)nb));

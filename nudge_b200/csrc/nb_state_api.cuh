@@ -14,10 +14,12 @@
 //   filter (category | mask << 16)                 4            boxes + spheres  reserved[1] != 0
 //   sensor (0 or 1)                                1            boxes + spheres  reserved[2] != 0
 //   kinematic (body indices, ascending)            4            reserved[4]      reserved[4] != 0
+//   body forces (nb_body_force rows, body = row)   48           bodies           reserved[5] != 0
 // Each version defines more reserved words: version 2 reserved[0] = filter flags and reserved[1]; version 3 reserved[2] = 1 and
-// reserved[3] = max_sensor_pairs; version 4 reserved[2] = 0 or 1 and reserved[4] >= 1.  A context writes version 4 with a kinematic set,
-// else 3 with sensors, else 2 with a filter table or flags, else 1.  Every version loads; words a version does not define are ignored, and
-// a file without a table or flags removes the context's.  A kinematic body's velocities are its momentum row.
+// reserved[3] = max_sensor_pairs; version 4 reserved[2] = 0 or 1 and reserved[4] >= 1; version 5 reserved[2] = 0 or 1, reserved[4] >= 0 and
+// reserved[5] = 1.  A context writes version 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
+// filter table or flags, else 1.  Every version loads; words a version does not define are ignored, and a file without a table or flags
+// removes the context's.  A kinematic body's velocities are its momentum row.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
@@ -29,17 +31,19 @@ static bool state_header_read(FILE* f, NbStateHeader& h) {
 	if (h.version < 2) h.reserved[0] = h.reserved[1] = 0;
 	if (h.version < 3) h.reserved[2] = h.reserved[3] = 0;
 	if (h.version < 4) h.reserved[4] = 0;
-	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1);
+	if (h.version < 5) h.reserved[5] = 0;
+	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1) ||
+		   (h.version == 5 && h.reserved[2] <= 1 && h.reserved[5] == 1);
 }
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
 // `host` when it is given and then copies to `dev` when that is given.
 struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; };
-struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin; };
+struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc; };
 
 // The sections of the file with header `h`, in file order.  A load keeps in `hc` the momentum rows (the kinematic velocities), the tags
-// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors) and the kinematic indices; a save writes the
-// kinematic indices from hc.kin.
+// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices and the body force rows (checked
+// before they are copied to the device); a save writes the kinematic indices from hc.kin.
 static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, StateHostCopies& hc, bool load) {
 	const size_t K = (size_t)h.boxes + h.spheres;
 	return {
@@ -54,6 +58,7 @@ static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHe
 		{ ctx->filter, nullptr, 4, K, h.reserved[1] != 0 },
 		{ load ? nullptr : ctx->sensor, &hc.sensor, 1, K, h.reserved[2] != 0 },
 		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0 },
+		{ load ? nullptr : ctx->frc, &hc.frc, sizeof(nb_body_force), h.bodies, h.reserved[5] != 0 },
 	};
 }
 
@@ -89,10 +94,11 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
+	if (ctx->has_frc) h.reserved[5] = 1;
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = c[CNT_CACHE]; h.solver_mode = (u32)ctx->solver_mode;
 	StateHostCopies hc;
 	const unsigned char* kin = reinterpret_cast<const unsigned char*>(ctx->kin_list.data());
@@ -147,6 +153,9 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 		memset(&kin[i], 0, sizeof(kin[i])); kin[i].body = idx[i];
 		for (int c = 0; c < 3; ++c) { kin[i].velocity[c] = mom[idx[i]].velocity[c]; kin[i].angular_velocity[c] = mom[idx[i]].angular_velocity[c]; }
 	}
+	// the body force rows: each names its own row and passes nb_set_body_forces' entry checks
+	const nb_body_force* frc = reinterpret_cast<const nb_body_force*>(hc.frc.data());
+	for (u32 i = 0; ok && h.reserved[5] && i < h.bodies; ++i) ok = frc[i].body == i && !body_force_problem(frc[i]);
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->B = h.bodies; ctx->nboxes = h.boxes; ctx->nspheres = h.spheres; ctx->nconn = h.connections;
@@ -164,6 +173,11 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	// the scatter rewrites the loaded momentum rows with their own values
 	drop_kinematic(ctx);
 	if (!kin.empty()) { int r = nb_upload_kinematic_bodies(ctx, kin.data(), (u32)kin.size(), st); if (r) return r; }
+	drop_body_forces(ctx);
+	if (h.reserved[5]) {
+		{ int r = ensure_body_forces(ctx, st); if (r) return r; }
+		CK(cudaMemcpyAsync(ctx->frc, frc, sizeof(nb_body_force) * (size_t)h.bodies, cudaMemcpyHostToDevice, st));
+	}
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }

@@ -37,10 +37,24 @@ KINEMATIC = np.dtype([("body", "<u4"), ("velocity", "<f4", 3), ("angular_velocit
 # explosion over every body whose position lies inside the sphere
 BODY_IMPULSE = np.dtype([("body", "<u4"), ("offset", "<f4", 3), ("impulse", "<f4", 3), ("angular_impulse", "<f4", 3), ("reserved", "<u4", 2)])
 RADIAL_IMPULSE = np.dtype([("center", "<f4", 3), ("radius", "<f4"), ("impulse", "<f4"), ("reserved", "<u4", 3)])
+# nb_body_force (include/nudge_b200.h): one body's gravity scale, extra damping and constant force and torque, applied inside the step;
+# BODY_FORCE_LOCAL: force and torque are in the body frame
+BODY_FORCE = np.dtype([("body", "<u4"), ("flags", "<u4"), ("gravity_scale", "<f4"), ("linear_damping", "<f4"), ("angular_damping", "<f4"),
+                       ("force", "<f4", 3), ("torque", "<f4", 3), ("reserved", "<u4")])
+BODY_FORCE_LOCAL = 1
 
 assert TRANSFORM.itemsize == 32 and MOMENTUM.itemsize == 32 and CONTACT.itemsize == 32 and CONTACT_EVENT.itemsize == 80 and FILTER.itemsize == 4 and SENSOR_OVERLAP.itemsize == 16
 assert KINEMATIC.itemsize == 32
 assert BODY_IMPULSE.itemsize == 48 and RADIAL_IMPULSE.itemsize == 32
+assert BODY_FORCE.itemsize == 48
+
+
+def default_body_forces(bodies):
+    """BODY_FORCE rows with the default entry (gravity scale 1, everything else 0) for the given body indices."""
+    b = np.asarray(bodies, np.uint32).reshape(-1)
+    r = np.zeros(len(b), BODY_FORCE)
+    r["body"] = b; r["gravity_scale"] = 1.0
+    return r
 
 
 class Scene:
@@ -68,6 +82,8 @@ class Scene:
         self.sensors = None
         # optional kinematic bodies: KINEMATIC rows (body, velocity, angular velocity) or None
         self.kinematic = None
+        # optional per-body forces: BODY_FORCE rows (one per listed body; every other body has the default entry) or None for no table
+        self.body_forces = None
         # step parameters the reference leaves to the caller (example/main.cpp:275-305)
         self.time_step = np.float32(1.0 / 120.0)
         self.iterations = 8
