@@ -23,6 +23,7 @@
  *   nb_apply_radial_impulse         <- no reference counterpart: the application's edit of BodyData between calls
  *   nb_add_bodies / nb_remove_bodies <- no reference counterpart: the application's edit of its caller-owned arrays between steps
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
+ *   nb_snapshot_*                   <- no reference counterpart: the application's copy of its caller-owned arrays, kept in HBM
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -435,6 +436,35 @@ int nb_stream_synchronize(nb_context*, void* stream);
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);
+
+/* Device-resident snapshots (DESIGN.md section 8.12): the whole between-steps state in HBM, saved cheaply enough to do every step and restored
+ * bit for bit, so that re-stepping with the same inputs repeats the run byte for byte (rollback netcode, resets, what-if planning).
+ * A snapshot holds what the next nb_collide / nb_step and everything after it depend on: bodies (transforms, properties, momentum with its
+ * unused lanes, idle counters); boxes and spheres (tags, data, transforms); connections; the contact cache (as many entries as the device count
+ * says); the filter table, its flags and the NB_FILTER_SKIP_CONNECTED key list; the sensor table, max_sensor_pairs and the sensor overlap list
+ * as of the last nb_write_cached_impulses; the kinematic set and its kind bytes; the body force table; the user constraint rows with their
+ * accumulated impulses and their levelling; the solver mode; the contact-event step counter; the body, collider and connection counts and the
+ * tag and key bits.  It does not hold whether contact events are enabled, the undrained events, or the outputs of the last nb_collide.
+ *
+ * nb_snapshot_create allocates device memory for the context's capacities (DESIGN.md section 8.12 gives the bytes); nb_snapshot_destroy frees
+ * it, and nb_destroy frees a context's remaining snapshots (their handles are then invalid).
+ * nb_snapshot_save is legal between steps and after nb_add_bodies / nb_remove_bodies; between nb_collide and the nb_advance that ends its step
+ * it is NB_ERR_ARGUMENT.  It is asynchronous on `stream`, ordered after a pending nb_upload_bodies copy, and is ONE kernel launch with no
+ * synchronisation and no allocation, so it can be captured into the application's CUDA graph (the counts, bits and table set it records are
+ * those at capture time).  The user rows and the sensor overlap list are sized at the save: a save that finds them grown beyond the snapshot's
+ * room grows it, synchronises and allocates, and cannot be captured.
+ * nb_snapshot_restore makes the context what it was at the save, bit for bit: tables that exist now and did not then are removed, missing
+ * ones are created.  nb_download_sensor_overlaps then returns the overlap list of the save, and the stage calls that read the last collide's
+ * outputs are refused until the next nb_collide or nb_step, as after nb_add_bodies.  With every table already allocated it is one kernel
+ * launch and host bookkeeping, without synchronisation.  nb_step keeps its graph when the step's launches and their arguments are unchanged:
+ * the same counts, tag and key bits, table set, kinematic set and user-row set; otherwise it re-records once.
+ * NB_ERR_ARGUMENT, changing nothing: a snapshot of another context, restoring a snapshot that was never saved, a context that nb_shard_create
+ * was called on. */
+typedef struct nb_snapshot nb_snapshot;
+int nb_snapshot_create(nb_context*, nb_snapshot** out);
+void nb_snapshot_destroy(nb_snapshot*);
+int nb_snapshot_save(nb_context*, nb_snapshot*, void* stream);
+int nb_snapshot_restore(nb_context*, const nb_snapshot*, void* stream);
 
 /* Renderer read-back (SURVEY.md section 8 f4; replaces the per-collider host loop of example/main.cpp:224-268 with its helpers at :53-110):
  * one column-major 4x4 model matrix (16 floats) per collider, boxes first, then spheres; rotation = body * collider, translation =

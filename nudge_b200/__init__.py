@@ -25,7 +25,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_enable_contact_events", "nb_download_contact_events", "nb_upload_collision_filters",
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
-           "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces"]
+           "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
+           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore"]
 
 
 class Config(C.Structure):
@@ -113,6 +114,10 @@ def load_library():
         lib.nb_set_body_forces.argtypes = [V, V, C.c_uint32, V]
         lib.nb_clear_body_forces.argtypes = [V, V]
         lib.nb_download_body_forces.argtypes = [V, V, C.c_uint32, V, V]
+        lib.nb_snapshot_create.argtypes = [V, V]
+        lib.nb_snapshot_destroy.argtypes = [V]; lib.nb_snapshot_destroy.restype = None
+        lib.nb_snapshot_save.argtypes = [V, V, V]
+        lib.nb_snapshot_restore.argtypes = [V, V, V]
         _lib = lib
     return _lib
 
@@ -123,6 +128,29 @@ class SpawnTables(C.Structure):
 
 class NudgeError(RuntimeError):
     pass
+
+
+class Snapshot:
+    """A device-resident snapshot of one Sim (nb_snapshot_*, include/nudge_b200.h): its handle, and the Sim's scene as of the last save.
+    Sim.snapshot() makes one; Sim.snapshot(into=snap) saves into an existing one, Sim.restore(snap) goes back to it.  Freed by close(), when
+    collected, or with its Sim."""
+
+    def __init__(self, sim):
+        self.sim = sim
+        self.handle = C.c_void_p()
+        self.scene = None
+        sim._ck(sim.lib.nb_snapshot_create(sim.ctx, C.byref(self.handle)), "nb_snapshot_create")
+
+    def close(self):
+        if self.handle and self.sim.ctx:   # a closed Sim has freed its snapshots (nb_destroy)
+            self.sim.lib.nb_snapshot_destroy(self.handle)
+        self.handle = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 # nb_constraint_row (80 bytes)
@@ -601,6 +629,24 @@ class Sim(abi.HostState):
         if r != -4:   # NB_ERR_OVERFLOW fills the outputs: the caller reads `dropped`
             self._ck(r, "nb_download_contact_events")
         return out[:n.value].copy(), int(dropped.value)
+
+    # ---- device-resident snapshots (nb_snapshot_save / nb_snapshot_restore, include/nudge_b200.h): rollback and re-simulation ----
+    def snapshot(self, into=None):
+        """Saves the whole between-steps state into a Snapshot in HBM (a new one, or `into`) and returns it: one kernel launch, no
+        synchronisation.  The snapshot keeps a reference to sim.scene; the next edit of the scene copies it instead of changing it in place."""
+        snap = into if into is not None else Snapshot(self)
+        self._ck(self.lib.nb_snapshot_save(self.ctx, snap.handle, self.stream), "nb_snapshot_save")
+        snap.scene = self.scene
+        self._owned_scene = None   # shared with the snapshot from here on: _own_scene copies before the next edit
+        return snap
+
+    def restore(self, snap):
+        """Makes the device state what it was at `snap`'s save, bit for bit.  sim.scene and the host mirrors become those of the save; the
+        stage calls that read the last collide's outputs are refused until the next collide() or step()."""
+        self._ck(self.lib.nb_snapshot_restore(self.ctx, snap.handle, self.stream), "nb_snapshot_restore")
+        if snap.scene is not self.scene:
+            self._mirror(snap.scene)
+        self._owned_scene = None
 
     # ---- state files (nb_save_state / nb_load_state; tools/nb_replay steps them headless) ----
     def save_state(self, path):

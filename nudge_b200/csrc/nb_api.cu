@@ -75,6 +75,9 @@ struct nb_context {
 	// frc_seen = the duplicate check's byte per body, all zeros between calls
 	nb_body_force* frc; nb_body_force* frc_spare; bool has_frc; nb_body_force* frc_rows; u32 frc_rows_cap; std::vector<nb_body_force> frc_host;
 	std::vector<uint8_t> frc_seen;
+	// snapshots (nb_snapshot_save / nb_snapshot_restore, DESIGN.md section 8.12): in_step = between nb_collide and the nb_advance that ends its
+	// step, where a save is refused; the context's snapshots, freed by nb_destroy; graph_records = captures of a step graph (nb_debug_read)
+	bool in_step; std::vector<nb_snapshot*> snapshots; unsigned long long graph_records;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -132,6 +135,7 @@ struct NbRange { NbRange(const char* name) { nvtxRangePushA(name); } ~NbRange() 
 #define NB_RANGE(name) NbRange nb_range_(name)
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb_rows_api.cuh
 static void free_impulse_rows(nb_context* ctx);                            // nb_impulse_api.cuh
+static void free_snapshots(nb_context* ctx);                               // nb_snapshot_api.cuh
 // The stage calls that read the last nb_collide's outputs: refused after nb_add_bodies / nb_remove_bodies until the next collide
 #define NOT_AFTER_EDIT() do { if (ctx->scene_edited) { ctx->error = "the scene was edited (nb_add_bodies / nb_remove_bodies) since the last nb_collide"; return NB_ERR_ARGUMENT; } } while (0)
 
@@ -211,6 +215,7 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 		if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 		if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
 			const unsigned long long before = ctx->launches;
+			++ctx->graph_records;
 			ctx->capturing = true;
 			int r = body();
 			ctx->capturing = false;
@@ -261,6 +266,18 @@ static void free_sensor_lists(nb_context* ctx) {
 	ctx->sensor_keys = nullptr; ctx->sensor_sb.keys[0] = ctx->sensor_sb.keys[1] = nullptr; ctx->sensor_sb.vals[0] = ctx->sensor_sb.vals[1] = nullptr;
 	ctx->sensor_cur = ctx->sensor_old = nullptr; ctx->sensor_alloc = 0;
 }
+// The candidate keys, sort buffers and overlap lists with room for `cap` entries (reallocated only when they are smaller).
+static int ensure_sensor_lists(nb_context* ctx, u32 cap) {
+	if (cap > ctx->sensor_alloc) {
+		free_sensor_lists(ctx);
+		CK(cudaMalloc(&ctx->sensor_keys, sizeof(u64) * (size_t)cap));
+		for (int i = 0; i < 2; ++i) { CK(cudaMalloc(&ctx->sensor_sb.keys[i], sizeof(u64) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_sb.vals[i], sizeof(u32) * (size_t)cap)); }
+		CK(cudaMalloc(&ctx->sensor_cur, sizeof(uint4) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_old, sizeof(uint4) * (size_t)cap));
+		ctx->sensor_alloc = cap;
+	}
+	ctx->sensor_sb.hist = ctx->sb.hist; ctx->sensor_sb.bar = ctx->sb.bar;
+	return NB_OK;
+}
 static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pairs, cudaStream_t st) {
 	CK(cudaStreamSynchronize(st));
 	u32 cap = 0;
@@ -273,14 +290,7 @@ static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pair
 			ctx->error = "max_sensor_pairs exceeds the context's scratch capacity (" + std::to_string(ctx->stride) + ": the largest of max_pairs, max_contacts, bodies, colliders)";
 			return NB_ERR_CAPACITY;
 		}
-		if (cap > ctx->sensor_alloc) {
-			free_sensor_lists(ctx);
-			CK(cudaMalloc(&ctx->sensor_keys, sizeof(u64) * (size_t)cap));
-			for (int i = 0; i < 2; ++i) { CK(cudaMalloc(&ctx->sensor_sb.keys[i], sizeof(u64) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_sb.vals[i], sizeof(u32) * (size_t)cap)); }
-			CK(cudaMalloc(&ctx->sensor_cur, sizeof(uint4) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_old, sizeof(uint4) * (size_t)cap));
-			ctx->sensor_alloc = cap;
-		}
-		ctx->sensor_sb.hist = ctx->sb.hist; ctx->sensor_sb.bar = ctx->sb.bar;
+		{ int r = ensure_sensor_lists(ctx, cap); if (r) return r; }
 		CK(cudaMemcpyAsync(ctx->sensor, f.data(), n, cudaMemcpyHostToDevice, st));
 	}
 	CK(cudaMemsetAsync(ctx->counts + CNT_SENSOR_PAIRS, 0, 3 * sizeof(u32), st));   // candidates, current and old overlaps
@@ -445,6 +455,7 @@ void nb_destroy(nb_context* ctx) {
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
 	if (ctx->events) cudaFree(ctx->events);
 	free_sensor_lists(ctx);
+	free_snapshots(ctx);
 	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
 	if (ctx->frc_rows) cudaFree(ctx->frc_rows);
 	free_impulse_rows(ctx);
@@ -667,6 +678,7 @@ int nb_download_cache(nb_context* ctx, nb_contact_cache* h, void* stream) {
 int nb_collide(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_collide");
 	ctx->scene_edited = false;
+	ctx->in_step = true;   // until the nb_advance that ends the step
 	Launch L = mk_launch(ctx, stream);
 	cudaStream_t st = L.stream;
 	const u32 K = ctx->nboxes + ctx->nspheres, B = ctx->B, nboxes = ctx->nboxes;
@@ -1007,6 +1019,7 @@ int nb_advance(nb_context* ctx, float time_step, void* stream) {
 	JOIN_UPLOADS();
 	k_advance<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts);
 	++ctx->launches;
+	ctx->in_step = false;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -1032,8 +1045,10 @@ int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
 	ctx->scene_edited = false;     // the step begins with nb_collide (also when its graph is replayed)
-	return run_graphed(ctx, ctx->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, 0, 0,
-					   [&] { return step_body(ctx, time_step, iterations, gravity, damping, stream); });
+	const int r = run_graphed(ctx, ctx->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, 0, 0,
+							  [&] { return step_body(ctx, time_step, iterations, gravity, damping, stream); });
+	if (r == NB_OK) ctx->in_step = false;   // the step ended with nb_advance (also when its graph was replayed)
+	return r;
 }
 
 // ---------------- streams for hosts that do not link the CUDA runtime themselves ----------------
@@ -1103,6 +1118,8 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }
+	// how many times a step graph (nb_step, nb_shard_step) was captured since nb_create
+	if (!strcmp(name, "graph_records")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)ctx->graph_records; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
@@ -1169,3 +1186,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_render_api.cuh"
 #include "nb_impulse_api.cuh"
 #include "nb_spawn_api.cuh"
+#include "nb_snapshot_api.cuh"

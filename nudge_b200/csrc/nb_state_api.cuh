@@ -37,29 +37,93 @@ static bool state_header_read(FILE* f, NbStateHeader& h) {
 }
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
-// `host` when it is given and then copies to `dev` when that is given.
-struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; };
+// `host` when it is given and then copies to `dev` when that is given.  word >= 0: a context holds the element count in counts[word] (a
+// file holds it in the header; a snapshot copies it on the device, nb_snapshot_api.cuh).
+struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; int word; };
 struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc; };
 
 // The sections of the file with header `h`, in file order.  A load keeps in `hc` the momentum rows (the kinematic velocities), the tags
 // (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices and the body force rows (checked
-// before they are copied to the device); a save writes the kinematic indices from hc.kin.
+// before they are copied to the device); a save writes the kinematic indices from hc.kin.  Snapshots extend this list (snapshot_sections).
 static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, StateHostCopies& hc, bool load) {
 	const size_t K = (size_t)h.boxes + h.spheres;
 	return {
-		{ ctx->xf, nullptr, sizeof(nb_transform), h.bodies, true }, { ctx->props, nullptr, sizeof(nb_body_properties), h.bodies, true },
-		{ ctx->mom, &hc.mom, sizeof(nb_body_momentum), h.bodies, true }, { ctx->idle, nullptr, 1, h.bodies, true },
-		{ ctx->box_tags, &hc.box_tags, 4, h.boxes, true }, { ctx->box_data, nullptr, sizeof(nb_box_collider), h.boxes, true },
-		{ ctx->box_xf, nullptr, sizeof(nb_transform), h.boxes, true },
-		{ ctx->sph_tags, &hc.sph_tags, 4, h.spheres, true }, { ctx->sph_data, nullptr, sizeof(nb_sphere_collider), h.spheres, true },
-		{ ctx->sph_xf, nullptr, sizeof(nb_transform), h.spheres, true },
-		{ ctx->conn, &hc.conn, sizeof(nb_body_pair), h.connections, true },
-		{ ctx->cache_tags, nullptr, 8, h.cache, true }, { ctx->cache_features, nullptr, 4, h.cache, true }, { ctx->cache_data, nullptr, 16, h.cache, true },
-		{ ctx->filter, nullptr, 4, K, h.reserved[1] != 0 },
-		{ load ? nullptr : ctx->sensor, &hc.sensor, 1, K, h.reserved[2] != 0 },
-		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0 },
-		{ load ? nullptr : ctx->frc, &hc.frc, sizeof(nb_body_force), h.bodies, h.reserved[5] != 0 },
+		{ ctx->xf, nullptr, sizeof(nb_transform), h.bodies, true, -1 }, { ctx->props, nullptr, sizeof(nb_body_properties), h.bodies, true, -1 },
+		{ ctx->mom, &hc.mom, sizeof(nb_body_momentum), h.bodies, true, -1 }, { ctx->idle, nullptr, 1, h.bodies, true, -1 },
+		{ ctx->box_tags, &hc.box_tags, 4, h.boxes, true, -1 }, { ctx->box_data, nullptr, sizeof(nb_box_collider), h.boxes, true, -1 },
+		{ ctx->box_xf, nullptr, sizeof(nb_transform), h.boxes, true, -1 },
+		{ ctx->sph_tags, &hc.sph_tags, 4, h.spheres, true, -1 }, { ctx->sph_data, nullptr, sizeof(nb_sphere_collider), h.spheres, true, -1 },
+		{ ctx->sph_xf, nullptr, sizeof(nb_transform), h.spheres, true, -1 },
+		{ ctx->conn, &hc.conn, sizeof(nb_body_pair), h.connections, true, -1 },
+		{ ctx->cache_tags, nullptr, 8, h.cache, true, CNT_CACHE }, { ctx->cache_features, nullptr, 4, h.cache, true, CNT_CACHE },
+		{ ctx->cache_data, nullptr, 16, h.cache, true, CNT_CACHE },
+		{ ctx->filter, nullptr, 4, K, h.reserved[1] != 0, -1 },
+		{ load ? nullptr : ctx->sensor, &hc.sensor, 1, K, h.reserved[2] != 0, -1 },
+		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0, -1 },
+		{ load ? nullptr : ctx->frc, &hc.frc, sizeof(nb_body_force), h.bodies, h.reserved[5] != 0, -1 },
 	};
+}
+
+// The header a save of the context writes, with `cache` cache entries.
+static NbStateHeader state_header_of(const nb_context* ctx, u32 cache) {
+	NbStateHeader h; memset(&h, 0, sizeof(h));
+	memcpy(h.magic, "NBSTATE1", 8);
+	const bool filtered = ctx->has_filter || ctx->filter_flags;
+	h.version = ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
+	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
+	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
+	if (ctx->has_frc) h.reserved[5] = 1;
+	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = cache; h.solver_mode = (u32)ctx->solver_mode;
+	return h;
+}
+
+// The host side of a state that replaces the context's (nb_load_state, nb_snapshot_restore): the counts, the connections' host copy, the tag
+// and key bits, the solver mode and the table set.  sensor_cap is max_sensor_pairs as the state gives it (0 in a file: the default).
+struct StateShape {
+	u32 B, nboxes, nspheres, nconn, tagbits, kbits, solver_mode, filter_flags, sensor_cap;
+	bool has_filter, has_sensor, has_frc;
+	std::vector<nb_body_pair> conn; std::vector<u32> kin;
+};
+static StateShape state_shape_of(const nb_context* ctx) {
+	return { ctx->B, ctx->nboxes, ctx->nspheres, ctx->nconn, ctx->tagbits, ctx->kbits, (u32)ctx->solver_mode, ctx->filter_flags, ctx->has_sensor ? ctx->sensor_cap : 0,
+			 ctx->has_filter, ctx->has_sensor, ctx->has_frc, ctx->conn_host, ctx->kin_list };
+}
+// A load's tables, from the file's host copies: the sensor flags (boxes + spheres of them while has_sensor), the kinematic rows (one per
+// entry of StateShape::kin, with the loaded velocities) and the body force rows (B while has_frc).
+struct StateFileTables { const uint8_t* sensor; const nb_kinematic_body* kin; const nb_body_force* frc; };
+
+// Installs `s` in place of the context's shape.  A load (`file` non-null) rebuilds the tables on the device from the file's host copies and
+// re-records nb_step's graph.  A restore finds the table contents already copied to the device and re-records only when the table set or the
+// kinematic set changes (the graph's key holds the counts, the bits and the solver mode).
+static int install_state(nb_context* ctx, StateShape& s, const StateFileTables* file, cudaStream_t st) {
+	const bool same_tables = s.has_filter == ctx->has_filter && s.filter_flags == ctx->filter_flags && s.has_sensor == ctx->has_sensor &&
+							 (!s.has_sensor || s.sensor_cap == ctx->sensor_cap) && s.kin == ctx->kin_list && s.has_frc == ctx->has_frc;
+	ctx->B = s.B; ctx->nboxes = s.nboxes; ctx->nspheres = s.nspheres; ctx->nconn = s.nconn;
+	ctx->conn_host.swap(s.conn);
+	ctx->tagbits = s.tagbits; ctx->kbits = s.kbits;
+	if (s.solver_mode == NB_SOLVER_PARITY || s.solver_mode == NB_SOLVER_THROUGHPUT) ctx->solver_mode = (int)s.solver_mode;
+	ctx->has_filter = s.has_filter; ctx->filter_flags = s.filter_flags;
+	if (!file) {
+		if (!same_tables) ++ctx->graph_epoch;
+		ctx->conn_probe = (ctx->filter_flags & NB_FILTER_SKIP_CONNECTED) ? ctx->nconn : 0;   // the key list itself was copied
+		ctx->has_sensor = s.has_sensor; ctx->sensor_cap = s.has_sensor ? s.sensor_cap : 0;
+		ctx->has_kin = !s.kin.empty(); ctx->kin_list.swap(s.kin);
+		ctx->has_frc = s.has_frc;
+		return NB_OK;
+	}
+	++ctx->graph_epoch;
+	{ int r = build_conn_lookup(ctx, st); if (r) return r; }
+	{ int r = set_sensors(ctx, file->sensor, s.has_sensor ? s.nboxes + s.nspheres : 0, s.sensor_cap, st); if (r) return r; }
+	// the scatter rewrites the loaded momentum rows with their own values
+	drop_kinematic(ctx);
+	if (!s.kin.empty()) { int r = nb_upload_kinematic_bodies(ctx, file->kin, (u32)s.kin.size(), st); if (r) return r; }
+	drop_body_forces(ctx);
+	if (s.has_frc) {
+		{ int r = ensure_body_forces(ctx, st); if (r) return r; }
+		CK(cudaMemcpyAsync(ctx->frc, file->frc, sizeof(nb_body_force) * (size_t)s.B, cudaMemcpyHostToDevice, st));
+	}
+	return NB_OK;
 }
 
 static bool state_put(FILE* f, const StateSection& s, std::vector<unsigned char>& tmp, cudaStream_t st) {
@@ -91,15 +155,7 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	int r = get_counts(ctx, c, stream); if (r) return r;
 	FILE* f = fopen(path, "wb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
-	NbStateHeader h; memset(&h, 0, sizeof(h));
-	memcpy(h.magic, "NBSTATE1", 8);
-	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
-	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
-	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
-	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
-	if (ctx->has_frc) h.reserved[5] = 1;
-	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = c[CNT_CACHE]; h.solver_mode = (u32)ctx->solver_mode;
+	const NbStateHeader h = state_header_of(ctx, c[CNT_CACHE]);
 	StateHostCopies hc;
 	const unsigned char* kin = reinterpret_cast<const unsigned char*>(ctx->kin_list.data());
 	hc.kin.assign(kin, kin + 4 * ctx->kin_list.size());
@@ -158,26 +214,15 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	for (u32 i = 0; ok && h.reserved[5] && i < h.bodies; ++i) ok = frc[i].body == i && !body_force_problem(frc[i]);
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
-	ctx->B = h.bodies; ctx->nboxes = h.boxes; ctx->nspheres = h.spheres; ctx->nconn = h.connections;
-	{ const nb_body_pair* p = reinterpret_cast<const nb_body_pair*>(hc.conn.data()); ctx->conn_host.assign(p, p + h.connections); }
 	ctx->scene_edited = false;   // the loaded scene replaces an edited one
-	ctx->tagbits = bits_for((u64)maxtag + 1);
-	ctx->kbits = bits_for(std::max(1u, h.boxes + h.spheres));
 	CK(cudaMemcpyAsync(ctx->counts + CNT_CACHE, &h.cache, 4, cudaMemcpyHostToDevice, st));
 	CK(cudaStreamSynchronize(st));
-	if (h.solver_mode == NB_SOLVER_PARITY || h.solver_mode == NB_SOLVER_THROUGHPUT) ctx->solver_mode = (int)h.solver_mode;
-	ctx->has_filter = h.reserved[1] != 0; ctx->filter_flags = h.reserved[0] & NB_FILTER_SKIP_CONNECTED;
-	++ctx->graph_epoch;
-	{ int r = build_conn_lookup(ctx, st); if (r) return r; }
-	{ int r = set_sensors(ctx, hc.sensor.data(), h.reserved[2] ? h.boxes + h.spheres : 0, h.reserved[3], st); if (r) return r; }
-	// the scatter rewrites the loaded momentum rows with their own values
-	drop_kinematic(ctx);
-	if (!kin.empty()) { int r = nb_upload_kinematic_bodies(ctx, kin.data(), (u32)kin.size(), st); if (r) return r; }
-	drop_body_forces(ctx);
-	if (h.reserved[5]) {
-		{ int r = ensure_body_forces(ctx, st); if (r) return r; }
-		CK(cudaMemcpyAsync(ctx->frc, frc, sizeof(nb_body_force) * (size_t)h.bodies, cudaMemcpyHostToDevice, st));
-	}
+	StateShape shape = { h.bodies, h.boxes, h.spheres, h.connections, bits_for((u64)maxtag + 1), bits_for(std::max(1u, h.boxes + h.spheres)), h.solver_mode,
+						 h.reserved[0] & NB_FILTER_SKIP_CONNECTED, h.reserved[3], h.reserved[1] != 0, h.reserved[2] != 0, h.reserved[5] != 0, {}, {} };
+	{ const nb_body_pair* p = reinterpret_cast<const nb_body_pair*>(hc.conn.data()); shape.conn.assign(p, p + h.connections); }
+	shape.kin.assign(idx, idx + kin.size());
+	const StateFileTables file = { hc.sensor.data(), kin.data(), frc };
+	{ int r = install_state(ctx, shape, &file, st); if (r) return r; }
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
