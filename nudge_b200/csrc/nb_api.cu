@@ -35,10 +35,11 @@ struct nb_context {
 	u32 slots_per_bucket;
 	int coop_blocks_solve;
 	u64* keybits;  // OR, AND of the Morton codes of the current collide
-	bool defer_warm_start;  // nb_step: the warm start runs inside the first solver launch
+	bool defer_warm_start;  // nb_step: the warm start runs with the sweeps (nb_apply_impulses), not in setup
 	StepGraph graph; bool capturing;  // nb_step's graph; capturing: run_graphed is recording a step of this context
 	unsigned long long graph_epoch;   // in the graphs' key: bumped by every change of which kernels a step launches or of their arguments
 	u32* chain_start; u32* chain_len;  // per body: segment cursor (the segment's end once k_chain_scatter ran) / number of chain entries
+	float4* warm;   // two rows per chain entry: the warm start's share of the entry's side (k_build_rows -> k_warm_start)
 	bool contacts_internal;  // the current contact set came from nb_collide (not nb_upload_contacts)
 	// throughput mode (nb_set_solver_mode): mass-splitting Jacobi, nb_jacobi.cuh
 	int solver_mode; u32* jcnt; float4* jd; int jacobi_blocks1, jacobi_blocks2;
@@ -120,8 +121,13 @@ static int dev_alloc(nb_context* ctx, T** p, size_t n) {
 	size_t bytes = (n ? n : 1) * sizeof(T);
 	cudaError_t e = cudaMalloc(&q, bytes);
 	if (e != cudaSuccess) { ctx->error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
-	cudaMemset(q, 0, bytes);
 	ctx->allocs.push_back(q);
+	// Zeroed before the first use, which may come on a non-blocking stream that the legacy stream does not order against: a buffer
+	// allocated on first use (the body-force table, the kinematic table, ...) would otherwise be cleared AFTER the kernels that fill it
+	// when the legacy stream still holds other work (another context's step).
+	e = cudaMemsetAsync(q, 0, bytes, cudaStreamLegacy);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
+	if (e != cudaSuccess) { ctx->error = std::string("cudaMemset: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
 	*p = (T*)q;
 	return 0;
 }
@@ -405,6 +411,7 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->sched_pick, 16 * NB_SCHED_SEGS * 8); ALLOC(ctx->sched_pick_res, 16 * NB_SCHED_SEGS);
 	ALLOC(ctx->rows.plane, (size_t)ROW_PLANES_TOTAL * ctx->cstride); ALLOC(ctx->rows.state, 3 * (size_t)ctx->cstride);
 	ALLOC(ctx->rows.a, ctx->cstride); ALLOC(ctx->rows.b, ctx->cstride); ALLOC(ctx->rows.contact, ctx->cstride); ALLOC(ctx->rows.wait, 2 * (size_t)ctx->cstride); ALLOC(ctx->chain_start, B); ALLOC(ctx->chain_len, B);
+	ALLOC(ctx->warm, 4 * (size_t)C);
 	ctx->rows.stride = ctx->cstride;
 	ALLOC(ctx->jcnt, B); ALLOC(ctx->jd, 2 * (size_t)B);
 	// upload of the rows `collide` does not read, on a copy stream of its own (NB_COPY_OVERLAP=0: everything on the caller's stream)
@@ -914,21 +921,26 @@ static int launch_solve_jacobi(nb_context* ctx, int mode, u32 sweeps, cudaStream
 	return NB_OK;
 }
 
+// mode 0: the warm start; mode 1: `sweeps` sweeps; mode 2: the warm start, then `sweeps` sweeps.  The warm start is k_warm_start
+// (the working rows with the warm start applied, from the shares k_build_rows left), the sweeps one k_solve launch.
 static int launch_solve(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) {
 	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) return launch_solve_jacobi(ctx, mode, sweeps, st);
 	const u32 B = ctx->B;
-	k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
-	Rows R = ctx->rows;
-	const float4* impulses = ctx->impulses;
-	float4* mw = ctx->mw;
-	u32* counts = ctx->counts;
-	u32 backoff = NB_SOLVE_BACKOFF_NS;
-	void* args[] = { &R, &impulses, &mw, &mode, &sweeps, &backoff, &counts };
-	if (mode) timing_begin(ctx, st);
-	CK(cudaLaunchCooperativeKernel(ctx->has_kin ? (void*)k_solve_kin : (void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
-	if (mode) timing_end(ctx, st);
+	if (mode == 1) k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
+	else k_warm_start<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->chain_start, ctx->chain_len, ctx->warm, ctx->mw);
+	if (mode) {
+		Rows R = ctx->rows;
+		float4* mw = ctx->mw;
+		u32* counts = ctx->counts;
+		u32 backoff = NB_SOLVE_BACKOFF_NS;
+		void* args[] = { &R, &mw, &sweeps, &backoff, &counts };
+		timing_begin(ctx, st);
+		CK(cudaLaunchCooperativeKernel(ctx->has_kin ? (void*)k_solve_kin : (void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
+		timing_end(ctx, st);
+		++ctx->launches;
+	}
 	k_mw_out<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, mode ? 1 : 0);
-	ctx->launches += 3;
+	ctx->launches += 2;
 	return NB_OK;
 }
 
@@ -947,7 +959,8 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 		CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
 		CK(cudaMemsetAsync(ctx->jcnt, 0, sizeof(u32) * B, st));
 		k_jacobi_prepare<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->jcnt, ctx->rows, ctx->cstride, counts);
-		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, ctx->jcnt);
+		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, ctx->jcnt,
+			nullptr, nullptr, nullptr);
 		ctx->launches += 3;
 		if (!ctx->defer_warm_start) {
 			int r = launch_solve(ctx, 0, 1, st); if (r) return r; if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
@@ -976,7 +989,8 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	k_chain_alloc<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->chain_len, ctx->chain_start, counts);
 	k_chain_scatter<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->chain_start, ctx->sb.keys[0], counts);
 	k_chain_rank<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->sb.keys[0], ctx->rows.wait, ctx->cstride, counts);
-	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, nullptr);
+	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, nullptr,
+		ctx->impulses, ctx->chain_start, ctx->warm);
 	ctx->launches += 5;
 	if (!ctx->defer_warm_start) {  // warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
 		int r = launch_solve(ctx, 0, 1, st); if (r) return r;
@@ -1029,7 +1043,7 @@ static int step_body(nb_context* ctx, float time_step, uint32_t iterations, floa
 	if ((r = nb_collide(ctx, stream))) return r;
 	if ((r = nb_apply_gravity_damping(ctx, time_step, gravity, damping, stream))) return r;
 	if ((r = nb_read_cached_impulses(ctx, stream))) return r;
-	ctx->defer_warm_start = iterations > 0 && !ctx->urow_n;  // warm start + sweeps in one solver launch (same arithmetic, same order); not with user rows between the sweeps
+	ctx->defer_warm_start = iterations > 0 && !ctx->urow_n;  // warm start straight into the sweeps' working rows (same arithmetic, same order); not with user rows between the sweeps
 	r = nb_setup_contact_constraints(ctx, stream);
 	if (!r) r = nb_apply_impulses(ctx, iterations, stream);
 	ctx->defer_warm_start = false;

@@ -687,6 +687,48 @@ __global__ void __launch_bounds__(NB_BLOCK) k_chain_rank(const u32* sorted, cons
 	}
 }
 
+// rcpps / rsqrtps of the solver arithmetic as a policy: LutMath reproduces the host CPU's instructions bit for bit (parity mode),
+// FastMath uses the GPU's own reciprocal / rsqrt (throughput mode: more accurate, not bit-comparable with the reference).
+struct LutMath {
+	const u32* rcp_lut; const u32* rsqrt_lut;
+	NB_DEV float rcp(float x) const { return nb_rcp_t(x, rcp_lut); }
+	NB_DEV float rsqrt(float x) const { return nb_rsqrt_t(x, rsqrt_lut); }
+};
+struct FastMath {
+	NB_DEV float rcp(float x) const { return __frcp_rn(x); }
+	NB_DEV float rsqrt(float x) const { return rsqrtf(x); }   // rsqrt(0) = inf, rsqrt(<0) = NaN like rsqrtps
+};
+
+// The warm start of one contact (nudge.cpp:4563-4632) in two parts: the contact's own terms (the three state values and the linear
+// impulse), then the angular impulse of one side from the terms and that side's planes (u, v, n = UA_X, VA_X, NA_X or UB_X, VB_X, NB_X).
+// P[k*S] = row plane k of this contact (global planes: P = R.plane + slot, S = R.stride; a shared-memory tile: P = tile + lane, S = tile width).
+struct WarmTerms { float normal_impulse, fix, fiy, lx, ly, lz; };
+template<class M>
+NB_DEV WarmTerms warm_start_terms(const float* P, const u32 S, const float4 ci, const M m) {
+	float n_x = P[N_X*S], n_y = P[N_Y*S], n_z = P[N_Z*S];
+	float u_x = P[U_X*S], u_y = P[U_Y*S], u_z = P[U_Z*S], v_x = P[V_X*S], v_y = P[V_Y*S], v_z = P[V_Z*S];
+	float normal_impulse = nb_max(n_x*ci.x + n_y*ci.y + n_z*ci.z, 0.0f);
+	float max_friction_impulse = normal_impulse * P[FRICTION*S];
+	float fix = u_x*ci.x + u_y*ci.y + u_z*ci.z;
+	float fiy = v_x*ci.x + v_y*ci.y + v_z*ci.z;
+	float fcs = fix*fix + fiy*fiy;
+	fcs = m.rsqrt(fcs);
+	fcs = fcs * max_friction_impulse;
+	fcs = nb_min(1.0f, fcs);  // first operand on NaN
+	fix = fix * fcs; fiy = fiy * fcs;
+	WarmTerms t;
+	t.normal_impulse = normal_impulse; t.fix = fix; t.fiy = fiy;
+	t.lx = fix*u_x + fiy*v_x + n_x * normal_impulse;
+	t.ly = fix*u_y + fiy*v_y + n_y * normal_impulse;
+	t.lz = fix*u_z + fiy*v_z + n_z * normal_impulse;
+	return t;
+}
+NB_DEV float3 warm_start_angular(const float* P, const u32 S, const WarmTerms& t, const u32 u, const u32 v, const u32 n) {
+	return make_float3(t.fix*P[u*S] + t.fiy*P[v*S] + t.normal_impulse*P[n*S],
+	                   t.fix*P[(u + 1)*S] + t.fiy*P[(v + 1)*S] + t.normal_impulse*P[(n + 1)*S],
+	                   t.fix*P[(u + 2)*S] + t.fiy*P[(v + 2)*S] + t.normal_impulse*P[(n + 2)*S]);
+}
+
 // ---------------- constraint rows (nudge.cpp:4350-4561), one thread per contact, SoA planes ----------------
 struct Rows { float* plane; u32 stride; u32* a; u32* b; u32* contact; float* state; uint2* wait; };  // plane[k*stride + slot], wait[side*stride + slot] = (seq, len)
 // a[slot] / b[slot] carry NB_READ_ONLY on a kinematic side: the solvers read that body's velocity and never write it.  A side is written
@@ -697,9 +739,11 @@ struct Rows { float* plane; u32 stride; u32* a; u32* b; u32* contact; float* sta
 // SPLIT (throughput mode, nb_jacobi.cuh): body i is split into cnt[i] sub-bodies of mass m_i / cnt[i], one per contact (Tonge et al.,
 // "Mass splitting for jitter-free parallel rigid body simulation", 2012), so every effective-mass term of body i is scaled by
 // cnt[i]; the planes that APPLY an impulse to a body (NA.., UA.., MASS_A/B) stay unscaled because the sub-bodies are averaged back.
+// !SPLIT (exact order, after k_chain_rank): also the warm start's per-contact part, see k_warm_start.
 template<bool SPLIT>
 __global__ void __launch_bounds__(NB_BLOCK) k_build_rows(const float4* contacts, const uint2* bodies,
-		const nb_transform* xf, const float4* inertia, const nb_body_momentum* momentum, const uint8_t* kind, Rows R, const u32* counts, const u32* cnt) {
+		const nb_transform* xf, const float4* inertia, const nb_body_momentum* momentum, const uint8_t* kind, Rows R, const u32* counts, const u32* cnt,
+		const float4* impulses, const u32* chain_end, float4* warm) {
 	__shared__ u32 s_rsqrt[2048];
 	for (u32 i = threadIdx.x; i < 2048; i += blockDim.x) s_rsqrt[i] = g_rsqrt_lut[i];
 	__syncthreads();
@@ -788,6 +832,25 @@ __global__ void __launch_bounds__(NB_BLOCK) k_build_rows(const float4* contacts,
 		P[NB_X*S] = nb_x; P[NB_Y*S] = nb_y; P[NB_Z*S] = nb_z;
 		P[MASS_A*S] = a_mass_inverse; P[MASS_B*S] = b_mass_inverse;
 		R.a[j] = kin_is(kind, a) ? a | NB_READ_ONLY : a; R.b[j] = kin_is(kind, b) ? b | NB_READ_ONLY : b;
+		if (!SPLIT) {
+			// The warm start's contact terms from the planes just written, and per side with a chain the side's share of the update, at
+			// the entry's place in its body's chain (k_warm_start): (lx, ly, lz) * mass_inverse and side, then the angular impulse.
+			const WarmTerms t = warm_start_terms(P, S, impulses[c], LutMath{ g_rcp_lut, s_rsqrt });
+			R.state[j] = t.normal_impulse; R.state[S + j] = t.fix; R.state[2*S + j] = t.fiy;
+			const uint2 wa = R.wait[j], wb = R.wait[S + j];   // (seq, len); len = 0: body 0 or a kinematic side
+			if (wa.y) {
+				const u32 e = chain_end[a] - wa.y + wa.x;
+				const float3 aa = warm_start_angular(P, S, t, UA_X, VA_X, NA_X);
+				warm[2*e] = make_float4(t.lx * a_mass_inverse, t.ly * a_mass_inverse, t.lz * a_mass_inverse, asf(0u));
+				warm[2*e + 1] = make_float4(aa.x, aa.y, aa.z, 0.0f);
+			}
+			if (wb.y) {
+				const u32 e = chain_end[b] - wb.y + wb.x;
+				const float3 ba = warm_start_angular(P, S, t, UB_X, VB_X, NB_X);
+				warm[2*e] = make_float4(t.lx * b_mass_inverse, t.ly * b_mass_inverse, t.lz * b_mass_inverse, asf(1u));
+				warm[2*e + 1] = make_float4(ba.x, ba.y, ba.z, 0.0f);
+			}
+		}
 	}
 }
 
@@ -812,6 +875,29 @@ __global__ void __launch_bounds__(NB_BLOCK) k_mw_in(u32 B, const nb_body_momentu
 		mw[2*i] = l; mw[2*i + 1] = w;
 	}
 }
+// k_mw_in with the warm start applied.  The warm start reads no velocity, so a body's result depends on its own chain only: each body
+// walks its chain in order, applying the shares k_build_rows left at the chain's entries (warm[2e] = linear share, side; warm[2e + 1] =
+// angular share) with the same operations as warm_start_contact_p, which gives the bits the dataflow pass gave without its hand-offs.
+// Body 0 and kinematic bodies have no chain: their rows are copied.
+__global__ void __launch_bounds__(NB_BLOCK) k_warm_start(u32 B, const nb_body_momentum* momentum, const u32* chain_end, const u32* chain_len, const float4* warm, float4* mw) {
+	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
+		const float4* p = reinterpret_cast<const float4*>(momentum + i);
+		float4 l = p[0], w = p[1];
+		const u32 len = chain_len[i];
+		if (len) {
+			const u32 end = chain_end[i];
+			#pragma unroll 4
+			for (u32 e = end - len; e < end; ++e) {
+				const float4 dl = warm[2*e], dw = warm[2*e + 1];
+				if (asu(dl.w)) { l.x += dl.x; l.y += dl.y; l.z += dl.z; }   // side b
+				else { l.x -= dl.x; l.y -= dl.y; l.z -= dl.z; }            // side a
+				w.x += dw.x; w.y += dw.y; w.z += dw.z;
+			}
+		}
+		l.w = 0.0f; w.w = 0.0f;  // token 0, as k_mw_in
+		mw[2*i] = l; mw[2*i + 1] = w;
+	}
+}
 // mode 1 (sweeps): unused1 of touched bodies is zeroed like nudge.cpp:4823, 4849; unused0 keeps the inverse mass (4825-4827)
 __global__ void __launch_bounds__(NB_BLOCK) k_mw_out(u32 B, nb_body_momentum* momentum, const float4* mw, int mode) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
@@ -824,49 +910,18 @@ __global__ void __launch_bounds__(NB_BLOCK) k_mw_out(u32 B, nb_body_momentum* mo
 	}
 }
 
-// rcpps / rsqrtps of the solver arithmetic as a policy: LutMath reproduces the host CPU's instructions bit for bit (parity mode),
-// FastMath uses the GPU's own reciprocal / rsqrt (throughput mode: more accurate, not bit-comparable with the reference).
-struct LutMath {
-	const u32* rcp_lut; const u32* rsqrt_lut;
-	NB_DEV float rcp(float x) const { return nb_rcp_t(x, rcp_lut); }
-	NB_DEV float rsqrt(float x) const { return nb_rsqrt_t(x, rsqrt_lut); }
-};
-struct FastMath {
-	NB_DEV float rcp(float x) const { return __frcp_rn(x); }
-	NB_DEV float rsqrt(float x) const { return rsqrtf(x); }   // rsqrt(0) = inf, rsqrt(<0) = NaN like rsqrtps
-};
-
-// One contact of the warm start (nudge.cpp:4563-4632); momentum rows passed in registers and updated in place.
-// `state` points at the contact's slot in the three state planes (stride S floats apart).
-// P[k*PS] = row plane k of this contact (global planes: P = R.plane + slot, PS = R.stride; a shared-memory tile: P = tile + lane, PS = tile width).
+// One contact of the warm start; momentum rows passed in registers and updated in place.  `state` points at the contact's slot in the
+// three state planes (stride SS floats apart).
 template<class M>
 NB_DEV void warm_start_contact_p(const float* P, const u32 S, const float4 ci, float* state, const u32 SS, float4& al, float4& aw, float4& bl, float4& bw, const M m) {
 	float a_mass_inverse = P[MASS_A*S], b_mass_inverse = P[MASS_B*S];
-	float n_x = P[N_X*S], n_y = P[N_Y*S], n_z = P[N_Z*S];
-	float u_x = P[U_X*S], u_y = P[U_Y*S], u_z = P[U_Z*S], v_x = P[V_X*S], v_y = P[V_Y*S], v_z = P[V_Z*S];
-	float normal_impulse = nb_max(n_x*ci.x + n_y*ci.y + n_z*ci.z, 0.0f);
-	float max_friction_impulse = normal_impulse * P[FRICTION*S];
-	float fix = u_x*ci.x + u_y*ci.y + u_z*ci.z;
-	float fiy = v_x*ci.x + v_y*ci.y + v_z*ci.z;
-	float fcs = fix*fix + fiy*fiy;
-	fcs = m.rsqrt(fcs);
-	fcs = fcs * max_friction_impulse;
-	fcs = nb_min(1.0f, fcs);  // first operand on NaN
-	fix = fix * fcs; fiy = fiy * fcs;
-	float lx = fix*u_x + fiy*v_x + n_x * normal_impulse;
-	float ly = fix*u_y + fiy*v_y + n_y * normal_impulse;
-	float lz = fix*u_z + fiy*v_z + n_z * normal_impulse;
-	float aax = fix*P[UA_X*S] + fiy*P[VA_X*S] + normal_impulse*P[NA_X*S];
-	float aay = fix*P[UA_Y*S] + fiy*P[VA_Y*S] + normal_impulse*P[NA_Y*S];
-	float aaz = fix*P[UA_Z*S] + fiy*P[VA_Z*S] + normal_impulse*P[NA_Z*S];
-	float bax = fix*P[UB_X*S] + fiy*P[VB_X*S] + normal_impulse*P[NB_X*S];
-	float bay = fix*P[UB_Y*S] + fiy*P[VB_Y*S] + normal_impulse*P[NB_Y*S];
-	float baz = fix*P[UB_Z*S] + fiy*P[VB_Z*S] + normal_impulse*P[NB_Z*S];
-	al.x -= lx * a_mass_inverse; al.y -= ly * a_mass_inverse; al.z -= lz * a_mass_inverse;
-	aw.x += aax; aw.y += aay; aw.z += aaz;
-	bl.x += lx * b_mass_inverse; bl.y += ly * b_mass_inverse; bl.z += lz * b_mass_inverse;
-	bw.x += bax; bw.y += bay; bw.z += baz;
-	state[0] = normal_impulse; state[SS] = fix; state[2*SS] = fiy;
+	const WarmTerms t = warm_start_terms(P, S, ci, m);
+	const float3 aa = warm_start_angular(P, S, t, UA_X, VA_X, NA_X), ba = warm_start_angular(P, S, t, UB_X, VB_X, NB_X);
+	al.x -= t.lx * a_mass_inverse; al.y -= t.ly * a_mass_inverse; al.z -= t.lz * a_mass_inverse;
+	aw.x += aa.x; aw.y += aa.y; aw.z += aa.z;
+	bl.x += t.lx * b_mass_inverse; bl.y += t.ly * b_mass_inverse; bl.z += t.lz * b_mass_inverse;
+	bw.x += ba.x; bw.y += ba.y; bw.z += ba.z;
+	state[0] = t.normal_impulse; state[SS] = t.fix; state[2*SS] = t.fiy;
 }
 template<class M>
 NB_DEV void warm_start_contact(const Rows& R, u32 j, const float4* impulses, float4& al, float4& aw, float4& bl, float4& bw, const M m) {
@@ -969,12 +1024,11 @@ NB_DEV void solve_contact(const Rows& R, u32 j, const float (&rv)[ROW_PLANES_TOT
 	bw.z = nb_madd(rv[VB_Z], friction_impulse_y, b_angular_velocity_z);
 }
 
-// mode 0: warm start (one pass); mode 1: `sweeps` PGS sweeps; mode 2: the warm start followed by `sweeps` sweeps in the same
-// launch (nb_step: nothing happens between setup and the first sweep, so the two pipelines can overlap).  Co-resident grid, no barrier.  Thread t owns slots t, t+T, ...
+// `sweeps` PGS sweeps (the warm start is k_warm_start's).  Co-resident grid, no barrier.  Thread t owns slots t, t+T, ...
 // (so the per-contact solver state stays private to one thread) and walks them sweep by sweep; within and across threads the
 // items are visited in increasing (sweep, slot), which is a topological order of the dependency graph, so the lowest
 // unfinished item is always runnable.  Inside a warp the lanes poll instead of blocking, so a lane may depend on another
-// lane of its own warp.  mw must come from k_mw_in (all tokens 0).
+// lane of its own warp.  mw must come from k_mw_in or k_warm_start (all tokens 0).
 //
 // Waiting: the body's token says how many applications are still ahead of this contact (k_chain_rank).  While that number is
 // >= 2 on either body only the linear halves are polled, and the warp sleeps hop_ns per missing application when all of its

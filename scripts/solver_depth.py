@@ -1,5 +1,9 @@
-"""Dependency depth of the exact Gauss-Seidel order vs the time the dataflow solver takes (development aid, GPU)."""
+"""Dependency depth of the exact Gauss-Seidel order vs the time the dataflow solver takes (development aid, GPU).
+
+Also the depth the warm start had as a dataflow pass over the same slots (one pass of hops, like a sweep), and the longest body chain:
+the serial walk k_warm_start does instead (no hand-offs, DESIGN.md section 2.8)."""
 import sys, os
+from collections import Counter
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 import nudge_b200, bench
@@ -20,6 +24,10 @@ def depth(a, b, sweeps):
         per_sweep.append(max(last.values()))
     return per_sweep
 
+def longest_chain(a, b):
+    n = Counter(x for x in a + b if x and not x >> 31)
+    return max(n.values())
+
 for n in [int(x) for x in sys.argv[1:]] or [16384, 65536]:
     scene = scenes.box_drop(n, iterations=8, seed=2)
     sim = nudge_b200.Sim(scene, device=0, stream=torch.cuda.current_stream().cuda_stream)
@@ -37,4 +45,5 @@ for n in [int(x) for x in sys.argv[1:]] or [16384, 65536]:
         torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
     d = depth(a, b, 8)
     t = float(np.median(ts[2:]))
-    print("boxes %d slots %d depth/sweep %d total-depth(8) %d apply_impulses %.3f ms -> %.3f us/hop" % (n, len(a), d[0], d[-1], t, 1000 * t / d[-1]), flush=True)
+    print("boxes %d slots %d depth/sweep %d total-depth(8) %d apply_impulses %.3f ms -> %.3f us/hop; warm start as a dataflow pass: depth %d "
+          "(9 passes: %d); k_warm_start: longest chain %d" % (n, len(a), d[0], d[-1], t, 1000 * t / d[-1], d[0], depth(a, b, 9)[-1], longest_chain(a, b)), flush=True)
