@@ -21,6 +21,14 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long plan_version, graph_epoch; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
+// A device buffer of `cap` elements, freed with its owner (the context or a snapshot); the editing calls grow theirs on demand (grow, below).
+// Move-only: the move swaps, so the buffer it replaces is freed with the temporary.
+template<class T> struct DevBuf {
+	T* p = nullptr; size_t cap = 0;
+	DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+	~DevBuf() { if (p) cudaFree(p); }
+};
+
 struct nb_context {
 	nb_config cfg;
 	int sms;
@@ -28,6 +36,11 @@ struct nb_context {
 	unsigned long long launches;
 	int lut_exact;
 	std::vector<void*> allocs;
+	// device bytes held by the context and its snapshots (dev_alloc, grow, nb_snapshot_create / nb_snapshot_destroy; nb_debug_read)
+	unsigned long long device_bytes;
+	// the editing calls' shared host side: the staging copy of a caller's array (put_staged) and the duplicate check's byte per body, all
+	// zeros between calls (bodies_distinct)
+	std::vector<unsigned char> host_stage; std::vector<uint8_t> body_seen;
 	u32 B, nboxes, nspheres, nconn;  // uploaded sizes
 	u32 tagbits, kbits, bodybits;
 	u32 stride;    // scratch stride
@@ -50,32 +63,31 @@ struct nb_context {
 	// nb_upload_bodies sends what the collision stage does not read (momentum, properties) on a second stream, so that copy runs under
 	// `collide`; the first consumer waits for ev_up_done (inside a captured step: an external event-wait node, re-armed by every upload)
 	cudaStream_t copy_stream; cudaEvent_t ev_up_begin, ev_up_done; bool upload_pending, capture_joined; int copy_overlap;
-	nb_constraint_row* urows; u32 urow_cap, urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order;
-	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer holds ev_alloc events and is kept while it is large enough
-	nb_contact_event* events; u32 ev_cap, ev_alloc;
+	DevBuf<nb_constraint_row> urows; u32 urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order;
+	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer is kept while it holds ev_cap events
+	DevBuf<nb_contact_event> events; u32 ev_cap;
 	// collision filters (nb_upload_collision_filters): one category | mask << 16 word per collider while has_filter; with
 	// NB_FILTER_SKIP_CONNECTED and connections, conn_keys holds the sorted connection keys and conn_probe = their count (else 0)
 	u32* filter; bool has_filter; u32 filter_flags; u64* conn_keys; u64* conn_scratch; u32* conn_sort_n; u32 conn_probe;
 	// sensor colliders (nb_upload_sensors, DESIGN.md section 8.7): one 0/1 byte per collider while has_sensor; sensor_cap = candidate sensor
-	// pairs per collide.  The candidate keys, the sort buffers and the current / old overlap lists hold sensor_alloc entries and are kept while
-	// large enough.
-	uint8_t* sensor; bool has_sensor; u32 sensor_cap, sensor_alloc; u64* sensor_keys; SortBuffers sensor_sb; uint4* sensor_cur; uint4* sensor_old;
+	// pairs per collide.  The candidate keys, the sort buffers (sensor_sb points into sensor_sort_keys / _vals) and the current / old overlap
+	// lists are kept while they hold sensor_cap entries.
+	uint8_t* sensor; bool has_sensor; u32 sensor_cap; DevBuf<u64> sensor_keys, sensor_sort_keys[2]; DevBuf<u32> sensor_sort_vals[2]; SortBuffers sensor_sb;
+	DevBuf<uint4> sensor_cur, sensor_old;
 	// kinematic bodies (nb_upload_kinematic_bodies, DESIGN.md section 8.8): kind[body] as in nb_collide.cuh (bit 0 kinematic, bit 1 moving),
 	// allocated for max_bodies on the first upload of a set; kin_list = the set (host copy, ascending); kin_rows = the scatter's staging rows
-	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; nb_kinematic_body* kin_rows; u32 kin_rows_cap;
-	// body impulses (nb_apply_body_impulses, DESIGN.md section 8.9): the call's own staging rows and sort buffers (imp_cap entries, kept while
-	// large enough), host staging, and its sort histogram, grid barrier and key count; none of it is shared with the step
-	nb_body_impulse* imp_rows; u32 imp_cap; SortBuffers imp_sb; u32* imp_n; std::vector<nb_body_impulse> imp_host;
+	uint8_t* kind; bool has_kin; std::vector<u32> kin_list; DevBuf<nb_kinematic_body> kin_rows;
+	// body impulses (nb_apply_body_impulses, DESIGN.md section 8.9): the call's own staging rows and sort keys (imp_sb points into imp_keys),
+	// and its sort histogram, grid barrier and key count; none of it is shared with the step
+	DevBuf<nb_body_impulse> imp_rows; DevBuf<u64> imp_keys[2]; SortBuffers imp_sb; u32* imp_n;
 	// spawning (nb_add_bodies, nb_remove_bodies, DESIGN.md section 8.10): scene_edited refuses the stage calls that read the last collide's
 	// outputs until the next collide; sharded = nb_shard_create was called on this context (edits are refused); urow_ab = each user row's
 	// (a, b) in upload order, for re-levelling after a removal; spawn_idx / urows_spare = the removal's index staging and row gather buffers
 	// conn_host = the connections as uploaded or loaded, for the removal's index checks
-	bool scene_edited, sharded; std::vector<nb_body_pair> urow_ab, conn_host; u32* spawn_idx; u32 spawn_idx_cap; nb_constraint_row* urows_spare; u32 urows_spare_cap;
+	bool scene_edited, sharded; std::vector<nb_body_pair> urow_ab, conn_host; DevBuf<u32> spawn_idx; DevBuf<nb_constraint_row> urows_spare;
 	// per-body forces (nb_set_body_forces, DESIGN.md section 8.11): frc = one entry per body while has_frc, allocated for max_bodies on the
-	// first call, together with frc_spare (nb_remove_bodies gathers into it); frc_rows = the scatter's staging rows (frc_rows_cap entries);
-	// frc_seen = the duplicate check's byte per body, all zeros between calls
-	nb_body_force* frc; nb_body_force* frc_spare; bool has_frc; nb_body_force* frc_rows; u32 frc_rows_cap; std::vector<nb_body_force> frc_host;
-	std::vector<uint8_t> frc_seen;
+	// first call, together with frc_spare (nb_remove_bodies gathers into it); frc_rows = the scatter's staging rows
+	nb_body_force* frc; nb_body_force* frc_spare; bool has_frc; DevBuf<nb_body_force> frc_rows;
 	// snapshots (nb_snapshot_save / nb_snapshot_restore, DESIGN.md section 8.12): in_step = between nb_collide and the nb_advance that ends its
 	// step, where a save is refused; the context's snapshots, freed by nb_destroy; graph_records = captures of a step graph (nb_debug_read)
 	bool in_step; std::vector<nb_snapshot*> snapshots; unsigned long long graph_records;
@@ -122,6 +134,7 @@ static int dev_alloc(nb_context* ctx, T** p, size_t n) {
 	cudaError_t e = cudaMalloc(&q, bytes);
 	if (e != cudaSuccess) { ctx->error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
 	ctx->allocs.push_back(q);
+	ctx->device_bytes += bytes;
 	// Zeroed before the first use, which may come on a non-blocking stream that the legacy stream does not order against: a buffer
 	// allocated on first use (the body-force table, the kinematic table, ...) would otherwise be cleared AFTER the kernels that fill it
 	// when the legacy stream still holds other work (another context's step).
@@ -133,6 +146,31 @@ static int dev_alloc(nb_context* ctx, T** p, size_t n) {
 }
 #define ALLOC(p, n) do { int r_ = dev_alloc(ctx, &(p), (size_t)(n)); if (r_) return r_; } while (0)
 
+// Makes `b` hold at least n elements.  A larger buffer replaces the old one once `st` has drained, since earlier work on it may still read
+// the old one; the contents are neither kept nor cleared.  On failure the buffer is empty.
+template<class T>
+static int grow(nb_context* ctx, DevBuf<T>& b, size_t n, cudaStream_t st) {
+	if (n <= b.cap) return NB_OK;
+	CK(cudaStreamSynchronize(st));
+	ctx->device_bytes -= b.cap * sizeof(T);
+	b = DevBuf<T>();
+	CK(cudaMalloc(&b.p, n * sizeof(T)));
+	b.cap = n;
+	ctx->device_bytes += n * sizeof(T);
+	return NB_OK;
+}
+#define GROW(b, n, st) do { int r_ = grow(ctx, b, (size_t)(n), st); if (r_) return r_; } while (0)
+
+// The host staging of the editing calls: enqueues the copy of `bytes` from the caller's `src` to `dst` on `st` through the context's pageable
+// staging vector, which a pageable cudaMemcpyAsync has consumed when it returns, so the caller's array may be reused on return, pinned or not.
+// `edit`, when given, rewrites the staged bytes first.
+static cudaError_t put_staged(nb_context* ctx, void* dst, const void* src, size_t bytes, cudaStream_t st, void (*edit)(unsigned char*, size_t) = nullptr) {
+	if (!bytes) return cudaSuccess;
+	ctx->host_stage.assign((const unsigned char*)src, (const unsigned char*)src + bytes);
+	if (edit) edit(ctx->host_stage.data(), bytes);
+	return cudaMemcpyAsync(dst, ctx->host_stage.data(), bytes, cudaMemcpyHostToDevice, st);
+}
+
 static u32 bits_for(u64 n) { u32 b = 1; while (((u64)1 << b) < n) ++b; return b; }
 static Launch mk_launch(nb_context* ctx, void* stream) { Launch L = { (cudaStream_t)stream, &ctx->launches, ctx->sms }; return L; }
 #define GRID(n) nb_grid_for((unsigned)(n), ctx->sms)
@@ -140,7 +178,6 @@ static Launch mk_launch(nb_context* ctx, void* stream) { Launch L = { (cudaStrea
 struct NbRange { NbRange(const char* name) { nvtxRangePushA(name); } ~NbRange() { nvtxRangePop(); } };
 #define NB_RANGE(name) NbRange nb_range_(name)
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb_rows_api.cuh
-static void free_impulse_rows(nb_context* ctx);                            // nb_impulse_api.cuh
 static void free_snapshots(nb_context* ctx);                               // nb_snapshot_api.cuh
 // The stage calls that read the last nb_collide's outputs: refused after nb_add_bodies / nb_remove_bodies until the next collide
 #define NOT_AFTER_EDIT() do { if (ctx->scene_edited) { ctx->error = "the scene was edited (nb_add_bodies / nb_remove_bodies) since the last nb_collide"; return NB_ERR_ARGUMENT; } } while (0)
@@ -190,6 +227,33 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
 static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->graph_epoch; } }
 static void drop_body_forces(nb_context* ctx) { if (ctx->has_frc) { ctx->has_frc = false; ++ctx->graph_epoch; } }   // the step launches k_gravity_damping again
+// The kind table, allocated for max_bodies on first use.
+static int ensure_kind_table(nb_context* ctx) { if (!ctx->kind) ALLOC(ctx->kind, ctx->cfg.max_bodies); return NB_OK; }
+
+// The checks of entry i of a body list (kinematic bodies, impulses, forces, removals): not body 0, the static world; below the body count;
+// and, unless kinematic_ok, not kinematic.  A refused entry is NB_ERR_ARGUMENT with the message "<list> <i>: body <b> ...".
+static int check_body(nb_context* ctx, const char* list, u32 i, u32 b, bool kinematic_ok) {
+	std::string why;
+	if (b == 0) why = "is the static world";
+	else if (b >= ctx->B) why = "is at or beyond the body count (" + std::to_string(ctx->B) + ")";
+	else if (!kinematic_ok && ctx->has_kin && std::binary_search(ctx->kin_list.begin(), ctx->kin_list.end(), b))
+		why = "is kinematic (its velocity is set with nb_upload_kinematic_bodies)";
+	else return NB_OK;
+	ctx->error = std::string(list) + " " + std::to_string(i) + ": body " + std::to_string(b) + " " + why;
+	return NB_ERR_ARGUMENT;
+}
+// The duplicate check of a body list whose entries (body(i), each checked by check_body) may name a body once: one mark per body in
+// body_seen, which is all zeros between calls (O(n), where a sort of 65,536 entries costs ms).
+template<class Body>
+static int bodies_distinct(nb_context* ctx, const char* list, u32 n, Body body) {
+	ctx->body_seen.resize(std::max<size_t>(ctx->body_seen.size(), ctx->B), 0);
+	u32 twice = n;
+	for (u32 i = 0; i < n && twice == n; ++i) if (ctx->body_seen[body(i)]++) twice = i;
+	for (u32 i = 0; i < n; ++i) ctx->body_seen[body(i)] = 0;
+	if (twice == n) return NB_OK;
+	ctx->error = std::string(list) + " " + std::to_string(twice) + ": body " + std::to_string(body(twice)) + " is listed twice";
+	return NB_ERR_ARGUMENT;
+}
 
 // The velocity scatter of nb_upload_kinematic_bodies: each listed body's velocity and angular velocity into its momentum row (the unused lanes
 // are left alone), and its kind byte (the caller clears the table first when the set changes).
@@ -266,22 +330,11 @@ static int build_conn_lookup(nb_context* ctx, cudaStream_t st) {
 // nb_write_cached_impulses begins every overlap.  Synchronises `st`.
 #define NB_SENSOR_PAIRS_PER_SENSOR 256u
 #define NB_SENSOR_PAIRS_MIN 1024u
-static void free_sensor_lists(nb_context* ctx) {
-	void* p[] = { ctx->sensor_keys, ctx->sensor_sb.keys[0], ctx->sensor_sb.keys[1], ctx->sensor_sb.vals[0], ctx->sensor_sb.vals[1], ctx->sensor_cur, ctx->sensor_old };
-	for (void* q : p) if (q) cudaFree(q);
-	ctx->sensor_keys = nullptr; ctx->sensor_sb.keys[0] = ctx->sensor_sb.keys[1] = nullptr; ctx->sensor_sb.vals[0] = ctx->sensor_sb.vals[1] = nullptr;
-	ctx->sensor_cur = ctx->sensor_old = nullptr; ctx->sensor_alloc = 0;
-}
-// The candidate keys, sort buffers and overlap lists with room for `cap` entries (reallocated only when they are smaller).
-static int ensure_sensor_lists(nb_context* ctx, u32 cap) {
-	if (cap > ctx->sensor_alloc) {
-		free_sensor_lists(ctx);
-		CK(cudaMalloc(&ctx->sensor_keys, sizeof(u64) * (size_t)cap));
-		for (int i = 0; i < 2; ++i) { CK(cudaMalloc(&ctx->sensor_sb.keys[i], sizeof(u64) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_sb.vals[i], sizeof(u32) * (size_t)cap)); }
-		CK(cudaMalloc(&ctx->sensor_cur, sizeof(uint4) * (size_t)cap)); CK(cudaMalloc(&ctx->sensor_old, sizeof(uint4) * (size_t)cap));
-		ctx->sensor_alloc = cap;
-	}
-	ctx->sensor_sb.hist = ctx->sb.hist; ctx->sensor_sb.bar = ctx->sb.bar;
+// The candidate keys, sort buffers and overlap lists with room for `cap` entries (grown on `st` only when they are smaller).
+static int ensure_sensor_lists(nb_context* ctx, u32 cap, cudaStream_t st) {
+	GROW(ctx->sensor_keys, cap, st); GROW(ctx->sensor_cur, cap, st); GROW(ctx->sensor_old, cap, st);
+	for (int i = 0; i < 2; ++i) { GROW(ctx->sensor_sort_keys[i], cap, st); GROW(ctx->sensor_sort_vals[i], cap, st); }
+	ctx->sensor_sb = { { ctx->sensor_sort_keys[0].p, ctx->sensor_sort_keys[1].p }, { ctx->sensor_sort_vals[0].p, ctx->sensor_sort_vals[1].p }, ctx->sb.hist, ctx->sb.bar };
 	return NB_OK;
 }
 static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pairs, cudaStream_t st) {
@@ -296,7 +349,7 @@ static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pair
 			ctx->error = "max_sensor_pairs exceeds the context's scratch capacity (" + std::to_string(ctx->stride) + ": the largest of max_pairs, max_contacts, bodies, colliders)";
 			return NB_ERR_CAPACITY;
 		}
-		{ int r = ensure_sensor_lists(ctx, cap); if (r) return r; }
+		{ int r = ensure_sensor_lists(ctx, cap, st); if (r) return r; }
 		CK(cudaMemcpyAsync(ctx->sensor, f.data(), n, cudaMemcpyHostToDevice, st));
 	}
 	CK(cudaMemsetAsync(ctx->counts + CNT_SENSOR_PAIRS, 0, 3 * sizeof(u32), st));   // candidates, current and old overlaps
@@ -311,16 +364,16 @@ static void launch_sensor_overlaps(nb_context* ctx, const Launch& L) {
 	cudaStream_t st = L.stream;
 	u32* counts = ctx->counts;
 	const u32 cap = ctx->sensor_cap;
-	k_sensor_np<<<GRID((size_t)cap * 4), NB_BLOCK, 0, st>>>(ctx->sensor_keys, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
+	k_sensor_np<<<GRID((size_t)cap * 4), NB_BLOCK, 0, st>>>(ctx->sensor_keys.p, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
 		ctx->col_tag, ctx->col_body, ctx->flags, counts);
 	++ctx->launches;
 	nb_scan_reduce<1>(L, ctx->flags, ctx->stride, counts + CNT_SENSOR_PAIRS, 0, ctx->block_sums, counts + CNT_SENSOR_HITS);
-	k_sensor_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->sensor_keys, ctx->kbits, ctx->col_tag,
+	k_sensor_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->sensor_keys.p, ctx->kbits, ctx->col_tag,
 		ctx->sensor_sb.keys[0], ctx->sensor_sb.vals[0], counts);
 	++ctx->launches;
 	const int cur = nb_radix_sort(L, ctx->sensor_sb, counts + CNT_SENSOR_HITS, 0, (int)ctx->tagbits, true, 0, 32, (int)(32 + ctx->tagbits));
-	k_sensor_gather<<<GRID(cap), NB_BLOCK, 0, st>>>(ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys, ctx->kbits, ctx->col_tag, ctx->col_body,
-		ctx->sensor_cur, counts);
+	k_sensor_gather<<<GRID(cap), NB_BLOCK, 0, st>>>(ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys.p, ctx->kbits, ctx->col_tag, ctx->col_body,
+		ctx->sensor_cur.p, counts);
 	++ctx->launches;
 }
 
@@ -460,15 +513,8 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->tev_made) for (int i = 0; i < 64; ++i) { cudaEventDestroy(ctx->tev[0][i]); cudaEventDestroy(ctx->tev[1][i]); }
 	if (ctx->copy_stream) { cudaStreamDestroy(ctx->copy_stream); cudaEventDestroy(ctx->ev_up_begin); cudaEventDestroy(ctx->ev_up_done); }
 	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
-	if (ctx->events) cudaFree(ctx->events);
-	free_sensor_lists(ctx);
 	free_snapshots(ctx);
-	if (ctx->kin_rows) cudaFree(ctx->kin_rows);
-	if (ctx->frc_rows) cudaFree(ctx->frc_rows);
-	free_impulse_rows(ctx);
-	if (ctx->spawn_idx) cudaFree(ctx->spawn_idx);
-	if (ctx->urows_spare) cudaFree(ctx->urows_spare);
-	delete ctx;
+	delete ctx;   // and with it the grown buffers
 }
 
 const char* nb_last_error(const nb_context* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
@@ -550,30 +596,20 @@ int nb_upload_sensors(nb_context* ctx, const uint8_t* h, uint32_t n, uint32_t ma
 int nb_upload_kinematic_bodies(nb_context* ctx, const nb_kinematic_body* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_upload_kinematic_bodies");
 	if (n && !h) { ctx->error = "null kinematic body table"; return NB_ERR_ARGUMENT; }
+	for (u32 i = 0; i < n; ++i) if (int r = check_body(ctx, "kinematic body", i, h[i].body, true)) return r;
+	if (int r = bodies_distinct(ctx, "kinematic body", n, [&](u32 i) { return h[i].body; })) return r;
 	std::vector<u32> list(n);
-	for (u32 i = 0; i < n; ++i) {
-		const u32 b = h[i].body;
-		if (b == 0) { ctx->error = "body 0 is the static world and cannot be kinematic"; return NB_ERR_ARGUMENT; }
-		if (b >= ctx->B) { ctx->error = "kinematic body " + std::to_string(b) + " is at or beyond the body count (" + std::to_string(ctx->B) + ")"; return NB_ERR_ARGUMENT; }
-		list[i] = b;
-	}
+	for (u32 i = 0; i < n; ++i) list[i] = h[i].body;
 	std::sort(list.begin(), list.end());
-	if (std::adjacent_find(list.begin(), list.end()) != list.end()) { ctx->error = "a kinematic body is listed twice"; return NB_ERR_ARGUMENT; }
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
 	if (!n) { drop_kinematic(ctx); return NB_OK; }
-	if (!ctx->kind) ALLOC(ctx->kind, ctx->cfg.max_bodies);
-	if (n > ctx->kin_rows_cap) {
-		CK(cudaStreamSynchronize(st));   // the old staging rows may still be read by an earlier scatter
-		if (ctx->kin_rows) cudaFree(ctx->kin_rows);
-		ctx->kin_rows = nullptr; ctx->kin_rows_cap = 0;
-		CK(cudaMalloc(&ctx->kin_rows, sizeof(nb_kinematic_body) * (size_t)n));
-		ctx->kin_rows_cap = n;
-	}
+	{ int r = ensure_kind_table(ctx); if (r) return r; }
+	GROW(ctx->kin_rows, n, st);
 	const bool same = ctx->has_kin && list == ctx->kin_list;
 	if (!same) CK(cudaMemsetAsync(ctx->kind, 0, ctx->cfg.max_bodies, st));
-	CK(cudaMemcpyAsync(ctx->kin_rows, h, sizeof(nb_kinematic_body) * (size_t)n, cudaMemcpyHostToDevice, st));
-	k_kinematic_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->kin_rows, n, ctx->mom, ctx->kind);
+	CK(put_staged(ctx, ctx->kin_rows.p, h, sizeof(nb_kinematic_body) * (size_t)n, st));
+	k_kinematic_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->kin_rows.p, n, ctx->mom, ctx->kind);
 	++ctx->launches;
 	CK(cudaGetLastError());
 	if (!same) { ctx->has_kin = true; ctx->kin_list.swap(list); ++ctx->graph_epoch; }   // nb_step's graph re-records with the table
@@ -621,7 +657,7 @@ int nb_download_sensor_overlaps(nb_context* ctx, nb_sensor_overlap* host, uint32
 	if (count) *count = n;
 	if (n > capacity) { ctx->error = "host overlap buffer too small: " + std::to_string(n) + " overlaps"; return NB_ERR_CAPACITY; }
 	if (n && !host) { ctx->error = "null host overlap buffer"; return NB_ERR_ARGUMENT; }
-	D2H(host, ctx->sensor_cur, n, nb_sensor_overlap);
+	D2H(host, ctx->sensor_cur.p, n, nb_sensor_overlap);
 	CK(cudaStreamSynchronize((cudaStream_t)stream));
 	return NB_OK;
 }
@@ -706,9 +742,9 @@ int nb_collide(nb_context* ctx, void* stream) {
 	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
 	const uint8_t* sensor = ctx->has_sensor ? ctx->sensor : nullptr;   // null: the kernels never touch the sensor list
 	(kind ? k_grid_pairs<true> : k_grid_pairs<false>)<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	ctx->launches += 3;
 	// nudge.cpp:3498; the sort also clamps CNT_PAIRS to the capacity (the overflow bit is already set by emit_pair)
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);
@@ -833,12 +869,12 @@ int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_write_cached_impulses");
 	NOT_AFTER_EDIT();
 	const u32 C = ctx->cfg.max_contacts;
-	const uint4* s_old = ctx->has_sensor ? ctx->sensor_old : nullptr;
-	const uint4* s_cur = ctx->has_sensor ? ctx->sensor_cur : nullptr;
+	const uint4* s_old = ctx->has_sensor ? ctx->sensor_old.p : nullptr;
+	const uint4* s_cur = ctx->has_sensor ? ctx->sensor_cur.p : nullptr;
 	if (ctx->ev_cap)   // the old cache is still intact here
 		launch_contact_events(mk_launch(ctx, stream), GRID(2 * (size_t)C), ctx->flags, ctx->stride, ctx->block_sums, ctx->cache_tags, ctx->sorted, ctx->fin,
-							  ctx->culled_tags, ctx->impulses, s_old, s_cur, ctx->events, ctx->ev_cap, ctx->counts);
-	if (ctx->has_sensor) { k_sensor_keep<<<GRID(ctx->sensor_cap), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sensor_cur, ctx->sensor_old, ctx->counts); ++ctx->launches; }
+							  ctx->culled_tags, ctx->impulses, s_old, s_cur, ctx->events.p, ctx->ev_cap, ctx->counts);
+	if (ctx->has_sensor) { k_sensor_keep<<<GRID(ctx->sensor_cap), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sensor_cur.p, ctx->sensor_old.p, ctx->counts); ++ctx->launches; }
 	k_cache_merge<<<GRID(C), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sorted, ctx->fin.tags, ctx->fin.features, ctx->impulses,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->counts);
 	++ctx->launches;
@@ -851,12 +887,7 @@ int nb_enable_contact_events(nb_context* ctx, uint32_t capacity) {
 	CK(cudaDeviceSynchronize());   // nothing in flight may still write the counters or the buffer
 	ctx->ev_cap = 0;           // off until the buffer below exists (a failed allocation leaves events disabled)
 	++ctx->graph_epoch;        // nb_step's graph re-records with or without the event launches
-	if (capacity > ctx->ev_alloc) {
-		if (ctx->events) { cudaFree(ctx->events); ctx->events = nullptr; ctx->ev_alloc = 0; }
-		void* p = nullptr;
-		CK(cudaMalloc(&p, sizeof(nb_contact_event) * (size_t)capacity));
-		ctx->events = (nb_contact_event*)p; ctx->ev_alloc = capacity;
-	}
+	GROW(ctx->events, capacity, cudaStreamLegacy);   // the device is idle: the stream it waits for does not matter
 	CK(cudaMemset(ctx->counts + CNT_EV_COUNT, 0, 3 * sizeof(u32)));   // count, dropped, step
 	CK(cudaDeviceSynchronize());
 	ctx->ev_cap = capacity;
@@ -872,7 +903,7 @@ int nb_download_contact_events(nb_context* ctx, nb_contact_event* host, uint32_t
 	if (dropped) *dropped = d;
 	if (n > capacity) { ctx->error = "host event buffer too small: " + std::to_string(n) + " events are stored"; return NB_ERR_CAPACITY; }
 	if (n && !host) { ctx->error = "null host event buffer"; return NB_ERR_ARGUMENT; }
-	D2H(host, ctx->events, n, nb_contact_event);
+	D2H(host, ctx->events.p, n, nb_contact_event);
 	CK(cudaMemsetAsync(ctx->counts + CNT_EV_COUNT, 0, 2 * sizeof(u32), (cudaStream_t)stream));   // count, dropped; in stream order
 	CK(cudaStreamSynchronize((cudaStream_t)stream));
 	if (d) { ctx->error = std::to_string(d) + " contact events were dropped: the event buffer was full (raise the nb_enable_contact_events capacity or drain more often)"; return NB_ERR_OVERFLOW; }
@@ -1128,12 +1159,14 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
 		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
-		{ "sensor_pairs", ctx->sensor_keys, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
+		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }
 	// how many times a step graph (nb_step, nb_shard_step) was captured since nb_create
 	if (!strcmp(name, "graph_records")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)ctx->graph_records; if (bytes) *bytes = 4; return NB_OK; }
+	// the device bytes the context and its snapshots hold now, as a uint64_t
+	if (!strcmp(name, "device_bytes")) { if (max_bytes < 8) return NB_ERR_ARGUMENT; *(uint64_t*)dst = ctx->device_bytes; if (bytes) *bytes = 8; return NB_OK; }
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count

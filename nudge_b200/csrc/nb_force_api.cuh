@@ -47,10 +47,21 @@ __global__ void __launch_bounds__(NB_BLOCK) k_body_force_scatter(const nb_body_f
 	}
 }
 
+// The table and its gather buffer, allocated for max_bodies on first use.
+static int ensure_force_tables(nb_context* ctx) {
+	if (!ctx->frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
+	return NB_OK;
+}
+
+// Stored rows are canonical: the staged rows' reserved words are cleared before their copy.
+static void clear_reserved(unsigned char* rows, size_t bytes) {
+	for (size_t i = 0; i < bytes / sizeof(nb_body_force); ++i) reinterpret_cast<nb_body_force*>(rows)[i].reserved = 0;
+}
+
 // Creates the table (every body 0 .. B-1 with the default entry) unless it exists.
 static int ensure_body_forces(nb_context* ctx, cudaStream_t st) {
 	if (ctx->has_frc) return NB_OK;
-	if (!ctx->frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
+	{ int r = ensure_force_tables(ctx); if (r) return r; }
 	if (ctx->B) { k_body_force_defaults<<<GRID(ctx->B), NB_BLOCK, 0, st>>>(ctx->frc, ctx->B); ++ctx->launches; }
 	CK(cudaGetLastError());
 	ctx->has_frc = true;
@@ -63,36 +74,18 @@ extern "C" {
 int nb_set_body_forces(nb_context* ctx, const nb_body_force* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_set_body_forces");
 	if (n && !h) { ctx->error = "null body force list"; return NB_ERR_ARGUMENT; }
-	auto refuse = [&](u32 i, const std::string& why) { ctx->error = "body force " + std::to_string(i) + ": " + why; return NB_ERR_ARGUMENT; };
 	for (u32 i = 0; i < n; ++i) {
-		const u32 b = h[i].body;
-		if (b == 0) return refuse(i, "body 0 is the static world");
-		if (b >= ctx->B) return refuse(i, "body " + std::to_string(b) + " is at or beyond the body count (" + std::to_string(ctx->B) + ")");
-		if (ctx->has_kin && std::binary_search(ctx->kin_list.begin(), ctx->kin_list.end(), b)) return refuse(i, "body " + std::to_string(b) + " is kinematic");
-		if (const char* p = body_force_problem(h[i])) return refuse(i, p);
+		if (int r = check_body(ctx, "body force", i, h[i].body, false)) return r;
+		if (const char* p = body_force_problem(h[i])) { ctx->error = "body force " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
 	}
-	// duplicates: one mark per body in a host byte map that is all zeros between calls (O(n), where a sort of 65,536 entries costs ms)
-	ctx->frc_seen.resize(std::max<size_t>(ctx->frc_seen.size(), ctx->B), 0);
-	bool twice = false;
-	for (u32 i = 0; i < n && !twice; ++i) twice = ctx->frc_seen[h[i].body]++ != 0;
-	for (u32 i = 0; i < n; ++i) ctx->frc_seen[h[i].body] = 0;
-	if (twice) { ctx->error = "a body is listed twice in the body force list"; return NB_ERR_ARGUMENT; }
+	if (int r = bodies_distinct(ctx, "body force", n, [&](u32 i) { return h[i].body; })) return r;
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy (the scatter writes idle counters)
 	{ int r = ensure_body_forces(ctx, st); if (r) return r; }
 	if (!n) return NB_OK;
-	if (n > ctx->frc_rows_cap) {
-		CK(cudaStreamSynchronize(st));   // an earlier scatter may still read the old staging rows
-		if (ctx->frc_rows) cudaFree(ctx->frc_rows);
-		ctx->frc_rows = nullptr; ctx->frc_rows_cap = 0;
-		CK(cudaMalloc(&ctx->frc_rows, sizeof(nb_body_force) * (size_t)n));
-		ctx->frc_rows_cap = n;
-	}
-	// through pageable host memory, which the copy has consumed when it returns: the caller's array may be reused, pinned or not
-	ctx->frc_host.assign(h, h + n);
-	for (nb_body_force& e : ctx->frc_host) e.reserved = 0;
-	CK(cudaMemcpyAsync(ctx->frc_rows, ctx->frc_host.data(), sizeof(nb_body_force) * (size_t)n, cudaMemcpyHostToDevice, st));
-	k_body_force_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->frc_rows, n, ctx->frc, ctx->idle);
+	GROW(ctx->frc_rows, n, st);
+	CK(put_staged(ctx, ctx->frc_rows.p, h, sizeof(nb_body_force) * (size_t)n, st, clear_reserved));
+	k_body_force_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->frc_rows.p, n, ctx->frc, ctx->idle);
 	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;

@@ -71,47 +71,26 @@ __global__ void __launch_bounds__(NB_BLOCK) k_radial_impulse(nb_radial_impulse e
 	}
 }
 
-static void free_impulse_rows(nb_context* ctx) {
-	void* p[] = { ctx->imp_rows, ctx->imp_sb.keys[0], ctx->imp_sb.keys[1] };
-	for (void* q : p) if (q) cudaFree(q);
-	ctx->imp_rows = nullptr; ctx->imp_sb.keys[0] = ctx->imp_sb.keys[1] = nullptr; ctx->imp_cap = 0;
-}
-
 extern "C" {
 
 int nb_apply_body_impulses(nb_context* ctx, const nb_body_impulse* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_apply_body_impulses");
 	if (!n) return NB_OK;
 	if (!h) { ctx->error = "null body impulse list"; return NB_ERR_ARGUMENT; }
-	for (u32 i = 0; i < n; ++i) {
-		const u32 b = h[i].body;
-		if (b == 0) { ctx->error = "body impulse " + std::to_string(i) + ": body 0 is the static world"; return NB_ERR_ARGUMENT; }
-		if (b >= ctx->B) { ctx->error = "body impulse " + std::to_string(i) + ": body " + std::to_string(b) + " is at or beyond the body count (" + std::to_string(ctx->B) + ")"; return NB_ERR_ARGUMENT; }
-		if (ctx->has_kin && std::binary_search(ctx->kin_list.begin(), ctx->kin_list.end(), b)) {
-			ctx->error = "body impulse " + std::to_string(i) + ": body " + std::to_string(b) + " is kinematic (set its velocity with nb_upload_kinematic_bodies)";
-			return NB_ERR_ARGUMENT;
-		}
-	}
+	for (u32 i = 0; i < n; ++i) if (int r = check_body(ctx, "body impulse", i, h[i].body, false)) return r;   // a body may be listed again
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
 	if (!ctx->imp_n) {
 		ALLOC(ctx->imp_n, 1); ALLOC(ctx->imp_sb.hist, 256 * (size_t)ctx->sms); ALLOC(ctx->imp_sb.bar, 2);
 	}
-	if (n > ctx->imp_cap) {
-		CK(cudaStreamSynchronize(st));   // an earlier call may still read the old buffers
-		free_impulse_rows(ctx);
-		CK(cudaMalloc(&ctx->imp_rows, sizeof(nb_body_impulse) * (size_t)n));
-		for (int i = 0; i < 2; ++i) CK(cudaMalloc(&ctx->imp_sb.keys[i], sizeof(u64) * (size_t)n));
-		ctx->imp_cap = n;
-	}
-	// through pageable host memory, which the copy has consumed when it returns: the caller's array may be reused, pinned or not
-	ctx->imp_host.assign(h, h + n);
-	CK(cudaMemcpyAsync(ctx->imp_rows, ctx->imp_host.data(), sizeof(nb_body_impulse) * (size_t)n, cudaMemcpyHostToDevice, st));
+	GROW(ctx->imp_rows, n, st);
+	for (int i = 0; i < 2; ++i) { GROW(ctx->imp_keys[i], n, st); ctx->imp_sb.keys[i] = ctx->imp_keys[i].p; }
+	CK(put_staged(ctx, ctx->imp_rows.p, h, sizeof(nb_body_impulse) * (size_t)n, st));
 	const u32 ib = bits_for(n), bb = bits_for(ctx->B);
-	k_impulse_keys<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows, n, ib, ctx->imp_sb.keys[0], ctx->imp_n);
+	k_impulse_keys<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows.p, n, ib, ctx->imp_sb.keys[0], ctx->imp_n);
 	++ctx->launches;
 	const int cur = nb_radix_sort(mk_launch(ctx, stream), ctx->imp_sb, ctx->imp_n, 0, (int)(ib + bb), false, 0);
-	k_body_impulses<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows, ctx->imp_sb.keys[cur], n, ib, ctx->xf, ctx->props, ctx->mom, ctx->idle);
+	k_body_impulses<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows.p, ctx->imp_sb.keys[cur], n, ib, ctx->xf, ctx->props, ctx->mom, ctx->idle);
 	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;

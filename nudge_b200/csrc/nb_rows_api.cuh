@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows,
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st) {
 	for (u32 l = 0; l < ctx->urow_levels; ++l) {
 		const u32 b = ctx->urow_level_off[l], e = ctx->urow_level_off[l + 1];
-		if (e > b) { k_user_rows<<<GRID(e - b), NB_BLOCK, 0, st>>>(ctx->urows, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm); ++ctx->launches; }
+		if (e > b) { k_user_rows<<<GRID(e - b), NB_BLOCK, 0, st>>>(ctx->urows.p, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm); ++ctx->launches; }
 	}
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -95,11 +95,7 @@ extern "C" {
 int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, uint32_t n, void* stream) {
 	cudaStream_t st = (cudaStream_t)stream;
 	CK(cudaStreamSynchronize(st));
-	if (n > ctx->urow_cap) {
-		nb_constraint_row* p = nullptr;
-		ALLOC(p, (size_t)n + n / 2 + 64);
-		ctx->urows = p; ctx->urow_cap = n + n / 2 + 64;
-	}
+	if (n > ctx->urows.cap) GROW(ctx->urows, (size_t)n + n / 2 + 64, st);   // with headroom for a set that grows a little
 	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_ab.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->graph_epoch;
 	if (!n) return NB_OK;
 	std::vector<nb_body_pair> ab(n);
@@ -115,7 +111,7 @@ int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, ui
 	if (levels > 4096) { ctx->error = "constraint rows form a dependency chain longer than 4096 levels: reorder them (e.g. red-black along a chain)"; ctx->urow_n = 0; return NB_ERR_CAPACITY; }
 	std::vector<nb_constraint_row> sorted(n);
 	for (u32 i = 0; i < n; ++i) sorted[order[i]] = rows[i];
-	CK(cudaMemcpy(ctx->urows, sorted.data(), sizeof(nb_constraint_row) * n, cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(ctx->urows.p, sorted.data(), sizeof(nb_constraint_row) * n, cudaMemcpyHostToDevice));
 	ctx->urow_level_off.swap(level_off); ctx->urow_order.swap(order); ctx->urow_ab.swap(ab);
 	ctx->urow_levels = levels;
 	return NB_OK;
@@ -127,7 +123,7 @@ int nb_download_constraint_rows(nb_context* ctx, nb_constraint_row* rows, uint32
 	if (!n) return NB_OK;
 	CK(cudaStreamSynchronize((cudaStream_t)stream));
 	std::vector<nb_constraint_row> sorted(n);
-	CK(cudaMemcpy(sorted.data(), ctx->urows, sizeof(nb_constraint_row) * n, cudaMemcpyDeviceToHost));
+	CK(cudaMemcpy(sorted.data(), ctx->urows.p, sizeof(nb_constraint_row) * n, cudaMemcpyDeviceToHost));
 	for (u32 i = 0; i < n; ++i) rows[i] = sorted[ctx->urow_order[i]];
 	return NB_OK;
 }

@@ -48,10 +48,10 @@ __global__ void __launch_bounds__(NB_BLOCK) k_snapshot_copy(const __grid_constan
 struct nb_snapshot {
 	nb_context* ctx;
 	bool saved;
-	unsigned char* arena; std::vector<size_t> off;   // the fixed sections, by position in snapshot_sections; words = the count words
+	DevBuf<unsigned char> arena; std::vector<size_t> off;   // the fixed sections, by position in snapshot_sections; words = the count words
 	u32* words;
-	nb_constraint_row* rows; u32 rows_cap;           // user rows in device order
-	uint4* overlaps; u32 overlaps_cap;               // the sensor overlap list
+	DevBuf<nb_constraint_row> rows;                  // user rows in device order
+	DevBuf<uint4> overlaps;                          // the sensor overlap list
 	// the host side at the save
 	NbStateHeader h; StateShape shape;
 	u32 urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order; std::vector<nb_body_pair> urow_ab;
@@ -66,14 +66,14 @@ struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool presen
 static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 urow_n, u32 conn_probe) {
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
-	auto at = [&](size_t i) -> void* { return s ? s->arena + s->off[i] : nullptr; };
+	auto at = [&](size_t i) -> void* { return s ? s->arena.p + s->off[i] : nullptr; };
 	for (const StateSection& x : state_sections(ctx, h, hc, false))
 		p.push_back({ x.dev, at(p.size()), x.size, x.count, x.present && x.dev != nullptr, x.word });
 	p.push_back({ ctx->kind, at(p.size()), 1, h.bodies, h.reserved[4] != 0, -1 });
 	p.push_back({ ctx->conn_keys, at(p.size()), 8, conn_probe, conn_probe != 0, -1 });
 	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s ? s->words + j : nullptr, 4, 1, true, -1 });
-	p.push_back({ ctx->urows, s ? s->rows : nullptr, sizeof(nb_constraint_row), urow_n, urow_n != 0, -1 });
-	p.push_back({ ctx->sensor_old, s ? s->overlaps : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
+	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), urow_n, urow_n != 0, -1 });
+	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
 	return p;
 }
 static const size_t kSnapFixed = 18 + 2;   // the state file's sections, the kind bytes and the key list: the sections in the arena
@@ -85,7 +85,7 @@ static int snapshot_table(nb_context* ctx, const nb_snapshot* s, bool save, Snap
 	const u32 probe = (s->shape.filter_flags & NB_FILTER_SKIP_CONNECTED) ? s->shape.nconn : 0;
 	std::vector<SnapPart> parts = snapshot_sections(ctx, s, s->h, s->urow_n, probe);
 	if (!save && s->shape.has_sensor) {
-		parts.push_back({ ctx->sensor_cur, s->overlaps, sizeof(uint4), s->h.reserved[3], true, CNT_SENSOR_OLD });
+		parts.push_back({ ctx->sensor_cur.p, s->overlaps.p, sizeof(uint4), s->h.reserved[3], true, CNT_SENSOR_OLD });
 		parts.push_back({ ctx->counts + CNT_SENSOR_HITS, s->words + 2, 4, 1, true, -1 });
 	}
 	t.n = 0;
@@ -113,14 +113,8 @@ static int snapshot_launch(nb_context* ctx, const SnapTable& t, cudaStream_t st)
 	return NB_OK;
 }
 
-static void snapshot_free(nb_snapshot* s) {
-	if (s->arena) cudaFree(s->arena);
-	if (s->rows) cudaFree(s->rows);
-	if (s->overlaps) cudaFree(s->overlaps);
-	delete s;
-}
 static void free_snapshots(nb_context* ctx) {
-	for (nb_snapshot* s : ctx->snapshots) snapshot_free(s);
+	for (nb_snapshot* s : ctx->snapshots) delete s;
 	ctx->snapshots.clear();
 }
 
@@ -143,9 +137,11 @@ int nb_snapshot_create(nb_context* ctx, nb_snapshot** out) {
 	size_t bytes = 0;
 	const std::vector<SnapPart> parts = snapshot_sections(ctx, nullptr, cap, 0, c.max_connections);
 	for (size_t i = 0; i < kSnapFixed; ++i) { s->off.push_back(bytes); bytes += (parts[i].size * parts[i].count + 15) & ~(size_t)15; }
-	const cudaError_t e = cudaMalloc(&s->arena, bytes + 16);
+	const cudaError_t e = cudaMalloc(&s->arena.p, bytes + 16);
 	if (e != cudaSuccess) { delete s; ctx->error = std::string("nb_snapshot_create: cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
-	s->words = reinterpret_cast<u32*>(s->arena + bytes);
+	s->arena.cap = bytes + 16;
+	ctx->device_bytes += s->arena.cap;
+	s->words = reinterpret_cast<u32*>(s->arena.p + bytes);
 	ctx->snapshots.push_back(s);
 	*out = s;
 	return NB_OK;
@@ -153,9 +149,10 @@ int nb_snapshot_create(nb_context* ctx, nb_snapshot** out) {
 
 void nb_snapshot_destroy(nb_snapshot* s) {
 	if (!s) return;
-	std::vector<nb_snapshot*>& v = s->ctx->snapshots;
-	v.erase(std::remove(v.begin(), v.end(), s), v.end());
-	snapshot_free(s);   // cudaFree waits for the work that may still read it
+	nb_context* ctx = s->ctx;
+	ctx->snapshots.erase(std::remove(ctx->snapshots.begin(), ctx->snapshots.end(), s), ctx->snapshots.end());
+	ctx->device_bytes -= s->arena.cap + sizeof(nb_constraint_row) * s->rows.cap + sizeof(uint4) * s->overlaps.cap;
+	delete s;   // cudaFree waits for the work that may still read it
 }
 
 int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
@@ -164,22 +161,8 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	if (ctx->in_step && !ctx->scene_edited) { ctx->error = "nb_snapshot_save: between nb_collide and the nb_advance that ends its step"; return NB_ERR_ARGUMENT; }
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // the copy reads the momentum and property rows
-	const u32 nov = ctx->has_sensor ? ctx->sensor_cap : 0;
-	if (ctx->urow_n > s->rows_cap || nov > s->overlaps_cap) {   // grown: the only save that synchronises and allocates
-		CK(cudaStreamSynchronize(st));
-		if (ctx->urow_n > s->rows_cap) {
-			if (s->rows) cudaFree(s->rows);
-			s->rows = nullptr; s->rows_cap = 0;
-			CK(cudaMalloc(&s->rows, sizeof(nb_constraint_row) * (size_t)ctx->urow_n));
-			s->rows_cap = ctx->urow_n;
-		}
-		if (nov > s->overlaps_cap) {
-			if (s->overlaps) cudaFree(s->overlaps);
-			s->overlaps = nullptr; s->overlaps_cap = 0;
-			CK(cudaMalloc(&s->overlaps, sizeof(uint4) * (size_t)nov));
-			s->overlaps_cap = nov;
-		}
-	}
+	// grown: the only save that synchronises and allocates
+	GROW(s->rows, ctx->urow_n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
 	s->urow_n = ctx->urow_n; s->urow_levels = ctx->urow_levels;
@@ -197,17 +180,11 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (!s->saved) { ctx->error = "nb_snapshot_restore: the snapshot was never saved"; return NB_ERR_ARGUMENT; }
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // a pending side copy must not land on the restored rows
-	// tables the context has never had: created here, once (the only restore that synchronises and allocates)
-	const bool grow = (s->shape.has_frc && !ctx->frc) || (!s->shape.kin.empty() && !ctx->kind) || s->urow_n > ctx->urow_cap ||
-					  (s->shape.has_sensor && s->shape.sensor_cap > ctx->sensor_alloc);
-	if (grow) {
-		CK(cudaStreamSynchronize(st));
-		if (s->shape.has_frc && !ctx->frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
-		if (!s->shape.kin.empty() && !ctx->kind) ALLOC(ctx->kind, ctx->cfg.max_bodies);
-		if (s->urow_n > ctx->urow_cap) { nb_constraint_row* p = nullptr; ALLOC(p, (size_t)s->urow_n); ctx->urows = p; ctx->urow_cap = s->urow_n; }
-		if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap); if (r) return r; }
-		CK(cudaDeviceSynchronize());   // ALLOC's clears run on the legacy stream
-	}
+	// tables the context has never had, or has too small: created or grown here (the only restore that synchronises and allocates)
+	if (s->shape.has_frc) { int r = ensure_force_tables(ctx); if (r) return r; }
+	if (!s->shape.kin.empty()) { int r = ensure_kind_table(ctx); if (r) return r; }
+	GROW(ctx->urows, s->urow_n, st);
+	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, false, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }

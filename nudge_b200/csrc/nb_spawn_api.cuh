@@ -166,13 +166,10 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	if (ctx->sharded) { ctx->error = "nb_remove_bodies: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
 	if (!n) return NB_OK;
 	if (!h) { ctx->error = "null body list"; return NB_ERR_ARGUMENT; }
+	for (u32 i = 0; i < n; ++i) if (int r = check_body(ctx, "removed body", i, h[i], true)) return r;
+	if (int r = bodies_distinct(ctx, "removed body", n, [&](u32 i) { return h[i]; })) return r;
 	std::vector<u32> list(h, h + n);
-	for (u32 i = 0; i < n; ++i) {
-		if (list[i] == 0) { ctx->error = "body 0 is the static world and cannot be removed"; return NB_ERR_ARGUMENT; }
-		if (list[i] >= ctx->B) { ctx->error = "body " + std::to_string(list[i]) + " is at or beyond the body count (" + std::to_string(ctx->B) + ")"; return NB_ERR_ARGUMENT; }
-	}
-	std::sort(list.begin(), list.end());
-	if (std::adjacent_find(list.begin(), list.end()) != list.end()) { ctx->error = "a body is listed twice"; return NB_ERR_ARGUMENT; }
+	std::sort(list.begin(), list.end());   // for the binary searches of the remap
 	const u32 S = ctx->stride, B = ctx->B, nboxes = ctx->nboxes, K = ctx->nboxes + ctx->nspheres, nconn = ctx->nconn;
 	// the body map covers bodies below B: a row or connection naming a body beyond it (which their uploads allow) has no new index
 	for (u32 i = 0; i < ctx->urow_n; ++i)
@@ -207,22 +204,10 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // the gathers read the momentum and property rows
-	if (staging.size() > ctx->spawn_idx_cap) {
-		CK(cudaStreamSynchronize(st));   // an earlier call may still read the old buffer
-		if (ctx->spawn_idx) cudaFree(ctx->spawn_idx);
-		ctx->spawn_idx = nullptr; ctx->spawn_idx_cap = 0;
-		CK(cudaMalloc(&ctx->spawn_idx, sizeof(u32) * staging.size()));
-		ctx->spawn_idx_cap = (u32)staging.size();
-	}
-	if (nrows > ctx->urows_spare_cap) {
-		CK(cudaStreamSynchronize(st));
-		if (ctx->urows_spare) cudaFree(ctx->urows_spare);
-		ctx->urows_spare = nullptr; ctx->urows_spare_cap = 0;
-		CK(cudaMalloc(&ctx->urows_spare, sizeof(nb_constraint_row) * (size_t)nrows));
-		ctx->urows_spare_cap = nrows;
-	}
+	GROW(ctx->spawn_idx, staging.size(), st);
+	GROW(ctx->urows_spare, nrows, st);
 	// pageable staging: the copy has consumed it when cudaMemcpyAsync returns
-	CK(cudaMemcpyAsync(ctx->spawn_idx, staging.data(), sizeof(u32) * staging.size(), cudaMemcpyHostToDevice, st));
+	CK(cudaMemcpyAsync(ctx->spawn_idx.p, staging.data(), sizeof(u32) * staging.size(), cudaMemcpyHostToDevice, st));
 	Launch L = mk_launch(ctx, stream);
 	uint8_t* rem = reinterpret_cast<uint8_t*>(ctx->offs);
 	u32* flags = ctx->flags;
@@ -231,7 +216,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	const uint8_t* kind = kin_table(ctx);
 	const u32 kshift = bits_for(B) + 1;
 	CK(cudaMemsetAsync(rem, 0, B, st));
-	k_spawn_mark<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->spawn_idx, n, rem);
+	k_spawn_mark<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->spawn_idx.p, n, rem);
 	k_spawn_flags<<<GRID(std::max(B, std::max(K, nconn))), NB_BLOCK, 0, st>>>(B, nboxes, K, nconn, rem, ctx->box_xf, ctx->box_tags, ctx->sph_xf, ctx->sph_tags,
 		ctx->conn, kind, ctx->idle, flags, S, ctx->sb.keys[0], kshift, counts);
 	ctx->launches += 2;
@@ -259,8 +244,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		k_spawn_conns<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(nconn, flags + 3 * (size_t)S, ctx->block_sums, map, ctx->conn, reinterpret_cast<uint2*>(ctx->conn_scratch));
 		++ctx->launches;
 	}
-	if (nrows) { k_spawn_rows<<<GRID(nrows), NB_BLOCK, 0, st>>>(ctx->urows, ctx->spawn_idx + n, nrows, map, ctx->urows_spare); ++ctx->launches; }
-	if (ctx->has_sensor) { k_spawn_overlaps<<<GRID(2 * (size_t)ctx->sensor_cap), NB_BLOCK, 0, st>>>(ctx->sensor_cur, ctx->sensor_old, ctx->sensor_cap, map, counts); ++ctx->launches; }
+	if (nrows) { k_spawn_rows<<<GRID(nrows), NB_BLOCK, 0, st>>>(ctx->urows.p, ctx->spawn_idx.p + n, nrows, map, ctx->urows_spare.p); ++ctx->launches; }
+	if (ctx->has_sensor) { k_spawn_overlaps<<<GRID(2 * (size_t)ctx->sensor_cap), NB_BLOCK, 0, st>>>(ctx->sensor_cur.p, ctx->sensor_old.p, ctx->sensor_cap, map, counts); ++ctx->launches; }
 	CK(cudaGetLastError());
 	u32 c[CNT_SPAWN__N - CNT_SPAWN_B];
 	CK(cudaMemcpyAsync(c, counts + CNT_SPAWN_B, sizeof(c), cudaMemcpyDeviceToHost, st));
@@ -280,7 +265,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	if (ctx->has_filter) CK(d2d(ctx->filter, ctx->order, 4 * ((size_t)nb2 + ns2)));
 	if (ctx->has_sensor) CK(d2d(ctx->sensor, ctx->rank, (size_t)nb2 + ns2));
 	CK(d2d(ctx->conn, ctx->conn_scratch, sizeof(nb_body_pair) * (size_t)nc2));
-	CK(d2d(ctx->urows, ctx->urows_spare, sizeof(nb_constraint_row) * (size_t)nrows));
+	CK(d2d(ctx->urows.p, ctx->urows_spare.p, sizeof(nb_constraint_row) * (size_t)nrows));
 	ctx->B = B2; ctx->nboxes = nb2; ctx->nspheres = ns2; ctx->nconn = nc2;
 	ctx->conn_host.swap(conn);
 	ctx->tagbits = bits_for((u64)maxtag + 1);
@@ -324,31 +309,25 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 	if (!n && !nb && !ns) return NB_OK;
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
-	// through pageable host memory, which each copy has consumed when it returns: the caller's arrays may be reused, pinned or not
-	std::vector<unsigned char> stage;
-	auto put = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
-		if (!bytes) return cudaSuccess;
-		stage.assign((const unsigned char*)src, (const unsigned char*)src + bytes);
-		return cudaMemcpyAsync(dst, stage.data(), bytes, cudaMemcpyHostToDevice, st);
-	};
-	CK(put(ctx->xf + B0, bodies ? bodies->transforms : nullptr, sizeof(nb_transform) * (size_t)n));
-	CK(put(ctx->props + B0, bodies ? bodies->properties : nullptr, sizeof(nb_body_properties) * (size_t)n));
-	CK(put(ctx->mom + B0, bodies ? bodies->momentum : nullptr, sizeof(nb_body_momentum) * (size_t)n));
-	CK(put(ctx->idle + B0, bodies ? bodies->idle_counters : nullptr, (size_t)n));
+	// every host array through the staging copy: the caller's arrays may be reused when the call returns, pinned or not
+	CK(put_staged(ctx, ctx->xf + B0, bodies ? bodies->transforms : nullptr, sizeof(nb_transform) * (size_t)n, st));
+	CK(put_staged(ctx, ctx->props + B0, bodies ? bodies->properties : nullptr, sizeof(nb_body_properties) * (size_t)n, st));
+	CK(put_staged(ctx, ctx->mom + B0, bodies ? bodies->momentum : nullptr, sizeof(nb_body_momentum) * (size_t)n, st));
+	CK(put_staged(ctx, ctx->idle + B0, bodies ? bodies->idle_counters : nullptr, (size_t)n, st));
 	if (ctx->kind && n) CK(cudaMemsetAsync(ctx->kind + B0, 0, n, st));   // new bodies are dynamic
 	std::vector<nb_body_force> frc;   // with the default force entry
 	if (ctx->has_frc && n) {
 		for (u32 i = 0; i < n; ++i) frc.push_back(default_body_force(B0 + i));
-		CK(put(ctx->frc + B0, frc.data(), sizeof(nb_body_force) * (size_t)n));
+		CK(put_staged(ctx, ctx->frc + B0, frc.data(), sizeof(nb_body_force) * (size_t)n, st));
 	}
 	const u32 ob = ctx->nboxes, os = ctx->nspheres;
 	if (nb) {
-		CK(put(ctx->box_tags + ob, colliders->boxes.tags, 4 * (size_t)nb)); CK(put(ctx->box_data + ob, colliders->boxes.data, sizeof(nb_box_collider) * (size_t)nb));
-		CK(put(ctx->box_xf + ob, colliders->boxes.transforms, sizeof(nb_transform) * (size_t)nb));
+		CK(put_staged(ctx, ctx->box_tags + ob, colliders->boxes.tags, 4 * (size_t)nb, st)); CK(put_staged(ctx, ctx->box_data + ob, colliders->boxes.data, sizeof(nb_box_collider) * (size_t)nb, st));
+		CK(put_staged(ctx, ctx->box_xf + ob, colliders->boxes.transforms, sizeof(nb_transform) * (size_t)nb, st));
 	}
 	if (ns) {
-		CK(put(ctx->sph_tags + os, colliders->spheres.tags, 4 * (size_t)ns)); CK(put(ctx->sph_data + os, colliders->spheres.data, sizeof(nb_sphere_collider) * (size_t)ns));
-		CK(put(ctx->sph_xf + os, colliders->spheres.transforms, sizeof(nb_transform) * (size_t)ns));
+		CK(put_staged(ctx, ctx->sph_tags + os, colliders->spheres.tags, 4 * (size_t)ns, st)); CK(put_staged(ctx, ctx->sph_data + os, colliders->spheres.data, sizeof(nb_sphere_collider) * (size_t)ns, st));
+		CK(put_staged(ctx, ctx->sph_xf + os, colliders->spheres.transforms, sizeof(nb_transform) * (size_t)ns, st));
 	}
 	// per-collider tables [old boxes][new boxes][old spheres][new spheres]: the old sphere entries move up by nb through a staging copy in
 	// collide-stage scratch (the two ranges may overlap)
@@ -357,8 +336,8 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 			CK(cudaMemcpyAsync(ctx->order, ctx->filter + ob, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
 			CK(cudaMemcpyAsync(ctx->filter + ob + nb, ctx->order, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
 		}
-		CK(put(ctx->filter + ob, f, 4 * (size_t)nb));
-		CK(put(ctx->filter + ob + nb + os, f + nb, 4 * (size_t)ns));
+		CK(put_staged(ctx, ctx->filter + ob, f, 4 * (size_t)nb, st));
+		CK(put_staged(ctx, ctx->filter + ob + nb + os, f + nb, 4 * (size_t)ns, st));
 	}
 	if (ctx->has_sensor && nb + ns) {
 		uint8_t* s = ctx->sensor;
@@ -368,8 +347,8 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 		}
 		std::vector<uint8_t> flags01(nb + ns);
 		for (u32 i = 0; i < nb + ns; ++i) flags01[i] = sf[i] ? 1 : 0;
-		CK(put(s + ob, flags01.data(), nb));
-		CK(put(s + ob + nb + os, flags01.data() + nb, ns));
+		CK(put_staged(ctx, s + ob, flags01.data(), nb, st));
+		CK(put_staged(ctx, s + ob + nb + os, flags01.data() + nb, ns, st));
 	}
 	ctx->B = B2; ctx->nboxes = ob + nb; ctx->nspheres = os + ns;
 	ctx->tagbits = std::max(ctx->tagbits, bits_for((u64)maxtag + 1));   // bits_for is monotone: the same as over all tags
