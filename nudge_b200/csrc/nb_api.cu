@@ -48,7 +48,6 @@ struct nb_context {
 	u32 slots_per_bucket;
 	int coop_blocks_solve;
 	u64* keybits;  // OR, AND of the Morton codes of the current collide
-	bool defer_warm_start;  // nb_step: the warm start runs with the sweeps (nb_apply_impulses), not in setup
 	StepGraph graph; bool capturing;  // nb_step's graph; capturing: run_graphed is recording a step of this context
 	unsigned long long graph_epoch;   // in the graphs' key: bumped by every change of which kernels a step launches or of their arguments
 	u32* chain_start; u32* chain_len;  // per body: segment cursor (the segment's end once k_chain_scatter ran) / number of chain entries
@@ -311,16 +310,31 @@ static int run_graphed(nb_context* ctx, StepGraph& g, cudaStream_t st, float tim
 	return NB_OK;
 }
 
+// One sub-step (example/main.cpp:274-328) of nb_step and nb_shard_step around their solve section `solve()`, which sets up the contact
+// rows and sweeps them: nb_step's step_solve, or nb_shard_step's shard_solve with the ghost exchange.
+template<class Solve>
+static int step_body(nb_context* ctx, float time_step, float gravity, float damping, void* stream, Solve solve) {
+	int r;
+	if ((r = nb_collide(ctx, stream))) return r;
+	if ((r = nb_apply_gravity_damping(ctx, time_step, gravity, damping, stream))) return r;
+	if ((r = nb_read_cached_impulses(ctx, stream))) return r;
+	if ((r = solve())) return r;
+	if ((r = nb_update_cached_impulses(ctx, stream))) return r;
+	if ((r = nb_write_cached_impulses(ctx, stream))) return r;
+	return nb_advance(ctx, time_step, stream);
+}
+
 // The connected opt-out's lookup: the connection keys min(a,b) | max(a,b) << 32, radix sorted on the device, for the binary search of
 // the broadphase (nb_collide.cuh, connected()).  Rebuilt when connections are uploaded or loaded and when the flag is set; never per step.
 static int build_conn_lookup(nb_context* ctx, cudaStream_t st) {
 	const u32 n = (ctx->filter_flags & NB_FILTER_SKIP_CONNECTED) ? ctx->nconn : 0;
 	ctx->conn_probe = n;
 	if (!n) return NB_OK;
-	k_conn_keys<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->conn, n, ctx->conn_scratch); ++ctx->launches;
+	const Launch L = mk_launch(ctx, st);
+	launch_grid(L, k_conn_keys, GRID(n), ctx->conn, n, ctx->conn_scratch);
 	CK(cudaMemcpyAsync(ctx->conn_sort_n, &n, 4, cudaMemcpyHostToDevice, st));
 	SortBuffers cs = { { ctx->conn_scratch, ctx->conn_keys }, { nullptr, nullptr }, ctx->sb.hist, ctx->sb.bar };
-	nb_radix_sort(mk_launch(ctx, st), cs, ctx->conn_sort_n, 0, 64, false, 0);   // the result lands in keys[1] = conn_keys
+	nb_radix_sort(L, cs, ctx->conn_sort_n, 0, 64, false, 0);   // the result lands in keys[1] = conn_keys
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -361,20 +375,16 @@ static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pair
 
 // The sensor pairs' overlaps of one collide (nb_collide.cuh, below k_np_emit): test, compact, sort by key, gather.  5 launches.
 static void launch_sensor_overlaps(nb_context* ctx, const Launch& L) {
-	cudaStream_t st = L.stream;
 	u32* counts = ctx->counts;
 	const u32 cap = ctx->sensor_cap;
-	k_sensor_np<<<GRID((size_t)cap * 4), NB_BLOCK, 0, st>>>(ctx->sensor_keys.p, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
+	launch_grid(L, k_sensor_np, GRID((size_t)cap * 4), ctx->sensor_keys.p, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
 		ctx->col_tag, ctx->col_body, ctx->flags, counts);
-	++ctx->launches;
 	nb_scan_reduce<1>(L, ctx->flags, ctx->stride, counts + CNT_SENSOR_PAIRS, 0, ctx->block_sums, counts + CNT_SENSOR_HITS);
-	k_sensor_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->sensor_keys.p, ctx->kbits, ctx->col_tag,
+	launch_grid(L, k_sensor_compact, NB_SCAN_GRID, ctx->flags, ctx->block_sums, ctx->sensor_keys.p, ctx->kbits, ctx->col_tag,
 		ctx->sensor_sb.keys[0], ctx->sensor_sb.vals[0], counts);
-	++ctx->launches;
 	const int cur = nb_radix_sort(L, ctx->sensor_sb, counts + CNT_SENSOR_HITS, 0, (int)ctx->tagbits, true, 0, 32, (int)(32 + ctx->tagbits));
-	k_sensor_gather<<<GRID(cap), NB_BLOCK, 0, st>>>(ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys.p, ctx->kbits, ctx->col_tag, ctx->col_body,
+	launch_grid(L, k_sensor_gather, GRID(cap), ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys.p, ctx->kbits, ctx->col_tag, ctx->col_body,
 		ctx->sensor_cur.p, counts);
-	++ctx->launches;
 }
 
 extern "C" {
@@ -382,16 +392,14 @@ extern "C" {
 int nb_pack_momentum(nb_context* ctx, const uint32_t* dev_indices, uint32_t n, void* dev_out, void* stream) {
 	if (!n) return NB_OK;
 	JOIN_UPLOADS();
-	k_pack_rows<<<GRID(2 * n), NB_BLOCK, 0, (cudaStream_t)stream>>>((const float4*)ctx->mom, dev_indices, n, (float4*)dev_out);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, stream), k_pack_rows, GRID(2 * n), (const float4*)ctx->mom, dev_indices, n, (float4*)dev_out);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 int nb_unpack_momentum(nb_context* ctx, const uint32_t* dev_indices, const uint32_t* dev_sources, uint32_t n, const void* dev_in, void* stream) {
 	if (!n) return NB_OK;
 	JOIN_UPLOADS();
-	k_unpack_rows<<<GRID(2 * n), NB_BLOCK, 0, (cudaStream_t)stream>>>((float4*)ctx->mom, dev_indices, dev_sources, n, (const float4*)dev_in);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, stream), k_unpack_rows, GRID(2 * n), (float4*)ctx->mom, dev_indices, dev_sources, n, (const float4*)dev_in);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -609,8 +617,7 @@ int nb_upload_kinematic_bodies(nb_context* ctx, const nb_kinematic_body* h, uint
 	const bool same = ctx->has_kin && list == ctx->kin_list;
 	if (!same) CK(cudaMemsetAsync(ctx->kind, 0, ctx->cfg.max_bodies, st));
 	CK(put_staged(ctx, ctx->kin_rows.p, h, sizeof(nb_kinematic_body) * (size_t)n, st));
-	k_kinematic_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->kin_rows.p, n, ctx->mom, ctx->kind);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, st), k_kinematic_scatter, GRID(n), ctx->kin_rows.p, n, ctx->mom, ctx->kind);
 	CK(cudaGetLastError());
 	if (!same) { ctx->has_kin = true; ctx->kin_list.swap(list); ++ctx->graph_epoch; }   // nb_step's graph re-records with the table
 	return NB_OK;
@@ -728,74 +735,63 @@ int nb_collide(nb_context* ctx, void* stream) {
 	u32* counts = ctx->counts;
 	uint8_t* kind = ctx->has_kin ? ctx->kind : nullptr;
 	if (kind) JOIN_UPLOADS();   // k_uf_init reads the kinematic bodies' momentum rows
-	k_reset_collide<<<1, 32, 0, st>>>(counts, K, ctx->keybits); ++ctx->launches;
+	launch(L, k_reset_collide, 1, 32, 0, counts, K, ctx->keybits);
 	if (K == 0 || B == 0) return NB_OK;
-	k_collider_world<<<GRID(K), NB_BLOCK, 0, st>>>(ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
+	launch_grid(L, k_collider_world, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
 		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, kind, ctx->has_sensor ? ctx->sensor : nullptr, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
-	k_morton<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->aabb_min, ctx->aabb_max, counts, ctx->sb.keys[0], ctx->sb.vals[0], ctx->keybits);
-	ctx->launches += 2;
+	launch_grid(L, k_morton, GRID(K), K, ctx->aabb_min, ctx->aabb_max, counts, ctx->sb.keys[0], ctx->sb.vals[0], ctx->keybits);
 	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
 	int cur = nb_radix_sort(L, ctx->sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, ctx->keybits);
-	k_leaves<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->aabb_min, ctx->aabb_max, ctx->order, ctx->rank, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, counts);
-	++ctx->launches;
+	launch_grid(L, k_leaves, GRID(K), K, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->aabb_min, ctx->aabb_max, ctx->order, ctx->rank, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, counts);
 	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
-	k_grid_build<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
+	launch_grid(L, k_grid_build, GRID(K), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
 	const uint8_t* sensor = ctx->has_sensor ? ctx->sensor : nullptr;   // null: the kernels never touch the sensor list
-	(kind ? k_grid_pairs<true> : k_grid_pairs<false>)<<<GRID((size_t)K * 32), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
+	launch_grid(L, kind ? k_grid_pairs<true> : k_grid_pairs<false>, GRID((size_t)K * 32), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
 		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-	k_large_pairs<<<GRID(K), NB_BLOCK, 0, st>>>(K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
+	launch_grid(L, k_large_pairs, GRID(K), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
 		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-	ctx->launches += 3;
 	// nudge.cpp:3498; the sort also clamps CNT_PAIRS to the capacity (the overflow bit is already set by emit_pair)
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);
 	ctx->pair_keys = ctx->sb.keys[cur];
-	if (ctx->debug) { k_copy_u64<<<GRID(ctx->cfg.max_pairs), NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->pair_keys_debug, counts + CNT_PAIRS); ++ctx->launches; }
+	if (ctx->debug) launch_grid(L, k_copy_u64, GRID(ctx->cfg.max_pairs), ctx->pair_keys, ctx->pair_keys_debug, counts + CNT_PAIRS);
 
 	// coarse islands (nudge.cpp:3500-3703)
 	const u32 P = ctx->cfg.max_pairs, S = ctx->stride;
-	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B); ++ctx->launches;
-	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn); ++ctx->launches; }
-	k_uf_union_pairs<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->pair_keys, ctx->kbits, ctx->col_body, counts);
-	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
-	k_pair_flags<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->kbits, nboxes, ctx->col_body, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
-	ctx->launches += 3;
+	launch_grid(L, k_uf_init, GRID(B), ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B);
+	if (ctx->nconn) launch_grid(L, k_uf_union_conn, GRID(ctx->nconn), ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn);
+	launch_grid(L, k_uf_union_pairs, GRID(P), ctx->parent, ctx->taint, ctx->idle, kind, ctx->pair_keys, ctx->kbits, ctx->col_body, counts);
+	launch_grid(L, k_uf_flatten_active, GRID(B), ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
+	launch_grid(L, k_pair_flags, GRID(P), ctx->pair_keys, ctx->kbits, nboxes, ctx->col_body, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
 	nb_scan_reduce<5>(L, ctx->flags, S, counts + CNT_PAIRS, 0, ctx->block_sums, counts + CNT_LIVE0);  // -> LIVE0..3, SLEEP_COARSE
-	k_partition<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->pair_keys, ctx->kbits, ctx->flags, ctx->block_sums, S, ctx->col_tag, ctx->live, ctx->sleeping, counts);
-	++ctx->launches;
+	launch_grid(L, k_partition, NB_SCAN_GRID, ctx->pair_keys, ctx->kbits, ctx->flags, ctx->block_sums, S, ctx->col_tag, ctx->live, ctx->sleeping, counts);
 
 	// narrowphase: count, scan, emit (nudge.cpp:3753-3786)
-	k_np_faces<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->live, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag, ctx->flags, S, ctx->np_pen, ctx->np_info, counts);
-	++ctx->launches;
+	launch_grid(L, k_np_faces, GRID(P), ctx->live, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag, ctx->flags, S, ctx->np_pen, ctx->np_info, counts);
 	nb_scan_reduce<1>(L, ctx->flags + 3 * (size_t)S, S, counts + CNT_LIVE0, 0, ctx->block_sums, counts + CNT_SURV);
-	k_np_list<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, S, ctx->np_list, counts);
-	k_np_clip<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->live, ctx->np_list, ctx->np_pen, ctx->np_info, ctx->world_xf, ctx->box_data, ctx->col_tag, ctx->flags, S,
+	launch_grid(L, k_np_list, NB_SCAN_GRID, ctx->flags, ctx->block_sums, S, ctx->np_list, counts);
+	launch_grid(L, k_np_clip, GRID(P), ctx->live, ctx->np_list, ctx->np_pen, ctx->np_info, ctx->world_xf, ctx->box_data, ctx->col_tag, ctx->flags, S,
 		ctx->fin /* scratch: rewritten by k_contact_compact below */, ctx->np_start, ctx->cfg.max_contacts, counts);
-	ctx->launches += 2;
 	nb_scan<3>(L, ctx->flags, ctx->offs, S, counts + CNT_LIVE_TOTAL, 0, ctx->block_sums, counts + CNT_FACE);  // -> FACE, EDGE, OTHER
-	k_np_emit<<<GRID(P), NB_BLOCK, 0, st>>>(ctx->live, ctx->np_list, ctx->np_start, ctx->fin, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag,
+	launch_grid(L, k_np_emit, GRID(P), ctx->live, ctx->np_list, ctx->np_start, ctx->fin, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag,
 		ctx->flags, ctx->offs, S, ctx->staged, ctx->cfg.max_contacts, counts);
-	++ctx->launches;
 
 	// fine islands, active bodies, contact compaction (nudge.cpp:3788-4006)
 	const u32 C = ctx->cfg.max_contacts;
-	k_uf_init<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B); ++ctx->launches;
-	if (ctx->nconn) { k_uf_union_conn<<<GRID(ctx->nconn), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn); ++ctx->launches; }
-	k_uf_union_contacts<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->parent, ctx->taint, ctx->idle, kind, ctx->staged.bodies, counts);
-	k_uf_flatten_active<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
-	k_body_flags<<<GRID(B), NB_BLOCK, 0, st>>>(ctx->parent, ctx->active, ctx->flags, B);
-	ctx->launches += 3;
+	launch_grid(L, k_uf_init, GRID(B), ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B);
+	if (ctx->nconn) launch_grid(L, k_uf_union_conn, GRID(ctx->nconn), ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn);
+	launch_grid(L, k_uf_union_contacts, GRID(C), ctx->parent, ctx->taint, ctx->idle, kind, ctx->staged.bodies, counts);
+	launch_grid(L, k_uf_flatten_active, GRID(B), ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
+	launch_grid(L, k_body_flags, GRID(B), ctx->parent, ctx->active, ctx->flags, B);
 	nb_scan_reduce<1>(L, ctx->flags, S, nullptr, B, ctx->block_sums, counts + CNT_ACTIVE);
-	k_active_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->flags, ctx->block_sums, ctx->active_idx, B);
-	k_contact_flags<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->staged.bodies, ctx->staged.tags, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
-	ctx->launches += 2;
+	launch_grid(L, k_active_scatter, NB_SCAN_GRID, ctx->flags, ctx->block_sums, ctx->active_idx, B);
+	launch_grid(L, k_contact_flags, GRID(C), ctx->staged.bodies, ctx->staged.tags, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
 	nb_scan_reduce<2>(L, ctx->flags, S, counts + CNT_STAGED, 0, ctx->block_sums, counts + CNT_CONTACTS);  // -> CONTACTS, SLEEP_FINE
-	k_contact_compact<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(ctx->staged, ctx->fin, ctx->flags, ctx->block_sums, S, ctx->sleeping, counts);
-	++ctx->launches;
+	launch_grid(L, k_contact_compact, NB_SCAN_GRID, ctx->staged, ctx->fin, ctx->flags, ctx->block_sums, S, ctx->sleeping, counts);
 
 	// sort sleeping pairs (nudge.cpp:4008): key X | Y<<32, both below 2^tagbits
-	k_copy_u64<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sleeping, ctx->sb.keys[0], counts + CNT_SLEEPING); ++ctx->launches;
+	launch_grid(L, k_copy_u64, GRID(C), ctx->sleeping, ctx->sb.keys[0], counts + CNT_SLEEPING);
 	cur = nb_radix_sort(L, ctx->sb, counts + CNT_SLEEPING, 0, (int)ctx->tagbits, false, 0, 32, (int)(32 + ctx->tagbits));
-	k_copy_u64<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sb.keys[cur], ctx->sleeping, counts + CNT_SLEEPING); ++ctx->launches;
+	launch_grid(L, k_copy_u64, GRID(C), ctx->sb.keys[cur], ctx->sleeping, counts + CNT_SLEEPING);
 	if (ctx->has_sensor) launch_sensor_overlaps(ctx, L);   // the scratch planes are free again here
 	ctx->contacts_internal = true;
 	CK(cudaGetLastError());
@@ -805,12 +801,12 @@ int nb_collide(nb_context* ctx, void* stream) {
 int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_apply_gravity_damping");
 	JOIN_UPLOADS();   // first reader of the momentum rows in a step
+	const Launch L = mk_launch(ctx, stream);
 	if (ctx->has_frc)   // the per-body force table (nb_force_api.cuh): the same stage, one launch
-		k_body_forces<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->frc, ctx->xf, ctx->props, ctx->mom, ctx->idle,
+		launch_grid(L, k_body_forces, GRID(ctx->B), ctx->active_idx, kin_table(ctx), ctx->frc, ctx->xf, ctx->props, ctx->mom, ctx->idle,
 			time_step, gravity, damping, ctx->counts);
 	else
-		k_gravity_damping<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, kin_table(ctx), ctx->mom, time_step, gravity, damping, ctx->counts);
-	++ctx->launches;
+		launch_grid(L, k_gravity_damping, GRID(ctx->B), ctx->active_idx, kin_table(ctx), ctx->mom, time_step, gravity, damping, ctx->counts);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -819,41 +815,36 @@ int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, fl
 // The two halves of read_cached_impulses: (a) the tag ORDER of the contacts (one sort), (b) the cache LOOKUP of every contact's
 // impulse plus the entries of sleeping pairs that survive the frame.
 static int read_lookup(nb_context* ctx, void* stream) {
-	Launch L = mk_launch(ctx, stream);
-	cudaStream_t st = L.stream;
+	const Launch L = mk_launch(ctx, stream);
 	u32* counts = ctx->counts, *flags = ctx->flags;
 	const u32 C = ctx->cfg.max_contacts, S = ctx->stride;
-	k_cache_lookup<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->fin.tags, ctx->fin.features, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->impulses, counts);
-	k_culled_flags<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->cache_tags, ctx->sleeping, flags, counts);
-	ctx->launches += 2;
+	launch_grid(L, k_cache_lookup, GRID(C), ctx->fin.tags, ctx->fin.features, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->impulses, counts);
+	launch_grid(L, k_culled_flags, GRID(C), ctx->cache_tags, ctx->sleeping, flags, counts);
 	nb_scan_reduce<1>(L, flags, S, counts + CNT_CACHE, 0, ctx->block_sums, counts + CNT_CULLED);
-	k_culled_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(flags, ctx->block_sums, ctx->cache_tags, ctx->cache_features, ctx->cache_data,
+	launch_grid(L, k_culled_scatter, NB_SCAN_GRID, flags, ctx->block_sums, ctx->cache_tags, ctx->cache_features, ctx->cache_data,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, counts);
-	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
 static int read_sort(nb_context* ctx, void* stream) {
-	Launch L = mk_launch(ctx, stream);
-	cudaStream_t st = L.stream;
+	const Launch L = mk_launch(ctx, stream);
 	u32* counts = ctx->counts;
 	const u32 C = ctx->cfg.max_contacts;
 	// order contacts by tag: stable sort on the feature word, then on the pair word (nudge.cpp:4024-4044)
 	int cur;
 	if (ctx->contacts_internal && 2 * ctx->tagbits + 16 <= 64) {
 		const u32 spread = (ctx->tagbits >= 3 && 2 * ctx->tagbits + 17 <= 64) ? 1u : 0u;
-		k_tag_keys_packed<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->fin.tags, ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], ctx->tagbits, spread, counts); ++ctx->launches;
+		launch_grid(L, k_tag_keys_packed, GRID(C), ctx->fin.tags, ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], ctx->tagbits, spread, counts);
 		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, (int)(2 * ctx->tagbits + 16 + spread), true, 0);
 	}
 	else {  // contacts supplied through nb_upload_contacts: arbitrary feature words
-		k_tag_keys_feature<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], counts); ++ctx->launches;
+		launch_grid(L, k_tag_keys_feature, GRID(C), ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], counts);
 		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, 32, true, 0);
-		k_tag_keys_pair<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->fin.tags, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->tagbits, counts); ++ctx->launches;
+		launch_grid(L, k_tag_keys_pair, GRID(C), ctx->fin.tags, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->tagbits, counts);
 		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, (int)(2 * ctx->tagbits), true, cur);
 	}
-	k_copy_u32<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sb.vals[cur], ctx->sorted, counts + CNT_CONTACTS);
-	++ctx->launches;
+	launch_grid(L, k_copy_u32, GRID(C), ctx->sb.vals[cur], ctx->sorted, counts + CNT_CONTACTS);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -871,13 +862,13 @@ int nb_write_cached_impulses(nb_context* ctx, void* stream) {
 	const u32 C = ctx->cfg.max_contacts;
 	const uint4* s_old = ctx->has_sensor ? ctx->sensor_old.p : nullptr;
 	const uint4* s_cur = ctx->has_sensor ? ctx->sensor_cur.p : nullptr;
+	const Launch L = mk_launch(ctx, stream);
 	if (ctx->ev_cap)   // the old cache is still intact here
-		launch_contact_events(mk_launch(ctx, stream), GRID(2 * (size_t)C), ctx->flags, ctx->stride, ctx->block_sums, ctx->cache_tags, ctx->sorted, ctx->fin,
+		launch_contact_events(L, GRID(2 * (size_t)C), ctx->flags, ctx->stride, ctx->block_sums, ctx->cache_tags, ctx->sorted, ctx->fin,
 							  ctx->culled_tags, ctx->impulses, s_old, s_cur, ctx->events.p, ctx->ev_cap, ctx->counts);
-	if (ctx->has_sensor) { k_sensor_keep<<<GRID(ctx->sensor_cap), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sensor_cur.p, ctx->sensor_old.p, ctx->counts); ++ctx->launches; }
-	k_cache_merge<<<GRID(C), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->sorted, ctx->fin.tags, ctx->fin.features, ctx->impulses,
+	if (ctx->has_sensor) launch_grid(L, k_sensor_keep, GRID(ctx->sensor_cap), ctx->sensor_cur.p, ctx->sensor_old.p, ctx->counts);
+	launch_grid(L, k_cache_merge, GRID(C), ctx->sorted, ctx->fin.tags, ctx->fin.features, ctx->impulses,
 		ctx->culled_tags, ctx->culled_features, ctx->culled_data, ctx->cache_tags, ctx->cache_features, ctx->cache_data, ctx->counts);
-	++ctx->launches;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -925,53 +916,84 @@ static void timing_end(nb_context* ctx, cudaStream_t st) {
 // velocities + accumulators) take a large share of L2, else one stage and more CTAs.
 static int jacobi_stages(const nb_context* ctx) { return ctx->B > 600000u ? 2 : 1; }
 
-// throughput mode: warm start and sweeps as Jacobi passes (k_jacobi_sweep + k_jacobi_apply per pass), nb_jacobi.cuh
-static int launch_solve_jacobi(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) {
+// throughput mode: the warm start and the sweeps as Jacobi passes (k_jacobi_sweep + k_jacobi_apply per pass), nb_jacobi.cuh
+static int launch_solve_jacobi(nb_context* ctx, bool warm, u32 sweeps, cudaStream_t st) {
+	const Launch L = mk_launch(ctx, st);
 	Rows R = ctx->rows;
 	const u32 B = ctx->B;
-	k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
-	++ctx->launches;
+	launch_grid(L, k_mw_in, GRID(B), B, ctx->mom, ctx->mw);
 	const int stages = jacobi_stages(ctx);
-	if (mode == 0 || mode == 2) {
-		if (stages == 1) k_jacobi_sweep<true, 1><<<ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
-		else k_jacobi_sweep<true, 2><<<ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
-		k_jacobi_apply<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mw, ctx->jd, ctx->jcnt);
-		ctx->launches += 2;
+	if (warm) {
+		if (stages == 1) launch(L, k_jacobi_sweep<true, 1>, ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
+		else launch(L, k_jacobi_sweep<true, 2>, ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
+		launch_grid(L, k_jacobi_apply, GRID(B), B, ctx->mw, ctx->jd, ctx->jcnt);
 	}
-	if (mode != 0)
-		for (u32 w = 0; w < sweeps; ++w) {
-			timing_begin(ctx, st);
-			if (stages == 1) k_jacobi_sweep<false, 1><<<ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
-			else k_jacobi_sweep<false, 2><<<ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), st>>>(R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
-			timing_end(ctx, st);
-			k_jacobi_apply<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mw, ctx->jd, ctx->jcnt);
-			ctx->launches += 2;
-		}
-	k_mw_out<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, mode ? 1 : 0);
-	++ctx->launches;
+	for (u32 w = 0; w < sweeps; ++w) {
+		timing_begin(ctx, st);
+		if (stages == 1) launch(L, k_jacobi_sweep<false, 1>, ctx->jacobi_blocks1, NJ_TILE, sizeof(JacobiSmem<1>), R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
+		else launch(L, k_jacobi_sweep<false, 2>, ctx->jacobi_blocks2, NJ_TILE, sizeof(JacobiSmem<2>), R, ctx->impulses, ctx->mw, ctx->jd, ctx->counts);
+		timing_end(ctx, st);
+		launch_grid(L, k_jacobi_apply, GRID(B), B, ctx->mw, ctx->jd, ctx->jcnt);
+	}
+	launch_grid(L, k_mw_out, GRID(B), B, ctx->mom, ctx->mw, sweeps > 0);
 	return NB_OK;
 }
 
-// mode 0: the warm start; mode 1: `sweeps` sweeps; mode 2: the warm start, then `sweeps` sweeps.  The warm start is k_warm_start
-// (the working rows with the warm start applied, from the shares k_build_rows left), the sweeps one k_solve launch.
-static int launch_solve(nb_context* ctx, int mode, u32 sweeps, cudaStream_t st) {
-	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) return launch_solve_jacobi(ctx, mode, sweeps, st);
+// The solver on the bodies' working rows: loaded with the warm start applied (k_warm_start, from the shares k_build_rows left) or as
+// they are (k_mw_in), then `sweeps` sweeps in one k_solve launch (none: the warm start alone), then stored back (k_mw_out).
+static int launch_solve(nb_context* ctx, bool warm, u32 sweeps, cudaStream_t st) {
+	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) return launch_solve_jacobi(ctx, warm, sweeps, st);
+	const Launch L = mk_launch(ctx, st);
 	const u32 B = ctx->B;
-	if (mode == 1) k_mw_in<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw);
-	else k_warm_start<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->chain_start, ctx->chain_len, ctx->warm, ctx->mw);
-	if (mode) {
-		Rows R = ctx->rows;
-		float4* mw = ctx->mw;
-		u32* counts = ctx->counts;
-		u32 backoff = NB_SOLVE_BACKOFF_NS;
-		void* args[] = { &R, &mw, &sweeps, &backoff, &counts };
+	if (warm) launch_grid(L, k_warm_start, GRID(B), B, ctx->mom, ctx->chain_start, ctx->chain_len, ctx->warm, ctx->mw);
+	else launch_grid(L, k_mw_in, GRID(B), B, ctx->mom, ctx->mw);
+	if (sweeps) {
 		timing_begin(ctx, st);
-		CK(cudaLaunchCooperativeKernel(ctx->has_kin ? (void*)k_solve_kin : (void*)k_solve, dim3(ctx->coop_blocks_solve), dim3(NB_BLOCK), args, 0, st));
+		CK(launch_coop(L, ctx->has_kin ? k_solve_kin : k_solve, ctx->coop_blocks_solve, NB_BLOCK, 0, ctx->rows, ctx->mw, sweeps, NB_SOLVE_BACKOFF_NS, ctx->counts));
 		timing_end(ctx, st);
-		++ctx->launches;
 	}
-	k_mw_out<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, mode ? 1 : 0);
-	ctx->launches += 2;
+	launch_grid(L, k_mw_out, GRID(B), B, ctx->mom, ctx->mw, sweeps > 0);
+	return NB_OK;
+}
+
+// The contact rows of the current contact set, everything of nb_setup_contact_constraints before the warm start.
+static int build_contact_rows(nb_context* ctx, cudaStream_t st) {
+	const Launch L = mk_launch(ctx, st);
+	u32* counts = ctx->counts;
+	const u32 C = ctx->cfg.max_contacts, S = ctx->stride, B = ctx->B;
+	const uint8_t* kind = kin_table(ctx);
+	launch_grid(L, k_inertia, GRID(B), B, ctx->xf, ctx->props, kind, ctx->inertia, ctx->mom);
+	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) {
+		// no batch schedule, no per-body chains: slots in tag order, per-body contact counts for the mass split, split rows
+		CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
+		CK(cudaMemsetAsync(ctx->jcnt, 0, sizeof(u32) * B, st));
+		launch_grid(L, k_jacobi_prepare, GRID(C), ctx->sorted, ctx->fin.bodies, kind, ctx->jcnt, ctx->rows, ctx->cstride, counts);
+		launch_grid(L, k_build_rows<true>, GRID(ctx->cstride), ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, ctx->jcnt,
+			nullptr, nullptr, nullptr);
+		return NB_OK;
+	}
+	launch_grid(L, k_sched_prep, GRID(C), ctx->sorted, ctx->fin.bodies, kind, ctx->cab, ctx->back, ctx->sched_empty, counts);
+	// the scheduler replay in segments (nb_solver.cuh above k_schedule, DESIGN §2.7): speculative runs, the joins of every segment
+	// from every run of the previous one, then per bucket the chain of picked runs (or the sequential replay if it broke), and the
+	// merge of the picked joins and runs
+	launch(L, k_sched_spec, dim3(16, NB_SCHED_SEGS, 8), 32, 0, ctx->cab, ctx->back, ctx->sched_slot_v, ctx->sched_empty, C, ctx->sched_state, counts);
+	launch(L, k_sched_join, dim3(16, NB_SCHED_SEGS - 1, 8), 32, 0, ctx->cab, ctx->back, ctx->sched_join_slot, ctx->sched_empty, ctx->sched_state, ctx->sched_pick, counts);
+	launch(L, k_schedule, 16, 32, 0, ctx->cab, ctx->back, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
+		ctx->flags, ctx->left_count, ctx->sched_spill_ent, ctx->sched_spill_uid, ctx->sched_spill_cap, ctx->sched_state, ctx->sched_pick, ctx->sched_pick_res, counts);
+	launch_grid(L, k_sched_merge, GRID(C), ctx->slot_of, ctx->sched_slot_v, C, ctx->sched_join_slot, ctx->slot_done, ctx->slots_per_bucket, ctx->flags,
+		ctx->sched_pick_res, counts);
+	nb_scan<1>(L, ctx->flags, ctx->offs, S, counts + CNT_CONTACTS, 0, ctx->block_sums, counts + CNT_FULL_BATCHES);
+	// per-body chains (nb_solver.cuh, above k_chain_alloc): count, segment, scatter, rank.  chain_len is zero for bodies without
+	// entries, which nb_shard_step's dataflow solve relies on.  The entries go through sb.keys[0], free until the next collide.
+	CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
+	CK(cudaMemsetAsync(ctx->chain_len, 0, sizeof(u32) * B, st));
+	launch_grid(L, k_batch_index, GRID(C), ctx->sorted, ctx->fin.bodies, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
+		ctx->offs, ctx->left_count, kind, ctx->batch_of, ctx->slot_idx, ctx->rows.contact, ctx->cstride, ctx->chain_len, counts);
+	launch_grid(L, k_chain_alloc, GRID(B), B, ctx->chain_len, ctx->chain_start, counts);
+	launch_grid(L, k_chain_scatter, GRID(C), ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->chain_start, ctx->sb.keys[0], counts);
+	launch_grid(L, k_chain_rank, GRID(2 * C), ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->sb.keys[0], ctx->rows.wait, ctx->cstride, counts);
+	launch_grid(L, k_build_rows<false>, GRID(ctx->cstride), ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, nullptr,
+		ctx->impulses, ctx->chain_start, ctx->warm);
 	return NB_OK;
 }
 
@@ -979,54 +1001,11 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_setup_contact_constraints");
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
-	Launch L = mk_launch(ctx, stream);
-	cudaStream_t st = L.stream;
-	u32* counts = ctx->counts;
-	const u32 C = ctx->cfg.max_contacts, S = ctx->stride, B = ctx->B;
-	const uint8_t* kind = kin_table(ctx);
-	k_inertia<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->xf, ctx->props, kind, ctx->inertia, ctx->mom);
-	if (ctx->solver_mode == NB_SOLVER_THROUGHPUT) {
-		// no batch schedule, no per-body chains: slots in tag order, per-body contact counts for the mass split, split rows
-		CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
-		CK(cudaMemsetAsync(ctx->jcnt, 0, sizeof(u32) * B, st));
-		k_jacobi_prepare<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->jcnt, ctx->rows, ctx->cstride, counts);
-		k_build_rows<true><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, ctx->jcnt,
-			nullptr, nullptr, nullptr);
-		ctx->launches += 3;
-		if (!ctx->defer_warm_start) {
-			int r = launch_solve(ctx, 0, 1, st); if (r) return r; if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
-		}
-		CK(cudaGetLastError());
-		return NB_OK;
-	}
-	k_sched_prep<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->cab, ctx->back, ctx->sched_empty, counts);
-	// the scheduler replay in segments (nb_solver.cuh above k_schedule, DESIGN §2.7): speculative runs, the joins of every segment
-	// from every run of the previous one, then per bucket the chain of picked runs (or the sequential replay if it broke), and the
-	// merge of the picked joins and runs
-	k_sched_spec<<<dim3(16, NB_SCHED_SEGS, 8), 32, 0, st>>>(ctx->cab, ctx->back, ctx->sched_slot_v, ctx->sched_empty, C, ctx->sched_state, counts);
-	k_sched_join<<<dim3(16, NB_SCHED_SEGS - 1, 8), 32, 0, st>>>(ctx->cab, ctx->back, ctx->sched_join_slot, ctx->sched_empty, ctx->sched_state, ctx->sched_pick, counts);
-	k_schedule<<<16, 32, 0, st>>>(ctx->cab, ctx->back, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
-		ctx->flags, ctx->left_count, ctx->sched_spill_ent, ctx->sched_spill_uid, ctx->sched_spill_cap, ctx->sched_state, ctx->sched_pick, ctx->sched_pick_res, counts);
-	k_sched_merge<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->slot_of, ctx->sched_slot_v, C, ctx->sched_join_slot, ctx->slot_done, ctx->slots_per_bucket, ctx->flags,
-		ctx->sched_pick_res, counts);
-	ctx->launches += 5;
-	nb_scan<1>(L, ctx->flags, ctx->offs, S, counts + CNT_CONTACTS, 0, ctx->block_sums, counts + CNT_FULL_BATCHES);
-	// per-body chains (nb_solver.cuh, above k_chain_alloc): count, segment, scatter, rank.  chain_len is zero for bodies without
-	// entries, which nb_shard_step's dataflow solve relies on.  The entries go through sb.keys[0], free until the next collide.
-	CK(cudaMemsetAsync(ctx->rows.contact, 0xff, sizeof(u32) * ctx->cstride, st));
-	CK(cudaMemsetAsync(ctx->chain_len, 0, sizeof(u32) * B, st));
-	k_batch_index<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, ctx->slot_of, ctx->slot_done, ctx->slot_left, ctx->slots_per_bucket,
-		ctx->offs, ctx->left_count, kind, ctx->batch_of, ctx->slot_idx, ctx->rows.contact, ctx->cstride, ctx->chain_len, counts);
-	k_chain_alloc<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->chain_len, ctx->chain_start, counts);
-	k_chain_scatter<<<GRID(C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->chain_start, ctx->sb.keys[0], counts);
-	k_chain_rank<<<GRID(2 * C), NB_BLOCK, 0, st>>>(ctx->sorted, ctx->fin.bodies, kind, ctx->batch_of, ctx->slot_idx, ctx->chain_start, ctx->chain_len, ctx->sb.keys[0], ctx->rows.wait, ctx->cstride, counts);
-	k_build_rows<false><<<GRID(ctx->cstride), NB_BLOCK, 0, st>>>(ctx->fin.data, ctx->fin.bodies, ctx->xf, ctx->inertia, ctx->mom, kind, ctx->rows, counts, nullptr,
-		ctx->impulses, ctx->chain_start, ctx->warm);
-	ctx->launches += 5;
-	if (!ctx->defer_warm_start) {  // warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
-		int r = launch_solve(ctx, 0, 1, st); if (r) return r;
-		if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
-	}
+	cudaStream_t st = (cudaStream_t)stream;
+	int r = build_contact_rows(ctx, st); if (r) return r;
+	// the warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
+	if ((r = launch_solve(ctx, true, 0, st))) return r;
+	if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -1036,15 +1015,15 @@ int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	if (!sweeps) return NB_OK;
-	if (ctx->urow_n && !ctx->defer_warm_start) {   // user rows run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
+	cudaStream_t st = (cudaStream_t)stream;
+	if (ctx->urow_n) {   // user rows run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
 		for (uint32_t w = 0; w < sweeps; ++w) {
-			int r = launch_solve(ctx, 1, 1, (cudaStream_t)stream); if (r) return r;
-			if ((r = launch_user_rows(ctx, 0, (cudaStream_t)stream))) return r;
+			int r = launch_solve(ctx, false, 1, st); if (r) return r;
+			if ((r = launch_user_rows(ctx, 0, st))) return r;
 		}
 		return NB_OK;
 	}
-	int r = launch_solve(ctx, ctx->defer_warm_start ? 2 : 1, sweeps, (cudaStream_t)stream); if (r) return r;
-	ctx->defer_warm_start = false;
+	int r = launch_solve(ctx, false, sweeps, st); if (r) return r;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -1052,8 +1031,7 @@ int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 int nb_update_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_update_cached_impulses");
 	NOT_AFTER_EDIT();
-	k_update_impulses<<<GRID(ctx->cstride), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->rows, ctx->impulses, ctx->counts);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, stream), k_update_impulses, GRID(ctx->cstride), ctx->rows, ctx->impulses, ctx->counts);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -1062,36 +1040,34 @@ int nb_advance(nb_context* ctx, float time_step, void* stream) {
 	NB_RANGE("nb_advance");
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
-	k_advance<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, stream), k_advance, GRID(ctx->B), ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts);
 	ctx->in_step = false;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
-static int step_body(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
-	int r;
-	if ((r = nb_collide(ctx, stream))) return r;
-	if ((r = nb_apply_gravity_damping(ctx, time_step, gravity, damping, stream))) return r;
-	if ((r = nb_read_cached_impulses(ctx, stream))) return r;
-	ctx->defer_warm_start = iterations > 0 && !ctx->urow_n;  // warm start straight into the sweeps' working rows (same arithmetic, same order); not with user rows between the sweeps
-	r = nb_setup_contact_constraints(ctx, stream);
-	if (!r) r = nb_apply_impulses(ctx, iterations, stream);
-	ctx->defer_warm_start = false;
-	if (r) return r;
-	if ((r = nb_update_cached_impulses(ctx, stream))) return r;
-	if ((r = nb_write_cached_impulses(ctx, stream))) return r;
-	return nb_advance(ctx, time_step, stream);
+// nb_step's solve section: nb_setup_contact_constraints + nb_apply_impulses, or without user rows between the sweeps, the row build and
+// the warm start straight into the sweeps' working rows (the same arithmetic in the same order).
+static int step_solve(nb_context* ctx, uint32_t iterations, void* stream) {
+	if (iterations > 0 && !ctx->urow_n) {
+		cudaStream_t st = (cudaStream_t)stream;
+		int r = build_contact_rows(ctx, st); if (r) return r;
+		if ((r = launch_solve(ctx, true, iterations, st))) return r;
+		CK(cudaGetLastError());
+		return NB_OK;
+	}
+	int r = nb_setup_contact_constraints(ctx, stream);
+	return r ? r : nb_apply_impulses(ctx, iterations, stream);
 }
 
-// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (60 launches in parity mode, 3 more with contact events,
+// One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (61 launches in parity mode, 3 more with contact events,
 // 6 more with sensor colliders).
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
 	ctx->scene_edited = false;     // the step begins with nb_collide (also when its graph is replayed)
 	const int r = run_graphed(ctx, ctx->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, 0, 0,
-							  [&] { return step_body(ctx, time_step, iterations, gravity, damping, stream); });
+							  [&] { return step_body(ctx, time_step, gravity, damping, stream, [&] { return step_solve(ctx, iterations, stream); }); });
 	if (r == NB_OK) ctx->in_step = false;   // the step ended with nb_advance (also when its graph was replayed)
 	return r;
 }
@@ -1219,7 +1195,7 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 	float* dx = (float*)ctx->sb.keys[0]; float* dy = (float*)ctx->sb.keys[1];
 	if ((size_t)n * 4 > (size_t)ctx->sort_cap * 8) { ctx->error = "too many probes"; return NB_ERR_CAPACITY; }
 	CK(cudaMemcpy(dx, x, (size_t)n * 4, cudaMemcpyHostToDevice));
-	k_debug_rcp<<<GRID(n), NB_BLOCK>>>(dx, dy, n, rsq); ++ctx->launches;
+	launch_grid(mk_launch(ctx, nullptr), k_debug_rcp, GRID(n), dx, dy, n, rsq);
 	CK(cudaMemcpy(y, dy, (size_t)n * 4, cudaMemcpyDeviceToHost));
 	return NB_OK;
 }

@@ -125,11 +125,10 @@ __global__ void __launch_bounds__(NB_BLOCK) k_event_scatter(const u32* flags, co
 // The three launches of an enabled nb_write_cached_impulses.  `flags` holds the old cache, the contacts and both overlap lists.
 static void launch_contact_events(const Launch& L, u32 grid, u32* flags, u32 stride, u32* block_sums, const u64* cache_tags, const u32* sorted, const ContactOut& fin,
 								  const u64* culled_tags, const float4* impulses, const uint4* s_old, const uint4* s_cur, nb_contact_event* events, u32 capacity, u32* counts) {
-	k_event_flags<<<grid, NB_BLOCK, 0, L.stream>>>(cache_tags, sorted, fin.tags, culled_tags, s_old, s_cur, flags, counts);
+	launch_grid(L, k_event_flags, grid, cache_tags, sorted, fin.tags, culled_tags, s_old, s_cur, flags, counts);
 	nb_scan_reduce<1>(L, flags, stride, counts + CNT_EV_N, 0, block_sums, counts + CNT_EV_FLAGGED);
-	k_event_scatter<<<NB_SCAN_GRID, NB_BLOCK, 0, L.stream>>>(flags, block_sums, cache_tags, sorted, fin.tags, fin.data, fin.bodies, impulses, s_old, s_cur,
+	launch_grid(L, k_event_scatter, NB_SCAN_GRID, flags, block_sums, cache_tags, sorted, fin.tags, fin.data, fin.bodies, impulses, s_old, s_cur,
 		reinterpret_cast<uint4*>(events), capacity, counts);
-	*L.counter += 2;
 }
 
 // With sensors, at the end of every nb_write_cached_impulses (events on or off): the current overlaps become the old ones

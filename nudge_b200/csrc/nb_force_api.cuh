@@ -62,7 +62,7 @@ static void clear_reserved(unsigned char* rows, size_t bytes) {
 static int ensure_body_forces(nb_context* ctx, cudaStream_t st) {
 	if (ctx->has_frc) return NB_OK;
 	{ int r = ensure_force_tables(ctx); if (r) return r; }
-	if (ctx->B) { k_body_force_defaults<<<GRID(ctx->B), NB_BLOCK, 0, st>>>(ctx->frc, ctx->B); ++ctx->launches; }
+	if (ctx->B) launch_grid(mk_launch(ctx, st), k_body_force_defaults, GRID(ctx->B), ctx->frc, ctx->B);
 	CK(cudaGetLastError());
 	ctx->has_frc = true;
 	++ctx->graph_epoch;   // nb_step's graph re-records with k_body_forces
@@ -85,8 +85,7 @@ int nb_set_body_forces(nb_context* ctx, const nb_body_force* h, uint32_t n, void
 	if (!n) return NB_OK;
 	GROW(ctx->frc_rows, n, st);
 	CK(put_staged(ctx, ctx->frc_rows.p, h, sizeof(nb_body_force) * (size_t)n, st, clear_reserved));
-	k_body_force_scatter<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->frc_rows.p, n, ctx->frc, ctx->idle);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, st), k_body_force_scatter, GRID(n), ctx->frc_rows.p, n, ctx->frc, ctx->idle);
 	CK(cudaGetLastError());
 	return NB_OK;
 }

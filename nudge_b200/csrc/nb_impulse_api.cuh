@@ -87,11 +87,10 @@ int nb_apply_body_impulses(nb_context* ctx, const nb_body_impulse* h, uint32_t n
 	for (int i = 0; i < 2; ++i) { GROW(ctx->imp_keys[i], n, st); ctx->imp_sb.keys[i] = ctx->imp_keys[i].p; }
 	CK(put_staged(ctx, ctx->imp_rows.p, h, sizeof(nb_body_impulse) * (size_t)n, st));
 	const u32 ib = bits_for(n), bb = bits_for(ctx->B);
-	k_impulse_keys<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows.p, n, ib, ctx->imp_sb.keys[0], ctx->imp_n);
-	++ctx->launches;
-	const int cur = nb_radix_sort(mk_launch(ctx, stream), ctx->imp_sb, ctx->imp_n, 0, (int)(ib + bb), false, 0);
-	k_body_impulses<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->imp_rows.p, ctx->imp_sb.keys[cur], n, ib, ctx->xf, ctx->props, ctx->mom, ctx->idle);
-	++ctx->launches;
+	const Launch L = mk_launch(ctx, st);
+	launch_grid(L, k_impulse_keys, GRID(n), ctx->imp_rows.p, n, ib, ctx->imp_sb.keys[0], ctx->imp_n);
+	const int cur = nb_radix_sort(L, ctx->imp_sb, ctx->imp_n, 0, (int)(ib + bb), false, 0);
+	launch_grid(L, k_body_impulses, GRID(n), ctx->imp_rows.p, ctx->imp_sb.keys[cur], n, ib, ctx->xf, ctx->props, ctx->mom, ctx->idle);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -102,8 +101,7 @@ int nb_apply_radial_impulse(nb_context* ctx, const nb_radial_impulse* e, void* s
 	if (!(e->radius > 0.0f) || !std::isfinite(e->radius)) { ctx->error = "radial impulse radius must be finite and above 0"; return NB_ERR_ARGUMENT; }
 	JOIN_UPLOADS();
 	if (ctx->B > 1) {
-		k_radial_impulse<<<GRID(ctx->B), NB_BLOCK, 0, (cudaStream_t)stream>>>(*e, ctx->B, kin_table(ctx), ctx->xf, ctx->props, ctx->mom, ctx->idle);
-		++ctx->launches;
+		launch_grid(mk_launch(ctx, stream), k_radial_impulse, GRID(ctx->B), *e, ctx->B, kin_table(ctx), ctx->xf, ctx->props, ctx->mom, ctx->idle);
 	}
 	CK(cudaGetLastError());
 	return NB_OK;

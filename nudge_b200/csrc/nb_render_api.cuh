@@ -66,7 +66,7 @@ int nb_instance_matrices(nb_context* ctx, float* out, uint32_t capacity, int out
 		if (!ctx->instances) ALLOC(ctx->instances, 4 * ((size_t)ctx->cfg.max_boxes + ctx->cfg.max_spheres));
 		dst = ctx->instances;
 	}
-	k_instance_matrices<<<GRID(K), NB_BLOCK, 0, st>>>(ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->sph_xf, ctx->sph_data, dst); ++ctx->launches;
+	launch_grid(mk_launch(ctx, st), k_instance_matrices, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->sph_xf, ctx->sph_data, dst);
 	CK(cudaGetLastError());
 	if (!out_is_device) {
 		CK(cudaMemcpyAsync(out, dst, (size_t)K * 64, cudaMemcpyDeviceToHost, st));

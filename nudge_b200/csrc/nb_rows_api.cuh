@@ -55,9 +55,10 @@ __global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows,
 }
 
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st) {
+	const Launch L = mk_launch(ctx, st);
 	for (u32 l = 0; l < ctx->urow_levels; ++l) {
 		const u32 b = ctx->urow_level_off[l], e = ctx->urow_level_off[l + 1];
-		if (e > b) { k_user_rows<<<GRID(e - b), NB_BLOCK, 0, st>>>(ctx->urows.p, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm); ++ctx->launches; }
+		if (e > b) launch_grid(L, k_user_rows, GRID(e - b), ctx->urows.p, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm);
 	}
 	CK(cudaGetLastError());
 	return NB_OK;

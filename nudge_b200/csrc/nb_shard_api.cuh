@@ -157,21 +157,21 @@ int nb_shard_exchange(nb_shard* sh, int transport, void* stream) {
 	cudaStream_t st = (cudaStream_t)stream;
 	if (sh->world == 1) return NB_OK;
 	if (!ctx->capturing) { int jr = join_uploads(ctx, st); if (jr) return jr; }   // reads the momentum rows
+	const Launch L = mk_launch(ctx, st);
 	const ShardPlanDev P = sh->plan;
 	if (transport == NB_SHARD_NCCL) {
 		if (!sh->has_nccl) { ctx->error = "this shard was created without an NCCL id"; return NB_ERR_ARGUMENT; }
 		NcclApi* api = nccl_api(nullptr);
-		if (P.n_export) { k_pack_rows<<<GRID(2 * P.n_export), NB_BLOCK, 0, st>>>((const float4*)ctx->mom, P.export_local, P.n_export, sh->d_export); ++ctx->launches; }
+		if (P.n_export) launch_grid(L, k_pack_rows, GRID(2 * P.n_export), (const float4*)ctx->mom, P.export_local, P.n_export, sh->d_export);
 		ncclResult_t r = api->AllGather(sh->d_export, sh->d_gather, (size_t)sh->max_export * 8, ncclFloat, sh->comm, st);
 		if (r != ncclSuccess) { ctx->error = std::string("ncclAllGather: ") + api->GetErrorString(r); return NB_ERR_CUDA; }
-		if (P.n_ghost) { k_unpack_rows<<<GRID(2 * P.n_ghost), NB_BLOCK, 0, st>>>((float4*)ctx->mom, P.ghost_local, P.ghost_src, P.n_ghost, sh->d_gather); ++ctx->launches; }
+		if (P.n_ghost) launch_grid(L, k_unpack_rows, GRID(2 * P.n_ghost), (float4*)ctx->mom, P.ghost_local, P.ghost_src, P.n_ghost, sh->d_gather);
 	}
 	else if (transport == NB_SHARD_PEER) {
 		if (!sh->peers_ready) { ctx->error = "peer inboxes not opened (nb_shard_open_peer for every rank)"; return NB_ERR_ARGUMENT; }
 		const unsigned grid = std::max(1u, std::min(GRID(std::max(P.n_export, 1u)), 64u));
-		k_shard_push<<<grid, NB_BLOCK, 0, st>>>((const float4*)ctx->mom, P, sh->peers_dev, sh->ghost_cap, sh->rank, sh->world, sh->epoch, sh->done);
-		k_shard_pull<<<std::max(1u, std::min(GRID(2 * std::max(P.n_ghost, 1u)), 64u)), NB_BLOCK, 0, st>>>((float4*)ctx->mom, P, sh->inbox, sh->ghost_cap, sh->rank, sh->world, sh->epoch, ctx->counts, sh->pull_timeout_cycles);
-		ctx->launches += 2;
+		launch_grid(L, k_shard_push, grid, (const float4*)ctx->mom, P, sh->peers_dev, sh->ghost_cap, sh->rank, sh->world, sh->epoch, sh->done);
+		launch_grid(L, k_shard_pull, std::max(1u, std::min(GRID(2 * std::max(P.n_ghost, 1u)), 64u)), (float4*)ctx->mom, P, sh->inbox, sh->ghost_cap, sh->rank, sh->world, sh->epoch, ctx->counts, sh->pull_timeout_cycles);
 	}
 	else { ctx->error = "unknown transport"; return NB_ERR_ARGUMENT; }
 	SCK(cudaGetLastError());
@@ -182,54 +182,43 @@ int nb_shard_exchange(nb_shard* sh, int transport, void* stream) {
 // (k_solve_flow); the step ends with one regular push/pull of the final rows, which is also the handshake between the ranks
 static int shard_solve_flow(nb_shard* sh, uint32_t iterations, cudaStream_t st) {
 	nb_context* ctx = sh->ctx;
+	const Launch L = mk_launch(ctx, st);
 	const u32 B = ctx->B;
 	const ShardPlanDev P = sh->plan;
 	ShardFlow X;
 	X.inbox2 = reinterpret_cast<float4*>(sh->inbox + sh->inbox2_offset); X.peer_inbox2 = sh->peer_inbox2_dev;
 	X.export_row = sh->d_export_row; X.ghost_slot = sh->d_ghost_slot; X.ghost_cap = sh->ghost_cap; X.passes_cap = sh->passes_cap;
 	const u32 passes = iterations + 1;
-	k_mw_in_flow<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, ctx->chain_len, X, P, sh->epoch, passes); ++ctx->launches;
-	Rows R = ctx->rows; const float4* impulses = ctx->impulses; float4* mw = ctx->mw; u32* counts = ctx->counts; u32 hop = NB_SOLVE_BACKOFF_NS; u32 sweeps = iterations;
-	const u32* epoch = sh->epoch; long long timeout = sh->pull_timeout_cycles;
-	void* args[] = { &R, &impulses, &mw, &sweeps, &hop, &counts, &X, (void*)&P, &epoch, &timeout };
+	launch_grid(L, k_mw_in_flow, GRID(B), B, ctx->mom, ctx->mw, ctx->chain_len, X, P, sh->epoch, passes);
 	timing_begin(ctx, st);
-	SCK(cudaLaunchCooperativeKernel((void*)k_solve_flow, dim3(sh->flow_blocks), dim3(NB_BLOCK), args, 0, st));
+	SCK(launch_coop(L, k_solve_flow, sh->flow_blocks, NB_BLOCK, 0, ctx->rows, ctx->impulses, ctx->mw, iterations, NB_SOLVE_BACKOFF_NS, ctx->counts, X, P, sh->epoch,
+					sh->pull_timeout_cycles));
 	timing_end(ctx, st);
-	++ctx->launches;
-	k_mw_out_push<<<GRID(B), NB_BLOCK, 0, st>>>(B, ctx->mom, ctx->mw, 1, P, sh->peers_dev, sh->ghost_cap, sh->rank, sh->world, sh->epoch, sh->done);
-	k_shard_pull<<<std::max(1u, std::min(GRID(2 * std::max(P.n_ghost, 1u)), 64u)), NB_BLOCK, 0, st>>>((float4*)ctx->mom, P, sh->inbox, sh->ghost_cap, sh->rank, sh->world, sh->epoch, ctx->counts, sh->pull_timeout_cycles);
-	ctx->launches += 2;
+	launch_grid(L, k_mw_out_push, GRID(B), B, ctx->mom, ctx->mw, 1, P, sh->peers_dev, sh->ghost_cap, sh->rank, sh->world, sh->epoch, sh->done);
+	launch_grid(L, k_shard_pull, std::max(1u, std::min(GRID(2 * std::max(P.n_ghost, 1u)), 64u)), (float4*)ctx->mom, P, sh->inbox, sh->ghost_cap, sh->rank, sh->world, sh->epoch, ctx->counts, sh->pull_timeout_cycles);
 	SCK(cudaGetLastError());
 	return NB_OK;
 }
 
-static int shard_step_body(nb_shard* sh, float time_step, uint32_t iterations, float gravity, float damping, int transport, void* stream) {
+// nb_shard_step's solve section (step_body in nb_api.cu)
+static int shard_solve(nb_shard* sh, uint32_t iterations, int transport, void* stream) {
 	nb_context* ctx = sh->ctx;
 	int r;
-	if ((r = nb_collide(ctx, stream))) return r;
-	if ((r = nb_apply_gravity_damping(ctx, time_step, gravity, damping, stream))) return r;
-	if ((r = nb_read_cached_impulses(ctx, stream))) return r;
 	// the dataflow hand-over needs the peer inboxes, the exact-order solver without user rows between the sweeps, a solver grid and
 	// room for every pass in the pass-indexed inbox; everything else exchanges between the solver launches
 	if (sh->world > 1 && transport == NB_SHARD_PEER && sh->peers_ready && ctx->solver_mode == NB_SOLVER_PARITY && !ctx->urow_n &&
 		sh->flow_blocks > 0 && iterations > 0 && iterations + 1 <= sh->passes_cap) {
-		ctx->defer_warm_start = true;                          // setup without its warm-start launch: it runs inside k_solve_flow
-		r = nb_setup_contact_constraints(ctx, stream);         // (chain_len reads 0 for bodies without contacts on this rank)
-		ctx->defer_warm_start = false;
-		if (r) return r;
-		if ((r = shard_solve_flow(sh, iterations, (cudaStream_t)stream))) return r;
+		// the rows without the warm start, which runs inside k_solve_flow (chain_len reads 0 for bodies without contacts on this rank)
+		if ((r = build_contact_rows(ctx, (cudaStream_t)stream))) return r;
+		return shard_solve_flow(sh, iterations, (cudaStream_t)stream);
 	}
-	else {
-		if ((r = nb_setup_contact_constraints(ctx, stream))) return r;        // includes the warm start
+	if ((r = nb_setup_contact_constraints(ctx, stream))) return r;        // includes the warm start
+	if ((r = nb_shard_exchange(sh, transport, stream))) return r;
+	for (uint32_t i = 0; i < iterations; ++i) {
+		if ((r = nb_apply_impulses(ctx, 1, stream))) return r;
 		if ((r = nb_shard_exchange(sh, transport, stream))) return r;
-		for (uint32_t i = 0; i < iterations; ++i) {
-			if ((r = nb_apply_impulses(ctx, 1, stream))) return r;
-			if ((r = nb_shard_exchange(sh, transport, stream))) return r;
-		}
 	}
-	if ((r = nb_update_cached_impulses(ctx, stream))) return r;
-	if ((r = nb_write_cached_impulses(ctx, stream))) return r;
-	return nb_advance(ctx, time_step, stream);
+	return NB_OK;
 }
 
 // One sub-step of the sharded scene (example/main.cpp:274-328 with the ghost exchange after the warm start and after every sweep).
@@ -246,7 +235,7 @@ int nb_shard_step(nb_shard* sh, float time_step, uint32_t iterations, float grav
 	{ int jr = join_uploads(ctx, (cudaStream_t)stream); if (jr) return jr; }   // a pending side copy of nb_upload_bodies: ordered here, on the host side (the sharded graph has no event-wait node)
 	ctx->capture_joined = true;
 	return run_graphed(ctx, sh->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, transport, sh->plan_version,
-					   [&] { return shard_step_body(sh, time_step, iterations, gravity, damping, transport, stream); });
+					   [&] { return step_body(ctx, time_step, gravity, damping, stream, [&] { return shard_solve(sh, iterations, transport, stream); }); });
 }
 
 int nb_shard_graph_active(const nb_shard* sh) { return sh->graph.exec != nullptr; }

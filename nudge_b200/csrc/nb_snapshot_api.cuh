@@ -107,8 +107,7 @@ static int snapshot_table(nb_context* ctx, const nb_snapshot* s, bool save, Snap
 static int snapshot_launch(nb_context* ctx, const SnapTable& t, cudaStream_t st) {
 	size_t chunks = 0;   // an upper bound: device counts at their limits
 	for (u32 i = 0; i < t.n; ++i) chunks += ((size_t)t.s[i].size * t.s[i].count + 15) / 16;
-	k_snapshot_copy<<<GRID(std::max<size_t>(chunks, 1)), NB_BLOCK, 0, st>>>(t);
-	++ctx->launches;
+	launch_grid(mk_launch(ctx, st), k_snapshot_copy, GRID(std::max<size_t>(chunks, 1)), t);
 	CK(cudaGetLastError());
 	return NB_OK;
 }

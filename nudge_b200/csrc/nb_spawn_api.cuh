@@ -216,36 +216,31 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	const uint8_t* kind = kin_table(ctx);
 	const u32 kshift = bits_for(B) + 1;
 	CK(cudaMemsetAsync(rem, 0, B, st));
-	k_spawn_mark<<<GRID(n), NB_BLOCK, 0, st>>>(ctx->spawn_idx.p, n, rem);
-	k_spawn_flags<<<GRID(std::max(B, std::max(K, nconn))), NB_BLOCK, 0, st>>>(B, nboxes, K, nconn, rem, ctx->box_xf, ctx->box_tags, ctx->sph_xf, ctx->sph_tags,
+	launch_grid(L, k_spawn_mark, GRID(n), ctx->spawn_idx.p, n, rem);
+	launch_grid(L, k_spawn_flags, GRID(std::max(B, std::max(K, nconn))), B, nboxes, K, nconn, rem, ctx->box_xf, ctx->box_tags, ctx->sph_xf, ctx->sph_tags,
 		ctx->conn, kind, ctx->idle, flags, S, ctx->sb.keys[0], kshift, counts);
-	ctx->launches += 2;
 	if (K) {
 		const int cur = nb_radix_sort(L, ctx->sb, counts + CNT_SPAWN_KEYS, 0, (int)(ctx->tagbits + kshift), false, 0);
-		k_spawn_wake<<<GRID(ctx->cfg.max_contacts), NB_BLOCK, 0, st>>>(ctx->cache_tags, ctx->sb.keys[cur], K, kshift, kind, ctx->idle, counts);
-		++ctx->launches;
+		launch_grid(L, k_spawn_wake, GRID(ctx->cfg.max_contacts), ctx->cache_tags, ctx->sb.keys[cur], K, kshift, kind, ctx->idle, counts);
 	}
 	// bodies: xf -> mw, properties -> inertia, idle -> taint, kind -> active (each rewritten by the step before it is read: k_mw_in, k_inertia,
 	// k_uf_init); momentum -> jd, the throughput solver's accumulator, which must be all zeros between passes and is cleared after the copy back
 	nb_scan_reduce<1>(L, flags, S, nullptr, B, ctx->block_sums, counts + CNT_SPAWN_B);
-	k_spawn_bodies<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(B, flags, ctx->block_sums, ctx->xf, ctx->props, ctx->mom, ctx->idle, ctx->kind, ctx->has_frc ? ctx->frc : nullptr,
+	launch_grid(L, k_spawn_bodies, NB_SCAN_GRID, B, flags, ctx->block_sums, ctx->xf, ctx->props, ctx->mom, ctx->idle, ctx->kind, ctx->has_frc ? ctx->frc : nullptr,
 		reinterpret_cast<nb_transform*>(ctx->mw), ctx->inertia, ctx->jd, reinterpret_cast<uint8_t*>(ctx->taint), reinterpret_cast<uint8_t*>(ctx->active), ctx->frc_spare, map);
-	++ctx->launches;
 	// colliders, by table index: tags -> col_tag, transforms -> world_xf, filter -> order, sensor -> rank; box data -> aabb_min, radii -> col_body
 	if (K) {
 		nb_scan_reduce<2>(L, flags + S, S, nullptr, K, ctx->block_sums, counts + CNT_SPAWN_BOXES);
-		k_spawn_colliders<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(nboxes, K, flags + S, S, ctx->block_sums, map, ctx->box_tags, ctx->box_data, ctx->box_xf,
+		launch_grid(L, k_spawn_colliders, NB_SCAN_GRID, nboxes, K, flags + S, S, ctx->block_sums, map, ctx->box_tags, ctx->box_data, ctx->box_xf,
 			ctx->sph_tags, ctx->sph_data, ctx->sph_xf, ctx->has_filter ? ctx->filter : nullptr, ctx->has_sensor ? ctx->sensor : nullptr,
 			ctx->col_tag, ctx->aabb_min, reinterpret_cast<float*>(ctx->col_body), ctx->world_xf, ctx->order, reinterpret_cast<uint8_t*>(ctx->rank), counts);
-		++ctx->launches;
 	}
 	if (nconn) {
 		nb_scan_reduce<1>(L, flags + 3 * (size_t)S, S, nullptr, nconn, ctx->block_sums, counts + CNT_SPAWN_CONN);
-		k_spawn_conns<<<NB_SCAN_GRID, NB_BLOCK, 0, st>>>(nconn, flags + 3 * (size_t)S, ctx->block_sums, map, ctx->conn, reinterpret_cast<uint2*>(ctx->conn_scratch));
-		++ctx->launches;
+		launch_grid(L, k_spawn_conns, NB_SCAN_GRID, nconn, flags + 3 * (size_t)S, ctx->block_sums, map, ctx->conn, reinterpret_cast<uint2*>(ctx->conn_scratch));
 	}
-	if (nrows) { k_spawn_rows<<<GRID(nrows), NB_BLOCK, 0, st>>>(ctx->urows.p, ctx->spawn_idx.p + n, nrows, map, ctx->urows_spare.p); ++ctx->launches; }
-	if (ctx->has_sensor) { k_spawn_overlaps<<<GRID(2 * (size_t)ctx->sensor_cap), NB_BLOCK, 0, st>>>(ctx->sensor_cur.p, ctx->sensor_old.p, ctx->sensor_cap, map, counts); ++ctx->launches; }
+	if (nrows) launch_grid(L, k_spawn_rows, GRID(nrows), ctx->urows.p, ctx->spawn_idx.p + n, nrows, map, ctx->urows_spare.p);
+	if (ctx->has_sensor) launch_grid(L, k_spawn_overlaps, GRID(2 * (size_t)ctx->sensor_cap), ctx->sensor_cur.p, ctx->sensor_old.p, ctx->sensor_cap, map, counts);
 	CK(cudaGetLastError());
 	u32 c[CNT_SPAWN__N - CNT_SPAWN_B];
 	CK(cudaMemcpyAsync(c, counts + CNT_SPAWN_B, sizeof(c), cudaMemcpyDeviceToHost, st));

@@ -211,7 +211,7 @@ def test_graph_replay_with_edits_every_step_equals_plain_launches():
         c2 = a.launch_count()
         assert c2 - c1 == (1 if i % 2 else 0), i
         a.step(); p.step()
-        assert a.launch_count() - c2 == 60, i
+        assert a.launch_count() - c2 == 61, i
         assert _state(a) == _state(p), i
     assert a.debug_scalar("graph_active") == 1
 

@@ -170,7 +170,7 @@ def test_launch_counts_and_throughput_mode():
             before = x.launch_count()
             x.step() if i else x.step_staged()
             used.setdefault(name, []).append(x.launch_count() - before)
-    assert used["none"][1:] == [60, 60] and used["plain"] == used["none"] and used["removed"] == used["none"], used   # [0]: the stage calls
+    assert used["none"][1:] == [61, 61] and used["plain"] == used["none"] and used["removed"] == used["none"], used   # [0]: the stage calls
     assert used["sensors"] == used["zero"] == [n + 6 for n in used["none"]], used
     p = nudge_b200.Sim(s); t = nudge_b200.Sim(s)
     t.set_solver_mode("throughput")
