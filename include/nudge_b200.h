@@ -14,6 +14,7 @@
  *   nb_upload_connections           <- BodyConnections of nudge::collide  nudge.h:108-111, example/main.cpp:285
  *   nb_upload_contacts              <- "custom contacts can be added here" example/main.cpp:288
  *   nb_upload_constraint_rows       <- "custom constraint impulses"        example/main.cpp:316
+ *   nb_upload_joints                <- no reference counterpart: the rows an application would rebuild for example/main.cpp:316 every step
  *   nb_instance_matrices            <- the draw loops of render()          example/main.cpp:224-268 (helpers :53-110)
  *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
  *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
@@ -184,6 +185,66 @@ typedef struct {
 } nb_constraint_row;            /* 80 bytes */
 int nb_upload_constraint_rows(nb_context*, const nb_constraint_row* host_rows, uint32_t n, void* stream);   /* replaces the set; n = 0 removes it; synchronises */
 int nb_download_constraint_rows(nb_context*, nb_constraint_row* host_rows, uint32_t n, void* stream);       /* caller's order; synchronises */
+
+/* Joints (ragdolls, doors, chains, welded parts; DESIGN.md section 8.13): constraints between two bodies that stay on the device.  A joint is a
+ * producer of the user constraint rows above: once per step, inside nb_setup_contact_constraints (and so inside nb_step's graph), the library
+ * rebuilds each joint's rows from the two bodies' current transforms, and it applies them exactly as it applies user rows.  Nothing crosses
+ * PCIe and nothing synchronises between steps.
+ * Rows per joint, in this order: BALL 3 (point x, y, z), HINGE 5 (point x, y, z, angular 1, 2), FIXED 6 (point x, y, z, angular x, y, z),
+ * DISTANCE 1.  Every row has a, b and softness of its joint, lo = -inf, hi = +inf, reserved = 0, and keeps its accumulated impulse from the
+ * previous step.  The arithmetic is float32, left to right as written, without fused multiply-adds, with
+ *   cross(u, v) = (u.y*v.z - u.z*v.y, u.z*v.x - u.x*v.z, u.x*v.y - u.y*v.x),   dot(u, v) = (u.x*v.x + u.y*v.y) + u.z*v.z,
+ *   qrot(q, r):  t = 2 * cross(q.xyz, r);  (r + q.w * t) + cross(q.xyz, t)                                      (nudge.cpp:1117-1120)
+ *   qmul(l, r):  xyz = ((r.xyz * l.w) + (l.xyz * r.w)) + cross(l.xyz, r.xyz),  w = l.w*r.w - dot(l.xyz, r.xyz)  (nudge.cpp:1122-1126)
+ * (p_a, q_a) and (p_b, q_b) the bodies' positions and rotations, and k = beta / dt, dt being the step's time step: nb_step has it, the stage
+ * calls take it from the nb_apply_gravity_damping of the step (nb_setup_contact_constraints with joints and no nb_apply_gravity_damping since
+ * the last nb_collide is NB_ERR_ARGUMENT).
+ *   anchors:   ra = qrot(q_a, anchor_a);  wa = p_a + ra;  b != 0: rb = qrot(q_b, anchor_b), wb = p_b + rb;  b == 0: rb = (0, 0, 0), wb = anchor_b
+ *   point rows (BALL, HINGE, FIXED):  err = wa - wb;  for the axis e = x, y, z:  lin_a = e,  lin_b = -e (the other components +0),
+ *              ang_a = (0, ra.z, -ra.y) | (-ra.z, 0, ra.x) | (ra.y, -ra.x, 0),  ang_b = (0, -rb.z, rb.y) | (rb.z, 0, -rb.x) | (-rb.y, rb.x, 0),
+ *              bias = k * err.e
+ *   HINGE:     u = qrot(q_a, axis_a);  w = b != 0 ? qrot(q_b, axis_b) : axis_b;  c = cross(u, w)
+ *              t1 = fabsf(u.x) < 0.57735f ? (0, u.z, -u.y) : (-u.z, 0, u.x);  t1 = t1 * (1 / sqrtf(dot(t1, t1)));  t2 = cross(u, t1)
+ *              angular row i:  lin_a = lin_b = 0,  ang_a = t_i,  ang_b = -t_i,  bias = -(k * dot(c, t_i))
+ *   FIXED:     g = qmul(q_a, rel_rotation);  d = b != 0 ? qmul(g, (-q_b.xyz, q_b.w)) : g;  if d.w < 0: d.xyz = -d.xyz
+ *              angular row e = x, y, z:  lin_a = lin_b = 0,  ang_a = e,  ang_b = -e,  bias = k * (2 * d.e)
+ *   DISTANCE:  v = wa - wb;  dist = sqrtf(dot(v, v));  n = dist > 0 ? v * (1 / dist) : (0, 1, 0)
+ *              lin_a = n,  ang_a = cross(ra, n),  lin_b = -n,  ang_b = -cross(rb, n) (each component negated),  bias = k * (dist - length)
+ * With the row update impulse' = impulse - eff * (J v + bias + softness * impulse) these signs make every error shrink.
+ * Joints behave like their rows appended after the user rows: their accumulated impulses are applied in nb_setup_contact_constraints after the
+ * contacts' warm start and the user rows', and their rows run after every contact sweep after the user rows, in both solver modes.  Joints run
+ * in upload order wherever two joints share a body (one thread applies a joint's rows one after the other; joints of one dependency level
+ * touch disjoint bodies and run in one launch), so the result is the sequential host loop over all generated rows in joint order.  A kinematic
+ * side has infinite mass, as for rows.  Connect the joint's bodies with nb_upload_connections, and set NB_FILTER_SKIP_CONNECTED so that they do
+ * not also collide; the library does not edit the connection list.
+ * nb_upload_joints replaces the set (n = 0 removes it); impulse[0 .. rows-1] warm-start the joint's rows.  Every entry is checked on the host
+ * before any device work, and an error changes nothing.  NB_ERR_ARGUMENT: a == 0, a == b, a or b at or beyond the body count, an unknown
+ * type, a field that is not finite, a null pointer with n > 0.  NB_ERR_CAPACITY: the joints form a dependency chain of more than 4,096 levels
+ * (order a long chain red-black).  Asynchronous on `stream`; the host array may be reused when the call returns.  nb_step re-records its graph
+ * only when the structure (n, and each joint's type, a and b) changed: new parameters or impulses for the same structure keep it.
+ * nb_download_joints returns the joints in upload order with impulse[] = the rows' current accumulated impulses (what an application reads to
+ * break a joint) and the unused impulse slots 0.  *count = the number of joints; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
+ * nb_remove_bodies deletes the joints that name a removed body and remaps the others, keeping their order, parameters and accumulated
+ * impulses; the kept body on the other side of a deleted joint gets idle counter 0 (not body 0, not a kinematic body).  nb_add_bodies leaves
+ * the joints alone.  nb_upload_bodies keeps the set while the body count is unchanged and removes it when the count changes.
+ * nb_snapshot_save / nb_snapshot_restore carry the set with its impulses.  nb_save_state writes it (state version 6), nb_load_state restores
+ * it, and a file of an older version removes it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).
+ * Cost per step with L joint levels and s sweeps: 1 + L * (s + 1) launches, and the contact sweeps run one per solver launch as with user
+ * rows; without a set the step launches exactly what it launches without this feature. */
+enum nb_joint_type { NB_JOINT_BALL = 0, NB_JOINT_HINGE = 1, NB_JOINT_FIXED = 2, NB_JOINT_DISTANCE = 3 };
+typedef struct {
+	uint32_t type, a, b;        /* a != 0; b = 0 is the static world; a != b */
+	float anchor_a[3];          /* in a's body frame */
+	float anchor_b[3];          /* in b's body frame; a world point when b = 0 */
+	float axis_a[3], axis_b[3]; /* HINGE: the hinge axis in each body's frame (unit length; the world frame for b = 0) */
+	float rel_rotation[4];      /* FIXED: conj(q_a) * q_b at rest (x, y, z, w; q_b = identity for b = 0) */
+	float length;               /* DISTANCE: rest distance between the anchors */
+	float beta;                 /* Baumgarte factor: bias = beta / dt * error */
+	float softness;             /* copied into every row */
+	float impulse[6];           /* accumulated impulses of the joint's rows: warm start on upload, result on download */
+} nb_joint;                     /* 112 bytes */
+int nb_upload_joints(nb_context*, const nb_joint* host, uint32_t n, void* stream);
+int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t* count, void* stream);
 
 /* Contact events (collision callbacks; DESIGN.md section 8.5): which collider pairs started or stopped touching, computed on the device inside
  * nb_write_cached_impulses (so the stage calls, nb_step and its graph replay give the same stream).  A pair (key tags = A | (uint64)B << 32,
@@ -382,6 +443,9 @@ int nb_download_body_forces(nb_context*, nb_body_force* host, uint32_t capacity,
  *   forces:      the body force table's entries move with their bodies (a removed body's entry is dropped); the table stays.
  *   rows:        a user constraint row naming a removed body is deleted; the others keep their upload order, their accumulated impulse and the
  *                rest of the row, with a and b remapped (nb_download_constraint_rows then takes the new row count).
+ *   joints:      a joint naming a removed body is deleted and the kept dynamic body on its other side gets idle counter 0; the others keep their
+ *                upload order, parameters and accumulated impulses, with a and b remapped (as after nb_download_joints, the host edit and
+ *                nb_upload_joints).  One more launch when a body is woken this way.
  *   overlaps:    the sensor overlap lists (the current one and the one nb_write_cached_impulses compares against) keep their keys; body_a and
  *                body_b are remapped, a removed side becomes NB_REMOVED_BODY.
  *   The contact cache is NOT edited: its keys are collider tags, so the kept entries stay valid.  A removed collider's entries drop out at the
@@ -432,7 +496,8 @@ int nb_stream_synchronize(nb_context*, void* stream);
 /* State serialisation (SURVEY.md section 8 f3): the caller-owned PODs of nudge.h:73-129 (BodyData, ColliderData, BodyConnections,
  * ContactCache, widened layout) as one flat file, from / into the device-resident context.  Checkpoint, and what tools/nb_replay
  * steps headless; layout in nudge_b200/csrc/nb_state_api.cuh.  All three synchronise.  A context with a body force table writes version 5
- * (the table's B rows after the kinematic section); loading a file of versions 1-4 removes the context's table. */
+ * (the table's B rows after the kinematic section); loading a file of versions 1-4 removes the context's table.  A context with joints
+ * writes version 6 (the joints after the force table); loading a file of versions 1-5 removes the context's joints. */
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);
@@ -443,7 +508,7 @@ int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres
  * unused lanes, idle counters); boxes and spheres (tags, data, transforms); connections; the contact cache (as many entries as the device count
  * says); the filter table, its flags and the NB_FILTER_SKIP_CONNECTED key list; the sensor table, max_sensor_pairs and the sensor overlap list
  * as of the last nb_write_cached_impulses; the kinematic set and its kind bytes; the body force table; the user constraint rows with their
- * accumulated impulses and their levelling; the solver mode; the contact-event step counter; the body, collider and connection counts and the
+ * accumulated impulses and their levelling; the joints with theirs; the solver mode; the contact-event step counter; the body, collider and connection counts and the
  * tag and key bits.  It does not hold whether contact events are enabled, the undrained events, or the outputs of the last nb_collide.
  *
  * nb_snapshot_create allocates device memory for the context's capacities (DESIGN.md section 8.12 gives the bytes); nb_snapshot_destroy frees
@@ -457,7 +522,7 @@ int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres
  * ones are created.  nb_download_sensor_overlaps then returns the overlap list of the save, and the stage calls that read the last collide's
  * outputs are refused until the next nb_collide or nb_step, as after nb_add_bodies.  With every table already allocated it is one kernel
  * launch and host bookkeeping, without synchronisation.  nb_step keeps its graph when the step's launches and their arguments are unchanged:
- * the same counts, tag and key bits, table set, kinematic set and user-row set; otherwise it re-records once.
+ * the same counts, tag and key bits, table set, kinematic set, user-row set and joint structure; otherwise it re-records once.
  * NB_ERR_ARGUMENT, changing nothing: a snapshot of another context, restoring a snapshot that was never saved, a context that nb_shard_create
  * was called on. */
 typedef struct nb_snapshot nb_snapshot;

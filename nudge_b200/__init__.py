@@ -26,7 +26,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
-           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore"]
+           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints"]
 
 
 class Config(C.Structure):
@@ -96,6 +96,8 @@ def load_library():
         lib.nb_state_info.argtypes = [C.c_char_p, V]
         lib.nb_upload_constraint_rows.argtypes = [V, V, C.c_uint32, V]
         lib.nb_download_constraint_rows.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_upload_joints.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_download_joints.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_instance_matrices.argtypes = [V, V, C.c_uint32, C.c_int, V, V]
         lib.nb_shard_build_plan.argtypes = [V, C.c_uint32, V, V, C.c_uint32, C.c_uint32, V, V, V, V, V, V, V, V]
         lib.nb_shard_local_scene.argtypes = [V, C.c_uint32, V, C.c_uint32, C.c_uint32, V, C.c_uint32, V, C.c_uint32, V, V, V, V, V]
@@ -157,6 +159,8 @@ class Snapshot:
 ROW = np.dtype([("a", "<u4"), ("b", "<u4"), ("lin_a", "<f4", 3), ("ang_a", "<f4", 3), ("lin_b", "<f4", 3), ("ang_b", "<f4", 3),
                 ("bias", "<f4"), ("lo", "<f4"), ("hi", "<f4"), ("impulse", "<f4"), ("softness", "<f4"), ("reserved", "<f4")])
 assert ROW.itemsize == 80
+JOINT = abi.JOINT
+JOINT_BALL, JOINT_HINGE, JOINT_FIXED, JOINT_DISTANCE = 0, 1, 2, 3
 
 
 def nccl_unique_id():
@@ -413,6 +417,20 @@ class Sim(abi.HostState):
         rows = np.zeros(n, ROW)
         self._ck(self.lib.nb_download_constraint_rows(self.ctx, abi.ptr(rows) if n else None, n, self.stream), "nb_download_constraint_rows")
         return rows
+
+    # ---- joints (nb_joint, include/nudge_b200.h): rows rebuilt from the transforms on the device every step ----
+    def upload_joints(self, joints):
+        """Replaces the joint set with `joints` (JOINT rows; none removes it).  Asynchronous; the array may be reused on return."""
+        j = np.ascontiguousarray(np.asarray(joints if joints is not None else [], JOINT).reshape(-1))
+        self._ck(self.lib.nb_upload_joints(self.ctx, abi.ptr(j) if len(j) else None, len(j), self.stream), "nb_upload_joints")
+
+    def download_joints(self):
+        """The joints in upload order, impulse = the current accumulated impulses of each joint's rows."""
+        n = C.c_uint32(0)
+        self.lib.nb_download_joints(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there are none)
+        out = np.zeros(n.value, JOINT)
+        self._ck(self.lib.nb_download_joints(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_joints")
+        return out
 
     # ---- renderer read-back (example/main.cpp:224-268): one column-major 4x4 model matrix per collider, boxes first, then spheres ----
     def instance_matrices(self, out=None, device_ptr=None, capacity=0):

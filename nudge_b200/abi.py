@@ -38,6 +38,12 @@ class ActiveBodies(C.Structure):
     _fields_ = [("indices", C.c_void_p), ("capacity", C.c_uint32), ("count", C.c_uint32)]
 
 
+# nb_joint (112 bytes)
+JOINT = np.dtype([("type", "<u4"), ("a", "<u4"), ("b", "<u4"), ("anchor_a", "<f4", 3), ("anchor_b", "<f4", 3), ("axis_a", "<f4", 3), ("axis_b", "<f4", 3),
+                  ("rel_rotation", "<f4", 4), ("length", "<f4"), ("beta", "<f4"), ("softness", "<f4"), ("impulse", "<f4", 6)])
+assert JOINT.itemsize == 112
+
+
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 

@@ -29,6 +29,10 @@ template<class T> struct DevBuf {
 	~DevBuf() { if (p) cudaFree(p); }
 };
 
+// The host side of a joint set (nb_joint_api.cuh): per joint in upload order its (type, a, b) and its position in the device table, which
+// holds the joints by level; the levels' offsets into the table; the number of rows the joints generate.
+struct JointSet { u32 n = 0, nrows = 0, levels = 0; std::vector<u32> structure, level_off, order; };
+
 struct nb_context {
 	nb_config cfg;
 	int sms;
@@ -90,6 +94,9 @@ struct nb_context {
 	// snapshots (nb_snapshot_save / nb_snapshot_restore, DESIGN.md section 8.12): in_step = between nb_collide and the nb_advance that ends its
 	// step, where a save is refused; the context's snapshots, freed by nb_destroy; graph_records = captures of a step graph (nb_debug_read)
 	bool in_step; std::vector<nb_snapshot*> snapshots; unsigned long long graph_records;
+	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
+	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
+	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -177,6 +184,8 @@ static Launch mk_launch(nb_context* ctx, void* stream) { Launch L = { (cudaStrea
 struct NbRange { NbRange(const char* name) { nvtxRangePushA(name); } ~NbRange() { nvtxRangePop(); } };
 #define NB_RANGE(name) NbRange nb_range_(name)
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb_rows_api.cuh
+static int launch_joints(nb_context* ctx, const float* dt, cudaStream_t st);   // nb_joint_api.cuh
+static void drop_joints(nb_context* ctx);
 static void free_snapshots(nb_context* ctx);                               // nb_snapshot_api.cuh
 // The stage calls that read the last nb_collide's outputs: refused after nb_add_bodies / nb_remove_bodies until the next collide
 #define NOT_AFTER_EDIT() do { if (ctx->scene_edited) { ctx->error = "the scene was edited (nb_add_bodies / nb_remove_bodies) since the last nb_collide"; return NB_ERR_ARGUMENT; } } while (0)
@@ -535,7 +544,7 @@ int nb_lut_model_exact(const nb_context* ctx) { return ctx->lut_exact; }
 int nb_upload_bodies(nb_context* ctx, const nb_body_data* h, void* stream) {
 	NB_RANGE("nb_upload_bodies");
 	if (h->count > ctx->cfg.max_bodies) { ctx->error = "too many bodies"; return NB_ERR_CAPACITY; }
-	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); }   // the kinematic set and the force table belong to a body count
+	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); drop_joints(ctx); }   // the kinematic set, the force table and the joints belong to a body count
 	ctx->B = h->count;
 	cudaStream_t st = (cudaStream_t)stream;
 	H2D(ctx->xf, h->transforms, h->count, nb_transform); H2D(ctx->idle, h->idle_counters, h->count, uint8_t);   // all the collision stage reads
@@ -729,6 +738,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_collide");
 	ctx->scene_edited = false;
 	ctx->in_step = true;   // until the nb_advance that ends the step
+	ctx->step_dt = 0.0f;
 	Launch L = mk_launch(ctx, stream);
 	cudaStream_t st = L.stream;
 	const u32 K = ctx->nboxes + ctx->nspheres, B = ctx->B, nboxes = ctx->nboxes;
@@ -801,6 +811,7 @@ int nb_collide(nb_context* ctx, void* stream) {
 int nb_apply_gravity_damping(nb_context* ctx, float time_step, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_apply_gravity_damping");
 	JOIN_UPLOADS();   // first reader of the momentum rows in a step
+	ctx->step_dt = time_step;
 	const Launch L = mk_launch(ctx, stream);
 	if (ctx->has_frc)   // the per-body force table (nb_force_api.cuh): the same stage, one launch
 		launch_grid(L, k_body_forces, GRID(ctx->B), ctx->active_idx, kin_table(ctx), ctx->frc, ctx->xf, ctx->props, ctx->mom, ctx->idle,
@@ -1001,11 +1012,13 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_setup_contact_constraints");
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
+	if (ctx->jset.n && !(ctx->step_dt > 0.0f)) { ctx->error = "joints need the step's time step: call nb_apply_gravity_damping after nb_collide"; return NB_ERR_ARGUMENT; }
 	cudaStream_t st = (cudaStream_t)stream;
 	int r = build_contact_rows(ctx, st); if (r) return r;
-	// the warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses
+	// the warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses, then the joints' rows and theirs
 	if ((r = launch_solve(ctx, true, 0, st))) return r;
 	if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
+	if (ctx->jset.n && (r = launch_joints(ctx, &ctx->step_dt, st))) return r;
 	CK(cudaGetLastError());
 	return NB_OK;
 }
@@ -1016,10 +1029,11 @@ int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 	JOIN_UPLOADS();
 	if (!sweeps) return NB_OK;
 	cudaStream_t st = (cudaStream_t)stream;
-	if (ctx->urow_n) {   // user rows run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
+	if (ctx->urow_n || ctx->jset.n) {   // user rows, then joints, run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
 		for (uint32_t w = 0; w < sweeps; ++w) {
 			int r = launch_solve(ctx, false, 1, st); if (r) return r;
-			if ((r = launch_user_rows(ctx, 0, st))) return r;
+			if (ctx->urow_n && (r = launch_user_rows(ctx, 0, st))) return r;
+			if (ctx->jset.n && (r = launch_joints(ctx, nullptr, st))) return r;
 		}
 		return NB_OK;
 	}
@@ -1046,10 +1060,10 @@ int nb_advance(nb_context* ctx, float time_step, void* stream) {
 	return NB_OK;
 }
 
-// nb_step's solve section: nb_setup_contact_constraints + nb_apply_impulses, or without user rows between the sweeps, the row build and
+// nb_step's solve section: nb_setup_contact_constraints + nb_apply_impulses, or without user rows or joints between the sweeps, the row build and
 // the warm start straight into the sweeps' working rows (the same arithmetic in the same order).
 static int step_solve(nb_context* ctx, uint32_t iterations, void* stream) {
-	if (iterations > 0 && !ctx->urow_n) {
+	if (iterations > 0 && !ctx->urow_n && !ctx->jset.n) {
 		cudaStream_t st = (cudaStream_t)stream;
 		int r = build_contact_rows(ctx, st); if (r) return r;
 		if ((r = launch_solve(ctx, true, iterations, st))) return r;
@@ -1135,6 +1149,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
 		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
+		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ctx->jset.nrows },   // in table order: by joint level, upload order within one
 		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
@@ -1204,8 +1219,9 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 
 #include "nb_force_api.cuh"   // before nb_state_api.cuh, whose version-5 section uses its entry checks
 #include "nb_shard_api.cuh"
-#include "nb_state_api.cuh"
 #include "nb_rows_api.cuh"
+#include "nb_joint_api.cuh"
+#include "nb_state_api.cuh"   // after nb_joint_api.cuh, whose joints its version-6 section holds
 #include "nb_render_api.cuh"
 #include "nb_impulse_api.cuh"
 #include "nb_spawn_api.cuh"

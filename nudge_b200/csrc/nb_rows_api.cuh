@@ -20,37 +20,63 @@
 
 struct RowsDev { nb_constraint_row* rows; u32* level_off; u32 n, levels; };
 
-// A kinematic side (kind non-null) is like body 0: infinite mass, its velocity read and never written.
+// The two bodies of a row as the row update holds them: a kinematic side (kind non-null) is like body 0, infinite mass, its velocity read and
+// never written.  k_user_rows loads and stores them around one row, k_joint_solve (nb_joint_api.cuh) around all rows of a joint.
+struct RowBodies {
+	bool da, db;   // dynamic sides
+	float ma, mb; float4 Ad, Ao, Bd, Bo;   // inverse masses; world inverse inertia (xx,yy,zz,-) (xy,xz,yz,-)
+	float4 al, aw, bl, bw;   // momentum rows
+	float4* pa; float4* pb;
+};
+NB_DEV RowBodies row_bodies_load(u32 a, u32 b, nb_body_momentum* momentum, const nb_body_properties* props, const float4* inertia, const uint8_t* kind) {
+	RowBodies s;
+	s.da = solver_body(kind, a) != 0; s.db = solver_body(kind, b) != 0;
+	s.ma = s.da ? props[a].mass_inverse : 0.0f; s.mb = s.db ? props[b].mass_inverse : 0.0f;
+	s.Ad = inertia[2*a]; s.Ao = inertia[2*a + 1]; s.Bd = inertia[2*b]; s.Bo = inertia[2*b + 1];
+	if (!s.da) { s.Ad = make_float4(0, 0, 0, 0); s.Ao = s.Ad; }
+	if (!s.db) { s.Bd = make_float4(0, 0, 0, 0); s.Bo = s.Bd; }
+	s.pa = reinterpret_cast<float4*>(momentum + a); s.pb = reinterpret_cast<float4*>(momentum + b);
+	s.al = s.pa[0]; s.aw = s.pa[1]; s.bl = s.pb[0]; s.bw = s.pb[1];
+	return s;
+}
+NB_DEV void row_bodies_store(const RowBodies& s) {
+	if (s.da) { s.pa[0] = s.al; s.pa[1] = s.aw; }
+	if (s.db) { s.pb[0] = s.bl; s.pb[1] = s.bw; }
+}
+// One row on the bodies in `s`: the warm start (the accumulated impulse applied as it is) or one sequential-impulse update.  Returns the
+// row's accumulated impulse afterwards.
+NB_DEV float row_apply(const nb_constraint_row& r, RowBodies& s, int warm) {
+	const float4 Ad = s.Ad, Ao = s.Ao, Bd = s.Bd, Bo = s.Bo;
+	const float ma = s.ma, mb = s.mb;
+	float4& al = s.al; float4& aw = s.aw; float4& bl = s.bl; float4& bw = s.bw;
+	// I^-1 J_ang
+	const float iax = Ad.x*r.ang_a[0] + Ao.x*r.ang_a[1] + Ao.y*r.ang_a[2], iay = Ao.x*r.ang_a[0] + Ad.y*r.ang_a[1] + Ao.z*r.ang_a[2], iaz = Ao.y*r.ang_a[0] + Ao.z*r.ang_a[1] + Ad.z*r.ang_a[2];
+	const float ibx = Bd.x*r.ang_b[0] + Bo.x*r.ang_b[1] + Bo.y*r.ang_b[2], iby = Bo.x*r.ang_b[0] + Bd.y*r.ang_b[1] + Bo.z*r.ang_b[2], ibz = Bo.y*r.ang_b[0] + Bo.z*r.ang_b[1] + Bd.z*r.ang_b[2];
+	float delta, next = r.impulse;
+	if (warm) delta = r.impulse;
+	else {
+		const float k = ma * (r.lin_a[0]*r.lin_a[0] + r.lin_a[1]*r.lin_a[1] + r.lin_a[2]*r.lin_a[2]) + (r.ang_a[0]*iax + r.ang_a[1]*iay + r.ang_a[2]*iaz)
+					  + mb * (r.lin_b[0]*r.lin_b[0] + r.lin_b[1]*r.lin_b[1] + r.lin_b[2]*r.lin_b[2]) + (r.ang_b[0]*ibx + r.ang_b[1]*iby + r.ang_b[2]*ibz) + r.softness;
+		const float jv = r.lin_a[0]*al.x + r.lin_a[1]*al.y + r.lin_a[2]*al.z + r.ang_a[0]*aw.x + r.ang_a[1]*aw.y + r.ang_a[2]*aw.z
+					   + r.lin_b[0]*bl.x + r.lin_b[1]*bl.y + r.lin_b[2]*bl.z + r.ang_b[0]*bw.x + r.ang_b[1]*bw.y + r.ang_b[2]*bw.z;
+		const float eff = k > 0.0f ? 1.0f / k : 0.0f;
+		next = r.impulse - eff * (jv + r.bias + r.softness * r.impulse);
+		next = fminf(fmaxf(next, r.lo), r.hi);
+		delta = next - r.impulse;
+	}
+	if (s.da) { al.x += ma * r.lin_a[0] * delta; al.y += ma * r.lin_a[1] * delta; al.z += ma * r.lin_a[2] * delta; aw.x += iax * delta; aw.y += iay * delta; aw.z += iaz * delta; }
+	if (s.db) { bl.x += mb * r.lin_b[0] * delta; bl.y += mb * r.lin_b[1] * delta; bl.z += mb * r.lin_b[2] * delta; bw.x += ibx * delta; bw.y += iby * delta; bw.z += ibz * delta; }
+	return next;
+}
+
 __global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows, u32 begin, u32 end, nb_body_momentum* momentum, const nb_body_properties* props, const float4* inertia,
 		const uint8_t* kind, int warm) {
 	for (u32 i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
-		nb_constraint_row r = rows[i];
-		const u32 a = r.a, b = r.b;
-		const bool da = solver_body(kind, a) != 0, db = solver_body(kind, b) != 0;   // dynamic sides
-		const float ma = da ? props[a].mass_inverse : 0.0f, mb = db ? props[b].mass_inverse : 0.0f;
-		float4 Ad = inertia[2*a], Ao = inertia[2*a + 1], Bd = inertia[2*b], Bo = inertia[2*b + 1];   // (xx,yy,zz,-) (xy,xz,yz,-)
-		if (!da) { Ad = make_float4(0, 0, 0, 0); Ao = Ad; }
-		if (!db) { Bd = make_float4(0, 0, 0, 0); Bo = Bd; }
-		// I^-1 J_ang
-		const float iax = Ad.x*r.ang_a[0] + Ao.x*r.ang_a[1] + Ao.y*r.ang_a[2], iay = Ao.x*r.ang_a[0] + Ad.y*r.ang_a[1] + Ao.z*r.ang_a[2], iaz = Ao.y*r.ang_a[0] + Ao.z*r.ang_a[1] + Ad.z*r.ang_a[2];
-		const float ibx = Bd.x*r.ang_b[0] + Bo.x*r.ang_b[1] + Bo.y*r.ang_b[2], iby = Bo.x*r.ang_b[0] + Bd.y*r.ang_b[1] + Bo.z*r.ang_b[2], ibz = Bo.y*r.ang_b[0] + Bo.z*r.ang_b[1] + Bd.z*r.ang_b[2];
-		float4* pa = reinterpret_cast<float4*>(momentum + a); float4* pb = reinterpret_cast<float4*>(momentum + b);
-		float4 al = pa[0], aw = pa[1], bl = pb[0], bw = pb[1];
-		float delta;
-		if (warm) delta = r.impulse;
-		else {
-			const float k = ma * (r.lin_a[0]*r.lin_a[0] + r.lin_a[1]*r.lin_a[1] + r.lin_a[2]*r.lin_a[2]) + (r.ang_a[0]*iax + r.ang_a[1]*iay + r.ang_a[2]*iaz)
-						  + mb * (r.lin_b[0]*r.lin_b[0] + r.lin_b[1]*r.lin_b[1] + r.lin_b[2]*r.lin_b[2]) + (r.ang_b[0]*ibx + r.ang_b[1]*iby + r.ang_b[2]*ibz) + r.softness;
-			const float jv = r.lin_a[0]*al.x + r.lin_a[1]*al.y + r.lin_a[2]*al.z + r.ang_a[0]*aw.x + r.ang_a[1]*aw.y + r.ang_a[2]*aw.z
-						   + r.lin_b[0]*bl.x + r.lin_b[1]*bl.y + r.lin_b[2]*bl.z + r.ang_b[0]*bw.x + r.ang_b[1]*bw.y + r.ang_b[2]*bw.z;
-			const float eff = k > 0.0f ? 1.0f / k : 0.0f;
-			float next = r.impulse - eff * (jv + r.bias + r.softness * r.impulse);
-			next = fminf(fmaxf(next, r.lo), r.hi);
-			delta = next - r.impulse;
-			rows[i].impulse = next;
-		}
-		if (da) { al.x += ma * r.lin_a[0] * delta; al.y += ma * r.lin_a[1] * delta; al.z += ma * r.lin_a[2] * delta; aw.x += iax * delta; aw.y += iay * delta; aw.z += iaz * delta; pa[0] = al; pa[1] = aw; }
-		if (db) { bl.x += mb * r.lin_b[0] * delta; bl.y += mb * r.lin_b[1] * delta; bl.z += mb * r.lin_b[2] * delta; bw.x += ibx * delta; bw.y += iby * delta; bw.z += ibz * delta; pb[0] = bl; pb[1] = bw; }
+		const nb_constraint_row r = rows[i];
+		RowBodies s = row_bodies_load(r.a, r.b, momentum, props, inertia, kind);
+		const float next = row_apply(r, s, warm);
+		if (!warm) rows[i].impulse = next;
+		row_bodies_store(s);
 	}
 }
 

@@ -2,11 +2,11 @@
 // section 8.12).
 //
 // A snapshot is the context's between-steps state in HBM: the sections of a state file (state_sections, nb_state_api.cuh) plus what a file
-// lacks, the user rows, the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
+// lacks, the user rows, the joint table and the joints' rows, the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
 // (snapshot_sections).  Save and restore are one launch of k_snapshot_copy in opposite directions; the host side (counts, bits, table set,
 // the connections' host copy, the kinematic set, the rows' levelling) is kept in the snapshot and installed by install_state.
-// Every section but the user rows and the overlap list has its room at the context's capacities in one arena, laid out once from the
-// capacity header; those two are sized at the save and grown by it.  Included at the end of nb_api.cu.
+// Every section but the user rows, the joints and the overlap list has its room at the context's capacities in one arena, laid out once from the
+// capacity header; those are sized at the save and grown by it.  Included at the end of nb_api.cu.
 #pragma once
 
 #define NB_SNAP_SECTIONS 32
@@ -52,6 +52,7 @@ struct nb_snapshot {
 	u32* words;
 	DevBuf<nb_constraint_row> rows;                  // user rows in device order
 	DevBuf<uint4> overlaps;                          // the sensor overlap list
+	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset;   // the joint table, the joints' rows and their host side
 	// the host side at the save
 	NbStateHeader h; StateShape shape;
 	u32 urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order; std::vector<nb_body_pair> urow_ab;
@@ -64,6 +65,7 @@ struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool presen
 // snapshot keeps them in its host side and the kind bytes), then the snapshot's own.  The fixed sections come first, the rows and the
 // overlap list last.  With `s` null the snapshot pointers are offsets into the arena.
 static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 urow_n, u32 conn_probe) {
+	const JointSet none, &js = s ? s->jset : none;
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
 	auto at = [&](size_t i) -> void* { return s ? s->arena.p + s->off[i] : nullptr; };
@@ -73,10 +75,12 @@ static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapsho
 	p.push_back({ ctx->conn_keys, at(p.size()), 8, conn_probe, conn_probe != 0, -1 });
 	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s ? s->words + j : nullptr, 4, 1, true, -1 });
 	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), urow_n, urow_n != 0, -1 });
+	p.push_back({ ctx->joints.p, s ? s->joints.p : nullptr, sizeof(nb_joint), js.n, js.n != 0, -1 });
+	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), js.nrows, js.n != 0, -1 });
 	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
 	return p;
 }
-static const size_t kSnapFixed = 18 + 2;   // the state file's sections, the kind bytes and the key list: the sections in the arena
+static const size_t kSnapFixed = 19 + 2;   // the state file's sections, the kind bytes and the key list: the sections in the arena
 
 // The table of one copy.  save: context -> snapshot; restore: snapshot -> context, with the overlap list also copied to the current list
 // and its length to the current count (nb_download_sensor_overlaps returns what it returned at the save).  A device count is read on the
@@ -150,7 +154,7 @@ void nb_snapshot_destroy(nb_snapshot* s) {
 	if (!s) return;
 	nb_context* ctx = s->ctx;
 	ctx->snapshots.erase(std::remove(ctx->snapshots.begin(), ctx->snapshots.end(), s), ctx->snapshots.end());
-	ctx->device_bytes -= s->arena.cap + sizeof(nb_constraint_row) * s->rows.cap + sizeof(uint4) * s->overlaps.cap;
+	ctx->device_bytes -= s->arena.cap + sizeof(nb_constraint_row) * (s->rows.cap + s->jrows.cap) + sizeof(uint4) * s->overlaps.cap + sizeof(nb_joint) * s->joints.cap;
 	delete s;   // cudaFree waits for the work that may still read it
 }
 
@@ -162,6 +166,8 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	JOIN_UPLOADS();   // the copy reads the momentum and property rows
 	// grown: the only save that synchronises and allocates
 	GROW(s->rows, ctx->urow_n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
+	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, ctx->jset.nrows, st);
+	s->jset = ctx->jset;
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
 	s->urow_n = ctx->urow_n; s->urow_levels = ctx->urow_levels;
@@ -183,6 +189,8 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->shape.has_frc) { int r = ensure_force_tables(ctx); if (r) return r; }
 	if (!s->shape.kin.empty()) { int r = ensure_kind_table(ctx); if (r) return r; }
 	GROW(ctx->urows, s->urow_n, st);
+	const void* joint_bufs[2] = { ctx->joints.p, ctx->jrows.p };
+	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, s->jset.nrows, st);
 	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, false, t); if (r) return r; }
@@ -192,6 +200,9 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->urow_n != ctx->urow_n || s->urow_level_off != ctx->urow_level_off) ++ctx->graph_epoch;   // the row levels are host values in the graph
 	ctx->urow_n = s->urow_n; ctx->urow_levels = s->urow_levels;
 	ctx->urow_level_off = s->urow_level_off; ctx->urow_order = s->urow_order; ctx->urow_ab = s->urow_ab;
+	// likewise the joint levels, and the joint buffers are its kernel arguments
+	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
+	ctx->jset = s->jset;
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;
 	return NB_OK;

@@ -194,6 +194,20 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		const nb_body_pair p = ctx->conn_host[i];
 		if (!removed(p.a) && !removed(p.b)) conn.push_back({ remap(p.a), remap(p.b) });
 	}
+	// the kept joints with their current impulses, remapped, and the kept dynamic bodies that lose a joint
+	cudaStream_t st = (cudaStream_t)stream;
+	std::vector<nb_joint> old_joints, joints;
+	std::vector<u32> joint_wake;
+	if (int r = get_joints(ctx, old_joints, st)) return r;
+	for (nb_joint j : old_joints) {
+		if (removed(j.a) || removed(j.b)) {
+			const u32 other = removed(j.a) ? j.b : j.a;
+			if (other && !removed(other) && !std::binary_search(kin.begin(), kin.end(), remap(other))) joint_wake.push_back(remap(other));
+			continue;
+		}
+		j.a = remap(j.a); j.b = remap(j.b);
+		joints.push_back(j);
+	}
 	std::vector<u32> level_off, order;
 	const u32 levels = level_rows(ab, level_off, order);
 	const u32 nrows = (u32)ab.size();
@@ -202,9 +216,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	staging.resize((size_t)n + nrows);
 	for (u32 j = 0; j < nrows; ++j) staging[n + order[j]] = src[j];
 
-	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // the gathers read the momentum and property rows
-	GROW(ctx->spawn_idx, staging.size(), st);
+	GROW(ctx->spawn_idx, std::max(staging.size(), joint_wake.size()), st);
 	GROW(ctx->urows_spare, nrows, st);
 	// pageable staging: the copy has consumed it when cudaMemcpyAsync returns
 	CK(cudaMemcpyAsync(ctx->spawn_idx.p, staging.data(), sizeof(u32) * staging.size(), cudaMemcpyHostToDevice, st));
@@ -276,6 +289,11 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	// nb_step's graph keys on B, the collider and connection counts, tagbits and kbits, so it re-records when they change; table contents
 	// are read through unchanged pointers.  The row levels are host values inside the graph.
 	if (rows_changed) ++ctx->graph_epoch;
+	if (!joint_wake.empty()) {
+		CK(put_staged(ctx, ctx->spawn_idx.p, joint_wake.data(), sizeof(u32) * joint_wake.size(), st));
+		launch_grid(L, k_joint_wake, GRID(joint_wake.size()), ctx->spawn_idx.p, (u32)joint_wake.size(), ctx->idle);
+	}
+	if (!old_joints.empty()) { int r = set_joints(ctx, joints.data(), (u32)joints.size(), st); if (r) return r; }
 	return build_conn_lookup(ctx, st);
 }
 
