@@ -25,6 +25,7 @@
  *   nb_add_bodies / nb_remove_bodies <- no reference counterpart: the application's edit of its caller-owned arrays between steps
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_snapshot_*                   <- no reference counterpart: the application's copy of its caller-owned arrays, kept in HBM
+ *   nb_raycast                      <- no reference counterpart (the reference has no scene queries)
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -537,6 +538,43 @@ int nb_snapshot_restore(nb_context*, const nb_snapshot*, void* stream);
  * out_is_device != 0: `out` is a device pointer (a mapped GL / Vulkan buffer), the call is asynchronous on `stream`; otherwise `out`
  * is host memory and the call returns when it is filled.  *count = colliders; NB_ERR_CAPACITY if capacity (in matrices) is smaller. */
 int nb_instance_matrices(nb_context*, float* out, uint32_t capacity, int out_is_device, uint32_t* count, void* stream);
+
+/* Ray casts (picking, line of sight, bullets, wheel probes, lidar; DESIGN.md section 8.14): n rays against the colliders as the body
+ * transforms stand when the call runs on `stream` (not as of the last nb_collide), answered on the device.  A collider's world transform
+ * (p, q) is the one nb_collide computes: p = qrot(q_body, collider.position) + p_body, q = qmul(q_body, collider.rotation).  The point of a
+ * ray at t is origin + t * direction; direction need not be unit length, and t and max_t are in units of its length.
+ * Which colliders count: collider i is tested iff (category_i & ray.mask) != 0 (category_i from nb_upload_collision_filters, 0xffff without a
+ * table), its body != ignore_body (NB_RAY_NO_HIT: ignore none), and it is not a sensor collider unless flags has NB_RAY_SENSORS.  Body 0 and
+ * kinematic bodies are solid like any other.
+ * Result: the CLOSEST hit, the smallest t in [0, max_t], ties to the smaller collider index (boxes first, then spheres: the index order of the
+ * filter and sensor tables).  position = origin + t * direction (per component), collider, its body and tag, reserved 0.  An origin inside a
+ * collider hits it at t = 0 with normal (0, 0, 0).  No hit: collider = body = tag = NB_RAY_NO_HIT and every other field 0.  A degenerate ray
+ * (a field of origin, direction or max_t not finite, a zero direction, max_t < 0) hits nothing and does not fail the call.
+ * The arithmetic is float32, left to right as written, without fused multiply-adds, IEEE division and sqrtf, with cross, dot and qrot as in
+ * the joints' section above; o = origin, d = direction, (p, q) the collider's world transform, conj(q) = (-q.x, -q.y, -q.z, q.w):
+ *   BOX (half extents h = size):  m = o - p;  lo = qrot(conj(q), m);  ld = qrot(conj(q), d);  enter = 0, exit = max_t, axis = none;
+ *     for k = x, y, z in turn:  if ld.k == 0: miss when lo.k < -h.k or lo.k > h.k
+ *       else:  t1 = (-h.k - lo.k) / ld.k;  t2 = (h.k - lo.k) / ld.k;  near = t1 < t2 ? t1 : t2;  far = t1 < t2 ? t2 : t1
+ *              if near > enter: enter = near, axis = k, s = t1 < t2 ? -1 : +1;   if far < exit: exit = far;   miss when enter > exit
+ *     t = enter;  normal = axis == none ? (0, 0, 0) : qrot(q, n_l), n_l = s in component `axis` and +0 in the other two (the lowest axis
+ *     wins a tie, since enter only moves on a strictly greater near)
+ *   SPHERE (radius r, centre p):  m = o - p;  a = dot(d, d);  b = dot(m, d);  c = dot(m, m) - r*r
+ *     c <= 0: t = 0, normal (0, 0, 0);  otherwise disc = b*b - a*c, miss when disc < 0;  t = (-b - sqrtf(disc)) / a, miss unless
+ *     0 <= t <= max_t (so a NaN t misses);  t == 0 becomes +0;  normal = (position - p) * (1 / r)
+ * Which candidates the device tests is decided by a conservative grid walk (DESIGN.md section 8.14); whether and where a candidate is hit is
+ * decided by the arithmetic above alone, so any traversal gives the same bytes.
+ * on_device != 0: rays and hits are device pointers (4-byte alignment suffices, as for the host arrays); the call is asynchronous on `stream`, and after the first call on a context it makes no
+ * synchronisation and no allocation, so it can be captured into the application's CUDA graph (a replay reads the transforms of its moment).
+ * on_device == 0: host pointers; the rays are staged like the editing calls' arrays, and the call returns with `hits` filled.  Legal between
+ * any two calls, stage calls included; it changes nothing that a step, a download or a snapshot can observe (its scratch is its own:
+ * 181 to 213 bytes per collider of capacity, allocated on the first call).  NB_ERR_ARGUMENT, changing nothing: a null pointer with n > 0, unknown
+ * flag bits, a context that nb_shard_create was called on.  Launches: 7 per call with n > 0 (reset, world transforms and AABBs, Morton codes,
+ * one radix sort, leaves, grid table, the walk), 1 (the walk alone) when the scene has no collider or no body, none with n = 0. */
+typedef struct { float origin[3]; float max_t; float direction[3]; uint32_t mask; uint32_t ignore_body; uint32_t reserved[3]; } nb_ray;        /* 48 bytes */
+typedef struct { float position[3]; float t; float normal[3]; uint32_t collider; uint32_t body; uint32_t tag; uint32_t reserved[2]; } nb_ray_hit; /* 48 bytes */
+enum nb_ray_flags { NB_RAY_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
+#define NB_RAY_NO_HIT 0xffffffffu
+int nb_raycast(nb_context*, const nb_ray* rays, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

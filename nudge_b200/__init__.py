@@ -26,7 +26,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
-           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints"]
+           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast"]
 
 
 class Config(C.Structure):
@@ -120,6 +120,7 @@ def load_library():
         lib.nb_snapshot_destroy.argtypes = [V]; lib.nb_snapshot_destroy.restype = None
         lib.nb_snapshot_save.argtypes = [V, V, V]
         lib.nb_snapshot_restore.argtypes = [V, V, V]
+        lib.nb_raycast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         _lib = lib
     return _lib
 
@@ -445,6 +446,22 @@ class Sim(abi.HostState):
             out = np.zeros((k, 16), np.float32)
         self._ck(self.lib.nb_instance_matrices(self.ctx, abi.ptr(out), len(out), 0, C.byref(n), self.stream), "nb_instance_matrices")
         return out[:n.value]
+
+    # ---- ray casts (nb_raycast, include/nudge_b200.h): the closest hit of every ray against the colliders as the transforms stand ----
+    def raycast(self, rays, flags=0, device_ptrs=None, n=None):
+        """rays: abi.RAY rows; returns their abi.RAY_HIT rows (collider = body = tag = RAY_NO_HIT for a miss).  flags: RAY_SENSORS also tests
+        sensor colliders.  device_ptrs=(rays_ptr, hits_ptr) with n: device buffers of n rays and n hits instead; the call is then asynchronous on
+        the Sim's stream (capturable after a first call) and returns None."""
+        if device_ptrs is not None:
+            if n is None:
+                raise ValueError("Sim.raycast with device_ptrs needs n, the number of rays (and hits) the two device buffers hold")
+            self._ck(self.lib.nb_raycast(self.ctx, C.c_void_p(device_ptrs[0]), int(n), C.c_void_p(device_ptrs[1]), int(flags), 1, self.stream), "nb_raycast")
+            return None
+        r = np.ascontiguousarray(np.asarray(rays, abi.RAY).reshape(-1))
+        out = np.zeros(len(r), abi.RAY_HIT)
+        P = lambda a: abi.ptr(a) if len(a) else None
+        self._ck(self.lib.nb_raycast(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_raycast")
+        return out
 
     # ---- collision filters (nb_collision_filter, include/nudge_b200.h) ----
     def upload_collision_filters(self, filters, flags=0):

@@ -43,6 +43,13 @@ JOINT = np.dtype([("type", "<u4"), ("a", "<u4"), ("b", "<u4"), ("anchor_a", "<f4
                   ("rel_rotation", "<f4", 4), ("length", "<f4"), ("beta", "<f4"), ("softness", "<f4"), ("impulse", "<f4", 6)])
 assert JOINT.itemsize == 112
 
+# nb_ray, nb_ray_hit (48 bytes each)
+RAY = np.dtype([("origin", "<f4", 3), ("max_t", "<f4"), ("direction", "<f4", 3), ("mask", "<u4"), ("ignore_body", "<u4"), ("reserved", "<u4", 3)])
+RAY_HIT = np.dtype([("position", "<f4", 3), ("t", "<f4"), ("normal", "<f4", 3), ("collider", "<u4"), ("body", "<u4"), ("tag", "<u4"), ("reserved", "<u4", 2)])
+assert RAY.itemsize == 48 and RAY_HIT.itemsize == 48
+RAY_SENSORS = 1
+RAY_NO_HIT = 0xffffffff
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

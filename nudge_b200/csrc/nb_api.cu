@@ -33,6 +33,14 @@ template<class T> struct DevBuf {
 // holds the joints by level; the levels' offsets into the table; the number of rows the joints generate.
 struct JointSet { u32 n = 0, nrows = 0, levels = 0; std::vector<u32> structure, level_off, order; };
 
+// The ray casts' own copy of the collide front end's buffers (nb_query_api.cuh), allocated on the first nb_raycast for the collider
+// capacity, so that a query never touches what the step reads; rays / hits = the staging of a call with host pointers.
+struct RayScratch {
+	DevBuf<nb_transform> world_xf; DevBuf<float4> aabb_min, aabb_max, leaf_min, leaf_max;
+	DevBuf<u32> col_tag, col_body, order, rank, large_list, vals[2], counts, hist; DevBuf<u64> keys[2], mkeys, table_keys, table_vals, keybits;
+	DevBuf<uint8_t> smallf; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; u32 table_mask = 0; SortBuffers sb = {}; bool ready = false;
+};
+
 struct nb_context {
 	nb_config cfg;
 	int sms;
@@ -97,6 +105,8 @@ struct nb_context {
 	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
 	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
+	// ray casts (nb_raycast, DESIGN.md section 8.14)
+	RayScratch ray;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -1158,6 +1168,17 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	if (!strcmp(name, "graph_records")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)ctx->graph_records; if (bytes) *bytes = 4; return NB_OK; }
 	// the device bytes the context and its snapshots hold now, as a uint64_t
 	if (!strcmp(name, "device_bytes")) { if (max_bytes < 8) return NB_ERR_ARGUMENT; *(uint64_t*)dst = ctx->device_bytes; if (bytes) *bytes = 8; return NB_OK; }
+	// nb_raycast's own counters (0 before the first call): rays that tested every collider instead of walking the grid, summed over the
+	// context's calls, and the grid level of the last call's build
+	if (!strcmp(name, "ray_fallbacks") || !strcmp(name, "ray_grid_level")) {
+		if (max_bytes < 4) return NB_ERR_ARGUMENT;
+		u32 v = 0;
+		if (ctx->ray.ready) {
+			CK(cudaMemcpyAsync(&v, ctx->ray.counts.p + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+			CK(cudaStreamSynchronize((cudaStream_t)stream));
+		}
+		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
+	}
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
@@ -1226,3 +1247,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_impulse_api.cuh"
 #include "nb_spawn_api.cuh"
 #include "nb_snapshot_api.cuh"
+#include "nb_query_api.cuh"

@@ -1,0 +1,268 @@
+// nudge_b200 — ray casts against the current colliders (nb_raycast, include/nudge_b200.h; DESIGN.md section 8.14).
+// The build is nb_collide's front end, launched unchanged on buffers of the query's own (RayScratch): world transforms and AABBs
+// (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid table (k_grid_build).  One new kernel walks it.
+// Included at the end of nb_api.cu.
+#pragma once
+
+// ---------------- the per-collider arithmetic the header states ----------------
+NB_DEV bool ray_box(f3 o, f3 d, float max_t, const xform& w, float4 size, float& t, f3& n) {
+	const quat q = mkq(w.q);
+	quat qc = q; qc.v = mk3(-q.v.x, -q.v.y, -q.v.z);
+	const f3 lo = qrot(qc, sub3(o, mk3(w.p.x, w.p.y, w.p.z))), ld = qrot(qc, d);
+	const float los[3] = { lo.x, lo.y, lo.z }, lds[3] = { ld.x, ld.y, ld.z }, h[3] = { size.x, size.y, size.z };
+	float enter = 0.0f, exit = max_t, s = 0.0f;
+	int axis = -1;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) {
+		if (lds[k] == 0.0f) {
+			if (los[k] < -h[k] || los[k] > h[k]) return false;
+		}
+		else {
+			const float t1 = (-h[k] - los[k]) / lds[k], t2 = (h[k] - los[k]) / lds[k];
+			const bool lt = t1 < t2;
+			const float near = lt ? t1 : t2, far = lt ? t2 : t1;
+			if (near > enter) { enter = near; axis = k; s = lt ? -1.0f : 1.0f; }
+			if (far < exit) exit = far;
+			if (enter > exit) return false;
+		}
+	}
+	t = enter;
+	n = axis < 0 ? mk3(0.0f, 0.0f, 0.0f) : qrot(q, axis == 0 ? mk3(s, 0.0f, 0.0f) : axis == 1 ? mk3(0.0f, s, 0.0f) : mk3(0.0f, 0.0f, s));
+	return true;
+}
+NB_DEV bool ray_sphere(f3 o, f3 d, float max_t, const xform& w, float r, float& t, f3& n) {
+	const f3 c = mk3(w.p.x, w.p.y, w.p.z), m = sub3(o, c);
+	const float a = dot3(d, d), b = dot3(m, d), cc = dot3(m, m) - r * r;
+	if (cc <= 0.0f) { t = 0.0f; n = mk3(0.0f, 0.0f, 0.0f); return true; }
+	const float disc = b * b - a * cc;
+	if (disc < 0.0f) return false;
+	t = (-b - sqrtf(disc)) / a;
+	if (!(t >= 0.0f && t <= max_t)) return false;   // a NaN t (overflowed terms) is a miss too
+	if (t == 0.0f) t = 0.0f;   // -0 -> +0: the hit key orders t by its bits
+	const float inv = 1.0f / r;
+	n = mul3(sub3(add3(o, mul3(t, d)), c), inv);
+	return true;
+}
+
+struct RayScene {
+	u32 K, nboxes;
+	const nb_transform* world_xf; const float4* aabb_max; const u32* col_body; const u32* col_tag;
+	const nb_box_collider* box_data; const nb_sphere_collider* sph_data; const uint8_t* sensor;
+};
+// Tests collider i and keeps the lane's best (t bits << 32 | i) and the normal that goes with it.
+NB_DEV void ray_test(const RayScene& S, u32 i, f3 o, f3 d, float max_t, u32 mask, u32 ignore, bool sensors, u64& best, f3& bn) {
+	const u32 category = asu(reinterpret_cast<const float*>(S.aabb_max)[4 * (size_t)i + 3]) & 0xffffu;   // k_collider_world's filter word
+	if (!(category & mask) || __ldg(S.col_body + i) == ignore || (S.sensor && !sensors && __ldg(S.sensor + i))) return;
+	const xform w = ld_xform(S.world_xf, i);
+	float t; f3 n;
+	const bool hit = i < S.nboxes ? ray_box(o, d, max_t, w, reinterpret_cast<const float4*>(S.box_data)[i], t, n)
+								  : ray_sphere(o, d, max_t, w, S.sph_data[i - S.nboxes].radius, t, n);
+	if (!hit) return;
+	const u64 key = (u64)asu(t) << 32 | i;
+	if (key < best) { best = key; bn = n; }
+}
+NB_DEV u64 warp_min_u64(u64 v) {
+	#pragma unroll
+	for (int s = 16; s; s >>= 1) { const u64 o = __shfl_xor_sync(0xffffffffu, v, s); v = o < v ? o : v; }
+	return v;
+}
+
+// Segments per ray beyond which the walk gives up on the grid and tests every collider.
+#define NB_RAY_MAX_SEGMENTS 262144u
+// The query's own counters (RayScratch::counts) hold, in the slot the step's narrowphase uses, the number of rays that tested every
+// collider instead of walking the grid, summed over the context's calls (nb_debug_read "ray_fallbacks").
+#define CNT_RAY_FALLBACKS CNT_TMP
+
+// One warp per ray.  Without colliders (K = 0) every ray misses.  Otherwise the large list first (every ray tests it), then the grid:
+// the ray, clipped to the region that can hold a small collider's hit point, is cut into segments of at most one cell along its dominant
+// axis.  A small collider fits a cell and is binned by its min corner, so a collider whose hit point lies in a segment has its min-corner
+// cell in [floor((lo - mu - W) / W), floor((hi + mu) / W)] per axis, lo / hi = the segment's quantised extent and mu the rounding margin:
+// 2 units plus 2^-16 of the magnitudes involved, far above the rounding of the quantisation, the transform and the hit point, and with
+// spheres the cancellation term below, which grows with the segment's distance from the origin.  The lanes
+// look those cells up in the hash table, the ranges are flattened with a warp scan and tested round-robin, exactly as k_grid_pairs deals its
+// candidates.  Segments tile the clipped t range, so once the next segment starts beyond the best t every closer hit has been tested.  A ray
+// whose margin at the far end of its clipped range exceeds two cells, or whose frame is not finite, tests every collider instead (and is
+// counted in CNT_RAY_FALLBACKS): with boxes only, an origin about 2^16 cells' widths outside the grid; with spheres, also a clipped range
+// ending more than about 1,000 cells' widths from the origin, which needs a grid of more than 1,000 cells per axis or an origin far outside.
+__global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays, nb_ray_hit* hits, u32 flags, RayScene S, const u32* order,
+		const u64* table_keys, const u64* table_vals, u32 table_mask, const u32* large_list, u32* counts) {
+	const u32 lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+	const bool sensors = (flags & NB_RAY_SENSORS) != 0;
+	for (u32 ri = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; ri < n; ri += nwarps) {   // ri is warp-uniform
+		const nb_ray R = rays[ri];
+		const f3 o = ld3(R.origin), d = ld3(R.direction);
+		const float max_t = R.max_t;
+		const bool valid = isfinite(o.x) && isfinite(o.y) && isfinite(o.z) && isfinite(d.x) && isfinite(d.y) && isfinite(d.z) && isfinite(max_t)
+			&& max_t >= 0.0f && (d.x != 0.0f || d.y != 0.0f || d.z != 0.0f);
+		u64 best = ~(u64)0;
+		f3 bn = mk3(0.0f, 0.0f, 0.0f);
+		if (valid && S.K) {
+			const u32 nlarge = counts[CNT_LARGE];
+			for (u32 l = lane; l < nlarge; l += 32) ray_test(S, order[large_list[l]], o, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+			const MortonFrame f = morton_frame(counts);
+			const u32 j = counts[CNT_GRID_LEVEL];
+			const float W = (float)(1u << j), s = f.L[0];
+			const int ncell = 1 << (16 - j);
+			const float ou[3] = { o.x * s - f.ms[0], o.y * s - f.ms[1], o.z * s - f.ms[2] }, du[3] = { d.x * s, d.y * s, d.z * s };
+			const float oumax = fmaxf(fabsf(ou[0]), fmaxf(fabsf(ou[1]), fabsf(ou[2])));
+			const float M = 2.0f * oumax + fmaxf(fabsf(f.ms[0]), fmaxf(fabsf(f.ms[1]), fabsf(f.ms[2]))) + 262144.0f;
+			const float mu0 = 2.0f + M * (1.0f / 65536.0f);
+			// The sphere test's disc = b*b - a*c cancels: its rounding is below 14 * 2^-24 |m|^2 |d|^2 (m = origin - centre), so the stated
+			// arithmetic can hit a sphere whose centre lies up to sqrt(28 * 2^-24) |m| < 2^-10.5 |m| beyond its radius from the ray, and the hit
+			// point lies that far outside its AABB.  A hit at t has |m| <= t |d| + r + that reach, and a small sphere has r below half a cell, so
+			// 2^-9 (t |du| + W) covers it (quantised units).  mu_at(t) is the margin of a hit at t; mu_clip bounds it over the whole grid (|m| of
+			// a centre in the grid is at most sqrt(3) (|ou| + 65536 + W)) and only widens the clip.
+			const bool sph = S.K > S.nboxes;
+			const float dnorm = 1.01f * sqrtf(du[0] * du[0] + du[1] * du[1] + du[2] * du[2]);
+			auto mu_at = [&](float t) { return mu0 + (sph ? (t * dnorm + W) * (1.0f / 512.0f) : 0.0f); };
+			const float mu_clip = mu0 + (sph ? (1.75f * (oumax + 65536.0f + W) + W) * (1.0f / 512.0f) : 0.0f);
+			// the region holding every small collider's hit point (quantised min corners lie in [0, 65536)), widened by a second margin
+			float tlo = 0.0f, thi = max_t, dmax = 0.0f;
+			bool any = true;
+			#pragma unroll
+			for (int k = 0; k < 3; ++k) {
+				const float lo = -2.0f * mu_clip, hi = 65536.0f + W + 2.0f * mu_clip;
+				dmax = fmaxf(dmax, fabsf(du[k]));
+				if (du[k] == 0.0f) { if (ou[k] < lo || ou[k] > hi) any = false; }
+				else {
+					const float t1 = (lo - ou[k]) / du[k], t2 = (hi - ou[k]) / du[k];
+					tlo = fmaxf(tlo, fminf(t1, t2)); thi = fminf(thi, fmaxf(t1, t2));
+				}
+			}
+			const float nsegf = ceilf((thi - tlo) * dmax / W);
+			const bool grid = s > 0.0f && isfinite(s) && f.L[1] == s && f.L[2] == s && f.L[3] == s && isfinite(mu_clip) && mu_at(fmaxf(thi, tlo)) <= 2.0f * W && dmax > 0.0f
+				&& isfinite(nsegf) && nsegf <= (float)NB_RAY_MAX_SEGMENTS;
+			if (!grid) {
+				if (lane == 0) atomicAdd(&counts[CNT_RAY_FALLBACKS], 1u);
+				for (u32 i = lane; i < S.K; i += 32) ray_test(S, i, o, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+			}
+			else if (any && tlo <= thi) {
+				const u32 nseg = max(1u, (u32)nsegf);
+				const float step = (thi - tlo) / (float)nseg;
+				for (u32 k = 0; k < nseg; ++k) {
+					const float ta = k == 0 ? tlo : tlo + (float)k * step, tb = k + 1 == nseg ? thi : tlo + (float)(k + 1) * step;
+					const u64 wbest = warp_min_u64(best);
+					if (wbest != ~(u64)0 && ta > asf((u32)(wbest >> 32))) break;   // every hit up to ta was tested
+					const float mu = mu_at(fmaxf(ta, tb));
+					int c0[3], nc[3];
+					bool empty = false;
+					#pragma unroll
+					for (int a = 0; a < 3; ++a) {
+						const float ua = ou[a] + ta * du[a], ub = ou[a] + tb * du[a];
+						const float lo = fminf(ua, ub) - mu - W, hi = fmaxf(ua, ub) + mu;
+						const int l = (int)fminf(fmaxf(floorf(lo / W), 0.0f), (float)ncell), h = (int)fmaxf(fminf(floorf(hi / W), (float)(ncell - 1)), -1.0f);
+						c0[a] = l; nc[a] = h - l + 1;
+						if (h < l) empty = true;
+					}
+					if (empty) continue;
+					const u32 ncells = (u32)(nc[0] * nc[1] * nc[2]);
+					for (u32 cb = 0; cb < ncells; cb += 32) {
+						const u32 ci = cb + lane;
+						u32 qb = 0, len = 0;
+						if (ci < ncells) {
+							const u32 cx = (u32)c0[0] + ci % (u32)nc[0], cy = (u32)c0[1] + (ci / (u32)nc[0]) % (u32)nc[1], cz = (u32)c0[2] + ci / (u32)(nc[0] * nc[1]);
+							const u64 prefix = morton48_of(cx << j, cy << j, cz << j) >> (3 * j);
+							u32 slot = grid_hash(prefix, table_mask);
+							u64 key;
+							while ((key = table_keys[slot]) != prefix && key != NB_GRID_EMPTY) slot = (slot + 1) & table_mask;
+							if (key != NB_GRID_EMPTY) { const u64 range = table_vals[slot]; qb = (u32)range; len = (u32)(range >> 32) - qb; }
+						}
+						const u32 incl = warp_incl_scan(len), off = incl - len, total = __shfl_sync(0xffffffffu, incl, 31);
+						for (u32 t0 = 0; t0 < total; t0 += 32) {
+							const u32 t = t0 + lane;
+							u32 c = 0;   // the cell of candidate t: the last lane whose offset is <= t
+							#pragma unroll
+							for (int st = 16; st; st >>= 1) {
+								const u32 probe = __shfl_sync(0xffffffffu, off, (c + st) & 31);
+								if (c + st < 32 && probe <= t) c += st;
+							}
+							const u32 q = __shfl_sync(0xffffffffu, qb, c) + (t - __shfl_sync(0xffffffffu, off, c));
+							if (t < total) ray_test(S, order[q], o, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+						}
+					}
+				}
+			}
+		}
+		const u64 wbest = warp_min_u64(best);
+		const u32 winner = wbest == ~(u64)0 ? 0u : (u32)__ffs(__ballot_sync(0xffffffffu, best == wbest)) - 1;
+		if (lane == winner) {
+			u32 w[12] = { 0, 0, 0, 0, 0, 0, 0, NB_RAY_NO_HIT, NB_RAY_NO_HIT, NB_RAY_NO_HIT, 0, 0 };   // a miss
+			if (wbest != ~(u64)0) {
+				const float t = asf((u32)(wbest >> 32));
+				const u32 i = (u32)wbest;
+				const f3 p = add3(o, mul3(t, d));
+				w[0] = asu(p.x); w[1] = asu(p.y); w[2] = asu(p.z); w[3] = asu(t); w[4] = asu(bn.x); w[5] = asu(bn.y); w[6] = asu(bn.z);
+				w[7] = i; w[8] = __ldg(S.col_body + i); w[9] = __ldg(S.col_tag + i);
+			}
+			u32* out = reinterpret_cast<u32*>(hits + ri);   // 4-byte stores: nb_ray_hit is only 4-byte aligned
+			#pragma unroll
+			for (int k = 0; k < 12; ++k) out[k] = w[k];
+		}
+	}
+}
+
+// The query's scratch for the collider capacity, allocated once (synchronises `st` then; never again).
+static int ensure_ray_scratch(nb_context* ctx, cudaStream_t st) {
+	RayScratch& r = ctx->ray;
+	const size_t K = std::max<size_t>(1, (size_t)ctx->cfg.max_boxes + ctx->cfg.max_spheres);
+	if (r.ready) return NB_OK;
+	GROW(r.world_xf, K, st); GROW(r.aabb_min, K, st); GROW(r.aabb_max, K, st); GROW(r.leaf_min, K, st); GROW(r.leaf_max, K, st);
+	GROW(r.col_tag, K, st); GROW(r.col_body, K, st); GROW(r.order, K, st); GROW(r.rank, K, st); GROW(r.large_list, K, st);
+	GROW(r.mkeys, K, st); GROW(r.smallf, K, st);
+	for (int i = 0; i < 2; ++i) { GROW(r.keys[i], K, st); GROW(r.vals[i], K, st); }
+	size_t tsz = 1024; while (tsz < 2 * K) tsz *= 2;
+	r.table_mask = (u32)(tsz - 1);
+	GROW(r.table_keys, tsz, st); GROW(r.table_vals, tsz, st);
+	GROW(r.keybits, 2, st); GROW(r.hist, 256 * (size_t)ctx->sms, st); GROW(r.counts, CNT__COUNT, st);
+	CK(cudaMemsetAsync(r.counts.p, 0, sizeof(u32) * CNT__COUNT, st));   // the sort's grid barrier starts from zero arrivals
+	CK(cudaStreamSynchronize(st));
+	r.sb = { { r.keys[0].p, r.keys[1].p }, { r.vals[0].p, r.vals[1].p }, r.hist.p, r.counts.p + CNT_BAR0 };
+	r.ready = true;   // only once every buffer exists: a failed allocation leaves the next call to try again
+	return NB_OK;
+}
+
+extern "C" {
+
+int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream) {
+	NB_RANGE("nb_raycast");
+	if (ctx->sharded) { ctx->error = "nb_raycast: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
+	if (flags & ~(u32)NB_RAY_SENSORS) { ctx->error = "nb_raycast: unknown flags"; return NB_ERR_ARGUMENT; }
+	if (n && (!rays || !hits)) { ctx->error = "nb_raycast: null rays or hits"; return NB_ERR_ARGUMENT; }
+	if (!n) return NB_OK;
+	cudaStream_t st = (cudaStream_t)stream;
+	{ int r = ensure_ray_scratch(ctx, st); if (r) return r; }
+	RayScratch& q = ctx->ray;
+	const nb_ray* drays = rays;
+	nb_ray_hit* dhits = hits;
+	if (!on_device) {
+		GROW(q.rays, n, st); GROW(q.hits, n, st);
+		CK(put_staged(ctx, q.rays.p, rays, sizeof(nb_ray) * (size_t)n, st));
+		drays = q.rays.p; dhits = q.hits.p;
+	}
+	const Launch L = mk_launch(ctx, st);
+	const u32 K = ctx->B ? ctx->nboxes + ctx->nspheres : 0;
+	u32* counts = q.counts.p;
+	if (K) {   // nb_collide's front end (nb_api.cu, nb_collide), on the query's buffers, without the kinematic table
+		launch(L, k_reset_collide, 1, 32, 0, counts, K, q.keybits.p);
+		launch_grid(L, k_collider_world, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
+			ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr, q.world_xf.p, q.aabb_min.p, q.aabb_max.p,
+			q.col_tag.p, q.col_body.p, counts);
+		launch_grid(L, k_morton, GRID(K), K, q.aabb_min.p, q.aabb_max.p, counts, q.sb.keys[0], q.sb.vals[0], q.keybits.p);
+		const int cur = nb_radix_sort(L, q.sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, q.keybits.p);
+		launch_grid(L, k_leaves, GRID(K), K, q.sb.vals[cur], q.sb.keys[cur], q.aabb_min.p, q.aabb_max.p, q.order.p, q.rank.p, q.leaf_min.p, q.leaf_max.p, q.mkeys.p, counts);
+		CK(cudaMemsetAsync(q.table_keys.p, 0xff, sizeof(u64) * ((size_t)q.table_mask + 1), st));
+		launch_grid(L, k_grid_build, GRID(K), K, q.order.p, q.leaf_min.p, q.leaf_max.p, q.mkeys.p, q.smallf.p, q.large_list.p, q.table_keys.p, q.table_vals.p,
+			q.table_mask, counts);
+	}
+	const RayScene S = { K, ctx->nboxes, q.world_xf.p, q.aabb_max.p, q.col_body.p, q.col_tag.p, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
+	launch_grid(L, k_raycast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, drays, dhits, flags, S, q.order.p, q.table_keys.p, q.table_vals.p, q.table_mask,
+		q.large_list.p, counts);
+	CK(cudaGetLastError());
+	if (!on_device) {
+		CK(cudaMemcpyAsync(hits, dhits, sizeof(nb_ray_hit) * (size_t)n, cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+	}
+	return NB_OK;
+}
+
+}  // extern "C"
