@@ -1180,6 +1180,9 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
 	}
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
+	// the last collide's broadphase: the grid level (cell edge 2^level quantised units) and how many colliders went to k_large_pairs
+	if (!strcmp(name, "grid_level")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_GRID_LEVEL]; if (bytes) *bytes = 4; return NB_OK; }
+	if (!strcmp(name, "grid_large")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_LARGE]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
 	if (!strcmp(name, "jacobi_stages")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)jacobi_stages(ctx); if (bytes) *bytes = 4; return NB_OK; }

@@ -226,9 +226,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_leaves(u32 K, const u32* sorted_va
 // ---------------- K4: grid broadphase on top of the Morton order ----------------
 // The Morton-sorted colliders are already sorted by octree cell at every level: the colliders of the level-j cell with integer
 // coordinates (cx,cy,cz) are the contiguous range of sorted positions whose 48-bit code has the prefix morton(cx,cy,cz) >> 3j.
-// Level j is chosen per step so that a cell is at least twice the mean AABB extent.  A collider whose extent (in quantised
+// Level j is chosen per step from k_morton's histogram (grid_setup).  A collider whose extent (in quantised
 // units, +2 for rounding) fits one cell is "small": two overlapping small colliders have min-corner cells that differ by at
-// most 1 per axis, so a small collider only has to look into the 27 cells around its own (found through a hash table
+// most 1 per axis (the quantisation rounds once, DESIGN.md section 2.3), so a small collider only has to look into the 27 cells around its own (found through a hash table
 // cell -> sorted range).  The few "large" colliders (the ground; also anything whose quantised corner wrapped past 65535,
 // nudge.cpp:2613-2616 masks it) are tested against everybody by brute force.  The union is exactly the set of strictly
 // overlapping pairs, reported once, oriented by Morton position like nudge.cpp:3495.
