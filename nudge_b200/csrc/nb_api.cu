@@ -29,17 +29,24 @@ template<class T> struct DevBuf {
 	~DevBuf() { if (p) cudaFree(p); }
 };
 
-// The host side of a joint set (nb_joint_api.cuh): per joint in upload order its (type, a, b) and its position in the device table, which
-// holds the joints by level; the levels' offsets into the table; the number of rows the joints generate.
-struct JointSet { u32 n = 0, nrows = 0, levels = 0; std::vector<u32> structure, level_off, order; };
+// Entries levelled by body (level_rows, nb_rows_api.cuh), the user rows or the joints: each one's (a, b) in upload order and device position
+// (by level, upload order within one), and the levels' offsets (levels + 1, none without entries), host values in nb_step's graph.
+struct RowLevels { u32 n = 0, levels = 0; std::vector<u32> level_off, order; std::vector<nb_body_pair> ab; };
 
-// The ray casts' own copy of the collide front end's buffers (nb_query_api.cuh), allocated on the first nb_raycast for the collider
-// capacity, so that a query never touches what the step reads; rays / hits = the staging of a call with host pointers.
-struct RayScratch {
-	DevBuf<nb_transform> world_xf; DevBuf<float4> aabb_min, aabb_max, leaf_min, leaf_max;
-	DevBuf<u32> col_tag, col_body, order, rank, large_list, vals[2], counts, hist; DevBuf<u64> keys[2], mkeys, table_keys, table_vals, keybits;
-	DevBuf<uint8_t> smallf; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; u32 table_mask = 0; SortBuffers sb = {}; bool ready = false;
+// The host side of a joint set (nb_joint_api.cuh): its levels (the device table holds the joints by level), per joint in upload order its
+// (type, a, b), and the number of rows the joints generate.
+struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; };
+
+// The buffers of nb_collide's front end (launch_front_end); leaf_* = the AABBs in Morton order, keybits = the OR and AND of the Morton codes.
+// The context has one, the ray casts their own (nb_query_api.cuh), so that a query never touches what the step reads.
+struct FrontEnd {
+	nb_transform* world_xf; float4* aabb_min; float4* aabb_max; u32* col_tag; u32* col_body; u32* order; u32* rank;
+	float4* leaf_min; float4* leaf_max; u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask; u64* keybits;
 };
+
+// The ray casts' scratch (nb_query_api.cuh): the front end, its sort buffers and counters, allocated on the first nb_raycast for the
+// collider capacity; rays / hits = the staging of a call with host pointers.
+struct RayScratch { FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; bool ready; };
 
 struct nb_context {
 	nb_config cfg;
@@ -59,7 +66,6 @@ struct nb_context {
 	u32 cstride;   // row plane stride
 	u32 slots_per_bucket;
 	int coop_blocks_solve;
-	u64* keybits;  // OR, AND of the Morton codes of the current collide
 	StepGraph graph; bool capturing;  // nb_step's graph; capturing: run_graphed is recording a step of this context
 	unsigned long long graph_epoch;   // in the graphs' key: bumped by every change of which kernels a step launches or of their arguments
 	u32* chain_start; u32* chain_len;  // per body: segment cursor (the segment's end once k_chain_scatter ran) / number of chain entries
@@ -74,7 +80,7 @@ struct nb_context {
 	// nb_upload_bodies sends what the collision stage does not read (momentum, properties) on a second stream, so that copy runs under
 	// `collide`; the first consumer waits for ev_up_done (inside a captured step: an external event-wait node, re-armed by every upload)
 	cudaStream_t copy_stream; cudaEvent_t ev_up_begin, ev_up_done; bool upload_pending, capture_joined; int copy_overlap;
-	DevBuf<nb_constraint_row> urows; u32 urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order;
+	DevBuf<nb_constraint_row> urows; RowLevels urow_set;
 	// contact events (nb_enable_contact_events, nb_events.cuh): ev_cap = 0 is off; the buffer is kept while it holds ev_cap events
 	DevBuf<nb_contact_event> events; u32 ev_cap;
 	// collision filters (nb_upload_collision_filters): one category | mask << 16 word per collider while has_filter; with
@@ -92,10 +98,9 @@ struct nb_context {
 	// and its sort histogram, grid barrier and key count; none of it is shared with the step
 	DevBuf<nb_body_impulse> imp_rows; DevBuf<u64> imp_keys[2]; SortBuffers imp_sb; u32* imp_n;
 	// spawning (nb_add_bodies, nb_remove_bodies, DESIGN.md section 8.10): scene_edited refuses the stage calls that read the last collide's
-	// outputs until the next collide; sharded = nb_shard_create was called on this context (edits are refused); urow_ab = each user row's
-	// (a, b) in upload order, for re-levelling after a removal; spawn_idx / urows_spare = the removal's index staging and row gather buffers
-	// conn_host = the connections as uploaded or loaded, for the removal's index checks
-	bool scene_edited, sharded; std::vector<nb_body_pair> urow_ab, conn_host; DevBuf<u32> spawn_idx; DevBuf<nb_constraint_row> urows_spare;
+	// outputs until the next collide; sharded = nb_shard_create was called on this context (edits are refused); spawn_idx / urows_spare =
+	// the removal's index staging and row gather buffers; conn_host = the connections as uploaded or loaded, for the removal's index checks
+	bool scene_edited, sharded; std::vector<nb_body_pair> conn_host; DevBuf<u32> spawn_idx; DevBuf<nb_constraint_row> urows_spare;
 	// per-body forces (nb_set_body_forces, DESIGN.md section 8.11): frc = one entry per body while has_frc, allocated for max_bodies on the
 	// first call, together with frc_spare (nb_remove_bodies gathers into it); frc_rows = the scatter's staging rows
 	nb_body_force* frc; nb_body_force* frc_spare; bool has_frc; DevBuf<nb_body_force> frc_rows;
@@ -115,9 +120,7 @@ struct nb_context {
 	nb_body_pair* conn;
 	u32* counts;
 	// collide
-	nb_transform* world_xf; float4* aabb_min; float4* aabb_max; u32* col_tag; u32* col_body; u32* order; u32* rank;
-	float4* leaf_min; float4* leaf_max;  // AABBs in Morton order
-	u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask;
+	FrontEnd front;
 	SortBuffers sb; u32 sort_cap;
 	u64* pair_keys;  // alias into sb.keys[] after the pair sort
 	u64* pair_keys_debug;  // copy kept for parity tests when debug is enabled (the sort buffers are reused later in the step)
@@ -210,6 +213,40 @@ __global__ void k_reset_collide(u32* counts, u32 K, u64* keybits) {
 		for (int k = 0; k < 4; ++k) { counts[CNT_BMIN0 + k] = 0xffffffffu; counts[CNT_BMAX0 + k] = 0; }
 	}
 }
+
+// dev_alloc of a buffer that does not exist yet: a routine that allocates several can run again after a failure and allocates the rest.
+template<class T> static int alloc_once(nb_context* ctx, T*& p, size_t n) { return p ? NB_OK : dev_alloc(ctx, &p, n); }
+
+// The buffers of `f` for K colliders of capacity.
+static int alloc_front_end(nb_context* ctx, FrontEnd& f, u32 K) {
+	u32 tsz = 1024; while (tsz < 2 * K) tsz *= 2;
+	f.table_mask = tsz - 1;
+	if (alloc_once(ctx, f.keybits, 2) || alloc_once(ctx, f.world_xf, K) || alloc_once(ctx, f.aabb_min, K) || alloc_once(ctx, f.aabb_max, K) ||
+		alloc_once(ctx, f.col_tag, K) || alloc_once(ctx, f.col_body, K) || alloc_once(ctx, f.order, K) || alloc_once(ctx, f.rank, K) ||
+		alloc_once(ctx, f.leaf_min, K) || alloc_once(ctx, f.leaf_max, K) || alloc_once(ctx, f.mkeys, K) || alloc_once(ctx, f.smallf, K) ||
+		alloc_once(ctx, f.large_list, K) || alloc_once(ctx, f.table_keys, tsz) || alloc_once(ctx, f.table_vals, tsz)) return NB_ERR_CUDA;
+	return NB_OK;
+}
+
+// nb_collide's front end on `f`, with its counters in `counts` and the Morton sort on `sb`: the counters' reset, then, with colliders and
+// bodies, the world transforms and AABBs (with the filter, kinematic and sensor tables given; null: none), the Morton codes and their sort,
+// the leaves in Morton order and the grid table.
+static int launch_front_end(nb_context* ctx, const Launch& L, const FrontEnd& f, const SortBuffers& sb, u32* counts, const u32* filter,
+							const uint8_t* kind, const uint8_t* sensor) {
+	const u32 K = ctx->nboxes + ctx->nspheres;
+	launch(L, k_reset_collide, 1, 32, 0, counts, K, f.keybits);
+	if (K == 0 || ctx->B == 0) return NB_OK;
+	launch_grid(L, k_collider_world, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
+		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, filter, kind, sensor, f.world_xf, f.aabb_min, f.aabb_max, f.col_tag, f.col_body, counts);
+	launch_grid(L, k_morton, GRID(K), K, f.aabb_min, f.aabb_max, counts, sb.keys[0], sb.vals[0], f.keybits);
+	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
+	const int cur = nb_radix_sort(L, sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, f.keybits);
+	launch_grid(L, k_leaves, GRID(K), K, sb.vals[cur], sb.keys[cur], f.aabb_min, f.aabb_max, f.order, f.rank, f.leaf_min, f.leaf_max, f.mkeys, counts);
+	CK(cudaMemsetAsync(f.table_keys, 0xff, sizeof(u64) * ((size_t)f.table_mask + 1), L.stream));
+	launch_grid(L, k_grid_build, GRID(K), K, f.order, f.leaf_min, f.leaf_max, f.mkeys, f.smallf, f.large_list, f.table_keys, f.table_vals, f.table_mask, counts);
+	return NB_OK;
+}
+
 __global__ void __launch_bounds__(NB_BLOCK) k_copy_u64(const u64* src, u64* dst, const u32* n_ptr) {
 	u32 n = *n_ptr;
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = src[i];
@@ -396,13 +433,14 @@ static int set_sensors(nb_context* ctx, const uint8_t* host, u32 n, u32 max_pair
 static void launch_sensor_overlaps(nb_context* ctx, const Launch& L) {
 	u32* counts = ctx->counts;
 	const u32 cap = ctx->sensor_cap;
-	launch_grid(L, k_sensor_np, GRID((size_t)cap * 4), ctx->sensor_keys.p, cap, ctx->kbits, ctx->nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data,
-		ctx->col_tag, ctx->col_body, ctx->flags, counts);
+	const FrontEnd& f = ctx->front;
+	launch_grid(L, k_sensor_np, GRID((size_t)cap * 4), ctx->sensor_keys.p, cap, ctx->kbits, ctx->nboxes, f.world_xf, ctx->box_data, ctx->sph_data,
+		f.col_tag, f.col_body, ctx->flags, counts);
 	nb_scan_reduce<1>(L, ctx->flags, ctx->stride, counts + CNT_SENSOR_PAIRS, 0, ctx->block_sums, counts + CNT_SENSOR_HITS);
-	launch_grid(L, k_sensor_compact, NB_SCAN_GRID, ctx->flags, ctx->block_sums, ctx->sensor_keys.p, ctx->kbits, ctx->col_tag,
+	launch_grid(L, k_sensor_compact, NB_SCAN_GRID, ctx->flags, ctx->block_sums, ctx->sensor_keys.p, ctx->kbits, f.col_tag,
 		ctx->sensor_sb.keys[0], ctx->sensor_sb.vals[0], counts);
 	const int cur = nb_radix_sort(L, ctx->sensor_sb, counts + CNT_SENSOR_HITS, 0, (int)ctx->tagbits, true, 0, 32, (int)(32 + ctx->tagbits));
-	launch_grid(L, k_sensor_gather, GRID(cap), ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys.p, ctx->kbits, ctx->col_tag, ctx->col_body,
+	launch_grid(L, k_sensor_gather, GRID(cap), ctx->sensor_sb.keys[cur], ctx->sensor_sb.vals[cur], ctx->sensor_keys.p, ctx->kbits, f.col_tag, f.col_body,
 		ctx->sensor_cur.p, counts);
 }
 
@@ -455,15 +493,8 @@ int nb_create(const nb_config* config, nb_context** out) {
 	ALLOC(ctx->sph_tags, c.max_spheres); ALLOC(ctx->sph_data, c.max_spheres); ALLOC(ctx->sph_xf, c.max_spheres);
 	ALLOC(ctx->conn, c.max_connections);
 	ALLOC(ctx->filter, K); ALLOC(ctx->sensor, K); ALLOC(ctx->conn_keys, c.max_connections); ALLOC(ctx->conn_scratch, c.max_connections); ALLOC(ctx->conn_sort_n, 1);
-	ALLOC(ctx->counts, CNT__COUNT); ALLOC(ctx->keybits, 2);
-	ALLOC(ctx->world_xf, K); ALLOC(ctx->aabb_min, K); ALLOC(ctx->aabb_max, K); ALLOC(ctx->col_tag, K); ALLOC(ctx->col_body, K);
-	ALLOC(ctx->order, K); ALLOC(ctx->rank, K);
-	ALLOC(ctx->leaf_min, K); ALLOC(ctx->leaf_max, K);
-	{
-		u32 tsz = 1024; while (tsz < 2 * (K ? K : 1)) tsz *= 2;
-		ctx->table_mask = tsz - 1;
-		ALLOC(ctx->mkeys, K); ALLOC(ctx->smallf, K); ALLOC(ctx->large_list, K); ALLOC(ctx->table_keys, tsz); ALLOC(ctx->table_vals, tsz);
-	}
+	ALLOC(ctx->counts, CNT__COUNT);
+	{ int r = alloc_front_end(ctx, ctx->front, K); if (r) return r; }
 	ctx->sort_cap = std::max(std::max(K, P), 2 * C);
 	for (int i = 0; i < 2; ++i) { ALLOC(ctx->sb.keys[i], ctx->sort_cap); ALLOC(ctx->sb.vals[i], ctx->sort_cap); }
 	ALLOC(ctx->sb.hist, 256 * (size_t)ctx->sms);
@@ -750,28 +781,20 @@ int nb_collide(nb_context* ctx, void* stream) {
 	ctx->in_step = true;   // until the nb_advance that ends the step
 	ctx->step_dt = 0.0f;
 	Launch L = mk_launch(ctx, stream);
-	cudaStream_t st = L.stream;
 	const u32 K = ctx->nboxes + ctx->nspheres, B = ctx->B, nboxes = ctx->nboxes;
 	u32* counts = ctx->counts;
 	uint8_t* kind = ctx->has_kin ? ctx->kind : nullptr;
 	if (kind) JOIN_UPLOADS();   // k_uf_init reads the kinematic bodies' momentum rows
-	launch(L, k_reset_collide, 1, 32, 0, counts, K, ctx->keybits);
-	if (K == 0 || B == 0) return NB_OK;
-	launch_grid(L, k_collider_world, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
-		ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, kind, ctx->has_sensor ? ctx->sensor : nullptr, ctx->world_xf, ctx->aabb_min, ctx->aabb_max, ctx->col_tag, ctx->col_body, counts);
-	launch_grid(L, k_morton, GRID(K), K, ctx->aabb_min, ctx->aabb_max, counts, ctx->sb.keys[0], ctx->sb.vals[0], ctx->keybits);
-	// radix sort on the 48-bit code; ties keep index order like the stable sort of nudge.cpp:3165
-	int cur = nb_radix_sort(L, ctx->sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, ctx->keybits);
-	launch_grid(L, k_leaves, GRID(K), K, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->aabb_min, ctx->aabb_max, ctx->order, ctx->rank, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, counts);
-	CK(cudaMemsetAsync(ctx->table_keys, 0xff, sizeof(u64) * ((size_t)ctx->table_mask + 1), st));
-	launch_grid(L, k_grid_build, GRID(K), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->mkeys, ctx->smallf, ctx->large_list, ctx->table_keys, ctx->table_vals, ctx->table_mask, counts);
 	const uint8_t* sensor = ctx->has_sensor ? ctx->sensor : nullptr;   // null: the kernels never touch the sensor list
-	launch_grid(L, kind ? k_grid_pairs<true> : k_grid_pairs<false>, GRID((size_t)K * 32), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->mkeys, ctx->table_keys, ctx->table_vals, ctx->table_mask, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
-	launch_grid(L, k_large_pairs, GRID(K), K, ctx->order, ctx->leaf_min, ctx->leaf_max, ctx->smallf, ctx->large_list, ctx->kbits,
-		ctx->col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	const FrontEnd& f = ctx->front;
+	int r = launch_front_end(ctx, L, f, ctx->sb, counts, ctx->has_filter ? ctx->filter : nullptr, kind, sensor);
+	if (r || K == 0 || B == 0) return r;
+	launch_grid(L, kind ? k_grid_pairs<true> : k_grid_pairs<false>, GRID((size_t)K * 32), K, f.order, f.leaf_min, f.leaf_max, f.smallf, f.mkeys, f.table_keys, f.table_vals, f.table_mask, ctx->kbits,
+		f.col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
+	launch_grid(L, k_large_pairs, GRID(K), K, f.order, f.leaf_min, f.leaf_max, f.smallf, f.large_list, ctx->kbits,
+		f.col_body, ctx->conn_keys, ctx->conn_probe, sensor, ctx->sensor_keys.p, ctx->sensor_cap, ctx->sb.keys[0], ctx->cfg.max_pairs, counts);
 	// nudge.cpp:3498; the sort also clamps CNT_PAIRS to the capacity (the overflow bit is already set by emit_pair)
-	cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);
+	int cur = nb_radix_sort(L, ctx->sb, counts + CNT_PAIRS, 0, (int)(2 * ctx->kbits), false, 0, 0, 0, nullptr, ctx->cfg.max_pairs);
 	ctx->pair_keys = ctx->sb.keys[cur];
 	if (ctx->debug) launch_grid(L, k_copy_u64, GRID(ctx->cfg.max_pairs), ctx->pair_keys, ctx->pair_keys_debug, counts + CNT_PAIRS);
 
@@ -779,20 +802,20 @@ int nb_collide(nb_context* ctx, void* stream) {
 	const u32 P = ctx->cfg.max_pairs, S = ctx->stride;
 	launch_grid(L, k_uf_init, GRID(B), ctx->parent, ctx->active, ctx->taint, kind, ctx->mom, B);
 	if (ctx->nconn) launch_grid(L, k_uf_union_conn, GRID(ctx->nconn), ctx->parent, ctx->taint, ctx->idle, kind, ctx->conn, ctx->nconn);
-	launch_grid(L, k_uf_union_pairs, GRID(P), ctx->parent, ctx->taint, ctx->idle, kind, ctx->pair_keys, ctx->kbits, ctx->col_body, counts);
+	launch_grid(L, k_uf_union_pairs, GRID(P), ctx->parent, ctx->taint, ctx->idle, kind, ctx->pair_keys, ctx->kbits, f.col_body, counts);
 	launch_grid(L, k_uf_flatten_active, GRID(B), ctx->parent, ctx->active, ctx->taint, ctx->idle, kind, B);
-	launch_grid(L, k_pair_flags, GRID(P), ctx->pair_keys, ctx->kbits, nboxes, ctx->col_body, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
+	launch_grid(L, k_pair_flags, GRID(P), ctx->pair_keys, ctx->kbits, nboxes, f.col_body, ctx->parent, ctx->active, kind, ctx->flags, S, counts);
 	nb_scan_reduce<5>(L, ctx->flags, S, counts + CNT_PAIRS, 0, ctx->block_sums, counts + CNT_LIVE0);  // -> LIVE0..3, SLEEP_COARSE
-	launch_grid(L, k_partition, NB_SCAN_GRID, ctx->pair_keys, ctx->kbits, ctx->flags, ctx->block_sums, S, ctx->col_tag, ctx->live, ctx->sleeping, counts);
+	launch_grid(L, k_partition, NB_SCAN_GRID, ctx->pair_keys, ctx->kbits, ctx->flags, ctx->block_sums, S, f.col_tag, ctx->live, ctx->sleeping, counts);
 
 	// narrowphase: count, scan, emit (nudge.cpp:3753-3786)
-	launch_grid(L, k_np_faces, GRID(P), ctx->live, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag, ctx->flags, S, ctx->np_pen, ctx->np_info, counts);
+	launch_grid(L, k_np_faces, GRID(P), ctx->live, nboxes, f.world_xf, ctx->box_data, ctx->sph_data, f.col_tag, ctx->flags, S, ctx->np_pen, ctx->np_info, counts);
 	nb_scan_reduce<1>(L, ctx->flags + 3 * (size_t)S, S, counts + CNT_LIVE0, 0, ctx->block_sums, counts + CNT_SURV);
 	launch_grid(L, k_np_list, NB_SCAN_GRID, ctx->flags, ctx->block_sums, S, ctx->np_list, counts);
-	launch_grid(L, k_np_clip, GRID(P), ctx->live, ctx->np_list, ctx->np_pen, ctx->np_info, ctx->world_xf, ctx->box_data, ctx->col_tag, ctx->flags, S,
+	launch_grid(L, k_np_clip, GRID(P), ctx->live, ctx->np_list, ctx->np_pen, ctx->np_info, f.world_xf, ctx->box_data, f.col_tag, ctx->flags, S,
 		ctx->fin /* scratch: rewritten by k_contact_compact below */, ctx->np_start, ctx->cfg.max_contacts, counts);
 	nb_scan<3>(L, ctx->flags, ctx->offs, S, counts + CNT_LIVE_TOTAL, 0, ctx->block_sums, counts + CNT_FACE);  // -> FACE, EDGE, OTHER
-	launch_grid(L, k_np_emit, GRID(P), ctx->live, ctx->np_list, ctx->np_start, ctx->fin, nboxes, ctx->world_xf, ctx->box_data, ctx->sph_data, ctx->col_tag,
+	launch_grid(L, k_np_emit, GRID(P), ctx->live, ctx->np_list, ctx->np_start, ctx->fin, nboxes, f.world_xf, ctx->box_data, ctx->sph_data, f.col_tag,
 		ctx->flags, ctx->offs, S, ctx->staged, ctx->cfg.max_contacts, counts);
 
 	// fine islands, active bodies, contact compaction (nudge.cpp:3788-4006)
@@ -1027,7 +1050,7 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	int r = build_contact_rows(ctx, st); if (r) return r;
 	// the warm start (nudge.cpp:4563-4632), then the user rows' accumulated impulses, then the joints' rows and theirs
 	if ((r = launch_solve(ctx, true, 0, st))) return r;
-	if (ctx->urow_n && (r = launch_user_rows(ctx, 1, st))) return r;
+	if (ctx->urow_set.n && (r = launch_user_rows(ctx, 1, st))) return r;
 	if (ctx->jset.n && (r = launch_joints(ctx, &ctx->step_dt, st))) return r;
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -1039,10 +1062,10 @@ int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 	JOIN_UPLOADS();
 	if (!sweeps) return NB_OK;
 	cudaStream_t st = (cudaStream_t)stream;
-	if (ctx->urow_n || ctx->jset.n) {   // user rows, then joints, run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
+	if (ctx->urow_set.n || ctx->jset.n) {   // user rows, then joints, run after EVERY sweep (example/main.cpp:314-317): one sweep per solver launch
 		for (uint32_t w = 0; w < sweeps; ++w) {
 			int r = launch_solve(ctx, false, 1, st); if (r) return r;
-			if (ctx->urow_n && (r = launch_user_rows(ctx, 0, st))) return r;
+			if (ctx->urow_set.n && (r = launch_user_rows(ctx, 0, st))) return r;
 			if (ctx->jset.n && (r = launch_joints(ctx, nullptr, st))) return r;
 		}
 		return NB_OK;
@@ -1073,7 +1096,7 @@ int nb_advance(nb_context* ctx, float time_step, void* stream) {
 // nb_step's solve section: nb_setup_contact_constraints + nb_apply_impulses, or without user rows or joints between the sweeps, the row build and
 // the warm start straight into the sweeps' working rows (the same arithmetic in the same order).
 static int step_solve(nb_context* ctx, uint32_t iterations, void* stream) {
-	if (iterations > 0 && !ctx->urow_n && !ctx->jset.n) {
+	if (iterations > 0 && !ctx->urow_set.n && !ctx->jset.n) {
 		cudaStream_t st = (cudaStream_t)stream;
 		int r = build_contact_rows(ctx, st); if (r) return r;
 		if ((r = launch_solve(ctx, true, iterations, st))) return r;
@@ -1135,10 +1158,10 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	struct Entry { const char* name; const void* ptr; size_t bytes; };
 	const Entry table[] = {
 		{ "counts", ctx->counts, sizeof(u32) * CNT__COUNT },
-		{ "order", ctx->order, sizeof(u32) * K },
-		{ "aabb_min", ctx->aabb_min, sizeof(float4) * K },
-		{ "aabb_max", ctx->aabb_max, sizeof(float4) * K },
-		{ "world_xf", ctx->world_xf, sizeof(nb_transform) * K },
+		{ "order", ctx->front.order, sizeof(u32) * K },
+		{ "aabb_min", ctx->front.aabb_min, sizeof(float4) * K },
+		{ "aabb_max", ctx->front.aabb_max, sizeof(float4) * K },
+		{ "world_xf", ctx->front.world_xf, sizeof(nb_transform) * K },
 		{ "pair_keys", ctx->pair_keys_debug, sizeof(u64) * (ctx->pair_keys_debug ? c[CNT_PAIRS] : 0) },
 		{ "live", ctx->live, sizeof(uint2) * c[CNT_LIVE_TOTAL] },
 		{ "sorted", ctx->sorted, sizeof(u32) * c[CNT_CONTACTS] },
@@ -1174,7 +1197,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		if (max_bytes < 4) return NB_ERR_ARGUMENT;
 		u32 v = 0;
 		if (ctx->ray.ready) {
-			CK(cudaMemcpyAsync(&v, ctx->ray.counts.p + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+			CK(cudaMemcpyAsync(&v, ctx->ray.counts + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
 			CK(cudaStreamSynchronize((cudaStream_t)stream));
 		}
 		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;

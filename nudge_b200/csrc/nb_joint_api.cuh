@@ -7,8 +7,7 @@
 // accumulated impulses in the rows, which k_joint_rows rewrites around them.  Included at the end of nb_api.cu.
 #pragma once
 
-static const u32 kJointRows[4] = { 3, 5, 6, 1 };   // by nb_joint_type
-NB_DEV u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
+__host__ __device__ __forceinline__ u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
 
 NB_DEV f3 neg3(f3 a) { return mk3(-a.x, -a.y, -a.z); }
 // Writes one row around its accumulated impulse.
@@ -118,17 +117,15 @@ static int check_joints(nb_context* ctx, const nb_joint* h, u32 n, u32 B) {
 static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st) {
 	if (!n) { drop_joints(ctx); return NB_OK; }
 	JointSet js;
-	js.n = n;
 	std::vector<nb_body_pair> ab(n);
 	for (u32 i = 0; i < n; ++i) { ab[i].a = h[i].a; ab[i].b = h[i].b; js.structure.insert(js.structure.end(), { h[i].type, h[i].a, h[i].b }); }
-	js.levels = level_rows(ab, js.level_off, js.order);
-	if (js.levels > 4096) { ctx->error = "joints form a dependency chain longer than 4096 levels: reorder them (e.g. red-black along a chain)"; return NB_ERR_CAPACITY; }
+	if (int r = level_rows(ctx, std::move(ab), js, "joints")) return r;
 	std::vector<nb_joint> table(n);
 	for (u32 i = 0; i < n; ++i) table[js.order[i]] = h[i];
-	for (nb_joint& j : table) { const u32 type = j.type; j.type = type | js.nrows << 2; js.nrows += kJointRows[type]; }
+	for (nb_joint& j : table) { const u32 type = j.type; j.type = type | js.nrows << 2; js.nrows += joint_row_count(type); }
 	std::vector<nb_constraint_row> rows(js.nrows);
 	memset(rows.data(), 0, sizeof(nb_constraint_row) * rows.size());
-	for (const nb_joint& j : table) for (u32 k = 0; k < kJointRows[j.type & 3u]; ++k) rows[(j.type >> 2) + k].impulse = j.impulse[k];
+	for (const nb_joint& j : table) for (u32 k = 0; k < joint_row_count(j.type & 3u); ++k) rows[(j.type >> 2) + k].impulse = j.impulse[k];
 	const void* before[2] = { ctx->joints.p, ctx->jrows.p };
 	GROW(ctx->joints, n, st); GROW(ctx->jrows, js.nrows, st);
 	CK(put_staged(ctx, ctx->joints.p, table.data(), sizeof(nb_joint) * (size_t)n, st));
@@ -153,7 +150,7 @@ static int get_joints(nb_context* ctx, std::vector<nb_joint>& out, cudaStream_t 
 		nb_joint j = table[js.order[i]];
 		const u32 first = j.type >> 2;
 		j.type &= 3u;
-		for (u32 k = 0; k < 6; ++k) j.impulse[k] = k < kJointRows[j.type] ? rows[first + k].impulse : 0.0f;
+		for (u32 k = 0; k < 6; ++k) j.impulse[k] = k < joint_row_count(j.type) ? rows[first + k].impulse : 0.0f;
 		out[i] = j;
 	}
 	return NB_OK;

@@ -1,6 +1,6 @@
 // nudge_b200 — ray casts against the current colliders (nb_raycast, include/nudge_b200.h; DESIGN.md section 8.14).
-// The build is nb_collide's front end, launched unchanged on buffers of the query's own (RayScratch): world transforms and AABBs
-// (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid table (k_grid_build).  One new kernel walks it.
+// The build is nb_collide's front end (launch_front_end, nb_api.cu) on a FrontEnd of the query's own (RayScratch): world transforms and
+// AABBs (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid table (k_grid_build).  One new kernel walks it.
 // Included at the end of nb_api.cu.
 #pragma once
 
@@ -201,22 +201,14 @@ __global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays,
 	}
 }
 
-// The query's scratch for the collider capacity, allocated once (synchronises `st` then; never again).
-static int ensure_ray_scratch(nb_context* ctx, cudaStream_t st) {
+// The query's scratch for the collider capacity, allocated once from the context's arena (synchronises then; never again).
+static int ensure_ray_scratch(nb_context* ctx) {
 	RayScratch& r = ctx->ray;
-	const size_t K = std::max<size_t>(1, (size_t)ctx->cfg.max_boxes + ctx->cfg.max_spheres);
+	const u32 K = ctx->cfg.max_boxes + ctx->cfg.max_spheres;
 	if (r.ready) return NB_OK;
-	GROW(r.world_xf, K, st); GROW(r.aabb_min, K, st); GROW(r.aabb_max, K, st); GROW(r.leaf_min, K, st); GROW(r.leaf_max, K, st);
-	GROW(r.col_tag, K, st); GROW(r.col_body, K, st); GROW(r.order, K, st); GROW(r.rank, K, st); GROW(r.large_list, K, st);
-	GROW(r.mkeys, K, st); GROW(r.smallf, K, st);
-	for (int i = 0; i < 2; ++i) { GROW(r.keys[i], K, st); GROW(r.vals[i], K, st); }
-	size_t tsz = 1024; while (tsz < 2 * K) tsz *= 2;
-	r.table_mask = (u32)(tsz - 1);
-	GROW(r.table_keys, tsz, st); GROW(r.table_vals, tsz, st);
-	GROW(r.keybits, 2, st); GROW(r.hist, 256 * (size_t)ctx->sms, st); GROW(r.counts, CNT__COUNT, st);
-	CK(cudaMemsetAsync(r.counts.p, 0, sizeof(u32) * CNT__COUNT, st));   // the sort's grid barrier starts from zero arrivals
-	CK(cudaStreamSynchronize(st));
-	r.sb = { { r.keys[0].p, r.keys[1].p }, { r.vals[0].p, r.vals[1].p }, r.hist.p, r.counts.p + CNT_BAR0 };
+	if (alloc_front_end(ctx, r.front, K) || alloc_once(ctx, r.sb.keys[0], K) || alloc_once(ctx, r.sb.keys[1], K) || alloc_once(ctx, r.sb.vals[0], K) ||
+		alloc_once(ctx, r.sb.vals[1], K) || alloc_once(ctx, r.sb.hist, 256 * (size_t)ctx->sms) || alloc_once(ctx, r.counts, CNT__COUNT)) return NB_ERR_CUDA;
+	r.sb.bar = r.counts + CNT_BAR0;   // zeroed by dev_alloc: the sort's grid barrier starts from zero arrivals
 	r.ready = true;   // only once every buffer exists: a failed allocation leaves the next call to try again
 	return NB_OK;
 }
@@ -230,7 +222,7 @@ int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits
 	if (n && (!rays || !hits)) { ctx->error = "nb_raycast: null rays or hits"; return NB_ERR_ARGUMENT; }
 	if (!n) return NB_OK;
 	cudaStream_t st = (cudaStream_t)stream;
-	{ int r = ensure_ray_scratch(ctx, st); if (r) return r; }
+	{ int r = ensure_ray_scratch(ctx); if (r) return r; }
 	RayScratch& q = ctx->ray;
 	const nb_ray* drays = rays;
 	nb_ray_hit* dhits = hits;
@@ -241,22 +233,13 @@ int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits
 	}
 	const Launch L = mk_launch(ctx, st);
 	const u32 K = ctx->B ? ctx->nboxes + ctx->nspheres : 0;
-	u32* counts = q.counts.p;
-	if (K) {   // nb_collide's front end (nb_api.cu, nb_collide), on the query's buffers, without the kinematic table
-		launch(L, k_reset_collide, 1, 32, 0, counts, K, q.keybits.p);
-		launch_grid(L, k_collider_world, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->box_tags,
-			ctx->sph_xf, ctx->sph_data, ctx->sph_tags, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr, q.world_xf.p, q.aabb_min.p, q.aabb_max.p,
-			q.col_tag.p, q.col_body.p, counts);
-		launch_grid(L, k_morton, GRID(K), K, q.aabb_min.p, q.aabb_max.p, counts, q.sb.keys[0], q.sb.vals[0], q.keybits.p);
-		const int cur = nb_radix_sort(L, q.sb, counts + CNT_SCRATCH1, 0, 48, true, 0, 0, 0, q.keybits.p);
-		launch_grid(L, k_leaves, GRID(K), K, q.sb.vals[cur], q.sb.keys[cur], q.aabb_min.p, q.aabb_max.p, q.order.p, q.rank.p, q.leaf_min.p, q.leaf_max.p, q.mkeys.p, counts);
-		CK(cudaMemsetAsync(q.table_keys.p, 0xff, sizeof(u64) * ((size_t)q.table_mask + 1), st));
-		launch_grid(L, k_grid_build, GRID(K), K, q.order.p, q.leaf_min.p, q.leaf_max.p, q.mkeys.p, q.smallf.p, q.large_list.p, q.table_keys.p, q.table_vals.p,
-			q.table_mask, counts);
-	}
-	const RayScene S = { K, ctx->nboxes, q.world_xf.p, q.aabb_max.p, q.col_body.p, q.col_tag.p, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
-	launch_grid(L, k_raycast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, drays, dhits, flags, S, q.order.p, q.table_keys.p, q.table_vals.p, q.table_mask,
-		q.large_list.p, counts);
+	u32* counts = q.counts;
+	const FrontEnd& f = q.front;
+	// the front end without the kinematic and sensor tables
+	if (int r = K ? launch_front_end(ctx, L, f, q.sb, counts, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr) : NB_OK) return r;
+	const RayScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
+	launch_grid(L, k_raycast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, drays, dhits, flags, S, f.order, f.table_keys, f.table_vals, f.table_mask,
+		f.large_list, counts);
 	CK(cudaGetLastError());
 	if (!on_device) {
 		CK(cudaMemcpyAsync(hits, dhits, sizeof(nb_ray_hit) * (size_t)n, cudaMemcpyDeviceToHost, st));

@@ -18,8 +18,6 @@
 #pragma once
 #include <map>
 
-struct RowsDev { nb_constraint_row* rows; u32* level_off; u32 n, levels; };
-
 // The two bodies of a row as the row update holds them: a kinematic side (kind non-null) is like body 0, infinite mass, its velocity read and
 // never written.  k_user_rows loads and stores them around one row, k_joint_solve (nb_joint_api.cuh) around all rows of a joint.
 struct RowBodies {
@@ -82,37 +80,40 @@ __global__ void __launch_bounds__(NB_BLOCK) k_user_rows(nb_constraint_row* rows,
 
 static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st) {
 	const Launch L = mk_launch(ctx, st);
-	for (u32 l = 0; l < ctx->urow_levels; ++l) {
-		const u32 b = ctx->urow_level_off[l], e = ctx->urow_level_off[l + 1];
+	const RowLevels& us = ctx->urow_set;
+	for (u32 l = 0; l < us.levels; ++l) {
+		const u32 b = us.level_off[l], e = us.level_off[l + 1];
 		if (e > b) launch_grid(L, k_user_rows, GRID(e - b), ctx->urows.p, b, e, ctx->mom, ctx->props, ctx->inertia, kin_table(ctx), warm);
 	}
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
-// The levels of rows (a, b) in upload order: a row's level is 1 + the highest level of an earlier row on either of its bodies (body 0 is
-// shared freely).  Fills level_off (levels + 1 offsets) and order (upload index -> device position: rows by level, upload order within one);
-// returns the number of levels.
-static u32 level_rows(const std::vector<nb_body_pair>& ab, std::vector<u32>& level_off, std::vector<u32>& order) {
-	const u32 n = (u32)ab.size();
-	std::vector<u32> level(n);
-	std::map<u32, u32> last;   // body -> level of the last row that touched it
-	u32 levels = 0;
-	for (u32 i = 0; i < n; ++i) {
+// Levels the entries (a, b) in upload order into `out`: an entry's level is 1 + the highest level of an earlier entry on either of its bodies
+// (body 0 is shared freely).  More than 4096 levels are refused with "<what> form a dependency chain ...", and `out` is left as it was.
+static int level_rows(nb_context* ctx, std::vector<nb_body_pair> ab, RowLevels& out, const char* what) {
+	RowLevels s;
+	s.n = (u32)ab.size();
+	std::vector<u32> level(s.n);
+	std::map<u32, u32> last;   // body -> level of the last entry that touched it
+	for (u32 i = 0; i < s.n; ++i) {
 		const u32 a = ab[i].a, b = ab[i].b;
 		u32 l = 0;
 		if (a) { auto it = last.find(a); if (it != last.end()) l = std::max(l, it->second + 1); }
 		if (b) { auto it = last.find(b); if (it != last.end()) l = std::max(l, it->second + 1); }
 		level[i] = l; if (a) last[a] = l; if (b) last[b] = l;
-		levels = std::max(levels, l + 1);
+		s.levels = std::max(s.levels, l + 1);
 	}
-	level_off.assign(levels + 1, 0);
-	for (u32 i = 0; i < n; ++i) ++level_off[level[i] + 1];
-	for (u32 l = 0; l < levels; ++l) level_off[l + 1] += level_off[l];
-	std::vector<u32> cursor(level_off.begin(), level_off.end() - 1);
-	order.resize(n);
-	for (u32 i = 0; i < n; ++i) order[i] = cursor[level[i]]++;
-	return levels;
+	if (s.levels > 4096) { ctx->error = std::string(what) + " form a dependency chain longer than 4096 levels: reorder them (e.g. red-black along a chain)"; return NB_ERR_CAPACITY; }
+	s.level_off.assign(s.n ? s.levels + 1 : 0, 0);
+	for (u32 i = 0; i < s.n; ++i) ++s.level_off[level[i] + 1];
+	for (u32 l = 0; l < s.levels; ++l) s.level_off[l + 1] += s.level_off[l];
+	std::vector<u32> cursor(s.level_off);
+	s.order.resize(s.n);
+	for (u32 i = 0; i < s.n; ++i) s.order[i] = cursor[level[i]]++;
+	s.ab = std::move(ab);
+	out = std::move(s);
+	return NB_OK;
 }
 
 extern "C" {
@@ -123,35 +124,33 @@ int nb_upload_constraint_rows(nb_context* ctx, const nb_constraint_row* rows, ui
 	cudaStream_t st = (cudaStream_t)stream;
 	CK(cudaStreamSynchronize(st));
 	if (n > ctx->urows.cap) GROW(ctx->urows, (size_t)n + n / 2 + 64, st);   // with headroom for a set that grows a little
-	ctx->urow_order.resize(n); ctx->urow_level_off.clear(); ctx->urow_ab.clear(); ctx->urow_n = n; ctx->urow_levels = 0; ++ctx->graph_epoch;
+	ctx->urow_set = RowLevels(); ++ctx->graph_epoch;   // a refused set leaves none
 	if (!n) return NB_OK;
 	std::vector<nb_body_pair> ab(n);
 	for (u32 i = 0; i < n; ++i) {
 		const u32 a = rows[i].a, b = rows[i].b;
-		if (a >= ctx->cfg.max_bodies || b >= ctx->cfg.max_bodies) { ctx->error = "constraint row references a body beyond max_bodies"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
+		if (a >= ctx->cfg.max_bodies || b >= ctx->cfg.max_bodies) { ctx->error = "constraint row references a body beyond max_bodies"; return NB_ERR_ARGUMENT; }
 		// k_user_rows gives each side its own read-modify-write of the momentum row, and the effective mass has no cross terms
-		if (a && a == b) { ctx->error = "constraint row names the same body as a and b: put the whole Jacobian on a and set b = 0"; ctx->urow_n = 0; return NB_ERR_ARGUMENT; }
+		if (a && a == b) { ctx->error = "constraint row names the same body as a and b: put the whole Jacobian on a and set b = 0"; return NB_ERR_ARGUMENT; }
 		ab[i].a = a; ab[i].b = b;
 	}
-	std::vector<u32> level_off, order;
-	const u32 levels = level_rows(ab, level_off, order);
-	if (levels > 4096) { ctx->error = "constraint rows form a dependency chain longer than 4096 levels: reorder them (e.g. red-black along a chain)"; ctx->urow_n = 0; return NB_ERR_CAPACITY; }
+	RowLevels set;
+	if (int r = level_rows(ctx, std::move(ab), set, "constraint rows")) return r;
 	std::vector<nb_constraint_row> sorted(n);
-	for (u32 i = 0; i < n; ++i) sorted[order[i]] = rows[i];
+	for (u32 i = 0; i < n; ++i) sorted[set.order[i]] = rows[i];
 	CK(cudaMemcpy(ctx->urows.p, sorted.data(), sizeof(nb_constraint_row) * n, cudaMemcpyHostToDevice));
-	ctx->urow_level_off.swap(level_off); ctx->urow_order.swap(order); ctx->urow_ab.swap(ab);
-	ctx->urow_levels = levels;
+	ctx->urow_set = std::move(set);
 	return NB_OK;
 }
 
 // Copies the rows back in the caller's order (the accumulated impulses are the result).  Synchronises.
 int nb_download_constraint_rows(nb_context* ctx, nb_constraint_row* rows, uint32_t n, void* stream) {
-	if (n != ctx->urow_n) { ctx->error = "row count differs from the uploaded set"; return NB_ERR_ARGUMENT; }
+	if (n != ctx->urow_set.n) { ctx->error = "row count differs from the uploaded set"; return NB_ERR_ARGUMENT; }
 	if (!n) return NB_OK;
 	CK(cudaStreamSynchronize((cudaStream_t)stream));
 	std::vector<nb_constraint_row> sorted(n);
 	CK(cudaMemcpy(sorted.data(), ctx->urows.p, sizeof(nb_constraint_row) * n, cudaMemcpyDeviceToHost));
-	for (u32 i = 0; i < n; ++i) rows[i] = sorted[ctx->urow_order[i]];
+	for (u32 i = 0; i < n; ++i) rows[i] = sorted[ctx->urow_set.order[i]];
 	return NB_OK;
 }
 

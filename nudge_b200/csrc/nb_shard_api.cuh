@@ -206,7 +206,7 @@ static int shard_solve(nb_shard* sh, uint32_t iterations, int transport, void* s
 	int r;
 	// the dataflow hand-over needs the peer inboxes, the exact-order solver without user rows between the sweeps, a solver grid and
 	// room for every pass in the pass-indexed inbox; everything else exchanges between the solver launches
-	if (sh->world > 1 && transport == NB_SHARD_PEER && sh->peers_ready && ctx->solver_mode == NB_SOLVER_PARITY && !ctx->urow_n &&
+	if (sh->world > 1 && transport == NB_SHARD_PEER && sh->peers_ready && ctx->solver_mode == NB_SOLVER_PARITY && !ctx->urow_set.n &&
 		sh->flow_blocks > 0 && iterations > 0 && iterations + 1 <= sh->passes_cap) {
 		// the rows without the warm start, which runs inside k_solve_flow (chain_len reads 0 for bodies without contacts on this rank)
 		if ((r = build_contact_rows(ctx, (cudaStream_t)stream))) return r;

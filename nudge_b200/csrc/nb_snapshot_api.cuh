@@ -52,20 +52,20 @@ struct nb_snapshot {
 	u32* words;
 	DevBuf<nb_constraint_row> rows;                  // user rows in device order
 	DevBuf<uint4> overlaps;                          // the sensor overlap list
-	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset;   // the joint table, the joints' rows and their host side
+	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows
 	// the host side at the save
-	NbStateHeader h; StateShape shape;
-	u32 urow_n, urow_levels; std::vector<u32> urow_level_off, urow_order; std::vector<nb_body_pair> urow_ab;
+	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset;
 };
 
 // A snapshot section: the context's buffer, the snapshot's copy, and the counter word (>= 0) that holds the element count on the device.
 struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool present; int word; };
 
-// The sections of a snapshot with header `h` and `urow_n` user rows: the state file's (a file keeps the kinematic indices on the host, the
-// snapshot keeps them in its host side and the kind bytes), then the snapshot's own.  The fixed sections come first, the rows and the
-// overlap list last.  With `s` null the snapshot pointers are offsets into the arena.
-static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 urow_n, u32 conn_probe) {
+// The sections of a snapshot with header `h`: the state file's (a file keeps the kinematic indices on the host, the snapshot keeps them in
+// its host side and the kind bytes), then the snapshot's own.  The fixed sections come first, the rows and the overlap list last.  With `s`
+// null the snapshot pointers are offsets into the arena, and there are no rows or joints.
+static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 conn_probe) {
 	const JointSet none, &js = s ? s->jset : none;
+	const u32 nrows = s ? s->urow_set.n : 0;
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
 	auto at = [&](size_t i) -> void* { return s ? s->arena.p + s->off[i] : nullptr; };
@@ -74,7 +74,7 @@ static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapsho
 	p.push_back({ ctx->kind, at(p.size()), 1, h.bodies, h.reserved[4] != 0, -1 });
 	p.push_back({ ctx->conn_keys, at(p.size()), 8, conn_probe, conn_probe != 0, -1 });
 	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s ? s->words + j : nullptr, 4, 1, true, -1 });
-	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), urow_n, urow_n != 0, -1 });
+	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), nrows, nrows != 0, -1 });
 	p.push_back({ ctx->joints.p, s ? s->joints.p : nullptr, sizeof(nb_joint), js.n, js.n != 0, -1 });
 	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), js.nrows, js.n != 0, -1 });
 	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
@@ -87,7 +87,7 @@ static const size_t kSnapFixed = 19 + 2;   // the state file's sections, the kin
 // side the copy comes from.
 static int snapshot_table(nb_context* ctx, const nb_snapshot* s, bool save, SnapTable& t) {
 	const u32 probe = (s->shape.filter_flags & NB_FILTER_SKIP_CONNECTED) ? s->shape.nconn : 0;
-	std::vector<SnapPart> parts = snapshot_sections(ctx, s, s->h, s->urow_n, probe);
+	std::vector<SnapPart> parts = snapshot_sections(ctx, s, s->h, probe);
 	if (!save && s->shape.has_sensor) {
 		parts.push_back({ ctx->sensor_cur.p, s->overlaps.p, sizeof(uint4), s->h.reserved[3], true, CNT_SENSOR_OLD });
 		parts.push_back({ ctx->counts + CNT_SENSOR_HITS, s->words + 2, 4, 1, true, -1 });
@@ -138,7 +138,7 @@ int nb_snapshot_create(nb_context* ctx, nb_snapshot** out) {
 	nb_snapshot* s = new nb_snapshot();
 	s->ctx = ctx;
 	size_t bytes = 0;
-	const std::vector<SnapPart> parts = snapshot_sections(ctx, nullptr, cap, 0, c.max_connections);
+	const std::vector<SnapPart> parts = snapshot_sections(ctx, nullptr, cap, c.max_connections);
 	for (size_t i = 0; i < kSnapFixed; ++i) { s->off.push_back(bytes); bytes += (parts[i].size * parts[i].count + 15) & ~(size_t)15; }
 	const cudaError_t e = cudaMalloc(&s->arena.p, bytes + 16);
 	if (e != cudaSuccess) { delete s; ctx->error = std::string("nb_snapshot_create: cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
@@ -165,13 +165,11 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // the copy reads the momentum and property rows
 	// grown: the only save that synchronises and allocates
-	GROW(s->rows, ctx->urow_n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
+	GROW(s->rows, ctx->urow_set.n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
 	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, ctx->jset.nrows, st);
-	s->jset = ctx->jset;
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
-	s->urow_n = ctx->urow_n; s->urow_levels = ctx->urow_levels;
-	s->urow_level_off = ctx->urow_level_off; s->urow_order = ctx->urow_order; s->urow_ab = ctx->urow_ab;
+	s->urow_set = ctx->urow_set; s->jset = ctx->jset;
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, true, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
@@ -188,7 +186,7 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	// tables the context has never had, or has too small: created or grown here (the only restore that synchronises and allocates)
 	if (s->shape.has_frc) { int r = ensure_force_tables(ctx); if (r) return r; }
 	if (!s->shape.kin.empty()) { int r = ensure_kind_table(ctx); if (r) return r; }
-	GROW(ctx->urows, s->urow_n, st);
+	GROW(ctx->urows, s->urow_set.n, st);
 	const void* joint_bufs[2] = { ctx->joints.p, ctx->jrows.p };
 	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, s->jset.nrows, st);
 	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
@@ -197,12 +195,10 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
 	StateShape shape = s->shape;
 	{ int r = install_state(ctx, shape, nullptr, st); if (r) return r; }
-	if (s->urow_n != ctx->urow_n || s->urow_level_off != ctx->urow_level_off) ++ctx->graph_epoch;   // the row levels are host values in the graph
-	ctx->urow_n = s->urow_n; ctx->urow_levels = s->urow_levels;
-	ctx->urow_level_off = s->urow_level_off; ctx->urow_order = s->urow_order; ctx->urow_ab = s->urow_ab;
-	// likewise the joint levels, and the joint buffers are its kernel arguments
+	// the row and joint levels are host values in the graph, the joint buffers its kernel arguments
+	if (s->urow_set.n != ctx->urow_set.n || s->urow_set.level_off != ctx->urow_set.level_off) ++ctx->graph_epoch;
 	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
-	ctx->jset = s->jset;
+	ctx->urow_set = s->urow_set; ctx->jset = s->jset;
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;
 	return NB_OK;

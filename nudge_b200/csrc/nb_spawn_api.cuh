@@ -172,8 +172,9 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	std::sort(list.begin(), list.end());   // for the binary searches of the remap
 	const u32 S = ctx->stride, B = ctx->B, nboxes = ctx->nboxes, K = ctx->nboxes + ctx->nspheres, nconn = ctx->nconn;
 	// the body map covers bodies below B: a row or connection naming a body beyond it (which their uploads allow) has no new index
-	for (u32 i = 0; i < ctx->urow_n; ++i)
-		if (ctx->urow_ab[i].a >= B || ctx->urow_ab[i].b >= B) { ctx->error = "constraint row " + std::to_string(i) + " names a body at or beyond the body count (" + std::to_string(B) + ")"; return NB_ERR_ARGUMENT; }
+	const RowLevels& us = ctx->urow_set;
+	for (u32 i = 0; i < us.n; ++i)
+		if (us.ab[i].a >= B || us.ab[i].b >= B) { ctx->error = "constraint row " + std::to_string(i) + " names a body at or beyond the body count (" + std::to_string(B) + ")"; return NB_ERR_ARGUMENT; }
 	for (u32 i = 0; i < nconn; ++i)
 		if (ctx->conn_host[i].a >= B || ctx->conn_host[i].b >= B) { ctx->error = "connection " + std::to_string(i) + " names a body at or beyond the body count (" + std::to_string(B) + ")"; return NB_ERR_ARGUMENT; }
 	if (nconn > S) { ctx->error = "more connections than the context's scratch stride (" + std::to_string(S) + ")"; return NB_ERR_CAPACITY; }
@@ -184,11 +185,13 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	for (u32 b : ctx->kin_list) if (!removed(b)) kin.push_back(remap(b));
 	std::vector<nb_body_pair> ab;
 	std::vector<u32> src;   // old device position of each kept row, in upload order
-	for (u32 i = 0; i < ctx->urow_n; ++i) {
-		const nb_body_pair p = ctx->urow_ab[i];
+	for (u32 i = 0; i < us.n; ++i) {
+		const nb_body_pair p = us.ab[i];
 		if (removed(p.a) || removed(p.b)) continue;
-		ab.push_back({ remap(p.a), remap(p.b) }); src.push_back(ctx->urow_order[i]);
+		ab.push_back({ remap(p.a), remap(p.b) }); src.push_back(us.order[i]);
 	}
+	RowLevels kept;   // fewer rows on the same bodies: no more levels than the set had
+	if (int r = level_rows(ctx, std::move(ab), kept, "constraint rows")) return r;
 	std::vector<nb_body_pair> conn;   // the host copy of the kept connections
 	for (u32 i = 0; i < nconn; ++i) {
 		const nb_body_pair p = ctx->conn_host[i];
@@ -208,13 +211,11 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		j.a = remap(j.a); j.b = remap(j.b);
 		joints.push_back(j);
 	}
-	std::vector<u32> level_off, order;
-	const u32 levels = level_rows(ab, level_off, order);
-	const u32 nrows = (u32)ab.size();
-	const bool rows_changed = nrows != ctx->urow_n;   // a deleted row can change the levels, which nb_step's graph holds
+	const u32 nrows = kept.n;
+	const bool rows_changed = nrows != us.n;   // a deleted row can change the levels, which nb_step's graph holds
 	std::vector<u32> staging(list);   // the list, then the rows' gather permutation (new device position -> old one)
 	staging.resize((size_t)n + nrows);
-	for (u32 j = 0; j < nrows; ++j) staging[n + order[j]] = src[j];
+	for (u32 j = 0; j < nrows; ++j) staging[n + kept.order[j]] = src[j];
 
 	JOIN_UPLOADS();   // the gathers read the momentum and property rows
 	GROW(ctx->spawn_idx, std::max(staging.size(), joint_wake.size()), st);
@@ -246,7 +247,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		nb_scan_reduce<2>(L, flags + S, S, nullptr, K, ctx->block_sums, counts + CNT_SPAWN_BOXES);
 		launch_grid(L, k_spawn_colliders, NB_SCAN_GRID, nboxes, K, flags + S, S, ctx->block_sums, map, ctx->box_tags, ctx->box_data, ctx->box_xf,
 			ctx->sph_tags, ctx->sph_data, ctx->sph_xf, ctx->has_filter ? ctx->filter : nullptr, ctx->has_sensor ? ctx->sensor : nullptr,
-			ctx->col_tag, ctx->aabb_min, reinterpret_cast<float*>(ctx->col_body), ctx->world_xf, ctx->order, reinterpret_cast<uint8_t*>(ctx->rank), counts);
+			ctx->front.col_tag, ctx->front.aabb_min, reinterpret_cast<float*>(ctx->front.col_body), ctx->front.world_xf, ctx->front.order, reinterpret_cast<uint8_t*>(ctx->front.rank), counts);
 	}
 	if (nconn) {
 		nb_scan_reduce<1>(L, flags + 3 * (size_t)S, S, nullptr, nconn, ctx->block_sums, counts + CNT_SPAWN_CONN);
@@ -267,11 +268,11 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	CK(cudaMemsetAsync(ctx->jd, 0, sizeof(nb_body_momentum) * (size_t)B2, st));
 	if (ctx->kind) { CK(d2d(ctx->kind, ctx->active, B2)); CK(cudaMemsetAsync(ctx->kind + B2, 0, B - B2, st)); }   // bodies added later are dynamic
 	if (ctx->has_frc) CK(d2d(ctx->frc, ctx->frc_spare, sizeof(nb_body_force) * (size_t)B2));
-	CK(d2d(ctx->box_tags, ctx->col_tag, 4 * (size_t)nb2)); CK(d2d(ctx->sph_tags, ctx->col_tag + nb2, 4 * (size_t)ns2));
-	CK(d2d(ctx->box_xf, ctx->world_xf, sizeof(nb_transform) * (size_t)nb2)); CK(d2d(ctx->sph_xf, ctx->world_xf + nb2, sizeof(nb_transform) * (size_t)ns2));
-	CK(d2d(ctx->box_data, ctx->aabb_min, sizeof(nb_box_collider) * (size_t)nb2)); CK(d2d(ctx->sph_data, ctx->col_body, sizeof(nb_sphere_collider) * (size_t)ns2));
-	if (ctx->has_filter) CK(d2d(ctx->filter, ctx->order, 4 * ((size_t)nb2 + ns2)));
-	if (ctx->has_sensor) CK(d2d(ctx->sensor, ctx->rank, (size_t)nb2 + ns2));
+	CK(d2d(ctx->box_tags, ctx->front.col_tag, 4 * (size_t)nb2)); CK(d2d(ctx->sph_tags, ctx->front.col_tag + nb2, 4 * (size_t)ns2));
+	CK(d2d(ctx->box_xf, ctx->front.world_xf, sizeof(nb_transform) * (size_t)nb2)); CK(d2d(ctx->sph_xf, ctx->front.world_xf + nb2, sizeof(nb_transform) * (size_t)ns2));
+	CK(d2d(ctx->box_data, ctx->front.aabb_min, sizeof(nb_box_collider) * (size_t)nb2)); CK(d2d(ctx->sph_data, ctx->front.col_body, sizeof(nb_sphere_collider) * (size_t)ns2));
+	if (ctx->has_filter) CK(d2d(ctx->filter, ctx->front.order, 4 * ((size_t)nb2 + ns2)));
+	if (ctx->has_sensor) CK(d2d(ctx->sensor, ctx->front.rank, (size_t)nb2 + ns2));
 	CK(d2d(ctx->conn, ctx->conn_scratch, sizeof(nb_body_pair) * (size_t)nc2));
 	CK(d2d(ctx->urows.p, ctx->urows_spare.p, sizeof(nb_constraint_row) * (size_t)nrows));
 	ctx->B = B2; ctx->nboxes = nb2; ctx->nspheres = ns2; ctx->nconn = nc2;
@@ -282,9 +283,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		if (kin.empty()) drop_kinematic(ctx);
 		else ctx->kin_list.swap(kin);
 	}
-	ctx->urow_n = nrows; ctx->urow_levels = nrows ? levels : 0;
-	ctx->urow_ab.swap(ab); ctx->urow_order.swap(order); ctx->urow_level_off.swap(level_off);
-	if (!nrows) ctx->urow_level_off.clear();
+	ctx->urow_set = std::move(kept);
 	ctx->scene_edited = true;
 	// nb_step's graph keys on B, the collider and connection counts, tagbits and kbits, so it re-records when they change; table contents
 	// are read through unchanged pointers.  The row levels are host values inside the graph.
@@ -346,8 +345,8 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 	// collide-stage scratch (the two ranges may overlap)
 	if (ctx->has_filter && nb + ns) {
 		if (nb && os) {
-			CK(cudaMemcpyAsync(ctx->order, ctx->filter + ob, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
-			CK(cudaMemcpyAsync(ctx->filter + ob + nb, ctx->order, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
+			CK(cudaMemcpyAsync(ctx->front.order, ctx->filter + ob, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
+			CK(cudaMemcpyAsync(ctx->filter + ob + nb, ctx->front.order, 4 * (size_t)os, cudaMemcpyDeviceToDevice, st));
 		}
 		CK(put_staged(ctx, ctx->filter + ob, f, 4 * (size_t)nb, st));
 		CK(put_staged(ctx, ctx->filter + ob + nb + os, f + nb, 4 * (size_t)ns, st));
@@ -355,8 +354,8 @@ int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider
 	if (ctx->has_sensor && nb + ns) {
 		uint8_t* s = ctx->sensor;
 		if (nb && os) {
-			CK(cudaMemcpyAsync(ctx->rank, s + ob, os, cudaMemcpyDeviceToDevice, st));
-			CK(cudaMemcpyAsync(s + ob + nb, ctx->rank, os, cudaMemcpyDeviceToDevice, st));
+			CK(cudaMemcpyAsync(ctx->front.rank, s + ob, os, cudaMemcpyDeviceToDevice, st));
+			CK(cudaMemcpyAsync(s + ob + nb, ctx->front.rank, os, cudaMemcpyDeviceToDevice, st));
 		}
 		std::vector<uint8_t> flags01(nb + ns);
 		for (u32 i = 0; i < nb + ns; ++i) flags01[i] = sf[i] ? 1 : 0;
