@@ -126,7 +126,8 @@ int nb_unpack_momentum(nb_context*, const uint32_t* dev_indices, const uint32_t*
  * (NB_SHARD_PEER: neighbour-only traffic over NVLink, no collective).  Both give bit-identical ghost rows.
  *   rank 0: nb_shard_unique_id -> broadcast the 128 bytes -> every rank: nb_shard_create;  every rank: nb_shard_ipc_handle -> all-gather
  *   the 64-byte handles -> nb_shard_open_peer for every other rank;  after every (re)partition: nb_shard_plan;  then nb_shard_step per
- *   sub-step (or nb_shard_exchange between the stage calls).  nb_shard_partition is the (host, deterministic) partition rule. */
+ *   sub-step (or nb_shard_exchange between the stage calls).  nb_shard_partition is the (host, deterministic) partition rule.
+ * The shard's device memory is its own: nb_shard_destroy frees it.  A failed nb_shard_create sets *out to null and leaves the context as it was. */
 typedef struct nb_shard nb_shard;
 enum nb_shard_transport { NB_SHARD_NCCL = 0, NB_SHARD_PEER = 1 };
 int nb_shard_unique_id(void* nccl_id_out /* 128 bytes */);

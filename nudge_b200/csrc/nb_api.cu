@@ -1,7 +1,8 @@
 // nudge_b200 — host side of the C ABI (include/nudge_b200.h): context, HBM arena, kernel sequencing.
 // The reference keeps all memory caller-owned and bump-allocates scratch from an Arena (nudge.cpp:990-1055);
-// here the context plays both roles for device memory: every buffer is carved once from cudaMalloc at
-// nb_create and reused every step, nothing is allocated or synchronised inside the step.
+// here the context plays both roles for device memory: the step's buffers are allocated at nb_create and reused every step, nothing is
+// allocated or synchronised inside the step; a feature allocates its tables on its first call.  Every buffer is a DevBuf held by its
+// owner (the context, a shard or a snapshot), which frees it and counts its bytes.
 #include "nb_shard.cuh"
 #include "nb_events.cuh"
 #include <stdio.h>
@@ -10,6 +11,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <memory>
 #include <math.h>
 #include <nvtx3/nvToolsExt.h>
 
@@ -21,12 +23,14 @@ extern "C" int nb_host_check_lut_model(const u32* rcp_lut, const u32* rsqrt_lut)
 struct StepKey { cudaStream_t stream; float ts, gravity, damping; u32 iterations, B, nboxes, nspheres, nconn, tagbits, kbits; int debug, solver_mode, transport; unsigned long long plan_version, graph_epoch; };
 struct StepGraph { cudaGraphExec_t exec; StepKey key; unsigned long long launches; int enabled; };
 
-// A device buffer of `cap` elements, freed with its owner (the context or a snapshot); the editing calls grow theirs on demand (grow, below).
-// Move-only: the move swaps, so the buffer it replaces is freed with the temporary.
+// A device buffer of `cap` elements, freed with its owner, its bytes charged to `charged` (the context's device_bytes) while it holds
+// them.  Move-only: the move swaps, so the buffer it replaces is freed and uncharged with the temporary.
 template<class T> struct DevBuf {
-	T* p = nullptr; size_t cap = 0;
-	DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
-	~DevBuf() { if (p) cudaFree(p); }
+	T* p = nullptr; size_t cap = 0; unsigned long long* charged = nullptr;
+	DevBuf() = default; DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+	DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); std::swap(charged, o.charged); return *this; }
+	~DevBuf() { if (p) { cudaFree(p); *charged -= cap * sizeof(T); } }
+	int alloc(nb_context* ctx, size_t n);   // below nb_context
 };
 
 // Entries levelled by body (level_rows, nb_rows_api.cuh), the user rows or the joints: each one's (a, b) in upload order and device position
@@ -54,9 +58,9 @@ struct nb_context {
 	std::string error;
 	unsigned long long launches;
 	int lut_exact;
-	std::vector<void*> allocs;
-	// device bytes held by the context and its snapshots (dev_alloc, grow, nb_snapshot_create / nb_snapshot_destroy; nb_debug_read)
-	unsigned long long device_bytes;
+	// device_bytes: what the DevBufs charged to it hold, the context's, its shard's and its snapshots' (nb_debug_read); declared before
+	// every buffer, which uncharges it when destroyed.  allocs: the context's buffers of alloc_zeroed.
+	unsigned long long device_bytes; std::vector<DevBuf<unsigned char>> allocs;
 	// the editing calls' shared host side: the staging copy of a caller's array (put_staged) and the duplicate check's byte per body, all
 	// zeros between calls (bodies_distinct)
 	std::vector<unsigned char> host_stage; std::vector<uint8_t> body_seen;
@@ -146,24 +150,35 @@ struct nb_context {
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { ctx->error = std::string(#call) + ": " + cudaGetErrorString(e_); return NB_ERR_CUDA; } } while (0)
 
+// Frees the buffer, then allocates n elements charged to the context's device_bytes.  On failure the buffer is empty, and the error, which
+// does not stick, is cleared, so that no later cudaGetLastError check reports it again.
+template<class T> int DevBuf<T>::alloc(nb_context* ctx, size_t n) {
+	*this = DevBuf();
+	const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+	if (e != cudaSuccess) { p = nullptr; cudaGetLastError(); ctx->error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
+	cap = n; charged = &ctx->device_bytes; *charged += n * sizeof(T);
+	return NB_OK;
+}
+
+// The allocator of the buffers kept for their owner's lifetime: unless `p` exists already, n elements (at least one), zero-filled, held
+// by `list`, the owner's (the context's allocs or a shard's).  A routine that allocates several can run again and allocate the rest.
 template<class T>
-static int dev_alloc(nb_context* ctx, T** p, size_t n) {
-	void* q = nullptr;
-	size_t bytes = (n ? n : 1) * sizeof(T);
-	cudaError_t e = cudaMalloc(&q, bytes);
-	if (e != cudaSuccess) { ctx->error = std::string("cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
-	ctx->allocs.push_back(q);
-	ctx->device_bytes += bytes;
+static int alloc_zeroed(nb_context* ctx, std::vector<DevBuf<unsigned char>>& list, T*& p, size_t n) {
+	if (p) return NB_OK;
+	DevBuf<unsigned char> b;
+	if (int r = b.alloc(ctx, (n ? n : 1) * sizeof(T))) return r;
 	// Zeroed before the first use, which may come on a non-blocking stream that the legacy stream does not order against: a buffer
 	// allocated on first use (the body-force table, the kinematic table, ...) would otherwise be cleared AFTER the kernels that fill it
 	// when the legacy stream still holds other work (another context's step).
-	e = cudaMemsetAsync(q, 0, bytes, cudaStreamLegacy);
+	cudaError_t e = cudaMemsetAsync(b.p, 0, b.cap, cudaStreamLegacy);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamLegacy);
 	if (e != cudaSuccess) { ctx->error = std::string("cudaMemset: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
-	*p = (T*)q;
-	return 0;
+	p = reinterpret_cast<T*>(b.p);
+	list.push_back(std::move(b));
+	return NB_OK;
 }
-#define ALLOC(p, n) do { int r_ = dev_alloc(ctx, &(p), (size_t)(n)); if (r_) return r_; } while (0)
+#define ALLOC_IN(list, p, n) do { int r_ = alloc_zeroed(ctx, list, p, (size_t)(n)); if (r_) return r_; } while (0)
+#define ALLOC(p, n) ALLOC_IN(ctx->allocs, p, n)
 
 // Makes `b` hold at least n elements.  A larger buffer replaces the old one once `st` has drained, since earlier work on it may still read
 // the old one; the contents are neither kept nor cleared.  On failure the buffer is empty.
@@ -171,12 +186,7 @@ template<class T>
 static int grow(nb_context* ctx, DevBuf<T>& b, size_t n, cudaStream_t st) {
 	if (n <= b.cap) return NB_OK;
 	CK(cudaStreamSynchronize(st));
-	ctx->device_bytes -= b.cap * sizeof(T);
-	b = DevBuf<T>();
-	CK(cudaMalloc(&b.p, n * sizeof(T)));
-	b.cap = n;
-	ctx->device_bytes += n * sizeof(T);
-	return NB_OK;
+	return b.alloc(ctx, n);
 }
 #define GROW(b, n, st) do { int r_ = grow(ctx, b, (size_t)(n), st); if (r_) return r_; } while (0)
 
@@ -214,17 +224,13 @@ __global__ void k_reset_collide(u32* counts, u32 K, u64* keybits) {
 	}
 }
 
-// dev_alloc of a buffer that does not exist yet: a routine that allocates several can run again after a failure and allocates the rest.
-template<class T> static int alloc_once(nb_context* ctx, T*& p, size_t n) { return p ? NB_OK : dev_alloc(ctx, &p, n); }
-
 // The buffers of `f` for K colliders of capacity.
 static int alloc_front_end(nb_context* ctx, FrontEnd& f, u32 K) {
 	u32 tsz = 1024; while (tsz < 2 * K) tsz *= 2;
 	f.table_mask = tsz - 1;
-	if (alloc_once(ctx, f.keybits, 2) || alloc_once(ctx, f.world_xf, K) || alloc_once(ctx, f.aabb_min, K) || alloc_once(ctx, f.aabb_max, K) ||
-		alloc_once(ctx, f.col_tag, K) || alloc_once(ctx, f.col_body, K) || alloc_once(ctx, f.order, K) || alloc_once(ctx, f.rank, K) ||
-		alloc_once(ctx, f.leaf_min, K) || alloc_once(ctx, f.leaf_max, K) || alloc_once(ctx, f.mkeys, K) || alloc_once(ctx, f.smallf, K) ||
-		alloc_once(ctx, f.large_list, K) || alloc_once(ctx, f.table_keys, tsz) || alloc_once(ctx, f.table_vals, tsz)) return NB_ERR_CUDA;
+	ALLOC(f.keybits, 2); ALLOC(f.world_xf, K); ALLOC(f.aabb_min, K); ALLOC(f.aabb_max, K); ALLOC(f.col_tag, K); ALLOC(f.col_body, K);
+	ALLOC(f.order, K); ALLOC(f.rank, K); ALLOC(f.leaf_min, K); ALLOC(f.leaf_max, K); ALLOC(f.mkeys, K); ALLOC(f.smallf, K);
+	ALLOC(f.large_list, K); ALLOC(f.table_keys, tsz); ALLOC(f.table_vals, tsz);
 	return NB_OK;
 }
 
@@ -282,8 +288,6 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
 static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->graph_epoch; } }
 static void drop_body_forces(nb_context* ctx) { if (ctx->has_frc) { ctx->has_frc = false; ++ctx->graph_epoch; } }   // the step launches k_gravity_damping again
-// The kind table, allocated for max_bodies on first use.
-static int ensure_kind_table(nb_context* ctx) { if (!ctx->kind) ALLOC(ctx->kind, ctx->cfg.max_bodies); return NB_OK; }
 
 // The checks of entry i of a body list (kinematic bodies, impulses, forces, removals): not body 0, the static world; below the body count;
 // and, unless kinematic_ok, not kinematic.  A refused entry is NB_ERR_ARGUMENT with the message "<list> <i>: body <b> ...".
@@ -570,9 +574,8 @@ void nb_destroy(nb_context* ctx) {
 	if (ctx->graph.exec) cudaGraphExecDestroy(ctx->graph.exec);
 	if (ctx->tev_made) for (int i = 0; i < 64; ++i) { cudaEventDestroy(ctx->tev[0][i]); cudaEventDestroy(ctx->tev[1][i]); }
 	if (ctx->copy_stream) { cudaStreamDestroy(ctx->copy_stream); cudaEventDestroy(ctx->ev_up_begin); cudaEventDestroy(ctx->ev_up_done); }
-	for (size_t i = 0; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
 	free_snapshots(ctx);
-	delete ctx;   // and with it the grown buffers
+	delete ctx;   // and with it its buffers
 }
 
 const char* nb_last_error(const nb_context* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
@@ -662,7 +665,7 @@ int nb_upload_kinematic_bodies(nb_context* ctx, const nb_kinematic_body* h, uint
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
 	if (!n) { drop_kinematic(ctx); return NB_OK; }
-	{ int r = ensure_kind_table(ctx); if (r) return r; }
+	ALLOC(ctx->kind, ctx->cfg.max_bodies);   // the kind table, on first use
 	GROW(ctx->kin_rows, n, st);
 	const bool same = ctx->has_kin && list == ctx->kin_list;
 	if (!same) CK(cudaMemsetAsync(ctx->kind, 0, ctx->cfg.max_bodies, st));
@@ -1225,7 +1228,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 
 // Keeps a copy of the sorted broadphase pair list for nb_debug_read("pair_keys") (one extra copy kernel per collide).
 int nb_debug_enable(nb_context* ctx, int on) {
-	if (on && !ctx->pair_keys_debug) ALLOC(ctx->pair_keys_debug, ctx->cfg.max_pairs);
+	if (on) ALLOC(ctx->pair_keys_debug, ctx->cfg.max_pairs);
 	ctx->debug = on;
 	return NB_OK;
 }

@@ -47,12 +47,6 @@ __global__ void __launch_bounds__(NB_BLOCK) k_body_force_scatter(const nb_body_f
 	}
 }
 
-// The table and its gather buffer, allocated for max_bodies on first use.
-static int ensure_force_tables(nb_context* ctx) {
-	if (!ctx->frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
-	return NB_OK;
-}
-
 // Stored rows are canonical: the staged rows' reserved words are cleared before their copy.
 static void clear_reserved(unsigned char* rows, size_t bytes) {
 	for (size_t i = 0; i < bytes / sizeof(nb_body_force); ++i) reinterpret_cast<nb_body_force*>(rows)[i].reserved = 0;
@@ -61,7 +55,7 @@ static void clear_reserved(unsigned char* rows, size_t bytes) {
 // Creates the table (every body 0 .. B-1 with the default entry) unless it exists.
 static int ensure_body_forces(nb_context* ctx, cudaStream_t st) {
 	if (ctx->has_frc) return NB_OK;
-	{ int r = ensure_force_tables(ctx); if (r) return r; }
+	ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies);   // the table and its gather buffer, on first use
 	if (ctx->B) launch_grid(mk_launch(ctx, st), k_body_force_defaults, GRID(ctx->B), ctx->frc, ctx->B);
 	CK(cudaGetLastError());
 	ctx->has_frc = true;

@@ -80,9 +80,7 @@ int nb_apply_body_impulses(nb_context* ctx, const nb_body_impulse* h, uint32_t n
 	for (u32 i = 0; i < n; ++i) if (int r = check_body(ctx, "body impulse", i, h[i].body, false)) return r;   // a body may be listed again
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // ordered like nb_upload_momentum, after a pending nb_upload_bodies side copy
-	if (!ctx->imp_n) {
-		ALLOC(ctx->imp_n, 1); ALLOC(ctx->imp_sb.hist, 256 * (size_t)ctx->sms); ALLOC(ctx->imp_sb.bar, 2);
-	}
+	ALLOC(ctx->imp_n, 1); ALLOC(ctx->imp_sb.hist, 256 * (size_t)ctx->sms); ALLOC(ctx->imp_sb.bar, 2);
 	GROW(ctx->imp_rows, n, st);
 	for (int i = 0; i < 2; ++i) { GROW(ctx->imp_keys[i], n, st); ctx->imp_sb.keys[i] = ctx->imp_keys[i].p; }
 	CK(put_staged(ctx, ctx->imp_rows.p, h, sizeof(nb_body_impulse) * (size_t)n, st));

@@ -206,9 +206,10 @@ static int ensure_ray_scratch(nb_context* ctx) {
 	RayScratch& r = ctx->ray;
 	const u32 K = ctx->cfg.max_boxes + ctx->cfg.max_spheres;
 	if (r.ready) return NB_OK;
-	if (alloc_front_end(ctx, r.front, K) || alloc_once(ctx, r.sb.keys[0], K) || alloc_once(ctx, r.sb.keys[1], K) || alloc_once(ctx, r.sb.vals[0], K) ||
-		alloc_once(ctx, r.sb.vals[1], K) || alloc_once(ctx, r.sb.hist, 256 * (size_t)ctx->sms) || alloc_once(ctx, r.counts, CNT__COUNT)) return NB_ERR_CUDA;
-	r.sb.bar = r.counts + CNT_BAR0;   // zeroed by dev_alloc: the sort's grid barrier starts from zero arrivals
+	{ int e = alloc_front_end(ctx, r.front, K); if (e) return e; }
+	for (int i = 0; i < 2; ++i) { ALLOC(r.sb.keys[i], K); ALLOC(r.sb.vals[i], K); }
+	ALLOC(r.sb.hist, 256 * (size_t)ctx->sms); ALLOC(r.counts, CNT__COUNT);
+	r.sb.bar = r.counts + CNT_BAR0;   // zeroed by alloc_zeroed: the sort's grid barrier starts from zero arrivals
 	r.ready = true;   // only once every buffer exists: a failed allocation leaves the next call to try again
 	return NB_OK;
 }

@@ -63,7 +63,7 @@ int nb_instance_matrices(nb_context* ctx, float* out, uint32_t capacity, int out
 	if (!K) return NB_OK;
 	float4* dst = reinterpret_cast<float4*>(out);
 	if (!out_is_device) {
-		if (!ctx->instances) ALLOC(ctx->instances, 4 * ((size_t)ctx->cfg.max_boxes + ctx->cfg.max_spheres));
+		ALLOC(ctx->instances, 4 * ((size_t)ctx->cfg.max_boxes + ctx->cfg.max_spheres));
 		dst = ctx->instances;
 	}
 	launch_grid(mk_launch(ctx, st), k_instance_matrices, GRID(K), ctx->nboxes, ctx->nspheres, ctx->xf, ctx->box_xf, ctx->box_data, ctx->sph_xf, ctx->sph_data, dst);

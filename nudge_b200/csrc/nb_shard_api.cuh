@@ -20,6 +20,7 @@ struct nb_shard {
 	StepGraph graph;   // the sharded step as a CUDA graph
 	long long pull_timeout_cycles;
 	int no_exchange;   // nb_shard_debug_no_exchange: time the rank's local problem without the ghost hand-over (results are then not a simulation of the global scene)
+	std::vector<DevBuf<unsigned char>> allocs;   // the buffers above, charged to the context's device_bytes and freed with the shard
 };
 
 #define SCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { sh->ctx->error = std::string(#call) + ": " + cudaGetErrorString(e_); return NB_ERR_CUDA; } } while (0)
@@ -37,29 +38,27 @@ int nb_shard_unique_id(void* id_out) {
 }
 
 // ghost_capacity / export_capacity: upper bounds for the plans this shard will see (every rank must pass the same ghost_capacity).
-// nccl_id: the 128 bytes rank 0 obtained from nb_shard_unique_id, or null to run without NCCL (peer transport only).
+// nccl_id: the 128 bytes rank 0 obtained from nb_shard_unique_id, or null to run without NCCL (peer transport only).  A failure leaves no shard.
 int nb_shard_create(nb_context* ctx, uint32_t rank, uint32_t world, const void* nccl_id, uint32_t ghost_capacity, uint32_t export_capacity, nb_shard** out) {
 	if (!ctx || !out || !world || rank >= world || world > NB_SHARD_FLAG_WORDS || !ghost_capacity || !export_capacity) { if (ctx) ctx->error = "bad shard configuration"; return NB_ERR_ARGUMENT; }
-	nb_shard* sh = new nb_shard();
-	*out = sh;
+	*out = nullptr;
+	std::unique_ptr<nb_shard> sh(new nb_shard());   // deleted, with its buffers, by every return but the last
 	sh->ctx = ctx; sh->rank = rank; sh->world = world; sh->ghost_cap = ghost_capacity;
-	ctx->sharded = true;   // nb_add_bodies / nb_remove_bodies refuse a rank's context
 	sh->cap_export = export_capacity; sh->cap_ghost = ghost_capacity; sh->cap_sub = 4 * export_capacity + 64;
 	CK(cudaSetDevice(ctx->cfg.device));
 	sh->passes_cap = 24;
 	sh->inbox2_offset = NB_SHARD_FLAG_WORDS * 4 + sizeof(float4) * 2 * 2 * (size_t)ghost_capacity;
 	size_t inbox_bytes = sh->inbox2_offset + sizeof(float4) * 2 * 2 * (size_t)sh->passes_cap * ghost_capacity;
-	ALLOC(sh->inbox, inbox_bytes);
-	ALLOC(sh->peer_inbox2_dev, world); ALLOC(sh->d_export_row, ctx->cfg.max_bodies); ALLOC(sh->d_ghost_slot, ctx->cfg.max_bodies);
+	ALLOC_IN(sh->allocs, sh->inbox, inbox_bytes);
+	ALLOC_IN(sh->allocs, sh->peer_inbox2_dev, world); ALLOC_IN(sh->allocs, sh->d_export_row, ctx->cfg.max_bodies); ALLOC_IN(sh->allocs, sh->d_ghost_slot, ctx->cfg.max_bodies);
 	{
 		int per_sm = 0;
 		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_flow, NB_BLOCK, 0));
 		sh->flow_blocks = per_sm > 0 ? ctx->sms * per_sm : 0;
 	}
-	ALLOC(sh->peers_dev, world); ALLOC(sh->epoch, 1); ALLOC(sh->done, 1);
-	ALLOC(sh->d_export_local, sh->cap_export); ALLOC(sh->d_sub_off, (size_t)sh->cap_export + 1); ALLOC(sh->d_sub_tgt, sh->cap_sub);
-	ALLOC(sh->d_ghost_local, sh->cap_ghost); ALLOC(sh->d_ghost_src, sh->cap_ghost);
-	ALLOC(sh->d_export, 2 * (size_t)export_capacity); ALLOC(sh->d_gather, 2 * (size_t)export_capacity * world);
+	ALLOC_IN(sh->allocs, sh->peers_dev, world); ALLOC_IN(sh->allocs, sh->epoch, 1); ALLOC_IN(sh->allocs, sh->done, 1); ALLOC_IN(sh->allocs, sh->d_export_local, sh->cap_export);
+	ALLOC_IN(sh->allocs, sh->d_sub_off, (size_t)sh->cap_export + 1); ALLOC_IN(sh->allocs, sh->d_sub_tgt, sh->cap_sub); ALLOC_IN(sh->allocs, sh->d_ghost_local, sh->cap_ghost);
+	ALLOC_IN(sh->allocs, sh->d_ghost_src, sh->cap_ghost); ALLOC_IN(sh->allocs, sh->d_export, 2 * (size_t)export_capacity); ALLOC_IN(sh->allocs, sh->d_gather, 2 * (size_t)export_capacity * world);
 	sh->peers.assign(world, nullptr); sh->peers[rank] = sh->inbox;
 	sh->graph.enabled = ctx->graph.enabled;
 	int khz = 0; cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, ctx->cfg.device);
@@ -70,9 +69,11 @@ int nb_shard_create(nb_context* ctx, uint32_t rank, uint32_t world, const void* 
 		if (!api) { ctx->error = err; return NB_ERR_CUDA; }
 		ncclUniqueId id; memcpy(&id, nccl_id, sizeof(id));
 		ncclResult_t r = api->CommInitRank(&sh->comm, (int)world, id, (int)rank);
-		if (r != ncclSuccess) { ctx->error = std::string("ncclCommInitRank: ") + api->GetErrorString(r); delete sh; *out = nullptr; return NB_ERR_CUDA; }
+		if (r != ncclSuccess) { ctx->error = std::string("ncclCommInitRank: ") + api->GetErrorString(r); return NB_ERR_CUDA; }
 		sh->has_nccl = true;
 	}
+	ctx->sharded = true;   // nb_add_bodies / nb_remove_bodies refuse a rank's context
+	*out = sh.release();
 	return NB_OK;
 }
 
@@ -82,7 +83,7 @@ void nb_shard_destroy(nb_shard* sh) {
 	if (sh->graph.exec) cudaGraphExecDestroy(sh->graph.exec);
 	for (void* p : sh->opened) cudaIpcCloseMemHandle(p);
 	if (sh->has_nccl) { NcclApi* api = nccl_api(nullptr); if (api) api->CommDestroy(sh->comm); }
-	delete sh;   // device buffers belong to the nb_context's allocation list
+	delete sh;   // and with it its buffers, now that nothing in flight uses them
 }
 
 // CUDA IPC handle (64 bytes) of this rank's inbox; the ranks swap them out of band and call nb_shard_open_peer for every other rank.

@@ -140,10 +140,7 @@ int nb_snapshot_create(nb_context* ctx, nb_snapshot** out) {
 	size_t bytes = 0;
 	const std::vector<SnapPart> parts = snapshot_sections(ctx, nullptr, cap, c.max_connections);
 	for (size_t i = 0; i < kSnapFixed; ++i) { s->off.push_back(bytes); bytes += (parts[i].size * parts[i].count + 15) & ~(size_t)15; }
-	const cudaError_t e = cudaMalloc(&s->arena.p, bytes + 16);
-	if (e != cudaSuccess) { delete s; ctx->error = std::string("nb_snapshot_create: cudaMalloc: ") + cudaGetErrorString(e); return NB_ERR_CUDA; }
-	s->arena.cap = bytes + 16;
-	ctx->device_bytes += s->arena.cap;
+	if (int r = s->arena.alloc(ctx, bytes + 16)) { delete s; ctx->error = "nb_snapshot_create: " + ctx->error; return r; }
 	s->words = reinterpret_cast<u32*>(s->arena.p + bytes);
 	ctx->snapshots.push_back(s);
 	*out = s;
@@ -154,7 +151,6 @@ void nb_snapshot_destroy(nb_snapshot* s) {
 	if (!s) return;
 	nb_context* ctx = s->ctx;
 	ctx->snapshots.erase(std::remove(ctx->snapshots.begin(), ctx->snapshots.end(), s), ctx->snapshots.end());
-	ctx->device_bytes -= s->arena.cap + sizeof(nb_constraint_row) * (s->rows.cap + s->jrows.cap) + sizeof(uint4) * s->overlaps.cap + sizeof(nb_joint) * s->joints.cap;
 	delete s;   // cudaFree waits for the work that may still read it
 }
 
@@ -184,8 +180,8 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	cudaStream_t st = (cudaStream_t)stream;
 	JOIN_UPLOADS();   // a pending side copy must not land on the restored rows
 	// tables the context has never had, or has too small: created or grown here (the only restore that synchronises and allocates)
-	if (s->shape.has_frc) { int r = ensure_force_tables(ctx); if (r) return r; }
-	if (!s->shape.kin.empty()) { int r = ensure_kind_table(ctx); if (r) return r; }
+	if (s->shape.has_frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
+	if (!s->shape.kin.empty()) ALLOC(ctx->kind, ctx->cfg.max_bodies);
 	GROW(ctx->urows, s->urow_set.n, st);
 	const void* joint_bufs[2] = { ctx->joints.p, ctx->jrows.p };
 	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, s->jset.nrows, st);
