@@ -104,6 +104,9 @@ int nb_upload_bodies(nb_context*, const nb_body_data* host, void* stream);
 int nb_upload_colliders(nb_context*, const nb_collider_data* host, void* stream);
 int nb_upload_connections(nb_context*, const nb_body_connections* host, void* stream);
 int nb_upload_cache(nb_context*, const nb_contact_cache* host, void* stream);
+/* nb_upload_contacts replaces the contact set of the last nb_collide (custom contacts, e.g. against the static environment).  Their tags may be
+ * any uint32 A and B, including tags no collider carries, and their feature words any uint32: nb_read_cached_impulses orders them by
+ * (B, A, feature) over the full width of the largest uploaded tag. */
 int nb_upload_contacts(nb_context*, const nb_contact_data* host /* may be null */, const nb_active_bodies* host_active /* may be null */, void* stream); /* synchronises */
 int nb_download_bodies(nb_context*, nb_body_data* host, void* stream);
 int nb_download_contacts(nb_context*, nb_contact_data* host, nb_active_bodies* host_active, void* stream); /* synchronises */
@@ -303,7 +306,8 @@ int nb_upload_collision_filters(nb_context*, const nb_collision_filter* host, ui
  * the narrowphase would give it at least one contact (the same code and pair orientation as the contact pipeline), evaluated in every
  * nb_collide whether its bodies sleep or not.
  * Overlap list of the last nb_collide: one entry per overlapping pair, key tags = min(tag_i, tag_j) | (uint64)max(tag_i, tag_j) << 32 (the
- * collider tags, like the contact-event key), body_a = the body of the lower-tag collider, body_b = the other's; ascending by tags.
+ * collider tags, like the contact-event key), body_a = the body of the lower-tag collider, body_b = the other's (with equal tags, body_a is
+ * the lower of the two body indices); ascending by tags.
  * Events (with nb_enable_contact_events): nb_write_cached_impulses compares the overlap list of the step's nb_collide (cur) with the one as of
  * its previous call (old) and appends, after the contact ENDs and BEGINs, NB_SENSOR_END for every key in old and not in cur, then NB_SENSOR_BEGIN
  * for every key in cur and not in old, each in ascending key order.  A sensor event carries tags, kind, step, body_a and body_b; every other

@@ -75,6 +75,7 @@ struct nb_context {
 	u32* chain_start; u32* chain_len;  // per body: segment cursor (the segment's end once k_chain_scatter ran) / number of chain entries
 	float4* warm;   // two rows per chain entry: the warm start's share of the entry's side (k_build_rows -> k_warm_start)
 	bool contacts_internal;  // the current contact set came from nb_collide (not nb_upload_contacts)
+	u32 upload_tagbits;      // bits of the largest A or B among the contacts nb_upload_contacts put in place (any uint32, not only collider tags)
 	// throughput mode (nb_set_solver_mode): mass-splitting Jacobi, nb_jacobi.cuh
 	int solver_mode; u32* jcnt; float4* jd; int jacobi_blocks1, jacobi_blocks2;
 	// CUDA-event timing of the dominant solver kernel (nb_debug_timing): bench.py's roofline numerator is measured live
@@ -487,7 +488,7 @@ int nb_create(const nb_config* config, nb_context** out) {
 
 	const u32 B = c.max_bodies, P = c.max_pairs, C = c.max_contacts;
 	ctx->B = 0; ctx->nboxes = 0; ctx->nspheres = 0; ctx->nconn = 0;
-	ctx->tagbits = 1; ctx->kbits = bits_for(K ? K : 1); ctx->bodybits = bits_for(B);
+	ctx->tagbits = 1; ctx->upload_tagbits = 1; ctx->kbits = bits_for(K ? K : 1); ctx->bodybits = bits_for(B);
 	ctx->stride = ((std::max(std::max(P, C), std::max(B, K)) + 63) / 64) * 64;
 	ctx->cstride = ((C + 8 * 16 * NB_SCHED_MAXV + 31) / 32) * 32;  // slots = batch*8 + lane; leftover batches of the 16 buckets may be partly empty (a hub body beyond that: OVF_SCHED from k_batch_index)
 	ctx->slots_per_bucket = (C + 15) / 16 + 1;
@@ -749,6 +750,9 @@ int nb_upload_contacts(nb_context* ctx, const nb_contact_data* h, const nb_activ
 	if (h) {
 		if (h->count > ctx->cfg.max_contacts || h->sleeping_count > ctx->cfg.max_contacts) { ctx->error = "too many contacts"; return NB_ERR_CAPACITY; }
 		ctx->contacts_internal = false;
+		u32 maxtag = 1;
+		for (u32 i = 0; i < h->count; ++i) maxtag = std::max({ maxtag, (u32)h->tags[i], (u32)(h->tags[i] >> 32) });
+		ctx->upload_tagbits = bits_for((u64)maxtag + 1);
 		H2D(ctx->fin.data, h->data, h->count, nb_contact); H2D(ctx->fin.bodies, h->bodies, h->count, nb_body_pair);
 		H2D(ctx->fin.tags, h->tags, h->count, u64); H2D(ctx->fin.features, h->features, h->count, u32);
 		if (h->sleeping_count) H2D(ctx->sleeping, h->sleeping_pairs, h->sleeping_count, u64);
@@ -885,11 +889,12 @@ static int read_sort(nb_context* ctx, void* stream) {
 		launch_grid(L, k_tag_keys_packed, GRID(C), ctx->fin.tags, ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], ctx->tagbits, spread, counts);
 		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, (int)(2 * ctx->tagbits + 16 + spread), true, 0);
 	}
-	else {  // contacts supplied through nb_upload_contacts: arbitrary feature words
+	else {  // contacts supplied through nb_upload_contacts (arbitrary feature words, tags beyond the colliders'), or tags wider than 24 bits
+		const u32 pbits = ctx->contacts_internal ? ctx->tagbits : std::max(ctx->tagbits, ctx->upload_tagbits);
 		launch_grid(L, k_tag_keys_feature, GRID(C), ctx->fin.features, ctx->sb.keys[0], ctx->sb.vals[0], counts);
 		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, 32, true, 0);
-		launch_grid(L, k_tag_keys_pair, GRID(C), ctx->fin.tags, ctx->sb.vals[cur], ctx->sb.keys[cur], ctx->tagbits, counts);
-		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, (int)(2 * ctx->tagbits), true, cur);
+		launch_grid(L, k_tag_keys_pair, GRID(C), ctx->fin.tags, ctx->sb.vals[cur], ctx->sb.keys[cur], pbits, counts);
+		cur = nb_radix_sort(L, ctx->sb, counts + CNT_CONTACTS, 0, (int)(2 * pbits), true, cur);
 	}
 	launch_grid(L, k_copy_u32, GRID(C), ctx->sb.vals[cur], ctx->sorted, counts + CNT_CONTACTS);
 	CK(cudaGetLastError());
@@ -1210,6 +1215,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	if (!strcmp(name, "grid_level")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_GRID_LEVEL]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "grid_large")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_LARGE]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "kbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->kbits; if (bytes) *bytes = 4; return NB_OK; }
+	if (!strcmp(name, "tagbits")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->tagbits; if (bytes) *bytes = 4; return NB_OK; }
 	// the k_jacobi_sweep variant (shared-memory stages) and grid that throughput mode launches at the current body count
 	if (!strcmp(name, "jacobi_stages")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)jacobi_stages(ctx); if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "jacobi_blocks")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)(jacobi_stages(ctx) == 2 ? ctx->jacobi_blocks2 : ctx->jacobi_blocks1); if (bytes) *bytes = 4; return NB_OK; }

@@ -1155,7 +1155,8 @@ __global__ void __launch_bounds__(NB_BLOCK) k_sensor_gather(const u64* keys, con
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const u64 pk = sensor_keys[vals[i]], t = keys[i];
 		const u32 lo = (u32)(pk & mask), hi = (u32)(pk >> kbits);
-		const bool lo_first = col_tag[lo] == (u32)t;
-		out[i] = make_uint4((u32)t, (u32)(t >> 32), col_body[lo_first ? lo : hi], col_body[lo_first ? hi : lo]);
+		const u32 bl = col_body[lo], bh = col_body[hi];
+		const bool lo_first = col_tag[lo] != col_tag[hi] ? col_tag[lo] == (u32)t : bl < bh;   // equal tags: the lower body first
+		out[i] = make_uint4((u32)t, (u32)(t >> 32), lo_first ? bl : bh, lo_first ? bh : bl);
 	}
 }

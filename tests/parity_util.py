@@ -68,11 +68,14 @@ def rows_by_contact(view, n_contacts):
                 a=view["a"][first], b=view["b"][first])
 
 
-def ref_layout_stages(s, wide):
+def ref_layout_stages(s, wide, after_collide=None):
     """Runs one full step of `s` (the unmodified reference, wide=False, or the widened restatement, wide=True) and yields
-    (stage, array) after every stage, converted to the reference's uint16 / 64-bit-tag layout."""
+    (stage, array) after every stage, converted to the reference's uint16 / 64-bit-tag layout.  after_collide(s) may edit the contacts
+    (custom contacts, example/main.cpp:288) before they are read."""
     tag = (lambda t, f: abi.wide_tag_to_ref(t, f)) if wide else (lambda t, f: t)
     s.collide()
+    if after_collide:
+        after_collide(s)
     c = s.contacts_view()
     yield "contact count", np.array([c["count"]], np.uint32)
     yield "active", c["active"].astype(np.uint32)
@@ -132,22 +135,27 @@ def digest(a):
     return np.frombuffer(h.digest()[:8], np.uint8)
 
 
-def stage_digests(s, wide, steps, before_step=None, nan_blind=False):
-    """Labels and digests of every stage of `steps` steps of `s` (ref_layout_stages); before_step(i, s) runs ahead of step i.
+def stage_digests(s, wide, steps, before_step=None, nan_blind=False, after_collide=None):
+    """Labels and digests of every stage of `steps` steps of `s` (ref_layout_stages); before_step(i, s) runs ahead of step i,
+    after_collide(i, s) between its collide and the contacts' first read.
     nan_blind: digest nan_canonical(stage) instead, so that only the sign and payload of NaNs may differ."""
     labels, out = [], []
     for i in range(steps):
         if before_step:
             before_step(i, s)
-        for name, a in ref_layout_stages(s, wide):
+        hook = (lambda sim, i=i: after_collide(i, sim)) if after_collide else None
+        for name, a in ref_layout_stages(s, wide, hook):
             labels.append("step %d %s" % (i, name)); out.append(digest(nan_canonical(a) if nan_blind else a))
     return labels, np.array(out, np.uint8).reshape(-1, 8)
 
 
-def compare_oracle_gpu_step(o, g, rep, sweeps_individually=True):
-    """One full step, the widened CPU oracle against the CUDA path, every stage bit for bit.  Both must start from the same state."""
+def compare_oracle_gpu_step(o, g, rep, sweeps_individually=True, after_collide=None):
+    """One full step, the widened CPU oracle against the CUDA path, every stage bit for bit.  Both must start from the same state.
+    after_collide(o, g) runs after both collides (g's contacts downloaded) and may upload edited contacts to g."""
     o.collide(); g.collide()
     g.download_contacts()
+    if after_collide:
+        after_collide(o, g)
     oc, gc = o.contacts_view(), g.contacts_view()
     op, gp = o.pairs_view(), g.pairs_view()
     rep.eq("morton order", op["order"], gp["order"])

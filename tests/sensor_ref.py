@@ -83,7 +83,8 @@ class SensorOracleSim(FilteredOracleSim):
         hit = np.array([(x, y) in touching for x, y in zip(a.tolist(), b.tolist())], bool) if len(a) else np.zeros(0, bool)
         out = np.zeros(int(hit.sum()), scenes.SENSOR_OVERLAP)
         out["tags"] = a[hit] | (b[hit] << np.uint64(32))
-        first = np.where(tl <= th, lo, hi)[hit]; second = np.where(tl <= th, hi, lo)[hit]
+        lo_first = np.where(tl != th, tl < th, body[lo] < body[hi])   # equal tags: the lower body first
+        first = np.where(lo_first, lo, hi)[hit]; second = np.where(lo_first, hi, lo)[hit]
         out["body_a"] = body[first]; out["body_b"] = body[second]
         return out[np.argsort(out["tags"], kind="stable")]
 

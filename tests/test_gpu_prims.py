@@ -16,7 +16,7 @@ def test_scan_and_sort_match_numpy():
             out, tot = g.device_scan(d)
             ref = np.concatenate([[0], np.cumsum(d)[:-1]]).astype(np.uint32) if n else d
             assert np.array_equal(out, ref) and tot == int(d.sum())
-        for bits in (8, 17, 34, 48, 50):
+        for bits in (8, 17, 34, 48, 50, 63, 64):
             for ties in (True, False):   # heavy ties: stability, and one oversized bucket (the LSD fallback); uniform: the bucket path
                 keys = rng.integers(0, 1 << bits, n, dtype=np.uint64)
                 if ties and n > 10:
