@@ -25,7 +25,7 @@
  *   nb_add_bodies / nb_remove_bodies <- no reference counterpart: the application's edit of its caller-owned arrays between steps
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_snapshot_*                   <- no reference counterpart: the application's copy of its caller-owned arrays, kept in HBM
- *   nb_raycast                      <- no reference counterpart (the reference has no scene queries)
+ *   nb_raycast, nb_overlap          <- no reference counterpart (the reference has no scene queries)
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -580,6 +580,59 @@ typedef struct { float position[3]; float t; float normal[3]; uint32_t collider;
 enum nb_ray_flags { NB_RAY_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
 #define NB_RAY_NO_HIT 0xffffffffu
 int nb_raycast(nb_context*, const nb_ray* rays, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream);
+
+/* Overlap queries (area damage, perception cones and boxes, selection boxes, spawn-point checks, proximity observations; DESIGN.md section
+ * 8.15): which colliders touch each of n spheres or oriented boxes, against the colliders as the body transforms stand when the call runs on
+ * `stream`, answered on the device.  A collider's world transform is nb_raycast's, and which colliders count is nb_raycast's rule: collider i
+ * counts iff (category_i & query.mask) != 0, its body != ignore_body (NB_RAY_NO_HIT: ignore none), and it is not a sensor collider unless
+ * flags has NB_OVERLAP_SENSORS.  Body 0 and kinematic bodies are solid like any other.
+ * Result: the hits ordered by query, then by ascending collider index (boxes first, then spheres); offsets[q] .. offsets[q + 1] is query q's
+ * range and offsets[n] the total.  A hit is (query, collider, its body, its tag).  The order is defined without reference to any traversal,
+ * so any walk gives the same bytes.  Overflow: when the total exceeds `capacity` (in hits), only offsets[n] is defined and holds the total
+ * needed; a host-pointer call then returns NB_ERR_CAPACITY, a device-pointer call writes it and returns NB_OK.
+ * A degenerate query hits nothing and does not fail the call: an unknown shape, a field the shape reads that is not finite (SPHERE reads
+ * center and radius; BOX center, rotation and half_extents; fields a shape does not read are not read), a negative radius or half extent, a
+ * BOX rotation with dot(q, q) == 0.  The device decides this, since device-pointer queries cannot be checked on the host.
+ * The tests are float32, left to right as written, without fused multiply-adds, with cross, dot and qrot as in the joints' section above;
+ * (p, q) is the collider's world transform, h its half extents (box size), rc its radius, conj(q) = (-q.x, -q.y, -q.z, q.w), e_x, e_y, e_z
+ * the unit axes.  A BOX query's rotation is used as given, not normalised.  Touching counts: every comparison is closed, unlike the
+ * broadphase's strict AABB rule.
+ *   SPHERE (c, r) vs SPHERE:  d = c - p;  overlap iff dot(d, d) <= (r + rc) * (r + rc)
+ *   SPHERE (c, r) vs BOX:     l = qrot(conj(q), c - p);  per axis k: g_k = l_k < -h_k ? l_k + h_k : (l_k > h_k ? l_k - h_k : +0);
+ *                             overlap iff dot(g, g) <= r * r
+ *   BOX (c, Q, H) vs SPHERE:  the same with l = qrot(conj(Q), p - c), H for h and rc for r
+ *   BOX (c, Q, H) vs BOX:     u_k = qrot(Q, e_k), v_k = qrot(q, e_k);  t = p - c;  the axes in this order: u_x, u_y, u_z, v_x, v_y, v_z, then
+ *                             cross(u_i, v_j) for i = x, y, z and, inside, j = x, y, z;  for axis L:
+ *                             ra = (fabsf(H.x * dot(u_x, L)) + fabsf(H.y * dot(u_y, L))) + fabsf(H.z * dot(u_z, L)), rb likewise with h and v;
+ *                             separated when fabsf(dot(t, L)) > ra + rb;  overlap iff no axis separates
+ * No epsilon guards parallel edges: a zero cross axis cannot separate (0 > 0 is false), and any nonzero axis is a valid separating test.
+ * Which candidates the device tests is decided by a conservative grid walk (DESIGN.md section 8.15); whether a candidate overlaps is decided
+ * by the tests above alone.
+ * on_device != 0: queries, hits and offsets are device pointers (4-byte alignment suffices); the call is asynchronous on `stream`, and a call
+ * whose capacity is at most the largest an earlier call on the context used makes no synchronisation and no allocation, so it can be
+ * captured into the application's CUDA graph.  A call with a larger capacity grows the hit-key scratch (synchronises and allocates).
+ * on_device == 0: host pointers; the queries are staged like the editing calls' arrays, and the call returns with offsets and hits filled.
+ * Legal between any two calls, stage calls included; it changes nothing that a step, a download or a snapshot can observe.  Scratch: the
+ * ray casts' (181 to 213 bytes per collider of capacity, allocated on the first query of either kind) plus 16 bytes per hit of capacity, and
+ * for a host-pointer call 64 bytes per query, 4 per offset and 16 per hit of capacity.  NB_ERR_ARGUMENT, changing nothing: a null queries or
+ * offsets pointer with n > 0, a null hits pointer with n > 0 and capacity > 0, unknown flag bits, a context that nb_shard_create was called
+ * on.  Launches: 9 per call with n > 0 (reset, world transforms and AABBs, Morton codes, one radix sort, leaves, grid table, the walk, the
+ * hit sort, the write), 1 (the write alone) when the scene has no collider or no body, none with n = 0 or a refused call; none per step. */
+typedef struct {
+	uint32_t shape;             /* NB_OVERLAP_SPHERE or NB_OVERLAP_BOX */
+	float center[3];
+	float rotation[4];          /* BOX: x, y, z, w, used as given (not normalised) */
+	float half_extents[3];      /* BOX */
+	float radius;               /* SPHERE; 0 = a point query */
+	uint32_t mask;              /* collider i counts iff (category_i & mask) != 0, as for rays */
+	uint32_t ignore_body;       /* NB_RAY_NO_HIT: ignore none */
+	uint32_t reserved[2];
+} nb_overlap_query;             /* 64 bytes */
+typedef struct { uint32_t query, collider, body, tag; } nb_overlap_hit;   /* 16 bytes */
+enum nb_overlap_shape { NB_OVERLAP_SPHERE = 0, NB_OVERLAP_BOX = 1 };
+enum nb_overlap_flags { NB_OVERLAP_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
+int nb_overlap(nb_context*, const nb_overlap_query* queries, uint32_t n, nb_overlap_hit* hits, uint32_t capacity, uint32_t* offsets /* n + 1 */,
+               uint32_t flags, int on_device, void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

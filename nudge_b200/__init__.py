@@ -26,7 +26,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
-           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast"]
+           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap"]
 
 
 class Config(C.Structure):
@@ -121,6 +121,7 @@ def load_library():
         lib.nb_snapshot_save.argtypes = [V, V, V]
         lib.nb_snapshot_restore.argtypes = [V, V, V]
         lib.nb_raycast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
+        lib.nb_overlap.argtypes = [V, V, C.c_uint32, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         _lib = lib
     return _lib
 
@@ -463,7 +464,32 @@ class Sim(abi.HostState):
         self._ck(self.lib.nb_raycast(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_raycast")
         return out
 
-    # ---- collision filters (nb_collision_filter, include/nudge_b200.h) ----
+    # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----
+    def overlap(self, queries, flags=0, capacity=None, device_ptrs=None, n=None):
+        """queries: abi.OVERLAP_QUERY rows; returns (offsets, hits): offsets[q] .. offsets[q + 1] indexes query q's abi.OVERLAP_HIT rows, by
+        ascending collider.  flags: OVERLAP_SENSORS also tests sensor colliders.  capacity: room for that many hits; without one, a call
+        that needs more is repeated once with room for the total.  With a capacity that is too small, raises NudgeError.
+        device_ptrs=(queries_ptr, hits_ptr, offsets_ptr) with n and capacity: device buffers of n queries, capacity hits and n + 1 offsets
+        instead; the call is then asynchronous on the Sim's stream (capturable once the scratch holds the capacity) and returns None."""
+        if device_ptrs is not None:
+            if n is None or capacity is None:
+                raise ValueError("Sim.overlap with device_ptrs needs n (queries) and capacity (hits) of the device buffers")
+            q, h, o = (C.c_void_p(p) for p in device_ptrs)
+            self._ck(self.lib.nb_overlap(self.ctx, q, int(n), h, int(capacity), o, int(flags), 1, self.stream), "nb_overlap")
+            return None
+        qs = np.ascontiguousarray(np.asarray(queries, abi.OVERLAP_QUERY).reshape(-1))
+        P = lambda a: abi.ptr(a) if len(a) else None
+        cap = int(capacity) if capacity is not None else max(1024, 16 * len(qs))
+        for retry in (capacity is None, False):
+            offsets = np.zeros(len(qs) + 1, np.uint32)
+            hits = np.zeros(cap, abi.OVERLAP_HIT)
+            r = self.lib.nb_overlap(self.ctx, P(qs), len(qs), P(hits), cap, abi.ptr(offsets), int(flags), 0, self.stream)
+            if r == -2 and retry:   # NB_ERR_CAPACITY: offsets[n] holds the total
+                cap = int(offsets[-1])
+                continue
+            self._ck(r, "nb_overlap")
+            return offsets, hits[:offsets[-1]]
+
     def upload_collision_filters(self, filters, flags=0):
         """filters: one scenes.FILTER row (category, mask) per collider, boxes first then spheres, or None / empty to remove the table.
         flags: FILTER_SKIP_CONNECTED also rejects pairs whose bodies are joined by a connection.  Colliders i and j collide iff

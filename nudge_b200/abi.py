@@ -50,6 +50,15 @@ assert RAY.itemsize == 48 and RAY_HIT.itemsize == 48
 RAY_SENSORS = 1
 RAY_NO_HIT = 0xffffffff
 
+# nb_overlap_query (64 bytes), nb_overlap_hit (16 bytes)
+OVERLAP_QUERY = np.dtype([("shape", "<u4"), ("center", "<f4", 3), ("rotation", "<f4", 4), ("half_extents", "<f4", 3), ("radius", "<f4"),
+                          ("mask", "<u4"), ("ignore_body", "<u4"), ("reserved", "<u4", 2)])
+OVERLAP_HIT = np.dtype([("query", "<u4"), ("collider", "<u4"), ("body", "<u4"), ("tag", "<u4")])
+assert OVERLAP_QUERY.itemsize == 64 and OVERLAP_HIT.itemsize == 16
+OVERLAP_SPHERE = 0
+OVERLAP_BOX = 1
+OVERLAP_SENSORS = 1
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

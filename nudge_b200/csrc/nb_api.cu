@@ -42,15 +42,20 @@ struct RowLevels { u32 n = 0, levels = 0; std::vector<u32> level_off, order; std
 struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; };
 
 // The buffers of nb_collide's front end (launch_front_end); leaf_* = the AABBs in Morton order, keybits = the OR and AND of the Morton codes.
-// The context has one, the ray casts their own (nb_query_api.cuh), so that a query never touches what the step reads.
+// The context has one, the scene queries their own (nb_query_api.cuh), so that a query never touches what the step reads.
 struct FrontEnd {
 	nb_transform* world_xf; float4* aabb_min; float4* aabb_max; u32* col_tag; u32* col_body; u32* order; u32* rank;
 	float4* leaf_min; float4* leaf_max; u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask; u64* keybits;
 };
 
-// The ray casts' scratch (nb_query_api.cuh): the front end, its sort buffers and counters, allocated on the first nb_raycast for the
-// collider capacity; rays / hits = the staging of a call with host pointers.
-struct RayScratch { FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; bool ready; };
+// The scene queries' scratch (nb_query_api.cuh), shared by nb_raycast and nb_overlap: the front end, its sort buffers and counters,
+// allocated on the first query for the collider capacity; rays / hits = the staging of a ray call with host pointers.  The overlap call's
+// hit keys and their sort (osb points into okeys, with sb's histogram and grid barrier) hold the largest capacity a call asked for;
+// oq / oh / ooff = the staging of an overlap call with host pointers.
+struct QueryScratch {
+	FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; bool ready;
+	DevBuf<u64> okeys[2]; SortBuffers osb; DevBuf<nb_overlap_query> oq; DevBuf<nb_overlap_hit> oh; DevBuf<u32> ooff;
+};
 
 struct nb_context {
 	nb_config cfg;
@@ -115,8 +120,8 @@ struct nb_context {
 	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
 	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
-	// ray casts (nb_raycast, DESIGN.md section 8.14)
-	RayScratch ray;
+	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14) and overlap queries (nb_overlap, section 8.15)
+	QueryScratch query;
 
 	// scene
 	nb_transform* xf; nb_body_properties* props; nb_body_momentum* mom; uint8_t* idle;
@@ -1204,8 +1209,19 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	if (!strcmp(name, "ray_fallbacks") || !strcmp(name, "ray_grid_level")) {
 		if (max_bytes < 4) return NB_ERR_ARGUMENT;
 		u32 v = 0;
-		if (ctx->ray.ready) {
-			CK(cudaMemcpyAsync(&v, ctx->ray.counts + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+		if (ctx->query.ready) {
+			CK(cudaMemcpyAsync(&v, ctx->query.counts + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+			CK(cudaStreamSynchronize((cudaStream_t)stream));
+		}
+		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
+	}
+	// nb_overlap's counter (0 before the first query): queries that tested every collider instead of walking the grid, summed over the
+	// context's calls
+	if (!strcmp(name, "overlap_fallbacks")) {
+		if (max_bytes < 4) return NB_ERR_ARGUMENT;
+		u32 v = 0;
+		if (ctx->query.ready) {
+			CK(cudaMemcpyAsync(&v, ctx->query.counts + CNT_SURV, 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
 			CK(cudaStreamSynchronize((cudaStream_t)stream));
 		}
 		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;

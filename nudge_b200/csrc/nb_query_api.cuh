@@ -1,6 +1,7 @@
-// nudge_b200 — ray casts against the current colliders (nb_raycast, include/nudge_b200.h; DESIGN.md section 8.14).
-// The build is nb_collide's front end (launch_front_end, nb_api.cu) on a FrontEnd of the query's own (RayScratch): world transforms and
-// AABBs (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid table (k_grid_build).  One new kernel walks it.
+// nudge_b200 — scene queries against the current colliders: ray casts (nb_raycast, DESIGN.md section 8.14) and overlap queries (nb_overlap,
+// section 8.15; include/nudge_b200.h).  Both build with nb_collide's front end (launch_front_end, nb_api.cu) on the FrontEnd of the queries'
+// own scratch (QueryScratch): world transforms and AABBs (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid
+// table (k_grid_build).  k_raycast and k_overlap walk it; k_overlap's hit keys are sorted and written out by k_overlap_write.
 // Included at the end of nb_api.cu.
 #pragma once
 
@@ -44,13 +45,13 @@ NB_DEV bool ray_sphere(f3 o, f3 d, float max_t, const xform& w, float r, float& 
 	return true;
 }
 
-struct RayScene {
+struct QueryScene {
 	u32 K, nboxes;
 	const nb_transform* world_xf; const float4* aabb_max; const u32* col_body; const u32* col_tag;
 	const nb_box_collider* box_data; const nb_sphere_collider* sph_data; const uint8_t* sensor;
 };
 // Tests collider i and keeps the lane's best (t bits << 32 | i) and the normal that goes with it.
-NB_DEV void ray_test(const RayScene& S, u32 i, f3 o, f3 d, float max_t, u32 mask, u32 ignore, bool sensors, u64& best, f3& bn) {
+NB_DEV void ray_test(const QueryScene& S, u32 i, f3 o, f3 d, float max_t, u32 mask, u32 ignore, bool sensors, u64& best, f3& bn) {
 	const u32 category = asu(reinterpret_cast<const float*>(S.aabb_max)[4 * (size_t)i + 3]) & 0xffffu;   // k_collider_world's filter word
 	if (!(category & mask) || __ldg(S.col_body + i) == ignore || (S.sensor && !sensors && __ldg(S.sensor + i))) return;
 	const xform w = ld_xform(S.world_xf, i);
@@ -67,9 +68,41 @@ NB_DEV u64 warp_min_u64(u64 v) {
 	return v;
 }
 
+// Looks up the level-j cells c0 + [0, nc) per axis (nc >= 1) in the grid's hash table, flattens their ranges of Morton positions with a
+// warp scan and deals the positions round-robin to the lanes, as k_grid_pairs deals its candidates: visit(position) runs once for every
+// position of every cell, on one lane.  Warp-uniform arguments; the whole warp calls it.
+template<class F>
+NB_DEV void grid_cells_visit(const int c0[3], const int nc[3], u32 j, const u64* table_keys, const u64* table_vals, u32 table_mask, u32 lane, F visit) {
+	const u32 ncells = (u32)(nc[0] * nc[1] * nc[2]);
+	for (u32 cb = 0; cb < ncells; cb += 32) {
+		const u32 ci = cb + lane;
+		u32 qb = 0, len = 0;
+		if (ci < ncells) {
+			const u32 cx = (u32)c0[0] + ci % (u32)nc[0], cy = (u32)c0[1] + (ci / (u32)nc[0]) % (u32)nc[1], cz = (u32)c0[2] + ci / (u32)(nc[0] * nc[1]);
+			const u64 prefix = morton48_of(cx << j, cy << j, cz << j) >> (3 * j);
+			u32 slot = grid_hash(prefix, table_mask);
+			u64 key;
+			while ((key = table_keys[slot]) != prefix && key != NB_GRID_EMPTY) slot = (slot + 1) & table_mask;
+			if (key != NB_GRID_EMPTY) { const u64 range = table_vals[slot]; qb = (u32)range; len = (u32)(range >> 32) - qb; }
+		}
+		const u32 incl = warp_incl_scan(len), off = incl - len, total = __shfl_sync(0xffffffffu, incl, 31);
+		for (u32 t0 = 0; t0 < total; t0 += 32) {
+			const u32 t = t0 + lane;
+			u32 c = 0;   // the cell of candidate t: the last lane whose offset is <= t
+			#pragma unroll
+			for (int st = 16; st; st >>= 1) {
+				const u32 probe = __shfl_sync(0xffffffffu, off, (c + st) & 31);
+				if (c + st < 32 && probe <= t) c += st;
+			}
+			const u32 q = __shfl_sync(0xffffffffu, qb, c) + (t - __shfl_sync(0xffffffffu, off, c));
+			if (t < total) visit(q);
+		}
+	}
+}
+
 // Segments per ray beyond which the walk gives up on the grid and tests every collider.
 #define NB_RAY_MAX_SEGMENTS 262144u
-// The query's own counters (RayScratch::counts) hold, in the slot the step's narrowphase uses, the number of rays that tested every
+// The query's own counters (QueryScratch::counts) hold, in the slot the step's narrowphase uses, the number of rays that tested every
 // collider instead of walking the grid, summed over the context's calls (nb_debug_read "ray_fallbacks").
 #define CNT_RAY_FALLBACKS CNT_TMP
 
@@ -84,7 +117,7 @@ NB_DEV u64 warp_min_u64(u64 v) {
 // whose margin at the far end of its clipped range exceeds two cells, or whose frame is not finite, tests every collider instead (and is
 // counted in CNT_RAY_FALLBACKS): with boxes only, an origin about 2^16 cells' widths outside the grid; with spheres, also a clipped range
 // ending more than about 1,000 cells' widths from the origin, which needs a grid of more than 1,000 cells per axis or an origin far outside.
-__global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays, nb_ray_hit* hits, u32 flags, RayScene S, const u32* order,
+__global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays, nb_ray_hit* hits, u32 flags, QueryScene S, const u32* order,
 		const u64* table_keys, const u64* table_vals, u32 table_mask, const u32* large_list, u32* counts) {
 	const u32 lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
 	const bool sensors = (flags & NB_RAY_SENSORS) != 0;
@@ -155,31 +188,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays,
 						if (h < l) empty = true;
 					}
 					if (empty) continue;
-					const u32 ncells = (u32)(nc[0] * nc[1] * nc[2]);
-					for (u32 cb = 0; cb < ncells; cb += 32) {
-						const u32 ci = cb + lane;
-						u32 qb = 0, len = 0;
-						if (ci < ncells) {
-							const u32 cx = (u32)c0[0] + ci % (u32)nc[0], cy = (u32)c0[1] + (ci / (u32)nc[0]) % (u32)nc[1], cz = (u32)c0[2] + ci / (u32)(nc[0] * nc[1]);
-							const u64 prefix = morton48_of(cx << j, cy << j, cz << j) >> (3 * j);
-							u32 slot = grid_hash(prefix, table_mask);
-							u64 key;
-							while ((key = table_keys[slot]) != prefix && key != NB_GRID_EMPTY) slot = (slot + 1) & table_mask;
-							if (key != NB_GRID_EMPTY) { const u64 range = table_vals[slot]; qb = (u32)range; len = (u32)(range >> 32) - qb; }
-						}
-						const u32 incl = warp_incl_scan(len), off = incl - len, total = __shfl_sync(0xffffffffu, incl, 31);
-						for (u32 t0 = 0; t0 < total; t0 += 32) {
-							const u32 t = t0 + lane;
-							u32 c = 0;   // the cell of candidate t: the last lane whose offset is <= t
-							#pragma unroll
-							for (int st = 16; st; st >>= 1) {
-								const u32 probe = __shfl_sync(0xffffffffu, off, (c + st) & 31);
-								if (c + st < 32 && probe <= t) c += st;
-							}
-							const u32 q = __shfl_sync(0xffffffffu, qb, c) + (t - __shfl_sync(0xffffffffu, off, c));
-							if (t < total) ray_test(S, order[q], o, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
-						}
-					}
+					grid_cells_visit(c0, nc, j, table_keys, table_vals, table_mask, lane, [&](u32 q) { ray_test(S, order[q], o, d, max_t, R.mask, R.ignore_body, sensors, best, bn); });
 				}
 			}
 		}
@@ -201,9 +210,180 @@ __global__ void __launch_bounds__(NB_BLOCK) k_raycast(u32 n, const nb_ray* rays,
 	}
 }
 
-// The query's scratch for the collider capacity, allocated once from the context's arena (synchronises then; never again).
-static int ensure_ray_scratch(nb_context* ctx) {
-	RayScratch& r = ctx->ray;
+// ---------------- overlap queries (nb_overlap): the per-collider arithmetic the header states ----------------
+NB_DEV bool overlap_sphere_sphere(f3 c, float r, f3 p, float rc) { const f3 d = sub3(c, p); return dot3(d, d) <= (r + rc) * (r + rc); }
+NB_DEV float box_gap(float l, float h) { return l < -h ? l + h : (l > h ? l - h : 0.0f); }
+// The sphere (c, r) against the box (p, q, h): also a BOX query against a sphere collider, with the roles swapped.
+NB_DEV bool overlap_sphere_box(f3 c, float r, f3 p, quat q, f3 h) {
+	quat qc = q; qc.v = mk3(-q.v.x, -q.v.y, -q.v.z);
+	const f3 l = qrot(qc, sub3(c, p));
+	const f3 g = mk3(box_gap(l.x, h.x), box_gap(l.y, h.y), box_gap(l.z, h.z));
+	return dot3(g, g) <= r * r;
+}
+NB_DEV float box_radius(f3 h, const f3 a[3], f3 L) { return (fabsf(h.x * dot3(a[0], L)) + fabsf(h.y * dot3(a[1], L))) + fabsf(h.z * dot3(a[2], L)); }
+NB_DEV void box_axes(quat q, f3 a[3]) { a[0] = qrot(q, mk3(1.0f, 0.0f, 0.0f)); a[1] = qrot(q, mk3(0.0f, 1.0f, 0.0f)); a[2] = qrot(q, mk3(0.0f, 0.0f, 1.0f)); }
+// The query box (c, axes u, H) against the box (p, q, h): the 15 axes in the header's order, the first that separates ends the test.
+NB_DEV bool overlap_box_box(f3 c, const f3 u[3], f3 H, f3 p, quat q, f3 h) {
+	f3 v[3]; box_axes(q, v);
+	const f3 t = sub3(p, c);
+	auto separates = [&](f3 L) { return fabsf(dot3(t, L)) > box_radius(H, u, L) + box_radius(h, v, L); };
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) if (separates(u[k])) return false;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) if (separates(v[k])) return false;
+	#pragma unroll
+	for (int i = 0; i < 3; ++i) {
+		#pragma unroll
+		for (int k = 0; k < 3; ++k) if (separates(cross3(u[i], v[k]))) return false;
+	}
+	return true;
+}
+
+// A query as the walk holds it: the shape, and for a box its axes u_k = qrot(Q, e_k), computed once per query.
+struct OverlapShape { bool box; f3 c; quat Q; f3 H; float r; f3 u[3]; };
+
+// The overlap call's use of the query counters (QueryScratch::counts): the append cursor of the hit keys (reset by the front end's
+// k_reset_collide; nb_radix_sort lowers it to the capacity), the total number of hits of the call (reset there too, never lowered), and the
+// number of queries that tested every collider instead of walking the grid, summed over the context's calls (nb_debug_read
+// "overlap_fallbacks"; nothing resets it).  None of the three is a counter the front end uses.
+#define CNT_OVERLAP_KEYS CNT_PAIRS
+#define CNT_OVERLAP_TOTAL CNT_SENSOR_PAIRS
+#define CNT_OVERLAP_FALLBACKS CNT_SURV
+
+// Tests collider i against the query; a hit appends (query << kq | i) while the capacity lasts and counts in nhits.
+NB_DEV void overlap_test(const QueryScene& S, u32 i, const OverlapShape& Q, u32 mask, u32 ignore, bool sensors, u64 qkey, u64* keys, u32 cap,
+		u32* counts, u32& nhits) {
+	const u32 category = asu(reinterpret_cast<const float*>(S.aabb_max)[4 * (size_t)i + 3]) & 0xffffu;   // k_collider_world's filter word
+	if (!(category & mask) || __ldg(S.col_body + i) == ignore || (S.sensor && !sensors && __ldg(S.sensor + i))) return;
+	const xform w = ld_xform(S.world_xf, i);
+	const f3 p = mk3(w.p.x, w.p.y, w.p.z);
+	bool hit;
+	if (i < S.nboxes) {
+		const float4 sz = reinterpret_cast<const float4*>(S.box_data)[i];
+		const f3 h = mk3(sz.x, sz.y, sz.z);
+		hit = Q.box ? overlap_box_box(Q.c, Q.u, Q.H, p, mkq(w.q), h) : overlap_sphere_box(Q.c, Q.r, p, mkq(w.q), h);
+	}
+	else {
+		const float rc = S.sph_data[i - S.nboxes].radius;
+		hit = Q.box ? overlap_sphere_box(p, rc, Q.c, Q.Q, Q.H) : overlap_sphere_sphere(Q.c, Q.r, p, rc);
+	}
+	if (!hit) return;
+	const u32 slot = warp_append_slot(&counts[CNT_OVERLAP_KEYS]);
+	if (slot < cap) keys[slot] = qkey | i;
+	++nhits;
+}
+
+// Cells per query beyond which the walk gives up on the grid and tests every collider.
+#define NB_OVERLAP_MAX_CELLS 4096u
+
+// One warp per query.  Without colliders (K = 0) k_overlap is not launched.  A query on the grid tests the large list first, then the
+// grid: the query's world AABB (a sphere's c -/+ r; a box's c -/+ the extent k_collider_world builds from qmatrix(Q) and H) is taken into
+// the Morton frame's quantised space.  A small collider fits a cell and is binned by its min corner, so a collider that touches the query
+// has its min-corner cell in [floor((lo - mu - W) / W), floor((hi + mu) / W)] per axis, lo / hi = the AABB's quantised extent.  mu is 2
+// units (the min corner's truncation and the cell-fit rule's +2) plus 2^-16 of the magnitudes involved (twice the quantised centre, the frame
+// offset, 4 x 65,536), which bounds the rounding of the quantisation, the transforms and the tests' differences of positions, plus 2^-6 of
+// (the query's quantised half extent + W), which bounds the tests' rounding relative to the query's and the collider's size and a query or
+// collider rotation up to 2^-10 away from unit length (DESIGN.md section 8.15).  Those cells are looked up and dealt to the lanes by
+// grid_cells_visit, skipping the large colliders (the large list tested them), so every collider is tested at most once.  A query that
+// tests every collider instead (counted in CNT_OVERLAP_FALLBACKS): a cell range of more than NB_OVERLAP_MAX_CELLS cells, a frame or margin
+// that is not finite, a BOX rotation with |dot(Q, Q) - 1| > 2^-10 (its extent need not bound what the stated test finds).
+__global__ void __launch_bounds__(NB_BLOCK) k_overlap(u32 n, const nb_overlap_query* queries, u32 flags, QueryScene S, const u32* order,
+		const uint8_t* smallf, const u64* table_keys, const u64* table_vals, u32 table_mask, const u32* large_list, u32 kq, u64* keys, u32 cap,
+		u32* counts) {
+	const u32 lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+	const bool sensors = (flags & NB_OVERLAP_SENSORS) != 0;
+	for (u32 qi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; qi < n; qi += nwarps) {   // qi is warp-uniform
+		const nb_overlap_query R = queries[qi];
+		OverlapShape Q;
+		Q.box = R.shape == NB_OVERLAP_BOX;
+		Q.c = ld3(R.center);
+		bool valid = (R.shape == NB_OVERLAP_SPHERE || Q.box) && isfinite(Q.c.x) && isfinite(Q.c.y) && isfinite(Q.c.z);
+		float qq = 1.0f;
+		f3 ext;
+		if (Q.box) {
+			Q.Q = mkq(make_float4(R.rotation[0], R.rotation[1], R.rotation[2], R.rotation[3]));
+			Q.H = ld3(R.half_extents);
+			qq = dot3(Q.Q.v, Q.Q.v) + Q.Q.s * Q.Q.s;
+			valid = valid && isfinite(Q.Q.v.x) && isfinite(Q.Q.v.y) && isfinite(Q.Q.v.z) && isfinite(Q.Q.s) && qq != 0.0f
+				&& isfinite(Q.H.x) && isfinite(Q.H.y) && isfinite(Q.H.z) && Q.H.x >= 0.0f && Q.H.y >= 0.0f && Q.H.z >= 0.0f;
+			box_axes(Q.Q, Q.u);
+			mat3 m = qmatrix(Q.Q);   // the extent as k_collider_world builds a box collider's
+			m.c0 = mul3(m.c0, Q.H.x); m.c1 = mul3(m.c1, Q.H.y); m.c2 = mul3(m.c2, Q.H.z);
+			ext = mk3(fabsf(m.c0.x) + fabsf(m.c1.x) + fabsf(m.c2.x), fabsf(m.c0.y) + fabsf(m.c1.y) + fabsf(m.c2.y), fabsf(m.c0.z) + fabsf(m.c1.z) + fabsf(m.c2.z));
+		}
+		else {
+			Q.r = R.radius;
+			valid = valid && isfinite(Q.r) && Q.r >= 0.0f;
+			ext = mk3(Q.r, Q.r, Q.r);
+		}
+		if (!valid) continue;
+		const u64 qkey = (u64)qi << kq;
+		u32 nhits = 0;
+		const MortonFrame f = morton_frame(counts);
+		const u32 j = counts[CNT_GRID_LEVEL];
+		const float W = (float)(1u << j), s = f.L[0];
+		const int ncell = 1 << (16 - j);
+		const float cu[3] = { Q.c.x * s - f.ms[0], Q.c.y * s - f.ms[1], Q.c.z * s - f.ms[2] }, eu[3] = { ext.x * s, ext.y * s, ext.z * s };
+		const float cumax = fmaxf(fabsf(cu[0]), fmaxf(fabsf(cu[1]), fabsf(cu[2]))), eumax = fmaxf(eu[0], fmaxf(eu[1], eu[2]));
+		const float M = 2.0f * cumax + fmaxf(fabsf(f.ms[0]), fmaxf(fabsf(f.ms[1]), fabsf(f.ms[2]))) + 262144.0f;
+		const float mu = 2.0f + M * (1.0f / 65536.0f) + (eumax + W) * (1.0f / 64.0f);
+		int c0[3], nc[3];
+		bool empty = false;
+		float ncells = 1.0f;
+		#pragma unroll
+		for (int a = 0; a < 3; ++a) {
+			const float lo = cu[a] - eu[a] - mu - W, hi = cu[a] + eu[a] + mu;
+			const int l = (int)fminf(fmaxf(floorf(lo / W), 0.0f), (float)ncell), h = (int)fmaxf(fminf(floorf(hi / W), (float)(ncell - 1)), -1.0f);
+			c0[a] = l; nc[a] = h - l + 1;
+			if (h < l) empty = true;
+			ncells *= (float)max(h - l + 1, 0);
+		}
+		const bool grid = s > 0.0f && isfinite(s) && f.L[1] == s && f.L[2] == s && f.L[3] == s && isfinite(mu) && fabsf(qq - 1.0f) <= 1.0f / 1024.0f
+			&& ncells <= (float)NB_OVERLAP_MAX_CELLS;
+		if (!grid) {
+			if (lane == 0) atomicAdd(&counts[CNT_OVERLAP_FALLBACKS], 1u);
+			for (u32 i = lane; i < S.K; i += 32) overlap_test(S, i, Q, R.mask, R.ignore_body, sensors, qkey, keys, cap, counts, nhits);
+		}
+		else {
+			const u32 nlarge = counts[CNT_LARGE];
+			for (u32 l = lane; l < nlarge; l += 32) overlap_test(S, order[large_list[l]], Q, R.mask, R.ignore_body, sensors, qkey, keys, cap, counts, nhits);
+			if (!empty)
+				grid_cells_visit(c0, nc, j, table_keys, table_vals, table_mask, lane, [&](u32 q) {
+					if (smallf[q]) overlap_test(S, order[q], Q, R.mask, R.ignore_body, sensors, qkey, keys, cap, counts, nhits);
+				});
+		}
+		#pragma unroll
+		for (int o = 16; o; o >>= 1) nhits += __shfl_xor_sync(0xffffffffu, nhits, o);
+		if (lane == 0 && nhits) atomicAdd(&counts[CNT_OVERLAP_TOTAL], nhits);
+	}
+}
+
+// The output: offsets[q] = the first sorted key of query q or later (a binary search; offsets[n] = the total), then the hits, written with
+// 4-byte stores since nb_overlap_hit and the offsets are only 4-byte aligned.  When the total exceeds the capacity only offsets[n] is
+// written.  counts null: no collider or body, every query's range is empty.
+__global__ void __launch_bounds__(NB_BLOCK) k_overlap_write(u32 n, const u64* keys, const u32* counts, u32 cap, u32 kq, const u32* col_body,
+		const u32* col_tag, nb_overlap_hit* hits, u32* offsets) {
+	const u32 total = counts ? counts[CNT_OVERLAP_TOTAL] : 0;
+	const u64 tid = blockIdx.x * (u64)blockDim.x + threadIdx.x, stride = (u64)gridDim.x * blockDim.x;
+	if (total > cap) { if (tid == 0) offsets[n] = total; return; }
+	for (u64 q = tid; q <= n; q += stride) {
+		const u64 first = q << kq;
+		u32 lo = 0, hi = total;
+		while (lo < hi) { const u32 mid = (lo + hi) >> 1; if (keys[mid] < first) lo = mid + 1; else hi = mid; }
+		offsets[q] = lo;
+	}
+	const u64 cmask = ((u64)1 << kq) - 1;
+	for (u64 i = tid; i < total; i += stride) {
+		const u64 key = keys[i];
+		const u32 c = (u32)(key & cmask);
+		u32* out = reinterpret_cast<u32*>(hits + i);
+		out[0] = (u32)(key >> kq); out[1] = c; out[2] = __ldg(col_body + c); out[3] = __ldg(col_tag + c);
+	}
+}
+
+// The queries' scratch for the collider capacity, allocated once from the context's arena (synchronises then; never again).
+static int ensure_query_scratch(nb_context* ctx) {
+	QueryScratch& r = ctx->query;
 	const u32 K = ctx->cfg.max_boxes + ctx->cfg.max_spheres;
 	if (r.ready) return NB_OK;
 	{ int e = alloc_front_end(ctx, r.front, K); if (e) return e; }
@@ -223,8 +403,8 @@ int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits
 	if (n && (!rays || !hits)) { ctx->error = "nb_raycast: null rays or hits"; return NB_ERR_ARGUMENT; }
 	if (!n) return NB_OK;
 	cudaStream_t st = (cudaStream_t)stream;
-	{ int r = ensure_ray_scratch(ctx); if (r) return r; }
-	RayScratch& q = ctx->ray;
+	{ int r = ensure_query_scratch(ctx); if (r) return r; }
+	QueryScratch& q = ctx->query;
 	const nb_ray* drays = rays;
 	nb_ray_hit* dhits = hits;
 	if (!on_device) {
@@ -238,13 +418,65 @@ int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits
 	const FrontEnd& f = q.front;
 	// the front end without the kinematic and sensor tables
 	if (int r = K ? launch_front_end(ctx, L, f, q.sb, counts, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr) : NB_OK) return r;
-	const RayScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
+	const QueryScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
 	launch_grid(L, k_raycast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, drays, dhits, flags, S, f.order, f.table_keys, f.table_vals, f.table_mask,
 		f.large_list, counts);
 	CK(cudaGetLastError());
 	if (!on_device) {
 		CK(cudaMemcpyAsync(hits, dhits, sizeof(nb_ray_hit) * (size_t)n, cudaMemcpyDeviceToHost, st));
 		CK(cudaStreamSynchronize(st));
+	}
+	return NB_OK;
+}
+
+int nb_overlap(nb_context* ctx, const nb_overlap_query* queries, uint32_t n, nb_overlap_hit* hits, uint32_t capacity, uint32_t* offsets,
+			   uint32_t flags, int on_device, void* stream) {
+	NB_RANGE("nb_overlap");
+	if (ctx->sharded) { ctx->error = "nb_overlap: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
+	if (flags & ~(u32)NB_OVERLAP_SENSORS) { ctx->error = "nb_overlap: unknown flags"; return NB_ERR_ARGUMENT; }
+	if (n && (!queries || !offsets || (capacity && !hits))) { ctx->error = "nb_overlap: null queries, offsets or hits"; return NB_ERR_ARGUMENT; }
+	if (!n) return NB_OK;
+	cudaStream_t st = (cudaStream_t)stream;
+	{ int r = ensure_query_scratch(ctx); if (r) return r; }
+	QueryScratch& q = ctx->query;
+	for (int i = 0; i < 2; ++i) { GROW(q.okeys[i], std::max(capacity, 1u), st); q.osb.keys[i] = q.okeys[i].p; q.osb.vals[i] = nullptr; }
+	q.osb.hist = q.sb.hist; q.osb.bar = q.sb.bar;   // the front end's sort has finished with them when the hit sort runs
+	const nb_overlap_query* dq = queries;
+	nb_overlap_hit* dh = hits;
+	u32* doff = offsets;
+	if (!on_device) {
+		GROW(q.oq, n, st); GROW(q.oh, std::max(capacity, 1u), st); GROW(q.ooff, (size_t)n + 1, st);
+		CK(put_staged(ctx, q.oq.p, queries, sizeof(nb_overlap_query) * (size_t)n, st));
+		dq = q.oq.p; dh = q.oh.p; doff = q.ooff.p;
+	}
+	const Launch L = mk_launch(ctx, st);
+	const u32 K = ctx->B ? ctx->nboxes + ctx->nspheres : 0;
+	const u32 grid_out = GRID(std::max<u64>((u64)n + 1, capacity));
+	if (K) {
+		u32* counts = q.counts;
+		const FrontEnd& f = q.front;
+		// the front end without the kinematic and sensor tables
+		if (int r = launch_front_end(ctx, L, f, q.sb, counts, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr)) return r;
+		const QueryScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
+		const u32 kq = bits_for(K);
+		launch_grid(L, k_overlap, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, dq, flags, S, f.order, f.smallf, f.table_keys, f.table_vals,
+			f.table_mask, f.large_list, kq, q.osb.keys[0], capacity, counts);
+		const int cur = nb_radix_sort(L, q.osb, counts + CNT_OVERLAP_KEYS, 0, (int)(kq + bits_for(n)), false, 0, 0, 0, nullptr, capacity);
+		launch_grid(L, k_overlap_write, grid_out, n, (const u64*)q.osb.keys[cur], (const u32*)counts, capacity, kq, (const u32*)f.col_body,
+			(const u32*)f.col_tag, dh, doff);
+	}
+	else launch_grid(L, k_overlap_write, grid_out, n, (const u64*)nullptr, (const u32*)nullptr, capacity, 1u, (const u32*)nullptr,
+			(const u32*)nullptr, dh, doff);
+	CK(cudaGetLastError());
+	if (!on_device) {
+		CK(cudaMemcpyAsync(offsets, doff, sizeof(u32) * ((size_t)n + 1), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		const u32 total = offsets[n];
+		if (total > capacity) { ctx->error = "nb_overlap: " + std::to_string(total) + " hits exceed the capacity"; return NB_ERR_CAPACITY; }
+		if (total) {
+			CK(cudaMemcpyAsync(hits, dh, sizeof(nb_overlap_hit) * (size_t)total, cudaMemcpyDeviceToHost, st));
+			CK(cudaStreamSynchronize(st));
+		}
 	}
 	return NB_OK;
 }
