@@ -25,7 +25,8 @@
  *   nb_add_bodies / nb_remove_bodies <- no reference counterpart: the application's edit of its caller-owned arrays between steps
  *   nb_save_state / nb_load_state   <- the caller-owned PODs               nudge.h:73-129
  *   nb_snapshot_*                   <- no reference counterpart: the application's copy of its caller-owned arrays, kept in HBM
- *   nb_raycast, nb_overlap          <- no reference counterpart (the reference has no scene queries)
+ *   nb_raycast, nb_overlap,
+ *   nb_shapecast                    <- no reference counterpart (the reference has no scene queries)
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -633,6 +634,61 @@ enum nb_overlap_shape { NB_OVERLAP_SPHERE = 0, NB_OVERLAP_BOX = 1 };
 enum nb_overlap_flags { NB_OVERLAP_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
 int nb_overlap(nb_context*, const nb_overlap_query* queries, uint32_t n, nb_overlap_hit* hits, uint32_t capacity, uint32_t* offsets /* n + 1 */,
                uint32_t flags, int on_device, void* stream);
+
+/* Shape casts (character controllers, thick projectiles, wheel probes, placement, camera collision; DESIGN.md section 8.16): where each of
+ * n spheres or oriented boxes first touches a collider when its centre moves from shape.center along direction, against the colliders as
+ * the body transforms stand when the call runs on `stream`, answered on the device.  The centre at t is center + t * direction; direction
+ * need not be unit length.  The shape translates only; it does not rotate during the sweep.  The shape, its mask and ignore_body follow
+ * nb_overlap's struct and rules, and so does which colliders count (NB_SHAPECAST_SENSORS also tests sensor colliders).
+ * Result: one nb_ray_hit per cast, the CLOSEST hit: the smallest t in [0, max_t], ties to the smaller collider index (boxes first, then
+ * spheres).  position = center + t * direction (per component); normal = the collider's surface normal at the contact, pointing from the
+ * collider towards the cast shape, of unit length up to rounding; collider, its body and tag as for rays; reserved 0.  No hit: collider =
+ * body = tag = NB_RAY_NO_HIT and every other field 0.  A degenerate cast hits nothing and does not fail the call: a shape nb_overlap calls
+ * degenerate, a field of direction or max_t that is not finite, a zero direction, max_t < 0.  The device decides this.
+ * The arithmetic is float32, left to right as written, without fused multiply-adds, IEEE division and sqrtf, with cross, dot and qrot as in
+ * the joints' section above and nb_overlap's notation; d = direction.  For each counted collider:
+ *   0. START:  if nb_overlap's test of the shape at center and this collider holds, the hit is t = 0 with normal (0, 0, 0).  Otherwise:
+ *   1. SPHERE (c, r) vs SPHERE:  nb_raycast's sphere test from origin c along d with radius rs = r + rc (its inside branch cannot be reached
+ *      after step 0); normal = (c + t*d - p) * (1 / rs)
+ *   2. SPHERE (c, r) vs BOX:  the ray lo + t*ld, lo = qrot(conj(q), c - p), ld = qrot(conj(q), d), against the box h rounded by r, which is
+ *      the union of 23 primitives tested in this order; the smallest t wins, ties to the earlier primitive; n_l = the local normal:
+ *      (a) three face boxes, k = x, y, z: nb_raycast's box test (the slab test) on lo, ld with h.k alone replaced by h.k + r; n_l = the slab
+ *          test's local normal (s in component `axis`, +0 elsewhere; (0, 0, 0) when no axis was recorded)
+ *      (b) twelve edge cylinders: axis k = x, y, z and, inside, the sign pairs (s_i, s_j) = (-,-), (-,+), (+,-), (+,+) of the other two axes
+ *          i < j:  m_i = lo.i - s_i h.i;  m_j = lo.j - s_j h.j;  a = ld.i*ld.i + ld.j*ld.j;  b = m_i*ld.i + m_j*ld.j;
+ *          cc = (m_i*m_i + m_j*m_j) - r*r;  miss when a == 0;  disc = b*b - a*cc, miss when disc < 0;  t = (-b - sqrtf(disc)) / a, miss
+ *          unless 0 <= t <= max_t (a NaN t misses), t == 0 becomes +0;  miss unless -h.k <= lo.k + t*ld.k <= h.k;
+ *          n_l = (m_i + t*ld.i) * (1 / r) in component i, (m_j + t*ld.j) * (1 / r) in j, +0 in k
+ *      (c) eight corner spheres at e = (s_x h.x, s_y h.y, s_z h.z), signs in binary order with x slowest ((-,-,-), (-,-,+), (-,+,-), ...):
+ *          m = lo - e;  a = dot(ld, ld);  b = dot(m, ld);  cc = dot(m, m) - r*r;  disc = b*b - a*cc, miss when disc < 0;
+ *          t = (-b - sqrtf(disc)) / a, miss unless 0 <= t <= max_t, t == 0 becomes +0;  n_l = (lo + t*ld - e) * (1 / r)
+ *      With r == 0 only (a) is tested (the three face boxes are then one box, so the cast is nb_raycast's ray).  normal = n_l == (0, 0, 0) ?
+ *      (0, 0, 0) : qrot(q, n_l)
+ *   3. BOX (c, Q, H) vs SPHERE:  test 2 with the roles swapped, the sphere collider moving along -d (negated per component) against the
+ *      query box: lo = qrot(conj(Q), p - c), ld = qrot(conj(Q), -d), H for h, rc for r;  normal = n_l == (0, 0, 0) ? (0, 0, 0) : -qrot(Q, n_l)
+ *   4. BOX (c, Q, H) vs BOX:  nb_overlap's 15 axes in its order with its ra and rb;  t0 = p - c;  enter = 0, exit = max_t, axis = none;  for
+ *      each axis L:  a = dot(t0, L);  b = dot(d, L);  R = ra + rb;
+ *        if b == 0: miss when fabsf(a) > R (otherwise the axis sets no bound)
+ *        else: t1 = (a - R) / b;  t2 = (a + R) / b;  near = t1 < t2 ? t1 : t2;  far = t1 < t2 ? t2 : t1;
+ *              if near > enter: enter = near, axis = L, sb = b;   if far < exit: exit = far;   miss when enter > exit
+ *      t = enter;  normal = axis == none ? (0, 0, 0) : (sb > 0 ? -L : L) * (1 / sqrtf(dot(L, L)))
+ *      A zero cross axis never bounds anything (b == 0 and fabsf(a) > R is false), as in nb_overlap's test.
+ * The hit key is (bits of t) << 32 | collider, so the smallest t, then the smallest collider, wins.  Which candidates the device tests is
+ * decided by a conservative grid walk (DESIGN.md section 8.16); whether and where a candidate is hit is decided by the arithmetic above alone.
+ * on_device != 0: casts and hits are device pointers (4-byte alignment suffices); the call is asynchronous on `stream`, and after the first
+ * scene query on the context it makes no synchronisation and no allocation, so it can be captured into the application's CUDA graph.
+ * on_device == 0: host pointers; the casts are staged like the editing calls' arrays (80 bytes per cast), and the call returns with `hits`
+ * filled.  Legal between any two calls, stage calls included; it changes nothing that a step, a download or a snapshot can observe.
+ * Scratch: the ray casts'.  NB_ERR_ARGUMENT, changing nothing: a null pointer with n > 0, unknown flag bits, a context that nb_shard_create
+ * was called on.  Launches: 7 per call with n > 0 (reset, world transforms and AABBs, Morton codes, one radix sort, leaves, grid table, the
+ * walk), 1 (the walk alone) when the scene has no collider or no body, none with n = 0; none per step. */
+typedef struct {
+	nb_overlap_query shape;     /* the shape at t = 0, its mask and ignore_body: nb_overlap's struct and rules */
+	float direction[3];         /* the shape's centre at t is center + t * direction; need not be unit length */
+	float max_t;
+} nb_shape_cast;                /* 80 bytes */
+enum nb_shapecast_flags { NB_SHAPECAST_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
+int nb_shapecast(nb_context*, const nb_shape_cast* casts, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

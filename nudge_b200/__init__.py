@@ -26,7 +26,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_upload_sensors", "nb_download_sensor_overlaps", "nb_upload_kinematic_bodies", "nb_apply_body_impulses", "nb_apply_radial_impulse",
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
-           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap"]
+           "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap",
+           "nb_shapecast"]
 
 
 class Config(C.Structure):
@@ -122,6 +123,7 @@ def load_library():
         lib.nb_snapshot_restore.argtypes = [V, V, V]
         lib.nb_raycast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         lib.nb_overlap.argtypes = [V, V, C.c_uint32, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
+        lib.nb_shapecast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         _lib = lib
     return _lib
 
@@ -462,6 +464,23 @@ class Sim(abi.HostState):
         out = np.zeros(len(r), abi.RAY_HIT)
         P = lambda a: abi.ptr(a) if len(a) else None
         self._ck(self.lib.nb_raycast(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_raycast")
+        return out
+
+    # ---- shape casts (nb_shapecast, include/nudge_b200.h): where a moving sphere or oriented box first touches a collider ----
+    def shapecast(self, casts, flags=0, device_ptrs=None, n=None):
+        """casts: abi.SHAPE_CAST rows; returns their abi.RAY_HIT rows (collider = body = tag = RAY_NO_HIT for a miss).  flags:
+        SHAPECAST_SENSORS also tests sensor colliders.  device_ptrs=(casts_ptr, hits_ptr) with n: device buffers of n casts and n hits
+        instead; the call is then asynchronous on the Sim's stream (capturable after a first scene query) and returns None."""
+        if device_ptrs is not None:
+            if n is None:
+                raise ValueError("Sim.shapecast with device_ptrs needs n, the number of casts (and hits) the two device buffers hold")
+            self._ck(self.lib.nb_shapecast(self.ctx, C.c_void_p(device_ptrs[0]), int(n), C.c_void_p(device_ptrs[1]), int(flags), 1, self.stream),
+                     "nb_shapecast")
+            return None
+        c = np.ascontiguousarray(np.asarray(casts, abi.SHAPE_CAST).reshape(-1))
+        out = np.zeros(len(c), abi.RAY_HIT)
+        P = lambda a: abi.ptr(a) if len(a) else None
+        self._ck(self.lib.nb_shapecast(self.ctx, P(c), len(c), P(out), int(flags), 0, self.stream), "nb_shapecast")
         return out
 
     # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----

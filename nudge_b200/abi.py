@@ -59,6 +59,11 @@ OVERLAP_SPHERE = 0
 OVERLAP_BOX = 1
 OVERLAP_SENSORS = 1
 
+# nb_shape_cast (80 bytes): an overlap query's shape moved along direction up to max_t; its hits are abi.RAY_HIT rows
+SHAPE_CAST = np.dtype([("shape", OVERLAP_QUERY), ("direction", "<f4", 3), ("max_t", "<f4")])
+assert SHAPE_CAST.itemsize == 80
+SHAPECAST_SENSORS = 1
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

@@ -48,12 +48,12 @@ struct FrontEnd {
 	float4* leaf_min; float4* leaf_max; u64* mkeys; uint8_t* smallf; u32* large_list; u64* table_keys; u64* table_vals; u32 table_mask; u64* keybits;
 };
 
-// The scene queries' scratch (nb_query_api.cuh), shared by nb_raycast and nb_overlap: the front end, its sort buffers and counters,
-// allocated on the first query for the collider capacity; rays / hits = the staging of a ray call with host pointers.  The overlap call's
-// hit keys and their sort (osb points into okeys, with sb's histogram and grid barrier) hold the largest capacity a call asked for;
-// oq / oh / ooff = the staging of an overlap call with host pointers.
+// The scene queries' scratch (nb_query_api.cuh), shared by nb_raycast, nb_overlap and nb_shapecast: the front end, its sort buffers and
+// counters, allocated on the first query for the collider capacity; rays / casts / hits = the staging of a ray or shape cast call with host
+// pointers.  The overlap call's hit keys and their sort (osb points into okeys, with sb's histogram and grid barrier) hold the largest
+// capacity a call asked for; oq / oh / ooff = the staging of an overlap call with host pointers.
 struct QueryScratch {
-	FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_ray_hit> hits; bool ready;
+	FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_shape_cast> casts; DevBuf<nb_ray_hit> hits; bool ready;
 	DevBuf<u64> okeys[2]; SortBuffers osb; DevBuf<nb_overlap_query> oq; DevBuf<nb_overlap_hit> oh; DevBuf<u32> ooff;
 };
 
@@ -120,7 +120,8 @@ struct nb_context {
 	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
 	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
-	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14) and overlap queries (nb_overlap, section 8.15)
+	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap, section 8.15) and shape casts
+	// (nb_shapecast, section 8.16)
 	QueryScratch query;
 
 	// scene
@@ -1215,13 +1216,13 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		}
 		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
 	}
-	// nb_overlap's counter (0 before the first query): queries that tested every collider instead of walking the grid, summed over the
-	// context's calls
-	if (!strcmp(name, "overlap_fallbacks")) {
+	// nb_overlap's and nb_shapecast's counters (0 before the first query): queries or casts that tested every collider instead of walking
+	// the grid, summed over the context's calls (CNT_SHAPECAST_FALLBACKS, nb_query_api.cuh, is the slot after CNT_SENSOR_TMP)
+	if (!strcmp(name, "overlap_fallbacks") || !strcmp(name, "shapecast_fallbacks")) {
 		if (max_bytes < 4) return NB_ERR_ARGUMENT;
 		u32 v = 0;
 		if (ctx->query.ready) {
-			CK(cudaMemcpyAsync(&v, ctx->query.counts + CNT_SURV, 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+			CK(cudaMemcpyAsync(&v, ctx->query.counts + (name[0] == 'o' ? CNT_SURV : CNT_SENSOR_TMP + 1), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
 			CK(cudaStreamSynchronize((cudaStream_t)stream));
 		}
 		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;

@@ -1,7 +1,8 @@
-// nudge_b200 — scene queries against the current colliders: ray casts (nb_raycast, DESIGN.md section 8.14) and overlap queries (nb_overlap,
-// section 8.15; include/nudge_b200.h).  Both build with nb_collide's front end (launch_front_end, nb_api.cu) on the FrontEnd of the queries'
-// own scratch (QueryScratch): world transforms and AABBs (k_collider_world), Morton codes and their sort, Morton-ordered leaves and the grid
-// table (k_grid_build).  k_raycast and k_overlap walk it; k_overlap's hit keys are sorted and written out by k_overlap_write.
+// nudge_b200 — scene queries against the current colliders: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap,
+// section 8.15) and shape casts (nb_shapecast, section 8.16; include/nudge_b200.h).  All three build with nb_collide's front end
+// (launch_front_end, nb_api.cu) on the FrontEnd of the queries' own scratch (QueryScratch): world transforms and AABBs (k_collider_world),
+// Morton codes and their sort, Morton-ordered leaves and the grid table (k_grid_build).  k_raycast, k_overlap and k_shapecast walk it;
+// k_overlap's hit keys are sorted and written out by k_overlap_write.
 // Included at the end of nb_api.cu.
 #pragma once
 
@@ -381,6 +382,286 @@ __global__ void __launch_bounds__(NB_BLOCK) k_overlap_write(u32 n, const u64* ke
 	}
 }
 
+// ---------------- shape casts (nb_shapecast): the per-collider arithmetic the header states ----------------
+// nb_raycast's slab test on a ray already in the box's frame; nl = s in component `axis`, (0, 0, 0) when no axis was recorded.
+NB_DEV bool sweep_slab(f3 lo, f3 ld, f3 hh, float max_t, float& t, f3& nl) {
+	const float los[3] = { lo.x, lo.y, lo.z }, lds[3] = { ld.x, ld.y, ld.z }, h[3] = { hh.x, hh.y, hh.z };
+	float enter = 0.0f, exit = max_t, s = 0.0f;
+	int axis = -1;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) {
+		if (lds[k] == 0.0f) {
+			if (los[k] < -h[k] || los[k] > h[k]) return false;
+		}
+		else {
+			const float t1 = (-h[k] - los[k]) / lds[k], t2 = (h[k] - los[k]) / lds[k];
+			const bool lt = t1 < t2;
+			const float near = lt ? t1 : t2, far = lt ? t2 : t1;
+			if (near > enter) { enter = near; axis = k; s = lt ? -1.0f : 1.0f; }
+			if (far < exit) exit = far;
+			if (enter > exit) return false;
+		}
+	}
+	t = enter;
+	nl = axis < 0 ? mk3(0.0f, 0.0f, 0.0f) : axis == 0 ? mk3(s, 0.0f, 0.0f) : axis == 1 ? mk3(0.0f, s, 0.0f) : mk3(0.0f, 0.0f, s);
+	return true;
+}
+// The quadratic of the edge cylinders and corner spheres: a, b, cc as stated, the entry t if it lies in [0, max_t] (-0 becomes +0).
+NB_DEV bool sweep_root(float a, float b, float cc, float max_t, float& t) {
+	const float disc = b * b - a * cc;
+	if (disc < 0.0f) return false;
+	t = (-b - sqrtf(disc)) / a;
+	if (!(t >= 0.0f && t <= max_t)) return false;   // a NaN t misses too
+	if (t == 0.0f) t = 0.0f;   // -0 -> +0: the hit key orders t by its bits
+	return true;
+}
+// A sphere of radius r from lo along ld (the box's frame) against the box h centred at the origin: the 23 primitives of the rounded box in
+// the header's order, the smallest t winning and the earlier primitive a tie.  nl = the local normal.
+NB_DEV bool sweep_rounded_box(f3 lo, f3 ld, f3 h, float r, float max_t, float& t, f3& nl) {
+	bool hit = false;
+	float tk; f3 nk;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) {   // (a) the face boxes; with r == 0 they are one box
+		if (k > 0 && r == 0.0f) break;
+		const f3 hk = mk3(k == 0 ? h.x + r : h.x, k == 1 ? h.y + r : h.y, k == 2 ? h.z + r : h.z);
+		if (sweep_slab(lo, ld, hk, max_t, tk, nk) && (!hit || tk < t)) { hit = true; t = tk; nl = nk; }
+	}
+	if (r == 0.0f) return hit;
+	const float los[3] = { lo.x, lo.y, lo.z }, lds[3] = { ld.x, ld.y, ld.z }, hs[3] = { h.x, h.y, h.z };
+	const float inv = 1.0f / r;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) {   // (b) the edge cylinders along k
+		const int i = k == 0 ? 1 : 0, j = k == 2 ? 1 : 2;
+		const float a = lds[i] * lds[i] + lds[j] * lds[j];
+		if (a == 0.0f) continue;
+		#pragma unroll
+		for (int e = 0; e < 4; ++e) {
+			const float mi = los[i] - (e & 2 ? hs[i] : -hs[i]), mj = los[j] - (e & 1 ? hs[j] : -hs[j]);
+			const float b = mi * lds[i] + mj * lds[j], cc = (mi * mi + mj * mj) - r * r;
+			if (!sweep_root(a, b, cc, max_t, tk)) continue;
+			const float z = los[k] + tk * lds[k];
+			if (!(z >= -hs[k] && z <= hs[k]) || (hit && !(tk < t))) continue;
+			float n3[3];
+			n3[i] = (mi + tk * lds[i]) * inv; n3[j] = (mj + tk * lds[j]) * inv; n3[k] = 0.0f;
+			hit = true; t = tk; nl = mk3(n3[0], n3[1], n3[2]);
+		}
+	}
+	const float a = dot3(ld, ld);
+	#pragma unroll
+	for (int e = 0; e < 8; ++e) {   // (c) the corner spheres, x slowest
+		const f3 c = mk3(e & 4 ? h.x : -h.x, e & 2 ? h.y : -h.y, e & 1 ? h.z : -h.z);
+		const f3 m = sub3(lo, c);
+		if (!sweep_root(a, dot3(m, ld), dot3(m, m) - r * r, max_t, tk) || (hit && !(tk < t))) continue;
+		hit = true; t = tk; nl = mul3(sub3(add3(lo, mul3(tk, ld)), c), inv);
+	}
+	return hit;
+}
+NB_DEV bool is_zero3(f3 v) { return v.x == 0.0f && v.y == 0.0f && v.z == 0.0f; }
+// The query box (c, axes u, H) moving along d against the box (p, q, h): the swept separating axes in nb_overlap's order.
+NB_DEV bool sweep_box_box(f3 c, const f3 u[3], f3 H, f3 d, float max_t, f3 p, quat q, f3 h, float& t, f3& n) {
+	f3 v[3]; box_axes(q, v);
+	const f3 t0 = sub3(p, c);
+	float enter = 0.0f, exit = max_t, sb = 0.0f;
+	f3 axis = mk3(0.0f, 0.0f, 0.0f);
+	bool rec = false;
+	auto bound = [&](f3 L) {   // false: the cast misses
+		const float a = dot3(t0, L), b = dot3(d, L), R = box_radius(H, u, L) + box_radius(h, v, L);
+		if (b == 0.0f) return !(fabsf(a) > R);
+		const float t1 = (a - R) / b, t2 = (a + R) / b;
+		const bool lt = t1 < t2;
+		const float near = lt ? t1 : t2, far = lt ? t2 : t1;
+		if (near > enter) { enter = near; axis = L; sb = b; rec = true; }
+		if (far < exit) exit = far;
+		return !(enter > exit);
+	};
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) if (!bound(u[k])) return false;
+	#pragma unroll
+	for (int k = 0; k < 3; ++k) if (!bound(v[k])) return false;
+	#pragma unroll
+	for (int i = 0; i < 3; ++i) {
+		#pragma unroll
+		for (int k = 0; k < 3; ++k) if (!bound(cross3(u[i], v[k]))) return false;
+	}
+	t = enter;
+	if (!rec) n = mk3(0.0f, 0.0f, 0.0f);
+	else {
+		const float inv = 1.0f / sqrtf(dot3(axis, axis));
+		n = mul3(sb > 0.0f ? mk3(-axis.x, -axis.y, -axis.z) : axis, inv);
+	}
+	return true;
+}
+
+// Tests collider i against the cast and keeps the lane's best (t bits << 32 | i) and the normal that goes with it.
+NB_DEV void cast_test(const QueryScene& S, u32 i, const OverlapShape& Q, f3 d, float max_t, u32 mask, u32 ignore, bool sensors, u64& best, f3& bn) {
+	const u32 category = asu(reinterpret_cast<const float*>(S.aabb_max)[4 * (size_t)i + 3]) & 0xffffu;   // k_collider_world's filter word
+	if (!(category & mask) || __ldg(S.col_body + i) == ignore || (S.sensor && !sensors && __ldg(S.sensor + i))) return;
+	const xform w = ld_xform(S.world_xf, i);
+	const f3 p = mk3(w.p.x, w.p.y, w.p.z);
+	const quat q = mkq(w.q);
+	float t = 0.0f;
+	f3 n = mk3(0.0f, 0.0f, 0.0f), nl;
+	bool hit;
+	if (i < S.nboxes) {
+		const float4 sz = reinterpret_cast<const float4*>(S.box_data)[i];
+		const f3 h = mk3(sz.x, sz.y, sz.z);
+		if (Q.box ? overlap_box_box(Q.c, Q.u, Q.H, p, q, h) : overlap_sphere_box(Q.c, Q.r, p, q, h)) hit = true;   // step 0
+		else if (Q.box) hit = sweep_box_box(Q.c, Q.u, Q.H, d, max_t, p, q, h, t, n);
+		else {
+			quat qc = q; qc.v = mk3(-q.v.x, -q.v.y, -q.v.z);
+			hit = sweep_rounded_box(qrot(qc, sub3(Q.c, p)), qrot(qc, d), h, Q.r, max_t, t, nl);
+			if (hit && !is_zero3(nl)) n = qrot(q, nl);
+		}
+	}
+	else {
+		const float rc = S.sph_data[i - S.nboxes].radius;
+		if (Q.box ? overlap_sphere_box(p, rc, Q.c, Q.Q, Q.H) : overlap_sphere_sphere(Q.c, Q.r, p, rc)) hit = true;   // step 0
+		else if (Q.box) {
+			quat qc = Q.Q; qc.v = mk3(-Q.Q.v.x, -Q.Q.v.y, -Q.Q.v.z);
+			hit = sweep_rounded_box(qrot(qc, sub3(p, Q.c)), qrot(qc, mk3(-d.x, -d.y, -d.z)), Q.H, rc, max_t, t, nl);
+			if (hit && !is_zero3(nl)) { const f3 m = qrot(Q.Q, nl); n = mk3(-m.x, -m.y, -m.z); }
+		}
+		else hit = ray_sphere(Q.c, d, max_t, w, Q.r + rc, t, n);
+	}
+	if (!hit) return;
+	const u64 key = (u64)asu(t) << 32 | i;
+	if (key < best) { best = key; bn = n; }
+}
+
+// The query counters' slot (QueryScratch::counts) of the casts that tested every collider instead of walking the grid, summed over the
+// context's calls (nb_debug_read "shapecast_fallbacks"); neither the front end nor the other queries use it, and nothing resets it.
+#define CNT_SHAPECAST_FALLBACKS (CNT_SENSOR_TMP + 1)
+
+// One warp per cast, k_raycast's walk along the centre's path.  Without colliders (K = 0) every cast misses.  Otherwise the large list first,
+// then the grid: the path, clipped to the region that can hold the centre while the shape touches a small collider, is cut into segments of
+// at most one cell along its dominant axis.  A small collider touching the shape while its centre lies in a segment has its min-corner cell
+// in [floor((lo - e - mu - W) / W), floor((hi + e + mu) / W)] per axis: lo / hi = the segment's quantised extent, e = the shape's quantised
+// extent (r for a sphere; for a box the extent k_collider_world builds from qmatrix(Q) and H, as k_overlap takes it), mu the margin
+// (DESIGN.md section 8.16): k_raycast's 2 units and 2^-16 of the magnitudes involved, with the shape's extent among them; k_overlap's 2^-6
+// (e + W), which covers the tests' rounding relative to the sizes and a rotation up to 2^-10 off unit length; and the quadratic's
+// cancellation, 2^-9 (t |du| + e + W), whenever a cylinder, corner or sphere quadratic can run.  Segments tile the clipped t range, so once
+// the next segment starts beyond the best t every closer hit has been tested.  A cast tests every collider instead (counted in
+// CNT_SHAPECAST_FALLBACKS) when its frame or margin is not finite, its BOX rotation is more than 2^-10 from unit length, the margin at the far
+// end exceeds two cells, the segments exceed NB_RAY_MAX_SEGMENTS, or one segment's cell range exceeds NB_OVERLAP_MAX_CELLS.
+// One block per SM: the inlined tests need 174 registers, and under the default bound ptxas caps them at 128 and spills.
+__global__ void __launch_bounds__(NB_BLOCK, 1) k_shapecast(u32 n, const nb_shape_cast* casts, nb_ray_hit* hits, u32 flags, QueryScene S, const u32* order,
+		const uint8_t* smallf, const u64* table_keys, const u64* table_vals, u32 table_mask, const u32* large_list, u32* counts) {
+	const u32 lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+	const bool sensors = (flags & NB_SHAPECAST_SENSORS) != 0;
+	for (u32 ci = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; ci < n; ci += nwarps) {   // ci is warp-uniform
+		const nb_shape_cast C = casts[ci];
+		const nb_overlap_query& R = C.shape;
+		OverlapShape Q;
+		Q.box = R.shape == NB_OVERLAP_BOX;
+		Q.c = ld3(R.center);
+		const f3 d = ld3(C.direction);
+		const float max_t = C.max_t;
+		bool valid = (R.shape == NB_OVERLAP_SPHERE || Q.box) && isfinite(Q.c.x) && isfinite(Q.c.y) && isfinite(Q.c.z)
+			&& isfinite(d.x) && isfinite(d.y) && isfinite(d.z) && isfinite(max_t) && max_t >= 0.0f && (d.x != 0.0f || d.y != 0.0f || d.z != 0.0f);
+		float qq = 1.0f;
+		f3 ext;
+		if (Q.box) {
+			Q.Q = mkq(make_float4(R.rotation[0], R.rotation[1], R.rotation[2], R.rotation[3]));
+			Q.H = ld3(R.half_extents);
+			qq = dot3(Q.Q.v, Q.Q.v) + Q.Q.s * Q.Q.s;
+			valid = valid && isfinite(Q.Q.v.x) && isfinite(Q.Q.v.y) && isfinite(Q.Q.v.z) && isfinite(Q.Q.s) && qq != 0.0f
+				&& isfinite(Q.H.x) && isfinite(Q.H.y) && isfinite(Q.H.z) && Q.H.x >= 0.0f && Q.H.y >= 0.0f && Q.H.z >= 0.0f;
+			box_axes(Q.Q, Q.u);
+			mat3 m = qmatrix(Q.Q);   // the extent as k_collider_world builds a box collider's
+			m.c0 = mul3(m.c0, Q.H.x); m.c1 = mul3(m.c1, Q.H.y); m.c2 = mul3(m.c2, Q.H.z);
+			ext = mk3(fabsf(m.c0.x) + fabsf(m.c1.x) + fabsf(m.c2.x), fabsf(m.c0.y) + fabsf(m.c1.y) + fabsf(m.c2.y), fabsf(m.c0.z) + fabsf(m.c1.z) + fabsf(m.c2.z));
+		}
+		else {
+			Q.r = R.radius;
+			valid = valid && isfinite(Q.r) && Q.r >= 0.0f;
+			ext = mk3(Q.r, Q.r, Q.r);
+		}
+		u64 best = ~(u64)0;
+		f3 bn = mk3(0.0f, 0.0f, 0.0f);
+		if (valid && S.K) {
+			const u32 nlarge = counts[CNT_LARGE];
+			for (u32 l = lane; l < nlarge; l += 32) cast_test(S, order[large_list[l]], Q, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+			const MortonFrame f = morton_frame(counts);
+			const u32 j = counts[CNT_GRID_LEVEL];
+			const float W = (float)(1u << j), s = f.L[0];
+			const int ncell = 1 << (16 - j);
+			const float ou[3] = { Q.c.x * s - f.ms[0], Q.c.y * s - f.ms[1], Q.c.z * s - f.ms[2] }, du[3] = { d.x * s, d.y * s, d.z * s };
+			const float eu[3] = { ext.x * s, ext.y * s, ext.z * s };
+			const float oumax = fmaxf(fabsf(ou[0]), fmaxf(fabsf(ou[1]), fabsf(ou[2]))), eumax = fmaxf(eu[0], fmaxf(eu[1], eu[2]));
+			const float M = 2.0f * (oumax + eumax) + fmaxf(fabsf(f.ms[0]), fmaxf(fabsf(f.ms[1]), fabsf(f.ms[2]))) + 262144.0f;
+			const float mu0 = 2.0f + M * (1.0f / 65536.0f) + (eumax + W) * (1.0f / 64.0f);
+			// A quadratic runs against a sphere collider, and for a SPHERE cast of r > 0 against a box (its cylinders and corners).  Its
+			// reach beyond the radius is below 2^-10.5 |m|, |m| <= t |d| + r + rc + that reach, with rc below half a cell: 2^-9 (t |du| + e + W).
+			const bool quad = S.K > S.nboxes || (!Q.box && Q.r > 0.0f);
+			const float dnorm = 1.01f * sqrtf(du[0] * du[0] + du[1] * du[1] + du[2] * du[2]);
+			auto mu_at = [&](float t) { return mu0 + (quad ? (t * dnorm + eumax + W) * (1.0f / 512.0f) : 0.0f); };
+			const float mu_clip = mu0 + (quad ? (1.75f * (oumax + 65536.0f + W + eumax) + eumax + W) * (1.0f / 512.0f) : 0.0f);
+			// the region holding the centre whenever the shape touches a small collider (quantised min corners lie in [0, 65536)), widened
+			float tlo = 0.0f, thi = max_t, dmax = 0.0f;
+			bool any = true;
+			#pragma unroll
+			for (int k = 0; k < 3; ++k) {
+				const float lo = -eu[k] - 2.0f * mu_clip, hi = 65536.0f + W + eu[k] + 2.0f * mu_clip;
+				dmax = fmaxf(dmax, fabsf(du[k]));
+				if (du[k] == 0.0f) { if (ou[k] < lo || ou[k] > hi) any = false; }
+				else {
+					const float t1 = (lo - ou[k]) / du[k], t2 = (hi - ou[k]) / du[k];
+					tlo = fmaxf(tlo, fminf(t1, t2)); thi = fminf(thi, fmaxf(t1, t2));
+				}
+			}
+			const float nsegf = ceilf((thi - tlo) * dmax / W);
+			bool grid = s > 0.0f && isfinite(s) && f.L[1] == s && f.L[2] == s && f.L[3] == s && isfinite(mu_clip) && fabsf(qq - 1.0f) <= 1.0f / 1024.0f
+				&& mu_at(fmaxf(thi, tlo)) <= 2.0f * W && dmax > 0.0f && isfinite(nsegf) && nsegf <= (float)NB_RAY_MAX_SEGMENTS;
+			if (grid && any && tlo <= thi) {
+				const u32 nseg = max(1u, (u32)nsegf);
+				const float step = (thi - tlo) / (float)nseg;
+				for (u32 k = 0; k < nseg; ++k) {
+					const float ta = k == 0 ? tlo : tlo + (float)k * step, tb = k + 1 == nseg ? thi : tlo + (float)(k + 1) * step;
+					const u64 wbest = warp_min_u64(best);
+					if (wbest != ~(u64)0 && ta > asf((u32)(wbest >> 32))) break;   // every hit up to ta was tested
+					const float mu = mu_at(fmaxf(ta, tb));
+					int c0[3], nc[3];
+					bool empty = false;
+					float ncells = 1.0f;
+					#pragma unroll
+					for (int a = 0; a < 3; ++a) {
+						const float ua = ou[a] + ta * du[a], ub = ou[a] + tb * du[a];
+						const float lo = fminf(ua, ub) - eu[a] - mu - W, hi = fmaxf(ua, ub) + eu[a] + mu;
+						const int l = (int)fminf(fmaxf(floorf(lo / W), 0.0f), (float)ncell), h = (int)fmaxf(fminf(floorf(hi / W), (float)(ncell - 1)), -1.0f);
+						c0[a] = l; nc[a] = h - l + 1;
+						if (h < l) empty = true;
+						ncells *= (float)max(h - l + 1, 0);
+					}
+					if (empty) continue;
+					if (ncells > (float)NB_OVERLAP_MAX_CELLS) { grid = false; break; }   // every collider below; repeated keys change nothing
+					grid_cells_visit(c0, nc, j, table_keys, table_vals, table_mask, lane, [&](u32 q) {
+						if (smallf[q]) cast_test(S, order[q], Q, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+					});
+				}
+			}
+			if (!grid) {
+				if (lane == 0) atomicAdd(&counts[CNT_SHAPECAST_FALLBACKS], 1u);
+				for (u32 i = lane; i < S.K; i += 32) cast_test(S, i, Q, d, max_t, R.mask, R.ignore_body, sensors, best, bn);
+			}
+		}
+		const u64 wbest = warp_min_u64(best);
+		const u32 winner = wbest == ~(u64)0 ? 0u : (u32)__ffs(__ballot_sync(0xffffffffu, best == wbest)) - 1;
+		if (lane == winner) {
+			u32 w[12] = { 0, 0, 0, 0, 0, 0, 0, NB_RAY_NO_HIT, NB_RAY_NO_HIT, NB_RAY_NO_HIT, 0, 0 };   // a miss
+			if (wbest != ~(u64)0) {
+				const float t = asf((u32)(wbest >> 32));
+				const u32 i = (u32)wbest;
+				const f3 p = add3(Q.c, mul3(t, d));
+				w[0] = asu(p.x); w[1] = asu(p.y); w[2] = asu(p.z); w[3] = asu(t); w[4] = asu(bn.x); w[5] = asu(bn.y); w[6] = asu(bn.z);
+				w[7] = i; w[8] = __ldg(S.col_body + i); w[9] = __ldg(S.col_tag + i);
+			}
+			u32* out = reinterpret_cast<u32*>(hits + ci);   // 4-byte stores: nb_ray_hit is only 4-byte aligned
+			#pragma unroll
+			for (int k = 0; k < 12; ++k) out[k] = w[k];
+		}
+	}
+}
+
 // The queries' scratch for the collider capacity, allocated once from the context's arena (synchronises then; never again).
 static int ensure_query_scratch(nb_context* ctx) {
 	QueryScratch& r = ctx->query;
@@ -421,6 +702,39 @@ int nb_raycast(nb_context* ctx, const nb_ray* rays, uint32_t n, nb_ray_hit* hits
 	const QueryScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
 	launch_grid(L, k_raycast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, drays, dhits, flags, S, f.order, f.table_keys, f.table_vals, f.table_mask,
 		f.large_list, counts);
+	CK(cudaGetLastError());
+	if (!on_device) {
+		CK(cudaMemcpyAsync(hits, dhits, sizeof(nb_ray_hit) * (size_t)n, cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+	}
+	return NB_OK;
+}
+
+int nb_shapecast(nb_context* ctx, const nb_shape_cast* casts, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream) {
+	NB_RANGE("nb_shapecast");
+	if (ctx->sharded) { ctx->error = "nb_shapecast: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
+	if (flags & ~(u32)NB_SHAPECAST_SENSORS) { ctx->error = "nb_shapecast: unknown flags"; return NB_ERR_ARGUMENT; }
+	if (n && (!casts || !hits)) { ctx->error = "nb_shapecast: null casts or hits"; return NB_ERR_ARGUMENT; }
+	if (!n) return NB_OK;
+	cudaStream_t st = (cudaStream_t)stream;
+	{ int r = ensure_query_scratch(ctx); if (r) return r; }
+	QueryScratch& q = ctx->query;
+	const nb_shape_cast* dcasts = casts;
+	nb_ray_hit* dhits = hits;
+	if (!on_device) {
+		GROW(q.casts, n, st); GROW(q.hits, n, st);
+		CK(put_staged(ctx, q.casts.p, casts, sizeof(nb_shape_cast) * (size_t)n, st));
+		dcasts = q.casts.p; dhits = q.hits.p;
+	}
+	const Launch L = mk_launch(ctx, st);
+	const u32 K = ctx->B ? ctx->nboxes + ctx->nspheres : 0;
+	u32* counts = q.counts;
+	const FrontEnd& f = q.front;
+	// the front end without the kinematic and sensor tables
+	if (int r = K ? launch_front_end(ctx, L, f, q.sb, counts, ctx->has_filter ? ctx->filter : nullptr, nullptr, nullptr) : NB_OK) return r;
+	const QueryScene S = { K, ctx->nboxes, f.world_xf, f.aabb_max, f.col_body, f.col_tag, ctx->box_data, ctx->sph_data, ctx->has_sensor ? ctx->sensor : nullptr };
+	launch_grid(L, k_shapecast, GRID(std::min<u64>((u64)n * 32, 0xffffffffu)), n, dcasts, dhits, flags, S, f.order, f.smallf, f.table_keys, f.table_vals,
+		f.table_mask, f.large_list, counts);
 	CK(cudaGetLastError());
 	if (!on_device) {
 		CK(cudaMemcpyAsync(hits, dhits, sizeof(nb_ray_hit) * (size_t)n, cudaMemcpyDeviceToHost, st));
