@@ -228,8 +228,9 @@ int nb_download_constraint_rows(nb_context*, nb_constraint_row* host_rows, uint3
  * type, a field that is not finite, a null pointer with n > 0.  NB_ERR_CAPACITY: the joints form a dependency chain of more than 4,096 levels
  * (order a long chain red-black).  Asynchronous on `stream`; the host array may be reused when the call returns.  nb_step re-records its graph
  * only when the structure (n, and each joint's type, a and b) changed: new parameters or impulses for the same structure keep it.
- * nb_download_joints returns the joints in upload order with impulse[] = the rows' current accumulated impulses (what an application reads to
- * break a joint) and the unused impulse slots 0.  *count = the number of joints; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
+ * nb_download_joints returns the joints in upload order with impulse[] = the rows' current accumulated impulses (a joint that should fail
+ * past a force takes a BREAKABLE drive instead, nb_joint_drive below, which breaks it on the device) and the unused impulse slots 0.
+ * *count = the number of joints; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
  * nb_remove_bodies deletes the joints that name a removed body and remaps the others, keeping their order, parameters and accumulated
  * impulses; the kept body on the other side of a deleted joint gets idle counter 0 (not body 0, not a kinematic body).  nb_add_bodies leaves
  * the joints alone.  nb_upload_bodies keeps the set while the body count is unchanged and removes it when the count changes.
@@ -243,7 +244,7 @@ typedef struct {
 	float anchor_a[3];          /* in a's body frame */
 	float anchor_b[3];          /* in b's body frame; a world point when b = 0 */
 	float axis_a[3], axis_b[3]; /* HINGE: the hinge axis in each body's frame (unit length; the world frame for b = 0) */
-	float rel_rotation[4];      /* FIXED: conj(q_a) * q_b at rest (x, y, z, w; q_b = identity for b = 0) */
+	float rel_rotation[4];      /* FIXED, and HINGE with a LIMIT drive: conj(q_a) * q_b at rest (x, y, z, w; q_b = identity for b = 0) */
 	float length;               /* DISTANCE: rest distance between the anchors */
 	float beta;                 /* Baumgarte factor: bias = beta / dt * error */
 	float softness;             /* copied into every row */
@@ -251,6 +252,70 @@ typedef struct {
 } nb_joint;                     /* 112 bytes */
 int nb_upload_joints(nb_context*, const nb_joint* host, uint32_t n, void* stream);
 int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t* count, void* stream);
+
+/* Joint drives (doors, knees, flippers, wheels, fans, ropes, breakable bridges and welds; DESIGN.md section 8.17): hinge angle limits, hinge
+ * motors, distance ranges and break thresholds, built and solved by the joints' own kernels inside the step.  A drive set is a sparse table
+ * keyed by joint: at most one drive per joint, naming it by its index in the current joint set's upload order.
+ * Rows: a drive appends rows to its joint, solved right after the joint's own rows in this order: motor (MOTOR), lower limit and upper limit
+ * (LIMIT).  Every appended row has the joint's a, b and softness, reserved = 0, and keeps its accumulated impulse from step to step.  In
+ * nb_debug_read("joint_rows") the joints' own rows come first, exactly as without drives, then the appended rows, per driven joint in the
+ * joint table's order (by joint level, upload order within one).  Same arithmetic rules as above (float32, left to right, no fused
+ * multiply-adds), with k = beta / dt and bias(C) = C > 0 ? C / dt : k * C (speculative: a limit row lets the coordinate reach its bound
+ * within the step, and pulls it back at the joint's Baumgarte rate once past it):
+ *   HINGE coordinate:  g = qmul(q_a, rel_rotation);  d = b != 0 ? qmul(g, (-q_b.xyz, q_b.w)) : g;  if d.w < 0: d = -d (all four);
+ *              u = qrot(q_a, axis_a);  sh = -dot(d.xyz, u);  ch = d.w.  (sh, ch) = (sin, cos) of half of theta, b's rotation relative to a
+ *              about u from the rest pose rel_rotation (b = 0: minus a's rotation); theta in (-pi, pi].  The hinge Jacobian: lin_a = lin_b = 0,
+ *              ang_a = -u, ang_b = u.  The limits are converted once on the host at upload, each to its pair (sin(x/2), cos(x/2)), rounded from
+ *              double to float32: (sl, cl) for lower, (su, cu) for upper.
+ *   HINGE motor:       the hinge Jacobian, bias = -motor_speed, lo = -(max_motor_torque * dt), hi = max_motor_torque * dt.
+ *   HINGE lower limit: C = 2 * (sh*cl - ch*sl), the hinge Jacobian;  upper: C = 2 * (su*ch - cu*sh), ang_a = u, ang_b = -u, lin_a = lin_b
+ *              = 0 (the hinge Jacobian with its angular parts negated);  both bias = bias(C), lo = 0, hi = +inf.
+ *   DISTANCE limit:    the joint's own row is written with lo = hi = 0 (it stays in place and applies nothing);  lower: the own row's
+ *              Jacobian with C = dist - lower;  upper: that Jacobian negated with C = upper - dist;  both bias = bias(C), lo = 0, hi = +inf.
+ *   Breaking:  when k_joint_rows is about to rewrite a BREAKABLE joint's rows it takes the accumulated impulses the previous step left:
+ *              P = the sum 0 + i*i in row order over the joint's linear rows (the point rows; DISTANCE's own and limit rows), A = the same over
+ *              its angular rows (HINGE's and FIXED's angular rows, the hinge's motor and limit rows).  The joint breaks when
+ *              P > (break_force*dt)*(break_force*dt) or A > (break_torque*dt)*(break_torque*dt); +inf never breaks.
+ *   Broken:    a drive with broken = 1 has every row of its joint, appended rows included, written as a zero row: zero Jacobian, bias = 0,
+ *              lo = hi = 0, impulse = 0, softness = 0, a and b kept, reserved = 0.  The rows stay in the set, so nothing structural changes
+ *              and nb_step keeps its graph; broken stays 1 until an upload re-arms it.  Connections and idle counters are not touched (edit the
+ *              connections to let the pieces collide).
+ *   position:  each build of an unbroken LIMIT drive records the coordinate it used: (sh, ch) for a hinge, dist for a distance joint.
+ * nb_upload_joint_drives replaces the drive set (n = 0 removes it); impulse[] warm-starts the appended rows, broken is installed as given (0
+ * re-arms a broken joint), position is ignored and reads 0 until the next row build.  Every entry is checked on the host before any device
+ * work, and an error changes nothing.  NB_ERR_ARGUMENT: a null pointer with n > 0; a joint index at or beyond the joint count, or two drives
+ * on one joint; a flag the joint's type does not take (LIMIT: HINGE, DISTANCE; MOTOR: HINGE; BREAKABLE: every type) or an unknown bit;
+ * lower > upper, a hinge limit outside [-pi, pi] (pi rounded to float32, 3.14159274f), a negative distance limit; a negative max_motor_torque,
+ * break_force or break_torque; a field that is not finite other than thresholds of +inf; broken > 1; a HINGE LIMIT whose joint's
+ * rel_rotation has |x*x + y*y + z*z + w*w - 1| > 1e-3 (in double).  Asynchronous on `stream`, staged like nb_upload_joints (the host array
+ * may be reused on return); it synchronises only when the joints' row buffer must grow.  nb_step re-records its graph only when the drive
+ * structure (which joints, which flags) changed or a buffer moved: new speeds, torques, limits, thresholds, impulses or broken flags for the
+ * same structure keep it, so a throttle may be uploaded every frame.
+ * nb_download_joint_drives returns the drives in joint-index order with impulse[] = the appended rows' current accumulated impulses (0 where
+ * a row is absent), broken, and position: 2*atan2(sh, ch) in double, rounded to float32, for a hinge, dist for a distance joint, 0 without
+ * LIMIT or before the first build.  *count = the number of drives; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
+ * The set follows its joints: nb_upload_joints keeps it (impulses and broken flags included) when the joint structure is unchanged and removes
+ * it otherwise; nb_remove_bodies drops the drives of deleted joints and renumbers the rest; nb_add_bodies leaves it alone; nb_upload_bodies
+ * removes it with the joints.  Snapshots carry it; nb_save_state writes it (state version 7) and nb_load_state installs it through the
+ * upload's checks; a file of an older version removes it.  nb_debug_read("joint_drives") returns the device table: one 64-byte entry per joint in table order, { flags, first appended row, lower, upper, sl, cl, su, cu, motor_speed, max_motor_torque,
+ * break_force, break_torque, position[2] (sh, ch or dist, 0), broken, 0 }, flags 0 and the rest 0 for a joint without a drive.
+ * Cost: no launch; k_joint_rows and k_joint_solve take the drive table as one more argument (null without a set), and without a set the
+ * joints' rows, the launches and the graph are what they are without this feature. */
+enum nb_joint_drive_flags { NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4 };
+typedef struct {
+	uint32_t joint;             /* index of the joint in the current set's upload order */
+	uint32_t flags;             /* LIMIT: HINGE, DISTANCE.  MOTOR: HINGE.  BREAKABLE: every type */
+	float lower, upper;         /* LIMIT: HINGE angle in radians, -pi <= lower <= upper <= pi; DISTANCE length, 0 <= lower <= upper */
+	float motor_speed;          /* MOTOR: target of the hinge's relative angular velocity (rad/s) */
+	float max_motor_torque;     /* MOTOR: >= 0; the motor row's impulse stays in [-max_motor_torque*dt, +max_motor_torque*dt] */
+	float break_force, break_torque;   /* BREAKABLE: >= 0, +inf = never */
+	float impulse[3];           /* accumulated impulses of the motor, lower-limit and upper-limit rows (0 where absent) */
+	float position;             /* download: the hinge angle or the distance at the last row build (0 without LIMIT) */
+	uint32_t broken;            /* 0 or 1; upload 0 to re-arm a broken joint */
+	uint32_t reserved;
+} nb_joint_drive;               /* 56 bytes */
+int nb_upload_joint_drives(nb_context*, const nb_joint_drive* host, uint32_t n, void* stream);
+int nb_download_joint_drives(nb_context*, nb_joint_drive* host, uint32_t capacity, uint32_t* count, void* stream);
 
 /* Contact events (collision callbacks; DESIGN.md section 8.5): which collider pairs started or stopped touching, computed on the device inside
  * nb_write_cached_impulses (so the stage calls, nb_step and its graph replay give the same stream).  A pair (key tags = A | (uint64)B << 32,
@@ -504,7 +569,9 @@ int nb_stream_synchronize(nb_context*, void* stream);
  * ContactCache, widened layout) as one flat file, from / into the device-resident context.  Checkpoint, and what tools/nb_replay
  * steps headless; layout in nudge_b200/csrc/nb_state_api.cuh.  All three synchronise.  A context with a body force table writes version 5
  * (the table's B rows after the kinematic section); loading a file of versions 1-4 removes the context's table.  A context with joints
- * writes version 6 (the joints after the force table); loading a file of versions 1-5 removes the context's joints. */
+ * writes version 6 (the joints after the force table); loading a file of versions 1-5 removes the context's joints.  A context with joint
+ * drives writes version 7 (reserved[7] = the drive count, the nb_joint_drive rows after the joints); loading a file of versions 1-6 removes
+ * the context's drives. */
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);
@@ -515,7 +582,7 @@ int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres
  * unused lanes, idle counters); boxes and spheres (tags, data, transforms); connections; the contact cache (as many entries as the device count
  * says); the filter table, its flags and the NB_FILTER_SKIP_CONNECTED key list; the sensor table, max_sensor_pairs and the sensor overlap list
  * as of the last nb_write_cached_impulses; the kinematic set and its kind bytes; the body force table; the user constraint rows with their
- * accumulated impulses and their levelling; the joints with theirs; the solver mode; the contact-event step counter; the body, collider and connection counts and the
+ * accumulated impulses and their levelling; the joints with theirs and their drive table; the solver mode; the contact-event step counter; the body, collider and connection counts and the
  * tag and key bits.  It does not hold whether contact events are enabled, the undrained events, or the outputs of the last nb_collide.
  *
  * nb_snapshot_create allocates device memory for the context's capacities (DESIGN.md section 8.12 gives the bytes); nb_snapshot_destroy frees
@@ -529,7 +596,7 @@ int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres
  * ones are created.  nb_download_sensor_overlaps then returns the overlap list of the save, and the stage calls that read the last collide's
  * outputs are refused until the next nb_collide or nb_step, as after nb_add_bodies.  With every table already allocated it is one kernel
  * launch and host bookkeeping, without synchronisation.  nb_step keeps its graph when the step's launches and their arguments are unchanged:
- * the same counts, tag and key bits, table set, kinematic set, user-row set and joint structure; otherwise it re-records once.
+ * the same counts, tag and key bits, table set, kinematic set, user-row set, joint structure and drive structure; otherwise it re-records once.
  * NB_ERR_ARGUMENT, changing nothing: a snapshot of another context, restoring a snapshot that was never saved, a context that nb_shard_create
  * was called on. */
 typedef struct nb_snapshot nb_snapshot;

@@ -27,7 +27,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
            "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap",
-           "nb_shapecast"]
+           "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives"]
 
 
 class Config(C.Structure):
@@ -99,6 +99,8 @@ def load_library():
         lib.nb_download_constraint_rows.argtypes = [V, V, C.c_uint32, V]
         lib.nb_upload_joints.argtypes = [V, V, C.c_uint32, V]
         lib.nb_download_joints.argtypes = [V, V, C.c_uint32, V, V]
+        lib.nb_upload_joint_drives.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_download_joint_drives.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_instance_matrices.argtypes = [V, V, C.c_uint32, C.c_int, V, V]
         lib.nb_shard_build_plan.argtypes = [V, C.c_uint32, V, V, C.c_uint32, C.c_uint32, V, V, V, V, V, V, V, V]
         lib.nb_shard_local_scene.argtypes = [V, C.c_uint32, V, C.c_uint32, C.c_uint32, V, C.c_uint32, V, C.c_uint32, V, V, V, V, V]
@@ -165,6 +167,8 @@ ROW = np.dtype([("a", "<u4"), ("b", "<u4"), ("lin_a", "<f4", 3), ("ang_a", "<f4"
 assert ROW.itemsize == 80
 JOINT = abi.JOINT
 JOINT_BALL, JOINT_HINGE, JOINT_FIXED, JOINT_DISTANCE = 0, 1, 2, 3
+JOINT_DRIVE = abi.JOINT_DRIVE
+JOINT_LIMIT, JOINT_MOTOR, JOINT_BREAKABLE = 1, 2, 4
 
 
 def nccl_unique_id():
@@ -434,6 +438,19 @@ class Sim(abi.HostState):
         self.lib.nb_download_joints(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there are none)
         out = np.zeros(n.value, JOINT)
         self._ck(self.lib.nb_download_joints(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_joints")
+        return out
+
+    def upload_joint_drives(self, drives):
+        """Replaces the joint drive set (limits, motors, break thresholds) with `drives` (JOINT_DRIVE rows; none removes it).  Asynchronous."""
+        d = np.ascontiguousarray(np.asarray(drives if drives is not None else [], JOINT_DRIVE).reshape(-1))
+        self._ck(self.lib.nb_upload_joint_drives(self.ctx, abi.ptr(d) if len(d) else None, len(d), self.stream), "nb_upload_joint_drives")
+
+    def download_joint_drives(self):
+        """The drives in joint order with their rows' current impulses, position and broken flag."""
+        n = C.c_uint32(0)
+        self.lib.nb_download_joint_drives(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there are none)
+        out = np.zeros(n.value, JOINT_DRIVE)
+        self._ck(self.lib.nb_download_joint_drives(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_joint_drives")
         return out
 
     # ---- renderer read-back (example/main.cpp:224-268): one column-major 4x4 model matrix per collider, boxes first, then spheres ----

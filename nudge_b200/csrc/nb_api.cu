@@ -39,7 +39,18 @@ struct RowLevels { u32 n = 0, levels = 0; std::vector<u32> level_off, order; std
 
 // The host side of a joint set (nb_joint_api.cuh): its levels (the device table holds the joints by level), per joint in upload order its
 // (type, a, b), and the number of rows the joints generate.
-struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; };
+struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; std::vector<uint8_t> unit_rel; };   // unit_rel: rel_rotation of unit length
+
+// One joint's drive on the device (nb_joint_api.cuh; DESIGN.md section 8.17): one entry per joint in table order while a drive set exists,
+// flags = 0 for a joint without a drive.  row = the first of its appended rows; (sl, cl) / (su, cu) = the hinge limits' half-angle pairs;
+// position = (sh, ch) of a hinge or (dist, 0), as of the last row build.  nb_debug_read("joint_drives") returns the table as it stands.
+struct JointDrive {
+	u32 flags, row; float lower, upper, sl, cl, su, cu;
+	float motor_speed, max_motor_torque, break_force, break_torque, position[2]; u32 broken, reserved;
+};
+// The host side of a drive set: the drive count, the appended rows (after the joints' own in the row buffer) and per drive in joint order
+// its (joint, flags), the structure nb_step's graph depends on.
+struct DriveSet { u32 n = 0, nrows = 0; std::vector<u32> structure; };
 
 // The buffers of nb_collide's front end (launch_front_end); leaf_* = the AABBs in Morton order, keybits = the OR and AND of the Morton codes.
 // The context has one, the scene queries their own (nb_query_api.cuh), so that a query never touches what the step reads.
@@ -120,6 +131,8 @@ struct nb_context {
 	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
 	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
+	// joint drives (nb_upload_joint_drives, DESIGN.md section 8.17): the device table while dset.n, the rows appended after the joints' own in jrows
+	DevBuf<JointDrive> drives; DriveSet dset;
 	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap, section 8.15) and shape casts
 	// (nb_shapecast, section 8.16)
 	QueryScratch query;
@@ -1196,7 +1209,8 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
 		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
-		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ctx->jset.nrows },   // in table order: by joint level, upload order within one
+		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ((size_t)ctx->jset.nrows + ctx->dset.nrows) },   // in table order: by joint level, upload order within one; then the drives' rows
+		{ "joint_drives", ctx->drives.p, ctx->dset.n ? sizeof(JointDrive) * (size_t)ctx->jset.n : 0 },
 		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }

@@ -4,29 +4,66 @@
 // arithmetic include/nudge_b200.h states, and k_joint_solve applies them with the row update of k_user_rows (row_apply), one thread per joint
 // and one launch per joint level (level_rows over the joints' bodies).  The device table holds the joints by level, upload order within one;
 // each entry's type word also carries the offset of the joint's first row (type | offset << 2).  The parameters live in the table, the
-// accumulated impulses in the rows, which k_joint_rows rewrites around them.  Included at the end of nb_api.cu.
+// accumulated impulses in the rows, which k_joint_rows rewrites around them.
+// Drives (nb_upload_joint_drives; DESIGN.md section 8.17) are one more table, JointDrive per joint in table order, that both kernels take as
+// an argument (null without a drive set).  A drive's rows (motor, lower, upper) sit after all joints' own rows, so that the joint table and
+// the own rows' offsets are the same with and without drives; k_joint_solve applies them after the joint's own rows.  The break test and the
+// broken flag live in k_joint_rows.  Included at the end of nb_api.cu.
 #pragma once
 
 __host__ __device__ __forceinline__ u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
+__host__ __device__ __forceinline__ u32 drive_row_count(u32 flags) { return (flags & NB_JOINT_MOTOR ? 1u : 0u) + (flags & NB_JOINT_LIMIT ? 2u : 0u); }
 
 NB_DEV f3 neg3(f3 a) { return mk3(-a.x, -a.y, -a.z); }
 // Writes one row around its accumulated impulse.
-NB_DEV void joint_row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float bias) {
+NB_DEV void joint_row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float bias, float lo = -INFINITY, float hi = INFINITY) {
 	nb_constraint_row r;
 	r.a = j.a; r.b = j.b;
 	r.lin_a[0] = lin_a.x; r.lin_a[1] = lin_a.y; r.lin_a[2] = lin_a.z; r.ang_a[0] = ang_a.x; r.ang_a[1] = ang_a.y; r.ang_a[2] = ang_a.z;
 	r.lin_b[0] = lin_b.x; r.lin_b[1] = lin_b.y; r.lin_b[2] = lin_b.z; r.ang_b[0] = ang_b.x; r.ang_b[1] = ang_b.y; r.ang_b[2] = ang_b.z;
-	r.bias = bias; r.lo = -INFINITY; r.hi = INFINITY; r.impulse = row->impulse; r.softness = j.softness; r.reserved = 0.0f;
+	r.bias = bias; r.lo = lo; r.hi = hi; r.impulse = row->impulse; r.softness = j.softness; r.reserved = 0.0f;
 	*row = r;
 }
+// A broken joint's row: everything zero but a and b.
+NB_DEV void joint_row_zero(nb_constraint_row* row, const nb_joint& j) {
+	nb_constraint_row r;
+	memset(&r, 0, sizeof(r));
+	r.a = j.a; r.b = j.b;
+	*row = r;
+}
+// A limit row's bias: speculative while the coordinate is inside (C > 0), Baumgarte once past the bound.
+NB_DEV float limit_bias(float C, float dt, float k) { return C > 0.0f ? C / dt : k * C; }
 
-// One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints).
-__global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints, u32 n, const nb_transform* xf, float dt, nb_constraint_row* rows) {
+// The break test of a BREAKABLE joint on the impulses the previous step left in its rows (own rows at `row`, appended ones at `drow`).
+NB_DEV bool joint_breaks(const nb_constraint_row* row, const nb_constraint_row* drow, u32 type, u32 flags, const JointDrive& d, float dt) {
+	float P = 0.0f, A = 0.0f;
+	for (u32 r = 0; r < joint_row_count(type); ++r) { const float x = row[r].impulse; if (type == NB_JOINT_DISTANCE || r < 3) P = P + x * x; else A = A + x * x; }
+	for (u32 r = 0; r < drive_row_count(flags); ++r) { const float x = drow[r].impulse; if (type == NB_JOINT_DISTANCE) P = P + x * x; else A = A + x * x; }
+	const float f = d.break_force * dt, t = d.break_torque * dt;
+	return P > f * f || A > t * t;
+}
+
+// One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints), and with a drive table its drive's rows.
+__global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints, u32 n, const nb_transform* xf, float dt, nb_constraint_row* rows, JointDrive* drives) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const nb_joint j = joints[i];
 		const u32 type = j.type & 3u;
 		nb_constraint_row* row = rows + (j.type >> 2);
 		const float k = j.beta / dt;
+		u32 flags = 0;
+		nb_constraint_row* drow = rows;
+		JointDrive d;
+		if (drives) {
+			d = drives[i];
+			flags = d.flags; drow = rows + d.row;
+			bool broken = d.broken != 0;
+			if (!broken && (flags & NB_JOINT_BREAKABLE) && joint_breaks(row, drow, type, flags, d, dt)) { broken = true; drives[i].broken = 1u; }
+			if (broken) {
+				for (u32 r = 0; r < joint_row_count(type); ++r) joint_row_zero(row + r, j);
+				for (u32 r = 0; r < drive_row_count(flags); ++r) joint_row_zero(drow + r, j);
+				continue;
+			}
+		}
 		const xform ta = ld_xform(xf, j.a);
 		const quat qa = mkq(ta.q);
 		const f3 zero = mk3(0.0f, 0.0f, 0.0f);
@@ -42,7 +79,14 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 		if (type == NB_JOINT_DISTANCE) {
 			const float dist = sqrtf(dot3(err, err));
 			const f3 dir = dist > 0.0f ? mul3(err, 1.0f / dist) : mk3(0.0f, 1.0f, 0.0f);
-			joint_row_put(row, j, dir, cross3(ra, dir), neg3(dir), neg3(cross3(rb, dir)), k * (dist - j.length));
+			const f3 ca = cross3(ra, dir), cb = neg3(cross3(rb, dir));
+			if (flags & NB_JOINT_LIMIT) {   // the own row stays in place with no force; the range rows push
+				joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length), 0.0f, 0.0f);
+				joint_row_put(drow + 0, j, dir, ca, neg3(dir), cb, limit_bias(dist - d.lower, dt, k), 0.0f, INFINITY);
+				joint_row_put(drow + 1, j, neg3(dir), neg3(ca), dir, neg3(cb), limit_bias(d.upper - dist, dt, k), 0.0f, INFINITY);
+				drives[i].position[0] = dist;
+			}
+			else joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length));
 			continue;
 		}
 		joint_row_put(row + 0, j, mk3(1.0f, 0.0f, 0.0f), mk3(0.0f, ra.z, -ra.y), mk3(-1.0f, 0.0f, 0.0f), mk3(0.0f, -rb.z, rb.y), k * err.x);
@@ -55,6 +99,18 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			const f3 t2 = cross3(u, t1);
 			joint_row_put(row + 3, j, zero, t1, zero, neg3(t1), -(k * dot3(c, t1)));
 			joint_row_put(row + 4, j, zero, t2, zero, neg3(t2), -(k * dot3(c, t2)));
+			const f3 nu = neg3(u);   // the hinge Jacobian: ang_a = -u, ang_b = u
+			if (flags & NB_JOINT_MOTOR) { const float lim = d.max_motor_torque * dt; joint_row_put(drow++, j, zero, nu, zero, u, -d.motor_speed, -lim, lim); }
+			if (flags & NB_JOINT_LIMIT) {
+				const quat rel = { ld3(j.rel_rotation), j.rel_rotation[3] };
+				quat q = qmul(qa, rel);
+				if (j.b) { const quat cb = { neg3(qb.v), qb.s }; q = qmul(q, cb); }
+				if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
+				const float sh = -dot3(q.v, u), ch = q.s;
+				joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(2.0f * (sh * d.cl - ch * d.sl), dt, k), 0.0f, INFINITY);
+				joint_row_put(drow + 1, j, zero, u, zero, nu, limit_bias(2.0f * (d.su * ch - d.cu * sh), dt, k), 0.0f, INFINITY);
+				drives[i].position[0] = sh; drives[i].position[1] = ch;
+			}
 		}
 		else if (type == NB_JOINT_FIXED) {
 			const quat rel = { ld3(j.rel_rotation), j.rel_rotation[3] };
@@ -69,14 +125,22 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 }
 
 // One thread per joint of the level [begin, end): the joint's rows one after the other, the two bodies' momentum kept in registers across them.
+// With a drive table the drive's rows follow the joint's own.
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_solve(const nb_joint* joints, u32 begin, u32 end, nb_constraint_row* rows, nb_body_momentum* momentum,
-		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm) {
+		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm, const JointDrive* drives) {
 	for (u32 i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
 		const u32 packed = joints[i].type, first = packed >> 2, count = joint_row_count(packed & 3u);
 		RowBodies s = row_bodies_load(joints[i].a, joints[i].b, momentum, props, inertia, kind);
 		for (u32 r = first; r < first + count; ++r) {
 			const float next = row_apply(rows[r], s, warm);
 			if (!warm) rows[r].impulse = next;
+		}
+		if (drives) {
+			const u32 dfirst = drives[i].row, dcount = drive_row_count(drives[i].flags);
+			for (u32 r = dfirst; r < dfirst + dcount; ++r) {
+				const float next = row_apply(rows[r], s, warm);
+				if (!warm) rows[r].impulse = next;
+			}
 		}
 		row_bodies_store(s);
 	}
@@ -86,15 +150,23 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_solve(const nb_joint* joints
 static int launch_joints(nb_context* ctx, const float* dt, cudaStream_t st) {
 	const Launch L = mk_launch(ctx, st);
 	const JointSet& js = ctx->jset;
-	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p);
+	JointDrive* drives = ctx->dset.n ? ctx->drives.p : nullptr;
+	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p, drives);
 	for (u32 l = 0; l < js.levels; ++l)
 		launch_grid(L, k_joint_solve, GRID(js.level_off[l + 1] - js.level_off[l]), ctx->joints.p, js.level_off[l], js.level_off[l + 1], ctx->jrows.p, ctx->mom, ctx->props,
-			ctx->inertia, kin_table(ctx), dt ? 1 : 0);
+			ctx->inertia, kin_table(ctx), dt ? 1 : 0, (const JointDrive*)drives);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
-static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ++ctx->graph_epoch; } }
+static void drop_drives(nb_context* ctx) { if (ctx->dset.n) { ctx->dset = DriveSet(); ++ctx->graph_epoch; } }
+static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ctx->dset = DriveSet(); ++ctx->graph_epoch; } }
+
+// Whether a quaternion has unit length within the tolerance a HINGE LIMIT drive asks of its joint's rel_rotation.
+static bool unit_quat(const float* q) {
+	const double s = (double)q[0] * q[0] + (double)q[1] * q[1] + (double)q[2] * q[2] + (double)q[3] * q[3];
+	return fabs(s - 1.0) <= 1e-3;
+}
 
 // What nb_upload_joints refuses in a joint of a context with B bodies (also applied to a loaded state file); null if the joint is valid.
 static const char* joint_problem(const nb_joint& j, u32 B) {
@@ -118,7 +190,10 @@ static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st
 	if (!n) { drop_joints(ctx); return NB_OK; }
 	JointSet js;
 	std::vector<nb_body_pair> ab(n);
-	for (u32 i = 0; i < n; ++i) { ab[i].a = h[i].a; ab[i].b = h[i].b; js.structure.insert(js.structure.end(), { h[i].type, h[i].a, h[i].b }); }
+	for (u32 i = 0; i < n; ++i) {
+		ab[i].a = h[i].a; ab[i].b = h[i].b; js.structure.insert(js.structure.end(), { h[i].type, h[i].a, h[i].b });
+		js.unit_rel.push_back(unit_quat(h[i].rel_rotation) ? 1 : 0);
+	}
 	if (int r = level_rows(ctx, std::move(ab), js, "joints")) return r;
 	std::vector<nb_joint> table(n);
 	for (u32 i = 0; i < n; ++i) table[js.order[i]] = h[i];
@@ -130,7 +205,9 @@ static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st
 	GROW(ctx->joints, n, st); GROW(ctx->jrows, js.nrows, st);
 	CK(put_staged(ctx, ctx->joints.p, table.data(), sizeof(nb_joint) * (size_t)n, st));
 	CK(put_staged(ctx, ctx->jrows.p, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
-	// the levels are host values in nb_step's graph, the buffers its kernel arguments
+	// the levels are host values in nb_step's graph, the buffers its kernel arguments; the drives follow the structure (their rows stay
+	// beyond the joints' own, which the copy above leaves alone)
+	if (js.structure != ctx->jset.structure) drop_drives(ctx);
 	if (js.structure != ctx->jset.structure || before[0] != ctx->joints.p || before[1] != ctx->jrows.p) ++ctx->graph_epoch;
 	ctx->jset = std::move(js);
 	return NB_OK;
@@ -156,6 +233,117 @@ static int get_joints(nb_context* ctx, std::vector<nb_joint>& out, cudaStream_t 
 	return NB_OK;
 }
 
+// What nb_upload_joint_drives refuses in a drive of a joint set given by its structure ((type, a, b) per joint) and unit_rel; null if valid.
+static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* structure, const uint8_t* unit_rel) {
+	if (d.joint >= nj) return "a joint index at or beyond the joint count";
+	if (d.flags & ~(u32)(NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE)) return "an unknown flag";
+	const u32 type = structure[3 * (size_t)d.joint];
+	const u32 takes = type == NB_JOINT_HINGE ? NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : type == NB_JOINT_DISTANCE ? NB_JOINT_LIMIT | NB_JOINT_BREAKABLE : NB_JOINT_BREAKABLE;
+	if (d.flags & ~takes) return "a flag the joint's type does not take";
+	const float fields[] = { d.lower, d.upper, d.motor_speed, d.max_motor_torque, d.impulse[0], d.impulse[1], d.impulse[2], d.position };
+	for (float x : fields) if (!std::isfinite(x)) return "a field that is not finite";
+	for (float x : { d.break_force, d.break_torque }) if (!std::isfinite(x) && x != INFINITY) return "a threshold that is neither finite nor +inf";
+	if (d.max_motor_torque < 0.0f || d.break_force < 0.0f || d.break_torque < 0.0f) return "a negative torque or threshold";
+	if (d.broken > 1) return "broken is not 0 or 1";
+	if (d.flags & NB_JOINT_LIMIT) {
+		if (d.lower > d.upper) return "lower > upper";
+		const float pi = 3.14159265358979f;
+		if (type == NB_JOINT_HINGE && (d.lower < -pi || d.upper > pi)) return "a hinge limit outside [-pi, pi]";
+		if (type == NB_JOINT_DISTANCE && d.lower < 0.0f) return "a negative distance limit";
+		if (type == NB_JOINT_HINGE && !unit_rel[d.joint]) return "a HINGE LIMIT whose joint's rel_rotation is not of unit length";
+	}
+	return nullptr;
+}
+static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel) {
+	if (n && !h) { ctx->error = "null drive list"; return NB_ERR_ARGUMENT; }
+	for (u32 i = 0; i < n; ++i)
+		if (const char* p = drive_problem(h[i], nj, structure, unit_rel)) { ctx->error = "drive " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
+	std::vector<u32> joints(n);
+	for (u32 i = 0; i < n; ++i) joints[i] = h[i].joint;
+	std::sort(joints.begin(), joints.end());
+	for (u32 i = 1; i < n; ++i)
+		if (joints[i] == joints[i - 1]) { ctx->error = "two drives on joint " + std::to_string(joints[i]); return NB_ERR_ARGUMENT; }
+	return NB_OK;
+}
+
+// Installs n checked drives in place of the set: the table (one entry per joint in table order, with the limits' half-angle pairs) and the
+// appended rows holding the uploaded impulses, after the joints' own rows.
+static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStream_t st) {
+	if (!n) { drop_drives(ctx); return NB_OK; }
+	const JointSet& js = ctx->jset;
+	std::vector<u32> by_joint(n);
+	for (u32 i = 0; i < n; ++i) by_joint[i] = i;
+	std::sort(by_joint.begin(), by_joint.end(), [&](u32 x, u32 y) { return h[x].joint < h[y].joint; });
+	DriveSet ds;
+	ds.n = n;
+	std::vector<int> at(js.n, -1);   // table position -> drive
+	for (u32 i : by_joint) { ds.structure.insert(ds.structure.end(), { h[i].joint, h[i].flags }); at[js.order[h[i].joint]] = (int)i; }
+	std::vector<JointDrive> table(js.n);
+	memset(table.data(), 0, sizeof(JointDrive) * table.size());
+	std::vector<nb_constraint_row> rows;
+	for (u32 p = 0; p < js.n; ++p) {
+		if (at[p] < 0) continue;
+		const nb_joint_drive& d = h[at[p]];
+		JointDrive& e = table[p];
+		e.flags = d.flags; e.row = js.nrows + (u32)rows.size(); e.lower = d.lower; e.upper = d.upper;
+		if ((d.flags & NB_JOINT_LIMIT) && js.structure[3 * (size_t)d.joint] == NB_JOINT_HINGE) {
+			e.sl = (float)sin(0.5 * d.lower); e.cl = (float)cos(0.5 * d.lower); e.su = (float)sin(0.5 * d.upper); e.cu = (float)cos(0.5 * d.upper);
+		}
+		e.motor_speed = d.motor_speed; e.max_motor_torque = d.max_motor_torque; e.break_force = d.break_force; e.break_torque = d.break_torque;
+		e.broken = d.broken;
+		for (u32 k = 0; k < 3; ++k) {
+			if (!(d.flags & (k ? NB_JOINT_LIMIT : NB_JOINT_MOTOR))) continue;
+			nb_constraint_row r;
+			memset(&r, 0, sizeof(r));
+			r.impulse = d.impulse[k];
+			rows.push_back(r);
+		}
+	}
+	ds.nrows = (u32)rows.size();
+	const void* before[2] = { ctx->drives.p, ctx->jrows.p };
+	GROW(ctx->drives, js.n, st);
+	const size_t need = (size_t)js.nrows + ds.nrows;
+	if (need > ctx->jrows.cap) {   // a larger row buffer keeps the joints' own rows and their impulses
+		DevBuf<nb_constraint_row> b;
+		if (int r = b.alloc(ctx, need)) return r;
+		CK(cudaMemcpyAsync(b.p, ctx->jrows.p, sizeof(nb_constraint_row) * js.nrows, cudaMemcpyDeviceToDevice, st));
+		CK(cudaStreamSynchronize(st));
+		std::swap(ctx->jrows, b);
+	}
+	CK(put_staged(ctx, ctx->drives.p, table.data(), sizeof(JointDrive) * table.size(), st));
+	CK(put_staged(ctx, ctx->jrows.p + js.nrows, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
+	// the drive table is an argument of the joint kernels, null without a set; the structure decides which rows k_joint_solve applies
+	if (ds.structure != ctx->dset.structure || before[0] != ctx->drives.p || before[1] != ctx->jrows.p) ++ctx->graph_epoch;
+	ctx->dset = std::move(ds);
+	return NB_OK;
+}
+
+// The drives in joint-index order with their rows' current impulses, broken flags and positions.  Synchronises.
+static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStream_t st) {
+	const JointSet& js = ctx->jset;
+	const DriveSet& ds = ctx->dset;
+	out.resize(ds.n);
+	if (!ds.n) return NB_OK;
+	std::vector<JointDrive> table(js.n);
+	std::vector<nb_constraint_row> rows(ds.nrows);
+	CK(cudaMemcpyAsync(table.data(), ctx->drives.p, sizeof(JointDrive) * table.size(), cudaMemcpyDeviceToHost, st));
+	if (ds.nrows) CK(cudaMemcpyAsync(rows.data(), ctx->jrows.p + js.nrows, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	for (u32 m = 0; m < ds.n; ++m) {
+		const u32 joint = ds.structure[2 * (size_t)m];
+		const JointDrive& e = table[js.order[joint]];
+		nb_joint_drive& d = out[m];
+		memset(&d, 0, sizeof(d));
+		d.joint = joint; d.flags = e.flags; d.lower = e.lower; d.upper = e.upper; d.motor_speed = e.motor_speed; d.max_motor_torque = e.max_motor_torque;
+		d.break_force = e.break_force; d.break_torque = e.break_torque; d.broken = e.broken;
+		u32 r = e.row - js.nrows;
+		for (u32 k = 0; k < 3; ++k) if (e.flags & (k ? NB_JOINT_LIMIT : NB_JOINT_MOTOR)) d.impulse[k] = rows[r++].impulse;
+		if (e.flags & NB_JOINT_LIMIT)
+			d.position = js.structure[3 * (size_t)joint] == NB_JOINT_HINGE ? (float)(2.0 * atan2((double)e.position[0], (double)e.position[1])) : e.position[0];
+	}
+	return NB_OK;
+}
+
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_wake(const u32* bodies, u32 n, uint8_t* idle) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idle[bodies[i]] = 0;
 }
@@ -177,6 +365,25 @@ int nb_download_joints(nb_context* ctx, nb_joint* h, uint32_t capacity, uint32_t
 	std::vector<nb_joint> joints;
 	if (int r = get_joints(ctx, joints, (cudaStream_t)stream)) return r;
 	std::copy(joints.begin(), joints.end(), h);
+	return NB_OK;
+}
+
+int nb_upload_joint_drives(nb_context* ctx, const nb_joint_drive* h, uint32_t n, void* stream) {
+	NB_RANGE("nb_upload_joint_drives");
+	const JointSet& js = ctx->jset;
+	if (int r = check_drives(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data())) return r;
+	return set_drives(ctx, h, n, (cudaStream_t)stream);
+}
+
+int nb_download_joint_drives(nb_context* ctx, nb_joint_drive* h, uint32_t capacity, uint32_t* count, void* stream) {
+	NB_RANGE("nb_download_joint_drives");
+	const u32 n = ctx->dset.n;
+	if (count) *count = n;
+	if (capacity < n) { ctx->error = "host drive array too small: " + std::to_string(n) + " drives"; return NB_ERR_CAPACITY; }
+	if (n && !h) { ctx->error = "null drive array"; return NB_ERR_ARGUMENT; }
+	std::vector<nb_joint_drive> drives;
+	if (int r = get_drives(ctx, drives, (cudaStream_t)stream)) return r;
+	std::copy(drives.begin(), drives.end(), h);
 	return NB_OK;
 }
 

@@ -2,7 +2,7 @@
 // section 8.12).
 //
 // A snapshot is the context's between-steps state in HBM: the sections of a state file (state_sections, nb_state_api.cuh) plus what a file
-// lacks, the user rows, the joint table and the joints' rows, the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
+// lacks, the user rows, the joint table, the joints' rows and the joint drive table, the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
 // (snapshot_sections).  Save and restore are one launch of k_snapshot_copy in opposite directions; the host side (counts, bits, table set,
 // the connections' host copy, the kinematic set, the rows' levelling) is kept in the snapshot and installed by install_state.
 // Every section but the user rows, the joints and the overlap list has its room at the context's capacities in one arena, laid out once from the
@@ -52,9 +52,10 @@ struct nb_snapshot {
 	u32* words;
 	DevBuf<nb_constraint_row> rows;                  // user rows in device order
 	DevBuf<uint4> overlaps;                          // the sensor overlap list
-	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows
+	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows (the drives' appended rows included)
+	DevBuf<JointDrive> drives;                                  // the joint drive table
 	// the host side at the save
-	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset;
+	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset; DriveSet dset;
 };
 
 // A snapshot section: the context's buffer, the snapshot's copy, and the counter word (>= 0) that holds the element count on the device.
@@ -65,6 +66,7 @@ struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool presen
 // null the snapshot pointers are offsets into the arena, and there are no rows or joints.
 static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 conn_probe) {
 	const JointSet none, &js = s ? s->jset : none;
+	const DriveSet dnone, &ds = s ? s->dset : dnone;
 	const u32 nrows = s ? s->urow_set.n : 0;
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
@@ -76,11 +78,12 @@ static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapsho
 	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s ? s->words + j : nullptr, 4, 1, true, -1 });
 	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), nrows, nrows != 0, -1 });
 	p.push_back({ ctx->joints.p, s ? s->joints.p : nullptr, sizeof(nb_joint), js.n, js.n != 0, -1 });
-	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), js.nrows, js.n != 0, -1 });
+	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), (size_t)js.nrows + ds.nrows, js.n != 0, -1 });
+	p.push_back({ ctx->drives.p, s ? s->drives.p : nullptr, sizeof(JointDrive), js.n, ds.n != 0, -1 });
 	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
 	return p;
 }
-static const size_t kSnapFixed = 19 + 2;   // the state file's sections, the kind bytes and the key list: the sections in the arena
+static const size_t kSnapFixed = 20 + 2;   // the state file's 20 sections, the kind bytes and the key list: the sections in the arena
 
 // The table of one copy.  save: context -> snapshot; restore: snapshot -> context, with the overlap list also copied to the current list
 // and its length to the current count (nb_download_sensor_overlaps returns what it returned at the save).  A device count is read on the
@@ -162,10 +165,10 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	JOIN_UPLOADS();   // the copy reads the momentum and property rows
 	// grown: the only save that synchronises and allocates
 	GROW(s->rows, ctx->urow_set.n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
-	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, ctx->jset.nrows, st);
+	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, (size_t)ctx->jset.nrows + ctx->dset.nrows, st); GROW(s->drives, ctx->dset.n ? ctx->jset.n : 0, st);
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
-	s->urow_set = ctx->urow_set; s->jset = ctx->jset;
+	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset;
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, true, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
@@ -183,8 +186,8 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->shape.has_frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
 	if (!s->shape.kin.empty()) ALLOC(ctx->kind, ctx->cfg.max_bodies);
 	GROW(ctx->urows, s->urow_set.n, st);
-	const void* joint_bufs[2] = { ctx->joints.p, ctx->jrows.p };
-	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, s->jset.nrows, st);
+	const void* joint_bufs[3] = { ctx->joints.p, ctx->jrows.p, ctx->drives.p };
+	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, (size_t)s->jset.nrows + s->dset.nrows, st); GROW(ctx->drives, s->dset.n ? s->jset.n : 0, st);
 	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, false, t); if (r) return r; }
@@ -194,7 +197,8 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	// the row and joint levels are host values in the graph, the joint buffers its kernel arguments
 	if (s->urow_set.n != ctx->urow_set.n || s->urow_set.level_off != ctx->urow_set.level_off) ++ctx->graph_epoch;
 	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
-	ctx->urow_set = s->urow_set; ctx->jset = s->jset;
+	else if (s->dset.structure != ctx->dset.structure || joint_bufs[2] != ctx->drives.p) ++ctx->graph_epoch;
+	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->dset = s->dset;
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;
 	return NB_OK;

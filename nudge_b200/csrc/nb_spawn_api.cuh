@@ -200,17 +200,24 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	// the kept joints with their current impulses, remapped, and the kept dynamic bodies that lose a joint
 	cudaStream_t st = (cudaStream_t)stream;
 	std::vector<nb_joint> old_joints, joints;
-	std::vector<u32> joint_wake;
+	std::vector<u32> joint_wake, joint_new(ctx->jset.n, ~0u);   // joint_new: old joint index -> new one (~0u: deleted)
+	std::vector<nb_joint_drive> drives;
 	if (int r = get_joints(ctx, old_joints, st)) return r;
-	for (nb_joint j : old_joints) {
+	if (int r = get_drives(ctx, drives, st)) return r;
+	for (u32 i = 0; i < old_joints.size(); ++i) {
+		nb_joint j = old_joints[i];
 		if (removed(j.a) || removed(j.b)) {
 			const u32 other = removed(j.a) ? j.b : j.a;
 			if (other && !removed(other) && !std::binary_search(kin.begin(), kin.end(), remap(other))) joint_wake.push_back(remap(other));
 			continue;
 		}
 		j.a = remap(j.a); j.b = remap(j.b);
+		joint_new[i] = (u32)joints.size();
 		joints.push_back(j);
 	}
+	// the drives of the kept joints, renumbered, with their current impulses and broken flags
+	std::vector<nb_joint_drive> kept_drives;
+	for (nb_joint_drive d : drives) if (joint_new[d.joint] != ~0u) { d.joint = joint_new[d.joint]; kept_drives.push_back(d); }
 	const u32 nrows = kept.n;
 	const bool rows_changed = nrows != us.n;   // a deleted row can change the levels, which nb_step's graph holds
 	std::vector<u32> staging(list);   // the list, then the rows' gather permutation (new device position -> old one)
@@ -293,6 +300,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		launch_grid(L, k_joint_wake, GRID(joint_wake.size()), ctx->spawn_idx.p, (u32)joint_wake.size(), ctx->idle);
 	}
 	if (!old_joints.empty()) { int r = set_joints(ctx, joints.data(), (u32)joints.size(), st); if (r) return r; }
+	if (!drives.empty()) { int r = set_drives(ctx, kept_drives.data(), (u32)kept_drives.size(), st); if (r) return r; }
 	return build_conn_lookup(ctx, st);
 }
 

@@ -16,10 +16,11 @@
 //   kinematic (body indices, ascending)            4            reserved[4]      reserved[4] != 0
 //   body forces (nb_body_force rows, body = row)   48           bodies           reserved[5] != 0
 //   joints (nb_joint, upload order, current impulses) 112        reserved[6]      reserved[6] != 0
+//   joint drives (nb_joint_drive, joint order)      56           reserved[7]      reserved[7] != 0
 // Each version defines more reserved words: version 2 reserved[0] = filter flags and reserved[1]; version 3 reserved[2] = 1 and
 // reserved[3] = max_sensor_pairs; version 4 reserved[2] = 0 or 1 and reserved[4] >= 1; version 5 reserved[2] = 0 or 1, reserved[4] >= 0 and
-// reserved[5] = 1; version 6 reserved[2] and reserved[5] = 0 or 1, reserved[4] >= 0 and reserved[6] >= 1.  A context writes version 6 with
-// joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
+// reserved[5] = 1; version 6 reserved[2] and reserved[5] = 0 or 1, reserved[4] >= 0 and reserved[6] >= 1; version 7 as 6 and reserved[7] >= 1.
+// A context writes version 7 with joint drives, else 6 with joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
 // filter table or flags, else 1.  Every version loads; words a version does not define are ignored, and a file without a table or flags
 // removes the context's.  A kinematic body's velocities are its momentum row.
 #pragma once
@@ -35,19 +36,21 @@ static bool state_header_read(FILE* f, NbStateHeader& h) {
 	if (h.version < 4) h.reserved[4] = 0;
 	if (h.version < 5) h.reserved[5] = 0;
 	if (h.version < 6) h.reserved[6] = 0;
+	if (h.version < 7) h.reserved[7] = 0;
 	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1) ||
-		   (h.version == 5 && h.reserved[2] <= 1 && h.reserved[5] == 1) || (h.version == 6 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1);
+		   (h.version == 5 && h.reserved[2] <= 1 && h.reserved[5] == 1) || (h.version == 6 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1) ||
+		   (h.version == 7 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1 && h.reserved[7] >= 1);
 }
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
 // `host` when it is given and then copies to `dev` when that is given.  word >= 0: a context holds the element count in counts[word] (a
 // file holds it in the header; a snapshot copies it on the device, nb_snapshot_api.cuh).
 struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; int word; };
-struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc, joints; };
+struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc, joints, drives; };
 
 // The sections of the file with header `h`, in file order.  A load keeps in `hc` the momentum rows (the kinematic velocities), the tags
-// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices, the body force rows and the joints
-// (checked before they are copied to the device); a save writes the kinematic indices from hc.kin and the joints from hc.joints.  Snapshots extend this list (snapshot_sections).
+// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices, the body force rows, the joints
+// and their drives (checked before they are copied to the device); a save writes the kinematic indices, the joints and the drives from hc.  Snapshots extend this list (snapshot_sections).
 static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, StateHostCopies& hc, bool load) {
 	const size_t K = (size_t)h.boxes + h.spheres;
 	return {
@@ -65,6 +68,7 @@ static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHe
 		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0, -1 },
 		{ load ? nullptr : ctx->frc, &hc.frc, sizeof(nb_body_force), h.bodies, h.reserved[5] != 0, -1 },
 		{ nullptr, &hc.joints, sizeof(nb_joint), h.reserved[6], h.reserved[6] != 0, -1 },
+		{ nullptr, &hc.drives, sizeof(nb_joint_drive), h.reserved[7], h.reserved[7] != 0, -1 },
 	};
 }
 
@@ -73,12 +77,12 @@ static NbStateHeader state_header_of(const nb_context* ctx, u32 cache) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
 	if (ctx->has_frc) h.reserved[5] = 1;
-	h.reserved[6] = ctx->jset.n;
+	h.reserved[6] = ctx->jset.n; h.reserved[7] = ctx->dset.n;
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = cache; h.solver_mode = (u32)ctx->solver_mode;
 	return h;
 }
@@ -167,6 +171,9 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	std::vector<nb_joint> joints;
 	if ((r = get_joints(ctx, joints, st))) { fclose(f); return r; }
 	hc.joints.assign(reinterpret_cast<const unsigned char*>(joints.data()), reinterpret_cast<const unsigned char*>(joints.data() + joints.size()));
+	std::vector<nb_joint_drive> drives;
+	if ((r = get_drives(ctx, drives, st))) { fclose(f); return r; }
+	hc.drives.assign(reinterpret_cast<const unsigned char*>(drives.data()), reinterpret_cast<const unsigned char*>(drives.data() + drives.size()));
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
 	for (const StateSection& s : state_sections(ctx, h, hc, false)) if (s.present) ok = ok && state_put(f, s, tmp, st);
@@ -222,6 +229,11 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	for (u32 i = 0; ok && h.reserved[5] && i < h.bodies; ++i) ok = frc[i].body == i && !body_force_problem(frc[i]);
 	const nb_joint* joints = reinterpret_cast<const nb_joint*>(hc.joints.data());
 	ok = ok && check_joints(ctx, joints, h.reserved[6], h.bodies) == NB_OK;
+	// the drives against the file's joints, through the upload's checks
+	const nb_joint_drive* drives = reinterpret_cast<const nb_joint_drive*>(hc.drives.data());
+	std::vector<u32> structure; std::vector<uint8_t> unit_rel;
+	for (u32 i = 0; ok && i < h.reserved[6]; ++i) { structure.insert(structure.end(), { joints[i].type, joints[i].a, joints[i].b }); unit_rel.push_back(unit_quat(joints[i].rel_rotation) ? 1 : 0); }
+	ok = ok && check_drives(ctx, drives, h.reserved[7], h.reserved[6], structure.data(), unit_rel.data()) == NB_OK;
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->scene_edited = false;   // the loaded scene replaces an edited one
@@ -233,7 +245,9 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	shape.kin.assign(idx, idx + kin.size());
 	const StateFileTables file = { hc.sensor.data(), kin.data(), frc };
 	{ int r = install_state(ctx, shape, &file, st); if (r) return r; }
+	drop_drives(ctx);   // a file without drives removes them, also where its joints have the context's structure
 	{ int r = set_joints(ctx, joints, h.reserved[6], st); if (r) return r; }
+	{ int r = set_drives(ctx, drives, h.reserved[7], st); if (r) return r; }
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
