@@ -472,32 +472,27 @@ class Sim(abi.HostState):
         """rays: abi.RAY rows; returns their abi.RAY_HIT rows (collider = body = tag = RAY_NO_HIT for a miss).  flags: RAY_SENSORS also tests
         sensor colliders.  device_ptrs=(rays_ptr, hits_ptr) with n: device buffers of n rays and n hits instead; the call is then asynchronous on
         the Sim's stream (capturable after a first call) and returns None."""
-        if device_ptrs is not None:
-            if n is None:
-                raise ValueError("Sim.raycast with device_ptrs needs n, the number of rays (and hits) the two device buffers hold")
-            self._ck(self.lib.nb_raycast(self.ctx, C.c_void_p(device_ptrs[0]), int(n), C.c_void_p(device_ptrs[1]), int(flags), 1, self.stream), "nb_raycast")
-            return None
-        r = np.ascontiguousarray(np.asarray(rays, abi.RAY).reshape(-1))
-        out = np.zeros(len(r), abi.RAY_HIT)
-        P = lambda a: abi.ptr(a) if len(a) else None
-        self._ck(self.lib.nb_raycast(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_raycast")
-        return out
+        return self._sweep("raycast", "rays", abi.RAY, rays, flags, device_ptrs, n)
 
     # ---- shape casts (nb_shapecast, include/nudge_b200.h): where a moving sphere or oriented box first touches a collider ----
     def shapecast(self, casts, flags=0, device_ptrs=None, n=None):
         """casts: abi.SHAPE_CAST rows; returns their abi.RAY_HIT rows (collider = body = tag = RAY_NO_HIT for a miss).  flags:
         SHAPECAST_SENSORS also tests sensor colliders.  device_ptrs=(casts_ptr, hits_ptr) with n: device buffers of n casts and n hits
         instead; the call is then asynchronous on the Sim's stream (capturable after a first scene query) and returns None."""
+        return self._sweep("shapecast", "casts", abi.SHAPE_CAST, casts, flags, device_ptrs, n)
+
+    def _sweep(self, name, what, dtype, rows, flags, device_ptrs, n):
+        """Sim.raycast and Sim.shapecast: nb_<name> on `what` (rows of dtype) into as many abi.RAY_HIT rows."""
+        fn = getattr(self.lib, "nb_" + name)
         if device_ptrs is not None:
             if n is None:
-                raise ValueError("Sim.shapecast with device_ptrs needs n, the number of casts (and hits) the two device buffers hold")
-            self._ck(self.lib.nb_shapecast(self.ctx, C.c_void_p(device_ptrs[0]), int(n), C.c_void_p(device_ptrs[1]), int(flags), 1, self.stream),
-                     "nb_shapecast")
+                raise ValueError("Sim.%s with device_ptrs needs n, the number of %s (and hits) the two device buffers hold" % (name, what))
+            self._ck(fn(self.ctx, C.c_void_p(device_ptrs[0]), int(n), C.c_void_p(device_ptrs[1]), int(flags), 1, self.stream), "nb_" + name)
             return None
-        c = np.ascontiguousarray(np.asarray(casts, abi.SHAPE_CAST).reshape(-1))
-        out = np.zeros(len(c), abi.RAY_HIT)
+        r = np.ascontiguousarray(np.asarray(rows, dtype).reshape(-1))
+        out = np.zeros(len(r), abi.RAY_HIT)
         P = lambda a: abi.ptr(a) if len(a) else None
-        self._ck(self.lib.nb_shapecast(self.ctx, P(c), len(c), P(out), int(flags), 0, self.stream), "nb_shapecast")
+        self._ck(fn(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_" + name)
         return out
 
     # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----

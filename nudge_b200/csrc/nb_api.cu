@@ -67,6 +67,14 @@ struct QueryScratch {
 	FrontEnd front; SortBuffers sb; u32* counts; DevBuf<nb_ray> rays; DevBuf<nb_shape_cast> casts; DevBuf<nb_ray_hit> hits; bool ready;
 	DevBuf<u64> okeys[2]; SortBuffers osb; DevBuf<nb_overlap_query> oq; DevBuf<nb_overlap_hit> oh; DevBuf<u32> ooff;
 };
+// The slots of QueryScratch::counts the queries keep for themselves, in slots of nb_collide's counters the front end has no other use for.
+// The fallbacks (queries that tested every collider instead of walking the grid, read by nb_debug_read) are summed over the context's
+// calls, so none may be a slot launch_front_end writes or resets.  The overlap call's append cursor of its hit keys (nb_radix_sort lowers it
+// to the capacity) and its total of hits (never lowered) start each call from k_reset_collide's zero.
+enum {
+	CNT_RAY_FALLBACKS = CNT_TMP, CNT_OVERLAP_FALLBACKS = CNT_SURV, CNT_SHAPECAST_FALLBACKS = CNT_SENSOR_TMP + 1,
+	CNT_OVERLAP_KEYS = CNT_PAIRS, CNT_OVERLAP_TOTAL = CNT_SENSOR_PAIRS
+};
 
 struct nb_context {
 	nb_config cfg;
@@ -1219,28 +1227,22 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 	if (!strcmp(name, "graph_records")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = (u32)ctx->graph_records; if (bytes) *bytes = 4; return NB_OK; }
 	// the device bytes the context and its snapshots hold now, as a uint64_t
 	if (!strcmp(name, "device_bytes")) { if (max_bytes < 8) return NB_ERR_ARGUMENT; *(uint64_t*)dst = ctx->device_bytes; if (bytes) *bytes = 8; return NB_OK; }
-	// nb_raycast's own counters (0 before the first call): rays that tested every collider instead of walking the grid, summed over the
-	// context's calls, and the grid level of the last call's build
-	if (!strcmp(name, "ray_fallbacks") || !strcmp(name, "ray_grid_level")) {
-		if (max_bytes < 4) return NB_ERR_ARGUMENT;
-		u32 v = 0;
-		if (ctx->query.ready) {
-			CK(cudaMemcpyAsync(&v, ctx->query.counts + (name[4] == 'f' ? CNT_TMP : CNT_GRID_LEVEL), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-			CK(cudaStreamSynchronize((cudaStream_t)stream));
+	// the scene queries' own counters (0 before the first query): rays, overlap queries and shape casts that tested every collider instead
+	// of walking the grid, summed over the context's calls, and the grid level of the last query's build
+	const struct { const char* name; u32 slot; } query_counters[] = {
+		{ "ray_fallbacks", CNT_RAY_FALLBACKS }, { "ray_grid_level", CNT_GRID_LEVEL }, { "overlap_fallbacks", CNT_OVERLAP_FALLBACKS },
+		{ "shapecast_fallbacks", CNT_SHAPECAST_FALLBACKS },
+	};
+	for (const auto& e : query_counters)
+		if (!strcmp(name, e.name)) {
+			if (max_bytes < 4) return NB_ERR_ARGUMENT;
+			u32 v = 0;
+			if (ctx->query.ready) {
+				CK(cudaMemcpyAsync(&v, ctx->query.counts + e.slot, 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+				CK(cudaStreamSynchronize((cudaStream_t)stream));
+			}
+			*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
 		}
-		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
-	}
-	// nb_overlap's and nb_shapecast's counters (0 before the first query): queries or casts that tested every collider instead of walking
-	// the grid, summed over the context's calls (CNT_SHAPECAST_FALLBACKS, nb_query_api.cuh, is the slot after CNT_SENSOR_TMP)
-	if (!strcmp(name, "overlap_fallbacks") || !strcmp(name, "shapecast_fallbacks")) {
-		if (max_bytes < 4) return NB_ERR_ARGUMENT;
-		u32 v = 0;
-		if (ctx->query.ready) {
-			CK(cudaMemcpyAsync(&v, ctx->query.counts + (name[0] == 'o' ? CNT_SURV : CNT_SENSOR_TMP + 1), 4, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-			CK(cudaStreamSynchronize((cudaStream_t)stream));
-		}
-		*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
-	}
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	// the last collide's broadphase: the grid level (cell edge 2^level quantised units) and how many colliders went to k_large_pairs
 	if (!strcmp(name, "grid_level")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_GRID_LEVEL]; if (bytes) *bytes = 4; return NB_OK; }
