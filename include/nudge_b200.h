@@ -571,7 +571,9 @@ int nb_stream_synchronize(nb_context*, void* stream);
  * (the table's B rows after the kinematic section); loading a file of versions 1-4 removes the context's table.  A context with joints
  * writes version 6 (the joints after the force table); loading a file of versions 1-5 removes the context's joints.  A context with joint
  * drives writes version 7 (reserved[7] = the drive count, the nb_joint_drive rows after the joints); loading a file of versions 1-6 removes
- * the context's drives. */
+ * the context's drives.  A context with a continuous-collision set writes version 8 (a 16-byte header extension holding the entry count,
+ * the nb_ccd_body rows last); loading a file of versions 1-7 removes the context's set.  Without a set a context writes what it wrote
+ * before version 8 existed, byte for byte. */
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);
@@ -756,6 +758,52 @@ typedef struct {
 } nb_shape_cast;                /* 80 bytes */
 enum nb_shapecast_flags { NB_SHAPECAST_SENSORS = 1 };   /* also test sensor colliders (default: they are skipped) */
 int nb_shapecast(nb_context*, const nb_shape_cast* casts, uint32_t n, nb_ray_hit* hits, uint32_t flags, int on_device, void* stream);
+
+/* Continuous collision for fast bodies (bullets, dropped crates, debris; DESIGN.md section 8.18): CCD motion clamping, answered on the
+ * device inside the step.  The step is otherwise discrete: a body that moves further in one step than what it should hit is thick passes
+ * through it.  nb_upload_ccd_bodies replaces the set of listed bodies (n = 0 removes it; stored ascending by body);
+ * nb_download_ccd_bodies returns it in that order (*count = its size; NB_ERR_CAPACITY when capacity is smaller, nothing written).
+ * In every nb_advance (a stage call or inside nb_step, both solver modes) each listed body that the step advances (awake: its island is
+ * active in the last nb_collide, and not kinematic) is handled as follows, with p = its position as nb_advance finds it and v = its
+ * velocity after the solver:  d = (v.x*dt, v.y*dt, v.z*dt), the products the advance adds.  If (d.x*d.x + d.y*d.y) + d.z*d.z >
+ * motion_threshold * motion_threshold and d is a valid direction for nb_shapecast with max_t = 1 (finite, not zero), a sphere of `radius`
+ * is cast from p along d with max_t = 1, with nb_shapecast's sphere arithmetic above (steps 0, 1 and 2, float32, no fused multiply-adds),
+ * against every collider at its pose of this step's nb_collide except:
+ *   - the body's own colliders;  sensor colliders;
+ *   - colliders failing Box2D's rule against (category, mask): (category & collider mask) != 0 and (collider category & mask) != 0, the
+ *     collider's words from nb_upload_collision_filters (every bit set without a table);
+ *   - with NB_FILTER_SKIP_CONNECTED, colliders of a body connected to this one;
+ *   - colliders the sphere already touches at t = 0 (step 0 holds): unlike nb_shapecast they are not a t = 0 hit but are skipped, since
+ *     nb_collide gives the body a contact with them anyway (a body resting on the ground keeps moving along it);
+ *   - a hit at t = 0 on a collider step 0 does not hold for, unless d points into it: dot(g, d') < 0, with g the gap of nb_overlap's
+ *     sphere test and d' = qrot(conj(q), d) for a box (g = (gap(l.x, h.x), gap(l.y, h.y), gap(l.z, h.z)), l = qrot(conj(q), c - p),
+ *     gap(u, h) = u < -h ? u + h : (u > h ? u - h : 0)), g = c - p and d' = d for a sphere.  Where a clamp leaves the centre on a face, the
+ *     face slab of step 2 can count the start as inside while step 0, rounded the other way, does not; without this rule every later cast
+ *     from there would hit at t = 0, also one moving away from the face or along it.
+ * The hit is the smallest (bits of t) << 32 | collider among the rest.  With a hit the translation is ((v.x*dt) * t, (v.y*dt) * t,
+ * (v.z*dt) * t) in place of d (for t = 1 the same bits); the rotation, the velocity and the idle counter are integrated exactly as without
+ * a set.  So a clamped body stops where its swept sphere first touches something; with radius below the body's inscribed radius its collider
+ * then overlaps what it hit, and the next nb_collide gives an ordinary contact that the solver resolves.  Limitations: targets are taken at
+ * their pose before the advance (a moving target is not swept), rotation is not swept, and the remaining time after the impact is dropped.
+ * Refusals (NB_ERR_ARGUMENT, changing nothing; every entry checked on the host first): body 0, at or beyond the body count or kinematic; a
+ * body listed twice; a radius that is not finite or below 0; a NaN or negative threshold; a null list with n > 0; a context that
+ * nb_shard_create was called on.  nb_advance with a set refuses (NB_ERR_ARGUMENT, launching nothing) when no nb_collide ran since the last
+ * nb_advance: the collide's grid must describe this step's poses.  A body made kinematic after the upload keeps its entry but is not
+ * clamped while kinematic.  New radii, thresholds or filters for the same bodies keep nb_step's graph; another body list re-records it.
+ * nb_upload_bodies keeps the set while the body count is unchanged and removes it otherwise; nb_add_bodies adds no entries;
+ * nb_remove_bodies drops the removed bodies' entries and renumbers the rest.  Snapshots carry the set; nb_save_state writes it (state
+ * version 8) and nb_load_state installs it, a file of an older version removes it.  Not supported by nb_shard_step (NB_ERR_ARGUMENT).
+ * Launches: nb_step issues one more (the cast, k_ccd) with a set.  nb_debug_read("ccd_hits") returns, per entry of the last advance in set
+ * order, two uint32 (bits of t, collider), (1.0f, NB_RAY_NO_HIT) when the body was not clamped; nb_debug_read("ccd_fallbacks") the casts
+ * that tested every collider instead of walking the grid, summed over the context's advances. */
+typedef struct {
+	uint32_t body;
+	float radius;              /* the swept sphere, centred on the body's position; should not exceed the body's inscribed radius */
+	float motion_threshold;    /* cast only when the step's translation is longer than this; 0 = always, +inf = never */
+	uint16_t category, mask;   /* the collision filter the cast applies (nb_collision_filter's meaning) */
+} nb_ccd_body;                 /* 16 bytes */
+int nb_upload_ccd_bodies(nb_context*, const nb_ccd_body* host, uint32_t n, void* stream);   /* replaces the set; n = 0 removes it */
+int nb_download_ccd_bodies(nb_context*, nb_ccd_body* host, uint32_t capacity, uint32_t* count, void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

@@ -126,6 +126,8 @@ def load_library():
         lib.nb_raycast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         lib.nb_overlap.argtypes = [V, V, C.c_uint32, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         lib.nb_shapecast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
+        lib.nb_upload_ccd_bodies.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_download_ccd_bodies.argtypes = [V, V, C.c_uint32, V, V]
         _lib = lib
     return _lib
 
@@ -493,6 +495,22 @@ class Sim(abi.HostState):
         out = np.zeros(len(r), abi.RAY_HIT)
         P = lambda a: abi.ptr(a) if len(a) else None
         self._ck(fn(self.ctx, P(r), len(r), P(out), int(flags), 0, self.stream), "nb_" + name)
+        return out
+
+    # ---- continuous collision (nb_upload_ccd_bodies, include/nudge_b200.h): fast bodies stop where their swept sphere first hits ----
+    def upload_ccd_bodies(self, rows):
+        """rows: abi.CCD_BODY rows (or anything np.asarray turns into them, e.g. tuples (body, radius, motion_threshold, category, mask)), or
+        None / empty to remove the set.  Every step, each listed awake body whose translation is longer than its threshold casts its sphere
+        along it on the device and stops at the first collider it would reach.  Asynchronous; the array may be reused on return."""
+        r = np.ascontiguousarray(np.asarray(rows if rows is not None else [], abi.CCD_BODY).reshape(-1))
+        self._ck(self.lib.nb_upload_ccd_bodies(self.ctx, abi.ptr(r) if len(r) else None, len(r), self.stream), "nb_upload_ccd_bodies")
+
+    def download_ccd_bodies(self):
+        """The set as abi.CCD_BODY rows, ascending by body (none without a set)."""
+        n = C.c_uint32(0)
+        self.lib.nb_download_ccd_bodies(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there is no set)
+        out = np.zeros(n.value, abi.CCD_BODY)
+        self._ck(self.lib.nb_download_ccd_bodies(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_ccd_bodies")
         return out
 
     # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----

@@ -69,6 +69,10 @@ SHAPE_CAST = np.dtype([("shape", OVERLAP_QUERY), ("direction", "<f4", 3), ("max_
 assert SHAPE_CAST.itemsize == 80
 SHAPECAST_SENSORS = 1
 
+# nb_ccd_body (16 bytes): a body whose translation each step is clamped at the first hit of its swept sphere (continuous collision)
+CCD_BODY = np.dtype([("body", "<u4"), ("radius", "<f4"), ("motion_threshold", "<f4"), ("category", "<u2"), ("mask", "<u2")])
+assert CCD_BODY.itemsize == 16
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

@@ -75,6 +75,10 @@ enum {
 	CNT_RAY_FALLBACKS = CNT_TMP, CNT_OVERLAP_FALLBACKS = CNT_SURV, CNT_SHAPECAST_FALLBACKS = CNT_SENSOR_TMP + 1,
 	CNT_OVERLAP_KEYS = CNT_PAIRS, CNT_OVERLAP_TOTAL = CNT_SENSOR_PAIRS
 };
+// The step's counter slot of k_ccd's fallbacks (continuous collision, nb_ccd_api.cuh): summed over the context's advances, in a slot after
+// the scheduler's fall-back flags that nothing else writes.
+enum { CNT_CCD_FALLBACKS = CNT_SCHED_FB0 + 16 };
+static_assert((int)CNT_CCD_FALLBACKS < (int)CNT_EXT_HIST, "the fallback slot lies between the scheduler's flags and the extent histogram");
 
 struct nb_context {
 	nb_config cfg;
@@ -141,6 +145,10 @@ struct nb_context {
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
 	// joint drives (nb_upload_joint_drives, DESIGN.md section 8.17): the device table while dset.n, the rows appended after the joints' own in jrows
 	DevBuf<JointDrive> drives; DriveSet dset;
+	// continuous collision (nb_upload_ccd_bodies, DESIGN.md section 8.18, nb_ccd_api.cuh): ccd = the set (host copy, ascending by body) and
+	// ccd_rows its device copy; ccd_t = the advance's translation factor per body (max_bodies of them, 1 outside the set), allocated on the
+	// first upload; ccd_hits = (bits of t, collider) per entry of the last advance
+	std::vector<nb_ccd_body> ccd; DevBuf<nb_ccd_body> ccd_rows; float* ccd_t; DevBuf<uint2> ccd_hits;
 	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap, section 8.15) and shape casts
 	// (nb_shapecast, section 8.16)
 	QueryScratch query;
@@ -238,6 +246,9 @@ static int launch_user_rows(nb_context* ctx, int warm, cudaStream_t st);   // nb
 static int launch_joints(nb_context* ctx, const float* dt, cudaStream_t st);   // nb_joint_api.cuh
 static void drop_joints(nb_context* ctx);
 static void free_snapshots(nb_context* ctx);                               // nb_snapshot_api.cuh
+static int set_ccd(nb_context* ctx, std::vector<nb_ccd_body> set, cudaStream_t st);   // nb_ccd_api.cuh
+static int launch_ccd(nb_context* ctx, const Launch& L, float time_step);
+static const char* ccd_body_problem(const nb_ccd_body& e);
 // The stage calls that read the last nb_collide's outputs: refused after nb_add_bodies / nb_remove_bodies until the next collide
 #define NOT_AFTER_EDIT() do { if (ctx->scene_edited) { ctx->error = "the scene was edited (nb_add_bodies / nb_remove_bodies) since the last nb_collide"; return NB_ERR_ARGUMENT; } } while (0)
 
@@ -316,6 +327,7 @@ static int join_uploads(nb_context* ctx, cudaStream_t st) {
 static const uint8_t* kin_table(const nb_context* ctx) { return ctx->has_kin ? ctx->kind : nullptr; }
 static void drop_kinematic(nb_context* ctx) { if (ctx->has_kin) { ctx->has_kin = false; ctx->kin_list.clear(); ++ctx->graph_epoch; } }
 static void drop_body_forces(nb_context* ctx) { if (ctx->has_frc) { ctx->has_frc = false; ++ctx->graph_epoch; } }   // the step launches k_gravity_damping again
+static void drop_ccd(nb_context* ctx) { if (!ctx->ccd.empty()) { ctx->ccd.clear(); ++ctx->graph_epoch; } }   // the step launches k_advance<false> again
 
 // The checks of entry i of a body list (kinematic bodies, impulses, forces, removals): not body 0, the static world; below the body count;
 // and, unless kinematic_ok, not kinematic.  A refused entry is NB_ERR_ARGUMENT with the message "<list> <i>: body <b> ...".
@@ -616,7 +628,7 @@ int nb_lut_model_exact(const nb_context* ctx) { return ctx->lut_exact; }
 int nb_upload_bodies(nb_context* ctx, const nb_body_data* h, void* stream) {
 	NB_RANGE("nb_upload_bodies");
 	if (h->count > ctx->cfg.max_bodies) { ctx->error = "too many bodies"; return NB_ERR_CAPACITY; }
-	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); drop_joints(ctx); }   // the kinematic set, the force table and the joints belong to a body count
+	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); drop_joints(ctx); drop_ccd(ctx); }   // the kinematic set, the force table, the joints and the CCD set belong to a body count
 	ctx->B = h->count;
 	cudaStream_t st = (cudaStream_t)stream;
 	H2D(ctx->xf, h->transforms, h->count, nb_transform); H2D(ctx->idle, h->idle_counters, h->count, uint8_t);   // all the collision stage reads
@@ -1121,8 +1133,18 @@ int nb_update_cached_impulses(nb_context* ctx, void* stream) {
 int nb_advance(nb_context* ctx, float time_step, void* stream) {
 	NB_RANGE("nb_advance");
 	NOT_AFTER_EDIT();
+	if (!ctx->ccd.empty() && !ctx->in_step) {   // the cast walks the last collide's grid, which must describe this step's poses
+		ctx->error = "nb_advance: a continuous-collision set (nb_upload_ccd_bodies) needs an nb_collide since the last nb_advance";
+		return NB_ERR_ARGUMENT;
+	}
 	JOIN_UPLOADS();
-	launch_grid(mk_launch(ctx, stream), k_advance, GRID(ctx->B), ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts);
+	const Launch L = mk_launch(ctx, stream);
+	if (ctx->ccd.empty())
+		launch_grid(L, k_advance<false>, GRID(ctx->B), ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts, (const float*)nullptr);
+	else {   // the casts (nb_ccd_api.cuh), then the advance with their factors
+		if (int r = launch_ccd(ctx, L, time_step)) return r;
+		launch_grid(L, k_advance<true>, GRID(ctx->B), ctx->active_idx, ctx->xf, ctx->mom, ctx->idle, time_step, ctx->counts, (const float*)ctx->ccd_t);
+	}
 	ctx->in_step = false;
 	CK(cudaGetLastError());
 	return NB_OK;
@@ -1143,7 +1165,7 @@ static int step_solve(nb_context* ctx, uint32_t iterations, void* stream) {
 }
 
 // One sub-step (example/main.cpp:274-328), as a CUDA graph on a capturable stream (61 launches in parity mode, 3 more with contact events,
-// 6 more with sensor colliders).
+// 6 more with sensor colliders, 1 more with a continuous-collision set).
 int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity, float damping, void* stream) {
 	NB_RANGE("nb_step");
 	ctx->capture_joined = false;   // a capture records the event-wait node for nb_upload_bodies' side copy
@@ -1220,6 +1242,7 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ((size_t)ctx->jset.nrows + ctx->dset.nrows) },   // in table order: by joint level, upload order within one; then the drives' rows
 		{ "joint_drives", ctx->drives.p, ctx->dset.n ? sizeof(JointDrive) * (size_t)ctx->jset.n : 0 },
 		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
+		{ "ccd_hits", ctx->ccd_hits.p, sizeof(uint2) * ctx->ccd.size() },   // per entry of the last advance, in set order: (bits of t, collider)
 	};
 	if (!strcmp(name, "row_stride")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->cstride; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "graph_active")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = ctx->graph.exec != nullptr; if (bytes) *bytes = 4; return NB_OK; }
@@ -1243,6 +1266,8 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 			}
 			*(u32*)dst = v; if (bytes) *bytes = 4; return NB_OK;
 		}
+	// continuous collision: casts of the context's advances that tested every collider instead of walking the grid
+	if (!strcmp(name, "ccd_fallbacks")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_CCD_FALLBACKS]; if (bytes) *bytes = 4; return NB_OK; }
 	if (!strcmp(name, "sched_fallback")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_SCHED_FALLBACK]; if (bytes) *bytes = 4; return NB_OK; }
 	// the last collide's broadphase: the grid level (cell edge 2^level quantised units) and how many colliders went to k_large_pairs
 	if (!strcmp(name, "grid_level")) { if (max_bytes < 4) return NB_ERR_ARGUMENT; *(u32*)dst = c[CNT_GRID_LEVEL]; if (bytes) *bytes = 4; return NB_OK; }
@@ -1316,3 +1341,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_spawn_api.cuh"
 #include "nb_snapshot_api.cuh"
 #include "nb_query_api.cuh"
+#include "nb_ccd_api.cuh"     // after nb_query_api.cuh, whose walk and sphere cast k_ccd runs

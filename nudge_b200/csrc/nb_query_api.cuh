@@ -572,6 +572,76 @@ __global__ void __launch_bounds__(NB_BLOCK, 1) k_shapecast(u32 n, const nb_shape
 	}
 }
 
+// ---------------- continuous collision (nb_upload_ccd_bodies, DESIGN.md section 8.18) ----------------
+// Whether a cast whose sphere (c, r) touches collider i at t = 0 counts there: not when nb_overlap's test of the sphere holds (a start, which
+// nb_collide's contact covers), and otherwise only when d points into the collider, dot(g, d') < 0 with g the step-0 test's gap (for a box
+// in its frame, d' = d in that frame; for a sphere c - p, d' = d).  A sphere clamped onto a face can sit where the face slab counts its start
+// as inside while step 0, rounded the other way, does not; moving away or along the face must still be free.
+NB_DEV bool ccd_counts_at_zero(const QueryScene& S, u32 i, f3 c, float r, f3 d) {
+	const xform w = ld_xform(S.world_xf, i);
+	const f3 p = mk3(w.p.x, w.p.y, w.p.z);
+	if (i < S.nboxes) {
+		const float4 sz = reinterpret_cast<const float4*>(S.box_data)[i];
+		const f3 h = mk3(sz.x, sz.y, sz.z);
+		const quat q = mkq(w.q), qc = qconj(q);
+		if (overlap_sphere_box(c, r, p, q, h)) return false;
+		const f3 l = qrot(qc, sub3(c, p));
+		return dot3(mk3(box_gap(l.x, h.x), box_gap(l.y, h.y), box_gap(l.z, h.z)), qrot(qc, d)) < 0.0f;
+	}
+	if (overlap_sphere_sphere(c, r, p, S.sph_data[i - S.nboxes].radius)) return false;
+	return dot3(sub3(c, p), d) < 0.0f;
+}
+
+// Tests collider i against the swept sphere Q of body `body` along d (max_t = 1) and keeps the lane's best (t bits << 32 | i).  Only
+// colliders the step could give the body a contact with count: Box2D's rule between the entry's filter word and the collider's
+// (k_collider_world's, NB_FILTER_ALL without a table), not on a connected body under NB_FILTER_SKIP_CONNECTED (conn_n != 0), and
+// cast_test's own body and sensor skips; the sphere arithmetic is cast_test's, with its t = 0 hits filtered by ccd_counts_at_zero.
+NB_DEV void ccd_test(const QueryScene& S, u32 i, u32 body, u32 word, const u64* conn_keys, u32 conn_n, const OverlapShape& Q, f3 d, u64& best) {
+	if (!filter_pass(word, asu(reinterpret_cast<const float*>(S.aabb_max)[4 * (size_t)i + 3]))) return;
+	if (conn_n && connected(conn_keys, conn_n, body, __ldg(S.col_body + i))) return;
+	u64 key = ~(u64)0;
+	f3 n;
+	cast_test(S, i, Q, d, 1.0f, ~0u, body, false, key, n);
+	if (key >= best) return;
+	if ((u32)(key >> 32) == 0u && !ccd_counts_at_zero(S, i, Q.c, Q.r, d)) return;
+	best = key;
+}
+
+// One warp per set entry, on nb_advance's stream before k_advance<true>: the entry's body, when the step advances it (its island active in
+// the last collide, not kinematic) and its translation d = v * dt is longer than the threshold and valid for a sweep, casts its sphere from
+// its position along d against the step's front end (S: ctx->front as nb_collide left it) with swept_walk; fallbacks count in
+// counts[CNT_CCD_FALLBACKS].  Lane 0 writes the body's translation factor ccd_t[body] (the hit's t, else 1) and hits[e] = (bits of t,
+// collider or NB_RAY_NO_HIT).  One block per SM as for k_shapecast: the inlined walk and tests need 90 registers, and under the default bound
+// ptxas caps them at 80 and spills.
+__global__ void __launch_bounds__(NB_BLOCK, 1) k_ccd(u32 n, const nb_ccd_body* set, const nb_transform* xf, const nb_body_momentum* momentum,
+		const u32* parent, const u32* active, const uint8_t* kind, float time_step, QueryScene S, const u64* conn_keys, u32 conn_n, u32* counts,
+		float* ccd_t, uint2* hits) {
+	const u32 lane = threadIdx.x & 31, nwarps = (gridDim.x * blockDim.x) >> 5;
+	for (u32 e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < n; e += nwarps) {   // e is warp-uniform
+		const uint4 E = reinterpret_cast<const uint4*>(set)[e];
+		const u32 b = E.x, word = E.w;   // category | mask << 16, a collider filter word
+		const float r = asf(E.y), thr = asf(E.z);
+		const float4 l = reinterpret_cast<const float4*>(momentum + b)[0];
+		const f3 d = mk3(l.x * time_step, l.y * time_step, l.z * time_step);
+		u64 best = ~(u64)0;
+		const bool advanced = active[parent[b]] && !(kind && (kind[b] & 1u));
+		if (advanced && (d.x * d.x + d.y * d.y) + d.z * d.z > thr * thr && sweep_valid(d, 1.0f) && S.K) {
+			const xform x = ld_xform(xf, b);
+			OverlapShape Q;
+			Q.box = false; Q.c = mk3(x.p.x, x.p.y, x.p.z); Q.r = r;
+			swept_walk<true>(S, counts, CNT_CCD_FALLBACKS, lane, Q.c, d, 1.0f, mk3(r, r, r), S.K > S.nboxes || r > 0.0f, true, best,
+				[&](u32 i) { ccd_test(S, i, b, word, conn_keys, conn_n, Q, d, best); });
+		}
+		const u64 wbest = warp_min_u64(best);
+		if (lane == 0) {
+			const bool hit = wbest != ~(u64)0;
+			const u32 tb = hit ? (u32)(wbest >> 32) : asu(1.0f);
+			ccd_t[b] = asf(tb);
+			hits[e] = make_uint2(tb, hit ? (u32)wbest : NB_RAY_NO_HIT);
+		}
+	}
+}
+
 // The queries' scratch for the collider capacity, allocated once from the context's arena (synchronises then; never again).
 static int ensure_query_scratch(nb_context* ctx) {
 	QueryScratch& r = ctx->query;

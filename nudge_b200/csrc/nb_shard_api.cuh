@@ -233,6 +233,7 @@ int nb_shard_step(nb_shard* sh, float time_step, uint32_t iterations, float grav
 	if (ctx->has_kin) { ctx->error = "kinematic bodies are not supported by nb_shard_step"; return NB_ERR_ARGUMENT; }
 	if (ctx->has_frc) { ctx->error = "a body force table is not supported by nb_shard_step"; return NB_ERR_ARGUMENT; }
 	if (ctx->jset.n) { ctx->error = "joints are not supported by nb_shard_step"; return NB_ERR_ARGUMENT; }
+	if (!ctx->ccd.empty()) { ctx->error = "continuous collision (nb_upload_ccd_bodies) is not supported by nb_shard_step"; return NB_ERR_ARGUMENT; }
 	if (sh->no_exchange) return nb_step(ctx, time_step, iterations, gravity, damping, stream);   // diagnostic: this rank's local problem alone
 	{ int jr = join_uploads(ctx, (cudaStream_t)stream); if (jr) return jr; }   // a pending side copy of nb_upload_bodies: ordered here, on the host side (the sharded graph has no event-wait node)
 	ctx->capture_joined = true;

@@ -2,7 +2,7 @@
 // section 8.12).
 //
 // A snapshot is the context's between-steps state in HBM: the sections of a state file (state_sections, nb_state_api.cuh) plus what a file
-// lacks, the user rows, the joint table, the joints' rows and the joint drive table, the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
+// lacks, the user rows, the joint table, the joints' rows and the joint drive table, the continuous-collision set (host side), the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
 // (snapshot_sections).  Save and restore are one launch of k_snapshot_copy in opposite directions; the host side (counts, bits, table set,
 // the connections' host copy, the kinematic set, the rows' levelling) is kept in the snapshot and installed by install_state.
 // Every section but the user rows, the joints and the overlap list has its room at the context's capacities in one arena, laid out once from the
@@ -56,6 +56,7 @@ struct nb_snapshot {
 	DevBuf<JointDrive> drives;                                  // the joint drive table
 	// the host side at the save
 	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset; DriveSet dset;
+	std::vector<nb_ccd_body> ccd;                    // the continuous-collision set (its rows are host values; k_ccd rewrites the factors)
 };
 
 // A snapshot section: the context's buffer, the snapshot's copy, and the counter word (>= 0) that holds the element count on the device.
@@ -168,7 +169,7 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, (size_t)ctx->jset.nrows + ctx->dset.nrows, st); GROW(s->drives, ctx->dset.n ? ctx->jset.n : 0, st);
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
-	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset;
+	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset; s->ccd = ctx->ccd;
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, true, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
@@ -199,6 +200,7 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
 	else if (s->dset.structure != ctx->dset.structure || joint_bufs[2] != ctx->drives.p) ++ctx->graph_epoch;
 	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->dset = s->dset;
+	{ int r = set_ccd(ctx, s->ccd, st); if (r) return r; }   // nothing when the context holds the same set
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;
 	return NB_OK;

@@ -1127,7 +1127,11 @@ __global__ void __launch_bounds__(NB_BLOCK) k_body_forces(const u32* active_idx,
 	}
 }
 
-__global__ void __launch_bounds__(NB_BLOCK) k_advance(const u32* active_idx, nb_transform* xf, const nb_body_momentum* momentum, uint8_t* idle, float time_step, const u32* counts) {
+// CCD: with a continuous-collision set (nb_upload_ccd_bodies), each translation v * dt is scaled by ccd_t[body], the factor k_ccd wrote (1
+// outside the set: the same bits).  Without one ccd_t is not read.
+template<bool CCD>
+__global__ void __launch_bounds__(NB_BLOCK) k_advance(const u32* active_idx, nb_transform* xf, const nb_body_momentum* momentum, uint8_t* idle, float time_step, const u32* counts,
+		const float* ccd_t) {
 	u32 n = counts[CNT_ACTIVE];
 	float half_time_step = 0.5f * time_step;
 	for (u32 k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
@@ -1144,7 +1148,11 @@ __global__ void __launch_bounds__(NB_BLOCK) k_advance(const u32* active_idx, nb_
 		quat dr; dr.v = angular_velocity; dr.s = 0.0f;
 		dr = qmul(dr, mkq(t.q));
 		dr.v = mul3(dr.v, half_time_step); dr.s *= half_time_step;
-		t.p.x += velocity.x * time_step; t.p.y += velocity.y * time_step; t.p.z += velocity.z * time_step;
+		if (CCD) {
+			const float s = ccd_t[i];
+			t.p.x += (velocity.x * time_step) * s; t.p.y += (velocity.y * time_step) * s; t.p.z += (velocity.z * time_step) * s;
+		}
+		else { t.p.x += velocity.x * time_step; t.p.y += velocity.y * time_step; t.p.z += velocity.z * time_step; }
 		t.q.x += dr.v.x; t.q.y += dr.v.y; t.q.z += dr.v.z; t.q.w += dr.s;
 		float f = 1.0f / sqrtf(t.q.w*t.q.w + t.q.x*t.q.x + t.q.y*t.q.y + t.q.z*t.q.z);  // nudge.cpp:1128-1133
 		t.q.x *= f; t.q.y *= f; t.q.z *= f; t.q.w *= f;

@@ -183,6 +183,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	auto remap = [&](u32 b) { return b - (u32)(std::lower_bound(list.begin(), list.end(), b) - list.begin()); };
 	std::vector<u32> kin;
 	for (u32 b : ctx->kin_list) if (!removed(b)) kin.push_back(remap(b));
+	std::vector<nb_ccd_body> ccd;   // the kept continuous-collision entries, renumbered (the remap keeps them ascending)
+	for (nb_ccd_body e : ctx->ccd) if (!removed(e.body)) { e.body = remap(e.body); ccd.push_back(e); }
 	std::vector<nb_body_pair> ab;
 	std::vector<u32> src;   // old device position of each kept row, in upload order
 	for (u32 i = 0; i < us.n; ++i) {
@@ -301,6 +303,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	}
 	if (!old_joints.empty()) { int r = set_joints(ctx, joints.data(), (u32)joints.size(), st); if (r) return r; }
 	if (!drives.empty()) { int r = set_drives(ctx, kept_drives.data(), (u32)kept_drives.size(), st); if (r) return r; }
+	if (int r = set_ccd(ctx, std::move(ccd), st)) return r;
 	return build_conn_lookup(ctx, st);
 }
 

@@ -4,7 +4,8 @@
 // headless.  Included at the end of nb_api.cu.
 //
 // File layout (little endian): header { char magic[8] = "NBSTATE1"; u32 version; u32 bodies, boxes, spheres, connections, cache;
-// u32 solver_mode; u32 reserved[8]; } followed by these sections in this order (state_sections), each padded with zeros to 16 bytes:
+// u32 solver_mode; u32 reserved[8]; }, from version 8 a header extension { u32 ccd_bodies; u32 reserved[3]; }, and these sections in this
+// order (state_sections, then the continuous-collision rows), each padded with zeros to 16 bytes:
 //   section                                        element (B)  count            present when
 //   transforms | properties | momentum | idle      32 16 32 1   bodies           always
 //   box_tags | box_data | box_transforms           4 16 32      boxes            always
@@ -17,20 +18,25 @@
 //   body forces (nb_body_force rows, body = row)   48           bodies           reserved[5] != 0
 //   joints (nb_joint, upload order, current impulses) 112        reserved[6]      reserved[6] != 0
 //   joint drives (nb_joint_drive, joint order)      56           reserved[7]      reserved[7] != 0
+//   ccd bodies (nb_ccd_body, ascending by body)     16           ccd_bodies       version 8
 // Each version defines more reserved words: version 2 reserved[0] = filter flags and reserved[1]; version 3 reserved[2] = 1 and
 // reserved[3] = max_sensor_pairs; version 4 reserved[2] = 0 or 1 and reserved[4] >= 1; version 5 reserved[2] = 0 or 1, reserved[4] >= 0 and
-// reserved[5] = 1; version 6 reserved[2] and reserved[5] = 0 or 1, reserved[4] >= 0 and reserved[6] >= 1; version 7 as 6 and reserved[7] >= 1.
-// A context writes version 7 with joint drives, else 6 with joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
+// reserved[5] = 1; version 6 reserved[2] and reserved[5] = 0 or 1, reserved[4] >= 0 and reserved[6] >= 1; version 7 as 6 and reserved[7] >= 1;
+// version 8 as 7 with reserved[6] >= 0, reserved[7] >= 0 (drives only with joints) and ccd_bodies >= 1.  All eight reserved words being
+// taken, version 8 adds the extension.  A context writes version 8 with a continuous-collision set, else 7 with joint drives, else 6 with joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
 // filter table or flags, else 1.  Every version loads; words a version does not define are ignored, and a file without a table or flags
 // removes the context's.  A kinematic body's velocities are its momentum row.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
+struct NbStateExt { u32 ccd_bodies, reserved[3]; };   // version 8 on
 
-// Reads and checks a state file's header, and zeroes the reserved words its version does not define, so that each section's presence is a
-// plain word test.
-static bool state_header_read(FILE* f, NbStateHeader& h) {
+// Reads and checks a state file's header and, from version 8, its extension (all zeros before), and zeroes the reserved words its version
+// does not define, so that each section's presence is a plain word test.
+static bool state_header_read(FILE* f, NbStateHeader& h, NbStateExt& x) {
+	memset(&x, 0, sizeof(x));
 	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8)) return false;
+	if (h.version == 8 && fread(&x, sizeof(x), 1, f) != 1) return false;
 	if (h.version < 2) h.reserved[0] = h.reserved[1] = 0;
 	if (h.version < 3) h.reserved[2] = h.reserved[3] = 0;
 	if (h.version < 4) h.reserved[4] = 0;
@@ -39,7 +45,8 @@ static bool state_header_read(FILE* f, NbStateHeader& h) {
 	if (h.version < 7) h.reserved[7] = 0;
 	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1) ||
 		   (h.version == 5 && h.reserved[2] <= 1 && h.reserved[5] == 1) || (h.version == 6 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1) ||
-		   (h.version == 7 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1 && h.reserved[7] >= 1);
+		   (h.version == 7 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1 && h.reserved[7] >= 1) ||
+		   (h.version == 8 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && (h.reserved[7] == 0 || h.reserved[6] >= 1) && x.ccd_bodies >= 1);
 }
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
@@ -77,7 +84,7 @@ static NbStateHeader state_header_of(const nb_context* ctx, u32 cache) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = !ctx->ccd.empty() ? 8 : ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
@@ -176,7 +183,10 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	hc.drives.assign(reinterpret_cast<const unsigned char*>(drives.data()), reinterpret_cast<const unsigned char*>(drives.data() + drives.size()));
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
+	const NbStateExt x = { (u32)ctx->ccd.size(), { 0, 0, 0 } };
+	if (h.version == 8) ok = ok && fwrite(&x, sizeof(x), 1, f) == 1;
 	for (const StateSection& s : state_sections(ctx, h, hc, false)) if (s.present) ok = ok && state_put(f, s, tmp, st);
+	if (h.version == 8) ok = ok && fwrite(ctx->ccd.data(), sizeof(nb_ccd_body), ctx->ccd.size(), f) == ctx->ccd.size();   // 16 bytes each: no padding
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -187,7 +197,8 @@ int nb_state_info(const char* path, uint32_t counts[5]) {
 	FILE* f = fopen(path, "rb");
 	if (!f) return NB_ERR_ARGUMENT;
 	NbStateHeader h;
-	const bool ok = state_header_read(f, h);
+	NbStateExt x;
+	const bool ok = state_header_read(f, h, x);
 	fclose(f);
 	if (!ok) return NB_ERR_ARGUMENT;
 	counts[0] = h.bodies; counts[1] = h.boxes; counts[2] = h.spheres; counts[3] = h.connections; counts[4] = h.cache;
@@ -200,7 +211,8 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	FILE* f = fopen(path, "rb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
 	NbStateHeader h;
-	if (!state_header_read(f, h)) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
+	NbStateExt x;
+	if (!state_header_read(f, h, x)) { fclose(f); ctx->error = "not an nb state file"; return NB_ERR_ARGUMENT; }
 	const nb_config& c = ctx->cfg;
 	if (h.bodies > c.max_bodies || h.boxes > c.max_boxes || h.spheres > c.max_spheres || h.connections > c.max_connections || h.cache > c.max_contacts) {
 		fclose(f); ctx->error = "state file exceeds the context's capacities"; return NB_ERR_CAPACITY;
@@ -234,6 +246,11 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	std::vector<u32> structure; std::vector<uint8_t> unit_rel;
 	for (u32 i = 0; ok && i < h.reserved[6]; ++i) { structure.insert(structure.end(), { joints[i].type, joints[i].a, joints[i].b }); unit_rel.push_back(unit_quat(joints[i].rel_rotation) ? 1 : 0); }
 	ok = ok && check_drives(ctx, drives, h.reserved[7], h.reserved[6], structure.data(), unit_rel.data()) == NB_OK;
+	// the continuous-collision set: the upload's entry checks, bodies nonzero, in range and ascending (a kinematic body may keep its entry)
+	std::vector<nb_ccd_body> ccd(x.ccd_bodies);
+	ok = ok && (ccd.empty() || fread(ccd.data(), sizeof(nb_ccd_body), ccd.size(), f) == ccd.size());
+	for (size_t i = 0; ok && i < ccd.size(); ++i)
+		ok = ccd[i].body != 0 && ccd[i].body < h.bodies && (i == 0 || ccd[i].body > ccd[i - 1].body) && !ccd_body_problem(ccd[i]);
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->scene_edited = false;   // the loaded scene replaces an edited one
@@ -248,6 +265,7 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	drop_drives(ctx);   // a file without drives removes them, also where its joints have the context's structure
 	{ int r = set_joints(ctx, joints, h.reserved[6], st); if (r) return r; }
 	{ int r = set_drives(ctx, drives, h.reserved[7], st); if (r) return r; }
+	{ int r = set_ccd(ctx, std::move(ccd), st); if (r) return r; }   // a file of an older version removes the set
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
 }
