@@ -27,6 +27,8 @@
  *   nb_snapshot_*                   <- no reference counterpart: the application's copy of its caller-owned arrays, kept in HBM
  *   nb_raycast, nb_overlap,
  *   nb_shapecast                    <- no reference counterpart (the reference has no scene queries)
+ *   nb_get_body_states /
+ *   nb_set_body_states              <- no reference counterpart: the application's read and edit of BodyData between calls
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -804,6 +806,60 @@ typedef struct {
 } nb_ccd_body;                 /* 16 bytes */
 int nb_upload_ccd_bodies(nb_context*, const nb_ccd_body* host, uint32_t n, void* stream);   /* replaces the set; n = 0 removes it */
 int nb_download_ccd_bodies(nb_context*, nb_ccd_body* host, uint32_t capacity, uint32_t* count, void* stream);
+
+/* Body states (observations, environment resets, respawns, teleports, netcode corrections; DESIGN.md section 8.19): the indexed gather and
+ * scatter of chosen bodies' poses and velocities on the device, with one 64-byte row both ways, so that a gather, an edit in the
+ * application's own device buffers and a set work on one array.
+ * nb_get_body_states: row i holds body b = bodies[i] (bodies null: b = i): position and rotation from its transform, velocity and
+ * angular_velocity from its momentum row, idle_counter = its idle counter, body = b, reserved = 0.  Body 0 is legal.  Legal between any two
+ * calls; ordered after a pending nb_upload_bodies side copy.  One launch (none with n = 0).  A null out with n > 0 is NB_ERR_ARGUMENT.
+ *   on_device == 0: host pointers; an index at or beyond the body count or a null bodies with n > B is NB_ERR_ARGUMENT, changing nothing;
+ *   the call synchronises `stream` and returns with `out` filled.
+ *   on_device != 0: bodies (may be null) and out are device pointers, out 16-byte aligned; asynchronous on `stream`.  An index at or beyond
+ *   the body count gives body = NB_REMOVED_BODY and every other field 0.
+ * nb_set_body_states: the result is bit-identical to this host edit of the arrays the context holds followed by nb_upload_bodies:
+ *   for each entry, in list order (so where a body is listed twice the later entry's fields win):
+ *     NB_BODY_POSE:      the body's transform gets position and rotation as given (no normalisation; its body word is left alone)
+ *     NB_BODY_VELOCITY:  its momentum row gets velocity and angular_velocity as given (unused0 / unused1 are left alone); for a kinematic
+ *                        body this is its kinematic velocity, exactly as nb_upload_kinematic_bodies writes it (the set is not changed)
+ *     every listed dynamic body gets idle counter 0; a listed kinematic body keeps its idle counter
+ *   wake, NB_BODY_POSE only: nb_remove_bodies' rules (a) and (b) with "removed" read as "moved": a body gets idle counter 0 when (a) a
+ *     contact-cache entry's key pairs the tag of one of its colliders with the tag of a moved body's collider (tags are compared, so with
+ *     duplicate tags this over-wakes exactly as removal does), or (b) a connection joins it to a moved body.  Body 0 and kinematic bodies are
+ *     never woken.  With NB_BODY_VELOCITY alone no partner is woken, as with nb_apply_body_impulses: a woken body's island is found at the next
+ *     nb_collide through its unchanged pairs.
+ *   Not edited: the contact cache, the joints (their rows are rebuilt from the new transforms at the next step; their accumulated impulses
+ *   are kept), the sensor overlap lists (recomputed at the next nb_collide; events follow as usual), the continuous-collision set and the body
+ *   force table.  So a body moved to where it touches the same partner again warm-starts from the old cache entry, as the host edit would.
+ *   Refusals (NB_ERR_ARGUMENT, changing nothing): fields == 0 or an unknown field bit; a context that nb_shard_create was called on;
+ *   NB_BODY_POSE between nb_collide and the nb_advance that ends its step (the wake uses collide-stage scratch, and the advance's
+ *   continuous collision assumes that the last nb_collide's grid describes the poses); NB_BODY_POSE while a connection names a body at
+ *   or beyond the body count (nb_upload_connections accepts such indices; the wake, like nb_remove_bodies', needs them below it, and as
+ *   for removal every collider's body must be below it too).  NB_BODY_VELOCITY alone is legal between any two calls.
+ *   on_device == 0: host pointers; every entry is checked before any device work: body 0, a body at or beyond the body count, a selected
+ *   field that is not finite, or a null pointer with n > 0 is NB_ERR_ARGUMENT.  *skipped (when not null) is set to 0.  The array may be
+ *   reused when the call returns.
+ *   on_device != 0: states (16-byte aligned) and skipped (may be null) are device pointers.  An entry failing the host path's checks is
+ *   skipped on the device, and *skipped is written (not accumulated) with the number skipped.
+ *   Asynchronous on `stream`, ordered like nb_upload_momentum.  Launches: 3 (keys, one radix sort by (body, list position), one thread per
+ *   body run) for NB_BODY_VELOCITY alone; a pose set adds removal's wake: 3 more (flags and keys, one radix sort of (tag, body) keys, cache
+ *   wake), 1 more without colliders; none with n = 0.
+ * Neither call changes nb_step's graph, holds state, or adds anything to the step, a snapshot or a state file.  on_device != 0 can be captured
+ * into the application's CUDA graph once an earlier call on the context had at least n entries (a call with more grows the scratch:
+ * it synchronises and allocates, and a captured graph of the old size must be captured again).  A captured call holds the scene's shape
+ * as of its capture: the body count, and for a set the collider and connection counts, the sort's digit count and, for a pose set's wake,
+ * the tag bits; the refusals above are decided at capture.  Capture again after any edit of the scene's shape: nb_add_bodies,
+ * nb_remove_bodies, nb_upload_bodies with another count, nb_upload_colliders, nb_upload_connections, nb_load_state. */
+typedef struct {
+	float position[3]; uint32_t body;              /* get: the index read; set: the body to edit */
+	float rotation[4];                             /* x, y, z, w */
+	float velocity[3]; uint32_t idle_counter;      /* get: the body's idle counter; set: ignored */
+	float angular_velocity[3]; uint32_t reserved;  /* get: 0; set: ignored */
+} nb_body_state;                                   /* 64 bytes */
+enum nb_body_state_fields { NB_BODY_POSE = 1, NB_BODY_VELOCITY = 2 };
+int nb_get_body_states(nb_context*, const uint32_t* bodies /* null: bodies 0 .. n-1 */, uint32_t n, nb_body_state* out, int on_device, void* stream);
+int nb_set_body_states(nb_context*, const nb_body_state* states, uint32_t n, uint32_t fields, uint32_t* skipped /* may be null */, int on_device,
+                       void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

@@ -27,7 +27,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
            "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap",
-           "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives"]
+           "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives", "nb_get_body_states", "nb_set_body_states"]
 
 
 class Config(C.Structure):
@@ -128,6 +128,8 @@ def load_library():
         lib.nb_shapecast.argtypes = [V, V, C.c_uint32, V, C.c_uint32, C.c_int, V]
         lib.nb_upload_ccd_bodies.argtypes = [V, V, C.c_uint32, V]
         lib.nb_download_ccd_bodies.argtypes = [V, V, C.c_uint32, V, V]
+        lib.nb_get_body_states.argtypes = [V, V, C.c_uint32, V, C.c_int, V]
+        lib.nb_set_body_states.argtypes = [V, V, C.c_uint32, C.c_uint32, V, C.c_int, V]
         _lib = lib
     return _lib
 
@@ -512,6 +514,44 @@ class Sim(abi.HostState):
         out = np.zeros(n.value, abi.CCD_BODY)
         self._ck(self.lib.nb_download_ccd_bodies(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_ccd_bodies")
         return out
+
+    # ---- body states (nb_get_body_states, nb_set_body_states, include/nudge_b200.h): gather and scatter of chosen bodies' poses and velocities ----
+    def get_body_states(self, bodies=None, device_ptrs=None, n=None):
+        """The abi.BODY_STATE rows of `bodies` (None: bodies 0 .. B-1): position, rotation, velocity, angular velocity and idle counter as
+        they stand on the device.  device_ptrs=(bodies_ptr or None, out_ptr) with n: device buffers of n indices (None: bodies 0 .. n-1)
+        and n rows instead; the call is then asynchronous on the Sim's stream (capturable) and returns None, and an index at or beyond the
+        body count gives a row with body = REMOVED_BODY and zeros."""
+        if device_ptrs is not None:
+            if n is None:
+                raise ValueError("Sim.get_body_states with device_ptrs needs n, the number of rows the device buffers hold")
+            idx, out = device_ptrs
+            self._ck(self.lib.nb_get_body_states(self.ctx, C.c_void_p(idx) if idx else None, int(n), C.c_void_p(out), 1, self.stream), "nb_get_body_states")
+            return None
+        idx = None if bodies is None else np.ascontiguousarray(np.asarray(bodies, np.uint32).reshape(-1))
+        k = self.scene.n_bodies if idx is None else len(idx)
+        out = np.zeros(k, abi.BODY_STATE)
+        self._ck(self.lib.nb_get_body_states(self.ctx, abi.ptr(idx) if idx is not None and k else None, k, abi.ptr(out) if k else None, 0, self.stream),
+                 "nb_get_body_states")
+        return out
+
+    def set_body_states(self, states, fields, device_ptrs=None, n=None):
+        """Writes abi.BODY_STATE rows on the device in list order: fields BODY_POSE sets position and rotation (and wakes what the moved
+        bodies touched through the contact cache or a connection), BODY_VELOCITY velocity and angular velocity; every listed dynamic body
+        gets idle counter 0.  Host rows are checked first (NudgeError on body 0, a body at or beyond the body count or a non-finite selected
+        field) and the call returns 0.  device_ptrs=(states_ptr, skipped_ptr or None) with n: device buffers instead; invalid entries are
+        skipped, their number written to the uint32 at skipped_ptr, and the call returns None (asynchronous, capturable).  The host mirrors
+        (self.transforms, self.momentum, self.idle) are not updated; download_bodies() fetches the device's rows."""
+        if device_ptrs is not None:
+            if n is None:
+                raise ValueError("Sim.set_body_states with device_ptrs needs n, the number of rows the device buffer holds")
+            rows, skipped = device_ptrs
+            self._ck(self.lib.nb_set_body_states(self.ctx, C.c_void_p(rows), int(n), int(fields), C.c_void_p(skipped) if skipped else None, 1, self.stream),
+                     "nb_set_body_states")
+            return None
+        r = np.ascontiguousarray(np.asarray(states, abi.BODY_STATE).reshape(-1))
+        skipped = C.c_uint32(0)
+        self._ck(self.lib.nb_set_body_states(self.ctx, abi.ptr(r) if len(r) else None, len(r), int(fields), C.byref(skipped), 0, self.stream), "nb_set_body_states")
+        return int(skipped.value)
 
     # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----
     def overlap(self, queries, flags=0, capacity=None, device_ptrs=None, n=None):

@@ -73,6 +73,13 @@ SHAPECAST_SENSORS = 1
 CCD_BODY = np.dtype([("body", "<u4"), ("radius", "<f4"), ("motion_threshold", "<f4"), ("category", "<u2"), ("mask", "<u2")])
 assert CCD_BODY.itemsize == 16
 
+# nb_body_state (64 bytes): one row of nb_get_body_states / nb_set_body_states; fields: BODY_POSE = 1, BODY_VELOCITY = 2
+BODY_STATE = np.dtype([("position", "<f4", 3), ("body", "<u4"), ("rotation", "<f4", 4), ("velocity", "<f4", 3), ("idle_counter", "<u4"),
+                       ("angular_velocity", "<f4", 3), ("reserved", "<u4")])
+assert BODY_STATE.itemsize == 64
+BODY_POSE = 1
+BODY_VELOCITY = 2
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

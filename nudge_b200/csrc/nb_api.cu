@@ -149,6 +149,9 @@ struct nb_context {
 	// ccd_rows its device copy; ccd_t = the advance's translation factor per body (max_bodies of them, 1 outside the set), allocated on the
 	// first upload; ccd_hits = (bits of t, collider) per entry of the last advance
 	std::vector<nb_ccd_body> ccd; DevBuf<nb_ccd_body> ccd_rows; float* ccd_t; DevBuf<uint2> ccd_hits;
+	// body states (nb_get_body_states, nb_set_body_states, DESIGN.md section 8.19, nb_body_state_api.cuh): a host-pointer call's staging (rows in
+	// and out, the gather's indices), and the set's sort keys (bs_sb points into bs_keys) with its own histogram, grid barrier and key count
+	DevBuf<nb_body_state> bs_rows; DevBuf<u32> bs_idx; DevBuf<u64> bs_keys[2]; SortBuffers bs_sb; u32* bs_n;
 	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap, section 8.15) and shape casts
 	// (nb_shapecast, section 8.16)
 	QueryScratch query;
@@ -1342,3 +1345,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_snapshot_api.cuh"
 #include "nb_query_api.cuh"
 #include "nb_ccd_api.cuh"     // after nb_query_api.cuh, whose walk and sphere cast k_ccd runs
+#include "nb_body_state_api.cuh"   // after nb_spawn_api.cuh, whose wake a pose set runs

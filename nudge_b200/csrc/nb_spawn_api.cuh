@@ -9,9 +9,10 @@
 // number of added boxes through a staging copy.
 // Remove, nothing of it per step:
 //   k_spawn_mark     a "removed" byte per body, scattered from the list (in the offs planes, which nb_collide overwrites anyway)
-//   k_spawn_flags    keep flags of bodies, colliders (one counter for boxes, one for spheres, over boxes-then-spheres) and connections;
-//                    the colliders' (tag, body, removed) keys; the connection half of the wake set
-//   nb_radix_sort    of those keys; k_spawn_wake then binary-searches both tags of every cache entry: the other side of a removed tag wakes
+//   launch_wake      the wake, shared with nb_set_body_states (nb_body_state_api.cuh), where "removed" reads "moved":
+//     k_spawn_flags  the colliders' (tag, body, removed) keys; the connection half of the wake set; for the removal also the keep flags of
+//                    bodies, colliders (one counter for boxes, one for spheres, over boxes-then-spheres) and connections
+//     nb_radix_sort  of those keys; k_spawn_wake then binary-searches both tags of every cache entry: the other side of a removed tag wakes
 //   nb_scan_reduce + k_spawn_bodies / k_spawn_colliders / k_spawn_conns: the fused scan ranks each array once, and its consumer gathers the
 //                    kept rows out of place into collide-stage scratch (the body gather also writes the old -> new map, and moves the
 //                    body force rows into frc_spare)
@@ -31,25 +32,25 @@ __global__ void __launch_bounds__(NB_BLOCK) k_spawn_mark(const u32* list, u32 n,
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) removed[list[i]] = 1;
 }
 
-// flags[i] (body kept), flags[S + k] / flags[2S + k] (collider k kept and a box / a sphere), flags[3S + c] (connection kept); keys[k] =
-// tag << kshift | body << 1 | removed.  A connection with exactly one removed side wakes the other.
+// keys[k] = tag << kshift | body << 1 | removed.  A connection with exactly one removed side wakes the other.  With flags (the removal):
+// flags[i] (body kept), flags[S + k] / flags[2S + k] (collider k kept and a box / a sphere), flags[3S + c] (connection kept).
 __global__ void __launch_bounds__(NB_BLOCK) k_spawn_flags(u32 B, u32 nboxes, u32 K, u32 nconn, const uint8_t* removed, const nb_transform* box_xf,
 		const u32* box_tags, const nb_transform* sph_xf, const u32* sph_tags, const nb_body_pair* conn, const uint8_t* kind, uint8_t* idle,
 		u32* flags, u32 S, u64* keys, u32 kshift, u32* counts) {
 	const u32 n = max(B, max(K, nconn));
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		if (i == 0) { counts[CNT_SPAWN_MAXTAG] = 1; counts[CNT_SPAWN_KEYS] = K; counts[CNT_SPAWN_BOXES] = 0; counts[CNT_SPAWN_SPHERES] = 0; counts[CNT_SPAWN_CONN] = 0; }
-		if (i < B) flags[i] = removed[i] ? 0u : 1u;
+		if (flags && i < B) flags[i] = removed[i] ? 0u : 1u;
 		if (i < K) {
 			const bool box = i < nboxes;
 			const u32 body = box ? box_xf[i].body : sph_xf[i - nboxes].body, tag = box ? box_tags[i] : sph_tags[i - nboxes];
 			const u32 rem = removed[body];
-			flags[S + i] = box && !rem; flags[2 * (size_t)S + i] = !box && !rem;
+			if (flags) { flags[S + i] = box && !rem; flags[2 * (size_t)S + i] = !box && !rem; }
 			keys[i] = ((u64)tag << kshift) | ((u64)body << 1) | rem;
 		}
 		if (i < nconn) {
 			const u32 a = conn[i].a, b = conn[i].b, ra = removed[a], rb = removed[b];
-			flags[3 * (size_t)S + i] = !(ra | rb);
+			if (flags) flags[3 * (size_t)S + i] = !(ra | rb);
 			if (ra && !rb) spawn_wake(kind, idle, b);
 			if (rb && !ra) spawn_wake(kind, idle, a);
 		}
@@ -159,6 +160,21 @@ __global__ void __launch_bounds__(NB_BLOCK) k_spawn_overlaps(uint4* cur, uint4* 
 	}
 }
 
+// The wake of rules (a) and (b) from one byte per body (`marked`, B of them): k_spawn_flags, then with colliders the sort of the (tag, body,
+// marked) keys and k_spawn_wake over the contact cache.  keep_flags = the removal's keep-flag planes (ctx->flags), or null for a wake alone.
+// 3 launches, 1 without colliders.  It uses collide-stage scratch (the step's sort buffers and the spawn counters), so it runs between steps.
+static void launch_wake(nb_context* ctx, const Launch& L, const uint8_t* marked, u32* keep_flags) {
+	const u32 B = ctx->B, nboxes = ctx->nboxes, K = ctx->nboxes + ctx->nspheres, nconn = ctx->nconn;
+	const uint8_t* kind = kin_table(ctx);
+	const u32 kshift = bits_for(B) + 1;
+	launch_grid(L, k_spawn_flags, GRID(std::max(B, std::max(K, nconn))), B, nboxes, K, nconn, marked, ctx->box_xf, ctx->box_tags, ctx->sph_xf, ctx->sph_tags,
+		ctx->conn, kind, ctx->idle, keep_flags, ctx->stride, ctx->sb.keys[0], kshift, ctx->counts);
+	if (K) {
+		const int cur = nb_radix_sort(L, ctx->sb, ctx->counts + CNT_SPAWN_KEYS, 0, (int)(ctx->tagbits + kshift), false, 0);
+		launch_grid(L, k_spawn_wake, GRID(ctx->cfg.max_contacts), ctx->cache_tags, ctx->sb.keys[cur], K, kshift, kind, ctx->idle, ctx->counts);
+	}
+}
+
 extern "C" {
 
 int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* stream) {
@@ -236,16 +252,9 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	u32* flags = ctx->flags;
 	u32* counts = ctx->counts;
 	u32* map = ctx->parent;
-	const uint8_t* kind = kin_table(ctx);
-	const u32 kshift = bits_for(B) + 1;
 	CK(cudaMemsetAsync(rem, 0, B, st));
 	launch_grid(L, k_spawn_mark, GRID(n), ctx->spawn_idx.p, n, rem);
-	launch_grid(L, k_spawn_flags, GRID(std::max(B, std::max(K, nconn))), B, nboxes, K, nconn, rem, ctx->box_xf, ctx->box_tags, ctx->sph_xf, ctx->sph_tags,
-		ctx->conn, kind, ctx->idle, flags, S, ctx->sb.keys[0], kshift, counts);
-	if (K) {
-		const int cur = nb_radix_sort(L, ctx->sb, counts + CNT_SPAWN_KEYS, 0, (int)(ctx->tagbits + kshift), false, 0);
-		launch_grid(L, k_spawn_wake, GRID(ctx->cfg.max_contacts), ctx->cache_tags, ctx->sb.keys[cur], K, kshift, kind, ctx->idle, counts);
-	}
+	launch_wake(ctx, L, rem, flags);
 	// bodies: xf -> mw, properties -> inertia, idle -> taint, kind -> active (each rewritten by the step before it is read: k_mw_in, k_inertia,
 	// k_uf_init); momentum -> jd, the throughput solver's accumulator, which must be all zeros between passes and is cleared after the copy back
 	nb_scan_reduce<1>(L, flags, S, nullptr, B, ctx->block_sums, counts + CNT_SPAWN_B);

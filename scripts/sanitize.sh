@@ -11,6 +11,16 @@ g.enable_contact_events(4096)   # the event kernels run inside nb_write_cached_i
 for _ in range(6): g.step_staged()
 g.set_solver_mode("throughput")
 for _ in range(4): g.step_staged()
+st = g.get_body_states([1, 5, 9, 5]); g.get_body_states()   # body states: host mode, then device mode below
+st["position"][:, 1] += 0.5
+g.set_body_states(st, 3); g.set_body_states(st, 2)
+import torch
+t_idx = torch.tensor([1, 5, 9, 5], dtype=torch.int32, device="cuda"); t_out = torch.zeros(64, dtype=torch.int32, device="cuda")
+t_skip = torch.zeros(1, dtype=torch.int32, device="cuda")
+torch.cuda.synchronize()
+g.get_body_states(device_ptrs=(t_idx.data_ptr(), t_out.data_ptr()), n=4)
+g.set_body_states(None, 3, device_ptrs=(t_out.data_ptr(), t_skip.data_ptr()), n=4)
+g.step_staged()
 ev, dropped = g.contact_events()
 c = g.counts(); print("contacts", c.contacts, "overflow", c.overflow, "events", len(ev), "dropped", dropped)
 PY
