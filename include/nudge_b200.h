@@ -245,8 +245,10 @@ typedef struct {
 	uint32_t type, a, b;        /* a != 0; b = 0 is the static world; a != b */
 	float anchor_a[3];          /* in a's body frame */
 	float anchor_b[3];          /* in b's body frame; a world point when b = 0 */
-	float axis_a[3], axis_b[3]; /* HINGE: the hinge axis in each body's frame (unit length; the world frame for b = 0) */
-	float rel_rotation[4];      /* FIXED, and HINGE with a LIMIT drive: conj(q_a) * q_b at rest (x, y, z, w; q_b = identity for b = 0) */
+	float axis_a[3], axis_b[3]; /* HINGE: the hinge axis in each body's frame (unit length; the world frame for b = 0).  axis_a is also the
+	                               slide axis of FIXED with a SLIDE drive and the twist axis of BALL with a CONE or TWIST drive */
+	float rel_rotation[4];      /* FIXED, HINGE with a LIMIT drive and BALL with a CONE or TWIST drive: conj(q_a) * q_b at rest (x, y, z, w;
+	                               q_b = identity for b = 0) */
 	float length;               /* DISTANCE: rest distance between the anchors */
 	float beta;                 /* Baumgarte factor: bias = beta / dt * error */
 	float softness;             /* copied into every row */
@@ -256,10 +258,12 @@ int nb_upload_joints(nb_context*, const nb_joint* host, uint32_t n, void* stream
 int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t* count, void* stream);
 
 /* Joint drives (doors, knees, flippers, wheels, fans, ropes, breakable bridges and welds; DESIGN.md section 8.17): hinge angle limits, hinge
- * motors, distance ranges and break thresholds, built and solved by the joints' own kernels inside the step.  A drive set is a sparse table
+ * motors, distance ranges and break thresholds, built and solved by the joints' own kernels inside the step.  Sliders (pistons, drawers,
+ * rails, struts) and ragdoll shoulders, hips and necks (DESIGN.md section 8.20) are drives too: SLIDE frees a FIXED joint's translation along
+ * axis_a, and CONE and TWIST limit a BALL joint's swing away from axis_a and its twist about it.  A drive set is a sparse table
  * keyed by joint: at most one drive per joint, naming it by its index in the current joint set's upload order.
- * Rows: a drive appends rows to its joint, solved right after the joint's own rows in this order: motor (MOTOR), lower limit and upper limit
- * (LIMIT).  Every appended row has the joint's a, b and softness, reserved = 0, and keeps its accumulated impulse from step to step.  In
+ * Rows: a drive appends rows to its joint, solved right after the joint's own rows in this order: motor (MOTOR) or cone (CONE), lower limit
+ * and upper limit (LIMIT or TWIST); so a drive has (MOTOR|CONE ? 1 : 0) + (LIMIT|TWIST ? 2 : 0) appended rows.  Every appended row has the joint's a, b and softness, reserved = 0, and keeps its accumulated impulse from step to step.  In
  * nb_debug_read("joint_rows") the joints' own rows come first, exactly as without drives, then the appended rows, per driven joint in the
  * joint table's order (by joint level, upload order within one).  Same arithmetic rules as above (float32, left to right, no fused
  * multiply-adds), with k = beta / dt and bias(C) = C > 0 ? C / dt : k * C (speculative: a limit row lets the coordinate reach its bound
@@ -274,47 +278,79 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  *              = 0 (the hinge Jacobian with its angular parts negated);  both bias = bias(C), lo = 0, hi = +inf.
  *   DISTANCE limit:    the joint's own row is written with lo = hi = 0 (it stays in place and applies nothing);  lower: the own row's
  *              Jacobian with C = dist - lower;  upper: that Jacobian negated with C = upper - dist;  both bias = bias(C), lo = 0, hi = +inf.
+ *   Slider:    FIXED + SLIDE.  u = qrot(q_a, axis_a) is the slide axis, t1, t2 built from u exactly as HINGE builds them, sa = ra - err
+ *              (from a's position to b's anchor).  The joint's own rows 0 and 1 become, for t = t1, t2: lin_a = t, ang_a = cross(sa, t),
+ *              lin_b = -t, ang_b = -cross(rb, t) (each component negated), bias = k * dot(err, t); row 2 is the same form on u with lo = hi = 0
+ *              (it stays in place and applies nothing); rows 3 to 5 are FIXED's angular rows.  Each keeps its accumulated impulse.  The
+ *              coordinate s = dot(wb - wa, u) has the Jacobian J_s: lin_a = -u, ang_a = -cross(sa, u), lin_b = u, ang_b = cross(rb, u).
+ *   SLIDE motor:       J_s, bias = -motor_speed, lo = -(max_motor_torque * dt), hi = max_motor_torque * dt: for a slider motor_speed is
+ *              a linear speed and max_motor_torque a force.
+ *   SLIDE lower limit: J_s with C = s - lower;  upper: -J_s (every component negated) with C = upper - s;  both bias = bias(C), lo = 0,
+ *              hi = +inf.
+ *   Swing-twist:       BALL + CONE / TWIST.  d as the HINGE coordinate computes it (d.w >= 0), u = qrot(q_a, axis_a) the twist axis;
+ *              a_ = dot(d.xyz, u), sh = -a_, ch = d.w;  the swing p = d.xyz - u * a_ (per component);  ss = sqrtf(dot(p, p)) and
+ *              cs = sqrtf(sh*sh + ch*ch), the sine and cosine of half the swing angle;  the twist pair (sh', ch') = cs > 0 ? (sh * (1/cs),
+ *              ch * (1/cs)) : (0, 1).
+ *   TWIST limit:       the HINGE lower and upper limit rows, on the hinge Jacobian about u, with (sh', ch') in place of (sh, ch); lower and
+ *              upper in [-pi, pi] converted to (sl, cl), (su, cu) as for a hinge.
+ *   CONE:      (sc, cc) = (sin, cos) of cone/2, converted on the host in double and rounded to float32;  C = 2 * (sc*cs - cc*ss);
+ *              n = ss > 0 ? p * (1/ss) : (0, 0, 0) (a zero row has no effect);  ang_a = -n, ang_b = n, lin_a = lin_b = 0, bias = bias(C),
+ *              lo = 0, hi = +inf.
  *   Breaking:  when k_joint_rows is about to rewrite a BREAKABLE joint's rows it takes the accumulated impulses the previous step left:
- *              P = the sum 0 + i*i in row order over the joint's linear rows (the point rows; DISTANCE's own and limit rows), A = the same over
- *              its angular rows (HINGE's and FIXED's angular rows, the hinge's motor and limit rows).  The joint breaks when
+ *              P = the sum 0 + i*i in row order over the joint's linear rows (the point rows; DISTANCE's own and appended rows; a slider's
+ *              appended rows), A = the same over its angular rows (HINGE's and FIXED's angular rows, the hinge's motor and limit rows, the cone
+ *              and twist rows).  The joint breaks when
  *              P > (break_force*dt)*(break_force*dt) or A > (break_torque*dt)*(break_torque*dt); +inf never breaks.
  *   Broken:    a drive with broken = 1 has every row of its joint, appended rows included, written as a zero row: zero Jacobian, bias = 0,
  *              lo = hi = 0, impulse = 0, softness = 0, a and b kept, reserved = 0.  The rows stay in the set, so nothing structural changes
  *              and nb_step keeps its graph; broken stays 1 until an upload re-arms it.  Connections and idle counters are not touched (edit the
  *              connections to let the pieces collide).
- *   position:  each build of an unbroken LIMIT drive records the coordinate it used: (sh, ch) for a hinge, dist for a distance joint.
+ *   position:  each build of an unbroken LIMIT drive records the coordinate it used: (sh, ch) for a hinge, dist for a distance joint; each
+ *              build of an unbroken SLIDE drive records s, and of a CONE or TWIST drive (sh', ch') with TWIST, (ss, cs) with CONE alone.
  * nb_upload_joint_drives replaces the drive set (n = 0 removes it); impulse[] warm-starts the appended rows, broken is installed as given (0
  * re-arms a broken joint), position is ignored and reads 0 until the next row build.  Every entry is checked on the host before any device
  * work, and an error changes nothing.  NB_ERR_ARGUMENT: a null pointer with n > 0; a joint index at or beyond the joint count, or two drives
- * on one joint; a flag the joint's type does not take (LIMIT: HINGE, DISTANCE; MOTOR: HINGE; BREAKABLE: every type) or an unknown bit;
- * lower > upper, a hinge limit outside [-pi, pi] (pi rounded to float32, 3.14159274f), a negative distance limit; a negative max_motor_torque,
- * break_force or break_torque; a field that is not finite other than thresholds of +inf; broken > 1; a HINGE LIMIT whose joint's
- * rel_rotation has |x*x + y*y + z*z + w*w - 1| > 1e-3 (in double).  Asynchronous on `stream`, staged like nb_upload_joints (the host array
+ * on one joint; a flag the joint's type does not take (LIMIT: HINGE, DISTANCE, FIXED with SLIDE; MOTOR: HINGE, FIXED with SLIDE; SLIDE:
+ * FIXED; CONE, TWIST: BALL; BREAKABLE: every type) or an unknown bit; lower > upper (LIMIT, TWIST), a hinge or twist limit outside [-pi, pi]
+ * (pi rounded to float32, 3.14159274f), a negative distance limit; a CONE whose cone is outside (0, pi], or with a nonzero motor_speed or
+ * max_motor_torque; a negative max_motor_torque, break_force or break_torque; a field that is not finite other than thresholds of +inf (cone
+ * is read only with CONE); broken > 1; a HINGE LIMIT, CONE or TWIST whose joint's rel_rotation has |x*x + y*y + z*z + w*w - 1| > 1e-3 (in
+ * double); a SLIDE, CONE or TWIST whose joint's axis_a has |x*x + y*y + z*z - 1| > 1e-3 (in double).  Asynchronous on `stream`, staged like nb_upload_joints (the host array
  * may be reused on return); it synchronises only when the joints' row buffer must grow.  nb_step re-records its graph only when the drive
  * structure (which joints, which flags) changed or a buffer moved: new speeds, torques, limits, thresholds, impulses or broken flags for the
  * same structure keep it, so a throttle may be uploaded every frame.
  * nb_download_joint_drives returns the drives in joint-index order with impulse[] = the appended rows' current accumulated impulses (0 where
- * a row is absent), broken, and position: 2*atan2(sh, ch) in double, rounded to float32, for a hinge, dist for a distance joint, 0 without
- * LIMIT or before the first build.  *count = the number of drives; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
+ * a row is absent), broken, and position: 2*atan2(sh, ch) in double, rounded to float32, for a hinge, dist for a distance joint, s for a
+ * slider, 2*atan2 of the recorded pair for a BALL (the twist angle with TWIST, the swing angle with CONE alone), 0 without LIMIT, SLIDE, CONE
+ * or TWIST or before the first build.  A CONE drive returns motor_speed = max_motor_torque = 0 and its cone as uploaded; cone is 0 otherwise.  *count = the number of drives; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
  * The set follows its joints: nb_upload_joints keeps it (impulses and broken flags included) when the joint structure is unchanged and removes
  * it otherwise; nb_remove_bodies drops the drives of deleted joints and renumbers the rest; nb_add_bodies leaves it alone; nb_upload_bodies
  * removes it with the joints.  Snapshots carry it; nb_save_state writes it (state version 7) and nb_load_state installs it through the
- * upload's checks; a file of an older version removes it.  nb_debug_read("joint_drives") returns the device table: one 64-byte entry per joint in table order, { flags, first appended row, lower, upper, sl, cl, su, cu, motor_speed, max_motor_torque,
- * break_force, break_torque, position[2] (sh, ch or dist, 0), broken, 0 }, flags 0 and the rest 0 for a joint without a drive.
+ * upload's checks; a file of an older version removes it.  SLIDE, CONE and TWIST and the cone travel in the same rows (no new state version);
+ * a build without them refuses such a file's drives as an unknown flag.  nb_debug_read("joint_drives") returns the device table: one 64-byte
+ * entry per joint in table order, { flags, first appended row, lower, upper, sl, cl, su, cu, motor_speed, max_motor_torque, break_force,
+ * break_torque, position[2] (sh, ch; dist, 0; s, 0; sh', ch' or ss, cs), broken, cone }, flags 0 and the rest 0 for a joint without a drive.
+ * A SLIDE drive holds lower and upper raw, with sl .. cu 0; a TWIST drive holds their half-angle pairs as a hinge does; a CONE drive holds
+ * (sc, cc) in motor_speed and max_motor_torque and its cone as uploaded in the last word (0 without CONE).
  * Cost: no launch; k_joint_rows and k_joint_solve take the drive table as one more argument (null without a set), and without a set the
  * joints' rows, the launches and the graph are what they are without this feature. */
-enum nb_joint_drive_flags { NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4 };
+/* Bit 8 is unassigned (refused as an unknown flag). */
+enum nb_joint_drive_flags { NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4, NB_JOINT_SLIDE = 16, NB_JOINT_CONE = 32, NB_JOINT_TWIST = 64 };
 typedef struct {
 	uint32_t joint;             /* index of the joint in the current set's upload order */
-	uint32_t flags;             /* LIMIT: HINGE, DISTANCE.  MOTOR: HINGE.  BREAKABLE: every type */
-	float lower, upper;         /* LIMIT: HINGE angle in radians, -pi <= lower <= upper <= pi; DISTANCE length, 0 <= lower <= upper */
-	float motor_speed;          /* MOTOR: target of the hinge's relative angular velocity (rad/s) */
-	float max_motor_torque;     /* MOTOR: >= 0; the motor row's impulse stays in [-max_motor_torque*dt, +max_motor_torque*dt] */
+	uint32_t flags;             /* LIMIT: HINGE, DISTANCE, FIXED with SLIDE.  MOTOR: HINGE, FIXED with SLIDE.  SLIDE: FIXED.  CONE, TWIST:
+	                               BALL.  BREAKABLE: every type */
+	float lower, upper;         /* LIMIT: HINGE angle in radians, -pi <= lower <= upper <= pi; DISTANCE length, 0 <= lower <= upper; slider
+	                               coordinate s, lower <= upper.  TWIST: twist angle in radians, -pi <= lower <= upper <= pi */
+	float motor_speed;          /* MOTOR: target of the hinge's relative angular velocity (rad/s) or of the slider's speed (units/s) */
+	float max_motor_torque;     /* MOTOR: >= 0; the motor row's impulse stays in [-max_motor_torque*dt, +max_motor_torque*dt] (a force
+	                               for a slider).  CONE: both motor fields must be 0 */
 	float break_force, break_torque;   /* BREAKABLE: >= 0, +inf = never */
-	float impulse[3];           /* accumulated impulses of the motor, lower-limit and upper-limit rows (0 where absent) */
-	float position;             /* download: the hinge angle or the distance at the last row build (0 without LIMIT) */
+	float impulse[3];           /* accumulated impulses of the motor or cone, lower-limit and upper-limit rows (0 where absent) */
+	float position;             /* download: the hinge angle, the distance, the slider coordinate, the twist angle or, with CONE alone,
+	                               the swing angle at the last row build (0 without LIMIT, SLIDE, CONE or TWIST) */
 	uint32_t broken;            /* 0 or 1; upload 0 to re-arm a broken joint */
-	uint32_t reserved;
+	float cone;                 /* CONE: the swing cone's half-angle in radians, 0 < cone <= pi; ignored (and downloaded as 0) otherwise */
 } nb_joint_drive;               /* 56 bytes */
 int nb_upload_joint_drives(nb_context*, const nb_joint_drive* host, uint32_t n, void* stream);
 int nb_download_joint_drives(nb_context*, nb_joint_drive* host, uint32_t capacity, uint32_t* count, void* stream);

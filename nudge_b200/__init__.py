@@ -172,7 +172,7 @@ assert ROW.itemsize == 80
 JOINT = abi.JOINT
 JOINT_BALL, JOINT_HINGE, JOINT_FIXED, JOINT_DISTANCE = 0, 1, 2, 3
 JOINT_DRIVE = abi.JOINT_DRIVE
-JOINT_LIMIT, JOINT_MOTOR, JOINT_BREAKABLE = 1, 2, 4
+JOINT_LIMIT, JOINT_MOTOR, JOINT_BREAKABLE, JOINT_SLIDE, JOINT_CONE, JOINT_TWIST = 1, 2, 4, 16, 32, 64
 
 
 def nccl_unique_id():
@@ -445,7 +445,7 @@ class Sim(abi.HostState):
         return out
 
     def upload_joint_drives(self, drives):
-        """Replaces the joint drive set (limits, motors, break thresholds) with `drives` (JOINT_DRIVE rows; none removes it).  Asynchronous."""
+        """Replaces the joint drive set (limits, motors, sliders, swing cones, twist limits, break thresholds) with `drives` (JOINT_DRIVE rows; none removes it).  Asynchronous."""
         d = np.ascontiguousarray(np.asarray(drives if drives is not None else [], JOINT_DRIVE).reshape(-1))
         self._ck(self.lib.nb_upload_joint_drives(self.ctx, abi.ptr(d) if len(d) else None, len(d), self.stream), "nb_upload_joint_drives")
 

@@ -43,9 +43,10 @@ JOINT = np.dtype([("type", "<u4"), ("a", "<u4"), ("b", "<u4"), ("anchor_a", "<f4
                   ("rel_rotation", "<f4", 4), ("length", "<f4"), ("beta", "<f4"), ("softness", "<f4"), ("impulse", "<f4", 6)])
 assert JOINT.itemsize == 112
 
-# nb_joint_drive (56 bytes); flags: NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4
+# nb_joint_drive (56 bytes); flags: NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4, NB_JOINT_SLIDE = 16, NB_JOINT_CONE = 32,
+# NB_JOINT_TWIST = 64
 JOINT_DRIVE = np.dtype([("joint", "<u4"), ("flags", "<u4"), ("lower", "<f4"), ("upper", "<f4"), ("motor_speed", "<f4"), ("max_motor_torque", "<f4"),
-                        ("break_force", "<f4"), ("break_torque", "<f4"), ("impulse", "<f4", 3), ("position", "<f4"), ("broken", "<u4"), ("reserved", "<u4")])
+                        ("break_force", "<f4"), ("break_torque", "<f4"), ("impulse", "<f4", 3), ("position", "<f4"), ("broken", "<u4"), ("cone", "<f4")])
 assert JOINT_DRIVE.itemsize == 56
 
 # nb_ray, nb_ray_hit (48 bytes each)

@@ -39,14 +39,17 @@ struct RowLevels { u32 n = 0, levels = 0; std::vector<u32> level_off, order; std
 
 // The host side of a joint set (nb_joint_api.cuh): its levels (the device table holds the joints by level), per joint in upload order its
 // (type, a, b), and the number of rows the joints generate.
-struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; std::vector<uint8_t> unit_rel; };   // unit_rel: rel_rotation of unit length
+// unit_rel / unit_axis: rel_rotation / axis_a of unit length, as a drive that reads them needs.
+struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; std::vector<uint8_t> unit_rel, unit_axis; };
 
 // One joint's drive on the device (nb_joint_api.cuh; DESIGN.md section 8.17): one entry per joint in table order while a drive set exists,
-// flags = 0 for a joint without a drive.  row = the first of its appended rows; (sl, cl) / (su, cu) = the hinge limits' half-angle pairs;
-// position = (sh, ch) of a hinge or (dist, 0), as of the last row build.  nb_debug_read("joint_drives") returns the table as it stands.
+// flags = 0 for a joint without a drive.  row = the first of its appended rows; (sl, cl) / (su, cu) = the hinge or twist limits' half-angle
+// pairs; a CONE drive (section 8.20) keeps its half-angle pair (sc, cc) in motor_speed / max_motor_torque and the uploaded half-angle in
+// cone (0 otherwise).  position = (sh, ch) of a hinge, (dist, 0) or (s, 0) of a slider, the twist's pair or the swing's (ss, cs), as of the
+// last row build.  nb_debug_read("joint_drives") returns the table as it stands.
 struct JointDrive {
 	u32 flags, row; float lower, upper, sl, cl, su, cu;
-	float motor_speed, max_motor_torque, break_force, break_torque, position[2]; u32 broken, reserved;
+	float motor_speed, max_motor_torque, break_force, break_torque, position[2]; u32 broken; float cone;
 };
 // The host side of a drive set: the drive count, the appended rows (after the joints' own in the row buffer) and per drive in joint order
 // its (joint, flags), the structure nb_step's graph depends on.

@@ -8,11 +8,15 @@
 // Drives (nb_upload_joint_drives; DESIGN.md section 8.17) are one more table, JointDrive per joint in table order, that both kernels take as
 // an argument (null without a drive set).  A drive's rows (motor, lower, upper) sit after all joints' own rows, so that the joint table and
 // the own rows' offsets are the same with and without drives; k_joint_solve applies them after the joint's own rows.  The break test and the
-// broken flag live in k_joint_rows.  Included at the end of nb_api.cu.
+// broken flag live in k_joint_rows.  Sliders (FIXED + SLIDE) and ragdoll swing-cone and twist limits (BALL + CONE / TWIST; DESIGN.md section
+// 8.20) are drives too: a slider rewrites its joint's point rows, a cone takes the motor's slot and a twist limit the limit's.  Included at
+// the end of nb_api.cu.
 #pragma once
 
 __host__ __device__ __forceinline__ u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
-__host__ __device__ __forceinline__ u32 drive_row_count(u32 flags) { return (flags & NB_JOINT_MOTOR ? 1u : 0u) + (flags & NB_JOINT_LIMIT ? 2u : 0u); }
+__host__ __device__ __forceinline__ u32 drive_row_count(u32 flags) {
+	return (flags & (NB_JOINT_MOTOR | NB_JOINT_CONE) ? 1u : 0u) + (flags & (NB_JOINT_LIMIT | NB_JOINT_TWIST) ? 2u : 0u);
+}
 
 NB_DEV f3 neg3(f3 a) { return mk3(-a.x, -a.y, -a.z); }
 // Writes one row around its accumulated impulse.
@@ -35,12 +39,72 @@ NB_DEV void joint_row_zero(nb_constraint_row* row, const nb_joint& j) {
 NB_DEV float limit_bias(float C, float dt, float k) { return C > 0.0f ? C / dt : k * C; }
 
 // The break test of a BREAKABLE joint on the impulses the previous step left in its rows (own rows at `row`, appended ones at `drow`).
+// A distance joint's and a slider's appended rows are linear, every other joint's angular.
 NB_DEV bool joint_breaks(const nb_constraint_row* row, const nb_constraint_row* drow, u32 type, u32 flags, const JointDrive& d, float dt) {
 	float P = 0.0f, A = 0.0f;
+	const bool linear = type == NB_JOINT_DISTANCE || (flags & NB_JOINT_SLIDE);
 	for (u32 r = 0; r < joint_row_count(type); ++r) { const float x = row[r].impulse; if (type == NB_JOINT_DISTANCE || r < 3) P = P + x * x; else A = A + x * x; }
-	for (u32 r = 0; r < drive_row_count(flags); ++r) { const float x = drow[r].impulse; if (type == NB_JOINT_DISTANCE) P = P + x * x; else A = A + x * x; }
+	for (u32 r = 0; r < drive_row_count(flags); ++r) { const float x = drow[r].impulse; if (linear) P = P + x * x; else A = A + x * x; }
 	const float f = d.break_force * dt, t = d.break_torque * dt;
 	return P > f * f || A > t * t;
+}
+
+// The two unit vectors HINGE builds perpendicular to its axis u.
+NB_DEV void hinge_basis(f3 u, f3& t1, f3& t2) {
+	t1 = fabsf(u.x) < 0.57735f ? mk3(0.0f, u.z, -u.y) : mk3(-u.z, 0.0f, u.x);
+	t1 = mul3(t1, 1.0f / sqrtf(dot3(t1, t1)));
+	t2 = cross3(u, t1);
+}
+// qmul(q_a, rel_rotation), times conj(q_b) when b != 0: the rotation HINGE LIMIT, FIXED and the swing-twist limits measure.
+NB_DEV quat joint_rel(quat qa, const nb_joint& j, quat qb) {
+	const quat rel = { ld3(j.rel_rotation), j.rel_rotation[3] };
+	quat d = qmul(qa, rel);
+	if (j.b) { const quat cb = { neg3(qb.v), qb.s }; d = qmul(d, cb); }
+	return d;
+}
+
+// FIXED + SLIDE: the joint's point rows across the slide axis u (rows 0, 1) and along it (row 2, which applies nothing), and the drive's
+// rows on the slide coordinate s = dot(wb - wa, u).  sa = ra - err runs from a's position to b's anchor.
+NB_DEV void slider_rows(nb_constraint_row* row, nb_constraint_row* drow, const nb_joint& j, const JointDrive& d, u32 flags, f3 u, f3 ra, f3 rb,
+		f3 wa, f3 wb, float dt, float k, float* position) {
+	const f3 err = sub3(wa, wb), sa = sub3(ra, err);
+	f3 t1, t2;
+	hinge_basis(u, t1, t2);
+	joint_row_put(row + 0, j, t1, cross3(sa, t1), neg3(t1), neg3(cross3(rb, t1)), k * dot3(err, t1));
+	joint_row_put(row + 1, j, t2, cross3(sa, t2), neg3(t2), neg3(cross3(rb, t2)), k * dot3(err, t2));
+	const f3 cu = cross3(sa, u), cbu = cross3(rb, u);
+	joint_row_put(row + 2, j, u, cu, neg3(u), neg3(cbu), k * dot3(err, u), 0.0f, 0.0f);
+	const f3 nu = neg3(u), ncu = neg3(cu);   // J_s: lin_a = -u, ang_a = -cross(sa, u), lin_b = u, ang_b = cross(rb, u)
+	const float s = dot3(sub3(wb, wa), u);
+	if (flags & NB_JOINT_MOTOR) { const float lim = d.max_motor_torque * dt; joint_row_put(drow++, j, nu, ncu, u, cbu, -d.motor_speed, -lim, lim); }
+	if (flags & NB_JOINT_LIMIT) {
+		joint_row_put(drow + 0, j, nu, ncu, u, cbu, limit_bias(s - d.lower, dt, k), 0.0f, INFINITY);
+		joint_row_put(drow + 1, j, u, cu, nu, neg3(cbu), limit_bias(d.upper - s, dt, k), 0.0f, INFINITY);
+	}
+	position[0] = s;
+}
+
+// BALL + CONE / TWIST: the swing-twist split of the relative rotation d about the twist axis u, the cone row (in the motor's slot) and the
+// twist limit rows (HINGE LIMIT's rows on the twist's half-angle pair).
+NB_DEV void swing_twist_rows(nb_constraint_row* drow, const nb_joint& j, const JointDrive& d, u32 flags, f3 u, quat q, float dt, float k, float* position) {
+	const f3 zero = mk3(0.0f, 0.0f, 0.0f);
+	if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
+	const float a_ = dot3(q.v, u), sh = -a_, ch = q.s;
+	const f3 p = sub3(q.v, mul3(u, a_));
+	const float ss = sqrtf(dot3(p, p)), cs = sqrtf(sh * sh + ch * ch);
+	float st = 0.0f, ct = 1.0f;
+	if (cs > 0.0f) { const float r = 1.0f / cs; st = sh * r; ct = ch * r; }
+	if (flags & NB_JOINT_CONE) {   // (sc, cc) = (sin, cos) of cone / 2, in the motor's slots
+		const f3 n = ss > 0.0f ? mul3(p, 1.0f / ss) : zero;
+		joint_row_put(drow++, j, zero, neg3(n), zero, n, limit_bias(2.0f * (d.motor_speed * cs - d.max_motor_torque * ss), dt, k), 0.0f, INFINITY);
+	}
+	if (flags & NB_JOINT_TWIST) {
+		const f3 nu = neg3(u);
+		joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(2.0f * (st * d.cl - ct * d.sl), dt, k), 0.0f, INFINITY);
+		joint_row_put(drow + 1, j, zero, u, zero, nu, limit_bias(2.0f * (d.su * ct - d.cu * st), dt, k), 0.0f, INFINITY);
+		position[0] = st; position[1] = ct;
+	}
+	else { position[0] = ss; position[1] = cs; }
 }
 
 // One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints), and with a drive table its drive's rows.
@@ -89,22 +153,22 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			else joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length));
 			continue;
 		}
-		joint_row_put(row + 0, j, mk3(1.0f, 0.0f, 0.0f), mk3(0.0f, ra.z, -ra.y), mk3(-1.0f, 0.0f, 0.0f), mk3(0.0f, -rb.z, rb.y), k * err.x);
-		joint_row_put(row + 1, j, mk3(0.0f, 1.0f, 0.0f), mk3(-ra.z, 0.0f, ra.x), mk3(0.0f, -1.0f, 0.0f), mk3(rb.z, 0.0f, -rb.x), k * err.y);
-		joint_row_put(row + 2, j, mk3(0.0f, 0.0f, 1.0f), mk3(ra.y, -ra.x, 0.0f), mk3(0.0f, 0.0f, -1.0f), mk3(-rb.y, rb.x, 0.0f), k * err.z);
+		if (flags & NB_JOINT_SLIDE) slider_rows(row, drow, j, d, flags, qrot(qa, ld3(j.axis_a)), ra, rb, wa, wb, dt, k, drives[i].position);
+		else {
+			joint_row_put(row + 0, j, mk3(1.0f, 0.0f, 0.0f), mk3(0.0f, ra.z, -ra.y), mk3(-1.0f, 0.0f, 0.0f), mk3(0.0f, -rb.z, rb.y), k * err.x);
+			joint_row_put(row + 1, j, mk3(0.0f, 1.0f, 0.0f), mk3(-ra.z, 0.0f, ra.x), mk3(0.0f, -1.0f, 0.0f), mk3(rb.z, 0.0f, -rb.x), k * err.y);
+			joint_row_put(row + 2, j, mk3(0.0f, 0.0f, 1.0f), mk3(ra.y, -ra.x, 0.0f), mk3(0.0f, 0.0f, -1.0f), mk3(-rb.y, rb.x, 0.0f), k * err.z);
+		}
 		if (type == NB_JOINT_HINGE) {
 			const f3 u = qrot(qa, ld3(j.axis_a)), w = j.b ? qrot(qb, ld3(j.axis_b)) : ld3(j.axis_b), c = cross3(u, w);
-			f3 t1 = fabsf(u.x) < 0.57735f ? mk3(0.0f, u.z, -u.y) : mk3(-u.z, 0.0f, u.x);
-			t1 = mul3(t1, 1.0f / sqrtf(dot3(t1, t1)));
-			const f3 t2 = cross3(u, t1);
+			f3 t1, t2;
+			hinge_basis(u, t1, t2);
 			joint_row_put(row + 3, j, zero, t1, zero, neg3(t1), -(k * dot3(c, t1)));
 			joint_row_put(row + 4, j, zero, t2, zero, neg3(t2), -(k * dot3(c, t2)));
 			const f3 nu = neg3(u);   // the hinge Jacobian: ang_a = -u, ang_b = u
 			if (flags & NB_JOINT_MOTOR) { const float lim = d.max_motor_torque * dt; joint_row_put(drow++, j, zero, nu, zero, u, -d.motor_speed, -lim, lim); }
 			if (flags & NB_JOINT_LIMIT) {
-				const quat rel = { ld3(j.rel_rotation), j.rel_rotation[3] };
-				quat q = qmul(qa, rel);
-				if (j.b) { const quat cb = { neg3(qb.v), qb.s }; q = qmul(q, cb); }
+				quat q = joint_rel(qa, j, qb);
 				if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
 				const float sh = -dot3(q.v, u), ch = q.s;
 				joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(2.0f * (sh * d.cl - ch * d.sl), dt, k), 0.0f, INFINITY);
@@ -113,14 +177,13 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			}
 		}
 		else if (type == NB_JOINT_FIXED) {
-			const quat rel = { ld3(j.rel_rotation), j.rel_rotation[3] };
-			quat d = qmul(qa, rel);
-			if (j.b) { const quat cb = { neg3(qb.v), qb.s }; d = qmul(d, cb); }
+			quat d = joint_rel(qa, j, qb);
 			if (d.s < 0.0f) d.v = neg3(d.v);
 			joint_row_put(row + 3, j, zero, mk3(1.0f, 0.0f, 0.0f), zero, mk3(-1.0f, 0.0f, 0.0f), k * (2.0f * d.v.x));
 			joint_row_put(row + 4, j, zero, mk3(0.0f, 1.0f, 0.0f), zero, mk3(0.0f, -1.0f, 0.0f), k * (2.0f * d.v.y));
 			joint_row_put(row + 5, j, zero, mk3(0.0f, 0.0f, 1.0f), zero, mk3(0.0f, 0.0f, -1.0f), k * (2.0f * d.v.z));
 		}
+		else if (flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) swing_twist_rows(drow, j, d, flags, qrot(qa, ld3(j.axis_a)), joint_rel(qa, j, qb), dt, k, drives[i].position);
 	}
 }
 
@@ -167,6 +230,11 @@ static bool unit_quat(const float* q) {
 	const double s = (double)q[0] * q[0] + (double)q[1] * q[1] + (double)q[2] * q[2] + (double)q[3] * q[3];
 	return fabs(s - 1.0) <= 1e-3;
 }
+// Whether axis_a has unit length within the same tolerance, as a slider's or a swing-twist limit's axis must.
+static bool unit_axis(const float* v) {
+	const double s = (double)v[0] * v[0] + (double)v[1] * v[1] + (double)v[2] * v[2];
+	return fabs(s - 1.0) <= 1e-3;
+}
 
 // What nb_upload_joints refuses in a joint of a context with B bodies (also applied to a loaded state file); null if the joint is valid.
 static const char* joint_problem(const nb_joint& j, u32 B) {
@@ -192,7 +260,7 @@ static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st
 	std::vector<nb_body_pair> ab(n);
 	for (u32 i = 0; i < n; ++i) {
 		ab[i].a = h[i].a; ab[i].b = h[i].b; js.structure.insert(js.structure.end(), { h[i].type, h[i].a, h[i].b });
-		js.unit_rel.push_back(unit_quat(h[i].rel_rotation) ? 1 : 0);
+		js.unit_rel.push_back(unit_quat(h[i].rel_rotation) ? 1 : 0); js.unit_axis.push_back(unit_axis(h[i].axis_a) ? 1 : 0);
 	}
 	if (int r = level_rows(ctx, std::move(ab), js, "joints")) return r;
 	std::vector<nb_joint> table(n);
@@ -233,31 +301,43 @@ static int get_joints(nb_context* ctx, std::vector<nb_joint>& out, cudaStream_t 
 	return NB_OK;
 }
 
-// What nb_upload_joint_drives refuses in a drive of a joint set given by its structure ((type, a, b) per joint) and unit_rel; null if valid.
-static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* structure, const uint8_t* unit_rel) {
+// What nb_upload_joint_drives refuses in a drive of a joint set given by its structure ((type, a, b) per joint), unit_rel and unit_axis; null
+// if valid.
+static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
 	if (d.joint >= nj) return "a joint index at or beyond the joint count";
-	if (d.flags & ~(u32)(NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE)) return "an unknown flag";
+	if (d.flags & ~(u32)(NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE | NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST)) return "an unknown flag";
 	const u32 type = structure[3 * (size_t)d.joint];
-	const u32 takes = type == NB_JOINT_HINGE ? NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : type == NB_JOINT_DISTANCE ? NB_JOINT_LIMIT | NB_JOINT_BREAKABLE : NB_JOINT_BREAKABLE;
+	const u32 fixed = d.flags & NB_JOINT_SLIDE ? NB_JOINT_SLIDE | NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : NB_JOINT_SLIDE | NB_JOINT_BREAKABLE;
+	const u32 takes = type == NB_JOINT_HINGE ? NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : type == NB_JOINT_DISTANCE ? NB_JOINT_LIMIT | NB_JOINT_BREAKABLE
+		: type == NB_JOINT_FIXED ? fixed : NB_JOINT_CONE | NB_JOINT_TWIST | NB_JOINT_BREAKABLE;
 	if (d.flags & ~takes) return "a flag the joint's type does not take";
 	const float fields[] = { d.lower, d.upper, d.motor_speed, d.max_motor_torque, d.impulse[0], d.impulse[1], d.impulse[2], d.position };
 	for (float x : fields) if (!std::isfinite(x)) return "a field that is not finite";
 	for (float x : { d.break_force, d.break_torque }) if (!std::isfinite(x) && x != INFINITY) return "a threshold that is neither finite nor +inf";
 	if (d.max_motor_torque < 0.0f || d.break_force < 0.0f || d.break_torque < 0.0f) return "a negative torque or threshold";
 	if (d.broken > 1) return "broken is not 0 or 1";
+	const float pi = 3.14159265358979f;
 	if (d.flags & NB_JOINT_LIMIT) {
 		if (d.lower > d.upper) return "lower > upper";
-		const float pi = 3.14159265358979f;
 		if (type == NB_JOINT_HINGE && (d.lower < -pi || d.upper > pi)) return "a hinge limit outside [-pi, pi]";
 		if (type == NB_JOINT_DISTANCE && d.lower < 0.0f) return "a negative distance limit";
 		if (type == NB_JOINT_HINGE && !unit_rel[d.joint]) return "a HINGE LIMIT whose joint's rel_rotation is not of unit length";
 	}
+	if (d.flags & NB_JOINT_TWIST) {
+		if (d.lower > d.upper) return "lower > upper";
+		if (d.lower < -pi || d.upper > pi) return "a twist limit outside [-pi, pi]";
+	}
+	// a cone keeps its half-angle pair in the motor's slots of the device table
+	if ((d.flags & NB_JOINT_CONE) && !(d.cone > 0.0f && d.cone <= pi)) return "a cone outside (0, pi]";
+	if ((d.flags & NB_JOINT_CONE) && (d.motor_speed != 0.0f || d.max_motor_torque != 0.0f)) return "a CONE drive with a motor speed or torque";
+	if ((d.flags & (NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST)) && !unit_axis[d.joint]) return "a SLIDE, CONE or TWIST drive whose joint's axis_a is not of unit length";
+	if ((d.flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) && !unit_rel[d.joint]) return "a CONE or TWIST drive whose joint's rel_rotation is not of unit length";
 	return nullptr;
 }
-static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel) {
+static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
 	if (n && !h) { ctx->error = "null drive list"; return NB_ERR_ARGUMENT; }
 	for (u32 i = 0; i < n; ++i)
-		if (const char* p = drive_problem(h[i], nj, structure, unit_rel)) { ctx->error = "drive " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
+		if (const char* p = drive_problem(h[i], nj, structure, unit_rel, unit_axis)) { ctx->error = "drive " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
 	std::vector<u32> joints(n);
 	for (u32 i = 0; i < n; ++i) joints[i] = h[i].joint;
 	std::sort(joints.begin(), joints.end());
@@ -266,8 +346,8 @@ static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj,
 	return NB_OK;
 }
 
-// Installs n checked drives in place of the set: the table (one entry per joint in table order, with the limits' half-angle pairs) and the
-// appended rows holding the uploaded impulses, after the joints' own rows.
+// Installs n checked drives in place of the set: the table (one entry per joint in table order, with the limits' and the cone's half-angle
+// pairs) and the appended rows holding the uploaded impulses, after the joints' own rows.
 static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStream_t st) {
 	if (!n) { drop_drives(ctx); return NB_OK; }
 	const JointSet& js = ctx->jset;
@@ -286,13 +366,14 @@ static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStrea
 		const nb_joint_drive& d = h[at[p]];
 		JointDrive& e = table[p];
 		e.flags = d.flags; e.row = js.nrows + (u32)rows.size(); e.lower = d.lower; e.upper = d.upper;
-		if ((d.flags & NB_JOINT_LIMIT) && js.structure[3 * (size_t)d.joint] == NB_JOINT_HINGE) {
+		if (((d.flags & NB_JOINT_LIMIT) && js.structure[3 * (size_t)d.joint] == NB_JOINT_HINGE) || (d.flags & NB_JOINT_TWIST)) {
 			e.sl = (float)sin(0.5 * d.lower); e.cl = (float)cos(0.5 * d.lower); e.su = (float)sin(0.5 * d.upper); e.cu = (float)cos(0.5 * d.upper);
 		}
 		e.motor_speed = d.motor_speed; e.max_motor_torque = d.max_motor_torque; e.break_force = d.break_force; e.break_torque = d.break_torque;
 		e.broken = d.broken;
+		if (d.flags & NB_JOINT_CONE) { e.motor_speed = (float)sin(0.5 * d.cone); e.max_motor_torque = (float)cos(0.5 * d.cone); e.cone = d.cone; }
 		for (u32 k = 0; k < 3; ++k) {
-			if (!(d.flags & (k ? NB_JOINT_LIMIT : NB_JOINT_MOTOR))) continue;
+			if (!(d.flags & (k ? NB_JOINT_LIMIT | NB_JOINT_TWIST : NB_JOINT_MOTOR | NB_JOINT_CONE))) continue;
 			nb_constraint_row r;
 			memset(&r, 0, sizeof(r));
 			r.impulse = d.impulse[k];
@@ -337,9 +418,11 @@ static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStr
 		d.joint = joint; d.flags = e.flags; d.lower = e.lower; d.upper = e.upper; d.motor_speed = e.motor_speed; d.max_motor_torque = e.max_motor_torque;
 		d.break_force = e.break_force; d.break_torque = e.break_torque; d.broken = e.broken;
 		u32 r = e.row - js.nrows;
-		for (u32 k = 0; k < 3; ++k) if (e.flags & (k ? NB_JOINT_LIMIT : NB_JOINT_MOTOR)) d.impulse[k] = rows[r++].impulse;
-		if (e.flags & NB_JOINT_LIMIT)
-			d.position = js.structure[3 * (size_t)joint] == NB_JOINT_HINGE ? (float)(2.0 * atan2((double)e.position[0], (double)e.position[1])) : e.position[0];
+		for (u32 k = 0; k < 3; ++k) if (e.flags & (k ? NB_JOINT_LIMIT | NB_JOINT_TWIST : NB_JOINT_MOTOR | NB_JOINT_CONE)) d.impulse[k] = rows[r++].impulse;
+		const u32 type = js.structure[3 * (size_t)joint];
+		if (e.flags & (NB_JOINT_LIMIT | NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST))
+			d.position = type == NB_JOINT_HINGE || type == NB_JOINT_BALL ? (float)(2.0 * atan2((double)e.position[0], (double)e.position[1])) : e.position[0];
+		if (e.flags & NB_JOINT_CONE) { d.motor_speed = 0.0f; d.max_motor_torque = 0.0f; d.cone = e.cone; }
 	}
 	return NB_OK;
 }
@@ -371,7 +454,7 @@ int nb_download_joints(nb_context* ctx, nb_joint* h, uint32_t capacity, uint32_t
 int nb_upload_joint_drives(nb_context* ctx, const nb_joint_drive* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_upload_joint_drives");
 	const JointSet& js = ctx->jset;
-	if (int r = check_drives(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data())) return r;
+	if (int r = check_drives(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data(), js.unit_axis.data())) return r;
 	return set_drives(ctx, h, n, (cudaStream_t)stream);
 }
 

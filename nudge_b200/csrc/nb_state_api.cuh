@@ -243,9 +243,12 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	ok = ok && check_joints(ctx, joints, h.reserved[6], h.bodies) == NB_OK;
 	// the drives against the file's joints, through the upload's checks
 	const nb_joint_drive* drives = reinterpret_cast<const nb_joint_drive*>(hc.drives.data());
-	std::vector<u32> structure; std::vector<uint8_t> unit_rel;
-	for (u32 i = 0; ok && i < h.reserved[6]; ++i) { structure.insert(structure.end(), { joints[i].type, joints[i].a, joints[i].b }); unit_rel.push_back(unit_quat(joints[i].rel_rotation) ? 1 : 0); }
-	ok = ok && check_drives(ctx, drives, h.reserved[7], h.reserved[6], structure.data(), unit_rel.data()) == NB_OK;
+	std::vector<u32> structure; std::vector<uint8_t> unit_rel, unit_ax;
+	for (u32 i = 0; ok && i < h.reserved[6]; ++i) {
+		structure.insert(structure.end(), { joints[i].type, joints[i].a, joints[i].b });
+		unit_rel.push_back(unit_quat(joints[i].rel_rotation) ? 1 : 0); unit_ax.push_back(unit_axis(joints[i].axis_a) ? 1 : 0);
+	}
+	ok = ok && check_drives(ctx, drives, h.reserved[7], h.reserved[6], structure.data(), unit_rel.data(), unit_ax.data()) == NB_OK;
 	// the continuous-collision set: the upload's entry checks, bodies nonzero, in range and ascending (a kinematic body may keep its entry)
 	std::vector<nb_ccd_body> ccd(x.ccd_bodies);
 	ok = ok && (ccd.empty() || fread(ccd.data(), sizeof(nb_ccd_body), ccd.size(), f) == ccd.size());
