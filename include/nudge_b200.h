@@ -274,8 +274,11 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  *              ang_a = -u, ang_b = u.  The limits are converted once on the host at upload, each to its pair (sin(x/2), cos(x/2)), rounded from
  *              double to float32: (sl, cl) for lower, (su, cu) for upper.
  *   HINGE motor:       the hinge Jacobian, bias = -motor_speed, lo = -(max_motor_torque * dt), hi = max_motor_torque * dt.
- *   HINGE lower limit: C = 2 * (sh*cl - ch*sl), the hinge Jacobian;  upper: C = 2 * (su*ch - cu*sh), ang_a = u, ang_b = -u, lin_a = lin_b
- *              = 0 (the hinge Jacobian with its angular parts negated);  both bias = bias(C), lo = 0, hi = +inf.
+ *   Angle measure:     for the pair (s, c) = (sin x, cos x) of a half difference x in [-pi, pi],  m(s, c) = c >= 0 ? 2*s : (s >= 0 ?
+ *              4 - 2*s : -4 - 2*s):  continuous and increasing in x, with the sign of x, and (2/pi) * min(|2x|, pi) <= |m| <= |2x|.
+ *   HINGE lower limit: C = m(sh*cl - ch*sl, ch*cl + sh*sl) (x = (theta - lower) / 2), the hinge Jacobian;  upper: C = m(su*ch - cu*sh,
+ *              cu*ch + su*sh) (x = (upper - theta) / 2), ang_a = u, ang_b = -u, lin_a = lin_b = 0 (the hinge Jacobian with its angular
+ *              parts negated);  both bias = bias(C), lo = 0, hi = +inf.
  *   DISTANCE limit:    the joint's own row is written with lo = hi = 0 (it stays in place and applies nothing);  lower: the own row's
  *              Jacobian with C = dist - lower;  upper: that Jacobian negated with C = upper - dist;  both bias = bias(C), lo = 0, hi = +inf.
  *   Slider:    FIXED + SLIDE.  u = qrot(q_a, axis_a) is the slide axis, t1, t2 built from u exactly as HINGE builds them, sa = ra - err
@@ -294,7 +297,8 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  *   TWIST limit:       the HINGE lower and upper limit rows, on the hinge Jacobian about u, with (sh', ch') in place of (sh, ch); lower and
  *              upper in [-pi, pi] converted to (sl, cl), (su, cu) as for a hinge.
  *   CONE:      (sc, cc) = (sin, cos) of cone/2, converted on the host in double and rounded to float32;  C = 2 * (sc*cs - cc*ss);
- *              n = ss > 0 ? p * (1/ss) : (0, 0, 0) (a zero row has no effect);  ang_a = -n, ang_b = n, lin_a = lin_b = 0, bias = bias(C),
+ *              g = cross(qrot((-d.xyz, d.w), u), u), sg = sqrtf(dot(g, g)), n = sg > 0 ? g * (1/sg) : (0, 0, 0) (the direction in which
+ *              the swing changes fastest; a zero row has no effect);  ang_a = -n, ang_b = n, lin_a = lin_b = 0, bias = bias(C),
  *              lo = 0, hi = +inf.
  *   Breaking:  when k_joint_rows is about to rewrite a BREAKABLE joint's rows it takes the accumulated impulses the previous step left:
  *              P = the sum 0 + i*i in row order over the joint's linear rows (the point rows; DISTANCE's own and appended rows; a slider's

@@ -37,6 +37,16 @@ NB_DEV void joint_row_zero(nb_constraint_row* row, const nb_joint& j) {
 }
 // A limit row's bias: speculative while the coordinate is inside (C > 0), Baumgarte once past the bound.
 NB_DEV float limit_bias(float C, float dt, float k) { return C > 0.0f ? C / dt : k * C; }
+// An angle limit's C from (s, c) = (sin x, cos x) of the half difference x = (theta - stop) / 2, x in [-pi, pi]: 2 sin x while c >= 0, then
+// +-(4 - 2 |sin x|) with the sign of x.  Continuous and increasing in x, and (2/pi) * min(|2x|, pi) <= |C| <= |2x|: unlike 2 sin x it does not
+// fold back toward 0 past a half turn, where a wide range's far stop would otherwise cap the speed away from the near one.
+NB_DEV float angle_limit_measure(float s, float c) { const float t = 2.0f * s; return c >= 0.0f ? t : s >= 0.0f ? 4.0f - t : -4.0f - t; }
+// The lower and upper angle limit rows of HINGE LIMIT and TWIST on the hinge Jacobian about u, from the angle's half-angle pair (sh, ch).
+NB_DEV void angle_limit_rows(nb_constraint_row* drow, const nb_joint& j, const JointDrive& d, f3 u, float sh, float ch, float dt, float k) {
+	const f3 zero = mk3(0.0f, 0.0f, 0.0f), nu = neg3(u);
+	joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(angle_limit_measure(sh * d.cl - ch * d.sl, ch * d.cl + sh * d.sl), dt, k), 0.0f, INFINITY);
+	joint_row_put(drow + 1, j, zero, u, zero, nu, limit_bias(angle_limit_measure(d.su * ch - d.cu * sh, d.cu * ch + d.su * sh), dt, k), 0.0f, INFINITY);
+}
 
 // The break test of a BREAKABLE joint on the impulses the previous step left in its rows (own rows at `row`, appended ones at `drow`).
 // A distance joint's and a slider's appended rows are linear, every other joint's angular.
@@ -95,15 +105,15 @@ NB_DEV void swing_twist_rows(nb_constraint_row* drow, const nb_joint& j, const J
 	float st = 0.0f, ct = 1.0f;
 	if (cs > 0.0f) { const float r = 1.0f / cs; st = sh * r; ct = ch * r; }
 	if (flags & NB_JOINT_CONE) {   // (sc, cc) = (sin, cos) of cone / 2, in the motor's slots
-		const f3 n = ss > 0.0f ? mul3(p, 1.0f / ss) : zero;
+		// the swing's direction of steepest change: the axis that turns u toward conj(q) u (p, the swing's own axis, is that axis turned
+		// about u by half the twist)
+		const quat cq = { neg3(q.v), q.s };
+		const f3 g = cross3(qrot(cq, u), u);
+		const float sg = sqrtf(dot3(g, g));
+		const f3 n = sg > 0.0f ? mul3(g, 1.0f / sg) : zero;
 		joint_row_put(drow++, j, zero, neg3(n), zero, n, limit_bias(2.0f * (d.motor_speed * cs - d.max_motor_torque * ss), dt, k), 0.0f, INFINITY);
 	}
-	if (flags & NB_JOINT_TWIST) {
-		const f3 nu = neg3(u);
-		joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(2.0f * (st * d.cl - ct * d.sl), dt, k), 0.0f, INFINITY);
-		joint_row_put(drow + 1, j, zero, u, zero, nu, limit_bias(2.0f * (d.su * ct - d.cu * st), dt, k), 0.0f, INFINITY);
-		position[0] = st; position[1] = ct;
-	}
+	if (flags & NB_JOINT_TWIST) { angle_limit_rows(drow, j, d, u, st, ct, dt, k); position[0] = st; position[1] = ct; }
 	else { position[0] = ss; position[1] = cs; }
 }
 
@@ -171,8 +181,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 				quat q = joint_rel(qa, j, qb);
 				if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
 				const float sh = -dot3(q.v, u), ch = q.s;
-				joint_row_put(drow + 0, j, zero, nu, zero, u, limit_bias(2.0f * (sh * d.cl - ch * d.sl), dt, k), 0.0f, INFINITY);
-				joint_row_put(drow + 1, j, zero, u, zero, nu, limit_bias(2.0f * (d.su * ch - d.cu * sh), dt, k), 0.0f, INFINITY);
+				angle_limit_rows(drow, j, d, u, sh, ch, dt, k);
 				drives[i].position[0] = sh; drives[i].position[1] = ch;
 			}
 		}

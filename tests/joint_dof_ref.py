@@ -10,7 +10,7 @@ import numpy as np
 from nudge_b200 import ROW
 from oracle.joints_ref import ROWS_PER_TYPE, BALL, HINGE, FIXED, DISTANCE, ZERO, f, _v, add, sub, dot, neg, scale, cross, qrot, qmul, \
     joint_rows as own_rows
-from tests.joint_drives_ref import LIMIT, MOTOR, BREAKABLE, half_angle
+from tests.joint_drives_ref import LIMIT, MOTOR, BREAKABLE, half_angle, angle_limit_biases
 
 SLIDE, CONE, TWIST = 16, 32, 64
 # the device table of nb_debug_read("joint_drives"): one entry per joint (flags 0: none); a CONE drive's (sc, cc) sit in the motor slots
@@ -176,8 +176,9 @@ def joint_rows(joints, transforms, dt, drives=None, drive_impulse=None):
                 if fl & LIMIT:
                     q = relative(j, transforms)
                     sh, ch = -dot(q[:3], u), q[3]
-                    extra.append((ZERO, nu, ZERO, u, limit_bias(f(2.0) * (sh * e["cl"] - ch * e["sl"])), z, inf))
-                    extra.append((ZERO, u, ZERO, nu, limit_bias(f(2.0) * (e["su"] * ch - e["cu"] * sh)), z, inf))
+                    lo_bias, hi_bias = angle_limit_biases(sh, ch, e, limit_bias)
+                    extra.append((ZERO, nu, ZERO, u, lo_bias, z, inf))
+                    extra.append((ZERO, u, ZERO, nu, hi_bias, z, inf))
                     e["position"][0], e["position"][1] = sh, ch
             if typ == FIXED and fl & SLIDE:
                 u = qrot(qa, _v(j["axis_a"]))
@@ -197,14 +198,18 @@ def joint_rows(joints, transforms, dt, drives=None, drive_impulse=None):
                 e["position"][0] = s
             if typ == BALL and fl & (CONE | TWIST):
                 u = qrot(qa, _v(j["axis_a"]))
-                p, ss, cs, st, ct = swing_twist(relative(j, transforms), u)
+                q = relative(j, transforms)
+                p, ss, cs, st, ct = swing_twist(q, u)
                 if fl & CONE:
-                    nv = scale(p, f(1.0) / ss) if ss > 0 else ZERO
+                    c = cross(qrot(neg(q[:3]) + (q[3],), u), u)
+                    sc = np.sqrt(dot(c, c))
+                    nv = scale(c, f(1.0) / sc) if sc > 0 else ZERO
                     extra.append((ZERO, neg(nv), ZERO, nv, limit_bias(f(2.0) * (e["motor_speed"] * cs - e["max_motor_torque"] * ss)), z, inf))
                 if fl & TWIST:
                     nu = neg(u)
-                    extra.append((ZERO, nu, ZERO, u, limit_bias(f(2.0) * (st * e["cl"] - ct * e["sl"])), z, inf))
-                    extra.append((ZERO, u, ZERO, nu, limit_bias(f(2.0) * (e["su"] * ct - e["cu"] * st)), z, inf))
+                    lo_bias, hi_bias = angle_limit_biases(st, ct, e, limit_bias)
+                    extra.append((ZERO, nu, ZERO, u, lo_bias, z, inf))
+                    extra.append((ZERO, u, ZERO, nu, hi_bias, z, inf))
                 e["position"][0], e["position"][1] = (st, ct) if fl & TWIST else (ss, cs)
             for la, aa, lb, ab, bias, lo, hi in extra:
                 r = out[m]

@@ -24,6 +24,19 @@ def half_angle(x):
     return f(np.sin(0.5 * np.float64(f(x)))), f(np.cos(0.5 * np.float64(f(x))))
 
 
+def angle_limit_measure(s, c):
+    """An angle limit's C from (s, c) = (sin x, cos x) of the half difference x = (angle - stop) / 2: 2 sin x while c >= 0, then
+    +-(4 - 2 |sin x|) with the sign of x (float32 add, multiply and compare only)."""
+    t = f(2.0) * s
+    return t if c >= 0 else (f(4.0) - t if s >= 0 else f(-4.0) - t)
+
+
+def angle_limit_biases(sh, ch, e, limit_bias):
+    """The lower and upper angle limit rows' biases from the angle's half-angle pair (sh, ch) and the entry's limit pairs."""
+    return (limit_bias(angle_limit_measure(sh * e["cl"] - ch * e["sl"], ch * e["cl"] + sh * e["sl"])),
+            limit_bias(angle_limit_measure(e["su"] * ch - e["cu"] * sh, e["cu"] * ch + e["su"] * sh)))
+
+
 def drive_table(joints, drives):
     """The drive table for `joints` in the order given, from `drives` (nudge_b200.JOINT_DRIVE, joint = an index into `joints`): the entries of
     nb_upload_joint_drives with the half-angle pairs and each drive's first appended row; and the appended rows' impulses in row order."""
@@ -143,8 +156,9 @@ def joint_rows(joints, transforms, dt, drives=None, drive_impulse=None):
                     if q[3] < 0:
                         q = tuple(-x for x in q)
                     sh, ch = -dot(q[:3], u), q[3]
-                    extra.append((ZERO, nu, ZERO, u, limit_bias(f(2.0) * (sh * e["cl"] - ch * e["sl"])), z, inf))
-                    extra.append((ZERO, u, ZERO, nu, limit_bias(f(2.0) * (e["su"] * ch - e["cu"] * sh)), z, inf))
+                    lo_bias, hi_bias = angle_limit_biases(sh, ch, e, limit_bias)
+                    extra.append((ZERO, nu, ZERO, u, lo_bias, z, inf))
+                    extra.append((ZERO, u, ZERO, nu, hi_bias, z, inf))
                     e["position"][0], e["position"][1] = sh, ch
             for la, aa, lb, ab, bias, lo, hi in extra:
                 r = out[m]
