@@ -15,6 +15,8 @@
  *   nb_upload_contacts              <- "custom contacts can be added here" example/main.cpp:288
  *   nb_upload_constraint_rows       <- "custom constraint impulses"        example/main.cpp:316
  *   nb_upload_joints                <- no reference counterpart: the rows an application would rebuild for example/main.cpp:316 every step
+ *   nb_upload_joint_drives /
+ *   nb_upload_joint_springs         <- no reference counterpart: limits, motors and PD springs an application would build as rows every step
  *   nb_instance_matrices            <- the draw loops of render()          example/main.cpp:224-268 (helpers :53-110)
  *   nb_download_contact_events      <- a host diff of ContactData / ContactCache between steps (collision callbacks)
  *   nb_upload_collision_filters     <- no reference counterpart (the reference collides every overlapping pair)
@@ -359,6 +361,78 @@ typedef struct {
 int nb_upload_joint_drives(nb_context*, const nb_joint_drive* host, uint32_t n, void* stream);
 int nb_download_joint_drives(nb_context*, nb_joint_drive* host, uint32_t capacity, uint32_t* count, void* stream);
 
+/* Joint springs (PD actuators of robot arms and legs, vehicle suspension, bungee cords, powered ragdolls; DESIGN.md section 8.21): a joint
+ * coordinate pulled toward a target by a spring-damper given in physical units, built and solved by the joints' own kernels inside the step,
+ * so that an actuator needs no per-step host round trip.  The spring is Catto's soft step: the implicit (backward Euler) spring-damper
+ * m*x'' = -stiffness*(x - target) - damping*(x' - target_velocity) over one step is one ordinary constraint row, and for a single row one
+ * sweep of the row update gives exactly that step.  A spring set is a sparse table keyed by joint, like the drives: at most one spring per
+ * joint, naming it by its index in the current joint set's upload order; a joint may have a drive and a spring.
+ * Rows: HINGE, FIXED and DISTANCE springs have one spring row, BALL springs three.  k_joint_solve applies, per joint, its own rows, then its
+ * spring rows, then its drive rows (so limits act last and hold against a spring); the warm start follows the same order.  The spring rows sit
+ * in a row buffer of their own: nb_debug_read("joint_rows") is what it is without springs, and nb_debug_read("joint_spring_rows") returns
+ * the spring rows, per sprung joint in the joint table's order.  Same arithmetic rules as the joints' section (float32, left to right, no
+ * fused multiply-adds), dt the step's time step:
+ *   Spring row:  on a coordinate C with Jacobian J, of the joint's a and b:  den = damping + dt * stiffness;  softness = 1.0f / (dt * den);
+ *              bias = (stiffness * C - damping * target_velocity) / den;  lo = -(max_force * dt), hi = max_force * dt;  reserved = 0.  The row
+ *              keeps its accumulated impulse from step to step.
+ *   HINGE:     J = the hinge Jacobian (lin_a = lin_b = 0, ang_a = -u, ang_b = u);  C = m(sh*ct - ch*st, ch*ct + sh*st) with (sh, ch) the HINGE
+ *              coordinate and m the angle measure of the drives' section, and (st, ct) = (sin, cos) of target / 2, converted on the host in
+ *              double and rounded to float32.  C is continuous and increasing in theta - target over [-2pi, 2pi] and exact to first order at
+ *              the target; it never pushes across the +-pi seam, so a spring does not take the short way round through a limited hinge's gap
+ *              (a target near +pi and an angle near -pi pull the long way, the way a LIMIT lets the hinge turn).  Needs a unit rel_rotation.
+ *   FIXED:     J = J_s and C = s - target, with the slider's coordinate s = dot(wb - wa, u), u = qrot(q_a, axis_a), and sa = ra - err.  Meant
+ *              for a FIXED joint with a SLIDE drive; without one the joint's point rows hold s and the spring only adds load, bounded by
+ *              max_force (not refused, so that springs need not follow drive uploads).  Needs a unit axis_a.
+ *   DISTANCE:  J = the joint's own row's Jacobian and C = dist - target.  A sprung distance joint's own row is written with lo = hi = 0 (it
+ *              stays in place and applies nothing), as with LIMIT: the joint becomes a spring-damper, and with LIMIT a bungee with a range.
+ *   BALL:      three rows.  d = qmul(q_a, target);  b != 0: d = qmul(d, (-q_b.xyz, q_b.w));  if d.w < 0: d = -d (all four).  Row e = x, y, z:
+ *              lin_a = lin_b = 0, ang_a = e, ang_b = -e, C = 2 * d.e (FIXED's angular rows on the target rotation).  max_force bounds each
+ *              row on its own (a box, not a ball).
+ *   Breaking:  spring rows are not counted in the break test; a broken joint's spring rows are written as zero rows, like its drive rows.
+ *   position:  each build of an unbroken spring records its coordinate: (sh, ch) for a HINGE, s for FIXED, dist for DISTANCE,
+ *              (sqrtf(dot(d.xyz, d.xyz)), d.w) for a BALL.
+ * nb_upload_joint_springs replaces the spring set (n = 0 removes it); impulse[] warm-starts the spring rows; position is ignored and reads 0
+ * until the next row build.  Every entry is checked on the host before any device work, and an error changes nothing.  NB_ERR_ARGUMENT: a
+ * null pointer with n > 0; a joint index at or beyond the joint count, or two springs on one joint; reserved != 0; a field that is not finite
+ * other than max_force = +inf; a negative stiffness, damping or max_force; stiffness = damping = 0; a stiffness or damping that is neither 0
+ * nor in [1e-12, 1e12]; |target_velocity| > 1e12; a FIXED or DISTANCE target beyond 1e12 in magnitude; a nonzero target word the joint's type
+ * does not read; a HINGE target outside [-pi, pi] (pi rounded to float32) or whose joint's rel_rotation is not of unit length (as for HINGE
+ * LIMIT); a negative DISTANCE target; a FIXED spring whose joint's axis_a is not of unit length; a BALL spring with a nonzero
+ * target_velocity or a target with |x*x + y*y + z*z + w*w - 1| > 1e-3 (in double).  Within these bounds every spring row is finite for
+ * time steps 1e-6 <= dt <= 1 (dt * den >= 1e-24, so softness <= 1e24, and |bias| <= |C| / dt + |target_velocity|) as long as the
+ * coordinate is finite and within about 1e20 of its target.  The upload sets the idle counter of every dynamic body of a sprung joint to 0
+ * (one launch; not body 0, not a kinematic body), so that a new target reaches a body that has fallen asleep; a joint drive upload wakes
+ * nothing.  Asynchronous on `stream`, staged like nb_upload_joints; it synchronises only when the spring table, the row buffer or the wake's
+ * index buffer must grow.  nb_step re-records its graph only when the spring structure (which
+ * joints) changed or a buffer moved: new targets, gains, bounds or impulses for the same joints keep it, so targets may be uploaded every step.
+ * nb_download_joint_springs returns the springs in joint-index order, the target as uploaded, impulse[] = the spring rows' current
+ * accumulated impulses (0 where a row is absent), and position: 2*atan2(sh, ch) in double, rounded to float32, for a HINGE (its angle), s for
+ * FIXED, dist for DISTANCE, 2*atan2 of the recorded pair for a BALL (the angle between the rotation and the target).  *count = the number of
+ * springs; NB_ERR_CAPACITY when capacity is smaller.  Synchronises.
+ * The set follows its joints as the drives do: nb_upload_joints keeps it when the joint structure is unchanged and removes it otherwise;
+ * nb_remove_bodies drops the springs of deleted joints and renumbers the rest; nb_add_bodies leaves it alone; nb_upload_bodies removes it with
+ * the joints.  Snapshots carry it; nb_save_state writes it (state version 9) and nb_load_state installs it through the upload's checks; a
+ * file of an older version removes it.  nb_debug_read("joint_springs") returns the device table: one 64-byte entry per joint in table order,
+ * { present, first spring row, target[4] (a HINGE: st, ct, 0, 0), target_velocity, stiffness, damping, max_force, position[2] (sh, ch; s, 0;
+ * dist, 0; |d.xyz|, d.w), target angle (HINGE; else 0), reserved[3] = 0 }, all 0 for a joint without a spring.
+ * Cost: no launch in the step; k_joint_rows and k_joint_solve take the spring table and rows as two more arguments (null without a set), and without a
+ * set the joints' rows, the launches and the graph are what they are without this feature. */
+typedef struct {
+	uint32_t joint;             /* index of the joint in the current set's upload order */
+	uint32_t reserved;          /* must be 0 */
+	float target[4];            /* HINGE: the target angle (rad) in [0], -pi <= target <= pi;  FIXED: the target slide coordinate s in [0];
+	                               DISTANCE: the target length >= 0 in [0];  BALL: the target relative rotation conj(q_a) * q_b as (x, y, z, w),
+	                               rel_rotation's convention.  Words a type does not read must be 0 */
+	float target_velocity;      /* HINGE rad/s, FIXED and DISTANCE units/s; BALL: must be 0 */
+	float stiffness;            /* 0 or in [1e-12, 1e12]: force per unit or torque per radian */
+	float damping;              /* 0 or in [1e-12, 1e12]; stiffness + damping > 0 */
+	float max_force;            /* >= 0 or +inf: every spring row's impulse stays in [-max_force*dt, max_force*dt] (a torque for HINGE and BALL) */
+	float impulse[3];           /* the spring rows' accumulated impulses: warm start on upload, result on download (BALL 3 rows, else 1) */
+	float position;             /* download: the coordinate at the last row build; ignored on upload */
+} nb_joint_spring;              /* 56 bytes */
+int nb_upload_joint_springs(nb_context*, const nb_joint_spring* host, uint32_t n, void* stream);
+int nb_download_joint_springs(nb_context*, nb_joint_spring* host, uint32_t capacity, uint32_t* count, void* stream);
+
 /* Contact events (collision callbacks; DESIGN.md section 8.5): which collider pairs started or stopped touching, computed on the device inside
  * nb_write_cached_impulses (so the stage calls, nb_step and its graph replay give the same stream).  A pair (key tags = A | (uint64)B << 32,
  * the pair word of nb_contact_data.tags) is touching after a step if the contact cache that step wrote holds an entry with that key (the
@@ -615,7 +689,9 @@ int nb_stream_synchronize(nb_context*, void* stream);
  * drives writes version 7 (reserved[7] = the drive count, the nb_joint_drive rows after the joints); loading a file of versions 1-6 removes
  * the context's drives.  A context with a continuous-collision set writes version 8 (a 16-byte header extension holding the entry count,
  * the nb_ccd_body rows last); loading a file of versions 1-7 removes the context's set.  Without a set a context writes what it wrote
- * before version 8 existed, byte for byte. */
+ * before version 8 existed, byte for byte.  A context with joint springs writes version 9 (the extension as in version 8 with reserved[0] =
+ * the spring count, the nb_joint_spring rows after the nb_ccd_body rows, padded to 16 bytes); loading a file of versions 1-8 removes the
+ * context's springs, and without springs a context writes what it wrote before version 9 existed. */
 int nb_save_state(nb_context*, const char* path, void* stream);
 int nb_load_state(nb_context*, const char* path, void* stream);
 int nb_state_info(const char* path, uint32_t counts[5] /* bodies, boxes, spheres, connections, cache entries */);

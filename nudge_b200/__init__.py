@@ -27,7 +27,8 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_add_bodies", "nb_remove_bodies", "nb_download_colliders", "nb_download_connections",
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
            "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap",
-           "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives", "nb_get_body_states", "nb_set_body_states"]
+           "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives", "nb_get_body_states", "nb_set_body_states",
+           "nb_upload_joint_springs", "nb_download_joint_springs"]
 
 
 class Config(C.Structure):
@@ -101,6 +102,8 @@ def load_library():
         lib.nb_download_joints.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_upload_joint_drives.argtypes = [V, V, C.c_uint32, V]
         lib.nb_download_joint_drives.argtypes = [V, V, C.c_uint32, V, V]
+        lib.nb_upload_joint_springs.argtypes = [V, V, C.c_uint32, V]
+        lib.nb_download_joint_springs.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_instance_matrices.argtypes = [V, V, C.c_uint32, C.c_int, V, V]
         lib.nb_shard_build_plan.argtypes = [V, C.c_uint32, V, V, C.c_uint32, C.c_uint32, V, V, V, V, V, V, V, V]
         lib.nb_shard_local_scene.argtypes = [V, C.c_uint32, V, C.c_uint32, C.c_uint32, V, C.c_uint32, V, C.c_uint32, V, V, V, V, V]
@@ -173,6 +176,7 @@ JOINT = abi.JOINT
 JOINT_BALL, JOINT_HINGE, JOINT_FIXED, JOINT_DISTANCE = 0, 1, 2, 3
 JOINT_DRIVE = abi.JOINT_DRIVE
 JOINT_LIMIT, JOINT_MOTOR, JOINT_BREAKABLE, JOINT_SLIDE, JOINT_CONE, JOINT_TWIST = 1, 2, 4, 16, 32, 64
+JOINT_SPRING = abi.JOINT_SPRING
 
 
 def nccl_unique_id():
@@ -455,6 +459,20 @@ class Sim(abi.HostState):
         self.lib.nb_download_joint_drives(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there are none)
         out = np.zeros(n.value, JOINT_DRIVE)
         self._ck(self.lib.nb_download_joint_drives(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_joint_drives")
+        return out
+
+    def upload_joint_springs(self, springs):
+        """Replaces the joint spring set (position targets with stiffness and damping) with `springs` (JOINT_SPRING rows; none removes it).
+        Asynchronous; the array may be reused on return."""
+        d = np.ascontiguousarray(np.asarray(springs if springs is not None else [], JOINT_SPRING).reshape(-1))
+        self._ck(self.lib.nb_upload_joint_springs(self.ctx, abi.ptr(d) if len(d) else None, len(d), self.stream), "nb_upload_joint_springs")
+
+    def download_joint_springs(self):
+        """The springs in joint order with their rows' current impulses and position."""
+        n = C.c_uint32(0)
+        self.lib.nb_download_joint_springs(self.ctx, None, 0, C.byref(n), self.stream)   # the count (NB_ERR_CAPACITY unless there are none)
+        out = np.zeros(n.value, JOINT_SPRING)
+        self._ck(self.lib.nb_download_joint_springs(self.ctx, abi.ptr(out) if len(out) else None, len(out), C.byref(n), self.stream), "nb_download_joint_springs")
         return out
 
     # ---- renderer read-back (example/main.cpp:224-268): one column-major 4x4 model matrix per collider, boxes first, then spheres ----

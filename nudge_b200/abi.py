@@ -49,6 +49,11 @@ JOINT_DRIVE = np.dtype([("joint", "<u4"), ("flags", "<u4"), ("lower", "<f4"), ("
                         ("break_force", "<f4"), ("break_torque", "<f4"), ("impulse", "<f4", 3), ("position", "<f4"), ("broken", "<u4"), ("cone", "<f4")])
 assert JOINT_DRIVE.itemsize == 56
 
+# nb_joint_spring (56 bytes)
+JOINT_SPRING = np.dtype([("joint", "<u4"), ("reserved", "<u4"), ("target", "<f4", 4), ("target_velocity", "<f4"), ("stiffness", "<f4"), ("damping", "<f4"),
+                         ("max_force", "<f4"), ("impulse", "<f4", 3), ("position", "<f4")])
+assert JOINT_SPRING.itemsize == 56
+
 # nb_ray, nb_ray_hit (48 bytes each)
 RAY = np.dtype([("origin", "<f4", 3), ("max_t", "<f4"), ("direction", "<f4", 3), ("mask", "<u4"), ("ignore_body", "<u4"), ("reserved", "<u4", 3)])
 RAY_HIT = np.dtype([("position", "<f4", 3), ("t", "<f4"), ("normal", "<f4", 3), ("collider", "<u4"), ("body", "<u4"), ("tag", "<u4"), ("reserved", "<u4", 2)])

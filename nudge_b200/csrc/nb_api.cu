@@ -51,9 +51,20 @@ struct JointDrive {
 	u32 flags, row; float lower, upper, sl, cl, su, cu;
 	float motor_speed, max_motor_torque, break_force, break_torque, position[2]; u32 broken; float cone;
 };
-// The host side of a drive set: the drive count, the appended rows (after the joints' own in the row buffer) and per drive in joint order
-// its (joint, flags), the structure nb_step's graph depends on.
-struct DriveSet { u32 n = 0, nrows = 0; std::vector<u32> structure; };
+// The host side of a sparse table keyed by joint (the drives, the springs): the entry count, the entries' rows and per entry in joint order
+// the structure nb_step's graph depends on: (joint, flags) of a drive, the joint of a spring.  A drive's rows follow the joints' own in the
+// joints' row buffer, a spring's sit in a row buffer of their own.
+struct KeyedSet { u32 n = 0, nrows = 0; std::vector<u32> structure; };
+using DriveSet = KeyedSet;
+// One joint's spring on the device (nb_upload_joint_springs, nb_joint_api.cuh; DESIGN.md section 8.21): one entry per joint in table order
+// while a spring set exists, present = 0 for a joint without a spring.  row = its first spring row; target = the uploaded words, for a HINGE
+// (st, ct) = (sin, cos) of target / 2 with the uploaded angle in `angle`; position = (sh, ch) of a hinge, (s, 0), (dist, 0), or (|d.xyz|,
+// d.w) of a BALL, as of the last row build.  nb_debug_read("joint_springs") returns the table as it stands.
+struct JointSpring {
+	u32 present, row; float target[4];
+	float target_velocity, stiffness, damping, max_force, position[2], angle; u32 reserved[3];
+};
+static_assert(sizeof(JointSpring) == 64, "JointSpring is 64 bytes");
 
 // The buffers of nb_collide's front end (launch_front_end); leaf_* = the AABBs in Morton order, keybits = the OR and AND of the Morton codes.
 // The context has one, the scene queries their own (nb_query_api.cuh), so that a query never touches what the step reads.
@@ -148,6 +159,8 @@ struct nb_context {
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
 	// joint drives (nb_upload_joint_drives, DESIGN.md section 8.17): the device table while dset.n, the rows appended after the joints' own in jrows
 	DevBuf<JointDrive> drives; DriveSet dset;
+	// joint springs (nb_upload_joint_springs, DESIGN.md section 8.21): the device table while sset.n, and the spring rows in a buffer of their own
+	DevBuf<JointSpring> springs; DevBuf<nb_constraint_row> srows; KeyedSet sset;
 	// continuous collision (nb_upload_ccd_bodies, DESIGN.md section 8.18, nb_ccd_api.cuh): ccd = the set (host copy, ascending by body) and
 	// ccd_rows its device copy; ccd_t = the advance's translation factor per body (max_bodies of them, 1 outside the set), allocated on the
 	// first upload; ccd_hits = (bits of t, collider) per entry of the last advance
@@ -1247,6 +1260,8 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
 		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ((size_t)ctx->jset.nrows + ctx->dset.nrows) },   // in table order: by joint level, upload order within one; then the drives' rows
 		{ "joint_drives", ctx->drives.p, ctx->dset.n ? sizeof(JointDrive) * (size_t)ctx->jset.n : 0 },
+		{ "joint_springs", ctx->springs.p, ctx->sset.n ? sizeof(JointSpring) * (size_t)ctx->jset.n : 0 },
+		{ "joint_spring_rows", ctx->srows.p, sizeof(nb_constraint_row) * (size_t)ctx->sset.nrows },   // per sprung joint in table order
 		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 		{ "ccd_hits", ctx->ccd_hits.p, sizeof(uint2) * ctx->ccd.size() },   // per entry of the last advance, in set order: (bits of t, collider)
 	};

@@ -11,22 +11,35 @@
 // broken flag live in k_joint_rows.  Sliders (FIXED + SLIDE) and ragdoll swing-cone and twist limits (BALL + CONE / TWIST; DESIGN.md section
 // 8.20) are drives too: a slider rewrites its joint's point rows, a cone takes the motor's slot and a twist limit the limit's.  Included at
 // the end of nb_api.cu.
+// Springs (nb_upload_joint_springs; DESIGN.md section 8.21) are a second sparse table keyed by joint, JointSpring per joint in table order,
+// that both kernels take with its rows (a buffer of their own; null without a spring set).  A spring row is Catto's soft step on one joint
+// coordinate; k_joint_solve applies a joint's spring rows after its own rows and before its drive rows.
 #pragma once
 
 __host__ __device__ __forceinline__ u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
 __host__ __device__ __forceinline__ u32 drive_row_count(u32 flags) {
 	return (flags & (NB_JOINT_MOTOR | NB_JOINT_CONE) ? 1u : 0u) + (flags & (NB_JOINT_LIMIT | NB_JOINT_TWIST) ? 2u : 0u);
 }
+__host__ __device__ __forceinline__ u32 spring_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : 1u; }
 
 NB_DEV f3 neg3(f3 a) { return mk3(-a.x, -a.y, -a.z); }
-// Writes one row around its accumulated impulse.
-NB_DEV void joint_row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float bias, float lo = -INFINITY, float hi = INFINITY) {
+// Writes one row around its accumulated impulse, with the joint's softness or, for a spring row, its own.
+NB_DEV void row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float bias, float lo, float hi, float softness) {
 	nb_constraint_row r;
 	r.a = j.a; r.b = j.b;
 	r.lin_a[0] = lin_a.x; r.lin_a[1] = lin_a.y; r.lin_a[2] = lin_a.z; r.ang_a[0] = ang_a.x; r.ang_a[1] = ang_a.y; r.ang_a[2] = ang_a.z;
 	r.lin_b[0] = lin_b.x; r.lin_b[1] = lin_b.y; r.lin_b[2] = lin_b.z; r.ang_b[0] = ang_b.x; r.ang_b[1] = ang_b.y; r.ang_b[2] = ang_b.z;
-	r.bias = bias; r.lo = lo; r.hi = hi; r.impulse = row->impulse; r.softness = j.softness; r.reserved = 0.0f;
+	r.bias = bias; r.lo = lo; r.hi = hi; r.impulse = row->impulse; r.softness = softness; r.reserved = 0.0f;
 	*row = r;
+}
+NB_DEV void joint_row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float bias, float lo = -INFINITY, float hi = INFINITY) {
+	row_put(row, j, lin_a, ang_a, lin_b, ang_b, bias, lo, hi, j.softness);
+}
+// A spring row on the coordinate C with the Jacobian (lin_a, ang_a, lin_b, ang_b): the implicit spring-damper of stiffness k and damping c
+// over one step is the row with softness 1 / (dt * (c + dt * k)) and bias (k * C - c * target_velocity) / (c + dt * k).
+NB_DEV void spring_row_put(nb_constraint_row* row, const nb_joint& j, f3 lin_a, f3 ang_a, f3 lin_b, f3 ang_b, float C, const JointSpring& sp, float dt) {
+	const float den = sp.damping + dt * sp.stiffness, lim = sp.max_force * dt;
+	row_put(row, j, lin_a, ang_a, lin_b, ang_b, (sp.stiffness * C - sp.damping * sp.target_velocity) / den, -lim, lim, 1.0f / (dt * den));
 }
 // A broken joint's row: everything zero but a and b.
 NB_DEV void joint_row_zero(nb_constraint_row* row, const nb_joint& j) {
@@ -118,7 +131,9 @@ NB_DEV void swing_twist_rows(nb_constraint_row* drow, const nb_joint& j, const J
 }
 
 // One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints), and with a drive table its drive's rows.
-__global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints, u32 n, const nb_transform* xf, float dt, nb_constraint_row* rows, JointDrive* drives) {
+// With a spring table the spring's rows at srows + row.
+__global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints, u32 n, const nb_transform* xf, float dt, nb_constraint_row* rows, JointDrive* drives,
+		JointSpring* springs, nb_constraint_row* srows) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const nb_joint j = joints[i];
 		const u32 type = j.type & 3u;
@@ -127,6 +142,9 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 		u32 flags = 0;
 		nb_constraint_row* drow = rows;
 		JointDrive d;
+		const JointSpring* sp = springs ? springs + i : nullptr;   // read where used: the entry is 16 words
+		const bool sprung = sp && sp->present;
+		nb_constraint_row* srow = sprung ? srows + sp->row : srows;
 		if (drives) {
 			d = drives[i];
 			flags = d.flags; drow = rows + d.row;
@@ -135,6 +153,7 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			if (broken) {
 				for (u32 r = 0; r < joint_row_count(type); ++r) joint_row_zero(row + r, j);
 				for (u32 r = 0; r < drive_row_count(flags); ++r) joint_row_zero(drow + r, j);
+				if (sprung) for (u32 r = 0; r < spring_row_count(type); ++r) joint_row_zero(srow + r, j);
 				continue;
 			}
 		}
@@ -154,13 +173,15 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			const float dist = sqrtf(dot3(err, err));
 			const f3 dir = dist > 0.0f ? mul3(err, 1.0f / dist) : mk3(0.0f, 1.0f, 0.0f);
 			const f3 ca = cross3(ra, dir), cb = neg3(cross3(rb, dir));
-			if (flags & NB_JOINT_LIMIT) {   // the own row stays in place with no force; the range rows push
-				joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length), 0.0f, 0.0f);
+			// with a limit or a spring the own row stays in place with no force; the range rows and the spring row push
+			if ((flags & NB_JOINT_LIMIT) || sprung) joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length), 0.0f, 0.0f);
+			else joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length));
+			if (flags & NB_JOINT_LIMIT) {
 				joint_row_put(drow + 0, j, dir, ca, neg3(dir), cb, limit_bias(dist - d.lower, dt, k), 0.0f, INFINITY);
 				joint_row_put(drow + 1, j, neg3(dir), neg3(ca), dir, neg3(cb), limit_bias(d.upper - dist, dt, k), 0.0f, INFINITY);
 				drives[i].position[0] = dist;
 			}
-			else joint_row_put(row, j, dir, ca, neg3(dir), cb, k * (dist - j.length));
+			if (sprung) { spring_row_put(srow, j, dir, ca, neg3(dir), cb, dist - sp->target[0], *sp, dt); springs[i].position[0] = dist; }
 			continue;
 		}
 		if (flags & NB_JOINT_SLIDE) slider_rows(row, drow, j, d, flags, qrot(qa, ld3(j.axis_a)), ra, rb, wa, wb, dt, k, drives[i].position);
@@ -177,12 +198,16 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			joint_row_put(row + 4, j, zero, t2, zero, neg3(t2), -(k * dot3(c, t2)));
 			const f3 nu = neg3(u);   // the hinge Jacobian: ang_a = -u, ang_b = u
 			if (flags & NB_JOINT_MOTOR) { const float lim = d.max_motor_torque * dt; joint_row_put(drow++, j, zero, nu, zero, u, -d.motor_speed, -lim, lim); }
-			if (flags & NB_JOINT_LIMIT) {
+			if ((flags & NB_JOINT_LIMIT) || sprung) {
 				quat q = joint_rel(qa, j, qb);
 				if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
 				const float sh = -dot3(q.v, u), ch = q.s;
-				angle_limit_rows(drow, j, d, u, sh, ch, dt, k);
-				drives[i].position[0] = sh; drives[i].position[1] = ch;
+				if (flags & NB_JOINT_LIMIT) { angle_limit_rows(drow, j, d, u, sh, ch, dt, k); drives[i].position[0] = sh; drives[i].position[1] = ch; }
+				if (sprung) {   // x = (theta - target) / 2 from the target's pair (st, ct)
+					const float st = sp->target[0], ct = sp->target[1];
+					spring_row_put(srow, j, zero, nu, zero, u, angle_limit_measure(sh * ct - ch * st, ch * ct + sh * st), *sp, dt);
+					springs[i].position[0] = sh; springs[i].position[1] = ch;
+				}
 			}
 		}
 		else if (type == NB_JOINT_FIXED) {
@@ -193,19 +218,43 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 			joint_row_put(row + 5, j, zero, mk3(0.0f, 0.0f, 1.0f), zero, mk3(0.0f, 0.0f, -1.0f), k * (2.0f * d.v.z));
 		}
 		else if (flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) swing_twist_rows(drow, j, d, flags, qrot(qa, ld3(j.axis_a)), joint_rel(qa, j, qb), dt, k, drives[i].position);
+		if (sprung && type == NB_JOINT_FIXED) {   // J_s and s as a slider has them
+			const f3 u = qrot(qa, ld3(j.axis_a)), sa = sub3(ra, err);
+			const float s = dot3(sub3(wb, wa), u);
+			spring_row_put(srow, j, neg3(u), neg3(cross3(sa, u)), u, cross3(rb, u), s - sp->target[0], *sp, dt);
+			springs[i].position[0] = s;
+		}
+		else if (sprung && type == NB_JOINT_BALL) {   // FIXED's angular rows on the target rotation
+			const quat t = { mk3(sp->target[0], sp->target[1], sp->target[2]), sp->target[3] };
+			quat q = qmul(qa, t);
+			if (j.b) { const quat cb = { neg3(qb.v), qb.s }; q = qmul(q, cb); }
+			if (q.s < 0.0f) { q.v = neg3(q.v); q.s = -q.s; }
+			spring_row_put(srow + 0, j, zero, mk3(1.0f, 0.0f, 0.0f), zero, mk3(-1.0f, 0.0f, 0.0f), 2.0f * q.v.x, *sp, dt);
+			spring_row_put(srow + 1, j, zero, mk3(0.0f, 1.0f, 0.0f), zero, mk3(0.0f, -1.0f, 0.0f), 2.0f * q.v.y, *sp, dt);
+			spring_row_put(srow + 2, j, zero, mk3(0.0f, 0.0f, 1.0f), zero, mk3(0.0f, 0.0f, -1.0f), 2.0f * q.v.z, *sp, dt);
+			springs[i].position[0] = sqrtf(dot3(q.v, q.v)); springs[i].position[1] = q.s;
+		}
 	}
 }
 
 // One thread per joint of the level [begin, end): the joint's rows one after the other, the two bodies' momentum kept in registers across them.
-// With a drive table the drive's rows follow the joint's own.
+// With a spring table the spring's rows follow the joint's own, and with a drive table the drive's rows come last.
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_solve(const nb_joint* joints, u32 begin, u32 end, nb_constraint_row* rows, nb_body_momentum* momentum,
-		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm, const JointDrive* drives) {
+		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm, const JointDrive* drives, const JointSpring* springs,
+		nb_constraint_row* srows) {
 	for (u32 i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
 		const u32 packed = joints[i].type, first = packed >> 2, count = joint_row_count(packed & 3u);
 		RowBodies s = row_bodies_load(joints[i].a, joints[i].b, momentum, props, inertia, kind);
 		for (u32 r = first; r < first + count; ++r) {
 			const float next = row_apply(rows[r], s, warm);
 			if (!warm) rows[r].impulse = next;
+		}
+		if (springs && springs[i].present) {
+			const u32 sfirst = springs[i].row, scount = spring_row_count(packed & 3u);
+			for (u32 r = sfirst; r < sfirst + scount; ++r) {
+				const float next = row_apply(srows[r], s, warm);
+				if (!warm) srows[r].impulse = next;
+			}
 		}
 		if (drives) {
 			const u32 dfirst = drives[i].row, dcount = drive_row_count(drives[i].flags);
@@ -223,16 +272,20 @@ static int launch_joints(nb_context* ctx, const float* dt, cudaStream_t st) {
 	const Launch L = mk_launch(ctx, st);
 	const JointSet& js = ctx->jset;
 	JointDrive* drives = ctx->dset.n ? ctx->drives.p : nullptr;
-	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p, drives);
+	JointSpring* springs = ctx->sset.n ? ctx->springs.p : nullptr;
+	nb_constraint_row* srows = ctx->sset.n ? ctx->srows.p : nullptr;
+	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p, drives, springs, srows);
 	for (u32 l = 0; l < js.levels; ++l)
 		launch_grid(L, k_joint_solve, GRID(js.level_off[l + 1] - js.level_off[l]), ctx->joints.p, js.level_off[l], js.level_off[l + 1], ctx->jrows.p, ctx->mom, ctx->props,
-			ctx->inertia, kin_table(ctx), dt ? 1 : 0, (const JointDrive*)drives);
+			ctx->inertia, kin_table(ctx), dt ? 1 : 0, (const JointDrive*)drives, (const JointSpring*)springs, srows);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
-static void drop_drives(nb_context* ctx) { if (ctx->dset.n) { ctx->dset = DriveSet(); ++ctx->graph_epoch; } }
-static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ctx->dset = DriveSet(); ++ctx->graph_epoch; } }
+static void drop_keyed(nb_context* ctx, KeyedSet& set) { if (set.n) { set = KeyedSet(); ++ctx->graph_epoch; } }
+static void drop_drives(nb_context* ctx) { drop_keyed(ctx, ctx->dset); }
+static void drop_springs(nb_context* ctx) { drop_keyed(ctx, ctx->sset); }
+static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ctx->dset = KeyedSet(); ctx->sset = KeyedSet(); ++ctx->graph_epoch; } }
 
 // Whether a quaternion has unit length within the tolerance a HINGE LIMIT drive asks of its joint's rel_rotation.
 static bool unit_quat(const float* q) {
@@ -282,9 +335,9 @@ static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st
 	GROW(ctx->joints, n, st); GROW(ctx->jrows, js.nrows, st);
 	CK(put_staged(ctx, ctx->joints.p, table.data(), sizeof(nb_joint) * (size_t)n, st));
 	CK(put_staged(ctx, ctx->jrows.p, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
-	// the levels are host values in nb_step's graph, the buffers its kernel arguments; the drives follow the structure (their rows stay
-	// beyond the joints' own, which the copy above leaves alone)
-	if (js.structure != ctx->jset.structure) drop_drives(ctx);
+	// the levels are host values in nb_step's graph, the buffers its kernel arguments; the drives and springs follow the structure (the
+	// drives' rows stay beyond the joints' own, which the copy above leaves alone)
+	if (js.structure != ctx->jset.structure) { drop_drives(ctx); drop_springs(ctx); }
 	if (js.structure != ctx->jset.structure || before[0] != ctx->joints.p || before[1] != ctx->jrows.p) ++ctx->graph_epoch;
 	ctx->jset = std::move(js);
 	return NB_OK;
@@ -343,16 +396,64 @@ static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* str
 	if ((d.flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) && !unit_rel[d.joint]) return "a CONE or TWIST drive whose joint's rel_rotation is not of unit length";
 	return nullptr;
 }
-static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
-	if (n && !h) { ctx->error = "null drive list"; return NB_ERR_ARGUMENT; }
+
+// Sparse tables keyed by joint (the drives, the springs) share their checks, their order and their installation.
+// The checks: a null list with n > 0, each entry's own problem (`problem`, null if none), two entries on one joint; `what` names an entry.
+template<class T, class Problem> static int check_keyed(nb_context* ctx, const T* h, u32 n, const char* what, Problem problem) {
+	if (n && !h) { ctx->error = std::string("null ") + what + " list"; return NB_ERR_ARGUMENT; }
 	for (u32 i = 0; i < n; ++i)
-		if (const char* p = drive_problem(h[i], nj, structure, unit_rel, unit_axis)) { ctx->error = "drive " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
+		if (const char* p = problem(h[i])) { ctx->error = std::string(what) + " " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
 	std::vector<u32> joints(n);
 	for (u32 i = 0; i < n; ++i) joints[i] = h[i].joint;
 	std::sort(joints.begin(), joints.end());
 	for (u32 i = 1; i < n; ++i)
-		if (joints[i] == joints[i - 1]) { ctx->error = "two drives on joint " + std::to_string(joints[i]); return NB_ERR_ARGUMENT; }
+		if (joints[i] == joints[i - 1]) { ctx->error = std::string("two ") + what + "s on joint " + std::to_string(joints[i]); return NB_ERR_ARGUMENT; }
 	return NB_OK;
+}
+// The checked entries in joint order, and per table position of the joint set the entry on that joint (-1: none).
+template<class T> static void keyed_order(const JointSet& js, const T* h, u32 n, std::vector<u32>& by_joint, std::vector<int>& at) {
+	by_joint.resize(n);
+	for (u32 i = 0; i < n; ++i) by_joint[i] = i;
+	std::sort(by_joint.begin(), by_joint.end(), [&](u32 x, u32 y) { return h[x].joint < h[y].joint; });
+	at.assign(js.n, -1);
+	for (u32 i : by_joint) at[js.order[h[i].joint]] = (int)i;
+}
+// Installs `next` in place of `cur`: the device table (one entry per joint in table order) staged into tbuf, and its rows into rbuf after
+// the first `keep` rows, which a larger row buffer keeps (the joints' own rows under the drives').  Synchronises only when the row buffer
+// grows.  The table and the rows are arguments of the joint kernels, null without a set, and the structure decides which rows
+// k_joint_solve applies: nb_step's graph is re-recorded when the structure changed or a buffer moved.
+template<class E> static int put_keyed(nb_context* ctx, KeyedSet& cur, KeyedSet&& next, DevBuf<E>& tbuf, const std::vector<E>& table,
+		DevBuf<nb_constraint_row>& rbuf, size_t keep, const std::vector<nb_constraint_row>& rows, cudaStream_t st) {
+	const void* before[2] = { tbuf.p, rbuf.p };
+	GROW(tbuf, table.size(), st);
+	const size_t need = keep + rows.size();
+	if (need > rbuf.cap) {
+		DevBuf<nb_constraint_row> b;
+		if (int r = b.alloc(ctx, need)) return r;
+		if (keep) CK(cudaMemcpyAsync(b.p, rbuf.p, sizeof(nb_constraint_row) * keep, cudaMemcpyDeviceToDevice, st));
+		CK(cudaStreamSynchronize(st));
+		std::swap(rbuf, b);
+	}
+	CK(put_staged(ctx, tbuf.p, table.data(), sizeof(E) * table.size(), st));
+	CK(put_staged(ctx, rbuf.p + keep, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
+	if (next.structure != cur.structure || before[0] != tbuf.p || before[1] != rbuf.p) ++ctx->graph_epoch;
+	cur = std::move(next);
+	return NB_OK;
+}
+// The host side of the download calls: the count, the capacity and null checks, then `get`.  Synchronises.
+template<class T> static int download_keyed(nb_context* ctx, T* h, u32 capacity, u32* count, u32 n, const char* what,
+		int (*get)(nb_context*, std::vector<T>&, cudaStream_t), cudaStream_t st) {
+	if (count) *count = n;
+	if (capacity < n) { ctx->error = std::string("host ") + what + " array too small: " + std::to_string(n) + " " + what + "s"; return NB_ERR_CAPACITY; }
+	if (n && !h) { ctx->error = std::string("null ") + what + " array"; return NB_ERR_ARGUMENT; }
+	std::vector<T> out;
+	if (int r = get(ctx, out, st)) return r;
+	std::copy(out.begin(), out.end(), h);
+	return NB_OK;
+}
+
+static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
+	return check_keyed(ctx, h, n, "drive", [&](const nb_joint_drive& d) { return drive_problem(d, nj, structure, unit_rel, unit_axis); });
 }
 
 // Installs n checked drives in place of the set: the table (one entry per joint in table order, with the limits' and the cone's half-angle
@@ -360,13 +461,12 @@ static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj,
 static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStream_t st) {
 	if (!n) { drop_drives(ctx); return NB_OK; }
 	const JointSet& js = ctx->jset;
-	std::vector<u32> by_joint(n);
-	for (u32 i = 0; i < n; ++i) by_joint[i] = i;
-	std::sort(by_joint.begin(), by_joint.end(), [&](u32 x, u32 y) { return h[x].joint < h[y].joint; });
+	std::vector<u32> by_joint;
+	std::vector<int> at;   // table position -> drive
+	keyed_order(js, h, n, by_joint, at);
 	DriveSet ds;
 	ds.n = n;
-	std::vector<int> at(js.n, -1);   // table position -> drive
-	for (u32 i : by_joint) { ds.structure.insert(ds.structure.end(), { h[i].joint, h[i].flags }); at[js.order[h[i].joint]] = (int)i; }
+	for (u32 i : by_joint) ds.structure.insert(ds.structure.end(), { h[i].joint, h[i].flags });
 	std::vector<JointDrive> table(js.n);
 	memset(table.data(), 0, sizeof(JointDrive) * table.size());
 	std::vector<nb_constraint_row> rows;
@@ -390,22 +490,7 @@ static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStrea
 		}
 	}
 	ds.nrows = (u32)rows.size();
-	const void* before[2] = { ctx->drives.p, ctx->jrows.p };
-	GROW(ctx->drives, js.n, st);
-	const size_t need = (size_t)js.nrows + ds.nrows;
-	if (need > ctx->jrows.cap) {   // a larger row buffer keeps the joints' own rows and their impulses
-		DevBuf<nb_constraint_row> b;
-		if (int r = b.alloc(ctx, need)) return r;
-		CK(cudaMemcpyAsync(b.p, ctx->jrows.p, sizeof(nb_constraint_row) * js.nrows, cudaMemcpyDeviceToDevice, st));
-		CK(cudaStreamSynchronize(st));
-		std::swap(ctx->jrows, b);
-	}
-	CK(put_staged(ctx, ctx->drives.p, table.data(), sizeof(JointDrive) * table.size(), st));
-	CK(put_staged(ctx, ctx->jrows.p + js.nrows, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
-	// the drive table is an argument of the joint kernels, null without a set; the structure decides which rows k_joint_solve applies
-	if (ds.structure != ctx->dset.structure || before[0] != ctx->drives.p || before[1] != ctx->jrows.p) ++ctx->graph_epoch;
-	ctx->dset = std::move(ds);
-	return NB_OK;
+	return put_keyed(ctx, ctx->dset, std::move(ds), ctx->drives, table, ctx->jrows, js.nrows, rows, st);
 }
 
 // The drives in joint-index order with their rows' current impulses, broken flags and positions.  Synchronises.
@@ -436,6 +521,98 @@ static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStr
 	return NB_OK;
 }
 
+// What nb_upload_joint_springs refuses in a spring of a joint set given by its structure, unit_rel and unit_axis (as drive_problem); null
+// if valid.
+static const char* spring_problem(const nb_joint_spring& s, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
+	if (s.joint >= nj) return "a joint index at or beyond the joint count";
+	if (s.reserved) return "reserved is not 0";
+	const float fields[] = { s.target[0], s.target[1], s.target[2], s.target[3], s.target_velocity, s.stiffness, s.damping, s.impulse[0], s.impulse[1],
+							 s.impulse[2], s.position };
+	for (float x : fields) if (!std::isfinite(x)) return "a field that is not finite";
+	if (!std::isfinite(s.max_force) && s.max_force != INFINITY) return "a max_force that is neither finite nor +inf";
+	if (s.stiffness < 0.0f || s.damping < 0.0f || s.max_force < 0.0f) return "a negative stiffness, damping or max_force";
+	if (s.stiffness == 0.0f && s.damping == 0.0f) return "stiffness and damping both 0";
+	// bounds under which every row is finite for 1e-6 <= dt <= 1 (include/nudge_b200.h): dt * den >= 1e-24, so softness <= 1e24, and
+	// |bias| <= |C| / dt + |target_velocity|
+	const float gmin = 1e-12f, gmax = 1e12f;
+	for (float x : { s.stiffness, s.damping }) if (x != 0.0f && (x < gmin || x > gmax)) return "a stiffness or damping outside {0} and [1e-12, 1e12]";
+	if (fabsf(s.target_velocity) > gmax) return "a target velocity beyond 1e12";
+	const u32 type = structure[3 * (size_t)s.joint];
+	if ((type == NB_JOINT_FIXED || type == NB_JOINT_DISTANCE) && fabsf(s.target[0]) > gmax) return "a target beyond 1e12";
+	if (type != NB_JOINT_BALL && (s.target[1] != 0.0f || s.target[2] != 0.0f || s.target[3] != 0.0f)) return "a nonzero target word the joint's type does not read";
+	const float pi = 3.14159265358979f;
+	if (type == NB_JOINT_HINGE && (s.target[0] < -pi || s.target[0] > pi)) return "a hinge target outside [-pi, pi]";
+	if (type == NB_JOINT_HINGE && !unit_rel[s.joint]) return "a HINGE spring whose joint's rel_rotation is not of unit length";
+	if (type == NB_JOINT_FIXED && !unit_axis[s.joint]) return "a FIXED spring whose joint's axis_a is not of unit length";
+	if (type == NB_JOINT_DISTANCE && s.target[0] < 0.0f) return "a negative distance target";
+	if (type == NB_JOINT_BALL && s.target_velocity != 0.0f) return "a BALL spring with a target velocity";
+	if (type == NB_JOINT_BALL && !unit_quat(s.target)) return "a BALL target rotation not of unit length";
+	return nullptr;
+}
+static int check_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
+	return check_keyed(ctx, h, n, "spring", [&](const nb_joint_spring& s) { return spring_problem(s, nj, structure, unit_rel, unit_axis); });
+}
+
+// Installs n checked springs in place of the set: the table (one entry per joint in table order, a hinge's target as its half-angle pair)
+// and the spring rows holding the uploaded impulses, per sprung joint in table order.
+static int set_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, cudaStream_t st) {
+	if (!n) { drop_springs(ctx); return NB_OK; }
+	const JointSet& js = ctx->jset;
+	std::vector<u32> by_joint;
+	std::vector<int> at;   // table position -> spring
+	keyed_order(js, h, n, by_joint, at);
+	KeyedSet ss;
+	ss.n = n;
+	for (u32 i : by_joint) ss.structure.push_back(h[i].joint);
+	std::vector<JointSpring> table(js.n);
+	memset(table.data(), 0, sizeof(JointSpring) * table.size());
+	std::vector<nb_constraint_row> rows;
+	for (u32 p = 0; p < js.n; ++p) {
+		if (at[p] < 0) continue;
+		const nb_joint_spring& s = h[at[p]];
+		const u32 type = js.structure[3 * (size_t)s.joint];
+		JointSpring& e = table[p];
+		e.present = 1; e.row = (u32)rows.size();
+		for (u32 k = 0; k < 4; ++k) e.target[k] = s.target[k];
+		if (type == NB_JOINT_HINGE) { e.target[0] = (float)sin(0.5 * s.target[0]); e.target[1] = (float)cos(0.5 * s.target[0]); e.angle = s.target[0]; }
+		e.target_velocity = s.target_velocity; e.stiffness = s.stiffness; e.damping = s.damping; e.max_force = s.max_force;
+		for (u32 k = 0; k < spring_row_count(type); ++k) {
+			nb_constraint_row r;
+			memset(&r, 0, sizeof(r));
+			r.impulse = s.impulse[k];
+			rows.push_back(r);
+		}
+	}
+	ss.nrows = (u32)rows.size();
+	return put_keyed(ctx, ctx->sset, std::move(ss), ctx->springs, table, ctx->srows, 0, rows, st);
+}
+
+// The springs in joint-index order with their rows' current impulses and positions.  Synchronises.
+static int get_springs(nb_context* ctx, std::vector<nb_joint_spring>& out, cudaStream_t st) {
+	const JointSet& js = ctx->jset;
+	const KeyedSet& ss = ctx->sset;
+	out.resize(ss.n);
+	if (!ss.n) return NB_OK;
+	std::vector<JointSpring> table(js.n);
+	std::vector<nb_constraint_row> rows(ss.nrows);
+	CK(cudaMemcpyAsync(table.data(), ctx->springs.p, sizeof(JointSpring) * table.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(rows.data(), ctx->srows.p, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	for (u32 m = 0; m < ss.n; ++m) {
+		const u32 joint = ss.structure[m], type = js.structure[3 * (size_t)joint];
+		const JointSpring& e = table[js.order[joint]];
+		nb_joint_spring& s = out[m];
+		memset(&s, 0, sizeof(s));
+		s.joint = joint;
+		for (u32 k = 0; k < 4; ++k) s.target[k] = e.target[k];
+		if (type == NB_JOINT_HINGE) { s.target[0] = e.angle; s.target[1] = 0.0f; }
+		s.target_velocity = e.target_velocity; s.stiffness = e.stiffness; s.damping = e.damping; s.max_force = e.max_force;
+		for (u32 k = 0; k < spring_row_count(type); ++k) s.impulse[k] = rows[e.row + k].impulse;
+		s.position = type == NB_JOINT_HINGE || type == NB_JOINT_BALL ? (float)(2.0 * atan2((double)e.position[0], (double)e.position[1])) : e.position[0];
+	}
+	return NB_OK;
+}
+
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_wake(const u32* bodies, u32 n, uint8_t* idle) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idle[bodies[i]] = 0;
 }
@@ -450,14 +627,7 @@ int nb_upload_joints(nb_context* ctx, const nb_joint* h, uint32_t n, void* strea
 
 int nb_download_joints(nb_context* ctx, nb_joint* h, uint32_t capacity, uint32_t* count, void* stream) {
 	NB_RANGE("nb_download_joints");
-	const u32 n = ctx->jset.n;
-	if (count) *count = n;
-	if (capacity < n) { ctx->error = "host joint array too small: " + std::to_string(n) + " joints"; return NB_ERR_CAPACITY; }
-	if (n && !h) { ctx->error = "null joint array"; return NB_ERR_ARGUMENT; }
-	std::vector<nb_joint> joints;
-	if (int r = get_joints(ctx, joints, (cudaStream_t)stream)) return r;
-	std::copy(joints.begin(), joints.end(), h);
-	return NB_OK;
+	return download_keyed(ctx, h, capacity, count, ctx->jset.n, "joint", get_joints, (cudaStream_t)stream);
 }
 
 int nb_upload_joint_drives(nb_context* ctx, const nb_joint_drive* h, uint32_t n, void* stream) {
@@ -469,14 +639,36 @@ int nb_upload_joint_drives(nb_context* ctx, const nb_joint_drive* h, uint32_t n,
 
 int nb_download_joint_drives(nb_context* ctx, nb_joint_drive* h, uint32_t capacity, uint32_t* count, void* stream) {
 	NB_RANGE("nb_download_joint_drives");
-	const u32 n = ctx->dset.n;
-	if (count) *count = n;
-	if (capacity < n) { ctx->error = "host drive array too small: " + std::to_string(n) + " drives"; return NB_ERR_CAPACITY; }
-	if (n && !h) { ctx->error = "null drive array"; return NB_ERR_ARGUMENT; }
-	std::vector<nb_joint_drive> drives;
-	if (int r = get_drives(ctx, drives, (cudaStream_t)stream)) return r;
-	std::copy(drives.begin(), drives.end(), h);
+	return download_keyed(ctx, h, capacity, count, ctx->dset.n, "drive", get_drives, (cudaStream_t)stream);
+}
+
+int nb_upload_joint_springs(nb_context* ctx, const nb_joint_spring* h, uint32_t n, void* stream) {
+	NB_RANGE("nb_upload_joint_springs");
+	const JointSet& js = ctx->jset;
+	if (int r = check_springs(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data(), js.unit_axis.data())) return r;
+	cudaStream_t st = (cudaStream_t)stream;
+	if (int r = set_springs(ctx, h, n, st)) return r;
+	// the sprung joints' dynamic bodies get idle counter 0, so that a new target reaches a body that has fallen asleep (k_joint_wake, as
+	// nb_remove_bodies wakes a joint's kept side); not body 0, not a kinematic body
+	std::vector<u32> wake;
+	for (u32 i = 0; i < n; ++i)
+		for (u32 k = 0; k < 2; ++k) {
+			const u32 b = js.structure[3 * (size_t)h[i].joint + 1 + k];
+			if (b && !std::binary_search(ctx->kin_list.begin(), ctx->kin_list.end(), b)) wake.push_back(b);
+		}
+	std::sort(wake.begin(), wake.end());
+	wake.erase(std::unique(wake.begin(), wake.end()), wake.end());
+	if (wake.empty()) return NB_OK;
+	GROW(ctx->spawn_idx, wake.size(), st);
+	CK(put_staged(ctx, ctx->spawn_idx.p, wake.data(), sizeof(u32) * wake.size(), st));
+	launch_grid(mk_launch(ctx, st), k_joint_wake, GRID(wake.size()), ctx->spawn_idx.p, (u32)wake.size(), ctx->idle);
+	CK(cudaGetLastError());
 	return NB_OK;
+}
+
+int nb_download_joint_springs(nb_context* ctx, nb_joint_spring* h, uint32_t capacity, uint32_t* count, void* stream) {
+	NB_RANGE("nb_download_joint_springs");
+	return download_keyed(ctx, h, capacity, count, ctx->sset.n, "spring", get_springs, (cudaStream_t)stream);
 }
 
 }  // extern "C"

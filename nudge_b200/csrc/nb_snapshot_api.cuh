@@ -2,14 +2,14 @@
 // section 8.12).
 //
 // A snapshot is the context's between-steps state in HBM: the sections of a state file (state_sections, nb_state_api.cuh) plus what a file
-// lacks, the user rows, the joint table, the joints' rows and the joint drive table, the continuous-collision set (host side), the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
+// lacks, the user rows, the joint table, the joints' rows, the joint drive table, the joint spring table and rows, the continuous-collision set (host side), the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
 // (snapshot_sections).  Save and restore are one launch of k_snapshot_copy in opposite directions; the host side (counts, bits, table set,
 // the connections' host copy, the kinematic set, the rows' levelling) is kept in the snapshot and installed by install_state.
 // Every section but the user rows, the joints and the overlap list has its room at the context's capacities in one arena, laid out once from the
 // capacity header; those are sized at the save and grown by it.  Included at the end of nb_api.cu.
 #pragma once
 
-#define NB_SNAP_SECTIONS 32
+#define NB_SNAP_SECTIONS 64   // two per lane of k_snapshot_copy's first warp
 
 // One section of k_snapshot_copy: `size` * n bytes from src to dst, n = min(*count_dev, count) when count_dev is given, else count.  src and
 // dst are 16-byte aligned unless the section is shorter than 16 bytes.
@@ -21,16 +21,21 @@ static const int kSnapWords[3] = { CNT_CACHE, CNT_EV_STEP, CNT_SENSOR_OLD };
 
 // The table is a kernel parameter.  Each block sizes the sections (device counts included) into a prefix of 16-byte chunks, then walks
 // the chunks of the concatenated live ranges grid-stride; a section's last chunk copies only its live bytes.
+static_assert(NB_SNAP_SECTIONS == 64, "k_snapshot_copy's first warp sizes two sections per lane");
+__device__ __forceinline__ u64 snap_section_bytes(const SnapTable& t, u32 i) {
+	if (i >= t.n) return 0;
+	const SnapSection& s = t.s[i];
+	return (u64)s.size * (s.count_dev ? min(*s.count_dev, s.count) : s.count);
+}
 __global__ void __launch_bounds__(NB_BLOCK) k_snapshot_copy(const __grid_constant__ SnapTable t) {
 	__shared__ u64 first[NB_SNAP_SECTIONS + 1];   // first chunk of each section; first[n] = the total
 	__shared__ u64 bytes[NB_SNAP_SECTIONS];
-	if (threadIdx.x < 32) {
+	if (threadIdx.x < 32) {   // lane i: sections 2i and 2i + 1
 		const u32 i = threadIdx.x;
-		u64 b = 0;
-		if (i < t.n) { const SnapSection& s = t.s[i]; b = (u64)s.size * (s.count_dev ? min(*s.count_dev, s.count) : s.count); }
-		u64 c = (b + 15) >> 4;
+		const u64 b0 = snap_section_bytes(t, 2 * i), b1 = snap_section_bytes(t, 2 * i + 1), c1 = (b1 + 15) >> 4;
+		u64 c = ((b0 + 15) >> 4) + c1;
 		for (int d = 1; d < 32; d <<= 1) { const u64 y = __shfl_up_sync(0xffffffffu, c, d); if (i >= (u32)d) c += y; }
-		bytes[i] = b; first[i + 1] = c;
+		bytes[2 * i] = b0; bytes[2 * i + 1] = b1; first[2 * i + 1] = c - c1; first[2 * i + 2] = c;
 		if (i == 0) first[0] = 0;
 	}
 	__syncthreads();
@@ -54,8 +59,9 @@ struct nb_snapshot {
 	DevBuf<uint4> overlaps;                          // the sensor overlap list
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows (the drives' appended rows included)
 	DevBuf<JointDrive> drives;                                  // the joint drive table
+	DevBuf<JointSpring> springs; DevBuf<nb_constraint_row> srows;   // the joint spring table and the spring rows
 	// the host side at the save
-	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset; DriveSet dset;
+	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset; DriveSet dset; KeyedSet sset;
 	std::vector<nb_ccd_body> ccd;                    // the continuous-collision set (its rows are host values; k_ccd rewrites the factors)
 };
 
@@ -67,7 +73,7 @@ struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool presen
 // null the snapshot pointers are offsets into the arena, and there are no rows or joints.
 static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 conn_probe) {
 	const JointSet none, &js = s ? s->jset : none;
-	const DriveSet dnone, &ds = s ? s->dset : dnone;
+	const KeyedSet knone, &ds = s ? s->dset : knone, &ss = s ? s->sset : knone;
 	const u32 nrows = s ? s->urow_set.n : 0;
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
@@ -81,6 +87,8 @@ static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapsho
 	p.push_back({ ctx->joints.p, s ? s->joints.p : nullptr, sizeof(nb_joint), js.n, js.n != 0, -1 });
 	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), (size_t)js.nrows + ds.nrows, js.n != 0, -1 });
 	p.push_back({ ctx->drives.p, s ? s->drives.p : nullptr, sizeof(JointDrive), js.n, ds.n != 0, -1 });
+	p.push_back({ ctx->springs.p, s ? s->springs.p : nullptr, sizeof(JointSpring), js.n, ss.n != 0, -1 });
+	p.push_back({ ctx->srows.p, s ? s->srows.p : nullptr, sizeof(nb_constraint_row), ss.nrows, ss.n != 0, -1 });
 	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
 	return p;
 }
@@ -167,9 +175,10 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	// grown: the only save that synchronises and allocates
 	GROW(s->rows, ctx->urow_set.n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
 	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, (size_t)ctx->jset.nrows + ctx->dset.nrows, st); GROW(s->drives, ctx->dset.n ? ctx->jset.n : 0, st);
+	GROW(s->springs, ctx->sset.n ? ctx->jset.n : 0, st); GROW(s->srows, ctx->sset.nrows, st);
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
-	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset; s->ccd = ctx->ccd;
+	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset; s->sset = ctx->sset; s->ccd = ctx->ccd;
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, true, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
@@ -187,8 +196,9 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->shape.has_frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
 	if (!s->shape.kin.empty()) ALLOC(ctx->kind, ctx->cfg.max_bodies);
 	GROW(ctx->urows, s->urow_set.n, st);
-	const void* joint_bufs[3] = { ctx->joints.p, ctx->jrows.p, ctx->drives.p };
+	const void* joint_bufs[5] = { ctx->joints.p, ctx->jrows.p, ctx->drives.p, ctx->springs.p, ctx->srows.p };
 	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, (size_t)s->jset.nrows + s->dset.nrows, st); GROW(ctx->drives, s->dset.n ? s->jset.n : 0, st);
+	GROW(ctx->springs, s->sset.n ? s->jset.n : 0, st); GROW(ctx->srows, s->sset.nrows, st);
 	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, false, t); if (r) return r; }
@@ -199,7 +209,8 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->urow_set.n != ctx->urow_set.n || s->urow_set.level_off != ctx->urow_set.level_off) ++ctx->graph_epoch;
 	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
 	else if (s->dset.structure != ctx->dset.structure || joint_bufs[2] != ctx->drives.p) ++ctx->graph_epoch;
-	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->dset = s->dset;
+	else if (s->sset.structure != ctx->sset.structure || joint_bufs[3] != ctx->springs.p || joint_bufs[4] != ctx->srows.p) ++ctx->graph_epoch;
+	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->dset = s->dset; ctx->sset = s->sset;
 	{ int r = set_ccd(ctx, s->ccd, st); if (r) return r; }   // nothing when the context holds the same set
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;

@@ -220,8 +220,10 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	std::vector<nb_joint> old_joints, joints;
 	std::vector<u32> joint_wake, joint_new(ctx->jset.n, ~0u);   // joint_new: old joint index -> new one (~0u: deleted)
 	std::vector<nb_joint_drive> drives;
+	std::vector<nb_joint_spring> springs;
 	if (int r = get_joints(ctx, old_joints, st)) return r;
 	if (int r = get_drives(ctx, drives, st)) return r;
+	if (int r = get_springs(ctx, springs, st)) return r;
 	for (u32 i = 0; i < old_joints.size(); ++i) {
 		nb_joint j = old_joints[i];
 		if (removed(j.a) || removed(j.b)) {
@@ -236,6 +238,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	// the drives of the kept joints, renumbered, with their current impulses and broken flags
 	std::vector<nb_joint_drive> kept_drives;
 	for (nb_joint_drive d : drives) if (joint_new[d.joint] != ~0u) { d.joint = joint_new[d.joint]; kept_drives.push_back(d); }
+	std::vector<nb_joint_spring> kept_springs;   // and the springs
+	for (nb_joint_spring s : springs) if (joint_new[s.joint] != ~0u) { s.joint = joint_new[s.joint]; kept_springs.push_back(s); }
 	const u32 nrows = kept.n;
 	const bool rows_changed = nrows != us.n;   // a deleted row can change the levels, which nb_step's graph holds
 	std::vector<u32> staging(list);   // the list, then the rows' gather permutation (new device position -> old one)
@@ -312,6 +316,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	}
 	if (!old_joints.empty()) { int r = set_joints(ctx, joints.data(), (u32)joints.size(), st); if (r) return r; }
 	if (!drives.empty()) { int r = set_drives(ctx, kept_drives.data(), (u32)kept_drives.size(), st); if (r) return r; }
+	if (!springs.empty()) { int r = set_springs(ctx, kept_springs.data(), (u32)kept_springs.size(), st); if (r) return r; }
 	if (int r = set_ccd(ctx, std::move(ccd), st)) return r;
 	return build_conn_lookup(ctx, st);
 }

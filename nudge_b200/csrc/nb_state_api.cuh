@@ -5,7 +5,7 @@
 //
 // File layout (little endian): header { char magic[8] = "NBSTATE1"; u32 version; u32 bodies, boxes, spheres, connections, cache;
 // u32 solver_mode; u32 reserved[8]; }, from version 8 a header extension { u32 ccd_bodies; u32 reserved[3]; }, and these sections in this
-// order (state_sections, then the continuous-collision rows), each padded with zeros to 16 bytes:
+// order (state_sections, then the continuous-collision rows and the joint springs), each padded with zeros to 16 bytes:
 //   section                                        element (B)  count            present when
 //   transforms | properties | momentum | idle      32 16 32 1   bodies           always
 //   box_tags | box_data | box_transforms           4 16 32      boxes            always
@@ -18,25 +18,29 @@
 //   body forces (nb_body_force rows, body = row)   48           bodies           reserved[5] != 0
 //   joints (nb_joint, upload order, current impulses) 112        reserved[6]      reserved[6] != 0
 //   joint drives (nb_joint_drive, joint order)      56           reserved[7]      reserved[7] != 0
-//   ccd bodies (nb_ccd_body, ascending by body)     16           ccd_bodies       version 8
+//   ccd bodies (nb_ccd_body, ascending by body)     16           ccd_bodies       version 8 or 9
+//   joint springs (nb_joint_spring, joint order)    56           ext reserved[0]  version 9
 // Each version defines more reserved words: version 2 reserved[0] = filter flags and reserved[1]; version 3 reserved[2] = 1 and
 // reserved[3] = max_sensor_pairs; version 4 reserved[2] = 0 or 1 and reserved[4] >= 1; version 5 reserved[2] = 0 or 1, reserved[4] >= 0 and
 // reserved[5] = 1; version 6 reserved[2] and reserved[5] = 0 or 1, reserved[4] >= 0 and reserved[6] >= 1; version 7 as 6 and reserved[7] >= 1;
 // version 8 as 7 with reserved[6] >= 0, reserved[7] >= 0 (drives only with joints) and ccd_bodies >= 1.  All eight reserved words being
-// taken, version 8 adds the extension.  A context writes version 8 with a continuous-collision set, else 7 with joint drives, else 6 with joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
+// taken, version 8 adds the extension.  Version 9 as 8 with ccd_bodies >= 0, reserved[6] >= 1 and the extension's reserved[0] >= 1 (the
+// spring count; the extension's reserved words are ignored before version 9).  A context writes version 9 with joint springs, else 8 with a
+// continuous-collision set, else 7 with joint drives, else 6 with joints, else 5 with a body force table, else 4 with a kinematic set, else 3 with sensors, else 2 with a
 // filter table or flags, else 1.  Every version loads; words a version does not define are ignored, and a file without a table or flags
 // removes the context's.  A kinematic body's velocities are its momentum row.
 #pragma once
 
 struct NbStateHeader { char magic[8]; u32 version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]; };
-struct NbStateExt { u32 ccd_bodies, reserved[3]; };   // version 8 on
+struct NbStateExt { u32 ccd_bodies, reserved[3]; };   // version 8 on; version 9: reserved[0] = the spring count
 
 // Reads and checks a state file's header and, from version 8, its extension (all zeros before), and zeroes the reserved words its version
 // does not define, so that each section's presence is a plain word test.
 static bool state_header_read(FILE* f, NbStateHeader& h, NbStateExt& x) {
 	memset(&x, 0, sizeof(x));
 	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "NBSTATE1", 8)) return false;
-	if (h.version == 8 && fread(&x, sizeof(x), 1, f) != 1) return false;
+	if ((h.version == 8 || h.version == 9) && fread(&x, sizeof(x), 1, f) != 1) return false;
+	if (h.version < 9) x.reserved[0] = 0;
 	if (h.version < 2) h.reserved[0] = h.reserved[1] = 0;
 	if (h.version < 3) h.reserved[2] = h.reserved[3] = 0;
 	if (h.version < 4) h.reserved[4] = 0;
@@ -46,7 +50,8 @@ static bool state_header_read(FILE* f, NbStateHeader& h, NbStateExt& x) {
 	return h.version == 1 || h.version == 2 || (h.version == 3 && h.reserved[2] == 1) || (h.version == 4 && h.reserved[2] <= 1 && h.reserved[4] >= 1) ||
 		   (h.version == 5 && h.reserved[2] <= 1 && h.reserved[5] == 1) || (h.version == 6 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1) ||
 		   (h.version == 7 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1 && h.reserved[7] >= 1) ||
-		   (h.version == 8 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && (h.reserved[7] == 0 || h.reserved[6] >= 1) && x.ccd_bodies >= 1);
+		   (h.version == 8 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && (h.reserved[7] == 0 || h.reserved[6] >= 1) && x.ccd_bodies >= 1) ||
+		   (h.version == 9 && h.reserved[2] <= 1 && h.reserved[5] <= 1 && h.reserved[6] >= 1 && x.reserved[0] >= 1);
 }
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
@@ -84,7 +89,7 @@ static NbStateHeader state_header_of(const nb_context* ctx, u32 cache) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = !ctx->ccd.empty() ? 8 : ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = ctx->sset.n ? 9 : !ctx->ccd.empty() ? 8 : ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
@@ -181,12 +186,19 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	std::vector<nb_joint_drive> drives;
 	if ((r = get_drives(ctx, drives, st))) { fclose(f); return r; }
 	hc.drives.assign(reinterpret_cast<const unsigned char*>(drives.data()), reinterpret_cast<const unsigned char*>(drives.data() + drives.size()));
+	std::vector<nb_joint_spring> springs;
+	if ((r = get_springs(ctx, springs, st))) { fclose(f); return r; }
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
-	const NbStateExt x = { (u32)ctx->ccd.size(), { 0, 0, 0 } };
-	if (h.version == 8) ok = ok && fwrite(&x, sizeof(x), 1, f) == 1;
+	const NbStateExt x = { (u32)ctx->ccd.size(), { (u32)springs.size(), 0, 0 } };
+	if (h.version >= 8) ok = ok && fwrite(&x, sizeof(x), 1, f) == 1;
 	for (const StateSection& s : state_sections(ctx, h, hc, false)) if (s.present) ok = ok && state_put(f, s, tmp, st);
-	if (h.version == 8) ok = ok && fwrite(ctx->ccd.data(), sizeof(nb_ccd_body), ctx->ccd.size(), f) == ctx->ccd.size();   // 16 bytes each: no padding
+	if (h.version >= 8) ok = ok && fwrite(ctx->ccd.data(), sizeof(nb_ccd_body), ctx->ccd.size(), f) == ctx->ccd.size();   // 16 bytes each: no padding
+	if (h.version == 9) {   // 56 bytes each, the section padded to 16
+		std::vector<unsigned char> b(reinterpret_cast<const unsigned char*>(springs.data()), reinterpret_cast<const unsigned char*>(springs.data() + springs.size()));
+		b.resize((b.size() + 15) & ~(size_t)15, 0);
+		ok = ok && fwrite(b.data(), 1, b.size(), f) == b.size();
+	}
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -254,6 +266,13 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	ok = ok && (ccd.empty() || fread(ccd.data(), sizeof(nb_ccd_body), ccd.size(), f) == ccd.size());
 	for (size_t i = 0; ok && i < ccd.size(); ++i)
 		ok = ccd[i].body != 0 && ccd[i].body < h.bodies && (i == 0 || ccd[i].body > ccd[i - 1].body) && !ccd_body_problem(ccd[i]);
+	// the springs against the file's joints, through the upload's checks
+	std::vector<nb_joint_spring> springs(x.reserved[0]);
+	const size_t spring_bytes = sizeof(nb_joint_spring) * springs.size();
+	std::vector<unsigned char> sb((spring_bytes + 15) & ~(size_t)15);
+	ok = ok && (sb.empty() || fread(sb.data(), 1, sb.size(), f) == sb.size());
+	if (ok && spring_bytes) memcpy(springs.data(), sb.data(), spring_bytes);
+	ok = ok && check_springs(ctx, springs.data(), x.reserved[0], h.reserved[6], structure.data(), unit_rel.data(), unit_ax.data()) == NB_OK;
 	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->scene_edited = false;   // the loaded scene replaces an edited one
@@ -265,9 +284,10 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	shape.kin.assign(idx, idx + kin.size());
 	const StateFileTables file = { hc.sensor.data(), kin.data(), frc };
 	{ int r = install_state(ctx, shape, &file, st); if (r) return r; }
-	drop_drives(ctx);   // a file without drives removes them, also where its joints have the context's structure
+	drop_drives(ctx); drop_springs(ctx);   // a file without drives or springs removes them, also where its joints have the context's structure
 	{ int r = set_joints(ctx, joints, h.reserved[6], st); if (r) return r; }
 	{ int r = set_drives(ctx, drives, h.reserved[7], st); if (r) return r; }
+	{ int r = set_springs(ctx, springs.data(), x.reserved[0], st); if (r) return r; }
 	{ int r = set_ccd(ctx, std::move(ccd), st); if (r) return r; }   // a file of an older version removes the set
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;
