@@ -31,6 +31,8 @@
  *   nb_shapecast                    <- no reference counterpart (the reference has no scene queries)
  *   nb_get_body_states /
  *   nb_set_body_states              <- no reference counterpart: the application's read and edit of BodyData between calls
+ *   nb_get_body_contact_impulses /
+ *   nb_get_contact_pair_impulses    <- no reference counterpart: the application's host sums over ContactData and ContactCache after a step
  *   nb_shard_*                      <- no reference counterpart (the reference is single threaded): SURVEY.md section 8e
  *
  * Data layout: the reference's caller-owned SoA structs (nudge.h:29-129) with every index-carrying field
@@ -976,6 +978,77 @@ enum nb_body_state_fields { NB_BODY_POSE = 1, NB_BODY_VELOCITY = 2 };
 int nb_get_body_states(nb_context*, const uint32_t* bodies /* null: bodies 0 .. n-1 */, uint32_t n, nb_body_state* out, int on_device, void* stream);
 int nb_set_body_states(nb_context*, const nb_body_state* states, uint32_t n, uint32_t fields, uint32_t* skipped /* may be null */, int on_device,
                        void* stream);
+
+/* Contact impulse reports (net contact force per body for observations and rewards, impact strength per touching pair for sounds and damage,
+ * the load on a pressure plate or a kinematic platform; DESIGN.md section 8.22): read on the device from the contact set of the last solved
+ * step.  Nothing is computed per step: a step that nobody reports on costs nothing more, and neither call changes nb_step or its graph.
+ * What both read: the contacts c of the last nb_collide or nb_upload_contacts (index order = nb_download_contacts' order), their (tag,
+ * feature) order of nb_read_cached_impulses, and J_c, the world-frame impulse of contact c as nb_update_cached_impulses wrote it:
+ * J_c = s0*n + s1*u + s2*v of k_update_impulses, the value the contact cache receives.  J_c is the step's total impulse (warm start plus
+ * every sweep's delta); divide by the time step for a force.  Side a of a contact received -J_c, side b +J_c (the solver's convention).  In
+ * throughput mode the impulses vary from run to run (see nb_set_solver_mode); the reports are a deterministic function of them.  After a
+ * step whose schedule overflowed (NB_ERR_OVERFLOW with bit 4 from nb_download_counts) the per-body report has no contact sides and the
+ * pair report reads impulses that were not solved.
+ * When legal: from the end of nb_update_cached_impulses (also inside nb_step, and after its graph is replayed) until one of nb_collide,
+ * nb_upload_contacts, nb_read_cached_impulses, nb_setup_contact_constraints, nb_apply_impulses (they rewrite the contacts, the impulses or the
+ * solver rows), nb_add_bodies, nb_remove_bodies, nb_upload_bodies, nb_upload_colliders, nb_snapshot_restore or nb_load_state (they renumber or
+ * replace bodies or state), each of which ends it also when it fails.  nb_write_cached_impulses, nb_advance, nb_apply_body_impulses,
+ * nb_set_body_states, the scene queries and the gathers leave the report valid and unchanged.  Otherwise, on a fresh context, and on a
+ * context nb_shard_create was called on, both calls are NB_ERR_ARGUMENT, changing nothing.  A device-pointer call decides this when it is
+ * called or captured: capture it after nb_step in the same graph.
+ * The arithmetic is float32, left to right as written, without fused multiply-adds, with cross and dot of the joints section above.
+ *
+ * nb_get_body_contact_impulses: row i holds b = bodies[i] (bodies null: b = i).  acc = tq = (+0, +0, +0), k = 0; for every contact c in
+ * ascending index order, side a before side b, for each side of c whose body is b:
+ *   r = position_c - p_b (per component), p_b the body's position as the step's solve used it (its position at the step's start: nothing
+ *       moves a body between nb_collide and nb_advance), exactly the lever arm nb_setup_contact_constraints stored in the contact's row;
+ *   side a: acc = acc - J_c, tq = tq - cross(r, J_c);  side b: acc = acc + J_c, tq = tq + cross(r, J_c);  k = k + 1.
+ * impulse = acc, angular_impulse = tq (about p_b), contacts = k, body = b.  Body 0 and kinematic bodies report what acts on them (the load on
+ * the ground or on a platform), though the solver never moves them.  A body whose island sleeps reports zeros and contacts = 0: a sleeping
+ * island has no contacts in the step because it is not solved.  Joint and user-row impulses are not included; they are read with
+ * nb_download_joints, nb_download_joint_drives, nb_download_joint_springs and nb_download_constraint_rows.  A null out with n > 0 is
+ * NB_ERR_ARGUMENT.  Launches: 3 (one key per contact side, one radix sort by (body, contact, side), one warp per row that finds its body's
+ * keys by binary search and sums them in that order); none with n = 0.
+ *   on_device == 0: host pointers; an index at or beyond the body count or a null bodies with n > B is NB_ERR_ARGUMENT, changing nothing;
+ *   the call synchronises `stream` and returns with `out` filled.
+ *   on_device != 0: bodies (may be null) and out are device pointers, out 16-byte aligned; asynchronous on `stream`.  An index at or beyond
+ *   the body count gives body = NB_REMOVED_BODY and every other field 0.
+ *
+ * nb_get_contact_pair_impulses: a pair is a run of contacts with equal tags in (tag, feature) order (with duplicate collider tags two
+ * collider pairs may share a key and then form one row, as in the cache and the events).  Over the run, in that order from +0:
+ * normal_impulse = the sum of dot(J_c, n_c), impulse = the sum of J_c, contacts = the run's length.  The deepest contact is the run's first,
+ * replaced only by a later one with a strictly greater penetration (a tie keeps the earlier contact, a NaN never wins); body_a, body_b and
+ * penetration are that contact's.  impulse, contacts, penetration and the bodies are those of an NB_CONTACT_BEGIN event for the same pair in
+ * the same step, bit for bit.  A row is kept iff normal_impulse >= min_normal_impulse, or min_normal_impulse is -INFINITY (which keeps every
+ * pair); kept rows come in ascending tags order.  *count = the number of kept rows, and the first min(capacity, *count) of them are written.
+ * A NaN threshold or a null count is NB_ERR_ARGUMENT, and so is a null out with capacity > 0.  capacity = 0 asks for the count.
+ * Launches: 5 (run-head flags, a scan that counts the runs, one thread per run head for its sums and its kept flag, a scan of the kept
+ * flags into *count, the scatter).
+ *   on_device == 0: host pointers; the call synchronises `stream`, and returns NB_ERR_CAPACITY after writing capacity rows when *count >
+ *   capacity.
+ *   on_device != 0: out (16-byte aligned) and count are device pointers; asynchronous on `stream`, NB_OK whatever the count.
+ * Scratch: allocated for the context's contact capacity on a call's first use, which synchronises: 48 bytes per contact of capacity for the
+ * per-body call (its sort keys and slots) and 56 for the pair call (its flags and per-run rows), plus for a host-pointer call 32 bytes per
+ * row (and 4 per index) or 48 per row of min(capacity, contact capacity).  After that neither device-pointer call allocates or
+ * synchronises, so both can be captured into the application's CUDA graph.  A captured per-body call holds the body count as of its
+ * capture: capture again after nb_add_bodies, nb_remove_bodies or nb_upload_bodies with another count. */
+typedef struct {
+	float impulse[3]; uint32_t body;               /* net contact impulse on the body this step; the index read */
+	float angular_impulse[3]; uint32_t contacts;   /* net contact angular impulse about the body's position; contact sides counted */
+} nb_body_contact_impulse;                         /* 32 bytes */
+typedef struct {
+	uint64_t tags;                 /* the pair word A | (uint64)B << 32, the cache and event key */
+	uint32_t body_a, body_b;       /* bodies of the pair's deepest contact (the event rule) */
+	uint32_t contacts;
+	float normal_impulse;          /* sum of dot(J_c, n_c) over the pair's contacts */
+	float impulse[3];              /* sum of J_c (the impulse on body_b; body_a received its negation) */
+	float penetration;             /* the deepest contact's penetration */
+	uint32_t reserved[2];          /* 0 */
+} nb_contact_pair_impulse;         /* 48 bytes */
+int nb_get_body_contact_impulses(nb_context*, const uint32_t* bodies /* null: bodies 0 .. n-1 */, uint32_t n, nb_body_contact_impulse* out,
+                                 int on_device, void* stream);
+int nb_get_contact_pair_impulses(nb_context*, float min_normal_impulse, nb_contact_pair_impulse* out, uint32_t capacity, uint32_t* count,
+                                 int on_device, void* stream);
 
 /* Solver mode.  NB_SOLVER_PARITY (default): the reference's exact Gauss-Seidel order (nudge.cpp:4206-4340 schedule, 4640-4855 sweeps),
  * bit-identical impulses.  NB_SOLVER_THROUGHPUT: mass-splitting Jacobi over the same constraint rows (nudge_b200/csrc/nb_jacobi.cuh) -

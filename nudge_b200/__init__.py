@@ -28,7 +28,7 @@ EXPORTS = ["nb_create", "nb_destroy", "nb_last_error", "nb_upload_bodies", "nb_u
            "nb_set_body_forces", "nb_clear_body_forces", "nb_download_body_forces",
            "nb_snapshot_create", "nb_snapshot_destroy", "nb_snapshot_save", "nb_snapshot_restore", "nb_upload_joints", "nb_download_joints", "nb_raycast", "nb_overlap",
            "nb_shapecast", "nb_upload_joint_drives", "nb_download_joint_drives", "nb_get_body_states", "nb_set_body_states",
-           "nb_upload_joint_springs", "nb_download_joint_springs"]
+           "nb_upload_joint_springs", "nb_download_joint_springs", "nb_get_body_contact_impulses", "nb_get_contact_pair_impulses"]
 
 
 class Config(C.Structure):
@@ -133,6 +133,8 @@ def load_library():
         lib.nb_download_ccd_bodies.argtypes = [V, V, C.c_uint32, V, V]
         lib.nb_get_body_states.argtypes = [V, V, C.c_uint32, V, C.c_int, V]
         lib.nb_set_body_states.argtypes = [V, V, C.c_uint32, C.c_uint32, V, C.c_int, V]
+        lib.nb_get_body_contact_impulses.argtypes = [V, V, C.c_uint32, V, C.c_int, V]
+        lib.nb_get_contact_pair_impulses.argtypes = [V, C.c_float, V, C.c_uint32, V, C.c_int, V]
         _lib = lib
     return _lib
 
@@ -570,6 +572,51 @@ class Sim(abi.HostState):
         skipped = C.c_uint32(0)
         self._ck(self.lib.nb_set_body_states(self.ctx, abi.ptr(r) if len(r) else None, len(r), int(fields), C.byref(skipped), 0, self.stream), "nb_set_body_states")
         return int(skipped.value)
+
+    # ---- contact impulse reports (nb_get_body_contact_impulses, nb_get_contact_pair_impulses, include/nudge_b200.h) ----
+    def get_body_contact_impulses(self, bodies=None, device_ptrs=None, n=None):
+        """The abi.BODY_CONTACT_IMPULSE rows of `bodies` (None: bodies 0 .. B-1): the net contact impulse and angular impulse (about the
+        body's position) each body received in the last solved step, and its contact sides.  Divide by the time step for a force.
+        device_ptrs=(bodies_ptr or None, out_ptr) with n: device buffers of n indices (None: bodies 0 .. n-1) and n rows instead; the call
+        is then asynchronous on the Sim's stream (capturable) and returns None, and an index at or beyond the body count gives a row with
+        body = REMOVED_BODY and zeros.  NudgeError when no solved step is there to report on."""
+        if device_ptrs is not None:
+            if n is None:
+                raise ValueError("Sim.get_body_contact_impulses with device_ptrs needs n, the number of rows the device buffers hold")
+            idx, out = device_ptrs
+            self._ck(self.lib.nb_get_body_contact_impulses(self.ctx, C.c_void_p(idx) if idx else None, int(n), C.c_void_p(out), 1, self.stream),
+                     "nb_get_body_contact_impulses")
+            return None
+        idx = None if bodies is None else np.ascontiguousarray(np.asarray(bodies, np.uint32).reshape(-1))
+        k = self.scene.n_bodies if idx is None else len(idx)
+        out = np.zeros(k, abi.BODY_CONTACT_IMPULSE)
+        self._ck(self.lib.nb_get_body_contact_impulses(self.ctx, abi.ptr(idx) if idx is not None and k else None, k, abi.ptr(out) if k else None, 0,
+                                                       self.stream), "nb_get_body_contact_impulses")
+        return out
+
+    def get_contact_pair_impulses(self, min_normal_impulse=-np.inf, device_ptrs=None, capacity=None):
+        """The abi.CONTACT_PAIR_IMPULSE rows of the last solved step's touching pairs whose normal impulse is at least min_normal_impulse
+        (-inf: every pair), by ascending tags.  capacity: room for that many rows; with too few, raises NudgeError; without one, the count
+        is asked for first.  device_ptrs=(out_ptr, count_ptr) with capacity: a device buffer of capacity rows and a device uint32 for the
+        count instead; the call is then asynchronous on the Sim's stream (capturable) and returns None."""
+        thr = float(min_normal_impulse)
+        if device_ptrs is not None:
+            if capacity is None:
+                raise ValueError("Sim.get_contact_pair_impulses with device_ptrs needs capacity, the number of rows the device buffer holds")
+            out, count = device_ptrs
+            self._ck(self.lib.nb_get_contact_pair_impulses(self.ctx, thr, C.c_void_p(out), int(capacity), C.c_void_p(count), 1, self.stream),
+                     "nb_get_contact_pair_impulses")
+            return None
+        count = C.c_uint32(0)
+        if capacity is None:
+            r = self.lib.nb_get_contact_pair_impulses(self.ctx, thr, None, 0, C.byref(count), 0, self.stream)
+            if r != -2:   # NB_ERR_CAPACITY: count holds the number of rows
+                self._ck(r, "nb_get_contact_pair_impulses")
+            capacity = count.value
+        out = np.zeros(max(int(capacity), 1), abi.CONTACT_PAIR_IMPULSE)
+        self._ck(self.lib.nb_get_contact_pair_impulses(self.ctx, thr, abi.ptr(out) if capacity else None, int(capacity), C.byref(count), 0, self.stream),
+                 "nb_get_contact_pair_impulses")
+        return out[:count.value].copy()
 
     # ---- overlap queries (nb_overlap, include/nudge_b200.h): which colliders touch each sphere or oriented box ----
     def overlap(self, queries, flags=0, capacity=None, device_ptrs=None, n=None):

@@ -86,6 +86,13 @@ assert BODY_STATE.itemsize == 64
 BODY_POSE = 1
 BODY_VELOCITY = 2
 
+# nb_body_contact_impulse (32 bytes): one row of nb_get_body_contact_impulses; nb_contact_pair_impulse (48 bytes): one row of
+# nb_get_contact_pair_impulses
+BODY_CONTACT_IMPULSE = np.dtype([("impulse", "<f4", 3), ("body", "<u4"), ("angular_impulse", "<f4", 3), ("contacts", "<u4")])
+CONTACT_PAIR_IMPULSE = np.dtype([("tags", "<u8"), ("body_a", "<u4"), ("body_b", "<u4"), ("contacts", "<u4"), ("normal_impulse", "<f4"),
+                                 ("impulse", "<f4", 3), ("penetration", "<f4"), ("reserved", "<u4", 2)])
+assert BODY_CONTACT_IMPULSE.itemsize == 32 and CONTACT_PAIR_IMPULSE.itemsize == 48
+
 
 def ptr(a):
     return a.ctypes.data_as(C.c_void_p)

@@ -168,6 +168,13 @@ struct nb_context {
 	// body states (nb_get_body_states, nb_set_body_states, DESIGN.md section 8.19, nb_body_state_api.cuh): a host-pointer call's staging (rows in
 	// and out, the gather's indices), and the set's sort keys (bs_sb points into bs_keys) with its own histogram, grid barrier and key count
 	DevBuf<nb_body_state> bs_rows; DevBuf<u32> bs_idx; DevBuf<u64> bs_keys[2]; SortBuffers bs_sb; u32* bs_n;
+	// contact impulse reports (nb_get_body_contact_impulses, nb_get_contact_pair_impulses, DESIGN.md section 8.22, nb_contact_report_api.cuh):
+	// report_ok = the contact set, its order, its impulses and its rows are those of a solved step (set by nb_update_cached_impulses and
+	// nb_step, cleared by the calls that rewrite them or renumber bodies).  The per-body call's key count, sort buffers (2 keys per contact
+	// of capacity, cr_sb's own histogram and grid barrier) and host-pointer staging; the pair call's run and kept counts, flags, per-run
+	// rows, scan sums and host-pointer staging.
+	bool report_ok; u32* cr_n; SortBuffers cr_sb; DevBuf<nb_body_contact_impulse> cr_rows; DevBuf<u32> cr_idx;
+	u32* cp_n; u32* cp_heads; u32* cp_kept; nb_contact_pair_impulse* cp_rows; u32* cp_block_sums; DevBuf<nb_contact_pair_impulse> cp_out;
 	// scene queries: ray casts (nb_raycast, DESIGN.md section 8.14), overlap queries (nb_overlap, section 8.15) and shape casts
 	// (nb_shapecast, section 8.16)
 	QueryScratch query;
@@ -646,6 +653,7 @@ int nb_lut_model_exact(const nb_context* ctx) { return ctx->lut_exact; }
 
 int nb_upload_bodies(nb_context* ctx, const nb_body_data* h, void* stream) {
 	NB_RANGE("nb_upload_bodies");
+	ctx->report_ok = false;
 	if (h->count > ctx->cfg.max_bodies) { ctx->error = "too many bodies"; return NB_ERR_CAPACITY; }
 	if (h->count != ctx->B) { drop_kinematic(ctx); drop_body_forces(ctx); drop_joints(ctx); drop_ccd(ctx); }   // the kinematic set, the force table, the joints and the CCD set belong to a body count
 	ctx->B = h->count;
@@ -671,6 +679,7 @@ int nb_download_momentum(nb_context* ctx, nb_body_momentum* h, uint32_t count, v
 int nb_download_transforms(nb_context* ctx, nb_transform* h, uint32_t count, void* stream) { ROWS_OK(count); D2H(h, ctx->xf, count, nb_transform); return NB_OK; }
 
 int nb_upload_colliders(nb_context* ctx, const nb_collider_data* h, void* stream) {
+	ctx->report_ok = false;
 	if (h->boxes.count > ctx->cfg.max_boxes || h->spheres.count > ctx->cfg.max_spheres) { ctx->error = "too many colliders"; return NB_ERR_CAPACITY; }
 	if (ctx->has_filter && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_filter = false; ++ctx->graph_epoch; }  // the table belongs to a collider count
 	if (ctx->has_sensor && h->boxes.count + h->spheres.count != ctx->nboxes + ctx->nspheres) { ctx->has_sensor = false; ++ctx->graph_epoch; }  // so does the sensor table
@@ -805,6 +814,7 @@ int nb_download_contacts(nb_context* ctx, nb_contact_data* h, nb_active_bodies* 
 // Host -> HBM for the outputs of collide (the reference lets user code add or edit contacts between the calls, example/main.cpp:288).
 int nb_upload_contacts(nb_context* ctx, const nb_contact_data* h, const nb_active_bodies* ha, void* stream) {
 	ctx->scene_edited = false;
+	ctx->report_ok = false;
 	if (h) {
 		if (h->count > ctx->cfg.max_contacts || h->sleeping_count > ctx->cfg.max_contacts) { ctx->error = "too many contacts"; return NB_ERR_CAPACITY; }
 		ctx->contacts_internal = false;
@@ -843,6 +853,7 @@ int nb_download_cache(nb_context* ctx, nb_contact_cache* h, void* stream) {
 int nb_collide(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_collide");
 	ctx->scene_edited = false;
+	ctx->report_ok = false;
 	ctx->in_step = true;   // until the nb_advance that ends the step
 	ctx->step_dt = 0.0f;
 	Launch L = mk_launch(ctx, stream);
@@ -961,6 +972,7 @@ static int read_sort(nb_context* ctx, void* stream) {
 
 int nb_read_cached_impulses(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_read_cached_impulses");
+	ctx->report_ok = false;
 	NOT_AFTER_EDIT();
 	int r = read_sort(ctx, stream); if (r) return r;
 	return read_lookup(ctx, stream);
@@ -1109,6 +1121,7 @@ static int build_contact_rows(nb_context* ctx, cudaStream_t st) {
 
 int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 	NB_RANGE("nb_setup_contact_constraints");
+	ctx->report_ok = false;
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	if (ctx->jset.n && !(ctx->step_dt > 0.0f)) { ctx->error = "joints need the step's time step: call nb_apply_gravity_damping after nb_collide"; return NB_ERR_ARGUMENT; }
@@ -1124,6 +1137,7 @@ int nb_setup_contact_constraints(nb_context* ctx, void* stream) {
 
 int nb_apply_impulses(nb_context* ctx, uint32_t sweeps, void* stream) {
 	NB_RANGE("nb_apply_impulses");
+	ctx->report_ok = false;
 	NOT_AFTER_EDIT();
 	JOIN_UPLOADS();
 	if (!sweeps) return NB_OK;
@@ -1146,6 +1160,7 @@ int nb_update_cached_impulses(nb_context* ctx, void* stream) {
 	NOT_AFTER_EDIT();
 	launch_grid(mk_launch(ctx, stream), k_update_impulses, GRID(ctx->cstride), ctx->rows, ctx->impulses, ctx->counts);
 	CK(cudaGetLastError());
+	ctx->report_ok = true;   // the contact impulse reports read this step's contacts, impulses and rows
 	return NB_OK;
 }
 
@@ -1191,7 +1206,7 @@ int nb_step(nb_context* ctx, float time_step, uint32_t iterations, float gravity
 	ctx->scene_edited = false;     // the step begins with nb_collide (also when its graph is replayed)
 	const int r = run_graphed(ctx, ctx->graph, (cudaStream_t)stream, time_step, iterations, gravity, damping, 0, 0,
 							  [&] { return step_body(ctx, time_step, gravity, damping, stream, [&] { return step_solve(ctx, iterations, stream); }); });
-	if (r == NB_OK) ctx->in_step = false;   // the step ended with nb_advance (also when its graph was replayed)
+	if (r == NB_OK) { ctx->in_step = false; ctx->report_ok = true; }   // the step ended with nb_advance (also when its graph was replayed)
 	return r;
 }
 
@@ -1364,3 +1379,4 @@ int nb_debug_rcp(nb_context* ctx, const float* x, float* y, uint32_t n, int rsq)
 #include "nb_query_api.cuh"
 #include "nb_ccd_api.cuh"     // after nb_query_api.cuh, whose walk and sphere cast k_ccd runs
 #include "nb_body_state_api.cuh"   // after nb_spawn_api.cuh, whose wake a pose set runs
+#include "nb_contact_report_api.cuh"

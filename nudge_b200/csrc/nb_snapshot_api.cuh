@@ -188,6 +188,7 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 
 int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	NB_RANGE("nb_snapshot_restore");
+	ctx->report_ok = false;
 	SNAPSHOT_OF_CTX(s, "nb_snapshot_restore");
 	if (!s->saved) { ctx->error = "nb_snapshot_restore: the snapshot was never saved"; return NB_ERR_ARGUMENT; }
 	cudaStream_t st = (cudaStream_t)stream;

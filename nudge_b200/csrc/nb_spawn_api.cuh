@@ -179,6 +179,7 @@ extern "C" {
 
 int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_remove_bodies");
+	ctx->report_ok = false;
 	if (ctx->sharded) { ctx->error = "nb_remove_bodies: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
 	if (!n) return NB_OK;
 	if (!h) { ctx->error = "null body list"; return NB_ERR_ARGUMENT; }
@@ -323,6 +324,7 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 
 int nb_add_bodies(nb_context* ctx, const nb_body_data* bodies, const nb_collider_data* colliders, const nb_spawn_tables* tables, void* stream) {
 	NB_RANGE("nb_add_bodies");
+	ctx->report_ok = false;
 	if (ctx->sharded) { ctx->error = "nb_add_bodies: not supported on a context of nb_shard_create"; return NB_ERR_ARGUMENT; }
 	const u32 n = bodies ? bodies->count : 0, nb = colliders ? colliders->boxes.count : 0, ns = colliders ? colliders->spheres.count : 0;
 	if (n && (!bodies->transforms || !bodies->properties || !bodies->momentum || !bodies->idle_counters)) { ctx->error = "null body array"; return NB_ERR_ARGUMENT; }

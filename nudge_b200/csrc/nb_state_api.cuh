@@ -218,6 +218,7 @@ int nb_state_info(const char* path, uint32_t counts[5]) {
 }
 
 int nb_load_state(nb_context* ctx, const char* path, void* stream) {
+	ctx->report_ok = false;
 	cudaStream_t st = (cudaStream_t)stream;
 	{ int jr = join_uploads(ctx, st); if (jr) return jr; }
 	FILE* f = fopen(path, "rb");

@@ -21,6 +21,11 @@ torch.cuda.synchronize()
 g.get_body_states(device_ptrs=(t_idx.data_ptr(), t_out.data_ptr()), n=4)
 g.set_body_states(None, 3, device_ptrs=(t_out.data_ptr(), t_skip.data_ptr()), n=4)
 g.step_staged()
+g.get_body_contact_impulses(); g.get_body_contact_impulses([0, 3, 3]); g.get_contact_pair_impulses(0.0)   # contact impulse reports
+t_cb = torch.zeros(8 * s.n_bodies, dtype=torch.int32, device="cuda"); t_cp = torch.zeros(12 * 64, dtype=torch.int32, device="cuda")
+torch.cuda.synchronize()
+g.get_body_contact_impulses(device_ptrs=(t_idx.data_ptr(), t_cb.data_ptr()), n=4)
+g.get_contact_pair_impulses(device_ptrs=(t_cp.data_ptr(), t_skip.data_ptr()), capacity=64)
 ev, dropped = g.contact_events()
 c = g.counts(); print("contacts", c.contacts, "overflow", c.overflow, "events", len(ev), "dropped", dropped)
 PY
