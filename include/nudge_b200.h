@@ -267,9 +267,10 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  * axis_a, and CONE and TWIST limit a BALL joint's swing away from axis_a and its twist about it.  A drive set is a sparse table
  * keyed by joint: at most one drive per joint, naming it by its index in the current joint set's upload order.
  * Rows: a drive appends rows to its joint, solved right after the joint's own rows in this order: motor (MOTOR) or cone (CONE), lower limit
- * and upper limit (LIMIT or TWIST); so a drive has (MOTOR|CONE ? 1 : 0) + (LIMIT|TWIST ? 2 : 0) appended rows.  Every appended row has the joint's a, b and softness, reserved = 0, and keeps its accumulated impulse from step to step.  In
- * nb_debug_read("joint_rows") the joints' own rows come first, exactly as without drives, then the appended rows, per driven joint in the
- * joint table's order (by joint level, upload order within one).  Same arithmetic rules as above (float32, left to right, no fused
+ * and upper limit (LIMIT or TWIST); so a drive has (MOTOR|CONE ? 1 : 0) + (LIMIT|TWIST ? 2 : 0) appended rows.  Every appended row has the joint's a, b and softness, reserved = 0, and keeps its accumulated impulse from step to step.  The
+ * appended rows sit in a row buffer of their own: nb_debug_read("joint_rows") returns the joints' own rows, exactly as without drives, and
+ * nb_debug_read("joint_drive_rows") the appended rows, per driven joint in the joint table's order (by joint level, upload order within
+ * one).  Same arithmetic rules as above (float32, left to right, no fused
  * multiply-adds), with k = beta / dt and bias(C) = C > 0 ? C / dt : k * C (speculative: a limit row lets the coordinate reach its bound
  * within the step, and pulls it back at the joint's Baumgarte rate once past it):
  *   HINGE coordinate:  g = qmul(q_a, rel_rotation);  d = b != 0 ? qmul(g, (-q_b.xyz, q_b.w)) : g;  if d.w < 0: d = -d (all four);
@@ -324,7 +325,7 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  * max_motor_torque; a negative max_motor_torque, break_force or break_torque; a field that is not finite other than thresholds of +inf (cone
  * is read only with CONE); broken > 1; a HINGE LIMIT, CONE or TWIST whose joint's rel_rotation has |x*x + y*y + z*z + w*w - 1| > 1e-3 (in
  * double); a SLIDE, CONE or TWIST whose joint's axis_a has |x*x + y*y + z*z - 1| > 1e-3 (in double).  Asynchronous on `stream`, staged like nb_upload_joints (the host array
- * may be reused on return); it synchronises only when the joints' row buffer must grow.  nb_step re-records its graph only when the drive
+ * may be reused on return); it synchronises only when the drive table or its row buffer must grow.  nb_step re-records its graph only when the drive
  * structure (which joints, which flags) changed or a buffer moved: new speeds, torques, limits, thresholds, impulses or broken flags for the
  * same structure keep it, so a throttle may be uploaded every frame.
  * nb_download_joint_drives returns the drives in joint-index order with impulse[] = the appended rows' current accumulated impulses (0 where
@@ -336,12 +337,12 @@ int nb_download_joints(nb_context*, nb_joint* host, uint32_t capacity, uint32_t*
  * removes it with the joints.  Snapshots carry it; nb_save_state writes it (state version 7) and nb_load_state installs it through the
  * upload's checks; a file of an older version removes it.  SLIDE, CONE and TWIST and the cone travel in the same rows (no new state version);
  * a build without them refuses such a file's drives as an unknown flag.  nb_debug_read("joint_drives") returns the device table: one 64-byte
- * entry per joint in table order, { flags, first appended row, lower, upper, sl, cl, su, cu, motor_speed, max_motor_torque, break_force,
+ * entry per joint in table order, { flags, first appended row (an index into "joint_drive_rows"), lower, upper, sl, cl, su, cu, motor_speed, max_motor_torque, break_force,
  * break_torque, position[2] (sh, ch; dist, 0; s, 0; sh', ch' or ss, cs), broken, cone }, flags 0 and the rest 0 for a joint without a drive.
  * A SLIDE drive holds lower and upper raw, with sl .. cu 0; a TWIST drive holds their half-angle pairs as a hinge does; a CONE drive holds
  * (sc, cc) in motor_speed and max_motor_torque and its cone as uploaded in the last word (0 without CONE).
- * Cost: no launch; k_joint_rows and k_joint_solve take the drive table as one more argument (null without a set), and without a set the
- * joints' rows, the launches and the graph are what they are without this feature. */
+ * Cost: no launch; k_joint_rows and k_joint_solve take the drive table and its rows as two more arguments (null without a set), and
+ * without a set the joints' rows, the launches and the graph are what they are without this feature. */
 /* Bit 8 is unassigned (refused as an unknown flag). */
 enum nb_joint_drive_flags { NB_JOINT_LIMIT = 1, NB_JOINT_MOTOR = 2, NB_JOINT_BREAKABLE = 4, NB_JOINT_SLIDE = 16, NB_JOINT_CONE = 32, NB_JOINT_TWIST = 64 };
 typedef struct {
@@ -371,8 +372,8 @@ int nb_download_joint_drives(nb_context*, nb_joint_drive* host, uint32_t capacit
  * joint, naming it by its index in the current joint set's upload order; a joint may have a drive and a spring.
  * Rows: HINGE, FIXED and DISTANCE springs have one spring row, BALL springs three.  k_joint_solve applies, per joint, its own rows, then its
  * spring rows, then its drive rows (so limits act last and hold against a spring); the warm start follows the same order.  The spring rows sit
- * in a row buffer of their own: nb_debug_read("joint_rows") is what it is without springs, and nb_debug_read("joint_spring_rows") returns
- * the spring rows, per sprung joint in the joint table's order.  Same arithmetic rules as the joints' section (float32, left to right, no
+ * in a row buffer of their own, like the drive rows: nb_debug_read("joint_rows") and ("joint_drive_rows") are what they are without
+ * springs, and nb_debug_read("joint_spring_rows") returns the spring rows, per sprung joint in the joint table's order.  Same arithmetic rules as the joints' section (float32, left to right, no
  * fused multiply-adds), dt the step's time step:
  *   Spring row:  on a coordinate C with Jacobian J, of the joint's a and b:  den = damping + dt * stiffness;  softness = 1.0f / (dt * den);
  *              bias = (stiffness * C - damping * target_velocity) / den;  lo = -(max_force * dt), hi = max_force * dt;  reserved = 0.  The row
@@ -417,8 +418,8 @@ int nb_download_joint_drives(nb_context*, nb_joint_drive* host, uint32_t capacit
  * file of an older version removes it.  nb_debug_read("joint_springs") returns the device table: one 64-byte entry per joint in table order,
  * { present, first spring row, target[4] (a HINGE: st, ct, 0, 0), target_velocity, stiffness, damping, max_force, position[2] (sh, ch; s, 0;
  * dist, 0; |d.xyz|, d.w), target angle (HINGE; else 0), reserved[3] = 0 }, all 0 for a joint without a spring.
- * Cost: no launch in the step; k_joint_rows and k_joint_solve take the spring table and rows as two more arguments (null without a set), and without a
- * set the joints' rows, the launches and the graph are what they are without this feature. */
+ * Cost: no launch in the step; k_joint_rows and k_joint_solve take the spring table and its rows as two more arguments (null without a
+ * set), and without a set the joints' and drives' rows, the launches and the graph are what they are without this feature. */
 typedef struct {
 	uint32_t joint;             /* index of the joint in the current set's upload order */
 	uint32_t reserved;          /* must be 0 */

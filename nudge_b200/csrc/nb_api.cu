@@ -37,14 +37,16 @@ template<class T> struct DevBuf {
 // (by level, upload order within one), and the levels' offsets (levels + 1, none without entries), host values in nb_step's graph.
 struct RowLevels { u32 n = 0, levels = 0; std::vector<u32> level_off, order; std::vector<nb_body_pair> ab; };
 
-// The host side of a joint set (nb_joint_api.cuh): its levels (the device table holds the joints by level), per joint in upload order its
-// (type, a, b), and the number of rows the joints generate.
-// unit_rel / unit_axis: rel_rotation / axis_a of unit length, as a drive that reads them needs.
-struct JointSet : RowLevels { u32 nrows = 0; std::vector<u32> structure; std::vector<uint8_t> unit_rel, unit_axis; };
+// The shape of a joint set (joint_shape, nb_joint_api.cuh), what the drive and spring checks read: per joint in upload order its (type, a,
+// b), and whether its rel_rotation / axis_a has unit length, as a drive or spring that reads them needs.
+struct JointShape { std::vector<u32> structure; std::vector<uint8_t> unit_rel, unit_axis; };
+// The host side of a joint set (nb_joint_api.cuh): its levels (the device table holds the joints by level), its shape, and the number of
+// rows the joints generate.
+struct JointSet : RowLevels, JointShape { u32 nrows = 0; };
 
 // One joint's drive on the device (nb_joint_api.cuh; DESIGN.md section 8.17): one entry per joint in table order while a drive set exists,
-// flags = 0 for a joint without a drive.  row = the first of its appended rows; (sl, cl) / (su, cu) = the hinge or twist limits' half-angle
-// pairs; a CONE drive (section 8.20) keeps its half-angle pair (sc, cc) in motor_speed / max_motor_torque and the uploaded half-angle in
+// flags = 0 for a joint without a drive.  row = the first of its rows in the drive rows; (sl, cl) / (su, cu) = the hinge or twist limits'
+// half-angle pairs; a CONE drive (section 8.20) keeps its half-angle pair (sc, cc) in motor_speed / max_motor_torque and the uploaded half-angle in
 // cone (0 otherwise).  position = (sh, ch) of a hinge, (dist, 0) or (s, 0) of a slider, the twist's pair or the swing's (ss, cs), as of the
 // last row build.  nb_debug_read("joint_drives") returns the table as it stands.
 struct JointDrive {
@@ -52,10 +54,11 @@ struct JointDrive {
 	float motor_speed, max_motor_torque, break_force, break_torque, position[2]; u32 broken; float cone;
 };
 // The host side of a sparse table keyed by joint (the drives, the springs): the entry count, the entries' rows and per entry in joint order
-// the structure nb_step's graph depends on: (joint, flags) of a drive, the joint of a spring.  A drive's rows follow the joints' own in the
-// joints' row buffer, a spring's sit in a row buffer of their own.
+// the structure nb_step's graph depends on: (joint, flags) of a drive, the joint of a spring.
 struct KeyedSet { u32 n = 0, nrows = 0; std::vector<u32> structure; };
-using DriveSet = KeyedSet;
+// A sparse table keyed by joint: the device table (one entry per joint in table order while set.n), its rows (each entry's row is an
+// offset into them) and the host side.
+template<class E> struct KeyedTable { DevBuf<E> table; DevBuf<nb_constraint_row> rows; KeyedSet set; };
 // One joint's spring on the device (nb_upload_joint_springs, nb_joint_api.cuh; DESIGN.md section 8.21): one entry per joint in table order
 // while a spring set exists, present = 0 for a joint without a spring.  row = its first spring row; target = the uploaded words, for a HINGE
 // (st, ct) = (sin, cos) of target / 2 with the uploaded angle in `angle`; position = (sh, ch) of a hinge, (s, 0), (dist, 0), or (|d.xyz|,
@@ -157,10 +160,8 @@ struct nb_context {
 	// joints (nb_upload_joints, DESIGN.md section 8.13): the table by level, the rows k_joint_rows rebuilds every step around their accumulated
 	// impulses, and the host side; step_dt = the time step of the nb_apply_gravity_damping since the last nb_collide (0: none yet)
 	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows; JointSet jset; float step_dt;
-	// joint drives (nb_upload_joint_drives, DESIGN.md section 8.17): the device table while dset.n, the rows appended after the joints' own in jrows
-	DevBuf<JointDrive> drives; DriveSet dset;
-	// joint springs (nb_upload_joint_springs, DESIGN.md section 8.21): the device table while sset.n, and the spring rows in a buffer of their own
-	DevBuf<JointSpring> springs; DevBuf<nb_constraint_row> srows; KeyedSet sset;
+	// joint drives (nb_upload_joint_drives, DESIGN.md section 8.17) and joint springs (nb_upload_joint_springs, section 8.21)
+	KeyedTable<JointDrive> drives; KeyedTable<JointSpring> springs;
 	// continuous collision (nb_upload_ccd_bodies, DESIGN.md section 8.18, nb_ccd_api.cuh): ccd = the set (host copy, ascending by body) and
 	// ccd_rows its device copy; ccd_t = the advance's translation factor per body (max_bodies of them, 1 outside the set), allocated on the
 	// first upload; ccd_hits = (bits of t, collider) per entry of the last advance
@@ -1273,10 +1274,11 @@ int nb_debug_read(nb_context* ctx, const char* name, void* dst, size_t max_bytes
 		{ "row_planes_all", ctx->rows.plane, sizeof(float) * (size_t)ROW_PLANES_TOTAL * ctx->cstride },
 		{ "body_contacts", ctx->jcnt, sizeof(u32) * ctx->B },
 		{ "kind", ctx->kind, ctx->has_kin ? (size_t)ctx->B : 0 },
-		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * ((size_t)ctx->jset.nrows + ctx->dset.nrows) },   // in table order: by joint level, upload order within one; then the drives' rows
-		{ "joint_drives", ctx->drives.p, ctx->dset.n ? sizeof(JointDrive) * (size_t)ctx->jset.n : 0 },
-		{ "joint_springs", ctx->springs.p, ctx->sset.n ? sizeof(JointSpring) * (size_t)ctx->jset.n : 0 },
-		{ "joint_spring_rows", ctx->srows.p, sizeof(nb_constraint_row) * (size_t)ctx->sset.nrows },   // per sprung joint in table order
+		{ "joint_rows", ctx->jrows.p, sizeof(nb_constraint_row) * (size_t)ctx->jset.nrows },   // in table order: by joint level, upload order within one
+		{ "joint_drives", ctx->drives.table.p, ctx->drives.set.n ? sizeof(JointDrive) * (size_t)ctx->jset.n : 0 },
+		{ "joint_drive_rows", ctx->drives.rows.p, sizeof(nb_constraint_row) * (size_t)ctx->drives.set.nrows },   // per driven joint in table order
+		{ "joint_springs", ctx->springs.table.p, ctx->springs.set.n ? sizeof(JointSpring) * (size_t)ctx->jset.n : 0 },
+		{ "joint_spring_rows", ctx->springs.rows.p, sizeof(nb_constraint_row) * (size_t)ctx->springs.set.nrows },   // per sprung joint in table order
 		{ "sensor_pairs", ctx->sensor_keys.p, sizeof(u64) * (ctx->has_sensor ? std::min(c[CNT_SENSOR_PAIRS], ctx->sensor_cap) : 0) },
 		{ "ccd_hits", ctx->ccd_hits.p, sizeof(uint2) * ctx->ccd.size() },   // per entry of the last advance, in set order: (bits of t, collider)
 	};

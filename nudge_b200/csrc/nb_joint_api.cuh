@@ -5,15 +5,13 @@
 // and one launch per joint level (level_rows over the joints' bodies).  The device table holds the joints by level, upload order within one;
 // each entry's type word also carries the offset of the joint's first row (type | offset << 2).  The parameters live in the table, the
 // accumulated impulses in the rows, which k_joint_rows rewrites around them.
-// Drives (nb_upload_joint_drives; DESIGN.md section 8.17) are one more table, JointDrive per joint in table order, that both kernels take as
-// an argument (null without a drive set).  A drive's rows (motor, lower, upper) sit after all joints' own rows, so that the joint table and
-// the own rows' offsets are the same with and without drives; k_joint_solve applies them after the joint's own rows.  The break test and the
-// broken flag live in k_joint_rows.  Sliders (FIXED + SLIDE) and ragdoll swing-cone and twist limits (BALL + CONE / TWIST; DESIGN.md section
-// 8.20) are drives too: a slider rewrites its joint's point rows, a cone takes the motor's slot and a twist limit the limit's.  Included at
-// the end of nb_api.cu.
-// Springs (nb_upload_joint_springs; DESIGN.md section 8.21) are a second sparse table keyed by joint, JointSpring per joint in table order,
-// that both kernels take with its rows (a buffer of their own; null without a spring set).  A spring row is Catto's soft step on one joint
-// coordinate; k_joint_solve applies a joint's spring rows after its own rows and before its drive rows.
+// Drives (nb_upload_joint_drives; DESIGN.md section 8.17) and springs (nb_upload_joint_springs; DESIGN.md section 8.21) are sparse tables
+// keyed by joint (KeyedTable): an entry per joint in table order and the entries' rows in a buffer of their own, which both kernels take as
+// arguments (null without a set), so that the joints' own rows are the same with and without them.  A drive's rows are motor, lower, upper;
+// the break test and the broken flag live in k_joint_rows.  Sliders (FIXED + SLIDE) and ragdoll swing-cone and twist limits (BALL + CONE /
+// TWIST; DESIGN.md section 8.20) are drives too: a slider rewrites its joint's point rows, a cone takes the motor's slot and a twist limit
+// the limit's.  A spring row is Catto's soft step on one joint coordinate; k_joint_solve applies a joint's own rows, then its spring rows,
+// then its drive rows.  Included at the end of nb_api.cu.
 #pragma once
 
 __host__ __device__ __forceinline__ u32 joint_row_count(u32 type) { return type == NB_JOINT_BALL ? 3u : type == NB_JOINT_HINGE ? 5u : type == NB_JOINT_FIXED ? 6u : 1u; }
@@ -130,24 +128,24 @@ NB_DEV void swing_twist_rows(nb_constraint_row* drow, const nb_joint& j, const J
 	else { position[0] = ss; position[1] = cs; }
 }
 
-// One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints), and with a drive table its drive's rows.
-// With a spring table the spring's rows at srows + row.
+// One thread per joint: the joint's rows from the two transforms (include/nudge_b200.h, Joints), with a drive table its drive's rows at
+// drows + row, and with a spring table its spring's rows at srows + row.
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints, u32 n, const nb_transform* xf, float dt, nb_constraint_row* rows, JointDrive* drives,
-		JointSpring* springs, nb_constraint_row* srows) {
+		nb_constraint_row* drows, JointSpring* springs, nb_constraint_row* srows) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const nb_joint j = joints[i];
 		const u32 type = j.type & 3u;
 		nb_constraint_row* row = rows + (j.type >> 2);
 		const float k = j.beta / dt;
 		u32 flags = 0;
-		nb_constraint_row* drow = rows;
+		nb_constraint_row* drow = drows;
 		JointDrive d;
 		const JointSpring* sp = springs ? springs + i : nullptr;   // read where used: the entry is 16 words
 		const bool sprung = sp && sp->present;
 		nb_constraint_row* srow = sprung ? srows + sp->row : srows;
 		if (drives) {
 			d = drives[i];
-			flags = d.flags; drow = rows + d.row;
+			flags = d.flags; drow = drows + d.row;
 			bool broken = d.broken != 0;
 			if (!broken && (flags & NB_JOINT_BREAKABLE) && joint_breaks(row, drow, type, flags, d, dt)) { broken = true; drives[i].broken = 1u; }
 			if (broken) {
@@ -237,32 +235,25 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_rows(const nb_joint* joints,
 	}
 }
 
+// Applies rows [first, first + count) one after the other to the bodies in `s`, keeping each row's new impulse unless `warm`.
+NB_DEV void joint_rows_apply(nb_constraint_row* rows, u32 first, u32 count, RowBodies& s, int warm) {
+	for (u32 r = first; r < first + count; ++r) {
+		const float next = row_apply(rows[r], s, warm);
+		if (!warm) rows[r].impulse = next;
+	}
+}
+
 // One thread per joint of the level [begin, end): the joint's rows one after the other, the two bodies' momentum kept in registers across them.
 // With a spring table the spring's rows follow the joint's own, and with a drive table the drive's rows come last.
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_solve(const nb_joint* joints, u32 begin, u32 end, nb_constraint_row* rows, nb_body_momentum* momentum,
-		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm, const JointDrive* drives, const JointSpring* springs,
-		nb_constraint_row* srows) {
+		const nb_body_properties* props, const float4* inertia, const uint8_t* kind, int warm, const JointDrive* drives, nb_constraint_row* drows,
+		const JointSpring* springs, nb_constraint_row* srows) {
 	for (u32 i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
-		const u32 packed = joints[i].type, first = packed >> 2, count = joint_row_count(packed & 3u);
+		const u32 packed = joints[i].type;
 		RowBodies s = row_bodies_load(joints[i].a, joints[i].b, momentum, props, inertia, kind);
-		for (u32 r = first; r < first + count; ++r) {
-			const float next = row_apply(rows[r], s, warm);
-			if (!warm) rows[r].impulse = next;
-		}
-		if (springs && springs[i].present) {
-			const u32 sfirst = springs[i].row, scount = spring_row_count(packed & 3u);
-			for (u32 r = sfirst; r < sfirst + scount; ++r) {
-				const float next = row_apply(srows[r], s, warm);
-				if (!warm) srows[r].impulse = next;
-			}
-		}
-		if (drives) {
-			const u32 dfirst = drives[i].row, dcount = drive_row_count(drives[i].flags);
-			for (u32 r = dfirst; r < dfirst + dcount; ++r) {
-				const float next = row_apply(rows[r], s, warm);
-				if (!warm) rows[r].impulse = next;
-			}
-		}
+		joint_rows_apply(rows, packed >> 2, joint_row_count(packed & 3u), s, warm);
+		if (springs && springs[i].present) joint_rows_apply(srows, springs[i].row, spring_row_count(packed & 3u), s, warm);
+		if (drives) joint_rows_apply(drows, drives[i].row, drive_row_count(drives[i].flags), s, warm);
 		row_bodies_store(s);
 	}
 }
@@ -271,21 +262,20 @@ __global__ void __launch_bounds__(NB_BLOCK) k_joint_solve(const nb_joint* joints
 static int launch_joints(nb_context* ctx, const float* dt, cudaStream_t st) {
 	const Launch L = mk_launch(ctx, st);
 	const JointSet& js = ctx->jset;
-	JointDrive* drives = ctx->dset.n ? ctx->drives.p : nullptr;
-	JointSpring* springs = ctx->sset.n ? ctx->springs.p : nullptr;
-	nb_constraint_row* srows = ctx->sset.n ? ctx->srows.p : nullptr;
-	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p, drives, springs, srows);
+	JointDrive* drives = ctx->drives.set.n ? ctx->drives.table.p : nullptr;
+	nb_constraint_row* drows = ctx->drives.set.n ? ctx->drives.rows.p : nullptr;
+	JointSpring* springs = ctx->springs.set.n ? ctx->springs.table.p : nullptr;
+	nb_constraint_row* srows = ctx->springs.set.n ? ctx->springs.rows.p : nullptr;
+	if (dt) launch_grid(L, k_joint_rows, GRID(js.n), ctx->joints.p, js.n, ctx->xf, *dt, ctx->jrows.p, drives, drows, springs, srows);
 	for (u32 l = 0; l < js.levels; ++l)
 		launch_grid(L, k_joint_solve, GRID(js.level_off[l + 1] - js.level_off[l]), ctx->joints.p, js.level_off[l], js.level_off[l + 1], ctx->jrows.p, ctx->mom, ctx->props,
-			ctx->inertia, kin_table(ctx), dt ? 1 : 0, (const JointDrive*)drives, (const JointSpring*)springs, srows);
+			ctx->inertia, kin_table(ctx), dt ? 1 : 0, (const JointDrive*)drives, drows, (const JointSpring*)springs, srows);
 	CK(cudaGetLastError());
 	return NB_OK;
 }
 
-static void drop_keyed(nb_context* ctx, KeyedSet& set) { if (set.n) { set = KeyedSet(); ++ctx->graph_epoch; } }
-static void drop_drives(nb_context* ctx) { drop_keyed(ctx, ctx->dset); }
-static void drop_springs(nb_context* ctx) { drop_keyed(ctx, ctx->sset); }
-static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ctx->dset = KeyedSet(); ctx->sset = KeyedSet(); ++ctx->graph_epoch; } }
+template<class E> static void drop_keyed(nb_context* ctx, KeyedTable<E>& t) { if (t.set.n) { t.set = KeyedSet(); ++ctx->graph_epoch; } }
+static void drop_joints(nb_context* ctx) { if (ctx->jset.n) { ctx->jset = JointSet(); ctx->drives.set = ctx->springs.set = KeyedSet(); ++ctx->graph_epoch; } }
 
 // Whether a quaternion has unit length within the tolerance a HINGE LIMIT drive asks of its joint's rel_rotation.
 static bool unit_quat(const float* q) {
@@ -314,16 +304,23 @@ static int check_joints(nb_context* ctx, const nb_joint* h, u32 n, u32 B) {
 		if (const char* p = joint_problem(h[i], B)) { ctx->error = "joint " + std::to_string(i) + ": " + p; return NB_ERR_ARGUMENT; }
 	return NB_OK;
 }
+// The shape of n joints in upload order.
+static JointShape joint_shape(const nb_joint* h, u32 n) {
+	JointShape s;
+	for (u32 i = 0; i < n; ++i) {
+		s.structure.insert(s.structure.end(), { h[i].type, h[i].a, h[i].b });
+		s.unit_rel.push_back(unit_quat(h[i].rel_rotation) ? 1 : 0); s.unit_axis.push_back(unit_axis(h[i].axis_a) ? 1 : 0);
+	}
+	return s;
+}
 
 // Installs n checked joints in place of the set: levels, the table by level with the row offsets, and the rows holding the impulses.
 static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st) {
 	if (!n) { drop_joints(ctx); return NB_OK; }
 	JointSet js;
+	static_cast<JointShape&>(js) = joint_shape(h, n);
 	std::vector<nb_body_pair> ab(n);
-	for (u32 i = 0; i < n; ++i) {
-		ab[i].a = h[i].a; ab[i].b = h[i].b; js.structure.insert(js.structure.end(), { h[i].type, h[i].a, h[i].b });
-		js.unit_rel.push_back(unit_quat(h[i].rel_rotation) ? 1 : 0); js.unit_axis.push_back(unit_axis(h[i].axis_a) ? 1 : 0);
-	}
+	for (u32 i = 0; i < n; ++i) { ab[i].a = h[i].a; ab[i].b = h[i].b; }
 	if (int r = level_rows(ctx, std::move(ab), js, "joints")) return r;
 	std::vector<nb_joint> table(n);
 	for (u32 i = 0; i < n; ++i) table[js.order[i]] = h[i];
@@ -335,9 +332,8 @@ static int set_joints(nb_context* ctx, const nb_joint* h, u32 n, cudaStream_t st
 	GROW(ctx->joints, n, st); GROW(ctx->jrows, js.nrows, st);
 	CK(put_staged(ctx, ctx->joints.p, table.data(), sizeof(nb_joint) * (size_t)n, st));
 	CK(put_staged(ctx, ctx->jrows.p, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
-	// the levels are host values in nb_step's graph, the buffers its kernel arguments; the drives and springs follow the structure (the
-	// drives' rows stay beyond the joints' own, which the copy above leaves alone)
-	if (js.structure != ctx->jset.structure) { drop_drives(ctx); drop_springs(ctx); }
+	// the levels are host values in nb_step's graph, the buffers its kernel arguments; the drives and springs follow the structure
+	if (js.structure != ctx->jset.structure) { drop_keyed(ctx, ctx->drives); drop_keyed(ctx, ctx->springs); }
 	if (js.structure != ctx->jset.structure || before[0] != ctx->joints.p || before[1] != ctx->jrows.p) ++ctx->graph_epoch;
 	ctx->jset = std::move(js);
 	return NB_OK;
@@ -363,12 +359,11 @@ static int get_joints(nb_context* ctx, std::vector<nb_joint>& out, cudaStream_t 
 	return NB_OK;
 }
 
-// What nb_upload_joint_drives refuses in a drive of a joint set given by its structure ((type, a, b) per joint), unit_rel and unit_axis; null
-// if valid.
-static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
-	if (d.joint >= nj) return "a joint index at or beyond the joint count";
+// What nb_upload_joint_drives refuses in a drive of a joint set of shape `js`; null if valid.
+static const char* drive_problem(const nb_joint_drive& d, const JointShape& js) {
+	if (d.joint >= js.structure.size() / 3) return "a joint index at or beyond the joint count";
 	if (d.flags & ~(u32)(NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE | NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST)) return "an unknown flag";
-	const u32 type = structure[3 * (size_t)d.joint];
+	const u32 type = js.structure[3 * (size_t)d.joint];
 	const u32 fixed = d.flags & NB_JOINT_SLIDE ? NB_JOINT_SLIDE | NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : NB_JOINT_SLIDE | NB_JOINT_BREAKABLE;
 	const u32 takes = type == NB_JOINT_HINGE ? NB_JOINT_LIMIT | NB_JOINT_MOTOR | NB_JOINT_BREAKABLE : type == NB_JOINT_DISTANCE ? NB_JOINT_LIMIT | NB_JOINT_BREAKABLE
 		: type == NB_JOINT_FIXED ? fixed : NB_JOINT_CONE | NB_JOINT_TWIST | NB_JOINT_BREAKABLE;
@@ -383,7 +378,7 @@ static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* str
 		if (d.lower > d.upper) return "lower > upper";
 		if (type == NB_JOINT_HINGE && (d.lower < -pi || d.upper > pi)) return "a hinge limit outside [-pi, pi]";
 		if (type == NB_JOINT_DISTANCE && d.lower < 0.0f) return "a negative distance limit";
-		if (type == NB_JOINT_HINGE && !unit_rel[d.joint]) return "a HINGE LIMIT whose joint's rel_rotation is not of unit length";
+		if (type == NB_JOINT_HINGE && !js.unit_rel[d.joint]) return "a HINGE LIMIT whose joint's rel_rotation is not of unit length";
 	}
 	if (d.flags & NB_JOINT_TWIST) {
 		if (d.lower > d.upper) return "lower > upper";
@@ -392,8 +387,8 @@ static const char* drive_problem(const nb_joint_drive& d, u32 nj, const u32* str
 	// a cone keeps its half-angle pair in the motor's slots of the device table
 	if ((d.flags & NB_JOINT_CONE) && !(d.cone > 0.0f && d.cone <= pi)) return "a cone outside (0, pi]";
 	if ((d.flags & NB_JOINT_CONE) && (d.motor_speed != 0.0f || d.max_motor_torque != 0.0f)) return "a CONE drive with a motor speed or torque";
-	if ((d.flags & (NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST)) && !unit_axis[d.joint]) return "a SLIDE, CONE or TWIST drive whose joint's axis_a is not of unit length";
-	if ((d.flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) && !unit_rel[d.joint]) return "a CONE or TWIST drive whose joint's rel_rotation is not of unit length";
+	if ((d.flags & (NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST)) && !js.unit_axis[d.joint]) return "a SLIDE, CONE or TWIST drive whose joint's axis_a is not of unit length";
+	if ((d.flags & (NB_JOINT_CONE | NB_JOINT_TWIST)) && !js.unit_rel[d.joint]) return "a CONE or TWIST drive whose joint's rel_rotation is not of unit length";
 	return nullptr;
 }
 
@@ -418,26 +413,21 @@ template<class T> static void keyed_order(const JointSet& js, const T* h, u32 n,
 	at.assign(js.n, -1);
 	for (u32 i : by_joint) at[js.order[h[i].joint]] = (int)i;
 }
-// Installs `next` in place of `cur`: the device table (one entry per joint in table order) staged into tbuf, and its rows into rbuf after
-// the first `keep` rows, which a larger row buffer keeps (the joints' own rows under the drives').  Synchronises only when the row buffer
-// grows.  The table and the rows are arguments of the joint kernels, null without a set, and the structure decides which rows
+// A row as an upload installs it: zeros but its accumulated impulse, which k_joint_rows builds the row around.
+static nb_constraint_row impulse_row(float impulse) { nb_constraint_row r; memset(&r, 0, sizeof(r)); r.impulse = impulse; return r; }
+// Installs `next`, with the row count of `rows`, in place of t's set: the device table (one entry per joint in table order) and its rows,
+// staged.  Synchronises only when
+// a buffer grows.  The table and the rows are arguments of the joint kernels, null without a set, and the structure decides which rows
 // k_joint_solve applies: nb_step's graph is re-recorded when the structure changed or a buffer moved.
-template<class E> static int put_keyed(nb_context* ctx, KeyedSet& cur, KeyedSet&& next, DevBuf<E>& tbuf, const std::vector<E>& table,
-		DevBuf<nb_constraint_row>& rbuf, size_t keep, const std::vector<nb_constraint_row>& rows, cudaStream_t st) {
-	const void* before[2] = { tbuf.p, rbuf.p };
-	GROW(tbuf, table.size(), st);
-	const size_t need = keep + rows.size();
-	if (need > rbuf.cap) {
-		DevBuf<nb_constraint_row> b;
-		if (int r = b.alloc(ctx, need)) return r;
-		if (keep) CK(cudaMemcpyAsync(b.p, rbuf.p, sizeof(nb_constraint_row) * keep, cudaMemcpyDeviceToDevice, st));
-		CK(cudaStreamSynchronize(st));
-		std::swap(rbuf, b);
-	}
-	CK(put_staged(ctx, tbuf.p, table.data(), sizeof(E) * table.size(), st));
-	CK(put_staged(ctx, rbuf.p + keep, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
-	if (next.structure != cur.structure || before[0] != tbuf.p || before[1] != rbuf.p) ++ctx->graph_epoch;
-	cur = std::move(next);
+template<class E> static int put_keyed(nb_context* ctx, KeyedTable<E>& t, KeyedSet&& next, const std::vector<E>& table, const std::vector<nb_constraint_row>& rows,
+		cudaStream_t st) {
+	const void* before[2] = { t.table.p, t.rows.p };
+	GROW(t.table, table.size(), st); GROW(t.rows, rows.size(), st);
+	CK(put_staged(ctx, t.table.p, table.data(), sizeof(E) * table.size(), st));
+	CK(put_staged(ctx, t.rows.p, rows.data(), sizeof(nb_constraint_row) * rows.size(), st));
+	if (next.structure != t.set.structure || before[0] != t.table.p || before[1] != t.rows.p) ++ctx->graph_epoch;
+	t.set = std::move(next);
+	t.set.nrows = (u32)rows.size();
 	return NB_OK;
 }
 // The host side of the download calls: the count, the capacity and null checks, then `get`.  Synchronises.
@@ -452,19 +442,19 @@ template<class T> static int download_keyed(nb_context* ctx, T* h, u32 capacity,
 	return NB_OK;
 }
 
-static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
-	return check_keyed(ctx, h, n, "drive", [&](const nb_joint_drive& d) { return drive_problem(d, nj, structure, unit_rel, unit_axis); });
+static int check_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, const JointShape& js) {
+	return check_keyed(ctx, h, n, "drive", [&](const nb_joint_drive& d) { return drive_problem(d, js); });
 }
 
 // Installs n checked drives in place of the set: the table (one entry per joint in table order, with the limits' and the cone's half-angle
-// pairs) and the appended rows holding the uploaded impulses, after the joints' own rows.
+// pairs) and the drive rows holding the uploaded impulses, per driven joint in table order.
 static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStream_t st) {
-	if (!n) { drop_drives(ctx); return NB_OK; }
+	if (!n) { drop_keyed(ctx, ctx->drives); return NB_OK; }
 	const JointSet& js = ctx->jset;
 	std::vector<u32> by_joint;
 	std::vector<int> at;   // table position -> drive
 	keyed_order(js, h, n, by_joint, at);
-	DriveSet ds;
+	KeyedSet ds;
 	ds.n = n;
 	for (u32 i : by_joint) ds.structure.insert(ds.structure.end(), { h[i].joint, h[i].flags });
 	std::vector<JointDrive> table(js.n);
@@ -474,35 +464,29 @@ static int set_drives(nb_context* ctx, const nb_joint_drive* h, u32 n, cudaStrea
 		if (at[p] < 0) continue;
 		const nb_joint_drive& d = h[at[p]];
 		JointDrive& e = table[p];
-		e.flags = d.flags; e.row = js.nrows + (u32)rows.size(); e.lower = d.lower; e.upper = d.upper;
+		e.flags = d.flags; e.row = (u32)rows.size(); e.lower = d.lower; e.upper = d.upper;
 		if (((d.flags & NB_JOINT_LIMIT) && js.structure[3 * (size_t)d.joint] == NB_JOINT_HINGE) || (d.flags & NB_JOINT_TWIST)) {
 			e.sl = (float)sin(0.5 * d.lower); e.cl = (float)cos(0.5 * d.lower); e.su = (float)sin(0.5 * d.upper); e.cu = (float)cos(0.5 * d.upper);
 		}
 		e.motor_speed = d.motor_speed; e.max_motor_torque = d.max_motor_torque; e.break_force = d.break_force; e.break_torque = d.break_torque;
 		e.broken = d.broken;
 		if (d.flags & NB_JOINT_CONE) { e.motor_speed = (float)sin(0.5 * d.cone); e.max_motor_torque = (float)cos(0.5 * d.cone); e.cone = d.cone; }
-		for (u32 k = 0; k < 3; ++k) {
-			if (!(d.flags & (k ? NB_JOINT_LIMIT | NB_JOINT_TWIST : NB_JOINT_MOTOR | NB_JOINT_CONE))) continue;
-			nb_constraint_row r;
-			memset(&r, 0, sizeof(r));
-			r.impulse = d.impulse[k];
-			rows.push_back(r);
-		}
+		for (u32 k = 0; k < 3; ++k)
+			if (d.flags & (k ? NB_JOINT_LIMIT | NB_JOINT_TWIST : NB_JOINT_MOTOR | NB_JOINT_CONE)) rows.push_back(impulse_row(d.impulse[k]));
 	}
-	ds.nrows = (u32)rows.size();
-	return put_keyed(ctx, ctx->dset, std::move(ds), ctx->drives, table, ctx->jrows, js.nrows, rows, st);
+	return put_keyed(ctx, ctx->drives, std::move(ds), table, rows, st);
 }
 
 // The drives in joint-index order with their rows' current impulses, broken flags and positions.  Synchronises.
 static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStream_t st) {
 	const JointSet& js = ctx->jset;
-	const DriveSet& ds = ctx->dset;
+	const KeyedSet& ds = ctx->drives.set;
 	out.resize(ds.n);
 	if (!ds.n) return NB_OK;
 	std::vector<JointDrive> table(js.n);
 	std::vector<nb_constraint_row> rows(ds.nrows);
-	CK(cudaMemcpyAsync(table.data(), ctx->drives.p, sizeof(JointDrive) * table.size(), cudaMemcpyDeviceToHost, st));
-	if (ds.nrows) CK(cudaMemcpyAsync(rows.data(), ctx->jrows.p + js.nrows, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(table.data(), ctx->drives.table.p, sizeof(JointDrive) * table.size(), cudaMemcpyDeviceToHost, st));
+	if (ds.nrows) CK(cudaMemcpyAsync(rows.data(), ctx->drives.rows.p, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
 	for (u32 m = 0; m < ds.n; ++m) {
 		const u32 joint = ds.structure[2 * (size_t)m];
@@ -511,7 +495,7 @@ static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStr
 		memset(&d, 0, sizeof(d));
 		d.joint = joint; d.flags = e.flags; d.lower = e.lower; d.upper = e.upper; d.motor_speed = e.motor_speed; d.max_motor_torque = e.max_motor_torque;
 		d.break_force = e.break_force; d.break_torque = e.break_torque; d.broken = e.broken;
-		u32 r = e.row - js.nrows;
+		u32 r = e.row;
 		for (u32 k = 0; k < 3; ++k) if (e.flags & (k ? NB_JOINT_LIMIT | NB_JOINT_TWIST : NB_JOINT_MOTOR | NB_JOINT_CONE)) d.impulse[k] = rows[r++].impulse;
 		const u32 type = js.structure[3 * (size_t)joint];
 		if (e.flags & (NB_JOINT_LIMIT | NB_JOINT_SLIDE | NB_JOINT_CONE | NB_JOINT_TWIST))
@@ -521,10 +505,9 @@ static int get_drives(nb_context* ctx, std::vector<nb_joint_drive>& out, cudaStr
 	return NB_OK;
 }
 
-// What nb_upload_joint_springs refuses in a spring of a joint set given by its structure, unit_rel and unit_axis (as drive_problem); null
-// if valid.
-static const char* spring_problem(const nb_joint_spring& s, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
-	if (s.joint >= nj) return "a joint index at or beyond the joint count";
+// What nb_upload_joint_springs refuses in a spring of a joint set of shape `js`; null if valid.
+static const char* spring_problem(const nb_joint_spring& s, const JointShape& js) {
+	if (s.joint >= js.structure.size() / 3) return "a joint index at or beyond the joint count";
 	if (s.reserved) return "reserved is not 0";
 	const float fields[] = { s.target[0], s.target[1], s.target[2], s.target[3], s.target_velocity, s.stiffness, s.damping, s.impulse[0], s.impulse[1],
 							 s.impulse[2], s.position };
@@ -537,26 +520,26 @@ static const char* spring_problem(const nb_joint_spring& s, u32 nj, const u32* s
 	const float gmin = 1e-12f, gmax = 1e12f;
 	for (float x : { s.stiffness, s.damping }) if (x != 0.0f && (x < gmin || x > gmax)) return "a stiffness or damping outside {0} and [1e-12, 1e12]";
 	if (fabsf(s.target_velocity) > gmax) return "a target velocity beyond 1e12";
-	const u32 type = structure[3 * (size_t)s.joint];
+	const u32 type = js.structure[3 * (size_t)s.joint];
 	if ((type == NB_JOINT_FIXED || type == NB_JOINT_DISTANCE) && fabsf(s.target[0]) > gmax) return "a target beyond 1e12";
 	if (type != NB_JOINT_BALL && (s.target[1] != 0.0f || s.target[2] != 0.0f || s.target[3] != 0.0f)) return "a nonzero target word the joint's type does not read";
 	const float pi = 3.14159265358979f;
 	if (type == NB_JOINT_HINGE && (s.target[0] < -pi || s.target[0] > pi)) return "a hinge target outside [-pi, pi]";
-	if (type == NB_JOINT_HINGE && !unit_rel[s.joint]) return "a HINGE spring whose joint's rel_rotation is not of unit length";
-	if (type == NB_JOINT_FIXED && !unit_axis[s.joint]) return "a FIXED spring whose joint's axis_a is not of unit length";
+	if (type == NB_JOINT_HINGE && !js.unit_rel[s.joint]) return "a HINGE spring whose joint's rel_rotation is not of unit length";
+	if (type == NB_JOINT_FIXED && !js.unit_axis[s.joint]) return "a FIXED spring whose joint's axis_a is not of unit length";
 	if (type == NB_JOINT_DISTANCE && s.target[0] < 0.0f) return "a negative distance target";
 	if (type == NB_JOINT_BALL && s.target_velocity != 0.0f) return "a BALL spring with a target velocity";
 	if (type == NB_JOINT_BALL && !unit_quat(s.target)) return "a BALL target rotation not of unit length";
 	return nullptr;
 }
-static int check_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, u32 nj, const u32* structure, const uint8_t* unit_rel, const uint8_t* unit_axis) {
-	return check_keyed(ctx, h, n, "spring", [&](const nb_joint_spring& s) { return spring_problem(s, nj, structure, unit_rel, unit_axis); });
+static int check_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, const JointShape& js) {
+	return check_keyed(ctx, h, n, "spring", [&](const nb_joint_spring& s) { return spring_problem(s, js); });
 }
 
 // Installs n checked springs in place of the set: the table (one entry per joint in table order, a hinge's target as its half-angle pair)
 // and the spring rows holding the uploaded impulses, per sprung joint in table order.
 static int set_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, cudaStream_t st) {
-	if (!n) { drop_springs(ctx); return NB_OK; }
+	if (!n) { drop_keyed(ctx, ctx->springs); return NB_OK; }
 	const JointSet& js = ctx->jset;
 	std::vector<u32> by_joint;
 	std::vector<int> at;   // table position -> spring
@@ -576,27 +559,21 @@ static int set_springs(nb_context* ctx, const nb_joint_spring* h, u32 n, cudaStr
 		for (u32 k = 0; k < 4; ++k) e.target[k] = s.target[k];
 		if (type == NB_JOINT_HINGE) { e.target[0] = (float)sin(0.5 * s.target[0]); e.target[1] = (float)cos(0.5 * s.target[0]); e.angle = s.target[0]; }
 		e.target_velocity = s.target_velocity; e.stiffness = s.stiffness; e.damping = s.damping; e.max_force = s.max_force;
-		for (u32 k = 0; k < spring_row_count(type); ++k) {
-			nb_constraint_row r;
-			memset(&r, 0, sizeof(r));
-			r.impulse = s.impulse[k];
-			rows.push_back(r);
-		}
+		for (u32 k = 0; k < spring_row_count(type); ++k) rows.push_back(impulse_row(s.impulse[k]));
 	}
-	ss.nrows = (u32)rows.size();
-	return put_keyed(ctx, ctx->sset, std::move(ss), ctx->springs, table, ctx->srows, 0, rows, st);
+	return put_keyed(ctx, ctx->springs, std::move(ss), table, rows, st);
 }
 
 // The springs in joint-index order with their rows' current impulses and positions.  Synchronises.
 static int get_springs(nb_context* ctx, std::vector<nb_joint_spring>& out, cudaStream_t st) {
 	const JointSet& js = ctx->jset;
-	const KeyedSet& ss = ctx->sset;
+	const KeyedSet& ss = ctx->springs.set;
 	out.resize(ss.n);
 	if (!ss.n) return NB_OK;
 	std::vector<JointSpring> table(js.n);
 	std::vector<nb_constraint_row> rows(ss.nrows);
-	CK(cudaMemcpyAsync(table.data(), ctx->springs.p, sizeof(JointSpring) * table.size(), cudaMemcpyDeviceToHost, st));
-	CK(cudaMemcpyAsync(rows.data(), ctx->srows.p, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(table.data(), ctx->springs.table.p, sizeof(JointSpring) * table.size(), cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(rows.data(), ctx->springs.rows.p, sizeof(nb_constraint_row) * rows.size(), cudaMemcpyDeviceToHost, st));
 	CK(cudaStreamSynchronize(st));
 	for (u32 m = 0; m < ss.n; ++m) {
 		const u32 joint = ss.structure[m], type = js.structure[3 * (size_t)joint];
@@ -616,6 +593,39 @@ static int get_springs(nb_context* ctx, std::vector<nb_joint_spring>& out, cudaS
 __global__ void __launch_bounds__(NB_BLOCK) k_joint_wake(const u32* bodies, u32 n, uint8_t* idle) {
 	for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) idle[bodies[i]] = 0;
 }
+// Sets the idle counter of each listed body to 0: the list staged into spawn_idx, then one launch of k_joint_wake (none for an empty list).
+static int wake_bodies(nb_context* ctx, const std::vector<u32>& bodies, cudaStream_t st) {
+	if (bodies.empty()) return NB_OK;
+	GROW(ctx->spawn_idx, bodies.size(), st);
+	CK(put_staged(ctx, ctx->spawn_idx.p, bodies.data(), sizeof(u32) * bodies.size(), st));
+	launch_grid(mk_launch(ctx, st), k_joint_wake, GRID(bodies.size()), ctx->spawn_idx.p, (u32)bodies.size(), ctx->idle);
+	CK(cudaGetLastError());
+	return NB_OK;
+}
+
+// A whole joint set on the host in the public types, as a state file holds it and body removal renumbers it: the joints in upload order
+// with their current impulses, and the drives and springs in joint order.
+struct JointBundle { std::vector<nb_joint> joints; std::vector<nb_joint_drive> drives; std::vector<nb_joint_spring> springs; };
+// The context's joint set.  Synchronises.
+static int get_joint_bundle(nb_context* ctx, JointBundle& b, cudaStream_t st) {
+	if (int r = get_joints(ctx, b.joints, st)) return r;
+	if (int r = get_drives(ctx, b.drives, st)) return r;
+	return get_springs(ctx, b.springs, st);
+}
+// The upload's checks for a context with B bodies: the joints, then the drives and springs against the bundle's own joints.
+static int check_joint_bundle(nb_context* ctx, const JointBundle& b, u32 B) {
+	const u32 n = (u32)b.joints.size();
+	if (int r = check_joints(ctx, b.joints.data(), n, B)) return r;
+	const JointShape shape = joint_shape(b.joints.data(), n);
+	if (int r = check_drives(ctx, b.drives.data(), (u32)b.drives.size(), shape)) return r;
+	return check_springs(ctx, b.springs.data(), (u32)b.springs.size(), shape);
+}
+// Installs a checked bundle in place of the context's joint set; an empty table removes the context's.
+static int put_joint_bundle(nb_context* ctx, const JointBundle& b, cudaStream_t st) {
+	if (int r = set_joints(ctx, b.joints.data(), (u32)b.joints.size(), st)) return r;
+	if (int r = set_drives(ctx, b.drives.data(), (u32)b.drives.size(), st)) return r;
+	return set_springs(ctx, b.springs.data(), (u32)b.springs.size(), st);
+}
 
 extern "C" {
 
@@ -632,24 +642,23 @@ int nb_download_joints(nb_context* ctx, nb_joint* h, uint32_t capacity, uint32_t
 
 int nb_upload_joint_drives(nb_context* ctx, const nb_joint_drive* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_upload_joint_drives");
-	const JointSet& js = ctx->jset;
-	if (int r = check_drives(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data(), js.unit_axis.data())) return r;
+	if (int r = check_drives(ctx, h, n, ctx->jset)) return r;
 	return set_drives(ctx, h, n, (cudaStream_t)stream);
 }
 
 int nb_download_joint_drives(nb_context* ctx, nb_joint_drive* h, uint32_t capacity, uint32_t* count, void* stream) {
 	NB_RANGE("nb_download_joint_drives");
-	return download_keyed(ctx, h, capacity, count, ctx->dset.n, "drive", get_drives, (cudaStream_t)stream);
+	return download_keyed(ctx, h, capacity, count, ctx->drives.set.n, "drive", get_drives, (cudaStream_t)stream);
 }
 
 int nb_upload_joint_springs(nb_context* ctx, const nb_joint_spring* h, uint32_t n, void* stream) {
 	NB_RANGE("nb_upload_joint_springs");
 	const JointSet& js = ctx->jset;
-	if (int r = check_springs(ctx, h, n, js.n, js.structure.data(), js.unit_rel.data(), js.unit_axis.data())) return r;
+	if (int r = check_springs(ctx, h, n, js)) return r;
 	cudaStream_t st = (cudaStream_t)stream;
 	if (int r = set_springs(ctx, h, n, st)) return r;
-	// the sprung joints' dynamic bodies get idle counter 0, so that a new target reaches a body that has fallen asleep (k_joint_wake, as
-	// nb_remove_bodies wakes a joint's kept side); not body 0, not a kinematic body
+	// the sprung joints' dynamic bodies get idle counter 0, so that a new target reaches a body that has fallen asleep (as nb_remove_bodies
+	// wakes a joint's kept side); not body 0, not a kinematic body
 	std::vector<u32> wake;
 	for (u32 i = 0; i < n; ++i)
 		for (u32 k = 0; k < 2; ++k) {
@@ -658,17 +667,12 @@ int nb_upload_joint_springs(nb_context* ctx, const nb_joint_spring* h, uint32_t 
 		}
 	std::sort(wake.begin(), wake.end());
 	wake.erase(std::unique(wake.begin(), wake.end()), wake.end());
-	if (wake.empty()) return NB_OK;
-	GROW(ctx->spawn_idx, wake.size(), st);
-	CK(put_staged(ctx, ctx->spawn_idx.p, wake.data(), sizeof(u32) * wake.size(), st));
-	launch_grid(mk_launch(ctx, st), k_joint_wake, GRID(wake.size()), ctx->spawn_idx.p, (u32)wake.size(), ctx->idle);
-	CK(cudaGetLastError());
-	return NB_OK;
+	return wake_bodies(ctx, wake, st);
 }
 
 int nb_download_joint_springs(nb_context* ctx, nb_joint_spring* h, uint32_t capacity, uint32_t* count, void* stream) {
 	NB_RANGE("nb_download_joint_springs");
-	return download_keyed(ctx, h, capacity, count, ctx->sset.n, "spring", get_springs, (cudaStream_t)stream);
+	return download_keyed(ctx, h, capacity, count, ctx->springs.set.n, "spring", get_springs, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,12 +1,13 @@
 // nudge_b200 — device-resident snapshots (nb_snapshot_create, nb_snapshot_destroy, nb_snapshot_save, nb_snapshot_restore; DESIGN.md
 // section 8.12).
 //
-// A snapshot is the context's between-steps state in HBM: the sections of a state file (state_sections, nb_state_api.cuh) plus what a file
-// lacks, the user rows, the joint table, the joints' rows, the joint drive table, the joint spring table and rows, the continuous-collision set (host side), the kind bytes, the sensor overlap list, the count words the state owns and the NB_FILTER_SKIP_CONNECTED key list
-// (snapshot_sections).  Save and restore are one launch of k_snapshot_copy in opposite directions; the host side (counts, bits, table set,
-// the connections' host copy, the kinematic set, the rows' levelling) is kept in the snapshot and installed by install_state.
-// Every section but the user rows, the joints and the overlap list has its room at the context's capacities in one arena, laid out once from the
-// capacity header; those are sized at the save and grown by it.  Included at the end of nb_api.cu.
+// A snapshot is the context's between-steps state in HBM: the device sections of a state file (state_sections, nb_state_api.cuh) plus what
+// a file lacks, the kind bytes, the NB_FILTER_SKIP_CONNECTED key list, the count words the state owns, the user rows, the joint table and
+// rows, the joint drive and spring tables with their rows and the sensor overlap list (snapshot_sections).  Save and restore are one launch
+// of k_snapshot_copy in opposite directions; the host side (counts, bits, table set, the connections' host copy, the kinematic set, the
+// rows' levelling, the joint sets' host sides, the continuous-collision set) is kept in the snapshot and installed by install_state.  The
+// arena sections have their room at the context's capacities in one arena, laid out once from the capacity header; the rest are sized at
+// the save and grown by it.  Included at the end of nb_api.cu.
 #pragma once
 
 #define NB_SNAP_SECTIONS 64   // two per lane of k_snapshot_copy's first warp
@@ -57,49 +58,60 @@ struct nb_snapshot {
 	u32* words;
 	DevBuf<nb_constraint_row> rows;                  // user rows in device order
 	DevBuf<uint4> overlaps;                          // the sensor overlap list
-	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows (the drives' appended rows included)
-	DevBuf<JointDrive> drives;                                  // the joint drive table
-	DevBuf<JointSpring> springs; DevBuf<nb_constraint_row> srows;   // the joint spring table and the spring rows
+	DevBuf<nb_joint> joints; DevBuf<nb_constraint_row> jrows;   // the joint table and the joints' rows
+	KeyedTable<JointDrive> drives; KeyedTable<JointSpring> springs;   // with the host side of the sets at the save
 	// the host side at the save
-	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset; DriveSet dset; KeyedSet sset;
+	NbStateHeader h; StateShape shape; RowLevels urow_set; JointSet jset;
 	std::vector<nb_ccd_body> ccd;                    // the continuous-collision set (its rows are host values; k_ccd rewrites the factors)
 };
 
 // A snapshot section: the context's buffer, the snapshot's copy, and the counter word (>= 0) that holds the element count on the device.
 struct SnapPart { void* ctx_ptr; void* snap_ptr; size_t size, count; bool present; int word; };
 
-// The sections of a snapshot with header `h`: the state file's (a file keeps the kinematic indices on the host, the snapshot keeps them in
-// its host side and the kind bytes), then the snapshot's own.  The fixed sections come first, the rows and the overlap list last.  With `s`
-// null the snapshot pointers are offsets into the arena, and there are no rows or joints.
-static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 conn_probe) {
-	const JointSet none, &js = s ? s->jset : none;
-	const KeyedSet knone, &ds = s ? s->dset : knone, &ss = s ? s->sset : knone;
-	const u32 nrows = s ? s->urow_set.n : 0;
+// The sections a snapshot with header `h` keeps in its arena, in arena order: the state file's device sections (its host-only sections are
+// the snapshot's host side, the kinematic indices also its kind bytes), the kind bytes and the key list.  With `s` null the snapshot
+// pointers are null: the arena's layout.
+static std::vector<SnapPart> arena_sections(nb_context* ctx, const nb_snapshot* s, const NbStateHeader& h, u32 conn_probe) {
 	StateHostCopies hc;
 	std::vector<SnapPart> p;
 	auto at = [&](size_t i) -> void* { return s ? s->arena.p + s->off[i] : nullptr; };
-	for (const StateSection& x : state_sections(ctx, h, hc, false))
-		p.push_back({ x.dev, at(p.size()), x.size, x.count, x.present && x.dev != nullptr, x.word });
+	for (const StateSection& x : state_sections(ctx, h, NbStateExt(), hc, false))
+		if (!x.host_only) p.push_back({ x.dev, at(p.size()), x.size, x.count, x.present && x.dev != nullptr, x.word });
 	p.push_back({ ctx->kind, at(p.size()), 1, h.bodies, h.reserved[4] != 0, -1 });
 	p.push_back({ ctx->conn_keys, at(p.size()), 8, conn_probe, conn_probe != 0, -1 });
-	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s ? s->words + j : nullptr, 4, 1, true, -1 });
-	p.push_back({ ctx->urows.p, s ? s->rows.p : nullptr, sizeof(nb_constraint_row), nrows, nrows != 0, -1 });
-	p.push_back({ ctx->joints.p, s ? s->joints.p : nullptr, sizeof(nb_joint), js.n, js.n != 0, -1 });
-	p.push_back({ ctx->jrows.p, s ? s->jrows.p : nullptr, sizeof(nb_constraint_row), (size_t)js.nrows + ds.nrows, js.n != 0, -1 });
-	p.push_back({ ctx->drives.p, s ? s->drives.p : nullptr, sizeof(JointDrive), js.n, ds.n != 0, -1 });
-	p.push_back({ ctx->springs.p, s ? s->springs.p : nullptr, sizeof(JointSpring), js.n, ss.n != 0, -1 });
-	p.push_back({ ctx->srows.p, s ? s->srows.p : nullptr, sizeof(nb_constraint_row), ss.nrows, ss.n != 0, -1 });
-	p.push_back({ ctx->sensor_old.p, s ? s->overlaps.p : nullptr, sizeof(uint4), h.reserved[3], h.reserved[2] != 0, CNT_SENSOR_OLD });
 	return p;
 }
-static const size_t kSnapFixed = 20 + 2;   // the state file's 20 sections, the kind bytes and the key list: the sections in the arena
+// A keyed table's two sections, its entries (one per joint of a set of nj) and its rows: the context's `c`, the snapshot's `s`.
+template<class E> static void keyed_sections(std::vector<SnapPart>& p, const KeyedTable<E>& c, const KeyedTable<E>& s, u32 nj) {
+	p.push_back({ c.table.p, s.table.p, sizeof(E), nj, s.set.n != 0, -1 });
+	p.push_back({ c.rows.p, s.rows.p, sizeof(nb_constraint_row), s.set.nrows, s.set.n != 0, -1 });
+}
+// The sections of snapshot `s`: the arena's, then the count words and the sections sized at the save, the overlap list last.
+static std::vector<SnapPart> snapshot_sections(nb_context* ctx, const nb_snapshot* s, u32 conn_probe) {
+	const JointSet& js = s->jset;
+	const u32 nrows = s->urow_set.n;
+	std::vector<SnapPart> p = arena_sections(ctx, s, s->h, conn_probe);
+	for (int j = 0; j < 3; ++j) p.push_back({ ctx->counts + kSnapWords[j], s->words + j, 4, 1, true, -1 });
+	p.push_back({ ctx->urows.p, s->rows.p, sizeof(nb_constraint_row), nrows, nrows != 0, -1 });
+	p.push_back({ ctx->joints.p, s->joints.p, sizeof(nb_joint), js.n, js.n != 0, -1 });
+	p.push_back({ ctx->jrows.p, s->jrows.p, sizeof(nb_constraint_row), js.nrows, js.n != 0, -1 });
+	keyed_sections(p, ctx->drives, s->drives, js.n);
+	keyed_sections(p, ctx->springs, s->springs, js.n);
+	p.push_back({ ctx->sensor_old.p, s->overlaps.p, sizeof(uint4), s->h.reserved[3], s->h.reserved[2] != 0, CNT_SENSOR_OLD });
+	return p;
+}
+// Makes keyed table `t` hold `set` of a joint set of nj joints.
+template<class E> static int grow_keyed(nb_context* ctx, KeyedTable<E>& t, const KeyedSet& set, u32 nj, cudaStream_t st) {
+	GROW(t.table, set.n ? nj : 0, st); GROW(t.rows, set.nrows, st);
+	return NB_OK;
+}
 
 // The table of one copy.  save: context -> snapshot; restore: snapshot -> context, with the overlap list also copied to the current list
 // and its length to the current count (nb_download_sensor_overlaps returns what it returned at the save).  A device count is read on the
 // side the copy comes from.
 static int snapshot_table(nb_context* ctx, const nb_snapshot* s, bool save, SnapTable& t) {
 	const u32 probe = (s->shape.filter_flags & NB_FILTER_SKIP_CONNECTED) ? s->shape.nconn : 0;
-	std::vector<SnapPart> parts = snapshot_sections(ctx, s, s->h, probe);
+	std::vector<SnapPart> parts = snapshot_sections(ctx, s, probe);
 	if (!save && s->shape.has_sensor) {
 		parts.push_back({ ctx->sensor_cur.p, s->overlaps.p, sizeof(uint4), s->h.reserved[3], true, CNT_SENSOR_OLD });
 		parts.push_back({ ctx->counts + CNT_SENSOR_HITS, s->words + 2, 4, 1, true, -1 });
@@ -150,8 +162,7 @@ int nb_snapshot_create(nb_context* ctx, nb_snapshot** out) {
 	nb_snapshot* s = new nb_snapshot();
 	s->ctx = ctx;
 	size_t bytes = 0;
-	const std::vector<SnapPart> parts = snapshot_sections(ctx, nullptr, cap, c.max_connections);
-	for (size_t i = 0; i < kSnapFixed; ++i) { s->off.push_back(bytes); bytes += (parts[i].size * parts[i].count + 15) & ~(size_t)15; }
+	for (const SnapPart& x : arena_sections(ctx, nullptr, cap, c.max_connections)) { s->off.push_back(bytes); bytes += (x.size * x.count + 15) & ~(size_t)15; }
 	if (int r = s->arena.alloc(ctx, bytes + 16)) { delete s; ctx->error = "nb_snapshot_create: " + ctx->error; return r; }
 	s->words = reinterpret_cast<u32*>(s->arena.p + bytes);
 	ctx->snapshots.push_back(s);
@@ -174,11 +185,12 @@ int nb_snapshot_save(nb_context* ctx, nb_snapshot* s, void* stream) {
 	JOIN_UPLOADS();   // the copy reads the momentum and property rows
 	// grown: the only save that synchronises and allocates
 	GROW(s->rows, ctx->urow_set.n, st); GROW(s->overlaps, ctx->has_sensor ? ctx->sensor_cap : 0, st);
-	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, (size_t)ctx->jset.nrows + ctx->dset.nrows, st); GROW(s->drives, ctx->dset.n ? ctx->jset.n : 0, st);
-	GROW(s->springs, ctx->sset.n ? ctx->jset.n : 0, st); GROW(s->srows, ctx->sset.nrows, st);
+	GROW(s->joints, ctx->jset.n, st); GROW(s->jrows, ctx->jset.nrows, st);
+	if (int r = grow_keyed(ctx, s->drives, ctx->drives.set, ctx->jset.n, st)) return r;
+	if (int r = grow_keyed(ctx, s->springs, ctx->springs.set, ctx->jset.n, st)) return r;
 	s->h = state_header_of(ctx, ctx->cfg.max_contacts);   // the device count decides how many cache entries are copied
 	s->shape = state_shape_of(ctx);
-	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->dset = ctx->dset; s->sset = ctx->sset; s->ccd = ctx->ccd;
+	s->urow_set = ctx->urow_set; s->jset = ctx->jset; s->drives.set = ctx->drives.set; s->springs.set = ctx->springs.set; s->ccd = ctx->ccd;
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, true, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
@@ -197,21 +209,24 @@ int nb_snapshot_restore(nb_context* ctx, const nb_snapshot* s, void* stream) {
 	if (s->shape.has_frc) { ALLOC(ctx->frc, ctx->cfg.max_bodies); ALLOC(ctx->frc_spare, ctx->cfg.max_bodies); }
 	if (!s->shape.kin.empty()) ALLOC(ctx->kind, ctx->cfg.max_bodies);
 	GROW(ctx->urows, s->urow_set.n, st);
-	const void* joint_bufs[5] = { ctx->joints.p, ctx->jrows.p, ctx->drives.p, ctx->springs.p, ctx->srows.p };
-	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, (size_t)s->jset.nrows + s->dset.nrows, st); GROW(ctx->drives, s->dset.n ? s->jset.n : 0, st);
-	GROW(ctx->springs, s->sset.n ? s->jset.n : 0, st); GROW(ctx->srows, s->sset.nrows, st);
+	auto joint_bufs = [&] {
+		return std::vector<const void*>{ ctx->joints.p, ctx->jrows.p, ctx->drives.table.p, ctx->drives.rows.p, ctx->springs.table.p, ctx->springs.rows.p };
+	};
+	const std::vector<const void*> before = joint_bufs();
+	GROW(ctx->joints, s->jset.n, st); GROW(ctx->jrows, s->jset.nrows, st);
+	if (int r = grow_keyed(ctx, ctx->drives, s->drives.set, s->jset.n, st)) return r;
+	if (int r = grow_keyed(ctx, ctx->springs, s->springs.set, s->jset.n, st)) return r;
 	if (s->shape.has_sensor) { int r = ensure_sensor_lists(ctx, s->shape.sensor_cap, st); if (r) return r; }
 	SnapTable t;
 	{ int r = snapshot_table(ctx, s, false, t); if (r) return r; }
 	{ int r = snapshot_launch(ctx, t, st); if (r) return r; }
 	StateShape shape = s->shape;
 	{ int r = install_state(ctx, shape, nullptr, st); if (r) return r; }
-	// the row and joint levels are host values in the graph, the joint buffers its kernel arguments
+	// the row and joint levels are host values in the graph, the joint buffers its kernel arguments: a structure changed or a buffer moved
 	if (s->urow_set.n != ctx->urow_set.n || s->urow_set.level_off != ctx->urow_set.level_off) ++ctx->graph_epoch;
-	if (s->jset.structure != ctx->jset.structure || joint_bufs[0] != ctx->joints.p || joint_bufs[1] != ctx->jrows.p) ++ctx->graph_epoch;
-	else if (s->dset.structure != ctx->dset.structure || joint_bufs[2] != ctx->drives.p) ++ctx->graph_epoch;
-	else if (s->sset.structure != ctx->sset.structure || joint_bufs[3] != ctx->springs.p || joint_bufs[4] != ctx->srows.p) ++ctx->graph_epoch;
-	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->dset = s->dset; ctx->sset = s->sset;
+	if (s->jset.structure != ctx->jset.structure || s->drives.set.structure != ctx->drives.set.structure ||
+		s->springs.set.structure != ctx->springs.set.structure || before != joint_bufs()) ++ctx->graph_epoch;
+	ctx->urow_set = s->urow_set; ctx->jset = s->jset; ctx->drives.set = s->drives.set; ctx->springs.set = s->springs.set;
 	{ int r = set_ccd(ctx, s->ccd, st); if (r) return r; }   // nothing when the context holds the same set
 	ctx->scene_edited = true;   // the last collide's outputs belong to another state
 	ctx->in_step = false;

@@ -216,31 +216,30 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 		const nb_body_pair p = ctx->conn_host[i];
 		if (!removed(p.a) && !removed(p.b)) conn.push_back({ remap(p.a), remap(p.b) });
 	}
-	// the kept joints with their current impulses, remapped, and the kept dynamic bodies that lose a joint
+	// the kept joints with their current impulses, remapped, their drives and springs renumbered, and the kept dynamic bodies that lose a joint
 	cudaStream_t st = (cudaStream_t)stream;
-	std::vector<nb_joint> old_joints, joints;
-	std::vector<u32> joint_wake, joint_new(ctx->jset.n, ~0u);   // joint_new: old joint index -> new one (~0u: deleted)
-	std::vector<nb_joint_drive> drives;
-	std::vector<nb_joint_spring> springs;
-	if (int r = get_joints(ctx, old_joints, st)) return r;
-	if (int r = get_drives(ctx, drives, st)) return r;
-	if (int r = get_springs(ctx, springs, st)) return r;
-	for (u32 i = 0; i < old_joints.size(); ++i) {
-		nb_joint j = old_joints[i];
+	JointBundle jb;
+	if (int r = get_joint_bundle(ctx, jb, st)) return r;
+	std::vector<u32> joint_wake, joint_new(jb.joints.size(), ~0u);   // joint_new: old joint index -> new one (~0u: deleted)
+	u32 kept_joints = 0;
+	for (u32 i = 0; i < jb.joints.size(); ++i) {
+		nb_joint j = jb.joints[i];
 		if (removed(j.a) || removed(j.b)) {
 			const u32 other = removed(j.a) ? j.b : j.a;
 			if (other && !removed(other) && !std::binary_search(kin.begin(), kin.end(), remap(other))) joint_wake.push_back(remap(other));
 			continue;
 		}
 		j.a = remap(j.a); j.b = remap(j.b);
-		joint_new[i] = (u32)joints.size();
-		joints.push_back(j);
+		joint_new[i] = kept_joints;
+		jb.joints[kept_joints++] = j;
 	}
-	// the drives of the kept joints, renumbered, with their current impulses and broken flags
-	std::vector<nb_joint_drive> kept_drives;
-	for (nb_joint_drive d : drives) if (joint_new[d.joint] != ~0u) { d.joint = joint_new[d.joint]; kept_drives.push_back(d); }
-	std::vector<nb_joint_spring> kept_springs;   // and the springs
-	for (nb_joint_spring s : springs) if (joint_new[s.joint] != ~0u) { s.joint = joint_new[s.joint]; kept_springs.push_back(s); }
+	jb.joints.resize(kept_joints);
+	auto renumber = [&](auto& entries) {   // the entries of the kept joints, in joint order
+		size_t k = 0;
+		for (auto e : entries) if (joint_new[e.joint] != ~0u) { e.joint = joint_new[e.joint]; entries[k++] = e; }
+		entries.resize(k);
+	};
+	renumber(jb.drives); renumber(jb.springs);
 	const u32 nrows = kept.n;
 	const bool rows_changed = nrows != us.n;   // a deleted row can change the levels, which nb_step's graph holds
 	std::vector<u32> staging(list);   // the list, then the rows' gather permutation (new device position -> old one)
@@ -311,13 +310,8 @@ int nb_remove_bodies(nb_context* ctx, const uint32_t* h, uint32_t n, void* strea
 	// nb_step's graph keys on B, the collider and connection counts, tagbits and kbits, so it re-records when they change; table contents
 	// are read through unchanged pointers.  The row levels are host values inside the graph.
 	if (rows_changed) ++ctx->graph_epoch;
-	if (!joint_wake.empty()) {
-		CK(put_staged(ctx, ctx->spawn_idx.p, joint_wake.data(), sizeof(u32) * joint_wake.size(), st));
-		launch_grid(L, k_joint_wake, GRID(joint_wake.size()), ctx->spawn_idx.p, (u32)joint_wake.size(), ctx->idle);
-	}
-	if (!old_joints.empty()) { int r = set_joints(ctx, joints.data(), (u32)joints.size(), st); if (r) return r; }
-	if (!drives.empty()) { int r = set_drives(ctx, kept_drives.data(), (u32)kept_drives.size(), st); if (r) return r; }
-	if (!springs.empty()) { int r = set_springs(ctx, kept_springs.data(), (u32)kept_springs.size(), st); if (r) return r; }
+	if (int r = wake_bodies(ctx, joint_wake, st)) return r;
+	if (int r = put_joint_bundle(ctx, jb, st)) return r;
 	if (int r = set_ccd(ctx, std::move(ccd), st)) return r;
 	return build_conn_lookup(ctx, st);
 }

@@ -5,7 +5,7 @@
 //
 // File layout (little endian): header { char magic[8] = "NBSTATE1"; u32 version; u32 bodies, boxes, spheres, connections, cache;
 // u32 solver_mode; u32 reserved[8]; }, from version 8 a header extension { u32 ccd_bodies; u32 reserved[3]; }, and these sections in this
-// order (state_sections, then the continuous-collision rows and the joint springs), each padded with zeros to 16 bytes:
+// order (state_sections), each padded with zeros to 16 bytes:
 //   section                                        element (B)  count            present when
 //   transforms | properties | momentum | idle      32 16 32 1   bodies           always
 //   box_tags | box_data | box_transforms           4 16 32      boxes            always
@@ -56,14 +56,16 @@ static bool state_header_read(FILE* f, NbStateHeader& h, NbStateExt& x) {
 
 // One section: `count` elements of `size` bytes in device memory at `dev` or, without it, in the host buffer `host`.  A load reads into
 // `host` when it is given and then copies to `dev` when that is given.  word >= 0: a context holds the element count in counts[word] (a
-// file holds it in the header; a snapshot copies it on the device, nb_snapshot_api.cuh).
-struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; int word; };
-struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc, joints, drives; };
+// file holds it in the header; a snapshot copies it on the device, nb_snapshot_api.cuh).  host_only: the section never has a device
+// buffer; a snapshot keeps it in its host side instead.
+struct StateSection { void* dev; std::vector<unsigned char>* host; size_t size, count; bool present; int word; bool host_only = false; };
+struct StateHostCopies { std::vector<unsigned char> mom, box_tags, sph_tags, conn, sensor, kin, frc, joints, drives, ccd, springs; };
 
-// The sections of the file with header `h`, in file order.  A load keeps in `hc` the momentum rows (the kinematic velocities), the tags
-// (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices, the body force rows, the joints
-// and their drives (checked before they are copied to the device); a save writes the kinematic indices, the joints and the drives from hc.  Snapshots extend this list (snapshot_sections).
-static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, StateHostCopies& hc, bool load) {
+// The sections of the file with header `h` and extension `x`, in file order.  A load keeps in `hc` the momentum rows (the kinematic
+// velocities), the tags (tagbits), the connections (the context's host copy), the sensor flags (set_sensors), the kinematic indices, the body
+// force rows, the joint set and the continuous-collision rows (checked before they are installed); a save writes the host-only sections from
+// hc.  Snapshots extend this list (snapshot_sections).
+static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHeader& h, const NbStateExt& x, StateHostCopies& hc, bool load) {
 	const size_t K = (size_t)h.boxes + h.spheres;
 	return {
 		{ ctx->xf, nullptr, sizeof(nb_transform), h.bodies, true, -1 }, { ctx->props, nullptr, sizeof(nb_body_properties), h.bodies, true, -1 },
@@ -77,11 +79,23 @@ static std::vector<StateSection> state_sections(nb_context* ctx, const NbStateHe
 		{ ctx->cache_data, nullptr, 16, h.cache, true, CNT_CACHE },
 		{ ctx->filter, nullptr, 4, K, h.reserved[1] != 0, -1 },
 		{ load ? nullptr : ctx->sensor, &hc.sensor, 1, K, h.reserved[2] != 0, -1 },
-		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0, -1 },
+		{ nullptr, &hc.kin, 4, h.reserved[4], h.reserved[4] != 0, -1, true },
 		{ load ? nullptr : ctx->frc, &hc.frc, sizeof(nb_body_force), h.bodies, h.reserved[5] != 0, -1 },
-		{ nullptr, &hc.joints, sizeof(nb_joint), h.reserved[6], h.reserved[6] != 0, -1 },
-		{ nullptr, &hc.drives, sizeof(nb_joint_drive), h.reserved[7], h.reserved[7] != 0, -1 },
+		{ nullptr, &hc.joints, sizeof(nb_joint), h.reserved[6], h.reserved[6] != 0, -1, true },
+		{ nullptr, &hc.drives, sizeof(nb_joint_drive), h.reserved[7], h.reserved[7] != 0, -1, true },
+		{ nullptr, &hc.ccd, sizeof(nb_ccd_body), x.ccd_bodies, h.version >= 8, -1, true },
+		{ nullptr, &hc.springs, sizeof(nb_joint_spring), x.reserved[0], h.version == 9, -1, true },
 	};
+}
+// A host table's bytes, as a host-only section holds them.
+template<class T> static std::vector<unsigned char> as_bytes(const std::vector<T>& v) {
+	const unsigned char* p = reinterpret_cast<const unsigned char*>(v.data());
+	return std::vector<unsigned char>(p, p + sizeof(T) * v.size());
+}
+// The first n elements of a section read into `b`, fewer when the read stopped short.
+template<class T> static std::vector<T> from_bytes(const std::vector<unsigned char>& b, size_t n) {
+	const T* p = reinterpret_cast<const T*>(b.data());
+	return std::vector<T>(p, p + std::min(n, b.size() / sizeof(T)));
 }
 
 // The header a save of the context writes, with `cache` cache entries.
@@ -89,12 +103,12 @@ static NbStateHeader state_header_of(const nb_context* ctx, u32 cache) {
 	NbStateHeader h; memset(&h, 0, sizeof(h));
 	memcpy(h.magic, "NBSTATE1", 8);
 	const bool filtered = ctx->has_filter || ctx->filter_flags;
-	h.version = ctx->sset.n ? 9 : !ctx->ccd.empty() ? 8 : ctx->dset.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
+	h.version = ctx->springs.set.n ? 9 : !ctx->ccd.empty() ? 8 : ctx->drives.set.n ? 7 : ctx->jset.n ? 6 : ctx->has_frc ? 5 : ctx->has_kin ? 4 : ctx->has_sensor ? 3 : filtered ? 2 : 1;
 	if (filtered) { h.reserved[0] = ctx->filter_flags; h.reserved[1] = ctx->has_filter ? 1 : 0; }
 	if (ctx->has_sensor) { h.reserved[2] = 1; h.reserved[3] = ctx->sensor_cap; }
 	if (ctx->has_kin) h.reserved[4] = (u32)ctx->kin_list.size();
 	if (ctx->has_frc) h.reserved[5] = 1;
-	h.reserved[6] = ctx->jset.n; h.reserved[7] = ctx->dset.n;
+	h.reserved[6] = ctx->jset.n; h.reserved[7] = ctx->drives.set.n;
 	h.bodies = ctx->B; h.boxes = ctx->nboxes; h.spheres = ctx->nspheres; h.connections = ctx->nconn; h.cache = cache; h.solver_mode = (u32)ctx->solver_mode;
 	return h;
 }
@@ -177,28 +191,15 @@ int nb_save_state(nb_context* ctx, const char* path, void* stream) {
 	FILE* f = fopen(path, "wb");
 	if (!f) { ctx->error = std::string("cannot open ") + path; return NB_ERR_ARGUMENT; }
 	const NbStateHeader h = state_header_of(ctx, c[CNT_CACHE]);
+	JointBundle jb;
+	if ((r = get_joint_bundle(ctx, jb, st))) { fclose(f); return r; }
 	StateHostCopies hc;
-	const unsigned char* kin = reinterpret_cast<const unsigned char*>(ctx->kin_list.data());
-	hc.kin.assign(kin, kin + 4 * ctx->kin_list.size());
-	std::vector<nb_joint> joints;
-	if ((r = get_joints(ctx, joints, st))) { fclose(f); return r; }
-	hc.joints.assign(reinterpret_cast<const unsigned char*>(joints.data()), reinterpret_cast<const unsigned char*>(joints.data() + joints.size()));
-	std::vector<nb_joint_drive> drives;
-	if ((r = get_drives(ctx, drives, st))) { fclose(f); return r; }
-	hc.drives.assign(reinterpret_cast<const unsigned char*>(drives.data()), reinterpret_cast<const unsigned char*>(drives.data() + drives.size()));
-	std::vector<nb_joint_spring> springs;
-	if ((r = get_springs(ctx, springs, st))) { fclose(f); return r; }
+	hc.kin = as_bytes(ctx->kin_list); hc.joints = as_bytes(jb.joints); hc.drives = as_bytes(jb.drives); hc.ccd = as_bytes(ctx->ccd); hc.springs = as_bytes(jb.springs);
+	const NbStateExt x = { (u32)ctx->ccd.size(), { (u32)jb.springs.size(), 0, 0 } };
 	std::vector<unsigned char> tmp;
 	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
-	const NbStateExt x = { (u32)ctx->ccd.size(), { (u32)springs.size(), 0, 0 } };
 	if (h.version >= 8) ok = ok && fwrite(&x, sizeof(x), 1, f) == 1;
-	for (const StateSection& s : state_sections(ctx, h, hc, false)) if (s.present) ok = ok && state_put(f, s, tmp, st);
-	if (h.version >= 8) ok = ok && fwrite(ctx->ccd.data(), sizeof(nb_ccd_body), ctx->ccd.size(), f) == ctx->ccd.size();   // 16 bytes each: no padding
-	if (h.version == 9) {   // 56 bytes each, the section padded to 16
-		std::vector<unsigned char> b(reinterpret_cast<const unsigned char*>(springs.data()), reinterpret_cast<const unsigned char*>(springs.data() + springs.size()));
-		b.resize((b.size() + 15) & ~(size_t)15, 0);
-		ok = ok && fwrite(b.data(), 1, b.size(), f) == b.size();
-	}
+	for (const StateSection& s : state_sections(ctx, h, x, hc, false)) if (s.present) ok = ok && state_put(f, s, tmp, st);
 	ok = (fclose(f) == 0) && ok;
 	if (!ok) { ctx->error = std::string("write failed: ") + path; return NB_ERR_CUDA; }
 	return NB_OK;
@@ -233,7 +234,8 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	StateHostCopies hc;
 	std::vector<unsigned char> tmp;
 	bool ok = true;
-	for (const StateSection& s : state_sections(ctx, h, hc, true)) if (s.present) ok = ok && state_get(f, s, tmp, st);
+	for (const StateSection& s : state_sections(ctx, h, x, hc, true)) if (s.present) ok = ok && state_get(f, s, tmp, st);
+	fclose(f);
 	u32 maxtag = 1;
 	if (ok) {
 		for (u32 i = 0; i < h.boxes; ++i) maxtag = std::max(maxtag, reinterpret_cast<const u32*>(hc.box_tags.data())[i]);
@@ -252,29 +254,14 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	// the body force rows: each names its own row and passes nb_set_body_forces' entry checks
 	const nb_body_force* frc = reinterpret_cast<const nb_body_force*>(hc.frc.data());
 	for (u32 i = 0; ok && h.reserved[5] && i < h.bodies; ++i) ok = frc[i].body == i && !body_force_problem(frc[i]);
-	const nb_joint* joints = reinterpret_cast<const nb_joint*>(hc.joints.data());
-	ok = ok && check_joints(ctx, joints, h.reserved[6], h.bodies) == NB_OK;
-	// the drives against the file's joints, through the upload's checks
-	const nb_joint_drive* drives = reinterpret_cast<const nb_joint_drive*>(hc.drives.data());
-	std::vector<u32> structure; std::vector<uint8_t> unit_rel, unit_ax;
-	for (u32 i = 0; ok && i < h.reserved[6]; ++i) {
-		structure.insert(structure.end(), { joints[i].type, joints[i].a, joints[i].b });
-		unit_rel.push_back(unit_quat(joints[i].rel_rotation) ? 1 : 0); unit_ax.push_back(unit_axis(joints[i].axis_a) ? 1 : 0);
-	}
-	ok = ok && check_drives(ctx, drives, h.reserved[7], h.reserved[6], structure.data(), unit_rel.data(), unit_ax.data()) == NB_OK;
+	// the joint set through the upload's checks, the drives and springs against the file's joints
+	const JointBundle jb = { from_bytes<nb_joint>(hc.joints, h.reserved[6]), from_bytes<nb_joint_drive>(hc.drives, h.reserved[7]),
+							 from_bytes<nb_joint_spring>(hc.springs, x.reserved[0]) };
+	ok = ok && check_joint_bundle(ctx, jb, h.bodies) == NB_OK;
 	// the continuous-collision set: the upload's entry checks, bodies nonzero, in range and ascending (a kinematic body may keep its entry)
-	std::vector<nb_ccd_body> ccd(x.ccd_bodies);
-	ok = ok && (ccd.empty() || fread(ccd.data(), sizeof(nb_ccd_body), ccd.size(), f) == ccd.size());
+	std::vector<nb_ccd_body> ccd = from_bytes<nb_ccd_body>(hc.ccd, x.ccd_bodies);
 	for (size_t i = 0; ok && i < ccd.size(); ++i)
 		ok = ccd[i].body != 0 && ccd[i].body < h.bodies && (i == 0 || ccd[i].body > ccd[i - 1].body) && !ccd_body_problem(ccd[i]);
-	// the springs against the file's joints, through the upload's checks
-	std::vector<nb_joint_spring> springs(x.reserved[0]);
-	const size_t spring_bytes = sizeof(nb_joint_spring) * springs.size();
-	std::vector<unsigned char> sb((spring_bytes + 15) & ~(size_t)15);
-	ok = ok && (sb.empty() || fread(sb.data(), 1, sb.size(), f) == sb.size());
-	if (ok && spring_bytes) memcpy(springs.data(), sb.data(), spring_bytes);
-	ok = ok && check_springs(ctx, springs.data(), x.reserved[0], h.reserved[6], structure.data(), unit_rel.data(), unit_ax.data()) == NB_OK;
-	fclose(f);
 	if (!ok) { ctx->error = std::string("read failed: ") + path; return NB_ERR_CUDA; }
 	ctx->scene_edited = false;   // the loaded scene replaces an edited one
 	CK(cudaMemcpyAsync(ctx->counts + CNT_CACHE, &h.cache, 4, cudaMemcpyHostToDevice, st));
@@ -285,10 +272,7 @@ int nb_load_state(nb_context* ctx, const char* path, void* stream) {
 	shape.kin.assign(idx, idx + kin.size());
 	const StateFileTables file = { hc.sensor.data(), kin.data(), frc };
 	{ int r = install_state(ctx, shape, &file, st); if (r) return r; }
-	drop_drives(ctx); drop_springs(ctx);   // a file without drives or springs removes them, also where its joints have the context's structure
-	{ int r = set_joints(ctx, joints, h.reserved[6], st); if (r) return r; }
-	{ int r = set_drives(ctx, drives, h.reserved[7], st); if (r) return r; }
-	{ int r = set_springs(ctx, springs.data(), x.reserved[0], st); if (r) return r; }
+	{ int r = put_joint_bundle(ctx, jb, st); if (r) return r; }   // a file without drives or springs removes them
 	{ int r = set_ccd(ctx, std::move(ccd), st); if (r) return r; }   // a file of an older version removes the set
 	CK(cudaStreamSynchronize(st));
 	return NB_OK;

@@ -1,6 +1,7 @@
 """Test infrastructure shared by the GPU tests: a side stream, the hash nb_replay prints, and the state-file layout of
 nudge_b200/csrc/nb_state_api.cuh (the header builder is also used by the CPU tests of nb_state_info)."""
 import struct
+import numpy as np
 
 # magic, version, bodies, boxes, spheres, connections, cache, solver_mode, reserved[8]
 STATE_HEADER = struct.Struct("<8s15I")
@@ -18,6 +19,13 @@ def side_stream():
     """A new CUDA stream (nb_step captures its graph only on a stream of its own)."""
     import torch
     return torch.cuda.Stream().cuda_stream
+
+
+def joint_rows(g):
+    """The joints' own rows, then the drive rows per driven joint in table order: nb_debug_read's "joint_rows" and "joint_drive_rows"
+    concatenated, the layout the restatements' row functions return."""
+    import nudge_b200
+    return np.concatenate([g.debug("joint_rows", nudge_b200.ROW), g.debug("joint_drive_rows", nudge_b200.ROW)])
 
 
 def fnv1a(b):

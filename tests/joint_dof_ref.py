@@ -30,8 +30,7 @@ def drive_table(joints, drives):
     appended rows' impulses in row order."""
     table = np.zeros(len(joints), DRIVE_TABLE)
     by = {int(d["joint"]): d for d in drives}
-    row = sum(ROWS_PER_TYPE[int(j["type"])] for j in joints)
-    imp = []
+    row, imp = 0, []
     for i, j in enumerate(joints):
         if i not in by:
             continue

@@ -39,11 +39,11 @@ def angle_limit_biases(sh, ch, e, limit_bias):
 
 def drive_table(joints, drives):
     """The drive table for `joints` in the order given, from `drives` (nudge_b200.JOINT_DRIVE, joint = an index into `joints`): the entries of
-    nb_upload_joint_drives with the half-angle pairs and each drive's first appended row; and the appended rows' impulses in row order."""
+    nb_upload_joint_drives with the half-angle pairs and each drive's first row in the drive rows; and the appended rows' impulses in row
+    order."""
     table = np.zeros(len(joints), DRIVE_TABLE)
     by = {int(d["joint"]): d for d in drives}
-    row = sum(ROWS_PER_TYPE[int(j["type"])] for j in joints)
-    imp = []
+    row, imp = 0, []
     for i, j in enumerate(joints):
         if i not in by:
             continue

@@ -8,7 +8,7 @@ import nudge_b200
 from nudge_b200 import scenes
 from oracle import joints_ref
 from tests import joint_dof_ref as dof
-from tests.gpu_util import side_stream
+from tests.gpu_util import side_stream, joint_rows
 from tests.test_gpu_rows import _free_bodies, _pile, _quat_rotate
 from tests.test_gpu_joints import _joints_at_rest, _body_bytes
 from tests.test_gpu_joint_drives import _renumber, _breaks_mid_run, _without_position
@@ -65,7 +65,7 @@ def _drive_impulses(joints, table, imp, driven):
     return np.array([out[i] for i in driven], np.float32).reshape(-1, 3)
 
 
-def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
+def test_own_rows_drive_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     n = 60
     s, rng = _free_bodies(n, 4)
     g = nudge_b200.Sim(s)
@@ -86,13 +86,13 @@ def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     g.upload_joints(joints); g.upload_joint_drives(drives)
     order = joints_ref.table_order(joints)
     table = g.debug("joint_drives", dof.DRIVE_TABLE)
-    before = g.debug("joint_rows", nudge_b200.ROW)
+    before = joint_rows(g)
     n_own = int(sum(ROWS[t] for t in joints["type"]))
     want_table, want_imp = dof.drive_table(joints[order], _renumber(drives, order))
     assert table.tobytes() == want_table.tobytes()
     assert before["impulse"][n_own:].tobytes() == want_imp.tobytes()
     g.collide(); g.apply_gravity_damping(); g.read_cached_impulses(); g.setup_contact_constraints()
-    got = g.debug("joint_rows", nudge_b200.ROW)
+    got = joint_rows(g)
     g.download_bodies()
     dt = np.float32(s.time_step)
     jt = joints[order]

@@ -8,7 +8,7 @@ import nudge_b200
 from nudge_b200 import scenes
 from oracle import joints_ref
 from tests import joint_drives_ref as drives_ref
-from tests.gpu_util import side_stream, STATE_HEADER
+from tests.gpu_util import side_stream, joint_rows, STATE_HEADER
 from tests.test_gpu_rows import _free_bodies, _pile
 from tests.test_gpu_joints import _joints_at_rest, _body_bytes
 
@@ -53,7 +53,7 @@ def _drive_impulses(joints, table, imp, driven):
     return np.array([out[i] for i in driven], np.float32).reshape(-1, 3)
 
 
-def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
+def test_own_rows_drive_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     n = 60
     s, rng = _free_bodies(n, 4)
     g = nudge_b200.Sim(s)
@@ -74,14 +74,14 @@ def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     g.upload_joints(joints); g.upload_joint_drives(drives)
     order = joints_ref.table_order(joints)
     table = g.debug("joint_drives", drives_ref.DRIVE_TABLE)
-    before = g.debug("joint_rows", nudge_b200.ROW)
+    before = joint_rows(g)
     n_own = int(sum(ROWS[t] for t in joints["type"]))
     # the upload: the host's table and the uploaded impulses, in table order
     want_table, want_imp = drives_ref.drive_table(joints[order], _renumber(drives, order))
     assert table.tobytes() == want_table.tobytes()
     assert before["impulse"][n_own:].tobytes() == want_imp.tobytes()
     g.collide(); g.apply_gravity_damping(); g.read_cached_impulses(); g.setup_contact_constraints()
-    got = g.debug("joint_rows", nudge_b200.ROW)
+    got = joint_rows(g)
     g.download_bodies()
     dt = np.float32(s.time_step)
     jt = joints[order]
@@ -273,7 +273,7 @@ def test_throttle_keeps_the_graph_and_drives_add_no_launch():
     g.upload_joint_drives(None)
     before = g.launch_count(); g.step()
     assert g.launch_count() - before == per_step[0] and len(g.download_joint_drives()) == 0
-    assert len(g.debug("joint_rows", nudge_b200.ROW)) == sum(ROWS[t] for t in joints["type"])
+    assert len(joint_rows(g)) == sum(ROWS[t] for t in joints["type"])
 
 
 def test_snapshot_restore_repeats_a_run_with_a_break():

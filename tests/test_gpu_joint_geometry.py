@@ -12,7 +12,7 @@ from nudge_b200 import scenes
 from oracle import joints_ref
 from tests import joint_dof_ref as dof
 from tests import joint_geometry as geo
-from tests.gpu_util import side_stream
+from tests.gpu_util import side_stream, joint_rows
 from tests.test_joint_geometry_ref import COMBOS, BALL, HINGE, FIXED, DISTANCE, L, M, S, CN, TW, drive, random_joint, check_joint
 
 pytestmark = pytest.mark.gpu
@@ -58,7 +58,7 @@ def _poses():
     return out
 
 
-def test_device_rows_against_the_float64_geometry():
+def test_device_own_and_drive_rows_against_the_float64_geometry():
     cases = _poses()
     m = len(cases)
     s = _scene(2 * m)
@@ -86,7 +86,7 @@ def test_device_rows_against_the_float64_geometry():
     g = nudge_b200.Sim(s)
     g.upload_joints(joints); g.upload_joint_drives(drives)
     g.collide(); g.apply_gravity_damping(); g.read_cached_impulses(); g.setup_contact_constraints()
-    rows = g.debug("joint_rows", nudge_b200.ROW)
+    rows = joint_rows(g)
     table = g.debug("joint_drives", dof.DRIVE_TABLE)
     g.download_bodies()
     order = joints_ref.table_order(joints)

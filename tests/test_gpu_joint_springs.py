@@ -10,7 +10,7 @@ from nudge_b200 import scenes, abi
 from oracle import joints_ref
 from tests import joint_dof_ref as dof
 from tests import joint_spring_ref as spr
-from tests.gpu_util import side_stream
+from tests.gpu_util import side_stream, joint_rows
 from tests.test_gpu_rows import _free_bodies, _pile, _quat_rotate
 from tests.test_gpu_joints import _joints_at_rest, _body_bytes
 from tests.test_gpu_joint_drives import _renumber
@@ -45,7 +45,7 @@ def _random_springs(joints, rng, share=0.6):
     return np.array(out, nudge_b200.JOINT_SPRING)
 
 
-def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
+def test_own_rows_drive_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     n, m = 60, 320
     s, rng = _free_bodies(n, 4)
     g = nudge_b200.Sim(s)
@@ -70,10 +70,10 @@ def test_rows_and_table_equal_the_numpy_restatement_byte_for_byte():
     assert stable.tobytes() == want_stable.tobytes()
     assert g.debug("joint_spring_rows", nudge_b200.ROW)["impulse"].tobytes() == want_simp.tobytes()
     table = g.debug("joint_drives", dof.DRIVE_TABLE)
-    before = g.debug("joint_rows", nudge_b200.ROW)
+    before = joint_rows(g)
     n_own = int(sum(ROWS[t] for t in joints["type"]))
     g.collide(); g.apply_gravity_damping(); g.read_cached_impulses(); g.setup_contact_constraints()
-    got, sgot = g.debug("joint_rows", nudge_b200.ROW), g.debug("joint_spring_rows", nudge_b200.ROW)
+    got, sgot = joint_rows(g), g.debug("joint_spring_rows", nudge_b200.ROW)
     g.download_bodies()
     dt = np.float32(s.time_step)
     table["broken"] = dof.broken_after(jt, before, table, dt)
@@ -341,7 +341,7 @@ def _pile_with_springs(seed, m=40, stream=True):
     return s, g, joints, drives, springs, rng
 
 
-def test_targets_uploaded_every_step_keep_the_graph_and_add_no_launch():
+def test_targets_uploaded_every_step_keep_the_graph_add_no_launch_and_leave_the_drive_rows():
     s, g, joints, drives, springs, rng = _pile_with_springs(8)
     base = nudge_b200.Sim(s, stream=side_stream())
     base.upload_joints(joints); base.upload_joint_drives(drives)
@@ -366,7 +366,7 @@ def test_targets_uploaded_every_step_keep_the_graph_and_add_no_launch():
     before = g.launch_count(); g.step()
     assert g.launch_count() - before == without
     g.download_bodies()
-    assert len(g.debug("joint_rows", nudge_b200.ROW)) == sum(ROWS[t] for t in joints["type"]) + sum(dof.drive_row_count(int(f)) for f in drives["flags"])
+    assert len(joint_rows(g)) == sum(ROWS[t] for t in joints["type"]) + sum(dof.drive_row_count(int(f)) for f in drives["flags"])
 
 
 def test_snapshot_restore_repeats_a_run_with_every_table_present():

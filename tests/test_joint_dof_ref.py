@@ -181,8 +181,9 @@ def _random_old_set(seed):
 
 # sha256 of the bytes tests/joint_drives_ref.py gave for _random_old_set(11) before SLIDE, CONE and TWIST existed: the table, the first
 # build's rows, the break flags on those rows and the solve order; recorded again when the angle limit measure stopped folding back past a
-# half turn (DESIGN.md section 8.17), which changed the bias of six hinge limit rows and nothing else
-OLD_DIGEST = "c2debc07a0461ef725a2c0beb5542d0923de033afeaeb582a3c08d33e4166ed8"
+# half turn (DESIGN.md section 8.17), which changed the bias of six hinge limit rows and nothing else, and again when the drive rows got a
+# buffer of their own, which lowered each driven entry's row by the 214 own rows and changed nothing else
+OLD_DIGEST = "b4e7bd8a08829f2637ffe4e11d2a815584c92de646846c6235f2e9b3f0c0aef7"
 
 
 def _old_bytes(ref, joints, drives, xf):

@@ -100,7 +100,7 @@ def test_rows_without_drives_are_todays_and_the_table_order_is_kept():
     assert drives_ref.joint_rows(joints, xf, DT, table).tobytes() == plain.tobytes()
     table, imp = drives_ref.drive_table(joints, np.array([_drive(1, 3, lower=-1.0, upper=1.0, impulse=(0.5, 0.25, 0.125)),
                                                           _drive(3, 1, lower=0.1, upper=2.0, impulse=(0.0, 1.0, 2.0))]))
-    assert list(table["row"][[1, 3]]) == [15, 18] and list(imp) == [0.5, 0.25, 0.125, 1.0, 2.0]
+    assert list(table["row"][[1, 3]]) == [0, 3] and list(imp) == [0.5, 0.25, 0.125, 1.0, 2.0]
     rows = drives_ref.joint_rows(joints, xf, DT, table, imp)
     assert len(rows) == 20
     for k in rows.dtype.names:
